@@ -108,6 +108,8 @@ SIGNATURES = {
     "dbl_kernel_launches": (C.c_int64, [vp]),
     "dbl_set_link_mode": (C.c_int, [vp, C.c_int]),
     "dbl_link_kernel": (C.c_int, [vp, C.c_int]),
+    "dbl_set_link_mass_capture": (C.c_int, [vp, C.c_int]),
+    "dbl_link_mass": (C.c_int, [vp, f64p]),
     "dbl_index_hash_slots": (C.c_int32, [vp]),
     "dbl_set_graph_mode": (C.c_int, [vp, C.c_int]),
     "dbl_last_sweep_ms": (C.c_double, [vp]),

@@ -1363,6 +1363,8 @@ struct dbl_ctx {
   int64_t launches = 0;
   double link_ms = 0.0;
   int link_mode = 0;  // 0 auto, 1 generic kernel everywhere, 2 dense TMA kernels everywhere (no pruning)
+  bool link_mass_on = false;   // dbl_set_link_mass_capture: the link kernels store every record's total mass
+  DevBuf<double> link_mass;    // R entries, allocated by the first sweep with the capture on
   double last_sweep_ms = 0.0;
   int64_t link_launches = 0;
   // eager sweeps are timed phase by phase: events before / after the link kernel, after the value / distortion /
@@ -2189,6 +2191,13 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
   for (int k = 0; k < A; ++k) lp.perm[k] = ctx->perm[k];
   lp.blk_of_link = ctx->blk.p;
   lp.pack_consts = ctx->pack_consts;
+  if (ctx->link_mass_on) {
+    if (ctx->link_mass.n != (size_t)ctx->R) {  // the first sweep of a kind runs eagerly: never inside a graph capture
+      CUDA_TRY(ctx->link_mass.alloc((size_t)ctx->R));
+      CUDA_TRY(cudaMemsetAsync(ctx->link_mass.p, 0, sizeof(double) * (size_t)ctx->R, ctx->stream));
+    }
+    lp.link_mass = ctx->link_mass.p;
+  }
   const size_t ring = (size_t)LINK_STAGES * tile_words(A) * 4 + 128;
   const int mode = ctx->link_mode;  // 0 auto, 1 force generic
   lp.hslots = ctx->hslots; lp.hshift = ctx->hshift;
@@ -2911,6 +2920,30 @@ extern "C" int dbl_set_link_mode(dbl_ctx *ctx, int mode) {
   if (!ctx || mode < 0 || mode > 2) return DBL_ERR_INVALID;
   ctx->drop_graphs();
   ctx->link_mode = mode;
+  return DBL_OK;
+}
+
+extern "C" int dbl_set_link_mass_capture(dbl_ctx *ctx, int on) {
+  if (!ctx) return DBL_ERR_INVALID;
+  if (ctx->world > 1) { ctx->set_error("link-mass capture needs an unsharded context"); return DBL_ERR_STATE; }
+  ctx->drop_graphs();  // captured sweeps hold the link parameters by value
+  ctx->link_mass_on = on != 0;
+  if (!ctx->link_mass_on) ctx->link_mass.release();
+  return DBL_OK;
+}
+
+extern "C" int dbl_link_mass(dbl_ctx *ctx, double *mass_out) {
+  if (!ctx || !mass_out) return DBL_ERR_INVALID;
+  if (ctx->world > 1) { ctx->set_error("link-mass capture needs an unsharded context"); return DBL_ERR_STATE; }
+  if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
+  if (!ctx->link_mass_on || ctx->link_mass.n != (size_t)ctx->R) {
+    ctx->set_error("dbl_link_mass: no sweep has run with the capture on (dbl_set_link_mass_capture)");
+    return DBL_ERR_STATE;
+  }
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  CUDA_TRY(cudaMemcpyAsync(mass_out, ctx->link_mass.p, sizeof(double) * (size_t)ctx->R, cudaMemcpyDeviceToHost,
+                           ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return DBL_OK;
 }
 

@@ -92,6 +92,7 @@ struct LinkParams {
   int pack_consts;         // tiles carry the byte-packed constant attributes (1..4 of them, vocabularies <= 255)
   const int *blk_of_link;  // block id of every entity (k_link_pruned: block of a record = block of its entity)
   int hslots, hshift;  // common size of the per-row similarity hash tables (k_link_pcg2); 0 = unavailable
+  double *link_mass;   // R entries or null: every link kernel stores the total mass of each record's categorical
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -293,6 +294,10 @@ __device__ __forceinline__ void store_link(const LinkParams &p, int lane, int r,
     atomicAdd(p.pairs, (unsigned long long)visited);
   }
 }
+// the total a record's draw tests for zero / non-finite (dbl_link_mass), zero and non-finite totals included
+__device__ __forceinline__ void store_mass(const LinkParams &p, int lane, int r, double total) {
+  if (p.link_mass && lane == 0) p.link_mass[r] = total;
+}
 __device__ __forceinline__ void fail_link(const LinkParams &p, int lane, int r) {
   if (lane == 0) {  // reference: IllegalArgumentException("zero probability mass")
     atomicOr(p.status, (unsigned long long)ST_ZERO_MASS);
@@ -345,6 +350,7 @@ __global__ void __launch_bounds__(LINK_WARPS * 32) k_link_generic(LinkParams p) 
       mark = min(mark + spc, nsteps);
     }
   }
+  store_mass(p, lane, r, run);
   if (!(run > 0.0) || isinf(run)) { fail_link(p, lane, r); return; }
   const U2 u = uniform2(p.seed, PH_LINK, link_iter(p), (uint32_t)r, 0u);
   const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q, run, u.u0, wf);
@@ -551,6 +557,7 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
     if (lane == 0) mbar_arrive(&rg.empty[s]);
   }
   if (!active) return;
+  store_mass(p, lane, r, run);
   if (!(run > 0.0) || isinf(run)) { fail_link(p, lane, r); return; }
   auto wf = [&](int j) -> double {
     if (j >= n) return 0.0;
@@ -852,11 +859,13 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
   }
   __syncwarp();
   if (ns == 1) {  // a single candidate with positive weight is drawn whatever the uniform is: skip the search
+    store_mass(p, lane, r, s_sw[warp][0]);  // = the dense kernels' total: every other weight is an exact zero
     if (isinf(s_sw[warp][0])) { fail_link(p, lane, r); return; }
     store_link(p, lane, r, b, phi - plo, s_sj[warp][0]);
     return;
   }
   close_chunks_until(nchunks);
+  store_mass(p, lane, r, run);
   if (!(run > 0.0) || isinf(run)) { fail_link(p, lane, r); return; }
 
   // ---- pass 2: the same walk restricted to the chosen chunk
@@ -997,6 +1006,7 @@ __global__ void __launch_bounds__(HEAVY_WARPS * 32) k_link_heavy(PrunedParams pp
         run = run + butterfly_sum(s_sums[c * 32 + lane]);
         if (lane == c) Q = run;
       }
+      store_mass(p, lane, r, run);
       if (!(run > 0.0) || isinf(run)) {
         fail_link(p, lane, r);
       } else {

@@ -367,6 +367,7 @@ __global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_s
     for (int ri = 0; ri < RPW; ++ri) {
       if (!act[ri]) continue;
       const int r = rr[ri];
+      store_mass(p, lane, r, run[ri]);
       if (!(run[ri] > 0.0) || isinf(run[ri])) { fail_link(p, lane, r); continue; }
       auto wf = [&](int j) -> double {
         if (j >= n) return 0.0;

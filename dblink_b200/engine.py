@@ -446,6 +446,16 @@ class GibbsEngine:
                                                   "32" if k & 8 else "0", 1 if k & 4 else 0)
         return base
 
+    def set_link_mass_capture(self, on=True):
+        """Checking aid: make every link kernel store the total mass of each record's categorical (off by default)."""
+        _check(_lib.load().dbl_set_link_mass_capture(self._h, int(bool(on))), "set_link_mass_capture", self._h)
+
+    def link_mass(self):
+        """float64[R]: the total mass of each record's link categorical in the last sweep run with the capture on."""
+        out = np.zeros(self.num_records, np.float64)
+        _check(_lib.load().dbl_link_mass(self._h, _p(out, _lib.f64p)), "link_mass", self._h)
+        return out
+
     def set_graph_mode(self, mode):
         """0 = automatic (CUDA graph replay of a sweep for launch-bound sizes), 1 = never, 2 = whenever possible."""
         _check(_lib.load().dbl_set_graph_mode(self._h, int(mode)), "set_graph_mode", self._h)

@@ -252,6 +252,13 @@ int dbl_set_link_mode(dbl_ctx *, int mode);
  * kernel, 3 k_link_pcg2 (+4: byte-packed constants, +8: 32-slot tables known at compile time).  A model that falls
  * back to the generic kernel runs an order of magnitude slower: benches and tests assert what they expect. */
 int dbl_link_kernel(const dbl_ctx *, int sampler);
+/* Link-mass capture (checking only; off by default, free when off): with on != 0 every link kernel stores the total
+ * mass of each record's categorical -- the sum of its protocol weights over the block, the number the draw tests for
+ * zero / non-finite -- into a device array of R entries, from the link phase of the sweep that ran last.  Toggling
+ * drops captured sweep graphs.  dbl_link_mass copies the R totals (record order) to the host; DBL_ERR_STATE before a
+ * sweep with the capture on.  Both return DBL_ERR_STATE on a sharded context. */
+int dbl_set_link_mass_capture(dbl_ctx *, int on);
+int dbl_link_mass(dbl_ctx *, double *mass_out /*R*/);
 /* How dbl_sweep / dbl_sweep_async enqueue several sweeps: 0 = automatic (problems small enough to be bound by kernel
  * launches, and the index-pruned samplers at every size, replay a captured CUDA graph of one sweep), 1 = every sweep
  * enqueued kernel by kernel (and timed phase by phase, dbl_link_kernel_ms / dbl_phase_ms), 2 = graphs whenever

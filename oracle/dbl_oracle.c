@@ -533,6 +533,7 @@ static orc_state *state_alloc(const orc_model *m, int64_t R, int64_t E) {
   s->y = (int32_t *)malloc(sizeof(int32_t) * (size_t)(E * A + 1));
   s->blk = (int32_t *)malloc(sizeof(int32_t) * (size_t)(E + 1));
   s->theta = (double *)malloc(sizeof(double) * (size_t)(A * m->F));
+  s->mass = (double *)calloc((size_t)(R + 1), sizeof(double));
   s->file_sizes = (int64_t *)calloc((size_t)m->F, sizeof(int64_t));
   return s;
 }
@@ -598,7 +599,7 @@ orc_state *orc_state_from_arrays(const orc_model *m, int64_t R, int64_t E, const
 
 void orc_state_free(orc_state *s) {
   if (!s) return;
-  free(s->x); free(s->file); free(s->link); free(s->z); free(s->y); free(s->blk); free(s->theta);
+  free(s->x); free(s->file); free(s->link); free(s->z); free(s->y); free(s->blk); free(s->theta); free(s->mass);
   free(s->file_sizes); free(s);
 }
 int64_t orc_state_R(const orc_state *s) { return s->R; }
@@ -609,6 +610,7 @@ const int32_t *orc_state_link(const orc_state *s) { return s->link; }
 const uint8_t *orc_state_z(const orc_state *s) { return s->z; }
 const int32_t *orc_state_block(const orc_state *s) { return s->blk; }
 const double *orc_state_theta(const orc_state *s) { return s->theta; }
+const double *orc_state_last_link_mass(const orc_state *s) { return s->mass; }
 
 /* CSR entity -> linked records (ascending record id); LinksIndex, GU:84-119 */
 static void build_links_csr(const orc_state *s, int64_t **ptr_out, int64_t **rec_out) {
@@ -812,9 +814,11 @@ static void load_step(const double *w, int64_t n, int64_t step, double out[32]) 
   }
 }
 
-/* status: 0 ok, 1 zero/non-finite total mass (reference throws, IndexNonUniformDiscreteDist.scala:71-79) */
-int orc_draw_index(const double *w, int64_t n, double u, int *status) {
+/* status: 0 ok, 1 zero/non-finite total mass (reference throws, IndexNonUniformDiscreteDist.scala:71-79);
+   total_out (may be NULL): the total mass of pass 1, the number the zero / non-finite test looks at */
+int orc_draw_index(const double *w, int64_t n, double u, int *status, double *total_out) {
   if (status) *status = 0;
+  if (total_out) *total_out = 0.0;
   /* candidates are laid out in tiles of 128 (= 4 steps); a chunk is a whole number of tiles */
   int64_t ntiles = (n + 127) / 128;
   if (ntiles == 0) { if (status) *status = 1; return -1; }
@@ -839,6 +843,7 @@ int orc_draw_index(const double *w, int64_t n, double u, int *status) {
     Q[c] = run;
   }
   double total = run;
+  if (total_out) *total_out = total;
   if (!(total > 0.0) || isinf(total)) { if (status) *status = 1; return -1; }
   double t = u * total;
   int64_t chunk = nchunks - 1; /* u*total < total always holds for u < 1, so the scan below always hits */
@@ -1208,6 +1213,7 @@ typedef struct {
   const int32_t *ysorted; /* entity rows in block order: row i = entity bent[i] */
   const int64_t *rorder;  /* records grouped by block: consecutive records score the same (cache-resident) table */
   int32_t *newlink;
+  double *mass;           /* total mass of every record's categorical */
 } link_job;
 
 /* PCG-II weight with the record's sparse similarity rows scattered into dense per-attribute tables (0.0 = not
@@ -1282,7 +1288,7 @@ static void *link_worker(void *arg) {
     double u[2];
     orc_uniform2(m->seed, ORC_PHASE_LINK, jb->it, (uint32_t)r, 0, u);
     int st;
-    int j = orc_draw_index(w, n, u[0], &st);
+    int j = orc_draw_index(w, n, u[0], &st, &jb->mass[r]);
     if (st) { jb->status = 1; jb->newlink[r] = s->link[r]; } else jb->newlink[r] = cand[j];
   }
   for (int a = 0; a < A; ++a) free(dense[a]);
@@ -1478,7 +1484,7 @@ int orc_state_sweep(orc_state *s, int sampler) {
       link_job *jb = &jobs[t];
       jb->s = s; jb->sampler = sampler; jb->it = it; jb->tid = t; jb->nthreads = nthreads; jb->maxn = maxn;
       jb->bptr = bptr; jb->bent = bent; jb->entN = entN; jb->ysorted = ysorted; jb->rorder = rorder;
-      jb->newlink = newlink; jb->status = 0;
+      jb->newlink = newlink; jb->mass = s->mass; jb->status = 0;
       if (nthreads == 1) link_worker(jb);
       else pthread_create(&th[t], NULL, link_worker, jb);
     }

@@ -99,6 +99,9 @@ const int32_t *orc_state_link(const orc_state *);
 const uint8_t *orc_state_z(const orc_state *);
 const int32_t *orc_state_block(const orc_state *);
 const double *orc_state_theta(const orc_state *);
+/* R entries: the total mass of each record's link categorical (the sum orc_draw_index tests for zero / non-finite)
+   in the link phase of the last sweep; zeros before the first sweep */
+const double *orc_state_last_link_mass(const orc_state *);
 /* summary (GibbsUpdates.scala:219-301) -- recomputed on demand */
 typedef struct {
   int64_t iteration;
@@ -120,7 +123,7 @@ void orc_draw_theta(const orc_model *, const int64_t *agg_dist, const int64_t *f
                     double *theta_out);
 
 /* ---- protocol primitives exposed for unit tests ---- */
-int orc_draw_index(const double *w, int64_t n, double u, int *status);
+int orc_draw_index(const double *w, int64_t n, double u, int *status, double *total_out);
 int orc_invcdf(const double *cdf, int V, double u);
 /* literal restatements of the reference's per-record link weights (GU:363-466) for distribution tests */
 void orc_ref_link_weights(const orc_state *, int64_t r, int sampler, const int32_t *cand, int64_t n_cand,

@@ -40,6 +40,7 @@ struct orc_state {
   int32_t *x, *file, *link, *y, *blk;
   uint8_t *z;
   double *theta;       /* A x F */
+  double *mass;        /* R: total mass of each record's link categorical in the last sweep (0 before any) */
   int64_t *file_sizes; /* F */
 };
 

@@ -100,13 +100,14 @@ def lib():
         sig("orc_state_" + n, c_i32p, vp)
     sig("orc_state_z", c_u8p, vp)
     sig("orc_state_theta", c_dp, vp)
+    sig("orc_state_last_link_mass", c_dp, vp)
     sig("orc_state_summary", None, vp, C.c_void_p, c_i64p, c_i64p)
     sig("orc_state_sweep", C.c_int, vp, C.c_int)
     sig("orc_draw_theta", None, vp, c_i64p, c_i64p, C.c_uint32, c_dp)
     sig("orc_det_log", C.c_double, C.c_double)
     sig("orc_det_exp", C.c_double, C.c_double)
     sig("orc_rest_of_sweep_timed", None, vp, C.c_int, C.c_int, c_dp)
-    sig("orc_draw_index", C.c_int, c_dp, C.c_int64, C.c_double, C.POINTER(C.c_int))
+    sig("orc_draw_index", C.c_int, c_dp, C.c_int64, C.c_double, C.POINTER(C.c_int), c_dp)
     sig("orc_invcdf", C.c_int, c_dp, C.c_int, C.c_double)
     sig("orc_ref_link_weights", None, vp, C.c_int64, C.c_int, c_i32p, C.c_int64, c_dp)
     sig("orc_link_weights", None, vp, C.c_int64, C.c_int, c_i32p, C.c_int64, c_dp)
@@ -319,6 +320,10 @@ class State:
     def theta(self):
         return np.ctypeslib.as_array(lib().orc_state_theta(self.h), (self.model.A, self.model.F)).copy()
 
+    def last_link_mass(self):
+        """float64[R]: the total mass of each record's link categorical in the last sweep (zeros before any)"""
+        return np.ctypeslib.as_array(lib().orc_state_last_link_mass(self.h), (self.R,)).copy()
+
     def summary(self):
         head = SummaryHead()
         agg = np.zeros((self.model.A, self.model.F), np.int64)
@@ -354,11 +359,13 @@ class State:
         return lib().orc_ref_dist_prob(self.h, r, a)
 
 
-def draw_index(w, u):
+def draw_index(w, u, with_total=False):
+    """-> (index, status), or (index, status, total mass) with with_total"""
     w = _f64(w)
     st = C.c_int(0)
-    j = lib().orc_draw_index(_p(w, c_dp), len(w), u, C.byref(st))
-    return j, st.value
+    tot = C.c_double(0.0)
+    j = lib().orc_draw_index(_p(w, c_dp), len(w), u, C.byref(st), C.byref(tot))
+    return (j, st.value, tot.value) if with_total else (j, st.value)
 
 
 def draw_theta(model, agg_dist, file_sizes, it):

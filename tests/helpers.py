@@ -147,3 +147,77 @@ def host_threads(cap=256):
         except Exception:
             pass
     return max(1, min(cap, n))
+
+
+def threshold_problem(vocab, threshold, R=900, extra=(), n_files=1, seed=7):
+    """synth.generate(seed, R, [s0 ~ levenshtein over `vocab` strings] + extra) with s0's similarity threshold set to
+    `threshold`: a lower threshold makes more values similar, i.e. longer similarity rows and larger hash tables.
+    (n_files only adds the file column: the values do not depend on it.)"""
+    from dblink_b200 import synth
+    from dblink_b200.records import SimilarityFn
+
+    attrs = [synth.SynthAttr("s0", "levenshtein", vocab)] + list(extra)
+    g = synth.generate(seed, R, attrs, dup=0.3, distortion=0.15, missing=0.05, n_files=n_files)
+    g["attributes"][0].similarity_fn = SimilarityFn("LevenshteinSimilarityFn", threshold, 10.0)
+    return g
+
+
+# Tolerance of a link kernel's total mass against the literal reference below.  Both sides sum positive terms, so
+# relative errors add up without cancellation: a protocol weight is a product of at most ~3 rounded operations per
+# attribute, the total adds it in a lane sum of at most 16 steps (blocks up to 16 k entities), a 5-level butterfly and
+# at most 32 chunk totals; the literal side rounds about as often per weight, sums exactly (math.fsum) and divides by
+# a product of one factor per attribute.  At these block sizes that is fewer than ~150 rounded operations on any
+# path, i.e. a relative error below ~150 * 2^-53 = 2e-14.  1e-12 leaves a 50-fold margin and still fails a factor
+# that is off by 2^-40 on every candidate.
+LITERAL_MASS_REL = 1e-12
+
+
+def literal_link_mass(O, m, x, file, y, z, link, theta, sampler, records=None):
+    """Reference total mass of each record's link categorical for one sweep, from the literal GU conditionals.
+
+    (y, z, link) = the state BEFORE the sweep, theta = the sweep's theta (drawn before the links, so read after the
+    sweep).  Candidates = the entities of the record's block.  Weights = the oracle's literal restatements (GU:384-389
+    for PCG-II, GU:444-459 for the others), summed with math.fsum and divided by the record constant the protocol
+    drops: PCG-II prod over observed a of theta[a, file] * phi_a(x_a), the others prod over observed distorted a of
+    phi_a(x_a).  -> float64[len(records)] (all records by default)."""
+    import math
+
+    st = O.State.from_arrays(m, x, file, z, link, y, theta, 0)
+    block = st.block
+    sid = O.SAMPLERS[sampler]
+    members = {int(b): np.flatnonzero(block == b).astype(np.int32) for b in np.unique(block)}
+    x, z, file = np.asarray(x), np.asarray(z), np.asarray(file)
+    phi = [ix.phi for ix in m.indexes]
+    recs = range(x.shape[0]) if records is None else [int(r) for r in records]
+    out = np.empty(len(recs))
+    for i, r in enumerate(recs):
+        w = st.link_weights(r, sid, members[int(block[link[r]])], literal=True)
+        c = 1.0
+        for a in range(x.shape[1]):
+            v = x[r, a]
+            if v < 0:
+                continue
+            if sid == O.PCG_II:
+                c *= theta[a, file[r]] * phi[a][v]
+            elif z[r, a]:
+                c *= phi[a][v]
+        out[i] = math.fsum(w) / c
+    return out
+
+
+def assert_same_mass(got, want, what=""):
+    """bit-for-bit equality of two float64 arrays of totals, none of them NaN"""
+    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
+    assert got.shape == want.shape
+    assert not np.isnan(got).any() and not np.isnan(want).any(), what
+    bad = np.flatnonzero(got.view(np.uint64) != want.view(np.uint64))
+    assert bad.size == 0, f"{what}: {bad.size} totals differ, first record {bad[0]}: {got[bad[0]]!r} != {want[bad[0]]!r}"
+
+
+def assert_literal_mass(got, ref, what=""):
+    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
+    assert np.isfinite(got).all() and np.isfinite(ref).all(), what
+    err = np.abs(got - ref)
+    bad = np.flatnonzero(err > LITERAL_MASS_REL * np.abs(ref))
+    assert bad.size == 0, (f"{what}: {bad.size} totals off the literal reference, worst relative error "
+                           f"{np.max(err[bad] / np.abs(ref[bad]))!r} (record position {bad[0]})")

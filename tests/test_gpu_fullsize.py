@@ -96,7 +96,7 @@ def _full_config_against_oracle(monkeypatch, config, records, levels, split, sam
     import dblink_b200 as D
     from dblink_b200 import synth
     from dblink_b200.engine import combine_state_hash
-    from helpers import host_threads, state_hash_numpy
+    from helpers import assert_literal_mass, assert_same_mass, host_threads, literal_link_mass, state_hash_numpy
     from oracle import oracle as O
 
     monkeypatch.setenv("ORC_THREADS", str(host_threads()))
@@ -114,12 +114,20 @@ def _full_config_against_oracle(monkeypatch, config, records, levels, split, sam
     d = eng.download_state()
     for k in ("link", "y", "z", "theta", "block"):
         np.testing.assert_array_equal(d[k], getattr(st, k), err_msg="initial " + k)
+    eng.set_link_mass_capture(True)
+    sample = np.sort(np.random.default_rng(config).choice(records, 2000, replace=False))
     for sampler in samplers:
+        y0, z0, link0 = st.y, st.z, st.link
         eng.sweep(sampler, 1)
         assert st.sweep(O.SAMPLERS[sampler]) == 0
         d = eng.download_state()
         for k in ("theta", "link", "y", "z", "block"):
             np.testing.assert_array_equal(d[k], getattr(st, k), err_msg=f"{sampler} {k}")
+        # every record's total over its whole block (~15 k candidates at 64 blocks), bit for bit
+        mass = eng.link_mass()
+        assert_same_mass(mass, st.last_link_mass(), sampler)
+        ref = literal_link_mass(O, st.model, st.x, st.file, y0, z0, link0, st.theta, sampler, sample)
+        assert_literal_mass(mass[sample], ref, sampler)
         s = eng.summary()
         he, hr = eng.state_hash()
         assert combine_state_hash(he, hr, s["theta"], s["iteration"]) == \

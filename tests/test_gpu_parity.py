@@ -6,7 +6,7 @@ log-likelihood (a floating-point diagnostic reduced in a different order) to 1e-
 import numpy as np
 import pytest
 
-from helpers import oracle_setup, product_setup, random_state, synth_problem
+from helpers import assert_same_mass, oracle_setup, product_setup, random_state, synth_problem
 
 pytestmark = pytest.mark.gpu
 
@@ -48,15 +48,19 @@ def test_chain_from_init(oracle, sampler, levels, attr_ids, mode):
     g = synth_problem(seed=5, R=900, n_files=2)
     eng, rc, x, file = product_setup(g, 99, levels, attr_ids)
     eng.set_link_mode(mode)
+    eng.set_link_mass_capture(True)
     m, st, tree, ox, ofile = oracle_setup(oracle, g, 99, levels, attr_ids)
     for it in range(6):
         eng.sweep(sampler, 1)
         assert st.sweep(oracle.SAMPLERS[sampler]) == 0
         assert_same_state(eng, st)
+        # the total mass of every record's categorical, not just the one draw taken from it
+        assert_same_mass(eng.link_mass(), st.last_link_mass(), f"sweep {it}")
     # several sweeps in one call == the same sweeps one by one
     eng.sweep(sampler, 3)
     st.sweep(oracle.SAMPLERS[sampler], 3)
     assert_same_state(eng, st)
+    assert_same_mass(eng.link_mass(), st.last_link_mass(), "3 sweeps in one call")
 
 
 @pytest.mark.parametrize("sampler", SAMPLERS)
@@ -65,6 +69,7 @@ def test_random_states(oracle, sampler):
     distorted/non-distorted mixtures, several files and blocks"""
     g = synth_problem(seed=11, R=500, n_files=3, missing=0.08, distortion=0.2)
     eng, rc, x, file = product_setup(g, 7, 3, (3, 2, 0))
+    eng.set_link_mass_capture(True)
     m, st0, tree, ox, ofile = oracle_setup(oracle, g, 7, 3, (3, 2, 0))
     Vs = [ix.num_values for ix in rc.indexes]
     rng = np.random.default_rng(2024)
@@ -74,9 +79,11 @@ def test_random_states(oracle, sampler):
         eng.upload_state(x, file, z, link, y, theta, iteration=10 * trial)
         st = oracle.State.from_arrays(m, x, file, z, link, y, theta, 10 * trial)
         assert_same_state(eng, st)
-        eng.sweep(sampler, 2)
-        assert st.sweep(oracle.SAMPLERS[sampler], 2) == 0
-        assert_same_state(eng, st)
+        for it in range(2):
+            eng.sweep(sampler, 1)
+            assert st.sweep(oracle.SAMPLERS[sampler]) == 0
+            assert_same_state(eng, st)
+            assert_same_mass(eng.link_mass(), st.last_link_mass(), f"trial {trial} sweep {it}")
 
 
 @pytest.mark.parametrize("sampler", ["PCG-I", "Gibbs", "Gibbs-Sequential"])

@@ -190,3 +190,29 @@ def test_threaded_link_phase_gives_the_same_chain(oracle, monkeypatch):
     for nt in ("3", "8", "plain"):
         for a, b in zip(out["1"], out[nt]):
             assert np.array_equal(a, b)
+
+
+@pytest.mark.parametrize("row", ["hash64", "hash128", "hash256"])
+def test_oracle_link_mass_matches_literal_conditionals(oracle, row):
+    """the total mass the oracle's sweep draws each link from (protocol weights, its dense PCG-II tables, the
+    lane/chunk summation order) equals the sum of the literal GU:384-389 / GU:444-459 weights over the record's block
+    divided by the record constant, for every record of a 900-record, 2-file, 4-block problem; the models are those
+    whose similarity rows need 64, 128 and 256 hash slots on the GPU"""
+    from dblink_b200 import synth
+
+    from helpers import assert_literal_mass, literal_link_mass, threshold_problem
+
+    C = synth.SynthAttr
+    g = {"hash64": lambda: threshold_problem(60, 3.0, extra=[C("c0", "constant", 5), C("c1", "constant", 9)], n_files=2),
+         "hash128": lambda: threshold_problem(120, 3.0, extra=[C("s1", "levenshtein", 80)], n_files=2),
+         "hash256": lambda: threshold_problem(400, 3.0, n_files=2)}[row]()
+    m, st, tree, x, file = oracle_setup(oracle, g, 13, 2, (0,))
+    assert tree.n_leaves == 4
+    assert not st.last_link_mass().any()  # nothing drawn yet
+    for sampler in SAMPLERS:
+        for it in range(2):
+            y, z, link = st.y, st.z, st.link
+            assert st.sweep(oracle.SAMPLERS[sampler]) == 0
+            ref = literal_link_mass(oracle, m, x, file, y, z, link, st.theta, sampler)
+            assert (ref > 0).all()
+            assert_literal_mass(st.last_link_mass(), ref, f"{row} {sampler} sweep {it}")
