@@ -115,6 +115,11 @@ SIGNATURES = {
     "dbl_last_sweep_ms": (C.c_double, [vp]),
     "dbl_link_kernel_ms": (C.c_double, [vp, i64p]),
     "dbl_phase_ms": (C.c_int64, [vp, C.POINTER(C.c_double)]),
+    "dbl_posterior_create": (C.c_int, [C.POINTER(vp), C.c_int64, C.c_int32]),
+    "dbl_posterior_free": (None, [vp]),
+    "dbl_posterior_add_sample": (C.c_int, [vp, vp]),
+    "dbl_posterior_num_samples": (C.c_int32, [vp]),
+    "dbl_posterior_smpc": (C.c_int, [vp, i32p, f64p]),
     "dbl_version": (C.c_char_p, []),
 }
 

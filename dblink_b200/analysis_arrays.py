@@ -47,13 +47,13 @@ def read_chain_arrays(path, lower_iteration_cutoff=0):
     ids = pc.unique(first)
     samples = []
     for it in its:
-        mem, sizes, part = [], [], []
+        # one id lookup per sample over all its partitions: each index_in call hashes the R ids of the value set
+        idx = pc.index_in(pa.concat_arrays([cl.flatten() for _, cl in rows[it]]), value_set=ids)
+        if idx.null_count:
+            raise ValueError("a sample mentions a record id that the first sample does not")
+        mem = [idx.to_numpy(zero_copy_only=False).astype(np.int32)]
+        sizes, part = [], []
         for pid, cl in rows[it]:
-            flat = cl.flatten()
-            idx = pc.index_in(flat, value_set=ids)
-            if idx.null_count:
-                raise ValueError("a sample mentions a record id that the first sample does not")
-            mem.append(idx.to_numpy(zero_copy_only=False).astype(np.int32))
             off = cl.offsets.to_numpy().astype(np.int64)
             sz = np.diff(off)
             sizes.append(sz)

@@ -1,0 +1,93 @@
+"""Shared most probable clusters on the GPU (LinkageChain.scala:52-95) for chains of millions of records.
+
+Same results as analysis_arrays.shared_most_probable_clusters / most_probable_signature, bit for bit: the device
+computes the same 64-bit cluster signatures (dbl_posterior.cu), the same per-record mode with ties going to the
+earliest sample, and the same smallest-record-index labels.  The (S x R) signature matrix lives in device memory,
+filled one sample at a time; the host only turns each sample's (members, offsets) into a cluster label per record.
+"""
+import ctypes as C
+
+import numpy as np
+
+from . import _lib
+from .engine import DblinkError
+
+_STATUS = {_lib.ERR_INVALID: "invalid argument (bad size, label out of range or too many samples)",
+           _lib.ERR_CUDA: "CUDA failure (no device, or the signature matrix does not fit on it)",
+           _lib.ERR_STATE: "no sample added"}
+
+
+def _check(rc, what):
+    if rc == _lib.OK:
+        return
+    err = DblinkError(f"{what}: {_STATUS.get(rc, 'error %d' % rc)}")
+    err.status = rc
+    raise err
+
+
+def sample_clusters(num_records, members, offsets):
+    """One sample as int32 cluster[R]: the position of each record's cluster in (members, offsets)."""
+    R = num_records
+    members = np.asarray(members)
+    offsets = np.asarray(offsets, np.int64)
+    if len(members) != R or (R and (members.min() < 0 or members.max() >= R)):
+        raise ValueError("every sample must mention every record exactly once")
+    cluster = np.full(R, -1, np.int32)
+    cluster[members] = np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets))
+    if (cluster < 0).any():  # R members, one record missing: another is mentioned twice
+        raise ValueError("every sample must mention every record exactly once")
+    return cluster
+
+
+class Posterior:
+    """Owner of a dbl_posterior handle: samples go in one at a time, smpc() reads the summary."""
+
+    def __init__(self, num_records, max_samples):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        self.num_records = int(num_records)
+        _check(self._lib.dbl_posterior_create(C.byref(self._h), self.num_records, int(max_samples)),
+               "dbl_posterior_create")
+
+    def add_sample(self, cluster):
+        cluster = np.ascontiguousarray(cluster, np.int32)
+        if cluster.shape != (self.num_records,):
+            raise ValueError("a sample needs one cluster label per record")
+        _check(self._lib.dbl_posterior_add_sample(self._h, cluster.ctypes.data), "dbl_posterior_add_sample")
+
+    @property
+    def num_samples(self):
+        return self._lib.dbl_posterior_num_samples(self._h)
+
+    def smpc(self):
+        """(labels int64[R], freq float64[R])."""
+        labels = np.empty(self.num_records, np.int32)
+        freq = np.empty(self.num_records, np.float64)
+        _check(self._lib.dbl_posterior_smpc(self._h, labels.ctypes.data_as(_lib.i32p), freq.ctypes.data_as(_lib.f64p)),
+               "dbl_posterior_smpc")
+        return labels.astype(np.int64), freq
+
+    def close(self):
+        if self._h:
+            self._lib.dbl_posterior_free(self._h)
+            self._h = C.c_void_p()
+
+
+def most_probable_clusters(chain):
+    """(labels, freq) of a ChainArrays: labels = the sMPC labels (the smallest record index of each group of records
+    sharing their most probable cluster), freq = how often each record is in its most probable cluster."""
+    R = chain.num_records
+    if R == 0:
+        return np.zeros(0, np.int64), np.zeros(0)
+    post = Posterior(R, len(chain.samples))
+    try:
+        for mem, off, _ in chain.samples:
+            post.add_sample(sample_clusters(R, mem, off))
+        return post.smpc()
+    finally:
+        post.close()
+
+
+def shared_most_probable_clusters(chain):
+    """int64 labels[R], identical to analysis_arrays.shared_most_probable_clusters(chain)."""
+    return most_probable_clusters(chain)[0]

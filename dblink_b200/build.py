@@ -1,7 +1,8 @@
 """Builds libdblink_b200.so in-tree with nvcc for sm_90a (explicit nvcc; no JIT cache).
 
 Translation units: dbl_engine.cu (all kernels but the PCG-II link kernel), dbl_host.cpp (host-side model
-construction), and dbl_link_inst.cu compiled once per attribute count A = 1..16 (k_link_pcg2<A, 0..A>);
+construction), dbl_index_gpu.cu (attribute-index tables), dbl_posterior.cu (shared most probable clusters of a chain)
+and dbl_link_inst.cu compiled once per attribute count A = 1..16 (k_link_pcg2<A, 0..A>);
 objects are compiled in parallel and linked with `nvcc -shared`.
 """
 import os
@@ -40,7 +41,7 @@ def _deps():
 
 def units():
     u = [("dbl_engine.o", "dbl_engine.cu", []), ("dbl_host.o", "dbl_host.cpp", []),
-         ("dbl_index_gpu.o", "dbl_index_gpu.cu", [])]
+         ("dbl_index_gpu.o", "dbl_index_gpu.cu", []), ("dbl_posterior.o", "dbl_posterior.cu", [])]
     for a in range(1, MAX_A + 1):
         u.append((f"dbl_link_a{a}.o", "dbl_link_inst.cu", [f"-DDBL_INST_A={a}"]))
     return u

@@ -1,20 +1,29 @@
 """Project: a dblink configuration bound to its data (Project.scala:32-230, ProjectSteps.scala:53-84).
 
 Same HOCON surface as the reference (`dblink.data.*`, `dblink.partitioner`, `dblink.steps[*]`, ...); the sample
-step runs on the GPU engine, summarize / evaluate run on the host from linkage-chain.parquet.
+step runs on the GPU engine, summarize / evaluate read linkage-chain.parquet on the host and compute the shared most
+probable clusters on the GPU when there is one.
 """
 import os
 import shutil
 
 import numpy as np
 
-from . import analysis, analysis_arrays, config as hocon, sampler as chain, state_io, writers
+from . import _lib, analysis, analysis_arrays, analysis_gpu, config as hocon, sampler as chain, state_io, writers
 from .engine import GibbsEngine, KDTreePartitioner
 from .records import (Attribute, RecordsCache, SimilarityFn, build_cache_from_columns, read_csv,  # noqa: F401
                       read_csv_columns)
 
 SUPPORTED_METRICS = ("pairwise", "cluster")  # ProjectStep.scala:36
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters")  # :37
+
+
+def shared_most_probable_clusters(chain):
+    """sMPC labels of a ChainArrays: on the GPU when the platform has one (analysis_gpu), else on the host
+    (analysis_arrays).  Both give identical labels, so the output files do not depend on the platform."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.shared_most_probable_clusters(chain)
+    return analysis_arrays.shared_most_probable_clusters(chain)
 
 
 class Project:
@@ -256,7 +265,7 @@ class Project:
                     elif q == "partition-sizes":
                         writers.save_partition_sizes(analysis_arrays.partition_sizes(ch), self.output_path)
                     else:
-                        labels = analysis_arrays.shared_most_probable_clusters(ch)
+                        labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
             elif name == "evaluate":
                 true_labels = self.true_labels()
@@ -268,7 +277,7 @@ class Project:
                 if prm["use_existing_smpc"] and os.path.exists(smpc_path):  # ProjectStep.scala EvaluateStep
                     labels = self._read_smpc_labels(smpc_path, ch.record_ids)
                 else:
-                    labels = analysis_arrays.shared_most_probable_clusters(ch)
+                    labels = shared_most_probable_clusters(ch)
                     self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
                 truth = true_labels(ch.record_ids)
                 text = []

@@ -234,6 +234,28 @@ int dbl_download_owned(dbl_ctx *, int64_t *n_ent, int32_t *ent_ids, int32_t *y, 
 /* which entities / records this rank currently owns (host byte arrays of E and R entries) */
 int dbl_owned_masks(dbl_ctx *, uint8_t *ent_owned, uint8_t *rec_owned);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Posterior summary.  Replaces LinkageChain.mostProbableClusters / sharedMostProbableClusters
+ * (LinkageChain.scala:52-95): the shared most probable clusters (sMPC) of a chain, on the device that is current
+ * when dbl_posterior_create() is called (dbl_set_device).  Samples are fed one at a time as cluster[R], an int32 in
+ * [0, R) for every record (records with equal values share a cluster); the object keeps one 64-bit signature per
+ * (record, sample) -- sig = mix64(wrapping sum of mix64(r) over the cluster ^ mix64(cluster size)), splitmix64's
+ * finaliser -- in an R x max_samples device matrix.
+ *   dbl_posterior_add_sample  cluster may be a host or a device pointer (ready when the call is made); a label
+ *                             outside [0, R) or a sample beyond max_samples gives DBL_ERR_INVALID and adds nothing
+ *   dbl_posterior_smpc        per record the signature it carries most often (ties: the one seen in the earliest
+ *                             sample) and its frequency count / S (freq_out); records grouped by that signature, each
+ *                             labelled by the smallest record index of its group (labels_out); either may be NULL;
+ *                             DBL_ERR_STATE before the first sample
+ * DBL_ERR_CUDA: no device, or the signature matrix (8 R max_samples bytes) does not fit on it.
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct dbl_posterior dbl_posterior;
+int dbl_posterior_create(dbl_posterior **out, int64_t num_records, int32_t max_samples);
+void dbl_posterior_free(dbl_posterior *);
+int dbl_posterior_add_sample(dbl_posterior *, const int32_t *cluster /* R, host or device */);
+int32_t dbl_posterior_num_samples(const dbl_posterior *);
+int dbl_posterior_smpc(dbl_posterior *, int32_t *labels_out /* R, may be NULL */, double *freq_out /* R, may be NULL */);
+
 /* The protocol functions of the theta draw (DESIGN.md 4.5), exposed so that they can be checked without a GPU:
  * log / exp built from individually rounded binary64 operations, and updateDistProbs (GU:305-320) itself. */
 double dbl_det_log(double x);
