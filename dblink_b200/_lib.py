@@ -120,6 +120,12 @@ SIGNATURES = {
     "dbl_posterior_add_sample": (C.c_int, [vp, vp]),
     "dbl_posterior_num_samples": (C.c_int32, [vp]),
     "dbl_posterior_smpc": (C.c_int, [vp, i32p, f64p]),
+    "dbl_pairs_create": (C.c_int, [C.POINTER(vp), C.c_int64, C.c_int64]),
+    "dbl_pairs_free": (None, [vp]),
+    "dbl_pairs_add_sample": (C.c_int, [vp, vp]),
+    "dbl_pairs_num_samples": (C.c_int32, [vp]),
+    "dbl_pairs_count": (C.c_int, [vp, C.c_int32, i64p]),
+    "dbl_pairs_read": (C.c_int, [vp, C.c_int32, vp, vp, vp]),
     "dbl_version": (C.c_char_p, []),
 }
 

@@ -1,6 +1,7 @@
 """Posterior summaries of a linkage chain (host side; small inputs).
 
   most_probable_clusters / shared_most_probable_clusters  <- LinkageChain.scala:52-109
+  pairwise_match_probabilities                            <- posterior probability that two records are one entity
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
   pairwise_metrics                                        <- analysis/PairwiseMetrics.scala:44-63,
                                                              BinaryClassificationMetrics.scala:23-37
@@ -47,6 +48,18 @@ def shared_most_probable_clusters(chain_or_mpc):
     for r, (c, _) in mpc.items():
         groups[c].add(r)
     return [frozenset(v) for v in groups.values()]
+
+
+def pairwise_match_probabilities(chain):
+    """frozenset({id1, id2}) -> the fraction of samples in which the two records share a cluster, for every pair that
+    shares one in at least one sample."""
+    n = len({s[0] for s in chain})
+    count = collections.Counter()
+    for s in chain:
+        for c in clusters_of_sample(s):
+            for a, b in itertools.combinations(c, 2):
+                count[frozenset((a, b))] += 1
+    return {pair: k / n for pair, k in count.items()}
 
 
 def cluster_size_distribution(chain):

@@ -5,6 +5,7 @@ A sample is held as (members, offsets, partition_of_cluster): `members` = record
 dictionary) of all clusters back to back, `offsets[c]:offsets[c+1]` = cluster c.  The simple set-based functions in
 analysis.py stay as the readable restatement; tests compare the two on random chains.
 """
+import math
 import os
 
 import numpy as np
@@ -160,6 +161,71 @@ def shared_most_probable_clusters(chain):
     rep = np.full(inv.max() + 1 if len(inv) else 0, np.iinfo(np.int64).max, np.int64)
     np.minimum.at(rep, inv, np.arange(len(inv)))
     return rep[inv].astype(np.int64)
+
+
+# ---- posterior pairwise match probabilities ------------------------------------------------------------
+MAX_PAIRS = 1 << 28  # distinct record pairs a chain may put in a cluster (the GPU table: 12 bytes each, twice)
+
+
+def too_many_pairs(max_pairs):
+    return ValueError(f"the chain puts more than {max_pairs} distinct record pairs in a cluster")
+
+
+def min_match_count(threshold, num_samples):
+    """The smallest count c >= 1 with c / S >= threshold in float64, so that a pair is kept exactly when its
+    probability count / S is at least the threshold (threshold in [0, 1])."""
+    S = int(num_samples)
+    if S <= 0:
+        return 1
+    c = max(1, min(S, math.ceil(threshold * S)))
+    while c > 1 and (c - 1) / S >= threshold:
+        c -= 1
+    while c < S and c / S < threshold:
+        c += 1
+    return c
+
+
+def sample_pair_keys(num_records, members, offsets):
+    """Sorted int64 keys first << 32 | second (record indices, first < second) of the pairs of records that share a
+    cluster in one sample.  The record at position t of a cluster of k records (members in ascending index) is paired
+    with positions t+1 .. k-1: one row per record, generated without a loop over clusters."""
+    members = np.asarray(members)
+    sizes = np.diff(offsets).astype(np.int64)
+    n = len(members)
+    cl = np.repeat(np.arange(len(sizes), dtype=np.int64), sizes)
+    srt = np.sort(cl * num_records + members) - cl * num_records  # members of a cluster in ascending index
+    row = np.repeat(np.asarray(offsets[:-1], np.int64) + sizes, sizes) - 1 - np.arange(n)
+    row_off = np.r_[0, np.cumsum(row)]
+    shift = np.repeat(row_off[:-1] - np.arange(n) - 1, row)  # partner position = output index - shift
+    return np.sort((np.repeat(srt, row) << 32) | srt[np.arange(row_off[-1]) - shift])
+
+
+def pairwise_match_counts(chain, max_pairs=MAX_PAIRS, min_count=1):
+    """(first, second, count), int64: every pair of record indices (first < second, ascending (first, second) order)
+    that shares a cluster in at least min_count samples, and the number of samples in which it does.  The probability
+    that the two records are one entity is count / S.  Raises ValueError when the chain puts more than max_pairs
+    distinct pairs in a cluster; each sample's sum k(k-1)/2 is checked before its pairs are generated."""
+    R = chain.num_records
+    keys, cnt = np.zeros(0, np.int64), np.zeros(0, np.int64)
+    for mem, off, _ in chain.samples:
+        if len(mem) != R:
+            raise ValueError("every sample must mention every record exactly once")
+        if int(_comb2(np.diff(off)).sum()) > max_pairs:
+            raise too_many_pairs(max_pairs)
+        k = sample_pair_keys(R, mem, off)
+        pos = np.searchsorted(keys, k)
+        hit = np.zeros(len(k), bool)
+        inside = pos < len(keys)
+        hit[inside] = keys[pos[inside]] == k[inside]
+        new = ~hit
+        if len(keys) + int(new.sum()) > max_pairs:
+            raise too_many_pairs(max_pairs)
+        cnt[pos[hit]] += 1  # a sample's keys are distinct, so are their positions
+        keys = np.insert(keys, pos[new], k[new])
+        cnt = np.insert(cnt, pos[new], 1)
+    keep = cnt >= min_count
+    keys, cnt = keys[keep], cnt[keep]
+    return keys >> 32, keys & 0xFFFFFFFF, cnt
 
 
 def labels_to_clusters(labels, record_ids=None):

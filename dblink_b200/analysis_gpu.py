@@ -1,19 +1,23 @@
-"""Shared most probable clusters on the GPU (LinkageChain.scala:52-95) for chains of millions of records.
+"""Posterior summaries of chains of millions of records on the GPU: the shared most probable clusters
+(LinkageChain.scala:52-95) and the pairwise match counts.
 
 Same results as analysis_arrays.shared_most_probable_clusters / most_probable_signature, bit for bit: the device
 computes the same 64-bit cluster signatures (dbl_posterior.cu), the same per-record mode with ties going to the
 earliest sample, and the same smallest-record-index labels.  The (S x R) signature matrix lives in device memory,
 filled one sample at a time; the host only turns each sample's (members, offsets) into a cluster label per record.
+The pairwise match counts equal analysis_arrays.pairwise_match_counts exactly: the device keeps the sorted table of
+(pair, count) and merges each sample's pairs into it.
 """
 import ctypes as C
 
 import numpy as np
 
 from . import _lib
+from .analysis_arrays import MAX_PAIRS, too_many_pairs
 from .engine import DblinkError
 
-_STATUS = {_lib.ERR_INVALID: "invalid argument (bad size, label out of range or too many samples)",
-           _lib.ERR_CUDA: "CUDA failure (no device, or the signature matrix does not fit on it)",
+_STATUS = {_lib.ERR_INVALID: "invalid argument (bad size, label out of range, too many samples or pairs)",
+           _lib.ERR_CUDA: "CUDA failure (no device, or a device buffer does not fit on it)",
            _lib.ERR_STATE: "no sample added"}
 
 
@@ -91,3 +95,61 @@ def most_probable_clusters(chain):
 def shared_most_probable_clusters(chain):
     """int64 labels[R], identical to analysis_arrays.shared_most_probable_clusters(chain)."""
     return most_probable_clusters(chain)[0]
+
+
+class Pairs:
+    """Owner of a dbl_pairs handle: samples go in one at a time, read() gives the pairwise match counts."""
+
+    def __init__(self, num_records, max_pairs=MAX_PAIRS):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        self.num_records = int(num_records)
+        _check(self._lib.dbl_pairs_create(C.byref(self._h), self.num_records, int(max_pairs)), "dbl_pairs_create")
+
+    def add_sample(self, cluster):
+        cluster = np.ascontiguousarray(cluster, np.int32)
+        if cluster.shape != (self.num_records,):
+            raise ValueError("a sample needs one cluster label per record")
+        _check(self._lib.dbl_pairs_add_sample(self._h, cluster.ctypes.data), "dbl_pairs_add_sample")
+
+    @property
+    def num_samples(self):
+        return self._lib.dbl_pairs_num_samples(self._h)
+
+    def count(self, min_count=1):
+        n = C.c_int64()
+        _check(self._lib.dbl_pairs_count(self._h, int(min_count), C.byref(n)), "dbl_pairs_count")
+        return n.value
+
+    def read(self, min_count=1):
+        """(first, second, count), int64, the pairs with count >= min_count in ascending (first, second) order."""
+        n = self.count(min_count)
+        out = [np.empty(n, np.int32) for _ in range(3)]
+        if n:
+            _check(self._lib.dbl_pairs_read(self._h, int(min_count), *(a.ctypes.data for a in out)), "dbl_pairs_read")
+        return tuple(a.astype(np.int64) for a in out)
+
+    def close(self):
+        if self._h:
+            self._lib.dbl_pairs_free(self._h)
+            self._h = C.c_void_p()
+
+
+def pairwise_match_counts(chain, max_pairs=MAX_PAIRS, min_count=1):
+    """(first, second, count), identical to analysis_arrays.pairwise_match_counts(chain, max_pairs, min_count)."""
+    R = chain.num_records
+    if R == 0 or not chain.samples:
+        return tuple(np.zeros(0, np.int64) for _ in range(3))
+    pairs = Pairs(R, max_pairs)
+    try:
+        for mem, off, _ in chain.samples:
+            cluster = sample_clusters(R, mem, off)  # the labels are valid, so DBL_ERR_INVALID below means the cap
+            try:
+                pairs.add_sample(cluster)
+            except DblinkError as e:
+                if e.status == _lib.ERR_INVALID:
+                    raise too_many_pairs(max_pairs) from e
+                raise
+        return pairs.read(min_count)
+    finally:
+        pairs.close()

@@ -11,6 +11,11 @@
 //   * the sMPC label of a record is the smallest record index among the records with the same best signature.
 // Signatures live in a record-major device matrix [R][max_samples]; the mode runs over blocks of records, each a
 // stable segmented radix sort of (signature, sample index) pairs followed by one scan per record.
+//
+// Posterior pairwise match counts (dbl_pairs_*, same numbers as analysis_arrays.pairwise_match_counts): for every
+// unordered pair of records the number of samples in which they share a cluster.  The handle holds a sorted table of
+// (first << 32 | second, count) over the pairs seen so far; each sample's pairs are generated, sorted and merged into
+// it -- see dbl_pairs_add_sample.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -296,5 +301,356 @@ extern "C" int dbl_posterior_smpc(dbl_posterior *p, int32_t *labels_out, double 
   POST_TRY(cudaGetLastError());
   POST_TRY(cudaMemcpyAsync(labels_out, labels.p, sizeof(int32_t) * R, cudaMemcpyDeviceToHost, st));
   POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
+// ---- posterior pairwise match counts -------------------------------------------------------------------------------
+namespace {
+constexpr int WARPS_PER_BLOCK = THREADS / 32;
+
+// bits needed to hold every value in [0, n)
+int bits_for(int64_t n) {
+  int b = 1;
+  while (b < 62 && (int64_t(1) << b) < n) ++b;
+  return b;
+}
+
+__device__ __forceinline__ int64_t lower_bound_u64(const unsigned long long *__restrict__ a, int64_t n,
+                                                   unsigned long long key) {
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (a[mid] < key) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// records sorted stably by label: position of every run head (cluster start), 0 elsewhere; a max-scan then gives
+// every position the start of its cluster
+__global__ void k_label_heads(int64_t R, const int32_t *__restrict__ lab, int32_t *__restrict__ head) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x)
+    head[i] = (i == 0 || lab[i] != lab[i - 1]) ? (int32_t)i : 0;
+}
+
+// the last position of each cluster writes the cluster's size at its first position
+__global__ void k_cluster_sizes(int64_t R, const int32_t *__restrict__ lab, const int32_t *__restrict__ start,
+                                int32_t *__restrict__ size_at_start) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x)
+    if (i == R - 1 || lab[i] != lab[i + 1]) size_at_start[start[i]] = (int32_t)(i - start[i] + 1);
+}
+
+// row length of every sorted position: its partners are the later positions of its cluster; entry R is 0, so an
+// exclusive scan over R + 1 entries ends with the sample's pair count
+__global__ void k_row_lengths(int64_t R, const int32_t *__restrict__ start, const int32_t *__restrict__ size_at_start,
+                              long long *__restrict__ row) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= R; i += (int64_t)gridDim.x * blockDim.x)
+    row[i] = i < R ? (long long)start[i] + size_at_start[start[i]] - 1 - i : 0;
+}
+
+// one warp per sorted position writes that record's row of partners at its int64 offset: a cluster of k records is
+// spread over k warps, whatever k is.  Members of a cluster are in ascending record index (the label sort is
+// stable), so first < second.
+__global__ void k_emit_pairs(int64_t R, const int32_t *__restrict__ rec, const long long *__restrict__ off,
+                             unsigned long long *__restrict__ keys) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * WARPS_PER_BLOCK;
+  for (int64_t w = blockIdx.x * (int64_t)WARPS_PER_BLOCK + (threadIdx.x >> 5); w < R; w += nwarps) {
+    const long long o = off[w], n = off[w + 1] - o;
+    if (n == 0) continue;
+    const unsigned long long hi = (unsigned long long)(uint32_t)rec[w] << 32;
+    for (long long j = lane; j < n; j += 32) keys[o + j] = hi | (uint32_t)rec[w + 1 + j];
+  }
+}
+
+// 1 for a sample key the held table does not have yet; entry n is 0, so an exclusive scan gives every new key its
+// rank among the new ones and ends with their number
+__global__ void k_probe_new(int64_t n, const unsigned long long *__restrict__ keys, int64_t H,
+                            const unsigned long long *__restrict__ held, int32_t *__restrict__ is_new) {
+  for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j <= n; j += (int64_t)gridDim.x * blockDim.x) {
+    if (j == n) {
+      is_new[j] = 0;
+      continue;
+    }
+    const unsigned long long k = keys[j];
+    const int64_t b = lower_bound_u64(held, H, k);
+    is_new[j] = !(b < H && held[b] == k);
+  }
+}
+
+// merge, held side: an entry moves up by the number of new keys below it, and counts one more if the sample has it
+__global__ void k_merge_held(int64_t H, const unsigned long long *__restrict__ held, const int32_t *__restrict__ hcnt,
+                             int64_t n, const unsigned long long *__restrict__ keys, const int32_t *__restrict__ rank,
+                             unsigned long long *__restrict__ out_key, int32_t *__restrict__ out_cnt) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < H; i += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long k = held[i];
+    const int64_t lb = lower_bound_u64(keys, n, k);
+    const int64_t pos = i + rank[lb];
+    out_key[pos] = k;
+    out_cnt[pos] = hcnt[i] + (lb < n && keys[lb] == k);
+  }
+}
+
+// merge, sample side: a new key lands after the held entries below it and the new keys before it, with count 1
+__global__ void k_merge_new(int64_t n, const unsigned long long *__restrict__ keys, const int32_t *__restrict__ is_new,
+                            const int32_t *__restrict__ rank, int64_t H, const unsigned long long *__restrict__ held,
+                            unsigned long long *__restrict__ out_key, int32_t *__restrict__ out_cnt) {
+  for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+    if (!is_new[j]) continue;
+    const unsigned long long k = keys[j];
+    const int64_t pos = lower_bound_u64(held, H, k) + rank[j];
+    out_key[pos] = k;
+    out_cnt[pos] = 1;
+  }
+}
+
+__global__ void k_flag_min_count(int64_t H, const int32_t *__restrict__ cnt, int32_t min_count,
+                                 int32_t *__restrict__ flag) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= H; i += (int64_t)gridDim.x * blockDim.x)
+    flag[i] = i < H && cnt[i] >= min_count;
+}
+
+__global__ void k_scatter_pairs(int64_t H, const unsigned long long *__restrict__ key, const int32_t *__restrict__ cnt,
+                                const int32_t *__restrict__ flag, const int32_t *__restrict__ pos,
+                                int32_t *__restrict__ first, int32_t *__restrict__ second, int32_t *__restrict__ count) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < H; i += (int64_t)gridDim.x * blockDim.x) {
+    if (!flag[i]) continue;
+    const int32_t p = pos[i];
+    first[p] = (int32_t)(key[i] >> 32);
+    second[p] = (int32_t)(key[i] & 0xffffffffull);
+    count[p] = cnt[i];
+  }
+}
+
+// a device buffer that only grows: to at least twice its size, at most `limit` bytes unless more is needed.  A new
+// allocation replaces the old one only once it has succeeded.
+struct Grow {
+  Buf buf;
+  size_t cap = 0;
+  cudaError_t reserve(size_t need, size_t limit = SIZE_MAX) {
+    if (need <= cap) return cudaSuccess;
+    const size_t bytes = std::max(need, std::min(limit, cap > SIZE_MAX / 2 ? SIZE_MAX : 2 * cap));
+    Buf nb;
+    const cudaError_t e = nb.alloc(bytes);
+    if (e != cudaSuccess) return e;
+    std::swap(buf.p, nb.p);  // nb now frees the old buffer
+    cap = bytes;
+    return cudaSuccess;
+  }
+  template <class T> T *as() const { return buf.as<T>(); }
+};
+}  // namespace
+
+struct dbl_pairs {
+  int device = 0;
+  int64_t R = 0, max_pairs = 0, H = 0;  // H = distinct pairs held
+  int32_t S = 0;
+  int lab_bits = 1, key_bits = 33;      // radix sort end bits of the labels and of the pair keys
+  cudaStream_t stream = nullptr;
+  Buf cluster, bad;                     // the sample's labels, label check flag
+  Buf iota, lab_s, rec_s;               // record indices; labels and records sorted by label
+  Buf head, start, size;                // run heads, cluster start per position, cluster size at its start
+  Buf row, off;                         // int64 row lengths and their exclusive scan, R + 1 each
+  Grow key_in, key_s, is_new, rank;     // the sample's pair keys (unsorted, sorted) and their merge ranks
+  Grow tab_key[2], tab_cnt[2];          // held table (index cur) and the one the next sample merges into
+  int cur = 0;
+  Grow tmp;                             // CUB temporary storage
+};
+
+extern "C" int dbl_pairs_create(dbl_pairs **out, int64_t num_records, int64_t max_pairs) {
+  if (!out) return DBL_ERR_INVALID;
+  *out = nullptr;
+  if (num_records <= 0 || num_records > INT32_MAX || max_pairs <= 0 || max_pairs > INT32_MAX) return DBL_ERR_INVALID;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return DBL_ERR_CUDA; }
+  auto *p = new dbl_pairs();
+  const int64_t R = num_records;
+  p->R = R;
+  p->max_pairs = max_pairs;
+  p->lab_bits = bits_for(R);
+  p->key_bits = 32 + bits_for(R);
+  const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(long long) * (size_t)(R + 1);
+  if (cudaGetDevice(&p->device) != cudaSuccess ||
+      cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking) != cudaSuccess || p->cluster.alloc(r4) != cudaSuccess ||
+      p->bad.alloc(sizeof(int)) != cudaSuccess || p->iota.alloc(r4) != cudaSuccess || p->lab_s.alloc(r4) != cudaSuccess ||
+      p->rec_s.alloc(r4) != cudaSuccess || p->head.alloc(r4) != cudaSuccess || p->start.alloc(r4) != cudaSuccess ||
+      p->size.alloc(r4) != cudaSuccess || p->row.alloc(r8) != cudaSuccess || p->off.alloc(r8) != cudaSuccess) {
+    cudaGetLastError();
+    dbl_pairs_free(p);
+    return DBL_ERR_CUDA;
+  }
+  k_iota<<<grid_for(R), THREADS, 0, p->stream>>>(R, p->iota.as<int32_t>());
+  if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(p->stream) != cudaSuccess) {
+    cudaGetLastError();
+    dbl_pairs_free(p);
+    return DBL_ERR_CUDA;
+  }
+  *out = p;
+  return DBL_OK;
+}
+
+extern "C" void dbl_pairs_free(dbl_pairs *p) {
+  if (!p) return;
+  DeviceScope ds(p->device);
+  if (p->stream) {
+    cudaStreamSynchronize(p->stream);
+    cudaStreamDestroy(p->stream);
+  }
+  delete p;
+}
+
+extern "C" int32_t dbl_pairs_num_samples(const dbl_pairs *p) { return p ? p->S : 0; }
+
+// One sample: check the labels; stable radix sort of (label, record); cluster starts and sizes; every position's row
+// of partners and its int64 offset, whose total is the sample's pair count sum k(k-1)/2; refuse before allocating
+// anything for the pairs if that count alone exceeds max_pairs; emit the keys; radix-sort them; merge them into the
+// spare table (a binary search per key on either side gives its place); commit by swapping tables only if the union
+// fits max_pairs.  A refusal or failure leaves the held table and S as they were.
+extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
+  if (!p || !cluster || p->S == INT32_MAX) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  const int64_t R = p->R, H = p->H;
+  cudaStream_t st = p->stream;
+  POST_TRY(cudaMemcpyAsync(p->cluster.p, cluster, sizeof(int32_t) * R, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemsetAsync(p->bad.p, 0, sizeof(int), st));
+  k_check_labels<<<grid_for(R), THREADS, 0, st>>>(R, p->cluster.as<int32_t>(), p->bad.as<int>());
+  int bad = 0;
+  POST_TRY(cudaMemcpyAsync(&bad, p->bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaStreamSynchronize(st));
+  if (bad) return DBL_ERR_INVALID;
+
+  // records grouped by label, ascending record index within a cluster
+  size_t tb_sort = 0, tb_max = 0, tb_sum = 0;
+  POST_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb_sort, (const int32_t *)nullptr, (int32_t *)nullptr,
+                                           (const int32_t *)nullptr, (int32_t *)nullptr, R, 0, p->lab_bits, st));
+  POST_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb_max, (const int32_t *)nullptr, (int32_t *)nullptr, MaxOp(), R, st));
+  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb_sum, (const long long *)nullptr, (long long *)nullptr, R + 1, st));
+  POST_TRY(p->tmp.reserve(std::max({tb_sort, tb_max, tb_sum})));
+  size_t tb = p->tmp.cap;
+  POST_TRY(cub::DeviceRadixSort::SortPairs(p->tmp.buf.p, tb, p->cluster.as<int32_t>(), p->lab_s.as<int32_t>(),
+                                           p->iota.as<int32_t>(), p->rec_s.as<int32_t>(), R, 0, p->lab_bits, st));
+  k_label_heads<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_s.as<int32_t>(), p->head.as<int32_t>());
+  tb = p->tmp.cap;
+  POST_TRY(cub::DeviceScan::InclusiveScan(p->tmp.buf.p, tb, p->head.as<int32_t>(), p->start.as<int32_t>(), MaxOp(), R,
+                                          st));
+  k_cluster_sizes<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_s.as<int32_t>(), p->start.as<int32_t>(),
+                                                   p->size.as<int32_t>());
+  k_row_lengths<<<grid_for(R + 1), THREADS, 0, st>>>(R, p->start.as<int32_t>(), p->size.as<int32_t>(),
+                                                     p->row.as<long long>());
+  tb = p->tmp.cap;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(p->tmp.buf.p, tb, p->row.as<long long>(), p->off.as<long long>(), R + 1, st));
+  long long n = 0;
+  POST_TRY(cudaMemcpyAsync(&n, p->off.as<long long>() + R, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  if (n > p->max_pairs) return DBL_ERR_INVALID;  // this sample alone: nothing allocated for its pairs
+
+  // the sample's keys, sorted
+  const size_t cap8 = sizeof(unsigned long long) * (size_t)p->max_pairs, cap4 = sizeof(int32_t) * (size_t)(p->max_pairs + 1);
+  POST_TRY(p->key_in.reserve(sizeof(unsigned long long) * (size_t)n, cap8));
+  POST_TRY(p->key_s.reserve(sizeof(unsigned long long) * (size_t)n, cap8));
+  POST_TRY(p->is_new.reserve(sizeof(int32_t) * (size_t)(n + 1), cap4));
+  POST_TRY(p->rank.reserve(sizeof(int32_t) * (size_t)(n + 1), cap4));
+  const unsigned long long *keys = p->key_s.as<unsigned long long>();
+  if (n > 0) {
+    k_emit_pairs<<<(int)std::min<int64_t>((R + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, 8192), THREADS, 0, st>>>(
+        R, p->rec_s.as<int32_t>(), p->off.as<long long>(), p->key_in.as<unsigned long long>());
+    size_t tbk = 0;
+    POST_TRY(cub::DeviceRadixSort::SortKeys(nullptr, tbk, (const unsigned long long *)nullptr,
+                                            (unsigned long long *)nullptr, (int64_t)n, 0, p->key_bits, st));
+    POST_TRY(p->tmp.reserve(tbk));
+    tbk = p->tmp.cap;
+    POST_TRY(cub::DeviceRadixSort::SortKeys(p->tmp.buf.p, tbk, p->key_in.as<unsigned long long>(),
+                                            p->key_s.as<unsigned long long>(), (int64_t)n, 0, p->key_bits, st));
+  }
+
+  // which keys are new, and their ranks among the new ones
+  const unsigned long long *held = p->tab_key[p->cur].as<unsigned long long>();
+  const int32_t *hcnt = p->tab_cnt[p->cur].as<int32_t>();
+  k_probe_new<<<grid_for(n + 1), THREADS, 0, st>>>(n, keys, H, held, p->is_new.as<int32_t>());
+  size_t tbr = 0;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tbr, (const int32_t *)nullptr, (int32_t *)nullptr, (int64_t)n + 1,
+                                         st));
+  POST_TRY(p->tmp.reserve(tbr));
+  tbr = p->tmp.cap;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(p->tmp.buf.p, tbr, p->is_new.as<int32_t>(), p->rank.as<int32_t>(),
+                                         (int64_t)n + 1, st));
+  int32_t fresh = 0;
+  POST_TRY(cudaMemcpyAsync(&fresh, p->rank.as<int32_t>() + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  const int64_t H2 = H + fresh;
+  if (H2 > p->max_pairs) return DBL_ERR_INVALID;  // the union does not fit: the held table stays as it is
+
+  // merge into the spare table, then commit
+  const int nxt = p->cur ^ 1;
+  POST_TRY(p->tab_key[nxt].reserve(sizeof(unsigned long long) * (size_t)H2, cap8));
+  POST_TRY(p->tab_cnt[nxt].reserve(sizeof(int32_t) * (size_t)H2, sizeof(int32_t) * (size_t)p->max_pairs));
+  unsigned long long *ok = p->tab_key[nxt].as<unsigned long long>();
+  int32_t *oc = p->tab_cnt[nxt].as<int32_t>();
+  if (H > 0)
+    k_merge_held<<<grid_for(H), THREADS, 0, st>>>(H, held, hcnt, n, keys, p->rank.as<int32_t>(), ok, oc);
+  if (n > 0)
+    k_merge_new<<<grid_for(n), THREADS, 0, st>>>(n, keys, p->is_new.as<int32_t>(), p->rank.as<int32_t>(), H, held, ok,
+                                                 oc);
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  p->cur = nxt;
+  p->H = H2;
+  ++p->S;
+  return DBL_OK;
+}
+
+// the held pairs with count >= min_count, in table (ascending key) order: into device arrays when first != NULL
+static int pairs_select(dbl_pairs *p, int32_t min_count, int64_t *n_out, int32_t *first, int32_t *second,
+                        int32_t *count) {
+  if (!p || !n_out) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  const int64_t H = p->H;
+  cudaStream_t st = p->stream;
+  Buf flag, pos, tmp;
+  POST_TRY(flag.alloc(sizeof(int32_t) * (H + 1)));
+  POST_TRY(pos.alloc(sizeof(int32_t) * (H + 1)));
+  size_t tb = 0;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, (const int32_t *)nullptr, (int32_t *)nullptr, H + 1, st));
+  POST_TRY(tmp.alloc(tb));
+  const int32_t *cnt = p->tab_cnt[p->cur].as<int32_t>();
+  k_flag_min_count<<<grid_for(H + 1), THREADS, 0, st>>>(H, cnt, min_count, flag.as<int32_t>());
+  POST_TRY(cub::DeviceScan::ExclusiveSum(tmp.p, tb, flag.as<int32_t>(), pos.as<int32_t>(), H + 1, st));
+  int32_t n = 0;
+  POST_TRY(cudaMemcpyAsync(&n, pos.as<int32_t>() + H, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  *n_out = n;
+  if (!first || n == 0 || H == 0) return DBL_OK;
+  k_scatter_pairs<<<grid_for(H), THREADS, 0, st>>>(H, p->tab_key[p->cur].as<unsigned long long>(), cnt,
+                                                   flag.as<int32_t>(), pos.as<int32_t>(), first, second, count);
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
+extern "C" int dbl_pairs_count(dbl_pairs *p, int32_t min_count, int64_t *n_out) {
+  return pairs_select(p, min_count, n_out, nullptr, nullptr, nullptr);
+}
+
+extern "C" int dbl_pairs_read(dbl_pairs *p, int32_t min_count, int32_t *first, int32_t *second, int32_t *count) {
+  if (!p || !first || !second || !count) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  int64_t n = 0;
+  int rc = dbl_pairs_count(p, min_count, &n);
+  if (rc != DBL_OK || n == 0) return rc;
+  Buf f, s, c;
+  POST_TRY(f.alloc(sizeof(int32_t) * n));
+  POST_TRY(s.alloc(sizeof(int32_t) * n));
+  POST_TRY(c.alloc(sizeof(int32_t) * n));
+  rc = pairs_select(p, min_count, &n, f.as<int32_t>(), s.as<int32_t>(), c.as<int32_t>());
+  if (rc != DBL_OK) return rc;
+  // host or device outputs: unified addressing picks the copy direction
+  POST_TRY(cudaMemcpy(first, f.p, sizeof(int32_t) * n, cudaMemcpyDefault));
+  POST_TRY(cudaMemcpy(second, s.p, sizeof(int32_t) * n, cudaMemcpyDefault));
+  POST_TRY(cudaMemcpy(count, c.p, sizeof(int32_t) * n, cudaMemcpyDefault));
   return DBL_OK;
 }

@@ -15,7 +15,8 @@ from .records import (Attribute, RecordsCache, SimilarityFn, build_cache_from_co
                       read_csv_columns)
 
 SUPPORTED_METRICS = ("pairwise", "cluster")  # ProjectStep.scala:36
-SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters")  # :37
+SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
+                        "pairwise-match-probabilities")
 
 
 def shared_most_probable_clusters(chain):
@@ -24,6 +25,14 @@ def shared_most_probable_clusters(chain):
     if _lib.load().dbl_device_count() > 0:
         return analysis_gpu.shared_most_probable_clusters(chain)
     return analysis_arrays.shared_most_probable_clusters(chain)
+
+
+def pairwise_match_counts(chain, min_count=1):
+    """(first, second, count) of a ChainArrays, the pairs that share a cluster in at least min_count samples: on the
+    GPU when the platform has one (analysis_gpu), else on the host (analysis_arrays).  Both give identical arrays."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.pairwise_match_counts(chain, min_count=min_count)
+    return analysis_arrays.pairwise_match_counts(chain, min_count=min_count)
 
 
 class Project:
@@ -222,8 +231,12 @@ class Project:
                 q = list(prm["quantities"])
                 if not q or any(x not in SUPPORTED_QUANTITIES for x in q):
                     raise ValueError(f"quantities must be one of {SUPPORTED_QUANTITIES}.")
+                # minMatchProbability: pairwise-match-probabilities.csv keeps the pairs at least this probable
+                t = float(prm.get("minMatchProbability", 0.0))
+                if not 0.0 <= t <= 1.0:
+                    raise ValueError("minMatchProbability must be in [0, 1].")
                 out.append(("summarize", dict(lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)),
-                                              quantities=q)))
+                                              quantities=q, min_match_probability=t)))
             elif name == "evaluate":
                 m = list(prm["metrics"])
                 if not m or any(x not in SUPPORTED_METRICS for x in m):
@@ -264,6 +277,11 @@ class Project:
                                                                self.output_path)
                     elif q == "partition-sizes":
                         writers.save_partition_sizes(analysis_arrays.partition_sizes(ch), self.output_path)
+                    elif q == "pairwise-match-probabilities":
+                        S, t = len(ch.samples), prm["min_match_probability"]
+                        first, second, count = pairwise_match_counts(ch, min_count=analysis_arrays.min_match_count(t, S))
+                        writers.save_pairwise_match_probabilities(first, second, count, S, ch.record_ids, t,
+                                                                  self.output_path)
                     else:
                         labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))

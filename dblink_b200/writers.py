@@ -4,6 +4,7 @@
                       linkageStructure:list<list<string>> (package.scala:94-96, util/BufferedRDDWriter.scala:44-50)
   DiagnosticsWriter   diagnostics.csv with the header of DiagnosticsWriter.scala:39-45 and rows of :47-72
   save_cluster_size_distribution / save_partition_sizes   LinkageChain.scala:162-211
+  save_pairwise_match_probabilities   pairwise-match-probabilities.csv: recordId1,recordId2,probability
 """
 import os
 import time
@@ -165,3 +166,39 @@ def save_partition_sizes(sizes, path):
         fh.write("iteration," + ",".join(str(p) for p in pids) + "\n")
         for it in its:
             fh.write(str(it) + "," + ",".join(str(sizes[it].get(p, 0)) for p in pids) + "\n")
+
+
+def save_pairwise_match_probabilities(first, second, count, num_samples, record_ids, threshold, path):
+    """pairwise-match-probabilities.csv under `path`: header recordId1,recordId2,probability, then one row per pair
+    with count / S >= threshold (float64; the row's text parses back to exactly count / S).  In a row recordId1 <
+    recordId2 in code-point order; rows go by probability descending, then recordId1, then recordId2.  The R ids are
+    ranked once and the rows sorted on integer ranks; the rows are joined by Arrow, not by a Python loop."""
+    import pyarrow as pa
+    import pyarrow.compute as pc
+
+    from .analysis_arrays import min_match_count
+
+    S = int(num_samples)
+    with open(os.path.join(path, "pairwise-match-probabilities.csv"), "wb") as fh:
+        fh.write(b"recordId1,recordId2,probability\n")
+        if S == 0:
+            return
+        count = np.asarray(count, np.int64)
+        keep = count >= min_match_count(threshold, S)
+        first, second, count = np.asarray(first)[keep], np.asarray(second)[keep], count[keep]
+        ids = record_ids if isinstance(record_ids, pa.Array) else pa.array([str(r) for r in record_ids], pa.string())
+        ids = ids.cast(pa.large_string())
+        rank = np.empty(len(ids), np.int64)
+        rank[pc.sort_indices(ids).to_numpy()] = np.arange(len(ids))  # UTF-8 byte order = code-point order
+        swap = rank[first] > rank[second]
+        r1, r2 = np.where(swap, second, first), np.where(swap, first, second)
+        order = np.lexsort((rank[r2], rank[r1], -count))
+        r1, r2, count = r1[order], r2[order], count[order]
+        # repr: the shortest text that parses back to the same float64; one per possible count
+        text = pa.array([repr(c / S) + "\n" for c in range(S + 1)], pa.large_string())
+        step = 1 << 20
+        for lo in range(0, len(count), step):
+            rows = pc.binary_join_element_wise(ids.take(r1[lo:lo + step]), ids.take(r2[lo:lo + step]),
+                                               text.take(count[lo:lo + step]), pa.scalar(",", pa.large_string()))
+            offs = np.frombuffer(rows.buffers()[1], np.int64)[rows.offset:rows.offset + len(rows) + 1]
+            fh.write(memoryview(rows.buffers()[2])[offs[0]:offs[-1]])

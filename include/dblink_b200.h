@@ -256,6 +256,33 @@ int dbl_posterior_add_sample(dbl_posterior *, const int32_t *cluster /* R, host 
 int32_t dbl_posterior_num_samples(const dbl_posterior *);
 int dbl_posterior_smpc(dbl_posterior *, int32_t *labels_out /* R, may be NULL */, double *freq_out /* R, may be NULL */);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Posterior pairwise match probabilities: for every unordered pair of records {a, b} that share a cluster in at least
+ * one sample, count(a, b) = the number of samples in which they do (the probability is count / S), on the device that
+ * is current when dbl_pairs_create() is called.  Samples are fed one at a time as cluster[R], as for dbl_posterior_*.
+ * The object holds a sorted table of (first << 32 | second, int32 count) over the distinct pairs seen so far, at most
+ * max_pairs of them (12 bytes each, twice: the table and the one the next sample merges into; the buffers grow on
+ * demand, nothing is allocated up front for the cap).
+ *   dbl_pairs_add_sample  cluster may be a host or a device pointer (ready when the call is made); the sample's pairs
+ *                         (sum over its clusters of k(k-1)/2, counted in int64) are generated, radix-sorted and merged
+ *                         into the table.  DBL_ERR_INVALID, adding nothing: a label outside [0, R); a sample whose pairs
+ *                         alone exceed max_pairs (checked before anything is allocated for them); a sample whose pairs,
+ *                         together with those already held, exceed max_pairs distinct pairs; S reaching INT32_MAX
+ *   dbl_pairs_count       the number of held pairs with count >= min_count
+ *   dbl_pairs_read        those pairs, in ascending (first, second) order, first < second (record indices), with
+ *                         their counts; the three arrays (dbl_pairs_count entries) may be host or device pointers
+ *   count / read before the first sample give DBL_ERR_STATE.
+ * DBL_ERR_INVALID: num_records or max_pairs outside [1, 2^31 - 1].  DBL_ERR_CUDA: no device, or an allocation that
+ * fails (the held table and the sample count stay as they were).
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct dbl_pairs dbl_pairs;
+int dbl_pairs_create(dbl_pairs **out, int64_t num_records, int64_t max_pairs);
+void dbl_pairs_free(dbl_pairs *);
+int dbl_pairs_add_sample(dbl_pairs *, const int32_t *cluster /* R, host or device */);
+int32_t dbl_pairs_num_samples(const dbl_pairs *);
+int dbl_pairs_count(dbl_pairs *, int32_t min_count, int64_t *n_out);
+int dbl_pairs_read(dbl_pairs *, int32_t min_count, int32_t *first, int32_t *second, int32_t *count);
+
 /* The protocol functions of the theta draw (DESIGN.md 4.5), exposed so that they can be checked without a GPU:
  * log / exp built from individually rounded binary64 operations, and updateDistProbs (GU:305-320) itself. */
 double dbl_det_log(double x);
