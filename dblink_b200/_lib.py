@@ -78,6 +78,12 @@ SIGNATURES = {
     "dbl_num_records": (C.c_int64, [vp]),
     "dbl_num_entities": (C.c_int64, [vp]),
     "dbl_iteration": (C.c_int64, [vp]),
+    "dbl_chains_init": (C.c_int, [vp, C.c_int32, u64p, C.c_int64, i32p, i32p, C.c_int64]),
+    "dbl_chains_upload": (C.c_int, [vp, C.c_int32, u64p, C.c_int64, C.c_int64, i32p, i32p, u8p, i32p, i32p, f64p,
+                                    C.c_int64]),
+    "dbl_num_chains": (C.c_int32, [vp]),
+    "dbl_chains_download": (C.c_int, [vp, u8p, i32p, i32p, f64p, i32p]),
+    "dbl_chain_summary": (C.c_int, [vp, C.c_int32, C.POINTER(SummaryHead), i64p, i64p, f64p]),
     "dbl_sweep": (C.c_int, [vp, C.c_int, C.c_int32]),
     "dbl_links_download": (C.c_int, [vp, i32p, i32p]),
     "dbl_summary": (C.c_int, [vp, C.POINTER(SummaryHead), i64p, i64p, f64p]),

@@ -67,6 +67,33 @@ def read_chain_arrays(path, lower_iteration_cutoff=0):
     return ChainArrays(ids, np.asarray(its, np.int64), samples)
 
 
+def read_pooled_chain_arrays(paths, lower_iteration_cutoff=0):
+    """The samples of several chains (one linkage-chain.parquet each) at or after the cutoff, pooled into ONE
+    ChainArrays: chain-major, then by iteration (the order that defines the sMPC tie rule "earliest sample").  Every
+    chain's ids are mapped through the first chain's record-id dictionary; chains that mention different records are
+    refused.  `iterations` is then ascending within each chain only."""
+    import pyarrow as pa
+    import pyarrow.compute as pc
+
+    chains = [read_chain_arrays(p, lower_iteration_cutoff) for p in paths]
+    if not chains:
+        raise ValueError("no chains to pool")
+    ids = chains[0].record_ids
+    its, samples = [], []
+    for ch in chains:
+        if len(ch.record_ids) != len(ids):
+            raise ValueError("the chains mention different records")
+        pos = pc.index_in(ch.record_ids, value_set=ids)
+        if pos.null_count:
+            raise ValueError("the chains mention different records")
+        remap = pos.to_numpy(zero_copy_only=False).astype(np.int32)
+        for mem, off, part in ch.samples:
+            samples.append((remap[mem], off, part))
+        its.append(ch.iterations)
+    return ChainArrays(ids if len(ids) else pa.array([], pa.string()),
+                       np.concatenate(its) if its else np.zeros(0, np.int64), samples)
+
+
 def sample_from_links(link, block_of_entity):
     """One sample straight from the engine's arrays (record index = position): (members, offsets, partition)."""
     link = np.asarray(link)

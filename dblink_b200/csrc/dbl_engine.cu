@@ -119,6 +119,7 @@ __device__ __forceinline__ void warp_hist_add(unsigned long long *bins, int key)
 // ---------------------------------------------------------------------------------------------------
 struct EntPostParams {
   RowSet rows;
+  ChainMap cm;  // batched chains: block k * blocks + leaf; summary words of chain k at iso_slot + k / ll_slot + k
   int A;
   const int *y;
   const AttrDev *attrs;
@@ -129,14 +130,34 @@ struct EntPostParams {
   unsigned long long *part;
   int iso_slot, ll_slot, blk_slot;  // blk_slot < 0: no block histogram
 };
+// batched chains: a thread's rows come in chain order (rows are sorted by block, blocks are chain-major), so it adds
+// its sums into the chain's words whenever the chain changes, and once at the end
+__device__ __forceinline__ void flush_chain_sums(unsigned long long *part, int iso_slot, int ll_slot, int &iso,
+                                                 double &ll) {
+  if (ll != 0.0) atomicAdd(reinterpret_cast<double *>(&part[ll_slot]), ll);
+  if (iso) atomicAdd(&part[iso_slot], (unsigned long long)iso);
+  ll = 0.0;
+  iso = 0;
+}
+__device__ __forceinline__ void flush_chain_ll(unsigned long long *part, int ll_slot, double &ll) {
+  if (ll != 0.0) atomicAdd(reinterpret_cast<double *>(&part[ll_slot]), ll);
+  ll = 0.0;
+}
 __global__ void __launch_bounds__(256) k_entity_post(EntPostParams p) {
   if (p.rows.dead()) return;
   const int64_t n = p.rows.count();
   double ll = 0.0;
-  int iso = 0;
+  int iso = 0, ck = 0;  // ck: the chain ll / iso belong to (batched chains)
   GRID_STRIDE(i, n) {
     const int64_t e = p.rows.row(i);
     if (e < 0) continue;
+    int kb = 0;  // first block of the entity's chain
+    if (p.cm.K > 1) {
+      const int k = (int)e / p.cm.ents;
+      if (k != ck && p.ent_rec_ptr) flush_chain_sums(p.part, p.iso_slot + ck, p.ll_slot + ck, iso, ll);
+      ck = k;
+      kb = k * p.cm.blocks;
+    }
     const int *ye = p.y + e * p.A;
     double nn = 1.0;
     for (int a = 0; a < p.A; ++a) {
@@ -146,14 +167,16 @@ __global__ void __launch_bounds__(256) k_entity_post(EntPostParams p) {
       ll += at.logphi[v];
     }
     p.entN[e] = nn;
-    const int b = p.tree.n_nodes > 0 ? tree_leaf(p.tree, ye) : 0;
+    const int b = kb + (p.tree.n_nodes > 0 ? tree_leaf(p.tree, ye) : 0);
     p.blk[e] = b;
     if (p.ent_rec_ptr) {
       iso += (p.ent_rec_ptr[e] == p.ent_rec_ptr[e + 1]);
       if (p.blk_slot >= 0) warp_hist_add(p.part + p.blk_slot, b);
     }
   }
-  if (p.ent_rec_ptr) {
+  if (p.ent_rec_ptr && p.cm.K > 1) {
+    flush_chain_sums(p.part, p.iso_slot + ck, p.ll_slot + ck, iso, ll);
+  } else if (p.ent_rec_ptr) {
     typedef cub::BlockReduce<double, 256> BR;
     typedef cub::BlockReduce<int, 256> BRI;
     __shared__ typename BR::TempStorage t1;
@@ -340,7 +363,9 @@ __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__rest
 // updateDistProbs GU:305-320: theta[a,f] ~ Beta(alpha_a + aggDist[a,f], beta_a + N_f - aggDist[a,f]) from the GLOBAL
 // summary of the previous state.  Every rank draws the same values from the same counter-based stream (replaces
 // the broadcast, State.scala:84).  theta_prev keeps the old values: an abandoned sweep restores them.
-__global__ void k_theta(int A, int F, uint64_t seed, long long *__restrict__ ctl, const long long *__restrict__ glob,
+// Batched chains: column f belongs to chain f / files_per_chain, which draws with its own key and its own id a * F1 + f1.
+__global__ void k_theta(int A, int F, uint64_t seed, const uint64_t *__restrict__ seeds, int files_per_chain,
+                        long long *__restrict__ ctl, const long long *__restrict__ glob,
                         const double *__restrict__ alpha, const double *__restrict__ beta,
                         const double *__restrict__ file_size, double *__restrict__ theta,
                         double *__restrict__ theta_prev, unsigned long long *__restrict__ part, int nw) {
@@ -350,7 +375,14 @@ __global__ void k_theta(int A, int F, uint64_t seed, long long *__restrict__ ctl
   for (int i = threadIdx.x; i < A * F; i += blockDim.x) {
     const int a = i / F, f = i % F;
     theta_prev[i] = theta[i];
-    theta[i] = draw_theta_one(seed, it, (uint32_t)i, alpha[a], beta[a], (double)glob[i], file_size[f]);
+    uint64_t s = seed;
+    uint32_t id = (uint32_t)i;
+    if (seeds) {
+      const int k = f / files_per_chain;
+      s = seeds[k];
+      id = (uint32_t)(a * files_per_chain + (f - k * files_per_chain));
+    }
+    theta[i] = draw_theta_one(s, it, id, alpha[a], beta[a], (double)glob[i], file_size[f]);
   }
   if (threadIdx.x == 0) { ctl[CTL_MOVED_ENT] = 0; ctl[CTL_MOVED_REC] = 0; ctl[CTL_WORK] = 0; ctl[CTL_HEAVY] = 0; }
 }
@@ -376,6 +408,7 @@ __global__ void k_finish(long long *__restrict__ ctl) {
 struct ValParams {
   int A, F, sampler;
   uint64_t seed;
+  ChainMap cm;
   RowSet rows;  // owned entities
   const AttrDev *attrs;
   const int *x, *file;
@@ -459,7 +492,7 @@ template <int UB>
 __device__ int value_update(const ValParams &p, uint32_t iter, int64_t e, int a) {
   const AttrDev &at = p.attrs[a];
   const bool collapsed = (p.sampler == DBL_PCG_I || p.sampler == DBL_PCG_II);
-  const U2 u = uniform2(p.seed, PH_VALUE, iter, (uint32_t)e, (uint32_t)a);
+  const U2 u = chain_uniform2(p.seed, p.cm.seeds, p.cm.ents, PH_VALUE, iter, e, (uint32_t)a);
   const int lo = p.ent_rec_ptr[e], hi = p.ent_rec_ptr[e + 1];
   const int *rec = p.rec_by_ent;
 
@@ -652,6 +685,7 @@ __global__ void __launch_bounds__(128) k_values(ValParams p) {
 struct DistParams {
   int A, F, draw;
   uint64_t seed;
+  ChainMap cm;  // batched chains: recDist of chain k at [A*F + k(A+1)], log-likelihood at ll_slot + k
   RowSet rows;  // owned records
   const AttrDev *attrs;
   const int *x, *file, *link, *y, *blk;
@@ -666,9 +700,17 @@ __global__ void __launch_bounds__(256) k_dist(DistParams p) {
   const uint32_t iter = (uint32_t)(p.rows.ctl[CTL_ITER] + 1);
   const int64_t n = p.rows.count();
   double ll = 0.0;
+  int ck = 0;  // the chain ll belongs to (batched chains)
   GRID_STRIDE(i, n) {
     const int64_t r = p.rows.row(i);
     if (r < 0) continue;
+    int rd = 0;  // first recDist word of the record's chain
+    if (p.cm.K > 1) {
+      const int k = (int)r / p.cm.recs;
+      if (k != ck) flush_chain_ll(p.part, p.ll_slot + ck, ll);
+      ck = k;
+      rd = k * (p.A + 1);
+    }
     const int f = p.file[r];
     const int e = p.link[r];
     const int *ye = p.y + (int64_t)e * p.A;
@@ -682,12 +724,12 @@ __global__ void __launch_bounds__(256) k_dist(DistParams p) {
       if (p.draw) {
         const double th = p.theta[a * p.F + f];
         if (xv < 0) {
-          const U2 u = uniform2(p.seed, PH_DIST, iter, (uint32_t)r, (uint32_t)a);
+          const U2 u = chain_uniform2(p.seed, p.cm.seeds, p.cm.recs, PH_DIST, iter, r, (uint32_t)a);
           z = u.u0 < th;  // GU:331-334
         } else if (xv != yv) {
           z = true;  // GU:352-354
         } else {
-          const U2 u = uniform2(p.seed, PH_DIST, iter, (uint32_t)r, (uint32_t)a);
+          const U2 u = chain_uniform2(p.seed, p.cm.seeds, p.cm.recs, PH_DIST, iter, r, (uint32_t)a);
           double pr1 = th * at.phi[xv];
           if (!at.is_const) {
             pr1 = pr1 * at.norm[xv];
@@ -716,8 +758,12 @@ __global__ void __launch_bounds__(256) k_dist(DistParams p) {
       }
     }
     if (p.draw) p.zmask[r] = zm;
-    warp_hist_add(p.part + p.A * p.F, nd);  // GU:265
+    warp_hist_add(p.part + p.A * p.F, rd + nd);  // GU:265
     if (p.blk_slot >= 0) warp_hist_add(p.part + p.blk_slot, p.blk[e]);
+  }
+  if (p.cm.K > 1) {
+    flush_chain_ll(p.part, p.ll_slot + ck, ll);
+    return;
   }
   typedef cub::BlockReduce<double, 256> BR;
   __shared__ typename BR::TempStorage tmp;
@@ -729,24 +775,36 @@ __global__ void __launch_bounds__(256) k_dist(DistParams p) {
 // k_init_state: State.deterministic (State.scala:253-301) -- entity e copies record e (if any), missing
 // values drawn from phi; record r links to entity r mod E; z = (x>=0 && x!=y).
 // ---------------------------------------------------------------------------------------------------
-__global__ void k_init_entities(int64_t E, int64_t R, int A, uint64_t seed, const AttrDev *__restrict__ attrs,
+// batched chains: entity e of chain k copies record e of chain k
+__global__ void k_init_entities(int64_t E, int64_t R, int A, uint64_t seed, ChainMap cm, const AttrDev *__restrict__ attrs,
                                 const int *__restrict__ x, int *__restrict__ y) {
   const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (tid >= E * A) return;
   const int64_t e = tid / A;
   const int a = (int)(tid % A);
-  int v = (e < R) ? x[e * A + a] : -1;
+  int64_t el = e, rec = e, rc = R;  // chain-local entity id, the record it copies, records of its chain
+  if (cm.K > 1) {
+    const int64_t k = e / cm.ents;
+    el = e - k * cm.ents;
+    rec = k * cm.recs + el;
+    rc = cm.recs;
+  }
+  int v = (el < rc) ? x[rec * A + a] : -1;
   if (v < 0) {
-    const U2 u = uniform2(seed, PH_INIT, 0u, (uint32_t)e, (uint32_t)a);
+    const U2 u = chain_uniform2(seed, cm.seeds, cm.ents, PH_INIT, 0u, e, (uint32_t)a);
     v = invcdf(attrs[a].cdf, attrs[a].V, u.u1);
   }
   y[tid] = v;
 }
-__global__ void k_init_records(int64_t E, int64_t R, int A, const int *__restrict__ x, const int *__restrict__ y,
-                               int *__restrict__ link, unsigned *__restrict__ zmask) {
+__global__ void k_init_records(int64_t E, int64_t R, int A, ChainMap cm, const int *__restrict__ x,
+                               const int *__restrict__ y, int *__restrict__ link, unsigned *__restrict__ zmask) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= R) return;
-  const int64_t e = r % E;
+  int64_t e = r % E;
+  if (cm.K > 1) {  // record r of chain k links to entity (r mod E1) of chain k
+    const int64_t k = r / cm.recs;
+    e = k * cm.ents + (r - k * cm.recs) % cm.ents;
+  }
   link[r] = (int)e;
   unsigned zm = 0;
   for (int a = 0; a < A; ++a) {
@@ -1274,6 +1332,17 @@ struct dbl_ctx {
   TreeDev tree{};
   DevBuf<double> prior;  // alpha[A], beta[A], file sizes[F] (k_theta)
 
+  // batched chains (dbl_chains_*): K chains of the model, chain-major; F, P, R, E count all of them (F = K F1,
+  // P = K B), so every kernel indexes exactly as for one chain
+  int K = 1, F1 = 0, B = 1;
+  DevBuf<uint64_t> chain_seeds;  // K keys (K > 1 only)
+  ChainMap chain_map() const {
+    ChainMap m;
+    m.K = K; m.recs = (int)(R / K); m.ents = (int)(E / K); m.files = F1; m.blocks = B;
+    m.seeds = K > 1 ? chain_seeds.p : nullptr;
+    return m;
+  }
+
   // state
   int64_t R = 0, E = 0, iteration = 0;
   bool has_state = false;
@@ -1291,7 +1360,7 @@ struct dbl_ctx {
   DevBuf<long long> cb;
   long long *h_cb = nullptr;  // pinned
   size_t cb_words = 0;
-  int nw = 0;  // summary words: A*F + (A+1) + 2 + 2*P
+  int nw = 0;  // summary words: A*F + K(A+1) + 2K + 2*P
   long long *ctl() const { return cb.p; }
   unsigned long long *part() const { return reinterpret_cast<unsigned long long *>(cb.p + CTL_WORDS); }
   long long *glob() const { return cb.p + CTL_WORDS + nw; }
@@ -1302,9 +1371,11 @@ struct dbl_ctx {
   const long long *h_part() const { return h_cb + CTL_WORDS; }
   const long long *h_glob() const { return h_cb + CTL_WORDS + nw; }
   const double *h_theta_dev() const { return reinterpret_cast<const double *>(h_cb + CTL_WORDS + 2 * (size_t)nw); }
-  int n_counts() const { return A * F + (A + 1) + 2; }  // words a host-mediated all-reduce carries
-  int iso_slot() const { return A * F + (A + 1); }
-  int ll_slot() const { return A * F + (A + 1) + 1; }
+  // [A*F] aggDist, [K(A+1)] recDist of every chain, [K] isolates, [K] log-likelihood (f64 bits); one chain: the words
+  // a host-mediated all-reduce carries
+  int n_counts() const { return A * F + K * (A + 1) + 2 * K; }
+  int iso_slot() const { return A * F + K * (A + 1); }  // chain k: + k
+  int ll_slot() const { return A * F + K * (A + 1) + K; }
   int blk_ent_slot() const { return n_counts(); }
   int blk_rec_slot() const { return n_counts() + P; }
 
@@ -1445,11 +1516,12 @@ static int upload_tree(dbl_ctx *ctx, const dbl_kdtree *t) {
     ctx->tree.set_ptr = base + 3 * n;
     ctx->tree.leaf_no = base + 3 * n + (n + 1);
     ctx->tree.set_val = base + 4 * n + (n + 1);
-    ctx->P = t->n_leaves;
+    ctx->B = t->n_leaves;
   } else {
     ctx->tree.n_nodes = 0;
-    ctx->P = 1;
+    ctx->B = 1;
   }
+  ctx->P = ctx->K * ctx->B;  // every chain has the blocks of the one tree
   return DBL_OK;
 }
 
@@ -1590,6 +1662,7 @@ extern "C" int dbl_ctx_create(dbl_ctx **out, const dbl_model_desc *d) {
   auto *ctx = new dbl_ctx();
   ctx->A = d->num_attrs;
   ctx->F = d->num_files;
+  ctx->F1 = d->num_files;
   ctx->seed = d->seed;
   ctx->rank = d->rank;
   ctx->world = d->world_size > 0 ? d->world_size : 1;
@@ -1641,8 +1714,9 @@ extern "C" void dbl_ctx_destroy(dbl_ctx *ctx) {
   delete ctx;
 }
 extern "C" const char *dbl_last_error(const dbl_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
-extern "C" int64_t dbl_num_records(const dbl_ctx *ctx) { return ctx ? ctx->R : 0; }
-extern "C" int64_t dbl_num_entities(const dbl_ctx *ctx) { return ctx ? ctx->E : 0; }
+extern "C" int64_t dbl_num_records(const dbl_ctx *ctx) { return ctx ? ctx->R / ctx->K : 0; }  // of one chain
+extern "C" int64_t dbl_num_entities(const dbl_ctx *ctx) { return ctx ? ctx->E / ctx->K : 0; }
+extern "C" int32_t dbl_num_chains(const dbl_ctx *ctx) { return ctx ? ctx->K : 0; }
 extern "C" int64_t dbl_iteration(const dbl_ctx *ctx) { return ctx ? ctx->iteration : 0; }
 extern "C" int64_t dbl_kernel_launches(const dbl_ctx *ctx) { return ctx ? ctx->launches : 0; }
 extern "C" const char *dbl_version(void) { return "dblink_b200 0.2 (sm_90a)"; }
@@ -1821,12 +1895,13 @@ static int refresh_summary(dbl_ctx *ctx, bool in_sweep) {
   if (!in_sweep) CUDA_TRY(cudaMemsetAsync(ctx->part(), 0, sizeof(long long) * ctx->nw, ctx->stream));  // else: k_theta
   EntPostParams ep;
   ep.rows = in_sweep ? rows_prefix(ctx, true) : rows_masked(ctx, true);
+  ep.cm = ctx->chain_map();
   ep.A = A; ep.y = ctx->y.p; ep.attrs = ctx->attrs.p; ep.tree = ctx->tree; ep.entN = ctx->entN.p; ep.blk = ctx->blk.p;
   ep.ent_rec_ptr = ctx->ent_rec_ptr.p; ep.part = ctx->part(); ep.iso_slot = ctx->iso_slot(); ep.ll_slot = ctx->ll_slot();
   ep.blk_slot = ctx->world > 1 ? ctx->blk_ent_slot() : -1;
   k_entity_post<<<grid_rows(ctx, ctx->E, 256), 256, 0, ctx->stream>>>(ep);
   DistParams dp;
-  dp.A = A; dp.F = F; dp.draw = in_sweep ? 1 : 0; dp.seed = ctx->seed;
+  dp.A = A; dp.F = F; dp.draw = in_sweep ? 1 : 0; dp.seed = ctx->seed; dp.cm = ctx->chain_map();
   dp.rows = in_sweep ? rows_prefix(ctx, false) : rows_masked(ctx, false);
   dp.attrs = ctx->attrs.p; dp.x = ctx->x.p; dp.file = ctx->file.p; dp.link = ctx->link.p;
   dp.y = ctx->y.p; dp.blk = ctx->blk.p; dp.zmask = ctx->zmask.p; dp.theta = ctx->theta(); dp.part = ctx->part();
@@ -1972,8 +2047,41 @@ static int upload_theta(dbl_ctx *ctx) {
   return DBL_OK;  // h_theta is next written by snapshot(), i.e. after the stream has drained
 }
 
-extern "C" int dbl_state_init(dbl_ctx *ctx, int64_t R, const int32_t *x, const int32_t *file, int64_t pop) {
-  if (!ctx || !x || !file) return DBL_ERR_INVALID;
+// Number of chains and their keys.  Changing K re-shapes everything sized by F, P or the summary: the state that
+// follows (dbl_state_init / _upload, dbl_chains_init / _upload) is allocated afresh.
+static int set_chains(dbl_ctx *ctx, int K, const uint64_t *seeds) {
+  if (K == 1 && ctx->K == 1) return DBL_OK;
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  ctx->drop_graphs();  // captured sweeps hold the key table and the shapes
+  if (K > 1) {
+    if (ctx->chain_seeds.n != (size_t)K) CUDA_TRY(ctx->chain_seeds.alloc(K));
+    CUDA_TRY(cudaMemcpy(ctx->chain_seeds.p, seeds, sizeof(uint64_t) * K, cudaMemcpyHostToDevice));
+  } else {
+    ctx->chain_seeds.release();
+  }
+  if (K == ctx->K) return DBL_OK;
+  const int A = ctx->A;
+  ctx->K = K;
+  ctx->F = K * ctx->F1;
+  ctx->P = K * ctx->B;
+  ctx->has_state = false;
+  ctx->R = ctx->E = 0;  // alloc_state sizes every buffer for the new shape
+  CUDA_TRY(ctx->prior.alloc(2 * (size_t)A + ctx->F));
+  CUDA_TRY(cudaMemcpy(ctx->prior.p, ctx->alpha.data(), sizeof(double) * A, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(ctx->prior.p + A, ctx->beta.data(), sizeof(double) * A, cudaMemcpyHostToDevice));
+  ctx->h_theta.assign((size_t)A * ctx->F, 0.0);
+  ctx->file_sizes.clear();
+  // a control block of the new shape; the counters of the context (pairs scored, ...) carry over
+  long long keep[CTL_WORDS];
+  CUDA_TRY(cudaMemcpy(keep, ctx->ctl(), sizeof(keep), cudaMemcpyDeviceToHost));
+  ctx->cb.release();
+  int rc = alloc_control(ctx);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpy(ctx->ctl(), keep, sizeof(keep), cudaMemcpyHostToDevice));
+  return DBL_OK;
+}
+
+static int state_init(dbl_ctx *ctx, int64_t R, const int32_t *x, const int32_t *file, int64_t pop) {
   CUDA_TRY(cudaSetDevice(ctx->device));
   const int64_t E = pop > 0 ? pop : R;
   int rc = alloc_state(ctx, R, E);
@@ -1982,8 +2090,10 @@ extern "C" int dbl_state_init(dbl_ctx *ctx, int64_t R, const int32_t *x, const i
   CUDA_TRY(cudaMemcpyAsync(ctx->x.p, x, sizeof(int) * R * A, cudaMemcpyHostToDevice, ctx->stream));
   k_rec_class<<<grid_for(R, 256), 256, 0, ctx->stream>>>(R, A, ctx->attrs.p, ctx->x.p, ctx->rec_class.p);
   CUDA_TRY(cudaMemcpyAsync(ctx->file.p, file, sizeof(int) * R, cudaMemcpyHostToDevice, ctx->stream));
-  k_init_entities<<<grid_for(E * A, 256), 256, 0, ctx->stream>>>(E, R, A, ctx->seed, ctx->attrs.p, ctx->x.p, ctx->y.p);
-  k_init_records<<<grid_for(R, 256), 256, 0, ctx->stream>>>(E, R, A, ctx->x.p, ctx->y.p, ctx->link.p, ctx->zmask.p);
+  k_init_entities<<<grid_for(E * A, 256), 256, 0, ctx->stream>>>(E, R, A, ctx->seed, ctx->chain_map(), ctx->attrs.p,
+                                                                  ctx->x.p, ctx->y.p);
+  k_init_records<<<grid_for(R, 256), 256, 0, ctx->stream>>>(E, R, A, ctx->chain_map(), ctx->x.p, ctx->y.p, ctx->link.p,
+                                                            ctx->zmask.p);
   ctx->launches += 3;
   for (int a = 0; a < A; ++a)
     for (int f = 0; f < ctx->F; ++f)
@@ -1994,10 +2104,16 @@ extern "C" int dbl_state_init(dbl_ctx *ctx, int64_t R, const int32_t *x, const i
   return finish_new_state(ctx, false, true);
 }
 
-extern "C" int dbl_state_upload(dbl_ctx *ctx, int64_t R, int64_t E, const int32_t *x, const int32_t *file,
-                                const uint8_t *z, const int32_t *link, const int32_t *y, const double *theta,
-                                int64_t iteration) {
-  if (!ctx || !z || !link || !y || !theta || ((x == nullptr) != (file == nullptr))) return DBL_ERR_INVALID;
+extern "C" int dbl_state_init(dbl_ctx *ctx, int64_t R, const int32_t *x, const int32_t *file, int64_t pop) {
+  if (!ctx || !x || !file) return DBL_ERR_INVALID;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  int rc = set_chains(ctx, 1, nullptr);
+  if (rc) return rc;
+  return state_init(ctx, R, x, file, pop);
+}
+
+static int state_upload(dbl_ctx *ctx, int64_t R, int64_t E, const int32_t *x, const int32_t *file, const uint8_t *z,
+                        const int32_t *link, const int32_t *y, const double *theta, int64_t iteration) {
   const bool new_records = (x != nullptr);
   if (!new_records && (!ctx->x.p || ctx->R != R || ctx->E != E)) {
     ctx->set_error("dbl_state_upload without records: the context holds no records / state of that shape");
@@ -2025,9 +2141,29 @@ extern "C" int dbl_state_upload(dbl_ctx *ctx, int64_t R, int64_t E, const int32_
   return finish_new_state(ctx, true, new_records);
 }
 
-extern "C" int dbl_state_download(dbl_ctx *ctx, uint8_t *z, int32_t *link, int32_t *y, double *theta,
-                                  int32_t *block_of_entity) {
-  if (!ctx) return DBL_ERR_INVALID;
+extern "C" int dbl_state_upload(dbl_ctx *ctx, int64_t R, int64_t E, const int32_t *x, const int32_t *file,
+                                const uint8_t *z, const int32_t *link, const int32_t *y, const double *theta,
+                                int64_t iteration) {
+  if (!ctx || !z || !link || !y || !theta || ((x == nullptr) != (file == nullptr))) return DBL_ERR_INVALID;
+  if (!x && ctx->K > 1) {
+    ctx->set_error("dbl_state_upload without records: the context holds the records of several chains");
+    return DBL_ERR_STATE;
+  }
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  int rc = set_chains(ctx, 1, nullptr);
+  if (rc) return rc;
+  return state_upload(ctx, R, E, x, file, z, link, y, theta, iteration);
+}
+
+// the calls that read or drive ONE chain refuse a context holding several
+static int one_chain_only(dbl_ctx *ctx, const char *what) {
+  if (ctx->K == 1) return DBL_OK;
+  ctx->set_error(std::string(what) + " needs a context holding one chain (dbl_chains_download / dbl_chain_summary "
+                 "read batched chains)");
+  return DBL_ERR_STATE;
+}
+
+static int state_download(dbl_ctx *ctx, uint8_t *z, int32_t *link, int32_t *y, double *theta, int32_t *block_of_entity) {
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   const int A = ctx->A;
@@ -2046,8 +2182,108 @@ extern "C" int dbl_state_download(dbl_ctx *ctx, uint8_t *z, int32_t *link, int32
   return DBL_OK;
 }
 
+extern "C" int dbl_state_download(dbl_ctx *ctx, uint8_t *z, int32_t *link, int32_t *y, double *theta,
+                                  int32_t *block_of_entity) {
+  if (!ctx) return DBL_ERR_INVALID;
+  int rc = one_chain_only(ctx, "dbl_state_download");
+  if (rc) return rc;
+  return state_download(ctx, z, link, y, theta, block_of_entity);
+}
+
 extern "C" int dbl_links_download(dbl_ctx *ctx, int32_t *link_out, int32_t *block_out) {
   return dbl_state_download(ctx, nullptr, link_out, nullptr, nullptr, block_out);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// batched chains: K chains of the model in one context (DESIGN.md 4.6)
+// ---------------------------------------------------------------------------------------------------
+static int check_chains(dbl_ctx *ctx, int32_t K, const uint64_t *seeds, int64_t R, int64_t E) {
+  if (ctx->world > 1) { ctx->set_error("batched chains need an unsharded context"); return DBL_ERR_INVALID; }
+  if (K < 1 || !seeds) { ctx->set_error("num_chains must be >= 1, with one seed per chain"); return DBL_ERR_INVALID; }
+  std::vector<uint64_t> s(seeds, seeds + K);
+  std::sort(s.begin(), s.end());
+  if (std::adjacent_find(s.begin(), s.end()) != s.end()) { ctx->set_error("chain seeds must be distinct"); return DBL_ERR_INVALID; }
+  // one chain is the one-chain context, keyed by the model's seed: a different key would be silently ignored
+  if (K == 1 && seeds[0] != ctx->seed) {
+    ctx->set_error("one chain draws with the model's seed: seeds[0] must equal dbl_model_desc.seed");
+    return DBL_ERR_INVALID;
+  }
+  if (R <= 0 || E <= 0 || (int64_t)K * R > 0x7fffffff || (int64_t)K * E > 0x7fffffff) {
+    ctx->set_error("bad R/E for this number of chains");
+    return DBL_ERR_INVALID;
+  }
+  if (ctx->in_sweep || ctx->async_open) { ctx->set_error("a sweep is open"); return DBL_ERR_STATE; }
+  return DBL_OK;
+}
+// the records of one chain -> K chain-major copies; chain k reads files [k F1, (k+1) F1)
+static int replicate_records(dbl_ctx *ctx, int K, int64_t R, const int32_t *x, const int32_t *file,
+                             std::vector<int32_t> &xk, std::vector<int32_t> &fk) {
+  const int A = ctx->A;
+  for (int64_t r = 0; r < R; ++r)
+    if (file[r] < 0 || file[r] >= ctx->F1) { ctx->set_error("file id out of range"); return DBL_ERR_INVALID; }
+  xk.resize((size_t)K * R * A);
+  fk.resize((size_t)K * R);
+  for (int k = 0; k < K; ++k) {
+    std::copy(x, x + R * A, xk.begin() + (size_t)k * R * A);
+    for (int64_t r = 0; r < R; ++r) fk[(size_t)k * R + r] = k * ctx->F1 + file[r];
+  }
+  return DBL_OK;
+}
+
+extern "C" int dbl_chains_init(dbl_ctx *ctx, int32_t K, const uint64_t *seeds, int64_t R, const int32_t *x,
+                               const int32_t *file, int64_t pop) {
+  if (!ctx || !x || !file) return DBL_ERR_INVALID;
+  const int64_t E = pop > 0 ? pop : R;
+  int rc = check_chains(ctx, K, seeds, R, E);
+  if (rc) return rc;
+  std::vector<int32_t> xk, fk;
+  rc = replicate_records(ctx, K, R, x, file, xk, fk);
+  if (rc) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  rc = set_chains(ctx, K, seeds);
+  if (rc) return rc;
+  return state_init(ctx, K * R, xk.data(), fk.data(), K * E);
+}
+
+extern "C" int dbl_chains_upload(dbl_ctx *ctx, int32_t K, const uint64_t *seeds, int64_t R, int64_t E,
+                                 const int32_t *x, const int32_t *file, const uint8_t *z, const int32_t *link,
+                                 const int32_t *y, const double *theta, int64_t iteration) {
+  if (!ctx || !x || !file || !z || !link || !y || !theta) return DBL_ERR_INVALID;
+  int rc = check_chains(ctx, K, seeds, R, E);
+  if (rc) return rc;
+  std::vector<int32_t> xk, fk;
+  rc = replicate_records(ctx, K, R, x, file, xk, fk);
+  if (rc) return rc;
+  const int A = ctx->A, F1 = ctx->F1;
+  std::vector<int32_t> lk((size_t)K * R);  // chain-local links -> global entity ids
+  for (int64_t i = 0; i < (int64_t)K * R; ++i) {
+    if (link[i] < 0 || link[i] >= E) { ctx->set_error("link outside its chain"); return DBL_ERR_INVALID; }
+    lk[i] = (int32_t)((i / R) * E + link[i]);
+  }
+  std::vector<double> th((size_t)A * K * F1);  // K x A x F1 -> A x (K F1)
+  for (int k = 0; k < K; ++k)
+    for (int a = 0; a < A; ++a)
+      for (int f = 0; f < F1; ++f) th[((size_t)a * K + k) * F1 + f] = theta[((size_t)k * A + a) * F1 + f];
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  rc = set_chains(ctx, K, seeds);
+  if (rc) return rc;
+  return state_upload(ctx, K * R, K * E, xk.data(), fk.data(), z, lk.data(), y, th.data(), iteration);
+}
+
+extern "C" int dbl_chains_download(dbl_ctx *ctx, uint8_t *z, int32_t *link, int32_t *y, double *theta,
+                                   int32_t *block_of_entity) {
+  if (!ctx) return DBL_ERR_INVALID;
+  int rc = state_download(ctx, z, link, y, nullptr, block_of_entity);
+  if (rc) return rc;
+  const int K = ctx->K, A = ctx->A, F1 = ctx->F1;
+  const int64_t R1 = ctx->R / K, E1 = ctx->E / K;
+  if (link) for (int64_t i = 0; i < ctx->R; ++i) link[i] -= (int32_t)((i / R1) * E1);
+  if (block_of_entity) for (int64_t e = 0; e < ctx->E; ++e) block_of_entity[e] -= (int32_t)((e / E1) * ctx->B);
+  if (theta)
+    for (int k = 0; k < K; ++k)
+      for (int a = 0; a < A; ++a)
+        for (int f = 0; f < F1; ++f) theta[((size_t)k * A + a) * F1 + f] = ctx->h_theta[((size_t)a * K + k) * F1 + f];
+  return DBL_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -2191,6 +2427,8 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
   for (int k = 0; k < A; ++k) lp.perm[k] = ctx->perm[k];
   lp.blk_of_link = ctx->blk.p;
   lp.pack_consts = ctx->pack_consts;
+  lp.chain_seeds = ctx->chain_map().seeds;
+  lp.chain_recs = ctx->chain_map().recs;
   if (ctx->link_mass_on) {
     if (ctx->link_mass.n != (size_t)ctx->R) {  // the first sweep of a kind runs eagerly: never inside a graph capture
       CUDA_TRY(ctx->link_mass.alloc((size_t)ctx->R));
@@ -2267,7 +2505,8 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
 // ---------------------------------------------------------------------------------------------------
 // (1) theta | summary of the previous state (State.scala:83, GU:305-320)
 static int enqueue_theta(dbl_ctx *ctx) {
-  k_theta<<<1, 128, 0, ctx->stream>>>(ctx->A, ctx->F, ctx->seed, ctx->ctl(), ctx->glob(), ctx->prior.p,
+  k_theta<<<1, 128, 0, ctx->stream>>>(ctx->A, ctx->F, ctx->seed, ctx->chain_map().seeds, ctx->F1, ctx->ctl(), ctx->glob(),
+                                       ctx->prior.p,
                                        ctx->prior.p + ctx->A, ctx->prior.p + 2 * ctx->A, ctx->theta(), ctx->theta_prev(),
                                        ctx->part(), ctx->nw);
   ctx->launches += 1;
@@ -2292,7 +2531,7 @@ static int update_owned(dbl_ctx *ctx, int sampler) {
   int rc = build_links_csr(ctx, true);
   if (rc) return rc;
   ValParams vp;
-  vp.A = A; vp.F = F; vp.sampler = sampler; vp.seed = ctx->seed; vp.rows = rows_prefix(ctx, true);
+  vp.A = A; vp.F = F; vp.sampler = sampler; vp.seed = ctx->seed; vp.cm = ctx->chain_map(); vp.rows = rows_prefix(ctx, true);
   vp.attrs = ctx->attrs.p; vp.x = ctx->x.p; vp.file = ctx->file.p; vp.zmask = ctx->zmask.p; vp.theta = ctx->theta();
   vp.ent_rec_ptr = ctx->ent_rec_ptr.p; vp.rec_by_ent = ctx->rec_by_ent.p; vp.y = ctx->y.p;
   // latency-bound sizes (the grid does not fill the GPU a few times over): the variant with batched loads
@@ -2470,6 +2709,7 @@ extern "C" int dbl_sweep(dbl_ctx *ctx, int sampler, int32_t n_sweeps) {
 // ---------------------------------------------------------------------------------------------------
 extern "C" int dbl_block_sweep_begin(dbl_ctx *ctx, int sampler) {
   if (!ctx) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_block_sweep_begin")) return rc1;
   if (sampler < 0 || sampler > 3) { ctx->set_error("bad sampler"); return DBL_ERR_INVALID; }
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
   if (ctx->world > 1) { ctx->set_error("block-level sweeps need an unsharded context"); return DBL_ERR_STATE; }
@@ -2547,6 +2787,7 @@ static int apply_ownership(dbl_ctx *ctx) {
 
 extern "C" int dbl_set_block_owners(dbl_ctx *ctx, const int32_t *owner_of_block) {
   if (!ctx) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_set_block_owners")) return rc1;
   if (!ctx->has_state) { ctx->set_error("set_block_owners needs a (replicated) state"); return DBL_ERR_STATE; }
   if (!ctx->all_owned) { ctx->set_error("set_block_owners needs the replicated state: upload / init it again first"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
@@ -2622,6 +2863,7 @@ static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 extern "C" int dbl_comm_export(dbl_ctx *ctx, void *blob_out) {
   if (!ctx || !blob_out) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_comm_export")) return rc1;
   if (!ctx->has_state) { ctx->set_error("dbl_comm_export needs a state (the buffers are sized by it)"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
@@ -2711,6 +2953,7 @@ extern "C" int dbl_last_exchange(dbl_ctx *ctx, int64_t *ent_msgs, int64_t *rec_m
 // ---- host-mediated exchange ---------------------------------------------------------------------------------
 extern "C" int dbl_sweep_begin(dbl_ctx *ctx, int sampler, int64_t *ent_counts, int64_t *rec_counts) {
   if (!ctx || !ent_counts || !rec_counts) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_sweep_begin")) return rc1;
   if (sampler < 0 || sampler > 3) { ctx->set_error("bad sampler"); return DBL_ERR_INVALID; }
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
   if (ctx->in_sweep || ctx->async_open) { ctx->set_error("dbl_sweep_begin twice"); return DBL_ERR_STATE; }
@@ -2745,6 +2988,7 @@ extern "C" int dbl_sweep_begin(dbl_ctx *ctx, int sampler, int64_t *ent_counts, i
 
 extern "C" int dbl_exchange_pack(dbl_ctx *ctx, void *ent_buf_dev, void *rec_buf_dev) {
   if (!ctx) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_exchange_pack")) return rc1;
   if (!ctx->in_sweep) { ctx->set_error("dbl_exchange_pack outside a sweep"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   const int W = ctx->world;
@@ -2774,6 +3018,7 @@ extern "C" int dbl_exchange_pack(dbl_ctx *ctx, void *ent_buf_dev, void *rec_buf_
 extern "C" int dbl_exchange_unpack(dbl_ctx *ctx, const void *ent_buf_dev, int64_t n_ent, const void *rec_buf_dev,
                                    int64_t n_rec) {
   if (!ctx || n_ent < 0 || n_rec < 0) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_exchange_unpack")) return rc1;
   if (!ctx->in_sweep) { ctx->set_error("dbl_exchange_unpack outside a sweep"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   if (n_ent > 0)
@@ -2793,6 +3038,7 @@ extern "C" int dbl_exchange_unpack(dbl_ctx *ctx, const void *ent_buf_dev, int64_
 // reported an error for this sweep, so it is abandoned on every rank
 extern "C" int dbl_sweep_end(dbl_ctx *ctx, const int64_t *global_counts, double global_loglik, int32_t failed) {
   if (!ctx || !global_counts) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_sweep_end")) return rc1;
   if (!ctx->in_sweep) { ctx->set_error("dbl_sweep_end without dbl_sweep_begin"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   ctx->in_sweep = false;
@@ -2820,6 +3066,7 @@ extern "C" int dbl_sweep_end(dbl_ctx *ctx, const int64_t *global_counts, double 
 // partial summary of the shard after dbl_sweep_begin / dbl_set_block_owners (host copy, no device work)
 extern "C" int dbl_partial_summary(dbl_ctx *ctx, int64_t *counts, double *loglik) {
   if (!ctx || !counts || !loglik) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_partial_summary")) return rc1;
   for (int i = 0; i < ctx->n_counts(); ++i) counts[i] = ctx->h_part()[i];
   counts[ctx->ll_slot()] = 0;
   memcpy(loglik, &ctx->h_part()[ctx->ll_slot()], sizeof(double));
@@ -2829,6 +3076,7 @@ extern "C" int32_t dbl_summary_words(const dbl_ctx *ctx) { return ctx ? ctx->n_c
 
 extern "C" int dbl_export_owned_dev(dbl_ctx *ctx, void *y_dev, void *blk_dev, void *link_dev, void *z_dev) {
   if (!ctx || !y_dev || !blk_dev || !link_dev || !z_dev) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_export_owned_dev")) return rc1;
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   k_export_ent<<<grid_for(ctx->E, 256), 256, 0, ctx->stream>>>(ctx->E, ctx->A, ctx->ent_owned.p, ctx->y.p, ctx->blk.p,
@@ -2845,6 +3093,7 @@ extern "C" int dbl_export_owned_dev(dbl_ctx *ctx, void *y_dev, void *blk_dev, vo
 extern "C" int dbl_download_owned(dbl_ctx *ctx, int64_t *n_ent, int32_t *ent_ids, int32_t *y, int32_t *block,
                                   int64_t *n_rec, int32_t *rec_ids, int32_t *link, uint8_t *z) {
   if (!ctx || !n_ent || !n_rec) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_download_owned")) return rc1;
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
   if (ctx->world > 1 && ctx->all_owned) { ctx->set_error("dbl_download_owned before dbl_set_block_owners"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
@@ -2878,6 +3127,7 @@ extern "C" int dbl_download_owned(dbl_ctx *ctx, int64_t *n_ent, int32_t *ent_ids
 
 extern "C" int dbl_owned_masks(dbl_ctx *ctx, uint8_t *ent_owned, uint8_t *rec_owned) {
   if (!ctx) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_owned_masks")) return rc1;
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   if (ent_owned) CUDA_TRY(cudaMemcpyAsync(ent_owned, ctx->ent_owned.p, ctx->E, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2890,6 +3140,7 @@ extern "C" int dbl_owned_masks(dbl_ctx *ctx, uint8_t *ent_owned, uint8_t *rec_ow
 // the sums over ranks mod 2^64 identify the global state whatever the number of ranks or the placement
 extern "C" int dbl_state_hash(dbl_ctx *ctx, uint64_t *hash_out) {
   if (!ctx || !hash_out) return DBL_ERR_INVALID;
+  if (int rc1 = one_chain_only(ctx, "dbl_state_hash")) return rc1;
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   CUDA_TRY(cudaMemsetAsync(ctx->hash_words(), 0, 2 * sizeof(unsigned long long), ctx->stream));
@@ -2966,18 +3217,19 @@ extern "C" int64_t dbl_phase_ms(dbl_ctx *ctx, double *out4) {
   return n;
 }
 
-extern "C" int dbl_summary(dbl_ctx *ctx, dbl_summary_head *head, int64_t *agg_dist, int64_t *rec_dist, double *theta) {
-  if (!ctx) return DBL_ERR_INVALID;
+// summary of chain k: its files are the columns [k F1, (k+1) F1) of aggDist / theta
+static int chain_summary(dbl_ctx *ctx, int k, dbl_summary_head *head, int64_t *agg_dist, int64_t *rec_dist,
+                         double *theta) {
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
-  const int A = ctx->A, F = ctx->F;
+  const int A = ctx->A, F = ctx->F, F1 = ctx->F1, f0 = k * F1;
   const long long *g = ctx->h_glob();
   if (head) {
     head->iteration = ctx->iteration;
-    head->num_isolates = g[ctx->iso_slot()];
+    head->num_isolates = g[ctx->iso_slot() + k];
     double ll;
-    memcpy(&ll, &g[ctx->ll_slot()], sizeof(double));
+    memcpy(&ll, &g[ctx->ll_slot() + k], sizeof(double));
     for (int a = 0; a < A; ++a)
-      for (int f = 0; f < F; ++f) {  // GU:286-293
+      for (int f = f0; f < f0 + F1; ++f) {  // GU:286-293
         const double th = ctx->h_theta[a * F + f];
         const double nd = (double)g[a * F + f];
         ll += (ctx->alpha[a] + nd - 1.0) * std::log(th) +
@@ -2986,8 +3238,25 @@ extern "C" int dbl_summary(dbl_ctx *ctx, dbl_summary_head *head, int64_t *agg_di
     head->log_likelihood = ll;
     head->pairs_scored = ctx->h_pairs;
   }
-  if (agg_dist) for (int i = 0; i < A * F; ++i) agg_dist[i] = g[i];
-  if (rec_dist) for (int i = 0; i <= A; ++i) rec_dist[i] = g[A * F + i];
-  if (theta) std::copy(ctx->h_theta.begin(), ctx->h_theta.end(), theta);
+  for (int a = 0; a < A; ++a)
+    for (int f = 0; f < F1; ++f) {
+      if (agg_dist) agg_dist[a * F1 + f] = g[a * F + f0 + f];
+      if (theta) theta[a * F1 + f] = ctx->h_theta[a * F + f0 + f];
+    }
+  if (rec_dist) for (int i = 0; i <= A; ++i) rec_dist[i] = g[A * F + k * (A + 1) + i];
   return DBL_OK;
+}
+
+extern "C" int dbl_summary(dbl_ctx *ctx, dbl_summary_head *head, int64_t *agg_dist, int64_t *rec_dist, double *theta) {
+  if (!ctx) return DBL_ERR_INVALID;
+  int rc = one_chain_only(ctx, "dbl_summary");
+  if (rc) return rc;
+  return chain_summary(ctx, 0, head, agg_dist, rec_dist, theta);
+}
+
+extern "C" int dbl_chain_summary(dbl_ctx *ctx, int32_t chain, dbl_summary_head *head, int64_t *agg_dist,
+                                 int64_t *rec_dist, double *theta) {
+  if (!ctx) return DBL_ERR_INVALID;
+  if (chain < 0 || chain >= ctx->K) { ctx->set_error("chain out of range"); return DBL_ERR_INVALID; }
+  return chain_summary(ctx, chain, head, agg_dist, rec_dist, theta);
 }

@@ -69,6 +69,27 @@ enum : int {
 };
 constexpr long long ST_ZERO_MASS = 1, ST_PEER_TIMEOUT = 2, ST_PEER_ERROR = 4;
 
+// Batched chains (dbl_chains_*, DESIGN.md 4.6): K chains of one model in one context, chain-major.  Chain k owns
+// records [k recs, (k+1) recs), entities [k ents, (k+1) ents), files [k files, (k+1) files) and blocks
+// [k blocks, (k+1) blocks).  K == 1 (seeds == nullptr): one chain, the model's seed and global ids, as always.
+struct ChainMap {
+  int K, recs, ents, files, blocks;  // chains, then the counts of ONE chain
+  const uint64_t *seeds;             // K keys (device memory); nullptr when K == 1
+};
+// The uniforms of row `id` (a record, an entity, or attr * F + file for theta): chain k draws with key seeds[k] and
+// counts its rows from its own first row, i.e. exactly what a one-chain context with seed seeds[k] draws.  The seed
+// is loaded here, at the draw, and nowhere else.
+__device__ __forceinline__ U2 chain_uniform2(uint64_t seed, const uint64_t *seeds, int rows_per_chain, uint32_t phase,
+                                             uint32_t iter, int64_t id, uint32_t sub) {
+  uint32_t local = (uint32_t)id;
+  if (seeds) {
+    const int k = (int)id / rows_per_chain;
+    seed = seeds[k];
+    local = (uint32_t)((int)id - k * rows_per_chain);
+  }
+  return uniform2(seed, phase, iter, local, sub);
+}
+
 struct LinkParams {
   int A, F, P, sampler;
   uint64_t seed;
@@ -93,6 +114,8 @@ struct LinkParams {
   const int *blk_of_link;  // block id of every entity (k_link_pruned: block of a record = block of its entity)
   int hslots, hshift;  // common size of the per-row similarity hash tables (k_link_pcg2); 0 = unavailable
   double *link_mass;   // R entries or null: every link kernel stores the total mass of each record's categorical
+  const uint64_t *chain_seeds;  // batched chains: one key per chain (nullptr: one chain, `seed`)
+  int chain_recs;               // records per chain
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -124,6 +147,10 @@ __device__ __forceinline__ bool row_find(const AttrDev &at, int v1, int v2, doub
 }
 
 __device__ __forceinline__ uint32_t link_iter(const LinkParams &p) { return (uint32_t)(p.ctl[CTL_ITER] + 1); }
+// the uniforms of record r's link draw
+__device__ __forceinline__ U2 link_uniform(const LinkParams &p, int64_t r) {
+  return chain_uniform2(p.seed, p.chain_seeds, p.chain_recs, PH_LINK, link_iter(p), r, 0u);
+}
 // a failed sweep (zero-mass draw, peer error) is abandoned: every later kernel returns before it changes anything
 __device__ __forceinline__ bool sweep_dead(const long long *ctl) { return ctl[CTL_STATUS] != 0; }
 
@@ -352,7 +379,7 @@ __global__ void __launch_bounds__(LINK_WARPS * 32) k_link_generic(LinkParams p) 
   }
   store_mass(p, lane, r, run);
   if (!(run > 0.0) || isinf(run)) { fail_link(p, lane, r); return; }
-  const U2 u = uniform2(p.seed, PH_LINK, link_iter(p), (uint32_t)r, 0u);
+  const U2 u = link_uniform(p, r);
   const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q, run, u.u0, wf);
   store_link(p, lane, r, b, n, j);
 }
@@ -565,7 +592,7 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
     const int slot = j % TE;
     return generic_weight(ra, A, false, tile + slot, reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot]);
   };
-  const U2 u = uniform2(p.seed, PH_LINK, link_iter(p), (uint32_t)r, 0u);
+  const U2 u = link_uniform(p, r);
   const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q, run, u.u0, wf);
   store_link(p, lane, r, b, n, j);
 }
@@ -869,7 +896,7 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
   if (!(run > 0.0) || isinf(run)) { fail_link(p, lane, r); return; }
 
   // ---- pass 2: the same walk restricted to the chosen chunk
-  const U2 u = uniform2(p.seed, PH_LINK, link_iter(p), (uint32_t)r, 0u);
+  const U2 u = link_uniform(p, r);
   const double t = u.u0 * run;
   unsigned m = __ballot_sync(FULL, lane < nchunks && Q > t);
   const int chunk = m ? (__ffs(m) - 1) : (nchunks - 1);
@@ -1010,7 +1037,7 @@ __global__ void __launch_bounds__(HEAVY_WARPS * 32) k_link_heavy(PrunedParams pp
       if (!(run > 0.0) || isinf(run)) {
         fail_link(p, lane, r);
       } else {
-        const U2 u = uniform2(p.seed, PH_LINK, link_iter(p), (uint32_t)r, 0u);
+        const U2 u = link_uniform(p, r);
         const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q, run, u.u0, wf, s_sums);
         store_link(p, lane, r, b, n, j);
       }

@@ -375,7 +375,7 @@ __global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_s
         pcg2_load<A, NS, PK>(cd, gtiles + (size_t)(j / TE) * TW, j % TE);
         return pcg2_weight<A, NS, HC, false, PK>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
       };
-      const U2 u = uniform2(p.seed, PH_LINK, link_iter(p), (uint32_t)r, 0u);
+      const U2 u = link_uniform(p, r);
       const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q[ri], run[ri], u.u0, wf, my_sums + ri * 1024);
       store_link(p, lane, r, b, n, j);
     }

@@ -305,6 +305,72 @@ class GibbsEngine:
                                             cast(z_ptr, _lib.u8p), cast(link_ptr, _lib.i32p), cast(y_ptr, _lib.i32p),
                                             _p(theta, _lib.f64p), int(iteration)), "upload_state", self._h)
 
+    # ---- batched chains ---------------------------------------------------------------------------
+    def init_chains(self, x, file_ids=None, population_size=0, seeds=(0, 1)):
+        """State.deterministic for K = len(seeds) independent chains of the model in this one context, chain k drawn
+        with key seeds[k].  Chain k is bit-equal to a one-chain engine created with seed=seeds[k] and given the same
+        partitioner.  x / file_ids are the records once; the device replicates them."""
+        x = _i32(x)
+        if x.ndim != 2 or x.shape[1] != self.A:
+            raise ValueError("attribute specifications do not match the records")  # RecordsCache.scala:72
+        f = _i32(file_ids if file_ids is not None else np.zeros(x.shape[0], np.int32))
+        s = np.ascontiguousarray(seeds, dtype=np.uint64)
+        _check(_lib.load().dbl_chains_init(self._h, len(s), _p(s, _lib.u64p), x.shape[0], _p(x, _lib.i32p),
+                                           _p(f, _lib.i32p), int(population_size)), "init_chains", self._h)
+        self._records_src = (None, None)
+
+    def upload_chains(self, x, file_ids, states, seeds, iteration=0):
+        """Resume K = len(seeds) chains: `states` = one dict per chain in download_state's format (z, link with
+        chain-local entity ids, y, theta)."""
+        if len(states) != len(seeds):
+            raise ValueError("one state per chain")
+        xs, fs = _i32(x), _i32(file_ids)
+        z = np.ascontiguousarray(np.concatenate([st["z"] for st in states]), dtype=np.uint8)
+        link = _i32(np.concatenate([st["link"] for st in states]))
+        y = _i32(np.concatenate([st["y"] for st in states]))
+        theta = _f64(np.stack([np.asarray(st["theta"], np.float64).reshape(self.A, self.F) for st in states]))
+        R, E = xs.shape[0], len(states[0]["y"])
+        if (xs.ndim != 2 or xs.shape[1] != self.A or y.shape[1] != self.A or
+                any(len(st["link"]) != R or len(st["y"]) != E for st in states)):
+            raise ValueError("state arrays do not match the model")
+        s = np.ascontiguousarray(seeds, dtype=np.uint64)
+        _check(_lib.load().dbl_chains_upload(self._h, len(s), _p(s, _lib.u64p), R, E, _p(xs, _lib.i32p),
+                                             _p(fs, _lib.i32p), _p(z, _lib.u8p), _p(link, _lib.i32p), _p(y, _lib.i32p),
+                                             _p(theta, _lib.f64p), int(iteration)), "upload_chains", self._h)
+        self._records_src = (None, None)
+
+    @property
+    def num_chains(self):
+        return _lib.load().dbl_num_chains(self._h)
+
+    def download_chains(self, links_only=False):
+        """Every chain's state at once: a list of K dicts in download_state's format (chain-local link and entity ids,
+        block = leaf id of the shared tree).  links_only: only link and block (the linkage structure of each chain)."""
+        K, R, E, A = self.num_chains, self.num_records, self.num_entities, self.A
+        link, blk = np.zeros(K * R, np.int32), np.zeros(K * E, np.int32)
+        z = y = theta = None
+        if not links_only:
+            z, y, theta = np.zeros((K * R, A), np.uint8), np.zeros((K * E, A), np.int32), np.zeros((K, A, self.F))
+        ptr = lambda a, t: _p(a, t) if a is not None else None
+        _check(_lib.load().dbl_chains_download(self._h, ptr(z, _lib.u8p), _p(link, _lib.i32p), ptr(y, _lib.i32p),
+                                               ptr(theta, _lib.f64p), _p(blk, _lib.i32p)), "download_chains", self._h)
+        out = [{"link": link[k * R:(k + 1) * R], "block": blk[k * E:(k + 1) * E]} for k in range(K)]
+        if not links_only:
+            for k, d in enumerate(out):
+                d.update(z=z[k * R:(k + 1) * R], y=y[k * E:(k + 1) * E], theta=theta[k])
+        return out
+
+    def chain_summary(self, k):
+        """summary() of chain k."""
+        head = _lib.SummaryHead()
+        agg = np.zeros((self.A, self.F), np.int64)
+        rec = np.zeros(self.A + 1, np.int64)
+        theta = np.zeros((self.A, self.F))
+        _check(_lib.load().dbl_chain_summary(self._h, int(k), C.byref(head), _p(agg, _lib.i64p), _p(rec, _lib.i64p),
+                                             _p(theta, _lib.f64p)), "chain_summary", self._h)
+        return {"iteration": head.iteration, "num_isolates": head.num_isolates, "log_likelihood": head.log_likelihood,
+                "pairs_scored": head.pairs_scored, "agg_dist": agg, "rec_dist": rec, "theta": theta}
+
     def set_partitioner(self, partitioner):
         """Install the partition function fitted on the initial entity values (State.scala:309-316)."""
         self.partitioner = partitioner
@@ -451,8 +517,9 @@ class GibbsEngine:
         _check(_lib.load().dbl_set_link_mass_capture(self._h, int(bool(on))), "set_link_mass_capture", self._h)
 
     def link_mass(self):
-        """float64[R]: the total mass of each record's link categorical in the last sweep run with the capture on."""
-        out = np.zeros(self.num_records, np.float64)
+        """float64[R]: the total mass of each record's link categorical in the last sweep run with the capture on
+        (K R totals, chain-major, on an engine holding K chains)."""
+        out = np.zeros(self.num_chains * self.num_records, np.float64)
         _check(_lib.load().dbl_link_mass(self._h, _p(out, _lib.f64p)), "link_mass", self._h)
         return out
 

@@ -9,14 +9,15 @@ import shutil
 
 import numpy as np
 
-from . import _lib, analysis, analysis_arrays, analysis_gpu, config as hocon, sampler as chain, state_io, writers
+from . import (_lib, analysis, analysis_arrays, analysis_gpu, config as hocon, convergence, sampler as chain, state_io,
+               writers)
 from .engine import GibbsEngine, KDTreePartitioner
 from .records import (Attribute, RecordsCache, SimilarityFn, build_cache_from_columns, read_csv,  # noqa: F401
                       read_csv_columns)
 
 SUPPORTED_METRICS = ("pairwise", "cluster")  # ProjectStep.scala:36
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
-                        "pairwise-match-probabilities")
+                        "pairwise-match-probabilities", "convergence-diagnostics")
 
 
 def shared_most_probable_clusters(chain):
@@ -46,6 +47,11 @@ class Project:
         self.ent_id_attribute = g("dblink.data.entityIdentifier", None)
         self.null_value = cfg.get_string("dblink.data.nullValue")
         self.random_seed = cfg.get_int("dblink.randomSeed")
+        # dblink.numChains: independent chains of the model swept together on one GPU, chain k keyed by randomSeed + k
+        nc = g("dblink.numChains", 1)
+        if isinstance(nc, bool) or not isinstance(nc, int) or nc < 1:
+            raise ValueError("numChains must be a positive integer.")
+        self.num_chains = nc
         self.population_size = g("dblink.populationSize", None)
         self.expected_max_cluster_size = int(g("dblink.expectedMaxClusterSize", 10))
         self.matching_attributes = []
@@ -99,7 +105,12 @@ class Project:
         else:
             L.append(f"  * KDTreePartitioner(numLevels={self.num_levels}, attributeIds="
                      f"[{','.join(str(i) for i in self.partition_attribute_ids)}])")
-        L += ["", "Project settings", "----------------", f"  * Using randomSeed={self.random_seed}",
+        L += ["", "Project settings", "----------------", f"  * Using randomSeed={self.random_seed}"]
+        if self.num_chains > 1:
+            L.append(f"  * Running numChains={self.num_chains} chains with seeds "
+                     + ", ".join(str(s) for s in self.chain_seeds()) + " (one k-d tree, fitted on chain 0; chains "
+                     "start from State.deterministic, not over-dispersed), outputs under chain-<k>/")
+        L += [
               f"  * Using expectedMaxClusterSize={self.expected_max_cluster_size}",
               f"  * Saving Markov chain and complete final state to '{self.output_path}'",
               "  * Sweeps run on the CUDA device of this process (libdblink_b200); there are no Spark checkpoints"]
@@ -175,6 +186,15 @@ class Project:
 
         return lookup
 
+    def chain_seeds(self):
+        return [self.random_seed + k for k in range(self.num_chains)]
+
+    def chain_dirs(self):
+        """Where each chain's linkage-chain.parquet / diagnostics.csv / state.npz live."""
+        if self.num_chains == 1:
+            return [self.output_path]
+        return [os.path.join(self.output_path, f"chain-{k}") for k in range(self.num_chains)]
+
     def _new_engine(self):
         d = self.load()
         cache = d["cache"]
@@ -187,14 +207,20 @@ class Project:
                                           [a.alpha for a in self.matching_attributes],
                                           [a.beta for a in self.matching_attributes],
                                           extra=(int(self.random_seed), int(self.population_size or 0),
-                                                 int(self.num_levels), tuple(self.partition_attribute_ids)))
+                                                 int(self.num_levels), tuple(self.partition_attribute_ids))
+                                          + ((("numChains", self.num_chains),) if self.num_chains > 1 else ()))
 
     def generate_initial_state(self):
         """Project.generateInitialState (:130-145) -> a GibbsEngine at iteration 0."""
         d = self.load()
         eng = self._new_engine()
-        eng.init_state(d["x"], d["file"], int(self.population_size or 0))
-        part = KDTreePartitioner(self.num_levels, self.partition_attribute_ids).fit(eng.download_state()["y"])
+        if self.num_chains == 1:
+            eng.init_state(d["x"], d["file"], int(self.population_size or 0))
+            y0 = eng.download_state()["y"]
+        else:  # one tree for every chain, fitted on chain 0's initial entity values
+            eng.init_chains(d["x"], d["file"], int(self.population_size or 0), self.chain_seeds())
+            y0 = eng.download_chains()[0]["y"]
+        part = KDTreePartitioner(self.num_levels, self.partition_attribute_ids).fit(y0)
         eng.set_partitioner(part)
         eng._partitioner_keepalive = part
         return eng
@@ -205,16 +231,26 @@ class Project:
         fitted it, so the resumed chain continues as if it had never stopped; the fingerprint covers the data, the
         tables, the priors, randomSeed, populationSize and the partitioner settings, so a state saved under a
         different configuration is refused instead of being continued with another key / partition function."""
-        if not state_io.saved_state_exists(self.output_path):
+        dirs = self.chain_dirs()
+        if not all(state_io.saved_state_exists(p) for p in dirs):
             return None
-        st = state_io.load_state(self.output_path, self.fingerprint())
+        sts = [state_io.load_state(p, self.fingerprint()) for p in dirs]
         d = self.load()
         eng = self.generate_initial_state()
-        eng.upload_state(d["x"], d["file"], st["z"], st["link"], st["y"], st["theta"], st["iteration"])
+        if self.num_chains == 1:
+            st = sts[0]
+            eng.upload_state(d["x"], d["file"], st["z"], st["link"], st["y"], st["theta"], st["iteration"])
+        else:
+            if len({st["iteration"] for st in sts}) != 1:
+                raise ValueError("the chains' saved states are at different iterations")
+            eng.upload_chains(d["x"], d["file"], sts, self.chain_seeds(), sts[0]["iteration"])
         return eng
 
     def save_state(self, eng):
-        state_io.save_state(eng, self.output_path, self.fingerprint(), self.random_seed)
+        if self.num_chains == 1:
+            state_io.save_state(eng, self.output_path, self.fingerprint(), self.random_seed)
+        else:
+            state_io.save_chain_states(eng, self.chain_dirs(), self.fingerprint(), self.chain_seeds())
 
     # ---- steps (ProjectSteps.parseSteps) -------------------------------------------------------------
     def steps(self):
@@ -231,6 +267,8 @@ class Project:
                 q = list(prm["quantities"])
                 if not q or any(x not in SUPPORTED_QUANTITIES for x in q):
                     raise ValueError(f"quantities must be one of {SUPPORTED_QUANTITIES}.")
+                if "convergence-diagnostics" in q and self.num_chains < 2:
+                    raise ValueError("convergence-diagnostics needs numChains >= 2.")
                 # minMatchProbability: pairwise-match-probabilities.csv keeps the pairs at least this probable
                 t = float(prm.get("minMatchProbability", 0.0))
                 if not 0.0 <= t <= 1.0:
@@ -269,14 +307,22 @@ class Project:
                 self.save_state(eng)  # Sampler.scala:120
             elif name == "summarize":
                 # array implementations (analysis_arrays): same quantities as analysis.py, no loop over clusters
-                ch = analysis_arrays.read_chain_arrays(os.path.join(self.output_path, "linkage-chain.parquet"),
-                                                       prm["lower_iteration_cutoff"])
+                cut = prm["lower_iteration_cutoff"]
+                ch = self.read_chain(cut)  # several chains: their samples pooled, chain-major
                 for q in prm["quantities"]:
-                    if q == "cluster-size-distribution":
-                        writers.save_cluster_size_distribution(analysis_arrays.cluster_size_distribution(ch),
-                                                               self.output_path)
-                    elif q == "partition-sizes":
-                        writers.save_partition_sizes(analysis_arrays.partition_sizes(ch), self.output_path)
+                    if q in ("cluster-size-distribution", "partition-sizes"):  # per chain
+                        for dr in self.chain_dirs():
+                            one = (ch if self.num_chains == 1 else
+                                   analysis_arrays.read_chain_arrays(os.path.join(dr, "linkage-chain.parquet"), cut))
+                            if q == "cluster-size-distribution":
+                                writers.save_cluster_size_distribution(analysis_arrays.cluster_size_distribution(one),
+                                                                       dr)
+                            else:
+                                writers.save_partition_sizes(analysis_arrays.partition_sizes(one), dr)
+                    elif q == "convergence-diagnostics":
+                        rows = convergence.convergence_diagnostics(
+                            [os.path.join(dr, "diagnostics.csv") for dr in self.chain_dirs()], cut)
+                        convergence.save_convergence_diagnostics(rows, self.output_path)
                     elif q == "pairwise-match-probabilities":
                         S, t = len(ch.samples), prm["min_match_probability"]
                         first, second, count = pairwise_match_counts(ch, min_count=analysis_arrays.min_match_count(t, S))
@@ -289,8 +335,7 @@ class Project:
                 true_labels = self.true_labels()
                 if true_labels is None:
                     raise ValueError("Ground truth entity ids are required for evaluation")  # ProjectStep.scala:65
-                ch = analysis_arrays.read_chain_arrays(os.path.join(self.output_path, "linkage-chain.parquet"),
-                                                       prm["lower_iteration_cutoff"])
+                ch = self.read_chain(prm["lower_iteration_cutoff"])
                 smpc_path = os.path.join(self.output_path, "shared-most-probable-clusters.csv")
                 if prm["use_existing_smpc"] and os.path.exists(smpc_path):  # ProjectStep.scala EvaluateStep
                     labels = self._read_smpc_labels(smpc_path, ch.record_ids)
@@ -320,6 +365,13 @@ class Project:
                         if prm["delete_source"]:
                             (shutil.rmtree if os.path.isdir(src) else os.remove)(src)
         return results
+
+    def read_chain(self, lower_iteration_cutoff=0):
+        """The chain's samples at or after the cutoff; with several chains, all of them pooled chain-major."""
+        paths = [os.path.join(dr, "linkage-chain.parquet") for dr in self.chain_dirs()]
+        if self.num_chains == 1:
+            return analysis_arrays.read_chain_arrays(paths[0], lower_iteration_cutoff)
+        return analysis_arrays.read_pooled_chain_arrays(paths, lower_iteration_cutoff)
 
     @staticmethod
     def _read_smpc_labels(path, record_ids):

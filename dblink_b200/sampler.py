@@ -11,7 +11,11 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
     """Generates `sample_size` posterior samples by successively applying the transition operator; writes
     linkage-chain.parquet and diagnostics.csv under output_path.  Returns the number of sweeps performed.
     on_sample(summary, parts) sees every recorded sample; parts = {partition id: pyarrow ListArray of clusters}
-    (`.to_pylist()` gives the lists of record ids)."""
+    (`.to_pylist()` gives the lists of record ids).
+
+    An engine holding K > 1 chains (GibbsEngine.init_chains / upload_chains) writes chain k's linkage-chain.parquet
+    and diagnostics.csv under output_path/chain-<k>/, from one download of every chain's links per recorded sample;
+    on_sample then sees every chain's sample, chain-major."""
     if sample_size <= 0:
         raise ValueError("`sampleSize` must be positive.")            # Sampler.scala:61
     if burnin_interval < 0:
@@ -28,25 +32,35 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
     initial_iteration = engine.iteration
     continue_chain = initial_iteration != 0
     pop = population_size if population_size is not None else engine.num_entities
+    K = getattr(engine, "num_chains", 1)
+    dirs = [output_path] if K == 1 else [os.path.join(output_path, f"chain-{k}") for k in range(K)]
     lw = dw = ids = None
     if writer:
-        lw = LinkageChainWriter(os.path.join(output_path, "linkage-chain.parquet"), write_buffer_size, continue_chain)
-        dw = DiagnosticsWriter(os.path.join(output_path, "diagnostics.csv"), attribute_names, continue_chain)
+        lw, dw = [], []
+        for d in dirs:
+            os.makedirs(d, exist_ok=True)
+            lw.append(LinkageChainWriter(os.path.join(d, "linkage-chain.parquet"), write_buffer_size, continue_chain))
+            dw.append(DiagnosticsWriter(os.path.join(d, "diagnostics.csv"), attribute_names, continue_chain))
 
         import pyarrow as pa
 
         ids = pa.array([str(r) for r in record_ids], pa.string())
 
     def record():
-        link, blk = engine.links()  # sharded: a collective, every rank takes part
-        s = engine.summary()
+        if K == 1:
+            link, blk = engine.links()  # sharded: a collective, every rank takes part
+            samples = [(link, blk, engine.summary())]
+        else:
+            st = engine.download_chains(links_only=True)
+            samples = [(st[k]["link"], st[k]["block"], engine.chain_summary(k)) for k in range(K)]
         if not writer:
             return
-        parts = linkage_structure_arrow(link, blk, ids)  # {partition id: ListArray of clusters}
-        lw.append(s["iteration"], parts)
-        dw.write_row(s, pop)
-        if on_sample:
-            on_sample(s, parts)
+        for k, (link, blk, s) in enumerate(samples):
+            parts = linkage_structure_arrow(link, blk, ids)  # {partition id: ListArray of clusters}
+            lw[k].append(s["iteration"], parts)
+            dw[k].write_row(s, pop)
+            if on_sample:
+                on_sample(s, parts)
 
     if not continue_chain and burnin_interval == 0:
         record()  # the initial state is a sample (Sampler.scala:84-89)
@@ -64,6 +78,6 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
         record()
         count += 1
     if writer:
-        lw.close()
-        dw.close()
+        for w in lw + dw:
+            w.close()
     return done

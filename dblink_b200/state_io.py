@@ -40,6 +40,18 @@ def save_state(engine, output_path, fingerprint, seed):
     os.replace(tmp, os.path.join(output_path, STATE_FILE))
 
 
+def save_chain_states(engine, output_paths, fingerprint, seeds):
+    """The K chains of a batched engine, chain k's state.npz under output_paths[k] (same format as save_state)."""
+    for path, st, seed in zip(output_paths, engine.download_chains(), seeds):
+        os.makedirs(path, exist_ok=True)
+        tmp = os.path.join(path, STATE_FILE + ".tmp.npz")
+        np.savez_compressed(tmp, iteration=np.int64(engine.iteration), theta=st["theta"],
+                            z=np.packbits(st["z"], axis=1), n_attrs=np.int64(st["z"].shape[1]), link=st["link"],
+                            y=st["y"], population_size=np.int64(engine.num_entities), seed=np.int64(seed),
+                            fingerprint=np.array(fingerprint))
+        os.replace(tmp, os.path.join(path, STATE_FILE))
+
+
 def saved_state_exists(output_path):
     return os.path.exists(os.path.join(output_path, STATE_FILE))
 

@@ -128,9 +128,38 @@ int dbl_state_upload(dbl_ctx *, int64_t num_records, int64_t num_entities, const
                      int64_t iteration);
 /* Full state back to the host (State.save, State.scala:122-150); any pointer may be NULL. */
 int dbl_state_download(dbl_ctx *, uint8_t *z, int32_t *link, int32_t *y, double *theta, int32_t *block_of_entity);
-int64_t dbl_num_records(const dbl_ctx *);
-int64_t dbl_num_entities(const dbl_ctx *);
+int64_t dbl_num_records(const dbl_ctx *);  /* of one chain */
+int64_t dbl_num_entities(const dbl_ctx *); /* of one chain */
 int64_t dbl_iteration(const dbl_ctx *);
+
+/* ---------------------------------------------------------------------------------------------------
+ * Batched chains: K >= 1 independent chains of the model in one context, swept together (one launch sequence per
+ * sweep for all of them).  Chain k draws with Philox key seeds[k] and chain-local ids, so chain k is bit-equal to a
+ * one-chain context created with seed seeds[k] and given the same partition function.  Layout is chain-major: chain k
+ * owns records [kR, (k+1)R), entities [kE, (k+1)E), blocks [kB, (k+1)B) (B = leaves of the one tree all chains
+ * share).  x and file are ONE copy of the records (R rows, host memory); the context replicates them.
+ *   dbl_chains_init      State.deterministic for every chain (population_size <= 0 means R)
+ *   dbl_chains_upload    resume: z (K R x A), link (K R, chain-LOCAL entity ids in [0, E)), y (K E x A), theta
+ *                        (K x A x F), all chain-major, host memory
+ *   dbl_chains_download  every chain at once, in the same layout; block_of_entity = leaf id in [0, B); any pointer
+ *                        may be NULL
+ *   dbl_chain_summary    dbl_summary of chain `chain` (agg_dist / theta A x F, rec_dist A + 1)
+ * On a context holding K > 1 chains dbl_num_records / dbl_num_entities give one chain's R and E,
+ * dbl_num_partitions gives K B, dbl_link_mass returns K R totals (chain-major); dbl_sweep, dbl_sweep_async, dbl_sync,
+ * the link and graph modes and dbl_link_kernel work unchanged.  A zero-mass categorical in any chain abandons the
+ * sweep for every chain (they share one iteration counter).  The calls that read or drive one chain
+ * (dbl_state_download, dbl_links_download, dbl_summary, dbl_state_hash, the block-by-block API and the multi-GPU calls)
+ * give DBL_ERR_STATE; dbl_state_init / dbl_state_upload turn the context back into a one-chain context.
+ * DBL_ERR_INVALID: num_chains < 1, seeds NULL or not distinct, num_chains = 1 with seeds[0] other than the model's seed, a sharded context (world_size > 1), a file id outside
+ * [0, F), a link outside its chain, K R or K E beyond 2^31 - 1.
+ * ------------------------------------------------------------------------------------------------- */
+int dbl_chains_init(dbl_ctx *, int32_t num_chains, const uint64_t *seeds, int64_t num_records, const int32_t *x,
+                    const int32_t *file, int64_t population_size);
+int dbl_chains_upload(dbl_ctx *, int32_t num_chains, const uint64_t *seeds, int64_t num_records,
+                      int64_t num_entities, const int32_t *x, const int32_t *file, const uint8_t *z,
+                      const int32_t *link, const int32_t *y, const double *theta, int64_t iteration);
+int32_t dbl_num_chains(const dbl_ctx *);
+int dbl_chains_download(dbl_ctx *, uint8_t *z, int32_t *link, int32_t *y, double *theta, int32_t *block_of_entity);
 
 /* n_sweeps applications of the Markov transition operator State.nextState (State.scala:78-99):
  * updateDistProbs (GU:305-320) -> updatePartitions/updatePartition (GU:124-211: link draw per record
@@ -164,6 +193,8 @@ typedef struct {
 } dbl_summary_head;
 int dbl_summary(dbl_ctx *, dbl_summary_head *head, int64_t *agg_dist /*A*F*/, int64_t *rec_dist /*A+1*/,
                 double *theta /*A*F*/);
+int dbl_chain_summary(dbl_ctx *, int32_t chain, dbl_summary_head *head, int64_t *agg_dist /*A*F*/,
+                      int64_t *rec_dist /*A+1*/, double *theta /*A*F*/);
 
 /* n sweeps enqueued on the context's stream without waiting for them (dbl_sweep = dbl_sweep_async + dbl_sync).
  * Nothing in a sweep needs the host: theta is drawn on the device, sizes are read from device memory, the exchange
