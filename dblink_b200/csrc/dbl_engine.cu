@@ -1409,16 +1409,16 @@ struct dbl_ctx {
   DevBuf<double> lane_sums;  // k_link_pcg2 scratch: pass-1 lane sums per chunk of every resident warp
   int qtile_pk = 0;  // quad tiles carry the packed constants (PK instantiations of k_link_pcg2)
   bool tiles_valid[2] = {false, false};  // attribute-major / quad tiles match the current layout
-  // inverted index of the block tables for the pruned PCG-I link kernel (built on demand, once per sweep)
-  DevBuf<unsigned long long> inv_key_in, inv_key;
-  DevBuf<unsigned> inv_key32_in, inv_key32;
-  DevBuf<int> inv_pos_in, inv_pos, inv_seg, inv_vptr, heavy_list;
+  // inverted index of the block tables for the pruned PCG-I link kernel (built on demand, once per sweep): E * A ids,
+  // unsigned or (inv_ids64) unsigned long long, with their candidate positions
+  DevBuf<unsigned char> inv_ids_in, inv_ids;
+  bool inv_ids64 = false;
+  DevBuf<int> inv_pos_in, inv_pos, inv_vptr, heavy_list;
   InvDense inv_dense;
-  bool inv_use_dense = false;
+  bool inv_use_dense = false;  // inv_vptr holds the dense pointer table
   DevBuf<unsigned char> inv_tmp;
   size_t inv_tmp_bytes = 0;
   bool inv_valid = false;
-  int inv_vbits = 32;
   DevBuf<int> link_sorted, rec_by_ent, ent_rec_ptr;
   DevBuf<unsigned char> rec_class;  // static cost class of a record (k_rec_class)
   DevBuf<unsigned char> cub_tmp;
@@ -2294,21 +2294,37 @@ DBL_DECL(1) DBL_DECL(2) DBL_DECL(3) DBL_DECL(4) DBL_DECL(5) DBL_DECL(6) DBL_DECL
 DBL_DECL(9) DBL_DECL(10) DBL_DECL(11) DBL_DECL(12) DBL_DECL(13) DBL_DECL(14) DBL_DECL(15) DBL_DECL(16)
 #undef DBL_DECL
 
-// number of entities in owned blocks, on the host.  Unsharded contexts own everything; otherwise the count lives on
-// the device (the exchange changes it every sweep) and costs one small read-back.
-static int owned_entities_on_host(dbl_ctx *ctx, int64_t *out) {
-  if (ctx->all_owned && !ctx->in_block_sweep) { *out = ctx->E; return DBL_OK; }
-  if (ctx->h_owned_ent < 0) {
-    long long v = 0;
-    CUDA_TRY(cudaMemcpyAsync(&v, ctx->ctl() + CTL_OWNED_ENT, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    ctx->h_owned_ent = v;
+// The (block, attribute, value) ids of every slot of the block-sorted entity table, sorted with the candidate
+// positions as payload: a stable radix sort on the significant bits only, so positions stay ascending inside an id.
+template <class K>
+static int sort_inverted_index(dbl_ctx *ctx, long long n_ids, long long spread, int bits) {
+  const int64_t cap = ctx->E * ctx->A;
+  // the slot count (inv_pos) and the key bytes together identify (cap, key width); the byte size alone does not
+  if (ctx->inv_pos.n != (size_t)cap || ctx->inv_ids.n != (size_t)cap * sizeof(K)) {
+    CUDA_TRY(ctx->inv_ids_in.alloc((size_t)cap * sizeof(K)));
+    CUDA_TRY(ctx->inv_ids.alloc((size_t)cap * sizeof(K)));
+    CUDA_TRY(ctx->inv_pos_in.alloc(cap));
+    CUDA_TRY(ctx->inv_pos.alloc(cap));
+    size_t tb = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tb, (const K *)nullptr, (K *)nullptr, (const int *)nullptr, (int *)nullptr,
+                                    (int)cap, 0, 8 * (int)sizeof(K), ctx->stream);
+    if (ctx->inv_tmp_bytes < tb + 256) { ctx->inv_tmp_bytes = tb + 256; CUDA_TRY(ctx->inv_tmp.alloc(ctx->inv_tmp_bytes)); }
   }
-  *out = ctx->h_owned_ent;
+  K *ids_in = reinterpret_cast<K *>(ctx->inv_ids_in.p), *ids = reinterpret_cast<K *>(ctx->inv_ids.p);
+  k_inv_ids<<<grid_for(cap, 256), 256, 0, ctx->stream>>>(ctx->E, ctx->A, ctx->P, ctx->inv_dense, n_ids, spread, ctx->y.p,
+                                                       ctx->blk_sorted.p, ctx->ent_sorted.p, ctx->ent_ptr.p,
+                                                       ctx->perm_dev.p, ids_in, ctx->inv_pos_in.p);
+  size_t tb = ctx->inv_tmp_bytes;
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(ctx->inv_tmp.p, tb, (const K *)ids_in, ids, (const int *)ctx->inv_pos_in.p,
+                                           ctx->inv_pos.p, (int)cap, 0, bits, ctx->stream));
+  ctx->launches += 4;
   return DBL_OK;
 }
 
-// (block, attribute, value) -> candidate positions, for k_link_pruned
+// (block, attribute, value) -> candidate positions, for k_link_pruned.  One index whatever the sizes: 32-bit ids when
+// the id space and the sentinel spread fit, 64-bit otherwise.  When the dense pointer table is small enough (P * sum
+// of vocabulary sizes entries) a record finds its posting list with two loads; otherwise with two binary searches in
+// its block's range of the sorted ids.  No size depends on the shard: nothing is read back.
 static int ensure_inverted_index(dbl_ctx *ctx) {
   if (ctx->inv_valid) return DBL_OK;
   const int64_t cap = ctx->E * ctx->A;
@@ -2317,78 +2333,22 @@ static int ensure_inverted_index(dbl_ctx *ctx) {
   dn.A = ctx->A; dn.sumV = 0;
   for (int k = 0; k < ctx->A; ++k) { dn.voff[k] = dn.sumV; dn.sumV += ctx->h_attrs[ctx->perm[k]].V; }
   const long long n_ids = (long long)ctx->P * dn.sumV;
+  int bits;
+  long long spread;
+  sentinel_spread(n_ids, ctx->world, &bits, &spread);
+  ctx->inv_ids64 = bits > 32;
+  int rc = ctx->inv_ids64 ? sort_inverted_index<unsigned long long>(ctx, n_ids, spread, bits)
+                          : sort_inverted_index<unsigned>(ctx, n_ids, spread, bits);
+  if (rc) return rc;
   long long dense_max = 1ll << 25;  // entries; DBL_INV_DENSE_MAX overrides (tests force the binary-search path with 0)
   if (const char *ev = getenv("DBL_INV_DENSE_MAX")) dense_max = atoll(ev);
-  ctx->inv_use_dense = n_ids <= dense_max;
-  int vmax = 1;
-  for (int a = 0; a < ctx->A; ++a) vmax = std::max(vmax, ctx->h_attrs[a].V);
-  ctx->inv_vbits = bits_for(vmax + 1);
-  dn.vbits = ctx->inv_vbits;
-
+  ctx->inv_use_dense = !ctx->inv_ids64 && n_ids <= dense_max;  // 64-bit ids: a table of more than 2^32 entries
   if (ctx->inv_use_dense) {
-    // dense (block, attribute, value) -> posting pointers: the table is small enough (P * sum of vocabulary sizes
-    // entries).  32-bit keys (the dense id), every slot of the sorted table sorted (non-owned rows carry the
-    // sentinel id): no size depends on the shard, nothing is read back.
-    if (ctx->inv_key32.n != (size_t)cap) {
-      CUDA_TRY(ctx->inv_key32_in.alloc(cap));
-      CUDA_TRY(ctx->inv_key32.alloc(cap));
-      if (ctx->inv_pos.n != (size_t)cap) { CUDA_TRY(ctx->inv_pos_in.alloc(cap)); CUDA_TRY(ctx->inv_pos.alloc(cap)); }
-      size_t tb = 0;
-      cub::DeviceRadixSort::SortPairs(nullptr, tb, (const unsigned *)nullptr, (unsigned *)nullptr, (const int *)nullptr,
-                                      (int *)nullptr, (int)cap, 0, 32, ctx->stream);
-      if (ctx->inv_tmp_bytes < tb + 256) { ctx->inv_tmp_bytes = tb + 256; CUDA_TRY(ctx->inv_tmp.alloc(ctx->inv_tmp_bytes)); }
-    }
     if (ctx->inv_vptr.n != (size_t)n_ids + 1) CUDA_TRY(ctx->inv_vptr.alloc((size_t)n_ids + 1));
-    int ibits;
-    long long ispread;
-    sentinel_spread(n_ids, ctx->world, &ibits, &ispread);
-    k_inv_keys32<<<grid_for(cap, 256), 256, 0, ctx->stream>>>(ctx->E, ctx->A, ctx->P, dn, n_ids, ispread, ctx->y.p,
-                                                             ctx->blk_sorted.p, ctx->ent_sorted.p, ctx->ent_ptr.p,
-                                                             ctx->perm_dev.p, ctx->inv_key32_in.p, ctx->inv_pos_in.p);
-    size_t tb = ctx->inv_tmp_bytes;
-    // stable radix sort on the significant bits only: positions stay ascending inside a key
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(ctx->inv_tmp.p, tb, (const unsigned *)ctx->inv_key32_in.p, ctx->inv_key32.p,
-                                             (const int *)ctx->inv_pos_in.p, ctx->inv_pos.p, (int)cap, 0,
-                                             ibits, ctx->stream));
-    k_inv_value_ptr32<<<grid_for(cap + 1, 256), 256, 0, ctx->stream>>>(cap, n_ids, (long long)dn.sumV, ctx->inv_key32.p,
-                                                                       ctx->inv_vptr.p);
-    ctx->launches += 5;
-    ctx->inv_valid = true;
-    CUDA_TRY(cudaGetLastError());
-    return DBL_OK;
+    k_inv_value_ptr32<<<grid_for(cap + 1, 256), 256, 0, ctx->stream>>>(cap, n_ids, (long long)dn.sumV,
+                                                                       (const unsigned *)ctx->inv_ids.p, ctx->inv_vptr.p);
+    ctx->launches += 1;
   }
-
-  // too many (block, attribute, value) ids for a dense table: 64-bit keys ((block, attribute) group | value) over the
-  // entities of owned blocks (they come first in ent_sorted), (block, attribute) segment pointers, and a binary
-  // search per record.  The owned count sizes the sort, so a sharded context reads it back once per sweep.
-  int64_t owned = 0;
-  { int rc = owned_entities_on_host(ctx, &owned); if (rc) return rc; }
-  const int64_t n = owned * ctx->A;
-  if (ctx->inv_key.n != (size_t)cap) {
-    CUDA_TRY(ctx->inv_key_in.alloc(cap));
-    CUDA_TRY(ctx->inv_key.alloc(cap));
-    if (ctx->inv_pos.n != (size_t)cap) { CUDA_TRY(ctx->inv_pos_in.alloc(cap)); CUDA_TRY(ctx->inv_pos.alloc(cap)); }
-    size_t tb = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tb, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
-                                    (const int *)nullptr, (int *)nullptr, (int)cap, 0, 64, ctx->stream);
-    if (ctx->inv_tmp_bytes < tb + 256) { ctx->inv_tmp_bytes = tb + 256; CUDA_TRY(ctx->inv_tmp.alloc(ctx->inv_tmp_bytes)); }
-  }
-  const int nbits = ctx->inv_vbits + bits_for((int64_t)(ctx->P + 1) * ctx->A);
-  if (n > 0) {
-    k_inv_keys<<<grid_for(n, 256), 256, 0, ctx->stream>>>(owned, ctx->A, ctx->P, ctx->inv_vbits,
-                                                          ctx->y.p, ctx->blk_sorted.p, ctx->ent_sorted.p,
-                                                          ctx->ent_ptr.p, ctx->perm_dev.p, ctx->inv_key_in.p,
-                                                          ctx->inv_pos_in.p);
-    size_t tb = ctx->inv_tmp_bytes;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(ctx->inv_tmp.p, tb, (const unsigned long long *)ctx->inv_key_in.p,
-                                             ctx->inv_key.p, (const int *)ctx->inv_pos_in.p, ctx->inv_pos.p, (int)n,
-                                             0, std::min(64, nbits), ctx->stream));
-  }
-  const int n_groups = (ctx->P + 1) * ctx->A;
-  if (ctx->inv_seg.n != (size_t)n_groups + 1) CUDA_TRY(ctx->inv_seg.alloc((size_t)n_groups + 1));
-  k_inv_segments<<<grid_for(n + 1, 256), 256, 0, ctx->stream>>>(n, n_groups, ctx->inv_vbits, ctx->inv_key.p,
-                                                                ctx->inv_seg.p);
-  ctx->launches += 5;
   ctx->inv_valid = true;
   CUDA_TRY(cudaGetLastError());
   return DBL_OK;
@@ -2408,6 +2368,19 @@ static int dispatch_pcg2(dbl_ctx *ctx, int grid, const LinkParams &lp) {
   }
   if (rc != 0) { ctx->set_error(std::string("k_link_pcg2 launch: ") + cudaGetErrorString((cudaError_t)rc)); return DBL_ERR_CUDA; }
   return DBL_OK;
+}
+
+// k_link_match stages LINK_STAGES attribute-major tiles in dynamic shared memory
+static size_t match_ring_bytes(int A) { return (size_t)LINK_STAGES * tile_words(A) * 4 + 128; }
+
+// the link kernel a sweep with this sampler launches, numbered as dbl_link_kernel reports it
+enum LinkKernel { LINK_GENERIC = 0, LINK_MATCH = 1, LINK_PRUNED = 2, LINK_PCG2 = 3 };
+static LinkKernel link_kernel(const dbl_ctx *ctx, int sampler) {
+  const int mode = ctx->link_mode;  // 0 auto, 1 force generic, 2 dense kernels for every sampler
+  if (mode != 1 && sampler == DBL_PCG_II && pcg2_kernel_fits(ctx)) return LINK_PCG2;
+  if (mode == 0 && sampler != DBL_PCG_II) return LINK_PRUNED;
+  if (mode != 1 && sampler != DBL_PCG_II && match_ring_bytes(ctx->A) <= 160 * 1024) return LINK_MATCH;
+  return LINK_GENERIC;
 }
 
 static int launch_link(dbl_ctx *ctx, int sampler) {
@@ -2436,10 +2409,9 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
     }
     lp.link_mass = ctx->link_mass.p;
   }
-  const size_t ring = (size_t)LINK_STAGES * tile_words(A) * 4 + 128;
-  const int mode = ctx->link_mode;  // 0 auto, 1 force generic
   lp.hslots = ctx->hslots; lp.hshift = ctx->hshift;
-  if (mode != 1 && sampler == DBL_PCG_II && pcg2_kernel_fits(ctx)) {
+  const LinkKernel kernel = link_kernel(ctx, sampler);
+  if (kernel == LINK_PCG2) {
     // persistent CTAs: a few per SM, each takes groups of LINK_WARPS records from the work counter until none is left
     // (k_theta zeroed the counter; the block-level API launches the kernel once per block after one k_theta)
     if (ctx->in_block_sweep) CUDA_TRY(cudaMemsetAsync(lp.work, 0, sizeof(unsigned long long), ctx->stream));
@@ -2452,25 +2424,17 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
     int rc = ensure_tiles(ctx, 1);  // every other link kernel reads the attribute-major tiles
     if (rc) return rc;
   }
-  if (mode == 0 && sampler != DBL_PCG_II) {  // pruned scoring through the inverted index
+  if (kernel == LINK_PRUNED) {  // pruned scoring through the inverted index
     int rc = ensure_inverted_index(ctx);
     if (rc) return rc;
-    int64_t owned = 0;
-    if (!ctx->inv_use_dense) {
-      rc = owned_entities_on_host(ctx, &owned);
-      if (rc) return rc;
-    }
     PrunedParams pp;
     pp.lp = lp;
-    pp.inv_key = ctx->inv_key.p;
     pp.inv_pos = ctx->inv_pos.p;
-    pp.inv_n = (long long)owned * ctx->A;
-    pp.R = ctx->R;
-    pp.vbits = ctx->inv_vbits;
-    pp.inv_seg = ctx->inv_seg.p;
     pp.rec_key_sorted = ctx->rec_key_sorted.p;
     pp.rec_key_shift = REC_CLASS_BITS;
     pp.inv_vptr = ctx->inv_use_dense ? ctx->inv_vptr.p : nullptr;
+    pp.inv_key32 = ctx->inv_ids64 ? nullptr : reinterpret_cast<const unsigned *>(ctx->inv_ids.p);
+    pp.inv_key64 = ctx->inv_ids64 ? reinterpret_cast<const unsigned long long *>(ctx->inv_ids.p) : nullptr;
     pp.sumV = ctx->inv_dense.sumV;
     for (int k = 0; k < A; ++k) pp.voff[k] = ctx->inv_dense.voff[k];
     if (ctx->heavy_list.n != (size_t)ctx->R) CUDA_TRY(ctx->heavy_list.alloc((size_t)ctx->R));
@@ -2485,7 +2449,8 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
     ctx->launches += 1;
     return DBL_OK;
   }
-  if (mode != 1 && sampler != DBL_PCG_II && ring <= 160 * 1024) {
+  if (kernel == LINK_MATCH) {
+    const size_t ring = match_ring_bytes(A);
     if (ctx->match_smem_cfg < ring) {
       CUDA_TRY(cudaFuncSetAttribute(k_link_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring));
       ctx->match_smem_cfg = ring;
@@ -2501,7 +2466,7 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
 
 // ---------------------------------------------------------------------------------------------------
 // one application of State.nextState (State.scala:78-99), enqueued on the context's stream without any host
-// synchronisation (PCG-II; the pruned PCG-I kernel of a SHARDED context reads one count back per sweep)
+// synchronisation
 // ---------------------------------------------------------------------------------------------------
 // (1) theta | summary of the previous state (State.scala:83, GU:305-320)
 static int enqueue_theta(dbl_ctx *ctx) {
@@ -2616,9 +2581,6 @@ static int check_sweep_args(dbl_ctx *ctx, int sampler, int32_t n_sweeps) {
 // enqueueing it again: nothing in a sweep depends on the host, every varying quantity is read from device memory.
 static bool graph_allowed(const dbl_ctx *ctx, int sampler) {
   if (ctx->graph_mode == 1) return false;
-  // the pruned link update of a SHARDED context without the dense posting table reads the owned-entity count back
-  // every sweep (it sizes a sort)
-  if (ctx->world > 1 && sampler != DBL_PCG_II && ctx->link_mode == 0 && !ctx->inv_use_dense) return false;
   if (ctx->graph_mode == 2) return true;
   // PCG-II at large sizes: tens of milliseconds of GPU time per sweep hide the ~35 launches.  The pruned samplers
   // do not: their sweep is ~3 ms of GPU time at 1 M records and shrinks with the rank count while the host's share
@@ -2838,7 +2800,7 @@ static int preload_kernels(dbl_ctx *ctx) {
   DBL_LOAD(k_unpack_ent_p2p); DBL_LOAD(k_unpack_rec_p2p); DBL_LOAD(k_reduce_peers); DBL_LOAD(k_lpt);
   DBL_LOAD(k_link_generic); DBL_LOAD(k_link_match); DBL_LOAD(k_link_pruned); DBL_LOAD(k_state_hash);
   DBL_LOAD(k_gather_ent); DBL_LOAD(k_gather_rec); DBL_LOAD(k_export_ent); DBL_LOAD(k_export_rec);
-  DBL_LOAD(k_inv_keys); DBL_LOAD(k_inv_keys32); DBL_LOAD(k_inv_value_ptr32); DBL_LOAD(k_inv_segments);
+  DBL_LOAD(k_inv_ids<unsigned>); DBL_LOAD(k_inv_ids<unsigned long long>); DBL_LOAD(k_inv_value_ptr32);
 #undef DBL_LOAD
   if (pcg2_kernel_fits(ctx)) {
     LinkParams lp;
@@ -3158,13 +3120,9 @@ extern "C" int dbl_state_hash(dbl_ctx *ctx, uint64_t *hash_out) {
 // 3 k_link_pcg2 (+4 when the constants are byte-packed, +8 when the hash tables have the compile-time 32 slots)
 extern "C" int dbl_link_kernel(const dbl_ctx *ctx, int sampler) {
   if (!ctx || sampler < 0 || sampler > 3) return DBL_ERR_INVALID;
-  const int mode = ctx->link_mode;
-  if (mode != 1 && sampler == DBL_PCG_II && pcg2_kernel_fits(ctx))
-    return 3 + (ctx->qtile_pk ? 4 : 0) + (ctx->hslots == 32 ? 8 : 0);
-  if (mode == 0 && sampler != DBL_PCG_II) return 2;
-  const size_t ring = (size_t)LINK_STAGES * tile_words(ctx->A) * 4 + 128;
-  if (mode != 1 && sampler != DBL_PCG_II && ring <= 160 * 1024) return 1;
-  return 0;
+  const LinkKernel kernel = link_kernel(ctx, sampler);
+  if (kernel == LINK_PCG2) return kernel + (ctx->qtile_pk ? 4 : 0) + (ctx->hslots == 32 ? 8 : 0);
+  return kernel;
 }
 
 extern "C" int dbl_set_link_mode(dbl_ctx *ctx, int mode) {

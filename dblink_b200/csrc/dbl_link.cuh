@@ -604,53 +604,27 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
 // candidates that agree with the record on its most selective observed non-distorted attribute are visited;
 // every other candidate has weight exactly 0 in the dense kernel, and adding +0.0 never changes a sum, so the
 // lane sums, chunk totals and the draw are bit-identical to k_link_match / k_link_generic.
-// Index: entries (key = (block*A + kernel attribute) << 32 | value, payload = candidate position j) sorted by
-// key, positions ascending inside a key.
+// Index: entries (key = the dense id block * sumV + voff[kernel attribute] + value, payload = candidate position j)
+// sorted by key, positions ascending inside a key.
 // ---------------------------------------------------------------------------------------------------
 #ifdef DBL_ENGINE_TU
-// key = ((block * A + kernel attribute) << vbits) | value; rows this rank does not own go to the dummy block P
-__global__ void k_inv_keys(int64_t E, int A, int P, int vbits, const int *__restrict__ y,
-                           const int *__restrict__ blk_sorted, const int *__restrict__ ent_sorted,
-                           const int *__restrict__ ent_ptr, const int *__restrict__ perm,
-                           unsigned long long *__restrict__ key, int *__restrict__ pos) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= E * A) return;
-  const int64_t i = t / A;
-  const int k = (int)(t % A);
-  const int b = min(blk_sorted[i], P);
-  const int e = ent_sorted[i];
-  const unsigned long long v = (b < P) ? (unsigned)y[(int64_t)e * A + perm[k]] : 0u;
-  key[t] = ((unsigned long long)((unsigned)b * (unsigned)A + (unsigned)k) << vbits) | v;
-  pos[t] = (b < P) ? (int)(i - ent_ptr[b]) : -1;
-}
-
-// seg[g] = first index entry of group g = block * A + kernel attribute (one pass over the sorted keys)
-__global__ void k_inv_segments(int64_t n, int n_groups, int vbits, const unsigned long long *__restrict__ key,
-                               int *__restrict__ seg) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i > n) return;
-  const int cur = (i < n) ? (int)min((unsigned long long)n_groups, key[i] >> vbits) : n_groups;
-  const int prev = (i > 0) ? (int)min((unsigned long long)n_groups, key[i - 1] >> vbits) : -1;
-  for (int g = prev + 1; g <= cur; ++g) seg[g] = (int)i;
-}
-
-// vptr[(block * sumV) + voff[kernel attribute] + value] = first index entry of that (block, attribute, value); the
-// table is dense (values without entities get an empty range), so a record finds a posting list with two loads
+// offsets of the kernel attributes in the dense (block, attribute, value) id space
 struct InvDense {
-  int A, sumV, vbits;
+  int A, sumV;
   int voff[DBL_MAX_ATTRS];
 };
 
-// The same index with 32-bit keys = the dense (block, attribute, value) id itself, over ALL E * A slots of the sorted
-// entity table: rows of blocks this rank does not own get ids beyond n_ids and sort to the end.  Nothing here
-// depends on how many entities the rank owns, so a sharded sweep needs no read-back to size the sort.  The ids
-// beyond n_ids are spread over the rest of the key range (`spread` values): with ONE sentinel value 7/8 of the keys of an 8-rank shard were
-// equal, and a radix sort whose items all fall into one bin serialises on that bin (the sharded PCG-I sweep got slower
-// from 4 ranks to 8).
-__global__ void k_inv_keys32(int64_t E, int A, int P, InvDense d, long long n_ids, long long spread, const int *__restrict__ y,
-                             const int *__restrict__ blk_sorted, const int *__restrict__ ent_sorted,
-                             const int *__restrict__ ent_ptr, const int *__restrict__ perm,
-                             unsigned *__restrict__ key, int *__restrict__ pos) {
+// Keys over ALL E * A slots of the sorted entity table: rows of blocks this rank does not own get ids beyond n_ids
+// and sort to the end.  Nothing here depends on how many entities the rank owns, so a sharded sweep needs no read-back
+// to size the sort.  The ids beyond n_ids are spread over the rest of the key range (`spread` values): with ONE
+// sentinel value 7/8 of the keys of an 8-rank shard were equal, and a radix sort whose items all fall into one bin
+// serialises on that bin (the sharded PCG-I sweep got slower from 4 ranks to 8).  K is 32 bits wide unless the ids
+// and the spread need more.
+template <class K>
+__global__ void k_inv_ids(int64_t E, int A, int P, InvDense d, long long n_ids, long long spread, const int *__restrict__ y,
+                          const int *__restrict__ blk_sorted, const int *__restrict__ ent_sorted,
+                          const int *__restrict__ ent_ptr, const int *__restrict__ perm,
+                          K *__restrict__ key, int *__restrict__ pos) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= E * A) return;
   const int64_t i = t / A;
@@ -658,14 +632,15 @@ __global__ void k_inv_keys32(int64_t E, int A, int P, InvDense d, long long n_id
   const int b = blk_sorted[i];
   if (b < P) {
     const int e = ent_sorted[i];
-    key[t] = (unsigned)((long long)b * d.sumV + d.voff[k] + y[(int64_t)e * A + perm[k]]);
+    key[t] = (K)((long long)b * d.sumV + d.voff[k] + y[(int64_t)e * A + perm[k]]);
     pos[t] = (int)(i - ent_ptr[b]);
   } else {
-    key[t] = (unsigned)(n_ids + t % spread);
+    key[t] = (K)(n_ids + t % spread);
     pos[t] = -1;
   }
 }
-// vptr[id] = first sorted entry whose key is >= id.  The thread at a boundary between two different keys fills the ids
+// vptr[id] = first sorted entry whose key is >= id: a dense table (values without entities get an empty range), so a
+// record finds a posting list with two loads.  The thread at a boundary between two different keys fills the ids
 // in between.  On a shard the keys of whole blocks are missing (7/8 of the id space on 8 ranks): a boundary thread
 // filled up to ~2 million entries one after the other, and the sharded PCG-I sweep got SLOWER with every rank
 // added.  Nothing ever looks up an id of a block without entities (a record
@@ -688,30 +663,32 @@ __global__ void k_inv_value_ptr32(int64_t n, long long n_ids, long long sumV, co
   }
 }
 
-__device__ __forceinline__ int64_t inv_lower_bound(const unsigned long long *__restrict__ key, int64_t lo, int64_t hi,
-                                                   unsigned long long want) {
+struct PrunedParams {
+  LinkParams lp;
+  const int *inv_pos;
+  const int *rec_key_sorted;  // block-major sort key of rec_sorted[i]
+  int rec_key_shift;
+  // A posting list is [vptr[id], vptr[id + 1]).  Without the pointer table (nullptr) it is found by two binary
+  // searches in the sorted keys of the record's block b, positions [A * ent_ptr[b], A * ent_ptr[b + 1]): every owned
+  // entity contributes A keys inside its block's id range, and non-owned rows sort behind every id.
+  const int *inv_vptr;
+  const unsigned *inv_key32;  // the sorted keys, 32 or 64 bits wide: exactly one of the two is set
+  const unsigned long long *inv_key64;
+  int sumV;
+  int voff[DBL_MAX_ATTRS];
+  int *heavy_list;     // positions (in rec_sorted) of the records left to k_link_heavy; count in ctl[CTL_HEAVY]
+};
+
+// first position in [lo, hi) of the sorted keys whose key is >= want
+__device__ __forceinline__ long long inv_lower_bound(const PrunedParams &pp, long long lo, long long hi,
+                                                     unsigned long long want) {
   while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if (key[mid] < want) lo = mid + 1; else hi = mid;
+    const long long mid = (lo + hi) >> 1;
+    const unsigned long long key = pp.inv_key64 ? pp.inv_key64[mid] : pp.inv_key32[mid];
+    if (key < want) lo = mid + 1; else hi = mid;
   }
   return lo;
 }
-
-struct PrunedParams {
-  LinkParams lp;
-  const unsigned long long *inv_key;
-  const int *inv_pos;
-  long long inv_n;
-  long long R;
-  int vbits;
-  const int *rec_key_sorted;  // block-major sort key of rec_sorted[i]
-  int rec_key_shift;
-  const int *inv_vptr;  // dense (block, attribute, value) -> first entry; nullptr: binary search inside inv_seg
-  int sumV;
-  int voff[DBL_MAX_ATTRS];
-  const int *inv_seg;  // (P+1)*A + 1 group offsets
-  int *heavy_list;     // positions (in rec_sorted) of the records left to k_link_heavy; count in ctl[CTL_HEAVY]
-};
 
 // A record without any must-match attribute (every observed attribute distorted) has to score its whole block.  One
 // warp doing that is the tail of the whole kernel (RLdata10000 in steady state: one such record in a 2 500-entity
@@ -759,17 +736,14 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
       ra[lane] = c;
       mm = (c.kind == 4);
       if (mm) {
+        const long long id = (long long)b * pp.sumV + pp.voff[lane] + c.x;
         if (pp.inv_vptr) {
-          const long long id = (long long)b * pp.sumV + pp.voff[lane] + c.x;
           lo = pp.inv_vptr[id];
           len = pp.inv_vptr[id + 1] - lo;
         } else {
-          const unsigned long long base = (unsigned long long)((unsigned)b * (unsigned)A + (unsigned)lane) << pp.vbits;
-          const int g = b * A + lane;
-          const long long s0 = pp.inv_seg[g], s1 = pp.inv_seg[g + 1];  // the E_b entries of (block, attribute)
-          lo = inv_lower_bound(pp.inv_key, s0, s1, base | (unsigned)c.x);
-          const long long hi = inv_lower_bound(pp.inv_key, lo, s1, base | ((unsigned)c.x + 1u));
-          len = hi - lo;
+          const long long s1 = (long long)A * p.ent_ptr[b + 1];
+          lo = inv_lower_bound(pp, (long long)A * p.ent_ptr[b], s1, id);
+          len = inv_lower_bound(pp, lo, s1, id + 1) - lo;
         }
       }
     }

@@ -132,41 +132,89 @@ def test_chain_one_against_the_oracle(oracle):
     batch.close()
 
 
-def test_many_chains_take_the_wide_index_keys():
-    """enough chains that the PCG-I inverted index has more (block, attribute, value) ids than its dense table holds
-    (K B sum_a V_a > 2^25): the 64-bit-key path; a few chains checked against their one-chain runs"""
+def _many_chains(indexes, alpha, beta, x, file, F, more_ids_than):
+    """-> (batch, seeds): K chains on a 2-leaf tree, K just large enough that the PCG-I inverted index of the batch has
+    more than `more_ids_than` (block, attribute, value) ids (K B sum_a V_a), while the B sum_a V_a ids of one chain fit
+    the dense pointer table"""
     import dblink_b200 as D
 
-    g = synth_problem(seed=21, R=40, n_files=2)
-    rc, x, file, alpha, beta = _model(g)
-    F = len(rc.file_ids)
-    probe = D.GibbsEngine(rc.indexes, alpha, beta, None, 1000, F)
+    probe = D.GibbsEngine(indexes, alpha, beta, None, 1000, F)
     probe.init_state(x, file)
     part = D.KDTreePartitioner(1, [2]).fit(probe.download_state()["y"])
     probe.close()
     B = part.num_partitions
-    sum_v = sum(ix.num_values for ix in rc.indexes)
-    K = (1 << 25) // (B * sum_v) + 2
-    assert K * B * sum_v > (1 << 25)
+    sum_v = sum(ix.num_values for ix in indexes)
+    assert B * sum_v <= (1 << 25)
+    K = more_ids_than // (B * sum_v) + 2
+    assert K * B * sum_v > more_ids_than
     seeds = list(range(1000, 1000 + K))
-    batch = D.GibbsEngine(rc.indexes, alpha, beta, None, seeds[0], F)
+    batch = D.GibbsEngine(indexes, alpha, beta, None, seeds[0], F)
     batch.init_chains(x, file, 0, seeds)
     batch.set_partitioner(part)
     assert batch.num_partitions == K * B
     assert batch.link_kernel("PCG-I") == "k_link_pruned"
+    return batch, seeds
+
+
+def _equal_their_one_chain_runs(batch, seeds, indexes, alpha, beta, x, file, F, pop=0, part=None):
+    """chains 0, 1, K/2 and K-1 of the batch against one-chain runs: with the batch's partitioner (part=None), or with
+    `part` installed before the state is initialised, as it was on the batch"""
+    import dblink_b200 as D
+
+    K = len(seeds)
     check = [0, 1, K // 2, K - 1]
     ones = []
     for k in check:
-        e = D.GibbsEngine(rc.indexes, alpha, beta, None, seeds[k], F)
-        e.init_state(x, file)
-        e.set_partitioner(part)
+        e = D.GibbsEngine(indexes, alpha, beta, None, seeds[k], F)
+        if part is not None:
+            e.set_partitioner(part)
+        e.init_state(x, file, pop)
+        if part is None:
+            e.set_partitioner(batch.partitioner)
         ones.append(e)
     for n in (1, 2):
         for e in [batch] + ones:
             e.sweep("PCG-I", n)
         assert_chains_equal(batch, ones, chains=check)
-    for e in [batch] + ones:
+    for e in ones:
         e.close()
+
+
+def test_many_chains_take_the_wide_index_keys():
+    """enough chains that the PCG-I inverted index has more (block, attribute, value) ids than its dense pointer table
+    holds (K B sum_a V_a > 2^25): posting lists found by binary search in 32-bit ids"""
+    g = synth_problem(seed=21, R=40, n_files=2)
+    rc, x, file, alpha, beta = _model(g)
+    F = len(rc.file_ids)
+    batch, seeds = _many_chains(rc.indexes, alpha, beta, x, file, F, 1 << 25)
+    _equal_their_one_chain_runs(batch, seeds, rc.indexes, alpha, beta, x, file, F)
+    batch.close()
+
+
+def test_many_chains_take_the_64_bit_index_keys():
+    """a constant attribute with 2^22 values and enough chains that the (block, attribute, value) ids exceed 2^32:
+    the batch sorts 64-bit ids and finds posting lists by binary search, each one-chain run uses the pointer table.
+    Then the same context on one leaf with twice the entities: fewer than 2^32 ids, so 32-bit keys over twice the
+    slots -- as many key bytes as before, and the index buffers must still be resized for the new slot count."""
+    import dblink_b200 as D
+
+    g = synth_problem(seed=21, R=40, n_files=2)
+    rc, x, file, alpha, beta = _model(g)
+    V = 1 << 22
+    wide = D.AttributeIndex.from_tables(np.full(V, 1.0 / V), constant=True, expected_max_cluster_size=1)
+    s1 = x[:, 3].astype(np.int64)  # duplicates that agree on s1 agree on the new attribute too
+    x = np.ascontiguousarray(np.column_stack([x, np.where(s1 >= 0, (s1 * 40503 + 7) % V, -1)]), dtype=np.int32)
+    indexes, alpha, beta, F = list(rc.indexes) + [wide], alpha + [alpha[0]], beta + [beta[0]], len(rc.file_ids)
+    batch, seeds = _many_chains(indexes, alpha, beta, x, file, F, 1 << 32)
+    _equal_their_one_chain_runs(batch, seeds, indexes, alpha, beta, x, file, F)
+    K, R, sum_v = len(seeds), x.shape[0], sum(ix.num_values for ix in indexes)
+    assert (1 << 25) < K * sum_v < (1 << 32)
+    one_leaf = D.KDTreePartitioner(0, []).fit(batch.download_chains()[0]["y"])
+    batch.set_partitioner(one_leaf)
+    batch.init_chains(x, file, 2 * R, seeds)
+    assert batch.num_partitions == K and batch.num_entities == 2 * R
+    _equal_their_one_chain_runs(batch, seeds, indexes, alpha, beta, x, file, F, pop=2 * R, part=one_leaf)
+    batch.close()
 
 
 @pytest.mark.parametrize("sampler", ["PCG-I", "Gibbs"])

@@ -66,6 +66,26 @@ def test_sharded_chain_equals_oracle(oracle, world, sampler):
     sh.close()
 
 
+@pytest.mark.parametrize("world", [2, 3])
+@pytest.mark.parametrize("sampler", ["PCG-I", "Gibbs"])
+def test_sharded_chain_without_dense_pointers(oracle, world, sampler, monkeypatch):
+    """the pruned link update of every rank with the (block, attribute, value) pointer table disabled: posting lists
+    found by binary search in the record's block range of the sorted index ids, eagerly and replayed from a captured
+    graph (several sweeps per call); the chain is the oracle's"""
+    monkeypatch.setenv("DBL_INV_DENSE_MAX", "0")
+    g = synth_problem(seed=5, R=1500, n_files=2)
+    sh, rc, x, file = make(world, g, 99, 3, (2, 3))
+    m, st, tree, ox, ofile = oracle_setup(oracle, g, 99, 3, (2, 3))
+    for it in range(4):
+        sh.sweep(sampler, 1)
+        assert st.sweep(oracle.SAMPLERS[sampler]) == 0
+        assert_same(sh, st)
+    sh.sweep(sampler, 3)
+    assert st.sweep(oracle.SAMPLERS[sampler], 3) == 0
+    assert_same(sh, st)
+    sh.close()
+
+
 def test_device_side_replacement_keeps_the_chain(oracle):
     """blocks start on a deliberately bad placement (everything on rank 0); the LPT kernel re-places them from the
     global block sizes and the blocks migrate as cluster messages; the chain is the oracle's throughout"""

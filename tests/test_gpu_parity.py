@@ -320,8 +320,8 @@ def test_sweep_block_by_block(oracle, sampler):
 
 
 def test_pruned_link_update_without_dense_pointers(oracle, monkeypatch):
-    """PCG-I with the (block, attribute, value) pointer table disabled: posting lists found by binary search inside
-    the (block, attribute) segments; same draws."""
+    """PCG-I with the (block, attribute, value) pointer table disabled: posting lists found by binary search in the
+    record's block range of the sorted index ids; same draws."""
     monkeypatch.setenv("DBL_INV_DENSE_MAX", "0")
     g = synth_problem(seed=21, R=1000, n_files=2)
     eng, rc, x, file = product_setup(g, 5, 2, (2, 3))
