@@ -309,8 +309,8 @@ __global__ void k_block_scan(int P, const int *__restrict__ ent_ptr, const int *
   }
 }
 // Tiled, block-sorted copies of the entity table, one thread per tile slot (padding slots of a block's last tile are
-// zeroed here: no memset of the whole table).  fmt 1: attribute-major tiles { int32 y[A][TE]; f64 N[TE]; uint32
-// packed_consts[TE] } (k_link_generic / k_link_match / k_link_pruned); fmt 2: quad tiles (k_link_pcg2).
+// zeroed here: no memset of the whole table).  fmt 1: attribute-major tiles { int32 y[A][TE]; f64 N[TE] }
+// (k_link_generic / k_link_match / k_link_pruned); fmt 2: quad tiles (k_link_pcg2).
 __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__restrict__ y, const double *__restrict__ entN,
                               const int *__restrict__ ent_sorted, const int *__restrict__ ent_ptr,
                               const int *__restrict__ tile_ptr, int *__restrict__ tiles, const int *__restrict__ perm, int P,
@@ -328,16 +328,15 @@ __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__rest
   const int j = (T - tile_ptr[b]) * TE + slot;
   const bool real = j < ent_ptr[b + 1] - ent_ptr[b];
   const int64_t e = real ? ent_sorted[ent_ptr[b] + j] : 0;
-  unsigned pk = 0;  // constant attributes (kernel positions 0..npack-1), one byte each, for k_link_pcg2
-  if (real)
-    for (int k = 0; k < npack; ++k) pk |= ((unsigned)y[e * A + perm[k]] & 0xFFu) << (8 * k);
   const double nn = real ? entN[e] : 0.0;
   if (fmt == 1) {
     int *tile = tiles + (size_t)T * tile_words(A);
     for (int k = 0; k < A; ++k) tile[k * TE + slot] = real ? y[e * A + perm[k]] : 0;  // kernel order
     reinterpret_cast<double *>(tile + (size_t)A * TE)[slot] = nn;
-    tile[(size_t)(A + 2) * TE + slot] = (int)pk;
   } else {
+    unsigned pk = 0;  // constant attributes (kernel positions 0..npack-1), one byte each
+    if (real)
+      for (int k = 0; k < npack; ++k) pk |= ((unsigned)y[e * A + perm[k]] & 0xFFu) << (8 * k);
     const int nv = qtile_nv(A, n_str, qtile_pk != 0), ng = qtile_groups(nv), qw = qtile_words(nv);
     int *qt = qtiles + (size_t)T * qw * TE;
     int v[4];
@@ -402,9 +401,7 @@ __global__ void k_finish(long long *__restrict__ ctl) {
 // ---------------------------------------------------------------------------------------------------
 // batched loads of k_values on sizes that fill the GPU (see value_update): pairs (2) beat none (1) and four at a time
 // (64 registers either way: with four the spills grow)
-#ifndef DBL_VALUES_UB_LARGE
-#define DBL_VALUES_UB_LARGE 2
-#endif
+constexpr int VALUES_UB_LARGE = 2;
 struct ValParams {
   int A, F, sampler;
   uint64_t seed;
@@ -1325,7 +1322,7 @@ struct dbl_ctx {
   DevBuf<int> perm_dev;
   int perm[DBL_MAX_ATTRS] = {0};
   int n_str = 0;       // non-constant attributes
-  int pack_consts = 0; // constant attributes byte-packed into the tiles (0 = none)
+  int pack_consts = 0; // constant attributes byte-packed into the quad tiles (0 = none)
   int hslots = 32, hshift = 27;  // common hash-table size of the non-constant attributes; hslots = 0: none
   std::vector<AttrDev> h_attrs;
   DevBuf<int> tree_buf;
@@ -1448,7 +1445,7 @@ struct dbl_ctx {
   int64_t phase_sweeps = 0;
   size_t pcg2_smem_cfg = 0, match_smem_cfg = 0;  // dynamic shared memory opted in on THIS device
   int sm_count = 132;                           // replaced by the device's count in dbl_ctx_create
-  int pcg2_grid = 132 * DBL_PCG2_CTAS_PER_SM;   // persistent CTAs of k_link_pcg2
+  int pcg2_grid = 0;                            // persistent CTAs of k_link_pcg2 (set by alloc_blocks)
   int pcg2_recs = LINK_WARPS;                   // records per work item of k_link_pcg2
   bool async_open = false;  // sweeps enqueued by dbl_sweep_async, not yet collected by dbl_sync
   // CUDA graphs of one sweep (launch-bound problem sizes): key = sampler * 4 + link mode
@@ -1741,7 +1738,7 @@ static int alloc_blocks(dbl_ctx *ctx) {
   {
     // work item and grid of the persistent PCG-II kernel for this model shape (see pcg2_rpw)
     const int hc = ctx->hslots == 32 ? 32 : 0;
-    ctx->pcg2_recs = pcg2_warps(hc, ctx->n_str) * pcg2_rpw(hc, ctx->n_str);
+    ctx->pcg2_recs = LINK_WARPS * pcg2_rpw(hc, ctx->n_str);
     ctx->pcg2_grid = ctx->sm_count * pcg2_ctas_per_sm(hc, ctx->n_str);
     const size_t need = (size_t)ctx->pcg2_grid * ctx->pcg2_recs * 1024;
     if (ctx->lane_sums.n < need) CUDA_TRY(ctx->lane_sums.alloc(need));
@@ -2370,16 +2367,13 @@ static int dispatch_pcg2(dbl_ctx *ctx, int grid, const LinkParams &lp) {
   return DBL_OK;
 }
 
-// k_link_match stages LINK_STAGES attribute-major tiles in dynamic shared memory
-static size_t match_ring_bytes(int A) { return (size_t)LINK_STAGES * tile_words(A) * 4 + 128; }
-
 // the link kernel a sweep with this sampler launches, numbered as dbl_link_kernel reports it
 enum LinkKernel { LINK_GENERIC = 0, LINK_MATCH = 1, LINK_PRUNED = 2, LINK_PCG2 = 3 };
 static LinkKernel link_kernel(const dbl_ctx *ctx, int sampler) {
   const int mode = ctx->link_mode;  // 0 auto, 1 force generic, 2 dense kernels for every sampler
   if (mode != 1 && sampler == DBL_PCG_II && pcg2_kernel_fits(ctx)) return LINK_PCG2;
   if (mode == 0 && sampler != DBL_PCG_II) return LINK_PRUNED;
-  if (mode != 1 && sampler != DBL_PCG_II && match_ring_bytes(ctx->A) <= 160 * 1024) return LINK_MATCH;
+  if (mode != 1 && sampler != DBL_PCG_II) return LINK_MATCH;
   return LINK_GENERIC;
 }
 
@@ -2398,8 +2392,6 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
   lp.status = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_STATUS);
   lp.pairs = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_PAIRS);
   for (int k = 0; k < A; ++k) lp.perm[k] = ctx->perm[k];
-  lp.blk_of_link = ctx->blk.p;
-  lp.pack_consts = ctx->pack_consts;
   lp.chain_seeds = ctx->chain_map().seeds;
   lp.chain_recs = ctx->chain_map().recs;
   if (ctx->link_mass_on) {
@@ -2450,7 +2442,7 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
     return DBL_OK;
   }
   if (kernel == LINK_MATCH) {
-    const size_t ring = match_ring_bytes(A);
+    const size_t ring = (size_t)LINK_STAGES * tile_words(A) * 4 + 128;  // the tile ring of k_link_match
     if (ctx->match_smem_cfg < ring) {
       CUDA_TRY(cudaFuncSetAttribute(k_link_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring));
       ctx->match_smem_cfg = ring;
@@ -2501,7 +2493,7 @@ static int update_owned(dbl_ctx *ctx, int sampler) {
   vp.ent_rec_ptr = ctx->ent_rec_ptr.p; vp.rec_by_ent = ctx->rec_by_ent.p; vp.y = ctx->y.p;
   // latency-bound sizes (the grid does not fill the GPU a few times over): the variant with batched loads
   if (ctx->E * A <= (int64_t)ctx->sm_count * 2048 * 4) k_values<8><<<grid_rows(ctx, ctx->E * A, 128), 128, 0, ctx->stream>>>(vp);
-  else k_values<DBL_VALUES_UB_LARGE><<<grid_rows(ctx, ctx->E * A, 128), 128, 0, ctx->stream>>>(vp);
+  else k_values<VALUES_UB_LARGE><<<grid_rows(ctx, ctx->E * A, 128), 128, 0, ctx->stream>>>(vp);
   ctx->launches += 1;
   // (4) N(e), new block ids, distortions, partial summary
   return refresh_summary(ctx, true);
@@ -2795,7 +2787,7 @@ extern "C" int dbl_set_rebalance(dbl_ctx *ctx, int32_t period, double threshold)
 static int preload_kernels(dbl_ctx *ctx) {
   cudaFuncAttributes fa;
 #define DBL_LOAD(k) CUDA_TRY(cudaFuncGetAttributes(&fa, k))
-  DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_tiles); DBL_LOAD(k_values<DBL_VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
+  DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_tiles); DBL_LOAD(k_values<VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
   DBL_LOAD(k_reduce_local); DBL_LOAD(k_finish); DBL_LOAD(k_move_ent); DBL_LOAD(k_move_rec); DBL_LOAD(k_publish_barrier);
   DBL_LOAD(k_unpack_ent_p2p); DBL_LOAD(k_unpack_rec_p2p); DBL_LOAD(k_reduce_peers); DBL_LOAD(k_lpt);
   DBL_LOAD(k_link_generic); DBL_LOAD(k_link_match); DBL_LOAD(k_link_pruned); DBL_LOAD(k_state_hash);
@@ -2805,7 +2797,7 @@ static int preload_kernels(dbl_ctx *ctx) {
   if (pcg2_kernel_fits(ctx)) {
     LinkParams lp;
     memset(&lp, 0, sizeof(lp));
-    lp.hslots = ctx->hslots; lp.pack_consts = ctx->pack_consts; lp.qtile_pk = ctx->qtile_pk;
+    lp.hslots = ctx->hslots; lp.qtile_pk = ctx->qtile_pk;
     int rc = dispatch_pcg2(ctx, 0, lp);  // grid 0 = load only
     if (rc) return rc;
   }

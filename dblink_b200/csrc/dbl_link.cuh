@@ -19,20 +19,14 @@
 #include "dbl_internal.h"
 
 constexpr int TE = 128;          // entities per tile of the block-sorted entity table
-#ifndef DBL_LINK_WARPS
-#define DBL_LINK_WARPS 8
-#endif
-constexpr int LINK_WARPS = DBL_LINK_WARPS;  // consumer warps (= records) per CTA
+constexpr int LINK_WARPS = 8;    // consumer warps (= records) per CTA
 constexpr int MATCH_WARPS = 16;  // ... of k_link_match, which is bound by L2 -> shared-memory tile traffic
-#ifndef DBL_LINK_STAGES
-#define DBL_LINK_STAGES 4
-#endif
-constexpr int LINK_STAGES = DBL_LINK_STAGES;  // tile ring depth
+constexpr int LINK_STAGES = 4;   // tile ring depth
 constexpr int LINK_MAX_UNROLL_A = 16;
 constexpr unsigned FULL = 0xffffffffu;
 
-// int32 words per tile: A value rows (attribute-major), the f64 row N(e), one row of byte-packed constant attributes
-__host__ __device__ inline size_t tile_words(int A) { return (size_t)A * TE + 3 * TE; }
+// int32 words per tile: A value rows (attribute-major), then the f64 row N(e)
+__host__ __device__ inline size_t tile_words(int A) { return (size_t)A * TE + 2 * TE; }
 // "Quad tiles" (k_link_pcg2): the words a lane needs about ONE candidate sit in groups of four, group-major
 // ([group][slot][4] int32), so that a warp fetches a group with one conflict-free 128-bit load per lane.  Words of an
 // entity: nv values (packed kernels: the NS non-constant values then the byte-packed constants; else all A values in
@@ -110,8 +104,6 @@ struct LinkParams {
   // "kernel order" of the attributes: constant attributes first, then the others, each group in ascending
   // attribute id.  Tiles, per-record constants and the multiplication order of the protocol use this order.
   int perm[DBL_MAX_ATTRS];
-  int pack_consts;         // tiles carry the byte-packed constant attributes (1..4 of them, vocabularies <= 255)
-  const int *blk_of_link;  // block id of every entity (k_link_pruned: block of a record = block of its entity)
   int hslots, hshift;  // common size of the per-row similarity hash tables (k_link_pcg2); 0 = unavailable
   double *link_mass;   // R entries or null: every link kernel stores the total mass of each record's categorical
   const uint64_t *chain_seeds;  // batched chains: one key per chain (nullptr: one chain, `seed`)
@@ -164,31 +156,77 @@ __device__ __forceinline__ int find_block(const LinkParams &p, int cta) {
   return lo;
 }
 
-// Second half of the draw (DESIGN.md section 4.3): given the check-pointed running totals Q (lane c = end of
-// chunk c) locate u*total: chunk -> lane (Kogge-Stone scan of the chunk's lane sums) -> step.  wf(j) must
-// reproduce the pass-1 weight of candidate j bit for bit (0 for j >= n).
-// lane_sums (optional): the lane sums of EVERY chunk as pass 1 produced them ([chunk][lane], this warp's scratch):
-// the chosen chunk's sums are read back instead of being recomputed (1/nchunks of pass 1 per record otherwise).
-template <class WeightFn>
-__device__ __forceinline__ int finish_draw(int lane, int n, int nsteps, int spc, int nchunks, double Q, double total,
-                                           double u, WeightFn wf, const double *lane_sums = nullptr) {
-  const double t = u * total;
-  unsigned m = __ballot_sync(FULL, lane < nchunks && Q > t);
+// ---------------------------------------------------------------------------------------------------
+// the categorical draw of a record's new link (DESIGN.md section 4.2), one implementation for every link kernel
+// ---------------------------------------------------------------------------------------------------
+// Lane l scores candidate 32 step + l; a chunk is a whole number of tiles, at most 32 chunks per block.
+struct DrawGeom {
+  int nsteps;   // steps of 32 candidates; steps beyond the last candidate add zeros
+  int tpc;      // tiles per chunk
+  int spc;      // steps per chunk
+  int nchunks;
+};
+__device__ __forceinline__ DrawGeom draw_geom(int ntiles) {
+  DrawGeom g;
+  g.nsteps = ntiles * (TE / 32);
+  g.tpc = max(1, (ntiles + 31) >> 5);
+  g.spc = (TE / 32) * g.tpc;
+  g.nchunks = (g.nsteps + g.spc - 1) / g.spc;
+  return g;
+}
+
+// Closes chunk c of pass 1's running total: adds the chunk's total, the xor butterfly of the lanes' sums over it, and
+// lane c keeps the new total in Q, the chunk's check-point.  k_link_pcg2 calls it directly: its two records per warp
+// share one chunk counter (a Checkpoints per record added spill bytes to the unpacked instantiations).
+__device__ __forceinline__ void close_chunk(int lane, int c, double lane_sum, double &run, double &Q) {
+  run = run + butterfly_sum(lane_sum);
+  if (lane == c) Q = run;
+}
+// The check-points of one record's pass 1: chunks are closed in order, `chunk` is the one being accumulated.
+struct Checkpoints {
+  double run = 0.0, Q = 0.0;
+  int chunk = 0;
+  __device__ __forceinline__ void close(int lane, double lane_sum) { close_chunk(lane, chunk++, lane_sum, run, Q); }
+  // passes over the chunks before c_next that hold no mass: their check-points are the total so far
+  __device__ __forceinline__ void pass_to(int lane, int c_next) {
+    if (lane >= chunk && lane < c_next) Q = run;
+    chunk = c_next;
+  }
+};
+
+// The total of a record's categorical is stored for dbl_link_mass, zero and non-finite totals included.  A zero or
+// non-finite total fails the sweep and the record keeps its link.  Returns whether the draw can go on.
+__device__ __forceinline__ bool check_mass(const LinkParams &p, int lane, int r, double total) {
+  if (p.link_mass && lane == 0) p.link_mass[r] = total;
+  if (!(total > 0.0) || isinf(total)) {
+    if (lane == 0) {  // reference: IllegalArgumentException("zero probability mass")
+      atomicOr(p.status, (unsigned long long)ST_ZERO_MASS);
+      p.newlink[r] = p.link[r];
+    }
+    return false;
+  }
+  return true;
+}
+
+// Locating t = u * total, step one: the chunk whose check-point first exceeds t (the last chunk if none does) and,
+// in `before`, the total of the chunks ahead of it.
+__device__ __forceinline__ int draw_chunk(int lane, int nchunks, double Q, double t, double &before) {
+  const unsigned m = __ballot_sync(FULL, lane < nchunks && Q > t);
   const int chunk = m ? (__ffs(m) - 1) : (nchunks - 1);
-  double r = shfl_d(Q, chunk > 0 ? chunk - 1 : 0);
-  if (chunk == 0) r = 0.0;
-  const int s0 = chunk * spc, s1 = min(s0 + spc, nsteps);
-  double ls = 0.0;
-  if (lane_sums) ls = lane_sums[chunk * 32 + lane];
-  else
-    for (int s = s0; s < s1; ++s) ls = ls + wf((s << 5) + lane);
+  before = shfl_d(Q, chunk > 0 ? chunk - 1 : 0);
+  if (chunk == 0) before = 0.0;
+  return chunk;
+}
+// Step two: from the chunk's lane sums ls, the first lane whose inclusive Kogge-Stone scan exceeds t (if none does:
+// the last lane with mass, else lane 0) and, in `base`, the total ahead of that lane's candidates in the chunk.
+__device__ __forceinline__ int draw_lane(int lane, double ls, double before, double t, double &base) {
   double P = ls;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
     const double o = shfl_up_d(P, d);
     if (lane >= d) P = P + o;
   }
-  m = __ballot_sync(FULL, r + P > t);
+  const unsigned m = __ballot_sync(FULL, before + P > t);
   int L;
   if (m) L = __ffs(m) - 1;
   else {
@@ -196,8 +234,27 @@ __device__ __forceinline__ int finish_draw(int lane, int n, int nsteps, int spc,
     L = pos ? (31 - __clz(pos)) : 0;
   }
   const double Pprev = shfl_up_d(P, 1);
-  const double base_l = lane ? r + Pprev : r;
-  const double base = shfl_d(base_l, L);
+  const double base_l = lane ? before + Pprev : before;
+  base = shfl_d(base_l, L);
+  return L;
+}
+
+// The draw of the dense kernels with uniform u after pass 1: chunk -> lane -> step, the step by a walk of the chosen
+// lane's candidates in step order.  wf(j) must reproduce the pass-1 weight of candidate j bit for bit (0 for j >= n).
+// lane_sums (optional): the lane sums of EVERY chunk as pass 1 produced them ([chunk][lane], this warp's scratch):
+// the chosen chunk's sums are read back instead of being recomputed (1/nchunks of pass 1 per record otherwise).
+template <class WeightFn>
+__device__ __forceinline__ int finish_draw(int lane, int n, const DrawGeom &geo, double Q, double total, double u,
+                                           WeightFn wf, const double *lane_sums = nullptr) {
+  const double t = u * total;
+  double before, base;
+  const int chunk = draw_chunk(lane, geo.nchunks, Q, t, before);
+  const int s0 = chunk * geo.spc, s1 = min(s0 + geo.spc, geo.nsteps);
+  double ls = 0.0;
+  if (lane_sums) ls = lane_sums[chunk * 32 + lane];
+  else
+    for (int s = s0; s < s1; ++s) ls = ls + wf((s << 5) + lane);
+  const int L = draw_lane(lane, ls, before, t, base);
   double cum = 0.0;
   int step = -1, last_pos = -1;
   for (int g = s0; g < s1 && step < 0; g += 32) {
@@ -321,17 +378,6 @@ __device__ __forceinline__ void store_link(const LinkParams &p, int lane, int r,
     atomicAdd(p.pairs, (unsigned long long)visited);
   }
 }
-// the total a record's draw tests for zero / non-finite (dbl_link_mass), zero and non-finite totals included
-__device__ __forceinline__ void store_mass(const LinkParams &p, int lane, int r, double total) {
-  if (p.link_mass && lane == 0) p.link_mass[r] = total;
-}
-__device__ __forceinline__ void fail_link(const LinkParams &p, int lane, int r) {
-  if (lane == 0) {  // reference: IllegalArgumentException("zero probability mass")
-    atomicOr(p.status, (unsigned long long)ST_ZERO_MASS);
-    p.newlink[r] = p.link[r];
-  }
-}
-
 #ifdef DBL_ENGINE_TU  // non-template kernels live in exactly one translation unit (dbl_engine.cu)
 __global__ void __launch_bounds__(LINK_WARPS * 32) k_link_generic(LinkParams p) {
   __shared__ RecAttr s_ra[LINK_WARPS][DBL_MAX_ATTRS];
@@ -352,10 +398,7 @@ __global__ void __launch_bounds__(LINK_WARPS * 32) k_link_generic(LinkParams p) 
   }
   __syncwarp();
   const int n = p.ent_ptr[b + 1] - p.ent_ptr[b];
-  const int ntiles = (n + TE - 1) / TE;
-  const int nsteps = ntiles * (TE / 32);                       // steps beyond the last candidate add zeros
-  const int spc = (TE / 32) * max(1, (ntiles + 31) >> 5);      // a chunk is a whole number of tiles
-  const int nchunks = (nsteps + spc - 1) / spc;
+  const DrawGeom geo = draw_geom((n + TE - 1) / TE);
   const size_t tw = tile_words(A);
   const int *tiles = p.tiles + (size_t)p.tile_ptr[b] * tw;
   auto wf = [&](int j) -> double {
@@ -365,22 +408,20 @@ __global__ void __launch_bounds__(LINK_WARPS * 32) k_link_generic(LinkParams p) 
     const double N = reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot];
     return generic_weight(ra, A, pcg2, tile + slot, N);
   };
-  double run = 0.0, Q = 0.0, acc = 0.0;
-  int mark = min(spc, nsteps), chunk = 0;
-  for (int s = 0; s < nsteps; ++s) {
+  Checkpoints ck;
+  double acc = 0.0;
+  int mark = min(geo.spc, geo.nsteps);
+  for (int s = 0; s < geo.nsteps; ++s) {
     acc = acc + wf((s << 5) + lane);
     if (s + 1 == mark) {
-      run = run + butterfly_sum(acc);
-      if (lane == chunk) Q = run;
-      ++chunk;
+      ck.close(lane, acc);
       acc = 0.0;
-      mark = min(mark + spc, nsteps);
+      mark = min(mark + geo.spc, geo.nsteps);
     }
   }
-  store_mass(p, lane, r, run);
-  if (!(run > 0.0) || isinf(run)) { fail_link(p, lane, r); return; }
+  if (!check_mass(p, lane, r, ck.run)) return;
   const U2 u = link_uniform(p, r);
-  const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q, run, u.u0, wf);
+  const int j = finish_draw(lane, n, geo, ck.Q, ck.run, u.u0, wf);
   store_link(p, lane, r, b, n, j);
 }
 
@@ -413,10 +454,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, unsigned parity) {
         : "memory");
   }
 }
-#ifndef DBL_PRODUCER_HINT
-#define DBL_PRODUCER_HINT 0x989680u
-#endif
-// producer-side wait (off the critical path while the ring is full): long suspend-time hint so that the idle
+// producer-side wait (off the critical path while the ring is full): long suspend-time hint (10 ms) so that the idle
 // producer lane does not steal issue slots from the consumer warps
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t *bar, unsigned parity) {
   const uint32_t addr = smem_u32(bar);
@@ -425,7 +463,7 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint64_t *bar, unsigned parity
     asm volatile(
         "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\tselp.u32 %0, 1, 0, p;\n\t}"
         : "=r"(ok)
-        : "r"(addr), "r"(parity), "r"(DBL_PRODUCER_HINT)
+        : "r"(addr), "r"(parity), "r"(10000000u)
         : "memory");
   }
 }
@@ -444,9 +482,9 @@ struct TileRing {
   int tw;              // words per tile
 };
 
-__device__ __forceinline__ void ring_init(const TileRing &rg, int consumers, int producers = 1) {
+__device__ __forceinline__ void ring_init(const TileRing &rg, int consumers) {
   if (threadIdx.x == 0) {
-    for (int s = 0; s < LINK_STAGES; ++s) { mbar_init(&rg.full[s], producers); mbar_init(&rg.empty[s], consumers); }
+    for (int s = 0; s < LINK_STAGES; ++s) { mbar_init(&rg.full[s], 1); mbar_init(&rg.empty[s], consumers); }
     mbar_fence_init();
   }
   __syncthreads();
@@ -467,22 +505,6 @@ __device__ __forceinline__ void ring_produce(const TileRing &rg, const int *gsrc
     }
     mbar_arrive_expect_tx(&rg.full[s], bytes);
     tma_load_1d(rg.tiles + (size_t)s * rg.tw, gsrc + (size_t)t * rg.tw, bytes, &rg.full[s]);
-  }
-}
-
-// The same ring filled with 16-byte cp.async copies by all 32 lanes of the producer warp (SASS LDGSTS) instead of one
-// bulk copy per tile: every lane's copies arrive on the stage's barrier (initialised with 32 producers).
-__device__ __forceinline__ void ring_produce_ldgsts(const TileRing &rg, const int *gsrc, int ntiles, int base, int lane) {
-  const int vecs = rg.tw / 4;  // 16-byte pieces per tile
-  for (int t = 0; t < ntiles; ++t) {
-    const int g = base + t;
-    const int s = g % LINK_STAGES;
-    if (g >= LINK_STAGES) mbar_wait_relaxed(&rg.empty[s], ((g / LINK_STAGES) - 1) & 1);
-    const int *src = gsrc + (size_t)t * rg.tw;
-    int *dst = rg.tiles + (size_t)s * rg.tw;
-    for (int i = lane; i < vecs; i += 32)
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst + i * 4)), "l"(src + i * 4) : "memory");
-    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&rg.full[s])) : "memory");
   }
 }
 
@@ -541,17 +563,15 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
     nmm = __popc(__ballot_sync(FULL, mm));
     __syncwarp();
   }
-  const int nsteps = ntiles * (TE / 32);
-  const int tpc = max(1, (ntiles + 31) >> 5);
-  const int spc = (TE / 32) * tpc;
-  const int nchunks = (nsteps + spc - 1) / spc;
+  const DrawGeom geo = draw_geom(ntiles);
   const int *mma = s_mm_attr[warp];
   const int *mmx = s_mm_x[warp];
   const int off0 = nmm ? mma[0] * TE : 0;
   const int x0 = nmm ? mmx[0] : 0;
 
-  double run = 0.0, Q = 0.0, acc = 0.0;
-  int chunk = 0, tile_in_chunk = 0;
+  Checkpoints ck;
+  double acc = 0.0;
+  int tile_in_chunk = 0;
   for (int t = 0; t < ntiles; ++t) {
     const int s = t % LINK_STAGES;
     mbar_wait(&rg.full[s], (t / LINK_STAGES) & 1);
@@ -572,10 +592,8 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
           if (ok) acc = acc + generic_weight(ra, A, false, tile + slot, tileN[slot]);
         }
       }
-      if (++tile_in_chunk == tpc || t + 1 == ntiles) {
-        run = run + butterfly_sum(acc);
-        if (lane == chunk) Q = run;
-        ++chunk;
+      if (++tile_in_chunk == geo.tpc || t + 1 == ntiles) {
+        ck.close(lane, acc);
         acc = 0.0;
         tile_in_chunk = 0;
       }
@@ -583,9 +601,7 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
     __syncwarp();
     if (lane == 0) mbar_arrive(&rg.empty[s]);
   }
-  if (!active) return;
-  store_mass(p, lane, r, run);
-  if (!(run > 0.0) || isinf(run)) { fail_link(p, lane, r); return; }
+  if (!active || !check_mass(p, lane, r, ck.run)) return;
   auto wf = [&](int j) -> double {
     if (j >= n) return 0.0;
     const int *tile = gtiles + (size_t)(j / TE) * TW;
@@ -593,7 +609,7 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
     return generic_weight(ra, A, false, tile + slot, reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot]);
   };
   const U2 u = link_uniform(p, r);
-  const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q, run, u.u0, wf);
+  const int j = finish_draw(lane, n, geo, ck.Q, ck.run, u.u0, wf);
   store_link(p, lane, r, b, n, j);
 }
 #endif  // DBL_ENGINE_TU
@@ -777,11 +793,8 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
   }
   const int *mma = s_mm_attr[warp];
   const int *mmx = s_mm_x[warp];
-  const int nsteps = ntiles * (TE / 32);
-  const int tpc = max(1, (ntiles + 31) >> 5);
-  const int spc = (TE / 32) * tpc;
-  const int nchunks = (nsteps + spc - 1) / spc;
-  const int cand_per_chunk = TE * tpc;
+  const DrawGeom geo = draw_geom(ntiles);
+  const int cand_per_chunk = TE * geo.tpc;
 
   // candidate j of index entry idx, its protocol weight (0 unless it survives every must-match attribute)
   auto cand_weight = [&](long long idx, int &j) -> double {
@@ -799,14 +812,13 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
   };
 
   // ---- pass 1: lane sums per chunk from the survivors only
-  double run = 0.0, Q = 0.0, s = 0.0;
-  int cur = 0;
+  Checkpoints ck;
+  double s = 0.0;
   bool dirty = false;
-  auto close_chunks_until = [&](int c_next) {  // finalise chunks cur .. c_next-1 (only `cur` can hold mass)
-    if (cur < c_next) {
-      if (dirty) { run = run + butterfly_sum(s); s = 0.0; dirty = false; }
-      if (lane >= cur && lane < c_next) Q = run;
-      cur = c_next;
+  auto close_chunks_until = [&](int c_next) {  // finalise chunks ck.chunk .. c_next-1 (only the first can hold mass)
+    if (ck.chunk < c_next) {
+      if (dirty) { ck.close(lane, s); s = 0.0; dirty = false; }
+      ck.pass_to(lane, c_next);
     }
   };
   int ns = 0;  // survivors seen (stored while they fit)
@@ -860,22 +872,18 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
   }
   __syncwarp();
   if (ns == 1) {  // a single candidate with positive weight is drawn whatever the uniform is: skip the search
-    store_mass(p, lane, r, s_sw[warp][0]);  // = the dense kernels' total: every other weight is an exact zero
-    if (isinf(s_sw[warp][0])) { fail_link(p, lane, r); return; }
-    store_link(p, lane, r, b, phi - plo, s_sj[warp][0]);
+    // its weight is the dense kernels' total: every other weight is an exact zero
+    if (check_mass(p, lane, r, s_sw[warp][0])) store_link(p, lane, r, b, phi - plo, s_sj[warp][0]);
     return;
   }
-  close_chunks_until(nchunks);
-  store_mass(p, lane, r, run);
-  if (!(run > 0.0) || isinf(run)) { fail_link(p, lane, r); return; }
+  close_chunks_until(geo.nchunks);
+  if (!check_mass(p, lane, r, ck.run)) return;
 
   // ---- pass 2: the same walk restricted to the chosen chunk
   const U2 u = link_uniform(p, r);
-  const double t = u.u0 * run;
-  unsigned m = __ballot_sync(FULL, lane < nchunks && Q > t);
-  const int chunk = m ? (__ffs(m) - 1) : (nchunks - 1);
-  double rsum = shfl_d(Q, chunk > 0 ? chunk - 1 : 0);
-  if (chunk == 0) rsum = 0.0;
+  const double t = u.u0 * ck.run;
+  double before, base;
+  const int chunk = draw_chunk(lane, geo.nchunks, ck.Q, t, before);
   const bool stored = (ns <= SCAP);
   double ls = 0.0;
   if (stored) {
@@ -897,22 +905,7 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
       }
     }
   }
-  double Pfx = ls;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const double o = shfl_up_d(Pfx, d);
-    if (lane >= d) Pfx = Pfx + o;
-  }
-  m = __ballot_sync(FULL, rsum + Pfx > t);
-  int L;
-  if (m) L = __ffs(m) - 1;
-  else {
-    const unsigned pos = __ballot_sync(FULL, ls > 0.0);
-    L = pos ? (31 - __clz(pos)) : 0;
-  }
-  const double Pprev = shfl_up_d(Pfx, 1);
-  const double base_l = lane ? rsum + Pprev : rsum;
-  const double base = shfl_d(base_l, L);
+  const int L = draw_lane(lane, ls, before, t, base);
   double cum = 0.0;
   int pick = -1, last_pos = -1;
   if (stored) {
@@ -985,34 +978,26 @@ __global__ void __launch_bounds__(HEAVY_WARPS * 32) k_link_heavy(PrunedParams pp
       s_ra[lane] = c;
     }
     __syncthreads();
-    const int nsteps = ntiles * (TE / 32);
-    const int spc = (TE / 32) * max(1, (ntiles + 31) >> 5);
-    const int nchunks = (nsteps + spc - 1) / spc;
+    const DrawGeom geo = draw_geom(ntiles);
     auto wf = [&](int j) -> double {
       if (j >= n) return 0.0;
       const int *tile = tiles + (size_t)(j / TE) * tw;
       const int slot = j % TE;
       return generic_weight(s_ra, A, false, tile + slot, reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot]);
     };
-    for (int c = warp; c < nchunks; c += HEAVY_WARPS) {
+    for (int c = warp; c < geo.nchunks; c += HEAVY_WARPS) {
       double acc = 0.0;
-      const int s1 = min((c + 1) * spc, nsteps);
-      for (int st = c * spc; st < s1; ++st) acc = acc + wf((st << 5) + lane);
+      const int s1 = min((c + 1) * geo.spc, geo.nsteps);
+      for (int st = c * geo.spc; st < s1; ++st) acc = acc + wf((st << 5) + lane);
       s_sums[c * 32 + lane] = acc;
     }
     __syncthreads();
     if (warp == 0) {
-      double run = 0.0, Q = 0.0;
-      for (int c = 0; c < nchunks; ++c) {
-        run = run + butterfly_sum(s_sums[c * 32 + lane]);
-        if (lane == c) Q = run;
-      }
-      store_mass(p, lane, r, run);
-      if (!(run > 0.0) || isinf(run)) {
-        fail_link(p, lane, r);
-      } else {
+      Checkpoints ck;
+      while (ck.chunk < geo.nchunks) ck.close(lane, s_sums[ck.chunk * 32 + lane]);
+      if (check_mass(p, lane, r, ck.run)) {
         const U2 u = link_uniform(p, r);
-        const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q, run, u.u0, wf, s_sums);
+        const int j = finish_draw(lane, n, geo, ck.Q, ck.run, u.u0, wf, s_sums);
         store_link(p, lane, r, b, n, j);
       }
     }

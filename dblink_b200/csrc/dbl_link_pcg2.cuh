@@ -15,7 +15,7 @@
 //  * non-constant attributes: ONE probe per (candidate, attribute) of a 32-slot perfect-hash table in shared memory
 //    (one key word per bank = one conflict-free wavefront) that holds the record's similarity row INCLUDING the
 //    record's own value, whose entry carries the exact-match multiplier of protocol 4.1 -- so "equal" and "similar"
-//    are the same look-up and the multiply is skipped warp-wide by one vote per step when nobody hit (the usual case);
+//    are the same look-up, and a lane multiplies only where it hit (predicated, no warp vote);
 //  * lane l scores candidate 32*step + l; lane sums / chunk totals / draw as in DESIGN.md section 4.
 #pragma once
 #include <type_traits>
@@ -81,16 +81,7 @@ __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *til
 // With skewed (Zipf-like) value frequencies some lane of the warp finds an equal or similar value on almost every
 // step (96 % at BASELINE's 1M configuration), so a warp-wide vote that skips the multiplies does not pay: the
 // multiplies are predicated per lane and the compiler is free to overlap them with the next step's loads.
-// DBL_PCG2_VOTE=1 brings the vote back (CONVERGED = every lane of the warp executes the call, i.e. the main loop).
-#ifndef DBL_PCG2_VOTE
-#define DBL_PCG2_VOTE 0
-#endif
-// PK kernels: 1 = the product of the matching constant attributes comes from the record's 16-entry table in shared
-// memory (index from a SWAR byte compare), 0 = predicated multiplies
-#ifndef DBL_PCG2_CTAB
-#define DBL_PCG2_CTAB 1
-#endif
-template <int A, int NS, int HC, bool CONVERGED, bool PK, bool MISSING = true>
+template <int A, int NS, int HC, bool PK, bool MISSING = true>
 __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const LinkParams &p, const char *tab,
                                               const double *ctab, const Pcg2Cand<A, NS, PK> &cd) {
   const int hslots = HC ? HC : p.hslots;
@@ -101,16 +92,8 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const Li
   if constexpr (NS < A) {  // protocol 4.1: the constant attributes form their own product c; w = N * c
     double c = 1.0;
     if constexpr (PK) {
-#if DBL_PCG2_CTAB
+      // the record's 16-entry table of products, indexed by a SWAR byte compare of the packed values
       c = ctab[pcg2_const_index(cd.ypack, rc.xpack)];
-#else
-      // the same product, multiplied out: byte k of d is zero <=> constant attribute k matches (a missing record
-      // value is 0xFF and matches nothing); no table look-up, i.e. two shared-memory wavefronts less per candidate
-      const unsigned d = cd.ypack ^ rc.xpack;
-#pragma unroll
-      for (int k = 0; k < A - NS; ++k)
-        if ((d & (0xFFu << (8 * k))) == 0u) c = c * rc.rm[k];
-#endif
     } else {
 #pragma unroll
       for (int k = 0; k < A - NS; ++k) mul_if_eq(c, y[k], rc.x[k], rc.rm[k]);
@@ -119,33 +102,12 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const Li
   }
   // protocol 4.1: non-constant attributes in kernel order, each contributes at most one factor: the exact-match
   // multiplier when y == x, exp(similarity) when y is similar to x -- both sit in the record's hash table
-  if (CONVERGED && DBL_PCG2_VOTE) {
-    bool hit[NS > 0 ? NS : 1];
-    bool any = false;
 #pragma unroll
-    for (int q = 0; q < NS; ++q) {
-      const int yv = y[A - NS + q];
-      const unsigned slot = ((unsigned)yv * rc.hm[q]) >> hshift;
-      hit[q] = (reinterpret_cast<const int *>(tab + q * tabb)[slot] == yv);
-      any = any || hit[q];
-    }
-    if (NS > 0 && __any_sync(FULL, any)) {
-#pragma unroll
-      for (int q = 0; q < NS; ++q) {
-        if (hit[q]) {
-          const unsigned slot = ((unsigned)y[A - NS + q] * rc.hm[q]) >> hshift;
-          w = w * reinterpret_cast<const double *>(tab + q * tabb + hslots * 4)[slot];
-        }
-      }
-    }
-  } else {
-#pragma unroll
-    for (int q = 0; q < NS; ++q) {
-      const int yv = y[A - NS + q];
-      const unsigned slot = ((unsigned)yv * rc.hm[q]) >> hshift;
-      if (reinterpret_cast<const int *>(tab + q * tabb)[slot] == yv)
-        w = w * reinterpret_cast<const double *>(tab + q * tabb + hslots * 4)[slot];
-    }
+  for (int q = 0; q < NS; ++q) {
+    const int yv = y[A - NS + q];
+    const unsigned slot = ((unsigned)yv * rc.hm[q]) >> hshift;
+    if (reinterpret_cast<const int *>(tab + q * tabb)[slot] == yv)
+      w = w * reinterpret_cast<const double *>(tab + q * tabb + hslots * 4)[slot];
   }
   if (MISSING && rc.mmask) {
 #pragma unroll
@@ -155,38 +117,19 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const Li
   return w;
 }
 
-#ifndef DBL_PCG2_CTAS_PER_SM
-#define DBL_PCG2_CTAS_PER_SM 3
-#endif
-
 // Records per consumer warp.  With 2, a lane fetches its candidate once and scores it for both records: half the
 // tile loads and half the tile traffic through shared memory per (record, candidate) pair, two independent
 // dependency chains per warp; the price is registers (96 instead of 72: 2 CTAs per SM instead of 3) and twice the
 // per-record tables in shared memory -- so it is used for the 32-slot instantiations with up to 8 non-constant
-// attributes (faster at A = 10, NS = 6; three records per warp spill).
-#ifndef DBL_PCG2_RPW_MAX
-#define DBL_PCG2_RPW_MAX 2
-#endif
-__host__ __device__ constexpr int pcg2_rpw(int HC, int NS) { return (HC == 32 && NS >= 1 && NS <= 8) ? DBL_PCG2_RPW_MAX : 1; }
-// Consumer warps per CTA of the two-record shapes.  Every 32-byte sector a bulk copy lands in shared memory costs
-// the L1 data pipe about two wavefronts, so more records per staged tile should help -- but ONE CTA of 16 consumer
-// warps per SM was slower than two CTAs of 8 (one ring per SM: every warp waits for the slowest at each stage), so 8
-// it stays.
-#ifndef DBL_PCG2_WARPS2
-#define DBL_PCG2_WARPS2 8
-#endif
-__host__ __device__ constexpr int pcg2_warps(int HC, int NS) { return pcg2_rpw(HC, NS) >= 2 ? DBL_PCG2_WARPS2 : LINK_WARPS; }
+// attributes (faster at A = 10, NS = 6; three records per warp spill).  Every shape has LINK_WARPS consumer warps:
+// ONE CTA of 16 consumer warps per SM was slower than two CTAs of 8 (one ring per SM: every warp waits for the
+// slowest at each stage).
+__host__ __device__ constexpr int pcg2_rpw(int HC, int NS) { return (HC == 32 && NS >= 1 && NS <= 8) ? 2 : 1; }
 // 3 CTAs per SM (72 registers) only where one record per warp fits them: few non-constant attributes
-__host__ __device__ constexpr int pcg2_ctas_per_sm(int HC, int NS) {
-#ifdef DBL_PCG2_CTAS2
-  return pcg2_rpw(HC, NS) >= 2 ? DBL_PCG2_CTAS2 : (NS > 6 ? 2 : DBL_PCG2_CTAS_PER_SM);
-#else
-  return pcg2_rpw(HC, NS) >= 2 ? (pcg2_warps(HC, NS) > 8 ? 1 : 2) : (NS > 6 ? 2 : DBL_PCG2_CTAS_PER_SM);
-#endif
-}
+__host__ __device__ constexpr int pcg2_ctas_per_sm(int HC, int NS) { return (pcg2_rpw(HC, NS) >= 2 || NS > 6) ? 2 : 3; }
 
 template <int A, int NS, int HC, bool PK>
-__global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_sm(HC, NS)) k_link_pcg2(LinkParams p) {
+__global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS)) k_link_pcg2(LinkParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ int s_cta;
   if (sweep_dead(p.ctl)) return;
@@ -195,7 +138,7 @@ __global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_s
   constexpr int TW = qtile_words(NV) * TE;
   constexpr int NC = A - NS;
   constexpr int RPW = pcg2_rpw(HC, NS);
-  constexpr int WARPS = pcg2_warps(HC, NS);   // consumer warps; warp WARPS is the producer
+  constexpr int WARPS = LINK_WARPS;           // consumer warps; warp WARPS is the producer
   constexpr int PCG2_RECS = WARPS * RPW;      // records per work item (= per "CTA" of cta_ptr)
   TileRing rg;
   rg.tiles = reinterpret_cast<int *>(smem);
@@ -208,10 +151,7 @@ __global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_s
   // PK: products of the matching constant attributes, by match mask, 16 entries per record
   double *ctab0 = reinterpret_cast<double *>(reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 +
                                             (size_t)PCG2_RECS * tabrec) + warp * RPW * 16;
-#ifndef DBL_PCG2_LDGSTS
-#define DBL_PCG2_LDGSTS 0
-#endif
-  ring_init(rg, WARPS, DBL_PCG2_LDGSTS ? 32 : 1);
+  ring_init(rg, WARPS);
   const int total_ctas = p.cta_ptr[p.P];
   int tbase = 0;  // tiles this CTA has streamed so far: stage and phase of the ring continue across work items
 
@@ -227,11 +167,7 @@ __global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_s
     const int *gtiles = p.qtiles + (size_t)p.tile_ptr[b] * TW;
 
     if (warp == WARPS) {  // producer warp
-#if DBL_PCG2_LDGSTS
-      ring_produce_ldgsts(rg, gtiles, ntiles, tbase, lane);
-#else
       if (lane == 0) ring_produce<true>(rg, gtiles, ntiles, tbase);
-#endif
       tbase += ntiles;
       continue;
     }
@@ -313,14 +249,11 @@ __global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_s
     }
     __syncwarp();
 
-    const int nsteps = ntiles * (TE / 32);          // steps beyond the last candidate add zeros
-    const int tpc = max(1, (ntiles + 31) >> 5);     // a chunk is a whole number of tiles
-    const int spc = (TE / 32) * tpc;
-    const int nchunks = (nsteps + spc - 1) / spc;
+    const DrawGeom geo = draw_geom(ntiles);
 
     // ---- pass 1 over the TMA-staged tiles.  Records without a missing non-constant attribute (most of them) take a
     // loop body without the gather of 1/n(y): straight-line code the compiler can overlap across the steps of a tile
-    double run[RPW], Q[RPW], acc[RPW];
+    double run[RPW], Q[RPW], acc[RPW];  // run, Q: each record's Checkpoints, with `chunk` shared by the records
     unsigned any_missing = 0;
 #pragma unroll
     for (int ri = 0; ri < RPW; ++ri) { run[ri] = 0.0; Q[ri] = 0.0; acc[ri] = 0.0; any_missing |= rc[ri].mmask; }
@@ -340,15 +273,14 @@ __global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_s
             pcg2_load<A, NS, PK>(cd, tile, q * 32 + lane);
 #pragma unroll
             for (int ri = 0; ri < RPW; ++ri)
-              acc[ri] = acc[ri] + pcg2_weight<A, NS, HC, true, PK, MISSING>(rc[ri], p, tab0 + ri * tabrec,
-                                                                          ctab0 + ri * 16, cd);
+              acc[ri] = acc[ri] + pcg2_weight<A, NS, HC, PK, MISSING>(rc[ri], p, tab0 + ri * tabrec,
+                                                                    ctab0 + ri * 16, cd);
           }
-          if (++tile_in_chunk == tpc || t + 1 == ntiles) {
+          if (++tile_in_chunk == geo.tpc || t + 1 == ntiles) {
 #pragma unroll
             for (int ri = 0; ri < RPW; ++ri) {
               my_sums[ri * 1024 + chunk * 32 + lane] = acc[ri];  // pass 2 reads the chosen chunk's sums back
-              run[ri] = run[ri] + butterfly_sum(acc[ri]);
-              if (lane == chunk) Q[ri] = run[ri];
+              close_chunk(lane, chunk, acc[ri], run[ri], Q[ri]);
               acc[ri] = 0.0;
             }
             ++chunk;
@@ -367,23 +299,22 @@ __global__ void __launch_bounds__((pcg2_warps(HC, NS) + 1) * 32, pcg2_ctas_per_s
     for (int ri = 0; ri < RPW; ++ri) {
       if (!act[ri]) continue;
       const int r = rr[ri];
-      store_mass(p, lane, r, run[ri]);
-      if (!(run[ri] > 0.0) || isinf(run[ri])) { fail_link(p, lane, r); continue; }
+      if (!check_mass(p, lane, r, run[ri])) continue;
       auto wf = [&](int j) -> double {
         if (j >= n) return 0.0;
         Pcg2Cand<A, NS, PK> cd;
         pcg2_load<A, NS, PK>(cd, gtiles + (size_t)(j / TE) * TW, j % TE);
-        return pcg2_weight<A, NS, HC, false, PK>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
+        return pcg2_weight<A, NS, HC, PK>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
       };
       const U2 u = link_uniform(p, r);
-      const int j = finish_draw(lane, n, nsteps, spc, nchunks, Q[ri], run[ri], u.u0, wf, my_sums + ri * 1024);
+      const int j = finish_draw(lane, n, geo, Q[ri], run[ri], u.u0, wf, my_sums + ri * 1024);
       store_link(p, lane, r, b, n, j);
     }
   }
 }
 
 inline size_t pcg2_smem_bytes(int A, int NS, int H, bool PK) {
-  const size_t recs = (size_t)pcg2_warps(H == 32 ? 32 : 0, NS) * pcg2_rpw(H == 32 ? 32 : 0, NS);
+  const size_t recs = (size_t)LINK_WARPS * pcg2_rpw(H == 32 ? 32 : 0, NS);
   return (size_t)LINK_STAGES * qtile_words(qtile_nv(A, NS, PK)) * TE * 4 + 128 +
          recs * (NS > 0 ? NS : 1) * pcg2_tab_bytes(H) + recs * 16 * sizeof(double);
 }
@@ -403,7 +334,7 @@ int pcg2_launch_one(int grid, cudaStream_t stream, const LinkParams &lp, size_t 
     cudaFuncAttributes fa;
     return (int)cudaFuncGetAttributes(&fa, k_link_pcg2<A, NS, HC, PK>);
   }
-  k_link_pcg2<A, NS, HC, PK><<<grid, (pcg2_warps(HC, NS) + 1) * 32, smem, stream>>>(lp);
+  k_link_pcg2<A, NS, HC, PK><<<grid, (LINK_WARPS + 1) * 32, smem, stream>>>(lp);
   return (int)cudaGetLastError();
 }
 
