@@ -314,7 +314,7 @@ __global__ void k_block_scan(int P, const int *__restrict__ ent_ptr, const int *
 __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__restrict__ y, const double *__restrict__ entN,
                               const int *__restrict__ ent_sorted, const int *__restrict__ ent_ptr,
                               const int *__restrict__ tile_ptr, int *__restrict__ tiles, const int *__restrict__ perm, int P,
-                              int npack, int *__restrict__ qtiles, int n_str, int qtile_pk) {
+                              int npack, int *__restrict__ qtiles, int n_str, int qtile_pk, int qtile_id16) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_slots) return;
   const int T = (int)(i / TE), slot = (int)(i % TE);
@@ -337,7 +337,8 @@ __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__rest
     unsigned pk = 0;  // constant attributes (kernel positions 0..npack-1), one byte each
     if (real)
       for (int k = 0; k < npack; ++k) pk |= ((unsigned)y[e * A + perm[k]] & 0xFFu) << (8 * k);
-    const int nv = qtile_nv(A, n_str, qtile_pk != 0), ng = qtile_groups(nv), qw = qtile_words(nv);
+    const int nv = qtile_nv(A, n_str, qtile_pk != 0, qtile_id16 != 0), ng = qtile_groups(nv), qw = qtile_words(nv);
+    const int nid = qtile_id16 ? (n_str + 1) / 2 : n_str;  // words of non-constant values (packed tiles)
     int *qt = qtiles + (size_t)T * qw * TE;
     int v[4];
     for (int g = 0; g < ng; ++g) {
@@ -345,8 +346,19 @@ __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__rest
         const int w = 4 * g + c;
         int val = 0;
         if (real) {
-          if (qtile_pk) val = (w < n_str) ? y[e * A + perm[A - n_str + w]] : (w == n_str ? (int)pk : 0);
-          else val = (w < A) ? y[e * A + perm[w]] : 0;
+          if (qtile_pk && qtile_id16) {
+            if (w < nid) {  // values 2w (low half) and 2w + 1 (high half): vocabularies of <= 65536 values
+              const int k = A - n_str + 2 * w;
+              val = (int)(((unsigned)y[e * A + perm[k]] & 0xFFFFu) |
+                          (2 * w + 1 < n_str ? (unsigned)y[e * A + perm[k + 1]] << 16 : 0u));
+            } else if (w == nid) {
+              val = (int)pk;
+            }
+          } else if (qtile_pk) {
+            val = (w < n_str) ? y[e * A + perm[A - n_str + w]] : (w == n_str ? (int)pk : 0);
+          } else {
+            val = (w < A) ? y[e * A + perm[w]] : 0;
+          }
         }
         v[c] = val;
       }
@@ -1405,6 +1417,7 @@ struct dbl_ctx {
   DevBuf<int> ent_ptr, tile_ptr, rec_ptr, cta_ptr, cta_ptr2, cta_ptr3, tiles, qtiles;
   DevBuf<double> lane_sums;  // k_link_pcg2 scratch: pass-1 lane sums per chunk of every resident warp
   int qtile_pk = 0;  // quad tiles carry the packed constants (PK instantiations of k_link_pcg2)
+  int qtile_id16 = 0;  // ... and 16-bit non-constant values (every non-constant vocabulary has <= 65536 values)
   bool tiles_valid[2] = {false, false};  // attribute-major / quad tiles match the current layout
   // inverted index of the block tables for the pruned PCG-I link kernel (built on demand, once per sweep): E * A ids,
   // unsigned or (inv_ids64) unsigned long long, with their candidate positions
@@ -1735,6 +1748,10 @@ static int alloc_blocks(dbl_ctx *ctx) {
   const size_t max_tiles = (size_t)(ctx->E / TE) + (size_t)P + 1;
   CUDA_TRY(ctx->tiles.alloc(max_tiles * tile_words(ctx->A)));
   ctx->qtile_pk = (ctx->pack_consts && ctx->hslots == 32) ? 1 : 0;
+  ctx->qtile_id16 = ctx->qtile_pk;
+  for (int a = 0; a < ctx->A; ++a)
+    if (!ctx->h_attrs[a].is_const && ctx->h_attrs[a].V > 65536) ctx->qtile_id16 = 0;
+  if (getenv("DBL_NO_ID16")) ctx->qtile_id16 = 0;  // tests: the 32-bit packed tiles on a model that fits 16 bits
   {
     // work item and grid of the persistent PCG-II kernel for this model shape (see pcg2_rpw)
     const int hc = ctx->hslots == 32 ? 32 : 0;
@@ -1743,6 +1760,7 @@ static int alloc_blocks(dbl_ctx *ctx) {
     const size_t need = (size_t)ctx->pcg2_grid * ctx->pcg2_recs * 1024;
     if (ctx->lane_sums.n < need) CUDA_TRY(ctx->lane_sums.alloc(need));
   }
+  // sized for 32-bit values: the 16-bit format never needs more
   CUDA_TRY(ctx->qtiles.alloc(max_tiles * qtile_words(qtile_nv(ctx->A, ctx->n_str, ctx->qtile_pk != 0)) * TE));
   ctx->max_ctas = (int)((ctx->R + LINK_WARPS - 1) / LINK_WARPS) + P;
   return alloc_control(ctx);
@@ -1879,7 +1897,8 @@ static int ensure_tiles(dbl_ctx *ctx, int fmt) {
   k_build_tiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(n_slots, fmt, ctx->A, ctx->y.p, ctx->entN.p,
                                                                  ctx->ent_sorted.p, ctx->ent_ptr.p, ctx->tile_ptr.p,
                                                                  ctx->tiles.p, ctx->perm_dev.p, ctx->P, ctx->pack_consts,
-                                                                 ctx->qtiles.p, ctx->n_str, ctx->qtile_pk);
+                                                                 ctx->qtiles.p, ctx->n_str, ctx->qtile_pk,
+                                                                 ctx->qtile_id16);
   ctx->launches += 1;
   ctx->tiles_valid[fmt - 1] = true;
   CUDA_TRY(cudaGetLastError());
@@ -2353,7 +2372,7 @@ static int ensure_inverted_index(dbl_ctx *ctx) {
 
 static bool pcg2_kernel_fits(const dbl_ctx *ctx) {
   return ctx->hslots > 0 && ctx->A <= LINK_MAX_UNROLL_A &&
-         pcg2_smem_bytes(ctx->A, ctx->n_str, ctx->hslots, ctx->qtile_pk != 0) <= 100 * 1024;
+         pcg2_smem_bytes(ctx->A, ctx->n_str, ctx->hslots, ctx->qtile_pk != 0, ctx->qtile_id16 != 0) <= 100 * 1024;
 }
 static int dispatch_pcg2(dbl_ctx *ctx, int grid, const LinkParams &lp) {
   int rc = -1;
@@ -2386,7 +2405,7 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
   lp.theta = ctx->theta(); lp.ent_ptr = ctx->ent_ptr.p; lp.tile_ptr = ctx->tile_ptr.p; lp.rec_ptr = ctx->rec_ptr.p;
   lp.cta_ptr = ctx->cta_ptr.p; lp.ent_sorted = ctx->ent_sorted.p; lp.rec_sorted = ctx->rec_sorted.p;
   lp.tiles = ctx->tiles.p; lp.newlink = ctx->newlink.p;
-  lp.qtiles = ctx->qtiles.p; lp.qtile_pk = ctx->qtile_pk;
+  lp.qtiles = ctx->qtiles.p; lp.qtile_pk = ctx->qtile_pk; lp.qtile_id16 = ctx->qtile_id16;
   lp.work = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_WORK);
   lp.lane_sums = ctx->lane_sums.p;
   lp.status = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_STATUS);
@@ -2797,7 +2816,7 @@ static int preload_kernels(dbl_ctx *ctx) {
   if (pcg2_kernel_fits(ctx)) {
     LinkParams lp;
     memset(&lp, 0, sizeof(lp));
-    lp.hslots = ctx->hslots; lp.qtile_pk = ctx->qtile_pk;
+    lp.hslots = ctx->hslots; lp.qtile_pk = ctx->qtile_pk; lp.qtile_id16 = ctx->qtile_id16;
     int rc = dispatch_pcg2(ctx, 0, lp);  // grid 0 = load only
     if (rc) return rc;
   }

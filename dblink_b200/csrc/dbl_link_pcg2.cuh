@@ -1,14 +1,18 @@
-// k_link_pcg2<A, NS, HC, PK>: the PCG-II link update (updateEntityIdCollapsed, GU:363-395) with everything about
+// k_link_pcg2<A, NS, HC, PK, ID16>: the PCG-II link update (updateEntityIdCollapsed, GU:363-395) with everything about
 // the model shape known at compile time: A attributes in kernel order, the last NS of them non-constant; HC = 32
 // when the hash tables have 32 slots (else the size is a run-time parameter); PK = the constant attributes arrive
-// byte-packed.
+// byte-packed; ID16 (PK only) = the non-constant values arrive as 16-bit halves, two per word (every non-constant
+// vocabulary has <= 65536 values).  ID16 is a tile format, not a kernel shape: dbl_link_kernel does not report it.
 //
 //  * persistent CTAs: the grid is a few CTAs per SM; each takes the next group of LINK_WARPS records of some block
 //    from a device-side counter until none is left (no empty CTAs on a shard that owns 1/8 of the records, no tail);
 //  * the block's entity table streams through shared memory in TE-entity "quad tiles" moved by TMA bulk copies
 //    (cp.async.bulk.shared::cluster.global + mbarrier ring, one producer warp per CTA); a quad tile keeps the words
-//    of one entity in groups of four, so a lane fetches everything it needs about its candidate with QW/4 128-bit
-//    shared-memory loads (3 for 6 non-constant attributes + packed constants + N) instead of one load per word;
+//    of one entity in groups of four, so a lane fetches everything it needs about its candidate with 128-bit
+//    shared-memory loads instead of one load per word: at 6 non-constant attributes + packed constants, ONE LDS.128
+//    (ID16: 3 words of values + the packed word) and the LDS.64 of N = 6 wavefronts per warp-step, against two
+//    LDS.128 + N = 10 with 32-bit values; the unpacking costs one LOP3 or SHF per value (6 per candidate, shared by
+//    the warp's two records);
 //  * each consumer warp owns one record; its constants (value ids, hash multipliers) are registers;
 //  * constant attributes: the product of the exact-match multipliers comes from a 16-entry per-record table indexed
 //    by the byte-wise match mask of the packed values (PK), else from per-attribute compares;
@@ -16,6 +20,8 @@
 //    (one key word per bank = one conflict-free wavefront) that holds the record's similarity row INCLUDING the
 //    record's own value, whose entry carries the exact-match multiplier of protocol 4.1 -- so "equal" and "similar"
 //    are the same look-up, and a lane multiplies only where it hit (predicated, no warp vote);
+//  * records with a missing non-constant value multiply by 1/n(y): the two-record shapes keep the NS table pointers
+//    in registers for the whole work item (fetching them per step and attribute cost 15 % of the kernel at 1 M);
 //  * lane l scores candidate 32*step + l; lane sums / chunk totals / draw as in DESIGN.md section 4.
 #pragma once
 #include <type_traits>
@@ -40,13 +46,16 @@ struct Pcg2Rec {
   unsigned xpack;                // PK: the record's constant-attribute values, one byte each (0xFF = cannot match)
 };
 
-// PK kernels: index into the record's table of constant-attribute products from the byte-packed values of a
-// candidate: bit k of the index = (byte k of ypack == byte k of xpack)
-__device__ __forceinline__ unsigned pcg2_const_index(unsigned ypack, unsigned xpack) {
+// PK kernels: BYTE offset into the record's table of constant-attribute products (8-byte entries) from the
+// byte-packed values of a candidate: bit k of the entry index = (byte k of ypack == byte k of xpack)
+__device__ __forceinline__ unsigned pcg2_const_offset(unsigned ypack, unsigned xpack) {
   const unsigned d = ypack ^ xpack;
   const unsigned nz = ((d & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | d;  // bit 7 of a byte set <=> the byte of d is non-zero
-  const unsigned eq = (~nz & 0x80808080u) >> 7;               // bit 8k set <=> byte k equal
-  return (eq * 0x01020408u) >> 24;                            // gathers bits 0, 8, 16, 24 into bits 0..3
+  const unsigned eq = ~nz & 0x80808080u;                      // bit 8k+7 set <=> byte k equal
+  // the partial product of bit 8k+7 and bit 7j of the multiplier lands on bit 8k+7j+7: j = 3-k puts bit 8k+7 on bit
+  // 28+k, and no two of the 16 partial products share a bit (no carries), so bits 28..31 are the four flags and
+  // bits 25..27 are zero: the shift by 25 yields 8 * index, which ptxas adds to the table base in one LEA.HI
+  return (eq * 0x00204081u) >> 25;
 }
 
 // one candidate out of a quad tile: values in kernel order (PK: only the non-constant ones + the packed word), N
@@ -56,9 +65,10 @@ struct Pcg2Cand {
   unsigned ypack;
   double N;
 };
-template <int A, int NS, bool PK>
+template <int A, int NS, bool PK, bool ID16>
 __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *tile, int slot) {
-  constexpr int NV = qtile_nv(A, NS, PK), NG = qtile_groups(NV);
+  static_assert(PK || !ID16, "16-bit values only in the packed tiles");
+  constexpr int NV = qtile_nv(A, NS, PK, ID16), NG = qtile_groups(NV);
   int v[NG * 4];
   const int4 *q = reinterpret_cast<const int4 *>(tile);
 #pragma unroll
@@ -66,7 +76,11 @@ __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *til
     const int4 t = q[g * TE + slot];
     v[4 * g] = t.x; v[4 * g + 1] = t.y; v[4 * g + 2] = t.z; v[4 * g + 3] = t.w;
   }
-  if constexpr (PK) {
+  if constexpr (PK && ID16) {
+#pragma unroll
+    for (int q2 = 0; q2 < NS; ++q2) c.y[A - NS + q2] = (int)(q2 & 1 ? (unsigned)v[q2 >> 1] >> 16 : v[q2 >> 1] & 0xFFFF);
+    c.ypack = (unsigned)v[(NS + 1) / 2];
+  } else if constexpr (PK) {
 #pragma unroll
     for (int q2 = 0; q2 < NS; ++q2) c.y[A - NS + q2] = v[q2];
     c.ypack = (unsigned)v[NS];
@@ -81,9 +95,12 @@ __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *til
 // With skewed (Zipf-like) value frequencies some lane of the warp finds an equal or similar value on almost every
 // step (96 % at BASELINE's 1M configuration), so a warp-wide vote that skips the multiplies does not pay: the
 // multiplies are predicated per lane and the compiler is free to overlap them with the next step's loads.
+// invnorm: the 1/n(y) tables of the non-constant attributes in kernel order when the caller keeps them in registers;
+// nullptr: read through p.attrs.
 template <int A, int NS, int HC, bool PK, bool MISSING = true>
 __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const LinkParams &p, const char *tab,
-                                              const double *ctab, const Pcg2Cand<A, NS, PK> &cd) {
+                                              const double *ctab, const Pcg2Cand<A, NS, PK> &cd,
+                                              const double *const *invnorm = nullptr) {
   const int hslots = HC ? HC : p.hslots;
   const int hshift = HC ? 27 : p.hshift;
   const int tabb = pcg2_tab_bytes(hslots);
@@ -93,7 +110,7 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const Li
     double c = 1.0;
     if constexpr (PK) {
       // the record's 16-entry table of products, indexed by a SWAR byte compare of the packed values
-      c = ctab[pcg2_const_index(cd.ypack, rc.xpack)];
+      c = *reinterpret_cast<const double *>(reinterpret_cast<const char *>(ctab) + pcg2_const_offset(cd.ypack, rc.xpack));
     } else {
 #pragma unroll
       for (int k = 0; k < A - NS; ++k) mul_if_eq(c, y[k], rc.x[k], rc.rm[k]);
@@ -112,7 +129,8 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const Li
   if (MISSING && rc.mmask) {
 #pragma unroll
     for (int q = 0; q < NS; ++q)
-      if ((rc.mmask >> (A - NS + q)) & 1u) w = w * p.attrs[p.perm[A - NS + q]].invnorm[y[A - NS + q]];
+      if ((rc.mmask >> (A - NS + q)) & 1u)
+        w = w * (invnorm ? __ldg(invnorm[q] + y[A - NS + q]) : p.attrs[p.perm[A - NS + q]].invnorm[y[A - NS + q]]);
   }
   return w;
 }
@@ -128,13 +146,13 @@ __host__ __device__ constexpr int pcg2_rpw(int HC, int NS) { return (HC == 32 &&
 // 3 CTAs per SM (72 registers) only where one record per warp fits them: few non-constant attributes
 __host__ __device__ constexpr int pcg2_ctas_per_sm(int HC, int NS) { return (pcg2_rpw(HC, NS) >= 2 || NS > 6) ? 2 : 3; }
 
-template <int A, int NS, int HC, bool PK>
+template <int A, int NS, int HC, bool PK, bool ID16>
 __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS)) k_link_pcg2(LinkParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ int s_cta;
   if (sweep_dead(p.ctl)) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int NV = qtile_nv(A, NS, PK);
+  constexpr int NV = qtile_nv(A, NS, PK, ID16);
   constexpr int TW = qtile_words(NV) * TE;
   constexpr int NC = A - NS;
   constexpr int RPW = pcg2_rpw(HC, NS);
@@ -261,6 +279,12 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
     double *my_sums = p.lane_sums + ((size_t)blockIdx.x * WARPS + warp) * RPW * 1024;  // [record][chunk][lane]
     auto pass1 = [&](auto missing_tag) {
       constexpr bool MISSING = decltype(missing_tag)::value;
+      // the 1/n(y) tables of the non-constant attributes, loaded once instead of once per step and attribute
+      // (two-record shapes only: in the one-record shapes the NS pointers do not fit the register budget)
+      constexpr bool HOIST = MISSING && RPW == 2;
+      const double *invnorm[NS > 0 ? NS : 1];
+#pragma unroll
+      for (int q = 0; q < NS; ++q) invnorm[q] = HOIST ? p.attrs[p.perm[A - NS + q]].invnorm : nullptr;
       for (int t = 0; t < ntiles; ++t) {
         const int g = tbase + t;
         const int s = g % LINK_STAGES;
@@ -270,11 +294,11 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
 #pragma unroll
           for (int q = 0; q < TE / 32; ++q) {
             Pcg2Cand<A, NS, PK> cd;
-            pcg2_load<A, NS, PK>(cd, tile, q * 32 + lane);
+            pcg2_load<A, NS, PK, ID16>(cd, tile, q * 32 + lane);
 #pragma unroll
             for (int ri = 0; ri < RPW; ++ri)
               acc[ri] = acc[ri] + pcg2_weight<A, NS, HC, PK, MISSING>(rc[ri], p, tab0 + ri * tabrec,
-                                                                    ctab0 + ri * 16, cd);
+                                                                    ctab0 + ri * 16, cd, HOIST ? invnorm : nullptr);
           }
           if (++tile_in_chunk == geo.tpc || t + 1 == ntiles) {
 #pragma unroll
@@ -303,7 +327,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
       auto wf = [&](int j) -> double {
         if (j >= n) return 0.0;
         Pcg2Cand<A, NS, PK> cd;
-        pcg2_load<A, NS, PK>(cd, gtiles + (size_t)(j / TE) * TW, j % TE);
+        pcg2_load<A, NS, PK, ID16>(cd, gtiles + (size_t)(j / TE) * TW, j % TE);
         return pcg2_weight<A, NS, HC, PK>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
       };
       const U2 u = link_uniform(p, r);
@@ -313,28 +337,28 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
   }
 }
 
-inline size_t pcg2_smem_bytes(int A, int NS, int H, bool PK) {
+inline size_t pcg2_smem_bytes(int A, int NS, int H, bool PK, bool id16) {
   const size_t recs = (size_t)LINK_WARPS * pcg2_rpw(H == 32 ? 32 : 0, NS);
-  return (size_t)LINK_STAGES * qtile_words(qtile_nv(A, NS, PK)) * TE * 4 + 128 +
+  return (size_t)LINK_STAGES * qtile_words(qtile_nv(A, NS, PK, id16)) * TE * 4 + 128 +
          recs * (NS > 0 ? NS : 1) * pcg2_tab_bytes(H) + recs * 16 * sizeof(double);
 }
 
 // launch k_link_pcg2<A, NS, HC> for a runtime NS in [0, A]; HC = 32 (compile-time table size) when the model's
 // tables have 32 slots, else 0 (size read from the parameters); returns cudaError_t as int
-template <int A, int NS, int HC, bool PK>
+template <int A, int NS, int HC, bool PK, bool ID16>
 int pcg2_launch_one(int grid, cudaStream_t stream, const LinkParams &lp, size_t *configured) {
-  const size_t smem = pcg2_smem_bytes(A, NS, lp.hslots, PK);
+  const size_t smem = pcg2_smem_bytes(A, NS, lp.hslots, PK, ID16);
   // the opt-in is per device: the cache belongs to the context (one model shape = one instantiation per context)
   if (*configured < smem) {
-    cudaError_t e = cudaFuncSetAttribute(k_link_pcg2<A, NS, HC, PK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(k_link_pcg2<A, NS, HC, PK, ID16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     *configured = smem;
   }
   if (grid <= 0) {  // load the kernel without running it (see preload_kernels in dbl_engine.cu)
     cudaFuncAttributes fa;
-    return (int)cudaFuncGetAttributes(&fa, k_link_pcg2<A, NS, HC, PK>);
+    return (int)cudaFuncGetAttributes(&fa, k_link_pcg2<A, NS, HC, PK, ID16>);
   }
-  k_link_pcg2<A, NS, HC, PK><<<grid, (LINK_WARPS + 1) * 32, smem, stream>>>(lp);
+  k_link_pcg2<A, NS, HC, PK, ID16><<<grid, (LINK_WARPS + 1) * 32, smem, stream>>>(lp);
   return (int)cudaGetLastError();
 }
 
@@ -342,12 +366,14 @@ template <int A, int NS>
 struct Pcg2Launch {
   static int go(int ns, int grid, cudaStream_t stream, const LinkParams &lp, size_t *cfg) {
     if (ns == NS) {
-      // byte-packed constant attributes: 1..4 of them, every vocabulary <= 255, 32-slot tables (lp.qtile_pk)
+      // byte-packed constant attributes: 1..4 of them, every vocabulary <= 255, 32-slot tables (lp.qtile_pk);
+      // 16-bit non-constant values when every non-constant vocabulary has <= 65536 values (lp.qtile_id16)
       if constexpr (A - NS >= 1 && A - NS <= 4) {
-        if (lp.qtile_pk) return pcg2_launch_one<A, NS, 32, true>(grid, stream, lp, cfg);
+        if (lp.qtile_pk) return lp.qtile_id16 ? pcg2_launch_one<A, NS, 32, true, true>(grid, stream, lp, cfg)
+                                              : pcg2_launch_one<A, NS, 32, true, false>(grid, stream, lp, cfg);
       }
-      return lp.hslots == 32 ? pcg2_launch_one<A, NS, 32, false>(grid, stream, lp, cfg)
-                             : pcg2_launch_one<A, NS, 0, false>(grid, stream, lp, cfg);
+      return lp.hslots == 32 ? pcg2_launch_one<A, NS, 32, false, false>(grid, stream, lp, cfg)
+                             : pcg2_launch_one<A, NS, 0, false, false>(grid, stream, lp, cfg);
     }
     if constexpr (NS > 0) return Pcg2Launch<A, NS - 1>::go(ns, grid, stream, lp, cfg);
     return (int)cudaErrorInvalidValue;
