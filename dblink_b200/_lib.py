@@ -117,6 +117,7 @@ SIGNATURES = {
     "dbl_set_link_mass_capture": (C.c_int, [vp, C.c_int]),
     "dbl_link_mass": (C.c_int, [vp, f64p]),
     "dbl_index_hash_slots": (C.c_int32, [vp]),
+    "dbl_index_slot_codes": (C.c_int, [vp, i32p]),
     "dbl_set_graph_mode": (C.c_int, [vp, C.c_int]),
     "dbl_last_sweep_ms": (C.c_double, [vp]),
     "dbl_link_kernel_ms": (C.c_double, [vp, i64p]),

@@ -314,7 +314,8 @@ __global__ void k_block_scan(int P, const int *__restrict__ ent_ptr, const int *
 __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__restrict__ y, const double *__restrict__ entN,
                               const int *__restrict__ ent_sorted, const int *__restrict__ ent_ptr,
                               const int *__restrict__ tile_ptr, int *__restrict__ tiles, const int *__restrict__ perm, int P,
-                              int npack, int *__restrict__ qtiles, int n_str, int qtile_pk, int qtile_id16) {
+                              int npack, int *__restrict__ qtiles, int n_str, int qtile_pk, int qtile_id16,
+                              const AttrDev *__restrict__ sc_attrs) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_slots) return;
   const int T = (int)(i / TE), slot = (int)(i % TE);
@@ -339,6 +340,11 @@ __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__rest
       for (int k = 0; k < npack; ++k) pk |= ((unsigned)y[e * A + perm[k]] & 0xFFu) << (8 * k);
     const int nv = qtile_nv(A, n_str, qtile_pk != 0, qtile_id16 != 0), ng = qtile_groups(nv), qw = qtile_words(nv);
     const int nid = qtile_id16 ? (n_str + 1) / 2 : n_str;  // words of non-constant values (packed tiles)
+    // packed tiles: value (sc_attrs == null) or slot code (AttrDev::pcode) of kernel-order attribute k
+    auto ns_val = [&](int k) -> unsigned {
+      const int yv = y[e * A + perm[k]];
+      return (unsigned)(sc_attrs ? sc_attrs[perm[k]].pcode[yv] : yv);
+    };
     int *qt = qtiles + (size_t)T * qw * TE;
     int v[4];
     for (int g = 0; g < ng; ++g) {
@@ -349,13 +355,12 @@ __global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__rest
           if (qtile_pk && qtile_id16) {
             if (w < nid) {  // values 2w (low half) and 2w + 1 (high half): vocabularies of <= 65536 values
               const int k = A - n_str + 2 * w;
-              val = (int)(((unsigned)y[e * A + perm[k]] & 0xFFFFu) |
-                          (2 * w + 1 < n_str ? (unsigned)y[e * A + perm[k + 1]] << 16 : 0u));
+              val = (int)((ns_val(k) & 0xFFFFu) | (2 * w + 1 < n_str ? ns_val(k + 1) << 16 : 0u));
             } else if (w == nid) {
               val = (int)pk;
             }
           } else if (qtile_pk) {
-            val = (w < n_str) ? y[e * A + perm[A - n_str + w]] : (w == n_str ? (int)pk : 0);
+            val = (w < n_str) ? (int)ns_val(A - n_str + w) : (w == n_str ? (int)pk : 0);
           } else {
             val = (w < A) ? y[e * A + perm[w]] : 0;
           }
@@ -1418,6 +1423,8 @@ struct dbl_ctx {
   DevBuf<double> lane_sums;  // k_link_pcg2 scratch: pass-1 lane sums per chunk of every resident warp
   int qtile_pk = 0;  // quad tiles carry the packed constants (PK instantiations of k_link_pcg2)
   int qtile_id16 = 0;  // ... and 16-bit non-constant values (every non-constant vocabulary has <= 65536 values)
+  int qtile_sc = 0;    // ... and those values are slot codes (every non-constant attribute has them)
+  int sc_code_max = -1;  // largest slot code of the model's non-constant attributes; -1: some attribute has none
   bool tiles_valid[2] = {false, false};  // attribute-major / quad tiles match the current layout
   // inverted index of the block tables for the pruned PCG-I link kernel (built on demand, once per sweep): E * A ids,
   // unsigned or (inv_ids64) unsigned long long, with their candidate positions
@@ -1538,8 +1545,8 @@ static int upload_tree(dbl_ctx *ctx, const dbl_kdtree *t) {
 static int upload_model(dbl_ctx *ctx, const dbl_model_desc *d) {
   const int A = d->num_attrs;
   ctx->h_attrs.resize(A);
-  ctx->dtab.resize((size_t)A * 11);
-  ctx->itab.resize((size_t)A * 4);
+  ctx->dtab.resize((size_t)A * 13);
+  ctx->itab.resize((size_t)A * 6);
   auto up_d = [&](DevBuf<double> &b, const std::vector<double> &v) -> cudaError_t {
     cudaError_t e = b.alloc(v.size());
     if (e != cudaSuccess) return e;
@@ -1561,6 +1568,7 @@ static int upload_model(dbl_ctx *ctx, const dbl_model_desc *d) {
     Hmax = std::max(Hmax, d->indexes[a]->hsize);
   }
   std::vector<dbl_index> rehashed(A);
+  ctx->sc_code_max = 0;
   for (int a = 0; a < A; ++a) {
     const dbl_index *ix = d->indexes[a];
     if (hash_ok && !ix->is_const && ix->hsize != Hmax) {
@@ -1569,8 +1577,8 @@ static int upload_model(dbl_ctx *ctx, const dbl_model_desc *d) {
       if (rehashed[a].hsize != Hmax) hash_ok = false;
       ix = &rehashed[a];
     }
-    DevBuf<double> *t = &ctx->dtab[(size_t)a * 11];
-    DevBuf<int> *ti = &ctx->itab[(size_t)a * 4];
+    DevBuf<double> *t = &ctx->dtab[(size_t)a * 13];
+    DevBuf<int> *ti = &ctx->itab[(size_t)a * 6];
     CUDA_TRY(up_d(t[0], ix->phi));
     CUDA_TRY(up_d(t[1], ix->probs));
     CUDA_TRY(up_d(t[2], ix->norm));
@@ -1595,7 +1603,22 @@ static int upload_model(dbl_ctx *ctx, const dbl_model_desc *d) {
       std::vector<int32_t> hm(ix->hmult.begin(), ix->hmult.end());
       CUDA_TRY(up_i(ti[3], hm));
     }
+    const bool sc = !ix->pcode.empty();
+    if (!ix->is_const && !sc) ctx->sc_code_max = -1;
+    if (sc) {
+      CUDA_TRY(up_i(ti[4], ix->pcode));
+      CUDA_TRY(up_i(ti[5], ix->sckeys));
+      CUDA_TRY(up_d(t[11], ix->scvals));
+      // 1/n(y) of the missing-value records, indexed by the code the tiles carry (codes no value has: 1)
+      const int cmax = *std::max_element(ix->pcode.begin(), ix->pcode.end());
+      if (ctx->sc_code_max >= 0) ctx->sc_code_max = std::max(ctx->sc_code_max, cmax);
+      std::vector<double> inv((size_t)cmax + 1, 1.0);
+      for (int v = 0; v < ix->V; ++v) inv[ix->pcode[v]] = ix->invnorm[v];
+      CUDA_TRY(up_d(t[12], inv));
+    }
     AttrDev &h = ctx->h_attrs[a];
+    h.pcode = sc ? ti[4].p : nullptr; h.sckeys = sc ? ti[5].p : nullptr;
+    h.scvals = sc ? t[11].p : nullptr; h.scinvnorm = sc ? t[12].p : nullptr;
     h.V = ix->V; h.is_const = ix->is_const ? 1 : 0; h.kmax = ix->kmax; h.hsize = ix->hsize;
     h.hshift = ix->hshift; h.pad0 = h.pad1 = h.pad2 = 0;
     h.hvals = t[9].p; h.hkeys = ti[2].p; h.hmult = reinterpret_cast<const unsigned *>(ti[3].p);
@@ -1748,9 +1771,13 @@ static int alloc_blocks(dbl_ctx *ctx) {
   const size_t max_tiles = (size_t)(ctx->E / TE) + (size_t)P + 1;
   CUDA_TRY(ctx->tiles.alloc(max_tiles * tile_words(ctx->A)));
   ctx->qtile_pk = (ctx->pack_consts && ctx->hslots == 32) ? 1 : 0;
+  // slot codes in the packed tiles when every non-constant attribute has them
+  ctx->qtile_sc = (ctx->qtile_pk && ctx->n_str > 0 && ctx->sc_code_max >= 0) ? 1 : 0;
+  if (getenv("DBL_NO_SC")) ctx->qtile_sc = 0;  // tests: the per-record hash multipliers on a model that colours
   ctx->qtile_id16 = ctx->qtile_pk;
   for (int a = 0; a < ctx->A; ++a)
     if (!ctx->h_attrs[a].is_const && ctx->h_attrs[a].V > 65536) ctx->qtile_id16 = 0;
+  if (ctx->qtile_sc && ctx->sc_code_max > 65535) ctx->qtile_id16 = 0;  // the codes may exceed the value ids
   if (getenv("DBL_NO_ID16")) ctx->qtile_id16 = 0;  // tests: the 32-bit packed tiles on a model that fits 16 bits
   {
     // work item and grid of the persistent PCG-II kernel for this model shape (see pcg2_rpw)
@@ -1898,7 +1925,7 @@ static int ensure_tiles(dbl_ctx *ctx, int fmt) {
                                                                  ctx->ent_sorted.p, ctx->ent_ptr.p, ctx->tile_ptr.p,
                                                                  ctx->tiles.p, ctx->perm_dev.p, ctx->P, ctx->pack_consts,
                                                                  ctx->qtiles.p, ctx->n_str, ctx->qtile_pk,
-                                                                 ctx->qtile_id16);
+                                                                 ctx->qtile_id16, ctx->qtile_sc ? ctx->attrs.p : nullptr);
   ctx->launches += 1;
   ctx->tiles_valid[fmt - 1] = true;
   CUDA_TRY(cudaGetLastError());
@@ -2406,6 +2433,7 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
   lp.cta_ptr = ctx->cta_ptr.p; lp.ent_sorted = ctx->ent_sorted.p; lp.rec_sorted = ctx->rec_sorted.p;
   lp.tiles = ctx->tiles.p; lp.newlink = ctx->newlink.p;
   lp.qtiles = ctx->qtiles.p; lp.qtile_pk = ctx->qtile_pk; lp.qtile_id16 = ctx->qtile_id16;
+  lp.qtile_sc = ctx->qtile_sc;
   lp.work = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_WORK);
   lp.lane_sums = ctx->lane_sums.p;
   lp.status = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_STATUS);
@@ -2817,6 +2845,7 @@ static int preload_kernels(dbl_ctx *ctx) {
     LinkParams lp;
     memset(&lp, 0, sizeof(lp));
     lp.hslots = ctx->hslots; lp.qtile_pk = ctx->qtile_pk; lp.qtile_id16 = ctx->qtile_id16;
+    lp.qtile_sc = ctx->qtile_sc;
     int rc = dispatch_pcg2(ctx, 0, lp);  // grid 0 = load only
     if (rc) return rc;
   }

@@ -11,7 +11,9 @@
 #include <limits>
 #include <map>
 #include <numeric>
+#include <queue>
 #include <thread>
+#include <tuple>
 
 #include "dbl_internal.h"
 
@@ -120,6 +122,7 @@ void dbl_index::build_hash(int min_slots) {
   hsize = 0;
   hshift = 32;
   hmult.clear(); hkeys.clear(); hvals.clear();
+  pcode.clear(); sckeys.clear(); scvals.clear();
   if (is_const) return;
   int maxlen = 0;
   for (int v = 0; v < V; ++v) maxlen = std::max(maxlen, rowptr[v + 1] - rowptr[v] + 1);
@@ -160,9 +163,84 @@ void dbl_index::build_hash(int min_slots) {
     if (ok) {
       hsize = H; hshift = shift;
       hmult.swap(mult); hkeys.swap(keys); hvals.swap(vals);
+      build_slot_codes();
       return;
     }
   }
+}
+
+// Slot codes for the 32-slot tables: colour the values with 32 colours so that the values of every row's table
+// T(x) = {x} + row(x) get distinct colours; then pcode(v) = colour(v) + 32 k, k numbering the values of v's colour in
+// ascending id order, is a bijection whose low five bits are the slot of v in every table that holds v.  The link
+// kernel stores pcode(y) in its tiles and hashes a candidate once for all the records it scores.  Greedy colouring
+// (DSatur order: the value with the most distinct colours among its conflicts first, then the most conflicts), each
+// value taking the allowed colour used least so far, which keeps the code range close to V.  No table is built when
+// some value runs out of colours.
+void dbl_index::build_slot_codes() {
+  pcode.clear(); sckeys.clear(); scvals.clear();
+  if (is_const || hsize != 32) return;
+  constexpr int H = 32;
+  // T(x) without a duplicate of x (a row may hold its own diagonal), and its transpose: the x with v in T(x)
+  std::vector<int32_t> tptr(V + 1, 0), tval;
+  tval.reserve((size_t)V + rowptr[V]);
+  for (int x = 0; x < V; ++x) {
+    tval.push_back(x);
+    for (int p = rowptr[x]; p < rowptr[x + 1]; ++p)
+      if (col[p] != x) tval.push_back(col[p]);
+    tptr[x + 1] = (int32_t)tval.size();
+  }
+  std::vector<int32_t> iptr(V + 1, 0), ival(tval.size());
+  for (int32_t v : tval) ++iptr[v + 1];
+  for (int v = 0; v < V; ++v) iptr[v + 1] += iptr[v];
+  {
+    std::vector<int32_t> fill(iptr.begin(), iptr.end() - 1);
+    for (int x = 0; x < V; ++x)
+      for (int i = tptr[x]; i < tptr[x + 1]; ++i) ival[fill[tval[i]]++] = x;
+  }
+  std::vector<int64_t> deg(V, 0);  // conflicts counted with multiplicity: an ordering key only
+  for (int v = 0; v < V; ++v)
+    for (int i = iptr[v]; i < iptr[v + 1]; ++i) deg[v] += tptr[ival[i] + 1] - tptr[ival[i]] - 1;
+  std::vector<int> colour(V, -1);
+  std::vector<uint32_t> forbid(V, 0u);
+  int64_t used[H] = {};
+  using Key = std::tuple<int, int64_t, int>;  // (distinct forbidden colours, conflicts, -value): max-heap
+  std::priority_queue<Key> heap;
+  for (int v = 0; v < V; ++v) heap.emplace(0, deg[v], -v);
+  while (!heap.empty()) {
+    const auto [sat, dg, nv] = heap.top();
+    heap.pop();
+    const int v = -nv;
+    if (colour[v] >= 0 || sat != __builtin_popcount(forbid[v])) continue;  // stale entry
+    const uint32_t allowed = ~forbid[v];
+    if (!allowed) return;  // 32 colours are not enough: the kernel keeps the per-row multipliers
+    int c = -1;
+    for (int k = 0; k < H; ++k)
+      if (((allowed >> k) & 1u) && (c < 0 || used[k] < used[c])) c = k;
+    colour[v] = c;
+    ++used[c];
+    for (int i = iptr[v]; i < iptr[v + 1]; ++i) {
+      const int x = ival[i];
+      for (int j = tptr[x]; j < tptr[x + 1]; ++j) {
+        const int u = tval[j];
+        if (colour[u] >= 0 || ((forbid[u] >> c) & 1u)) continue;
+        forbid[u] |= 1u << c;
+        heap.emplace(__builtin_popcount(forbid[u]), deg[u], -u);
+      }
+    }
+  }
+  std::vector<int32_t> code(V);
+  int64_t seen[H] = {};
+  for (int v = 0; v < V; ++v) code[v] = colour[v] + H * (int32_t)seen[colour[v]]++;
+  std::vector<int32_t> keys((size_t)V * H, -1);
+  std::vector<double> vals((size_t)V * H, 1.0);
+  for (int x = 0; x < V; ++x) {
+    keys[(size_t)x * H + colour[x]] = code[x];  // value: the diagonal exp sim (1 when absent), as in build_hash
+    for (int p = rowptr[x]; p < rowptr[x + 1]; ++p) {
+      keys[(size_t)x * H + colour[col[p]]] = code[col[p]];
+      vals[(size_t)x * H + colour[col[p]]] = expsim[p];
+    }
+  }
+  pcode.swap(code); sckeys.swap(keys); scvals.swap(vals);
 }
 
 extern "C" int dbl_index_build(dbl_index **out, const char *const *values, const double *weights, int32_t V,
@@ -448,3 +526,9 @@ extern "C" int dbl_draw_theta(int32_t A, int32_t F, const double *alpha, const d
 }
 
 extern "C" int32_t dbl_index_hash_slots(const dbl_index *ix) { return ix ? ix->hsize : 0; }
+extern "C" int dbl_index_slot_codes(const dbl_index *ix, int32_t *out) {
+  if (!ix || !out) return DBL_ERR_INVALID;
+  if (ix->pcode.empty()) return DBL_ERR_STATE;
+  std::copy(ix->pcode.begin(), ix->pcode.end(), out);
+  return DBL_OK;
+}

@@ -223,8 +223,14 @@ struct dbl_index {
   std::vector<uint32_t> hmult;     // V
   std::vector<int32_t> hkeys;      // V x hsize, -1 = empty
   std::vector<double> hvals;       // V x hsize
+  // slot codes (hsize == 32 only; empty when the values do not colour): pcode[v] & 31 is the slot of v in EVERY row's
+  // table, so a candidate is hashed once for all records; the code-keyed tables lay each row out by those slots
+  std::vector<int32_t> pcode;      // V, a bijection onto a subset of [0, 32 * (largest colour class))
+  std::vector<int32_t> sckeys;     // V x 32, key = pcode of the entry's value, -1 = empty
+  std::vector<double> scvals;      // V x 32
   void finish();
   void build_hash(int min_slots = 32);
+  void build_slot_codes();
 };
 
 struct dbl_kdtree {

@@ -47,6 +47,9 @@ struct AttrDev {
   const double *diag;  // E(v, v) of every value (1 when the sparse row has no diagonal entry): no search per record
   const int *rowptr, *col, *hkeys;
   const unsigned *hmult;
+  // slot codes (32-slot tables that colour; else null): pcode[v], the code-keyed tables (V x 32) and invnorm by code
+  const int *pcode, *sckeys;
+  const double *scvals, *scinvnorm;
 };
 
 // Control block of a context (device memory, 64-bit words): the sweep is enqueued without host round trips, so
@@ -101,6 +104,7 @@ struct LinkParams {
   const int *qtiles;         // quad tiles (k_link_pcg2)
   int qtile_pk;              // quad tiles hold the non-constant values + the byte-packed constants (else all A values)
   int qtile_id16;            // ... and those non-constant values are 16-bit, two per word (qtile_nv)
+  int qtile_sc;              // ... and they are slot codes (AttrDev::pcode), not value ids
   unsigned long long *work;  // k_link_pcg2: next group of records to take (persistent CTAs); zeroed before the launch
   double *lane_sums;         // k_link_pcg2: scratch, [CTA][consumer warp][32 chunks][32 lanes] pass-1 lane sums
   int *newlink;

@@ -1,8 +1,10 @@
-// k_link_pcg2<A, NS, HC, PK, ID16>: the PCG-II link update (updateEntityIdCollapsed, GU:363-395) with everything about
-// the model shape known at compile time: A attributes in kernel order, the last NS of them non-constant; HC = 32
+// k_link_pcg2<A, NS, HC, PK, ID16, SC>: the PCG-II link update (updateEntityIdCollapsed, GU:363-395) with everything
+// about the model shape known at compile time: A attributes in kernel order, the last NS of them non-constant; HC = 32
 // when the hash tables have 32 slots (else the size is a run-time parameter); PK = the constant attributes arrive
 // byte-packed; ID16 (PK only) = the non-constant values arrive as 16-bit halves, two per word (every non-constant
-// vocabulary has <= 65536 values).  ID16 is a tile format, not a kernel shape: dbl_link_kernel does not report it.
+// value, or SC code, is < 65536); SC (PK only) = those values are slot codes (AttrDev::pcode, dbl_index::
+// build_slot_codes) whose low five bits are the value's slot in every record's table.  ID16 and SC are tile formats,
+// not kernel shapes: dbl_link_kernel does not report them.
 //
 //  * persistent CTAs: the grid is a few CTAs per SM; each takes the next group of LINK_WARPS records of some block
 //    from a device-side counter until none is left (no empty CTAs on a shard that owns 1/8 of the records, no tail);
@@ -13,13 +15,15 @@
 //    (ID16: 3 words of values + the packed word) and the LDS.64 of N = 6 wavefronts per warp-step, against two
 //    LDS.128 + N = 10 with 32-bit values; the unpacking costs one LOP3 or SHF per value (6 per candidate, shared by
 //    the warp's two records);
-//  * each consumer warp owns one record; its constants (value ids, hash multipliers) are registers;
+//  * each consumer warp owns one record (two in the 32-slot shapes); its constants (value ids, hash multipliers
+//    unless SC) are registers;
 //  * constant attributes: the product of the exact-match multipliers comes from a 16-entry per-record table indexed
 //    by the byte-wise match mask of the packed values (PK), else from per-attribute compares;
 //  * non-constant attributes: ONE probe per (candidate, attribute) of a 32-slot perfect-hash table in shared memory
 //    (one key word per bank = one conflict-free wavefront) that holds the record's similarity row INCLUDING the
 //    record's own value, whose entry carries the exact-match multiplier of protocol 4.1 -- so "equal" and "similar"
-//    are the same look-up, and a lane multiplies only where it hit (predicated, no warp vote);
+//    are the same look-up, and a lane multiplies only where it hit (predicated, no warp vote); with SC the slot is
+//    code & 31, computed once per (candidate, attribute) for both records of the warp (no per-record multiplier);
 //  * records with a missing non-constant value multiply by 1/n(y): the two-record shapes keep the NS table pointers
 //    in registers for the whole work item (fetching them per step and attribute cost 15 % of the kernel at 1 M);
 //  * lane l scores candidate 32*step + l; lane sums / chunk totals / draw as in DESIGN.md section 4.
@@ -37,11 +41,11 @@ __device__ __forceinline__ void mul_if_eq(double &w, int y, int x, double r) {
   if (y == x) w = w * r;
 }
 
-template <int A, int NS>
+template <int A, int NS, bool SC>
 struct Pcg2Rec {
-  int x[A];                      // record value id; -1 = missing (never equals an entity value)
-  double rm[A];                  // multiplier on an exact match
-  unsigned hm[NS > 0 ? NS : 1];  // hash multipliers of the non-constant attributes
+  int x[A];                                // record value id; -1 = missing (never equals an entity value)
+  double rm[A];                            // multiplier on an exact match
+  unsigned hm[(NS > 0 && !SC) ? NS : 1];  // hash multipliers of the non-constant attributes (SC: none)
   unsigned mmask;                // missing non-constant attributes (bit = kernel position)
   unsigned xpack;                // PK: the record's constant-attribute values, one byte each (0xFF = cannot match)
 };
@@ -95,12 +99,16 @@ __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *til
 // With skewed (Zipf-like) value frequencies some lane of the warp finds an equal or similar value on almost every
 // step (96 % at BASELINE's 1M configuration), so a warp-wide vote that skips the multiplies does not pay: the
 // multiplies are predicated per lane and the compiler is free to overlap them with the next step's loads.
-// invnorm: the 1/n(y) tables of the non-constant attributes in kernel order when the caller keeps them in registers;
-// nullptr: read through p.attrs.
-template <int A, int NS, int HC, bool PK, bool MISSING = true>
-__device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const LinkParams &p, const char *tab,
+// SC: the non-constant values are slot codes (AttrDev::pcode), whose low five bits are the slot in every record's
+// table: the slot of a probe does not depend on the record, so it is computed once for the warp's records, which need
+// no multipliers.
+// invnorm: the 1/n(y) tables of the non-constant attributes in kernel order (SC: indexed by code) when the caller
+// keeps them in registers; nullptr: read through p.attrs.
+template <int A, int NS, int HC, bool PK, bool SC, bool MISSING = true>
+__device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS, SC> &rc, const LinkParams &p, const char *tab,
                                               const double *ctab, const Pcg2Cand<A, NS, PK> &cd,
                                               const double *const *invnorm = nullptr) {
+  static_assert(!SC || (PK && HC == 32), "slot codes only in the packed 32-slot tiles");
   const int hslots = HC ? HC : p.hslots;
   const int hshift = HC ? 27 : p.hshift;
   const int tabb = pcg2_tab_bytes(hslots);
@@ -122,7 +130,11 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const Li
 #pragma unroll
   for (int q = 0; q < NS; ++q) {
     const int yv = y[A - NS + q];
-    const unsigned slot = ((unsigned)yv * rc.hm[q]) >> hshift;
+    unsigned slot;
+    // SC: the AND is opaque to the compiler, which would otherwise fold it into (y << 2) & 0x7C and (y << 3) & 0xF8
+    // (two more instructions per probe); kept as an AND, each table address is one multiply-add of the slot
+    if constexpr (SC) asm("and.b32 %0, %1, 31;" : "=r"(slot) : "r"(yv));
+    else slot = ((unsigned)yv * rc.hm[q]) >> hshift;
     if (reinterpret_cast<const int *>(tab + q * tabb)[slot] == yv)
       w = w * reinterpret_cast<const double *>(tab + q * tabb + hslots * 4)[slot];
   }
@@ -130,7 +142,8 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS> &rc, const Li
 #pragma unroll
     for (int q = 0; q < NS; ++q)
       if ((rc.mmask >> (A - NS + q)) & 1u)
-        w = w * (invnorm ? __ldg(invnorm[q] + y[A - NS + q]) : p.attrs[p.perm[A - NS + q]].invnorm[y[A - NS + q]]);
+        w = w * (invnorm ? __ldg(invnorm[q] + y[A - NS + q])
+                         : (SC ? p.attrs[p.perm[A - NS + q]].scinvnorm : p.attrs[p.perm[A - NS + q]].invnorm)[y[A - NS + q]]);
   }
   return w;
 }
@@ -146,7 +159,7 @@ __host__ __device__ constexpr int pcg2_rpw(int HC, int NS) { return (HC == 32 &&
 // 3 CTAs per SM (72 registers) only where one record per warp fits them: few non-constant attributes
 __host__ __device__ constexpr int pcg2_ctas_per_sm(int HC, int NS) { return (pcg2_rpw(HC, NS) >= 2 || NS > 6) ? 2 : 3; }
 
-template <int A, int NS, int HC, bool PK, bool ID16>
+template <int A, int NS, int HC, bool PK, bool ID16, bool SC>
 __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS)) k_link_pcg2(LinkParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ int s_cta;
@@ -191,7 +204,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
     }
 
     // ---- per-record constants: lane k prepares kernel-order attribute k, then everything is broadcast
-    Pcg2Rec<A, NS> rc[RPW];
+    Pcg2Rec<A, NS, SC> rc[RPW];
     int rr[RPW];
     bool act[RPW];
 #pragma unroll
@@ -220,7 +233,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
           } else {
             d = d * at.norm[xv];
             rmv = at.diag[xv] + (1.0 - th) / d;
-            hmv = at.hmult[xv];
+            if constexpr (!SC) hmv = at.hmult[xv];
           }
         }
       }
@@ -231,8 +244,10 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
         rc[ri].x[k] = __shfl_sync(FULL, xv, k);
         rc[ri].rm[k] = shfl_d(rmv, k);
       }
+      if constexpr (!SC) {
 #pragma unroll
-      for (int q = 0; q < NS; ++q) rc[ri].hm[q] = __shfl_sync(FULL, hmv, A - NS + q);
+        for (int q = 0; q < NS; ++q) rc[ri].hm[q] = __shfl_sync(FULL, hmv, A - NS + q);
+      }
       // hash tables of the record's similarity rows -> shared memory (all-empty table when the value is missing);
       // the entry of the record's own value gets the exact-match multiplier (it depends on theta of the record's file)
       const int H = HC ? HC : p.hslots;
@@ -243,10 +258,15 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
         int *kd = reinterpret_cast<int *>(tab + q * pcg2_tab_bytes(H));
         double *vd = reinterpret_cast<double *>(tab + q * pcg2_tab_bytes(H) + H * 4);
         const int xq = rc[ri].x[A - NS + q];
-        const unsigned own = (xq >= 0) ? (((unsigned)xq * rc[ri].hm[q]) >> hshift) : 0xFFFFFFFFu;
+        // SC: the code-keyed tables, each value at the slot its code names
+        const int *hkeys = SC ? at.sckeys : at.hkeys;
+        const double *hvals = SC ? at.scvals : at.hvals;
+        unsigned own;
+        if constexpr (SC) own = (xq >= 0) ? ((unsigned)at.pcode[xq] & 31u) : 0xFFFFFFFFu;
+        else own = (xq >= 0) ? (((unsigned)xq * rc[ri].hm[q]) >> hshift) : 0xFFFFFFFFu;
         for (int i = lane; i < H; i += 32) {
-          kd[i] = (xq >= 0) ? at.hkeys[(size_t)xq * H + i] : -1;
-          vd[i] = ((unsigned)i == own) ? rc[ri].rm[A - NS + q] : ((xq >= 0) ? at.hvals[(size_t)xq * H + i] : 1.0);
+          kd[i] = (xq >= 0) ? hkeys[(size_t)xq * H + i] : -1;
+          vd[i] = ((unsigned)i == own) ? rc[ri].rm[A - NS + q] : ((xq >= 0) ? hvals[(size_t)xq * H + i] : 1.0);
         }
       }
       rc[ri].xpack = 0xFFFFFFFFu;
@@ -284,7 +304,8 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
       constexpr bool HOIST = MISSING && RPW == 2;
       const double *invnorm[NS > 0 ? NS : 1];
 #pragma unroll
-      for (int q = 0; q < NS; ++q) invnorm[q] = HOIST ? p.attrs[p.perm[A - NS + q]].invnorm : nullptr;
+      for (int q = 0; q < NS; ++q)
+        invnorm[q] = HOIST ? (SC ? p.attrs[p.perm[A - NS + q]].scinvnorm : p.attrs[p.perm[A - NS + q]].invnorm) : nullptr;
       for (int t = 0; t < ntiles; ++t) {
         const int g = tbase + t;
         const int s = g % LINK_STAGES;
@@ -297,8 +318,8 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
             pcg2_load<A, NS, PK, ID16>(cd, tile, q * 32 + lane);
 #pragma unroll
             for (int ri = 0; ri < RPW; ++ri)
-              acc[ri] = acc[ri] + pcg2_weight<A, NS, HC, PK, MISSING>(rc[ri], p, tab0 + ri * tabrec,
-                                                                    ctab0 + ri * 16, cd, HOIST ? invnorm : nullptr);
+              acc[ri] = acc[ri] + pcg2_weight<A, NS, HC, PK, SC, MISSING>(rc[ri], p, tab0 + ri * tabrec,
+                                                                        ctab0 + ri * 16, cd, HOIST ? invnorm : nullptr);
           }
           if (++tile_in_chunk == geo.tpc || t + 1 == ntiles) {
 #pragma unroll
@@ -328,7 +349,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
         if (j >= n) return 0.0;
         Pcg2Cand<A, NS, PK> cd;
         pcg2_load<A, NS, PK, ID16>(cd, gtiles + (size_t)(j / TE) * TW, j % TE);
-        return pcg2_weight<A, NS, HC, PK>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
+        return pcg2_weight<A, NS, HC, PK, SC>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
       };
       const U2 u = link_uniform(p, r);
       const int j = finish_draw(lane, n, geo, Q[ri], run[ri], u.u0, wf, my_sums + ri * 1024);
@@ -345,20 +366,20 @@ inline size_t pcg2_smem_bytes(int A, int NS, int H, bool PK, bool id16) {
 
 // launch k_link_pcg2<A, NS, HC> for a runtime NS in [0, A]; HC = 32 (compile-time table size) when the model's
 // tables have 32 slots, else 0 (size read from the parameters); returns cudaError_t as int
-template <int A, int NS, int HC, bool PK, bool ID16>
+template <int A, int NS, int HC, bool PK, bool ID16, bool SC = false>
 int pcg2_launch_one(int grid, cudaStream_t stream, const LinkParams &lp, size_t *configured) {
   const size_t smem = pcg2_smem_bytes(A, NS, lp.hslots, PK, ID16);
   // the opt-in is per device: the cache belongs to the context (one model shape = one instantiation per context)
   if (*configured < smem) {
-    cudaError_t e = cudaFuncSetAttribute(k_link_pcg2<A, NS, HC, PK, ID16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(k_link_pcg2<A, NS, HC, PK, ID16, SC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     *configured = smem;
   }
   if (grid <= 0) {  // load the kernel without running it (see preload_kernels in dbl_engine.cu)
     cudaFuncAttributes fa;
-    return (int)cudaFuncGetAttributes(&fa, k_link_pcg2<A, NS, HC, PK, ID16>);
+    return (int)cudaFuncGetAttributes(&fa, k_link_pcg2<A, NS, HC, PK, ID16, SC>);
   }
-  k_link_pcg2<A, NS, HC, PK, ID16><<<grid, (LINK_WARPS + 1) * 32, smem, stream>>>(lp);
+  k_link_pcg2<A, NS, HC, PK, ID16, SC><<<grid, (LINK_WARPS + 1) * 32, smem, stream>>>(lp);
   return (int)cudaGetLastError();
 }
 
@@ -367,8 +388,14 @@ struct Pcg2Launch {
   static int go(int ns, int grid, cudaStream_t stream, const LinkParams &lp, size_t *cfg) {
     if (ns == NS) {
       // byte-packed constant attributes: 1..4 of them, every vocabulary <= 255, 32-slot tables (lp.qtile_pk);
-      // 16-bit non-constant values when every non-constant vocabulary has <= 65536 values (lp.qtile_id16)
+      // 16-bit non-constant values when every non-constant vocabulary (SC: every slot code) fits (lp.qtile_id16);
+      // slot codes when every non-constant attribute has them (lp.qtile_sc)
       if constexpr (A - NS >= 1 && A - NS <= 4) {
+        if constexpr (NS >= 1) {
+          if (lp.qtile_pk && lp.qtile_sc)
+            return lp.qtile_id16 ? pcg2_launch_one<A, NS, 32, true, true, true>(grid, stream, lp, cfg)
+                                 : pcg2_launch_one<A, NS, 32, true, false, true>(grid, stream, lp, cfg);
+        }
         if (lp.qtile_pk) return lp.qtile_id16 ? pcg2_launch_one<A, NS, 32, true, true>(grid, stream, lp, cfg)
                                               : pcg2_launch_one<A, NS, 32, true, false>(grid, stream, lp, cfg);
       }

@@ -106,6 +106,17 @@ class AttributeIndex:
                                             _p(col, _lib.i32p), _p(es, _lib.f64p)), "AttributeIndex.tables")
         return {"phi": phi, "norm": norm, "rowptr": rowptr, "col": col[:nnz], "expsim": es[:nnz]}
 
+    @property
+    def slot_codes(self):
+        """Slot codes of the 32-slot hash tables (int32, one per value id; code & 31 is the value's slot in every
+        row's table), or None when the index has none."""
+        out = np.zeros(self.num_values, np.int32)
+        rc = _lib.load().dbl_index_slot_codes(self._h, _p(out, _lib.i32p))
+        if rc == _lib.ERR_STATE:
+            return None
+        _check(rc, "AttributeIndex.slot_codes")
+        return out
+
     def _require(self, v):
         if not 0 <= v < self.num_values:
             raise IndexError("valueId is not in the index")  # AttributeIndex.scala:137

@@ -56,6 +56,10 @@ int32_t dbl_index_nnz(const dbl_index *);
 /* slots of the per-row perfect-hash tables the link kernel probes (32 = the fast instantiations; 0 = none: constant
  * attribute, or rows too long for a table) */
 int32_t dbl_index_hash_slots(const dbl_index *);
+/* slot codes of the 32-slot tables (num_values entries): a bijection of the value ids whose low five bits give each
+ * value the same slot in every row's table; DBL_ERR_STATE when the index has none (other table sizes, or values that
+ * did not colour) */
+int dbl_index_slot_codes(const dbl_index *, int32_t *out);
 int32_t dbl_index_value_id(const dbl_index *, const char *value); /* valueIdxOf; -1 when absent              */
 const char *dbl_index_value(const dbl_index *, int32_t value_id);
 /* copies of the tables (arrays sized num_values, num_values+1, nnz, nnz); any pointer may be NULL */
