@@ -2399,7 +2399,8 @@ static int ensure_inverted_index(dbl_ctx *ctx) {
 
 static bool pcg2_kernel_fits(const dbl_ctx *ctx) {
   return ctx->hslots > 0 && ctx->A <= LINK_MAX_UNROLL_A &&
-         pcg2_smem_bytes(ctx->A, ctx->n_str, ctx->hslots, ctx->qtile_pk != 0, ctx->qtile_id16 != 0) <= 100 * 1024;
+         pcg2_smem_bytes(ctx->A, ctx->n_str, ctx->hslots, ctx->qtile_pk != 0, ctx->qtile_id16 != 0,
+                         ctx->qtile_sc != 0) <= 100 * 1024;
 }
 static int dispatch_pcg2(dbl_ctx *ctx, int grid, const LinkParams &lp) {
   int rc = -1;

@@ -14,7 +14,7 @@
 //    shared-memory loads instead of one load per word: at 6 non-constant attributes + packed constants, ONE LDS.128
 //    (ID16: 3 words of values + the packed word) and the LDS.64 of N = 6 wavefronts per warp-step, against two
 //    LDS.128 + N = 10 with 32-bit values; the unpacking costs one LOP3 or SHF per value (6 per candidate, shared by
-//    the warp's two records);
+//    the warp's two records; one PRMT per value with paired tables);
 //  * each consumer warp owns one record (two in the 32-slot shapes); its constants (value ids, hash multipliers
 //    unless SC) are registers;
 //  * constant attributes: the product of the exact-match multipliers comes from a 16-entry per-record table indexed
@@ -24,6 +24,8 @@
 //    record's own value, whose entry carries the exact-match multiplier of protocol 4.1 -- so "equal" and "similar"
 //    are the same look-up, and a lane multiplies only where it hit (predicated, no warp vote); with SC the slot is
 //    code & 31, computed once per (candidate, attribute) for both records of the warp (no per-record multiplier);
+//    with ID16 and SC the two records' tables are paired (PAIR_KEYS): one key word holds both records' 16-bit keys
+//    of a slot, so one key load and one value address serve both records;
 //  * records with a missing non-constant value multiply by 1/n(y): the two-record shapes keep the NS table pointers
 //    in registers for the whole work item (fetching them per step and attribute cost 15 % of the kernel at 1 M);
 //  * lane l scores candidate 32*step + l; lane sums / chunk totals / draw as in DESIGN.md section 4.
@@ -35,6 +37,13 @@
 // Per (record, non-constant attribute): H key words then H f64 values, H = p.hslots (a power of two >= 32, the same
 // for every attribute of the model; 32 = one key per bank = conflict-free probes).
 __device__ __host__ __forceinline__ int pcg2_tab_bytes(int H) { return H * 12; }
+
+// Paired tables (16-bit slot codes, two records per warp: pcg2_paired): per (warp, non-constant attribute) 32 key
+// words, word s = the key of record 0 at slot s in the low half and record 1's in the high half (one word per bank:
+// one conflict-free probe serves both records), then record 0's 32 f64 values, then record 1's, PAIR_VALS bytes
+// further: both value loads of a probe share one address.  An empty half at slot s holds s ^ 1, which no code with
+// code & 31 == s equals.
+constexpr int PAIR_KEYS = 32 * 4, PAIR_VALS = 32 * 8, PAIR_ATTR_BYTES = PAIR_KEYS + 2 * PAIR_VALS;
 
 // w *= r when y == x (shapes without the packed-constant table; ptxas turns any predicated form into DMUL + 2 FSEL)
 __device__ __forceinline__ void mul_if_eq(double &w, int y, int x, double r) {
@@ -66,6 +75,7 @@ __device__ __forceinline__ unsigned pcg2_const_offset(unsigned ypack, unsigned x
 template <int A, int NS, bool PK>
 struct Pcg2Cand {
   int y[A];
+  unsigned y16[(NS + 1) / 2 > 0 ? (NS + 1) / 2 : 1];  // ID16: the words of 16-bit values as loaded
   unsigned ypack;
   double N;
 };
@@ -81,6 +91,8 @@ __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *til
     v[4 * g] = t.x; v[4 * g + 1] = t.y; v[4 * g + 2] = t.z; v[4 * g + 3] = t.w;
   }
   if constexpr (PK && ID16) {
+#pragma unroll
+    for (int q2 = 0; q2 < (NS + 1) / 2; ++q2) c.y16[q2] = (unsigned)v[q2];
 #pragma unroll
     for (int q2 = 0; q2 < NS; ++q2) c.y[A - NS + q2] = (int)(q2 & 1 ? (unsigned)v[q2 >> 1] >> 16 : v[q2 >> 1] & 0xFFFF);
     c.ypack = (unsigned)v[(NS + 1) / 2];
@@ -148,6 +160,47 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS, SC> &rc, cons
   return w;
 }
 
+// Paired tables (pcg2_paired): the weights of one candidate for the warp's records whose bit is set in `recs`, in w[0]
+// and w[1]; each is the product pcg2_weight forms, factor for factor in the same order.  Per (candidate, attribute):
+// one PRMT spreads the 16-bit code over both halves of a word, c2 = {code, code}; ONE key load at slot code & 31
+// serves both records, whose hits are the halves of k ^ c2 that are zero; one value address serves both predicated
+// value loads (record 1's values are PAIR_VALS bytes past record 0's).
+template <int A, int NS, bool MISSING = true>
+__device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc)[2], unsigned recs, const LinkParams &p,
+                                                 const char *tab, const double *ctab, const Pcg2Cand<A, NS, true> &cd,
+                                                 double (&w)[2], const double *const *invnorm = nullptr) {
+  static_assert(NS >= 1 && NS < A, "paired tables: packed constants and at least one non-constant attribute");
+#pragma unroll
+  for (int ri = 0; ri < 2; ++ri)  // protocol 4.1: w = N * (product of the constant attributes' multipliers)
+    w[ri] = cd.N * *reinterpret_cast<const double *>(reinterpret_cast<const char *>(ctab + ri * 16) +
+                                                     pcg2_const_offset(cd.ypack, rc[ri].xpack));
+#pragma unroll
+  for (int q = 0; q < NS; ++q) {
+    const unsigned c2 = __byte_perm(cd.y16[q >> 1], 0u, (q & 1) ? 0x3232 : 0x1010);
+    unsigned slot;  // opaque AND, as in pcg2_weight
+    asm("and.b32 %0, %1, 31;" : "=r"(slot) : "r"(c2));
+    const unsigned k = reinterpret_cast<const unsigned *>(tab + q * PAIR_ATTR_BYTES)[slot];
+    const double *v = reinterpret_cast<const double *>(tab + q * PAIR_ATTR_BYTES + PAIR_KEYS) + slot;
+    // the low half's AND is opaque too: the compiler would otherwise compare a sign-extended 16-bit value (PRMT,
+    // MOV and ISETP) instead of one LOP3 that writes the predicate
+    unsigned lo;
+    asm("and.b32 %0, %1, 0xFFFF;" : "=r"(lo) : "r"(k ^ c2));
+    if ((recs & 1u) && lo == 0u) w[0] = w[0] * v[0];
+    if ((recs & 2u) && ((k ^ c2) & 0xFFFF0000u) == 0u) w[1] = w[1] * v[PAIR_VALS / 8];
+  }
+  if (MISSING) {
+#pragma unroll
+    for (int ri = 0; ri < 2; ++ri) {
+      if (!((recs >> ri) & 1u) || !rc[ri].mmask) continue;
+#pragma unroll
+      for (int q = 0; q < NS; ++q)
+        if ((rc[ri].mmask >> (A - NS + q)) & 1u)
+          w[ri] = w[ri] * (invnorm ? __ldg(invnorm[q] + cd.y[A - NS + q])
+                                   : p.attrs[p.perm[A - NS + q]].scinvnorm[cd.y[A - NS + q]]);
+    }
+  }
+}
+
 // Records per consumer warp.  With 2, a lane fetches its candidate once and scores it for both records: half the
 // tile loads and half the tile traffic through shared memory per (record, candidate) pair, two independent
 // dependency chains per warp; the price is registers (96 instead of 72: 2 CTAs per SM instead of 3) and twice the
@@ -158,6 +211,14 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS, SC> &rc, cons
 __host__ __device__ constexpr int pcg2_rpw(int HC, int NS) { return (HC == 32 && NS >= 1 && NS <= 8) ? 2 : 1; }
 // 3 CTAs per SM (72 registers) only where one record per warp fits them: few non-constant attributes
 __host__ __device__ constexpr int pcg2_ctas_per_sm(int HC, int NS) { return (pcg2_rpw(HC, NS) >= 2 || NS > 6) ? 2 : 3; }
+// the two records of a warp share paired key tables (PAIR_KEYS) when every code fits 16 bits
+__host__ __device__ constexpr bool pcg2_paired(int HC, int NS, bool ID16, bool SC) {
+  return ID16 && SC && pcg2_rpw(HC, NS) == 2;
+}
+// bytes of one consumer warp's hash tables (H = the table size of the model)
+__host__ __device__ inline int pcg2_warp_tab_bytes(int H, int NS, bool paired) {
+  return paired ? NS * PAIR_ATTR_BYTES : pcg2_rpw(H == 32 ? 32 : 0, NS) * (NS > 0 ? NS : 1) * pcg2_tab_bytes(H);
+}
 
 template <int A, int NS, int HC, bool PK, bool ID16, bool SC>
 __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS)) k_link_pcg2(LinkParams p) {
@@ -177,11 +238,13 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
   rg.empty = rg.full + LINK_STAGES;
   rg.tw = TW;
   static_assert(2 * LINK_STAGES * 8 <= 128, "barrier area");
+  constexpr bool PAIR = pcg2_paired(HC, NS, ID16, SC);
   const int tabrec = (NS > 0 ? NS : 1) * pcg2_tab_bytes(HC ? HC : p.hslots);  // bytes of one record's hash tables
-  char *tab0 = reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 + (size_t)warp * RPW * tabrec;
+  const int wtab = pcg2_warp_tab_bytes(HC ? HC : p.hslots, NS, PAIR);         // ... of one warp's
+  char *tab0 = reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 + (size_t)warp * wtab;
   // PK: products of the matching constant attributes, by match mask, 16 entries per record
   double *ctab0 = reinterpret_cast<double *>(reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 +
-                                            (size_t)PCG2_RECS * tabrec) + warp * RPW * 16;
+                                            (size_t)WARPS * wtab) + warp * RPW * 16;
   ring_init(rg, WARPS);
   const int total_ctas = p.cta_ptr[p.P];
   int tbase = 0;  // tiles this CTA has streamed so far: stage and phase of the ring continue across work items
@@ -213,7 +276,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
       act[ri] = ridx < p.rec_ptr[b + 1];
       rr[ri] = act[ri] ? p.rec_sorted[ridx] : -1;
       const int r = rr[ri];
-      char *tab = tab0 + ri * tabrec;
+      char *tab = PAIR ? tab0 : tab0 + ri * tabrec;
       double *ctab = ctab0 + ri * 16;
       int xv = -1;
       double rmv = 1.0;
@@ -255,8 +318,9 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
 #pragma unroll
       for (int q = 0; q < NS; ++q) {
         const AttrDev &at = p.attrs[p.perm[A - NS + q]];
-        int *kd = reinterpret_cast<int *>(tab + q * pcg2_tab_bytes(H));
-        double *vd = reinterpret_cast<double *>(tab + q * pcg2_tab_bytes(H) + H * 4);
+        char *tq = tab + q * (PAIR ? PAIR_ATTR_BYTES : pcg2_tab_bytes(H));
+        int *kd = reinterpret_cast<int *>(tq);
+        double *vd = reinterpret_cast<double *>(tq + (PAIR ? PAIR_KEYS + ri * PAIR_VALS : H * 4));
         const int xq = rc[ri].x[A - NS + q];
         // SC: the code-keyed tables, each value at the slot its code names
         const int *hkeys = SC ? at.sckeys : at.hkeys;
@@ -265,7 +329,11 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
         if constexpr (SC) own = (xq >= 0) ? ((unsigned)at.pcode[xq] & 31u) : 0xFFFFFFFFu;
         else own = (xq >= 0) ? (((unsigned)xq * rc[ri].hm[q]) >> hshift) : 0xFFFFFFFFu;
         for (int i = lane; i < H; i += 32) {
-          kd[i] = (xq >= 0) ? hkeys[(size_t)xq * H + i] : -1;
+          const int key = (xq >= 0) ? hkeys[(size_t)xq * H + i] : -1;
+          if constexpr (PAIR)  // the record's half of the paired key word; empty: i ^ 1
+            reinterpret_cast<unsigned short *>(kd)[2 * i + ri] = (unsigned short)(key >= 0 ? key : i ^ 1);
+          else
+            kd[i] = key;
           vd[i] = ((unsigned)i == own) ? rc[ri].rm[A - NS + q] : ((xq >= 0) ? hvals[(size_t)xq * H + i] : 1.0);
         }
       }
@@ -316,10 +384,17 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
           for (int q = 0; q < TE / 32; ++q) {
             Pcg2Cand<A, NS, PK> cd;
             pcg2_load<A, NS, PK, ID16>(cd, tile, q * 32 + lane);
+            if constexpr (PAIR) {
+              double w[2];
+              pcg2_weight_pair<A, NS, MISSING>(rc, 3u, p, tab0, ctab0, cd, w, invnorm);
+              acc[0] = acc[0] + w[0];
+              acc[1] = acc[1] + w[1];
+            } else {
 #pragma unroll
-            for (int ri = 0; ri < RPW; ++ri)
-              acc[ri] = acc[ri] + pcg2_weight<A, NS, HC, PK, SC, MISSING>(rc[ri], p, tab0 + ri * tabrec,
-                                                                        ctab0 + ri * 16, cd, HOIST ? invnorm : nullptr);
+              for (int ri = 0; ri < RPW; ++ri)
+                acc[ri] = acc[ri] + pcg2_weight<A, NS, HC, PK, SC, MISSING>(rc[ri], p, tab0 + ri * tabrec,
+                                                                          ctab0 + ri * 16, cd, HOIST ? invnorm : nullptr);
+            }
           }
           if (++tile_in_chunk == geo.tpc || t + 1 == ntiles) {
 #pragma unroll
@@ -349,7 +424,13 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
         if (j >= n) return 0.0;
         Pcg2Cand<A, NS, PK> cd;
         pcg2_load<A, NS, PK, ID16>(cd, gtiles + (size_t)(j / TE) * TW, j % TE);
-        return pcg2_weight<A, NS, HC, PK, SC>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
+        if constexpr (PAIR) {  // record ri's half of the paired tables
+          double w[2];
+          pcg2_weight_pair<A, NS>(rc, 1u << ri, p, tab0, ctab0, cd, w);
+          return ri ? w[1] : w[0];
+        } else {
+          return pcg2_weight<A, NS, HC, PK, SC>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
+        }
       };
       const U2 u = link_uniform(p, r);
       const int j = finish_draw(lane, n, geo, Q[ri], run[ri], u.u0, wf, my_sums + ri * 1024);
@@ -358,17 +439,18 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
   }
 }
 
-inline size_t pcg2_smem_bytes(int A, int NS, int H, bool PK, bool id16) {
-  const size_t recs = (size_t)LINK_WARPS * pcg2_rpw(H == 32 ? 32 : 0, NS);
+inline size_t pcg2_smem_bytes(int A, int NS, int H, bool PK, bool id16, bool sc) {
+  const int HC = H == 32 ? 32 : 0;
+  const size_t recs = (size_t)LINK_WARPS * pcg2_rpw(HC, NS);
   return (size_t)LINK_STAGES * qtile_words(qtile_nv(A, NS, PK, id16)) * TE * 4 + 128 +
-         recs * (NS > 0 ? NS : 1) * pcg2_tab_bytes(H) + recs * 16 * sizeof(double);
+         (size_t)LINK_WARPS * pcg2_warp_tab_bytes(H, NS, pcg2_paired(HC, NS, id16, sc)) + recs * 16 * sizeof(double);
 }
 
 // launch k_link_pcg2<A, NS, HC> for a runtime NS in [0, A]; HC = 32 (compile-time table size) when the model's
 // tables have 32 slots, else 0 (size read from the parameters); returns cudaError_t as int
 template <int A, int NS, int HC, bool PK, bool ID16, bool SC = false>
 int pcg2_launch_one(int grid, cudaStream_t stream, const LinkParams &lp, size_t *configured) {
-  const size_t smem = pcg2_smem_bytes(A, NS, lp.hslots, PK, ID16);
+  const size_t smem = pcg2_smem_bytes(A, NS, lp.hslots, PK, ID16, SC);
   // the opt-in is per device: the cache belongs to the context (one model shape = one instantiation per context)
   if (*configured < smem) {
     cudaError_t e = cudaFuncSetAttribute(k_link_pcg2<A, NS, HC, PK, ID16, SC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
