@@ -3158,12 +3158,17 @@ extern "C" int dbl_state_hash(dbl_ctx *ctx, uint64_t *hash_out) {
 }
 
 // which link kernel a sweep with this sampler launches: 0 k_link_generic, 1 k_link_match, 2 k_link_pruned,
-// 3 k_link_pcg2 (+4 when the constants are byte-packed, +8 when the hash tables have the compile-time 32 slots)
+// 3 k_link_pcg2 (+4 when the constants are byte-packed, +8 when the hash tables have the compile-time 32 slots) and
+// its tile format, by the rules Pcg2Launch and k_link_pcg2 use (+16 16-bit ids, +32 slot codes, +64 paired key
+// tables, +128 two records per warp)
 extern "C" int dbl_link_kernel(const dbl_ctx *ctx, int sampler) {
   if (!ctx || sampler < 0 || sampler > 3) return DBL_ERR_INVALID;
   const LinkKernel kernel = link_kernel(ctx, sampler);
-  if (kernel == LINK_PCG2) return kernel + (ctx->qtile_pk ? 4 : 0) + (ctx->hslots == 32 ? 8 : 0);
-  return kernel;
+  if (kernel != LINK_PCG2) return kernel;
+  const int hc = ctx->hslots == 32 ? 32 : 0;
+  const bool id16 = ctx->qtile_id16 != 0, sc = ctx->qtile_sc != 0;
+  return kernel + (ctx->qtile_pk ? 4 : 0) + (hc == 32 ? 8 : 0) + (id16 ? 16 : 0) + (sc ? 32 : 0) +
+         (pcg2_paired(hc, ctx->n_str, id16, sc) ? 64 : 0) + (pcg2_rpw(hc, ctx->n_str) == 2 ? 128 : 0);
 }
 
 extern "C" int dbl_set_link_mode(dbl_ctx *ctx, int mode) {

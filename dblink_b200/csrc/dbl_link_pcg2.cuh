@@ -4,7 +4,7 @@
 // byte-packed; ID16 (PK only) = the non-constant values arrive as 16-bit halves, two per word (every non-constant
 // value, or SC code, is < 65536); SC (PK only) = those values are slot codes (AttrDev::pcode, dbl_index::
 // build_slot_codes) whose low five bits are the value's slot in every record's table.  ID16 and SC are tile formats,
-// not kernel shapes: dbl_link_kernel does not report them.
+// not kernel shapes: dbl_link_kernel reports them in bits of their own, beside pcg2_paired and pcg2_rpw.
 //
 //  * persistent CTAs: the grid is a few CTAs per SM; each takes the next group of LINK_WARPS records of some block
 //    from a device-side counter until none is left (no empty CTAs on a shard that owns 1/8 of the records, no tail);

@@ -333,8 +333,10 @@ int64_t dbl_kernel_launches(const dbl_ctx *);
  * All produce identical draws; this exists so tests can cover every kernel. */
 int dbl_set_link_mode(dbl_ctx *, int mode);
 /* which link kernel a sweep with this sampler launches: 0 generic fallback, 1 dense must-match kernel, 2 index-pruned
- * kernel, 3 k_link_pcg2 (+4: byte-packed constants, +8: 32-slot tables known at compile time).  A model that falls
- * back to the generic kernel runs an order of magnitude slower: benches and tests assert what they expect. */
+ * kernel, 3 k_link_pcg2 (+4: byte-packed constants, +8: 32-slot tables known at compile time) and, for k_link_pcg2
+ * only, the tile format it reads (+16: 16-bit non-constant values, +32: slot codes instead of value ids, +64: the two
+ * records of a warp share paired key tables, +128: two records per warp).  A model that falls back to the generic
+ * kernel runs an order of magnitude slower: benches and tests assert what they expect. */
 int dbl_link_kernel(const dbl_ctx *, int sampler);
 /* Link-mass capture (checking only; off by default, free when off): with on != 0 every link kernel stores the total
  * mass of each record's categorical -- the sum of its protocol weights over the block, the number the draw tests for

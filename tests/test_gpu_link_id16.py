@@ -34,6 +34,7 @@ def test_packed_tiles_against_oracle(oracle, monkeypatch, shape, width):
     eng, rc, x, file = product_setup(g, 17, 1, (A - 1,))
     eng.set_link_mass_capture(True)
     assert eng.link_kernel("PCG-II") == f"k_link_pcg2<A={A},NS={n_str},HC=32,PK=1>"
+    assert eng.link_tile_format("PCG-II")["id16"] == (width == "16")
     m, st, tree, ox, ofile = oracle_setup(oracle, g, 17, 1, (A - 1,))
     np.testing.assert_array_equal(x, ox)
     for it in range(3):

@@ -113,6 +113,7 @@ def test_paired_key_tables_against_oracle(oracle, monkeypatch, shape, width):
     assert eng.num_partitions == 1 and R % 2 == 1
     eng.set_link_mass_capture(True)
     assert eng.link_kernel("PCG-II") == f"k_link_pcg2<A={A},NS={n_str},HC=32,PK=1>"
+    assert eng.link_tile_format("PCG-II")["paired"] == (width == "16")  # the 32-bit tiles keep unpaired tables
 
     m0 = O.Model(o_idx, alpha, beta, None, seed, F)
     s0 = O.State.init(m0, x, file, 0)

@@ -40,6 +40,8 @@ def test_slot_code_tiles_against_oracle(oracle, monkeypatch, shape, width, codes
     assert (x < 0).any(axis=0)[n_const:].all()  # records with a missing value in every non-constant attribute
     eng.set_link_mass_capture(True)
     assert eng.link_kernel("PCG-II") == f"k_link_pcg2<A={A},NS={n_str},HC=32,PK=1>"
+    fmt = eng.link_tile_format("PCG-II")
+    assert (fmt["slot_codes"], fmt["id16"]) == (codes == "sc", width == "16")
     m, st, tree, ox, ofile = oracle_setup(oracle, g, 23, 1, (A - 1,))
     np.testing.assert_array_equal(x, ox)
     for it in range(3):
