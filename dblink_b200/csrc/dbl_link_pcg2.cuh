@@ -160,11 +160,24 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS, SC> &rc, cons
   return w;
 }
 
+// Paired tables: whether half H (0 low, 1 high) of k ^ c2 is zero, as one 3-input lop3, (k ^ c2) & mask, which ptxas
+// turns into one LOP3 that writes the predicate.  Written in C, the compiler computes the XOR once for both halves
+// and tests each with a LOP3 of its own (and the low half as a sign-extended 16-bit compare unless the AND is opaque).
+template <int H>
+__device__ __forceinline__ bool pcg2_half_hit(unsigned k, unsigned c2) {
+  unsigned hit;
+  asm("{\n\t.reg .pred p;\n\t.reg .b32 t;\n\tlop3.b32 t, %1, %2, %3, 0x28;\n\tsetp.eq.u32 p, t, 0;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(hit)
+      : "r"(k), "r"(c2), "n"(H ? 0xFFFF0000u : 0xFFFFu));
+  return hit != 0;
+}
+
 // Paired tables (pcg2_paired): the weights of one candidate for the warp's records whose bit is set in `recs`, in w[0]
 // and w[1]; each is the product pcg2_weight forms, factor for factor in the same order.  Per (candidate, attribute):
 // one PRMT spreads the 16-bit code over both halves of a word, c2 = {code, code}; ONE key load at slot code & 31
-// serves both records, whose hits are the halves of k ^ c2 that are zero; one value address serves both predicated
-// value loads (record 1's values are PAIR_VALS bytes past record 0's).
+// serves both records, whose hits are the halves of k ^ c2 that are zero (pcg2_half_hit); one value address serves
+// both predicated value loads (record 1's values are PAIR_VALS bytes past record 0's).
 template <int A, int NS, bool MISSING = true>
 __device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc)[2], unsigned recs, const LinkParams &p,
                                                  const char *tab, const double *ctab, const Pcg2Cand<A, NS, true> &cd,
@@ -181,12 +194,8 @@ __device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc
     asm("and.b32 %0, %1, 31;" : "=r"(slot) : "r"(c2));
     const unsigned k = reinterpret_cast<const unsigned *>(tab + q * PAIR_ATTR_BYTES)[slot];
     const double *v = reinterpret_cast<const double *>(tab + q * PAIR_ATTR_BYTES + PAIR_KEYS) + slot;
-    // the low half's AND is opaque too: the compiler would otherwise compare a sign-extended 16-bit value (PRMT,
-    // MOV and ISETP) instead of one LOP3 that writes the predicate
-    unsigned lo;
-    asm("and.b32 %0, %1, 0xFFFF;" : "=r"(lo) : "r"(k ^ c2));
-    if ((recs & 1u) && lo == 0u) w[0] = w[0] * v[0];
-    if ((recs & 2u) && ((k ^ c2) & 0xFFFF0000u) == 0u) w[1] = w[1] * v[PAIR_VALS / 8];
+    if ((recs & 1u) && pcg2_half_hit<0>(k, c2)) w[0] = w[0] * v[0];
+    if ((recs & 2u) && pcg2_half_hit<1>(k, c2)) w[1] = w[1] * v[PAIR_VALS / 8];
   }
   if (MISSING) {
 #pragma unroll
