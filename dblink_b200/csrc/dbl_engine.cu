@@ -309,68 +309,47 @@ __global__ void k_block_scan(int P, const int *__restrict__ ent_ptr, const int *
   }
 }
 // Tiled, block-sorted copies of the entity table, one thread per tile slot (padding slots of a block's last tile are
-// zeroed here: no memset of the whole table).  fmt 1: attribute-major tiles { int32 y[A][TE]; f64 N[TE] }
-// (k_link_generic / k_link_match / k_link_pruned); fmt 2: quad tiles (k_link_pcg2).
-__global__ void k_build_tiles(int64_t n_slots, int fmt, int A, const int *__restrict__ y, const double *__restrict__ entN,
-                              const int *__restrict__ ent_sorted, const int *__restrict__ ent_ptr,
-                              const int *__restrict__ tile_ptr, int *__restrict__ tiles, const int *__restrict__ perm, int P,
-                              int npack, int *__restrict__ qtiles, int n_str, int qtile_pk, int qtile_id16,
-                              const AttrDev *__restrict__ sc_attrs) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_slots) return;
-  const int T = (int)(i / TE), slot = (int)(i % TE);
-  if (T >= tile_ptr[P]) return;
-  int lo = 0, hi = P;  // block of tile T: last b with tile_ptr[b] <= T
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (tile_ptr[mid] <= T) lo = mid; else hi = mid;
-  }
-  const int b = lo;
-  const int j = (T - tile_ptr[b]) * TE + slot;
-  const bool real = j < ent_ptr[b + 1] - ent_ptr[b];
-  const int64_t e = real ? ent_sorted[ent_ptr[b] + j] : 0;
-  const double nn = real ? entN[e] : 0.0;
-  if (fmt == 1) {
-    int *tile = tiles + (size_t)T * tile_words(A);
-    for (int k = 0; k < A; ++k) tile[k * TE + slot] = real ? y[e * A + perm[k]] : 0;  // kernel order
-    reinterpret_cast<double *>(tile + (size_t)A * TE)[slot] = nn;
-  } else {
-    unsigned pk = 0;  // constant attributes (kernel positions 0..npack-1), one byte each
-    if (real)
-      for (int k = 0; k < npack; ++k) pk |= ((unsigned)y[e * A + perm[k]] & 0xFFu) << (8 * k);
-    const int nv = qtile_nv(A, n_str, qtile_pk != 0, qtile_id16 != 0), ng = qtile_groups(nv), qw = qtile_words(nv);
-    const int nid = qtile_id16 ? (n_str + 1) / 2 : n_str;  // words of non-constant values (packed tiles)
-    // packed tiles: value (sc_attrs == null) or slot code (AttrDev::pcode) of kernel-order attribute k
-    auto ns_val = [&](int k) -> unsigned {
-      const int yv = y[e * A + perm[k]];
-      return (unsigned)(sc_attrs ? sc_attrs[perm[k]].pcode[yv] : yv);
-    };
-    int *qt = qtiles + (size_t)T * qw * TE;
-    int v[4];
-    for (int g = 0; g < ng; ++g) {
-      for (int c = 0; c < 4; ++c) {
-        const int w = 4 * g + c;
-        int val = 0;
-        if (real) {
-          if (qtile_pk && qtile_id16) {
-            if (w < nid) {  // values 2w (low half) and 2w + 1 (high half): vocabularies of <= 65536 values
-              const int k = A - n_str + 2 * w;
-              val = (int)((ns_val(k) & 0xFFFFu) | (2 * w + 1 < n_str ? ns_val(k + 1) << 16 : 0u));
-            } else if (w == nid) {
-              val = (int)pk;
-            }
-          } else if (qtile_pk) {
-            val = (w < n_str) ? (int)ns_val(A - n_str + w) : (w == n_str ? (int)pk : 0);
-          } else {
-            val = (w < A) ? y[e * A + perm[w]] : 0;
-          }
-        }
-        v[c] = val;
-      }
-      reinterpret_cast<int4 *>(qt)[(size_t)g * TE + slot] = make_int4(v[0], v[1], v[2], v[3]);
+// zeroed here: no memset of the whole table).
+struct TileSrc {
+  int64_t n_slots;
+  int A, P;
+  const int *y, *ent_sorted, *ent_ptr, *tile_ptr, *perm;
+  const double *entN;
+  // tile T and slot of thread i, its entity's values (nullptr: padding) and N; false past the last tile
+  __device__ bool at(int64_t i, int &T, int &slot, const int *&yrow, double &N) const {
+    T = (int)(i / TE);
+    slot = (int)(i % TE);
+    if (i >= n_slots || T >= tile_ptr[P]) return false;
+    int lo = 0, hi = P;  // block of tile T: last b with tile_ptr[b] <= T
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (tile_ptr[mid] <= T) lo = mid; else hi = mid;
     }
-    reinterpret_cast<double *>(qt + (size_t)ng * 4 * TE)[slot] = nn;
+    const int j = (T - tile_ptr[lo]) * TE + slot;
+    const int64_t e = j < ent_ptr[lo + 1] - ent_ptr[lo] ? ent_sorted[ent_ptr[lo] + j] : -1;
+    yrow = e >= 0 ? y + e * A : nullptr;
+    N = e >= 0 ? entN[e] : 0.0;
+    return true;
   }
+};
+// attribute-major tiles { int32 y[A][TE]; f64 N[TE] } (k_link_generic / k_link_match / k_link_pruned)
+__global__ void k_build_tiles(TileSrc s, int *__restrict__ tiles) {
+  int T, slot;
+  const int *yrow;
+  double N;
+  if (!s.at((int64_t)blockIdx.x * blockDim.x + threadIdx.x, T, slot, yrow, N)) return;
+  int *tile = tiles + (size_t)T * tile_words(s.A);
+  for (int k = 0; k < s.A; ++k) tile[k * TE + slot] = yrow ? yrow[s.perm[k]] : 0;  // kernel order
+  reinterpret_cast<double *>(tile + (size_t)s.A * TE)[slot] = N;
+}
+// quad tiles of format f (k_link_pcg2), NS non-constant attributes
+__global__ void k_build_qtiles(TileSrc s, Pcg2Format f, int NS, const AttrDev *__restrict__ attrs,
+                               int *__restrict__ qtiles) {
+  int T, slot;
+  const int *yrow;
+  double N;
+  if (!s.at((int64_t)blockIdx.x * blockDim.x + threadIdx.x, T, slot, yrow, N)) return;
+  pcg2_store(f, s.A, NS, yrow, s.perm, attrs, qtiles + (size_t)T * f.words(s.A, NS) * TE, slot, N);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1339,8 +1318,8 @@ struct dbl_ctx {
   DevBuf<int> perm_dev;
   int perm[DBL_MAX_ATTRS] = {0};
   int n_str = 0;       // non-constant attributes
-  int pack_consts = 0; // constant attributes byte-packed into the quad tiles (0 = none)
   int hslots = 32, hshift = 27;  // common hash-table size of the non-constant attributes; hslots = 0: none
+  Pcg2Format pcg2_fmt{};         // tile format of k_link_pcg2 (pcg2_format)
   std::vector<AttrDev> h_attrs;
   DevBuf<int> tree_buf;
   TreeDev tree{};
@@ -1421,10 +1400,6 @@ struct dbl_ctx {
   DevBuf<int> iota, blk_sorted, ent_sorted, rec_key, rec_key_sorted, rec_sorted;
   DevBuf<int> ent_ptr, tile_ptr, rec_ptr, cta_ptr, cta_ptr2, cta_ptr3, tiles, qtiles;
   DevBuf<double> lane_sums;  // k_link_pcg2 scratch: pass-1 lane sums per chunk of every resident warp
-  int qtile_pk = 0;  // quad tiles carry the packed constants (PK instantiations of k_link_pcg2)
-  int qtile_id16 = 0;  // ... and 16-bit non-constant values (every non-constant vocabulary has <= 65536 values)
-  int qtile_sc = 0;    // ... and those values are slot codes (every non-constant attribute has them)
-  int sc_code_max = -1;  // largest slot code of the model's non-constant attributes; -1: some attribute has none
   bool tiles_valid[2] = {false, false};  // attribute-major / quad tiles match the current layout
   // inverted index of the block tables for the pruned PCG-I link kernel (built on demand, once per sweep): E * A ids,
   // unsigned or (inv_ids64) unsigned long long, with their candidate positions
@@ -1568,7 +1543,6 @@ static int upload_model(dbl_ctx *ctx, const dbl_model_desc *d) {
     Hmax = std::max(Hmax, d->indexes[a]->hsize);
   }
   std::vector<dbl_index> rehashed(A);
-  ctx->sc_code_max = 0;
   for (int a = 0; a < A; ++a) {
     const dbl_index *ix = d->indexes[a];
     if (hash_ok && !ix->is_const && ix->hsize != Hmax) {
@@ -1604,14 +1578,12 @@ static int upload_model(dbl_ctx *ctx, const dbl_model_desc *d) {
       CUDA_TRY(up_i(ti[3], hm));
     }
     const bool sc = !ix->pcode.empty();
-    if (!ix->is_const && !sc) ctx->sc_code_max = -1;
     if (sc) {
       CUDA_TRY(up_i(ti[4], ix->pcode));
       CUDA_TRY(up_i(ti[5], ix->sckeys));
       CUDA_TRY(up_d(t[11], ix->scvals));
       // 1/n(y) of the missing-value records, indexed by the code the tiles carry (codes no value has: 1)
       const int cmax = *std::max_element(ix->pcode.begin(), ix->pcode.end());
-      if (ctx->sc_code_max >= 0) ctx->sc_code_max = std::max(ctx->sc_code_max, cmax);
       std::vector<double> inv((size_t)cmax + 1, 1.0);
       for (int v = 0; v < ix->V; ++v) inv[ix->pcode[v]] = ix->invnorm[v];
       CUDA_TRY(up_d(t[12], inv));
@@ -1632,10 +1604,6 @@ static int upload_model(dbl_ctx *ctx, const dbl_model_desc *d) {
     int k = 0;
     for (int a = 0; a < A; ++a) if (ctx->h_attrs[a].is_const) ctx->perm[k++] = a;
     ctx->n_str = A - k;
-    // byte-packed copy of the constant attributes in the tiles (k_link_pcg2): 1..4 of them, every vocabulary <= 255
-    ctx->pack_consts = (k >= 1 && k <= 4) ? k : 0;
-    for (int q = 0; q < k; ++q) if (ctx->h_attrs[ctx->perm[q]].V > 255) ctx->pack_consts = 0;
-    if (getenv("DBL_NO_PACK")) ctx->pack_consts = 0;  // tests: the unpacked kernels on a packable model
     for (int a = 0; a < A; ++a) if (!ctx->h_attrs[a].is_const) ctx->perm[k++] = a;
     ctx->hslots = hash_ok ? Hmax : 0;
     ctx->hshift = 32;
@@ -1643,6 +1611,7 @@ static int upload_model(dbl_ctx *ctx, const dbl_model_desc *d) {
     CUDA_TRY(ctx->perm_dev.alloc(A));
     CUDA_TRY(cudaMemcpy(ctx->perm_dev.p, ctx->perm, sizeof(int) * A, cudaMemcpyHostToDevice));
   }
+  ctx->pcg2_fmt = pcg2_format(d, ctx->hslots);
   return upload_tree(ctx, d->tree);
 }
 
@@ -1770,25 +1739,12 @@ static int alloc_blocks(dbl_ctx *ctx) {
   CUDA_TRY(ctx->lpt_dscratch.alloc((size_t)P + MAX_WORLD));
   const size_t max_tiles = (size_t)(ctx->E / TE) + (size_t)P + 1;
   CUDA_TRY(ctx->tiles.alloc(max_tiles * tile_words(ctx->A)));
-  ctx->qtile_pk = (ctx->pack_consts && ctx->hslots == 32) ? 1 : 0;
-  // slot codes in the packed tiles when every non-constant attribute has them
-  ctx->qtile_sc = (ctx->qtile_pk && ctx->n_str > 0 && ctx->sc_code_max >= 0) ? 1 : 0;
-  if (getenv("DBL_NO_SC")) ctx->qtile_sc = 0;  // tests: the per-record hash multipliers on a model that colours
-  ctx->qtile_id16 = ctx->qtile_pk;
-  for (int a = 0; a < ctx->A; ++a)
-    if (!ctx->h_attrs[a].is_const && ctx->h_attrs[a].V > 65536) ctx->qtile_id16 = 0;
-  if (ctx->qtile_sc && ctx->sc_code_max > 65535) ctx->qtile_id16 = 0;  // the codes may exceed the value ids
-  if (getenv("DBL_NO_ID16")) ctx->qtile_id16 = 0;  // tests: the 32-bit packed tiles on a model that fits 16 bits
-  {
-    // work item and grid of the persistent PCG-II kernel for this model shape (see pcg2_rpw)
-    const int hc = ctx->hslots == 32 ? 32 : 0;
-    ctx->pcg2_recs = LINK_WARPS * pcg2_rpw(hc, ctx->n_str);
-    ctx->pcg2_grid = ctx->sm_count * pcg2_ctas_per_sm(hc, ctx->n_str);
-    const size_t need = (size_t)ctx->pcg2_grid * ctx->pcg2_recs * 1024;
-    if (ctx->lane_sums.n < need) CUDA_TRY(ctx->lane_sums.alloc(need));
-  }
-  // sized for 32-bit values: the 16-bit format never needs more
-  CUDA_TRY(ctx->qtiles.alloc(max_tiles * qtile_words(qtile_nv(ctx->A, ctx->n_str, ctx->qtile_pk != 0)) * TE));
+  // work item and grid of the persistent PCG-II kernel for this model shape (see Pcg2Format::rpw)
+  ctx->pcg2_recs = LINK_WARPS * ctx->pcg2_fmt.rpw(ctx->n_str);
+  ctx->pcg2_grid = ctx->sm_count * ctx->pcg2_fmt.ctas_per_sm(ctx->n_str);
+  const size_t need = (size_t)ctx->pcg2_grid * ctx->pcg2_recs * 1024;
+  if (ctx->lane_sums.n < need) CUDA_TRY(ctx->lane_sums.alloc(need));
+  CUDA_TRY(ctx->qtiles.alloc(max_tiles * ctx->pcg2_fmt.words(ctx->A, ctx->n_str) * TE));
   ctx->max_ctas = (int)((ctx->R + LINK_WARPS - 1) / LINK_WARPS) + P;
   return alloc_control(ctx);
 }
@@ -1921,11 +1877,12 @@ static int relayout(dbl_ctx *ctx, bool end_of_sweep = false) {
 static int ensure_tiles(dbl_ctx *ctx, int fmt) {
   if (ctx->tiles_valid[fmt - 1]) return DBL_OK;
   const int64_t n_slots = (int64_t)((size_t)(ctx->E / TE) + (size_t)ctx->P + 1) * TE;
-  k_build_tiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(n_slots, fmt, ctx->A, ctx->y.p, ctx->entN.p,
-                                                                 ctx->ent_sorted.p, ctx->ent_ptr.p, ctx->tile_ptr.p,
-                                                                 ctx->tiles.p, ctx->perm_dev.p, ctx->P, ctx->pack_consts,
-                                                                 ctx->qtiles.p, ctx->n_str, ctx->qtile_pk,
-                                                                 ctx->qtile_id16, ctx->qtile_sc ? ctx->attrs.p : nullptr);
+  const TileSrc s{n_slots, ctx->A, ctx->P, ctx->y.p, ctx->ent_sorted.p, ctx->ent_ptr.p, ctx->tile_ptr.p,
+                  ctx->perm_dev.p, ctx->entN.p};
+  if (fmt == 1) k_build_tiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(s, ctx->tiles.p);
+  else
+    k_build_qtiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(s, ctx->pcg2_fmt, ctx->n_str, ctx->attrs.p,
+                                                                    ctx->qtiles.p);
   ctx->launches += 1;
   ctx->tiles_valid[fmt - 1] = true;
   CUDA_TRY(cudaGetLastError());
@@ -2332,7 +2289,7 @@ extern "C" int dbl_chains_download(dbl_ctx *ctx, uint8_t *z, int32_t *link, int3
 // ---------------------------------------------------------------------------------------------------
 // link kernel dispatch
 // ---------------------------------------------------------------------------------------------------
-#define DBL_DECL(N) int dbl_launch_pcg2_a##N(int ns, int grid, cudaStream_t stream, const LinkParams &lp, size_t *cfg);
+#define DBL_DECL(N) Pcg2Kernel dbl_pcg2_kernel_a##N(int ns, Pcg2Format f);
 DBL_DECL(1) DBL_DECL(2) DBL_DECL(3) DBL_DECL(4) DBL_DECL(5) DBL_DECL(6) DBL_DECL(7) DBL_DECL(8)
 DBL_DECL(9) DBL_DECL(10) DBL_DECL(11) DBL_DECL(12) DBL_DECL(13) DBL_DECL(14) DBL_DECL(15) DBL_DECL(16)
 #undef DBL_DECL
@@ -2399,17 +2356,18 @@ static int ensure_inverted_index(dbl_ctx *ctx) {
 
 static bool pcg2_kernel_fits(const dbl_ctx *ctx) {
   return ctx->hslots > 0 && ctx->A <= LINK_MAX_UNROLL_A &&
-         pcg2_smem_bytes(ctx->A, ctx->n_str, ctx->hslots, ctx->qtile_pk != 0, ctx->qtile_id16 != 0,
-                         ctx->qtile_sc != 0) <= 100 * 1024;
+         pcg2_smem_bytes(ctx->pcg2_fmt, ctx->A, ctx->n_str, ctx->hslots) <= 100 * 1024;
 }
-static int dispatch_pcg2(dbl_ctx *ctx, int grid, const LinkParams &lp) {
-  int rc = -1;
+static int dispatch_pcg2(dbl_ctx *ctx, const LinkParams *lp, int grid = 0) {
+  Pcg2Kernel k = nullptr;
   switch (ctx->A) {
-#define DBL_CASE(N) case N: rc = dbl_launch_pcg2_a##N(ctx->n_str, grid, ctx->stream, lp, &ctx->pcg2_smem_cfg); break;
+#define DBL_CASE(N) case N: k = dbl_pcg2_kernel_a##N(ctx->n_str, ctx->pcg2_fmt); break;
     DBL_CASE(1) DBL_CASE(2) DBL_CASE(3) DBL_CASE(4) DBL_CASE(5) DBL_CASE(6) DBL_CASE(7) DBL_CASE(8)
     DBL_CASE(9) DBL_CASE(10) DBL_CASE(11) DBL_CASE(12) DBL_CASE(13) DBL_CASE(14) DBL_CASE(15) DBL_CASE(16)
 #undef DBL_CASE
   }
+  const int rc = pcg2_launch(k, pcg2_smem_bytes(ctx->pcg2_fmt, ctx->A, ctx->n_str, ctx->hslots), lp, grid,
+                             ctx->stream, &ctx->pcg2_smem_cfg);
   if (rc != 0) { ctx->set_error(std::string("k_link_pcg2 launch: ") + cudaGetErrorString((cudaError_t)rc)); return DBL_ERR_CUDA; }
   return DBL_OK;
 }
@@ -2433,8 +2391,7 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
   lp.theta = ctx->theta(); lp.ent_ptr = ctx->ent_ptr.p; lp.tile_ptr = ctx->tile_ptr.p; lp.rec_ptr = ctx->rec_ptr.p;
   lp.cta_ptr = ctx->cta_ptr.p; lp.ent_sorted = ctx->ent_sorted.p; lp.rec_sorted = ctx->rec_sorted.p;
   lp.tiles = ctx->tiles.p; lp.newlink = ctx->newlink.p;
-  lp.qtiles = ctx->qtiles.p; lp.qtile_pk = ctx->qtile_pk; lp.qtile_id16 = ctx->qtile_id16;
-  lp.qtile_sc = ctx->qtile_sc;
+  lp.qtiles = ctx->qtiles.p;
   lp.work = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_WORK);
   lp.lane_sums = ctx->lane_sums.p;
   lp.status = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_STATUS);
@@ -2458,7 +2415,7 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
     int rc = ensure_tiles(ctx, 2);
     if (rc) return rc;
     lp.cta_ptr = ctx->cta_ptr3.p;  // work items of PCG2_RECS records
-    return dispatch_pcg2(ctx, std::min(ctx->max_ctas, ctx->pcg2_grid), lp);
+    return dispatch_pcg2(ctx, &lp, std::min(ctx->max_ctas, ctx->pcg2_grid));
   }
   {
     int rc = ensure_tiles(ctx, 1);  // every other link kernel reads the attribute-major tiles
@@ -2835,7 +2792,7 @@ extern "C" int dbl_set_rebalance(dbl_ctx *ctx, int32_t period, double threshold)
 static int preload_kernels(dbl_ctx *ctx) {
   cudaFuncAttributes fa;
 #define DBL_LOAD(k) CUDA_TRY(cudaFuncGetAttributes(&fa, k))
-  DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_tiles); DBL_LOAD(k_values<VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
+  DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_tiles); DBL_LOAD(k_build_qtiles); DBL_LOAD(k_values<VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
   DBL_LOAD(k_reduce_local); DBL_LOAD(k_finish); DBL_LOAD(k_move_ent); DBL_LOAD(k_move_rec); DBL_LOAD(k_publish_barrier);
   DBL_LOAD(k_unpack_ent_p2p); DBL_LOAD(k_unpack_rec_p2p); DBL_LOAD(k_reduce_peers); DBL_LOAD(k_lpt);
   DBL_LOAD(k_link_generic); DBL_LOAD(k_link_match); DBL_LOAD(k_link_pruned); DBL_LOAD(k_state_hash);
@@ -2843,11 +2800,7 @@ static int preload_kernels(dbl_ctx *ctx) {
   DBL_LOAD(k_inv_ids<unsigned>); DBL_LOAD(k_inv_ids<unsigned long long>); DBL_LOAD(k_inv_value_ptr32);
 #undef DBL_LOAD
   if (pcg2_kernel_fits(ctx)) {
-    LinkParams lp;
-    memset(&lp, 0, sizeof(lp));
-    lp.hslots = ctx->hslots; lp.qtile_pk = ctx->qtile_pk; lp.qtile_id16 = ctx->qtile_id16;
-    lp.qtile_sc = ctx->qtile_sc;
-    int rc = dispatch_pcg2(ctx, 0, lp);  // grid 0 = load only
+    int rc = dispatch_pcg2(ctx, nullptr);
     if (rc) return rc;
   }
   int rc = build_links_csr(ctx);
@@ -3158,17 +3111,11 @@ extern "C" int dbl_state_hash(dbl_ctx *ctx, uint64_t *hash_out) {
 }
 
 // which link kernel a sweep with this sampler launches: 0 k_link_generic, 1 k_link_match, 2 k_link_pruned,
-// 3 k_link_pcg2 (+4 when the constants are byte-packed, +8 when the hash tables have the compile-time 32 slots) and
-// its tile format, by the rules Pcg2Launch and k_link_pcg2 use (+16 16-bit ids, +32 slot codes, +64 paired key
-// tables, +128 two records per warp)
+// 3 k_link_pcg2 plus the bits of the model's tile format (Pcg2Format::bits, decided by pcg2_format at model upload)
 extern "C" int dbl_link_kernel(const dbl_ctx *ctx, int sampler) {
   if (!ctx || sampler < 0 || sampler > 3) return DBL_ERR_INVALID;
   const LinkKernel kernel = link_kernel(ctx, sampler);
-  if (kernel != LINK_PCG2) return kernel;
-  const int hc = ctx->hslots == 32 ? 32 : 0;
-  const bool id16 = ctx->qtile_id16 != 0, sc = ctx->qtile_sc != 0;
-  return kernel + (ctx->qtile_pk ? 4 : 0) + (hc == 32 ? 8 : 0) + (id16 ? 16 : 0) + (sc ? 32 : 0) +
-         (pcg2_paired(hc, ctx->n_str, id16, sc) ? 64 : 0) + (pcg2_rpw(hc, ctx->n_str) == 2 ? 128 : 0);
+  return kernel == LINK_PCG2 ? LINK_PCG2 + ctx->pcg2_fmt.bits(ctx->n_str) : kernel;
 }
 
 extern "C" int dbl_set_link_mode(dbl_ctx *ctx, int mode) {

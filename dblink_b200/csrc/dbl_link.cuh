@@ -27,18 +27,6 @@ constexpr unsigned FULL = 0xffffffffu;
 
 // int32 words per tile: A value rows (attribute-major), then the f64 row N(e)
 __host__ __device__ inline size_t tile_words(int A) { return (size_t)A * TE + 2 * TE; }
-// "Quad tiles" (k_link_pcg2): the words a lane needs about ONE candidate sit in groups of four, group-major
-// ([group][slot][4] int32), so that a warp fetches a group with one conflict-free 128-bit load per lane.  Words of an
-// entity: nv values (packed kernels: the NS non-constant values then the byte-packed constants; else all A values in
-// kernel order) padded to a multiple of four; the f64 row N(e) follows the groups (8 contiguous bytes per lane: a
-// 64-bit load of a word pair inside a 16-byte group would cost twice the wavefronts).  id16 (packed kernels whose
-// non-constant vocabularies all have <= 65536 values): the NS values are 16-bit, two per word (value 2i in the low
-// half of word i), so A = 10 with 6 non-constant attributes needs one group instead of two.
-__host__ __device__ constexpr int qtile_nv(int A, int NS, bool packed, bool id16 = false) {
-  return packed ? (id16 ? (NS + 1) / 2 : NS) + 1 : A;
-}
-__host__ __device__ constexpr int qtile_groups(int nv) { return (nv + 3) / 4; }
-__host__ __device__ constexpr int qtile_words(int nv) { return qtile_groups(nv) * 4 + 2; }  // per entity
 
 struct AttrDev {
   int V, is_const, kmax, hsize;
@@ -102,9 +90,6 @@ struct LinkParams {
   const int *ent_ptr, *tile_ptr, *rec_ptr, *cta_ptr, *ent_sorted, *rec_sorted;
   const int *tiles;
   const int *qtiles;         // quad tiles (k_link_pcg2)
-  int qtile_pk;              // quad tiles hold the non-constant values + the byte-packed constants (else all A values)
-  int qtile_id16;            // ... and those non-constant values are 16-bit, two per word (qtile_nv)
-  int qtile_sc;              // ... and they are slot codes (AttrDev::pcode), not value ids
   unsigned long long *work;  // k_link_pcg2: next group of records to take (persistent CTAs); zeroed before the launch
   double *lane_sums;         // k_link_pcg2: scratch, [CTA][consumer warp][32 chunks][32 lanes] pass-1 lane sums
   int *newlink;

@@ -8,6 +8,6 @@
 #define DBL_CAT2(a, b) a##b
 #define DBL_CAT(a, b) DBL_CAT2(a, b)
 
-int DBL_CAT(dbl_launch_pcg2_a, DBL_INST_A)(int ns, int grid, cudaStream_t stream, const LinkParams &lp, size_t *smem_configured) {
-  return Pcg2Launch<DBL_INST_A, DBL_INST_A>::go(ns, grid, stream, lp, smem_configured);
+Pcg2Kernel DBL_CAT(dbl_pcg2_kernel_a, DBL_INST_A)(int ns, Pcg2Format f) {
+  return pcg2_kernel<DBL_INST_A, DBL_INST_A>(ns, f);
 }

@@ -3,8 +3,8 @@
 // when the hash tables have 32 slots (else the size is a run-time parameter); PK = the constant attributes arrive
 // byte-packed; ID16 (PK only) = the non-constant values arrive as 16-bit halves, two per word (every non-constant
 // value, or SC code, is < 65536); SC (PK only) = those values are slot codes (AttrDev::pcode, dbl_index::
-// build_slot_codes) whose low five bits are the value's slot in every record's table.  ID16 and SC are tile formats,
-// not kernel shapes: dbl_link_kernel reports them in bits of their own, beside pcg2_paired and pcg2_rpw.
+// build_slot_codes) whose low five bits are the value's slot in every record's table.  HC, PK, ID16 and SC are one
+// Pcg2Format, which pcg2_format decides once per model; the tiles, the launch and dbl_link_kernel's report follow it.
 //
 //  * persistent CTAs: the grid is a few CTAs per SM; each takes the next group of LINK_WARPS records of some block
 //    from a device-side counter until none is left (no empty CTAs on a shard that owns 1/8 of the records, no tail);
@@ -30,17 +30,79 @@
 //    in registers for the whole work item (fetching them per step and attribute cost 15 % of the kernel at 1 M);
 //  * lane l scores candidate 32*step + l; lane sums / chunk totals / draw as in DESIGN.md section 4.
 #pragma once
+#include <algorithm>
+#include <cstdlib>
 #include <type_traits>
 
 #include "dbl_link.cuh"
+
+// The tile format {HC, PK, ID16, SC} of k_link_pcg2 and what follows from it (A attributes, NS non-constant)
+struct Pcg2Format {
+  int hc;              // 32: the model's hash tables have 32 slots, a compile-time size; 0: p.hslots
+  __host__ __device__ static constexpr int hc_of(int hslots) { return hslots == 32 ? 32 : 0; }
+  bool pk, id16, sc;   // byte-packed constants; 16-bit non-constant values; slot codes in place of value ids
+  // "Quad tiles": the words a lane needs about ONE candidate sit in groups of four, group-major ([group][slot][4]
+  // int32), so that a warp fetches a group with one conflict-free 128-bit load per lane.  Words of an entity: nv
+  // values (pk: the NS non-constant values then the byte-packed constants; else all A values in kernel order) padded
+  // to a multiple of four; the f64 row N(e) follows the groups (8 contiguous bytes per lane: a 64-bit load of a word
+  // pair inside a 16-byte group would cost twice the wavefronts).  id16: the NS values are 16-bit, two per word
+  // (value 2i in the low half of word i), so A = 10 with 6 non-constant attributes needs one group instead of two.
+  // pcg2_store writes them, pcg2_load reads them.
+  __host__ __device__ constexpr int nv(int A, int NS) const { return pk ? (id16 ? (NS + 1) / 2 : NS) + 1 : A; }
+  __host__ __device__ constexpr int groups(int A, int NS) const { return (nv(A, NS) + 3) / 4; }
+  __host__ __device__ constexpr int words(int A, int NS) const { return groups(A, NS) * 4 + 2; }  // per entity
+  // Records per consumer warp.  With 2, a lane fetches its candidate once and scores it for both records: half the
+  // tile loads and half the tile traffic through shared memory per (record, candidate) pair, two independent
+  // dependency chains per warp; the price is registers (96 instead of 72: 2 CTAs per SM instead of 3) and twice the
+  // per-record tables in shared memory -- so it is used for the 32-slot instantiations with up to 8 non-constant
+  // attributes (faster at A = 10, NS = 6; three records per warp spill).  Every shape has LINK_WARPS consumer warps:
+  // ONE CTA of 16 consumer warps per SM was slower than two CTAs of 8 (one ring per SM: every warp waits for the
+  // slowest at each stage).
+  __host__ __device__ constexpr int rpw(int NS) const { return (hc == 32 && NS >= 1 && NS <= 8) ? 2 : 1; }
+  // 3 CTAs per SM (72 registers) only where one record per warp fits them: few non-constant attributes
+  __host__ __device__ constexpr int ctas_per_sm(int NS) const { return (rpw(NS) >= 2 || NS > 6) ? 2 : 3; }
+  // the two records of a warp share paired key tables (PAIR_KEYS) when every code fits 16 bits
+  __host__ __device__ constexpr bool paired(int NS) const { return id16 && sc && rpw(NS) == 2; }
+  // as dbl_link_kernel reports it: +4 pk, +8 hc = 32, +16 id16, +32 sc, +64 paired, +128 two records per warp
+  constexpr int bits(int NS) const {
+    return (pk ? 4 : 0) + (hc == 32 ? 8 : 0) + (id16 ? 16 : 0) + (sc ? 32 : 0) + (paired(NS) ? 64 : 0) +
+           (rpw(NS) == 2 ? 128 : 0);
+  }
+};
+
+// The tile format of a model, the one place its rules live.  hslots: the model's common hash-table size (0: none).
+// DBL_NO_PACK, DBL_NO_SC and DBL_NO_ID16 (tests) withhold a format from a model that would get it.
+inline Pcg2Format pcg2_format(const dbl_model_desc *d, int hslots) {
+  int nc = 0, code_max = 0;
+  bool const_bytes = true, ids16 = true, codes = true;
+  for (int a = 0; a < d->num_attrs; ++a) {
+    const dbl_index &ix = *d->indexes[a];
+    if (ix.is_const) {
+      ++nc;
+      const_bytes = const_bytes && ix.V <= 255;
+      continue;
+    }
+    ids16 = ids16 && ix.V <= 65536;
+    codes = codes && !ix.pcode.empty();
+    if (codes) code_max = std::max(code_max, *std::max_element(ix.pcode.begin(), ix.pcode.end()));
+  }
+  Pcg2Format f{Pcg2Format::hc_of(hslots), false, false, false};
+  // byte-packed constants: 1..4 of them, every vocabulary <= 255, 32-slot tables
+  f.pk = nc >= 1 && nc <= 4 && const_bytes && f.hc == 32 && !getenv("DBL_NO_PACK");
+  // slot codes: packed tiles, and every non-constant attribute has them
+  f.sc = f.pk && nc < d->num_attrs && codes && !getenv("DBL_NO_SC");
+  // 16-bit values: packed tiles, every non-constant vocabulary fits, and so does every code (codes may exceed the ids)
+  f.id16 = f.pk && ids16 && !(f.sc && code_max > 65535) && !getenv("DBL_NO_ID16");
+  return f;
+}
 
 // Per (record, non-constant attribute): H key words then H f64 values, H = p.hslots (a power of two >= 32, the same
 // for every attribute of the model; 32 = one key per bank = conflict-free probes).
 __device__ __host__ __forceinline__ int pcg2_tab_bytes(int H) { return H * 12; }
 
-// Paired tables (16-bit slot codes, two records per warp: pcg2_paired): per (warp, non-constant attribute) 32 key
-// words, word s = the key of record 0 at slot s in the low half and record 1's in the high half (one word per bank:
-// one conflict-free probe serves both records), then record 0's 32 f64 values, then record 1's, PAIR_VALS bytes
+// Paired tables (16-bit slot codes, two records per warp: Pcg2Format::paired): per (warp, non-constant attribute) 32
+// key words, word s = the key of record 0 at slot s in the low half and record 1's in the high half (one word per
+// bank: one conflict-free probe serves both records), then record 0's 32 f64 values, then record 1's, PAIR_VALS bytes
 // further: both value loads of a probe share one address.  An empty half at slot s holds s ^ 1, which no code with
 // code & 31 == s equals.
 constexpr int PAIR_KEYS = 32 * 4, PAIR_VALS = 32 * 8, PAIR_ATTR_BYTES = PAIR_KEYS + 2 * PAIR_VALS;
@@ -71,6 +133,32 @@ __device__ __forceinline__ unsigned pcg2_const_offset(unsigned ypack, unsigned x
   return (eq * 0x00204081u) >> 25;
 }
 
+// One entity into slot `slot` of a quad tile of format f (pcg2_load reads it back).  y: the entity's values by
+// attribute id, nullptr for a padding slot (all zero); perm: kernel order.  Packed tiles: the non-constant values
+// (f.sc: their slot codes, AttrDev::pcode) at 32 or (f.id16) 16 bits, then the constants, one byte each.
+__device__ __forceinline__ void pcg2_store(Pcg2Format f, int A, int NS, const int *y, const int *perm,
+                                           const AttrDev *attrs, int *tile, int slot, double N) {
+  const int ng = f.groups(A, NS);
+  const int nid = f.id16 ? (NS + 1) / 2 : NS;  // words of non-constant values (packed tiles)
+  auto ns_val = [&](int k) -> unsigned {       // value or slot code of kernel-order attribute k
+    const int yv = y[perm[k]];
+    return (unsigned)(f.sc ? attrs[perm[k]].pcode[yv] : yv);
+  };
+  for (int g = 0; g < ng; ++g) {
+    unsigned v[4] = {0u, 0u, 0u, 0u};
+    for (int c = 0, w = 4 * g; c < 4 && y; ++c, ++w) {
+      if (!f.pk) v[c] = w < A ? (unsigned)y[perm[w]] : 0u;
+      else if (w < nid && f.id16)  // values 2w (low half) and 2w + 1 (high half)
+        v[c] = (ns_val(A - NS + 2 * w) & 0xFFFFu) | (2 * w + 1 < NS ? ns_val(A - NS + 2 * w + 1) << 16 : 0u);
+      else if (w < nid) v[c] = ns_val(A - NS + w);
+      else if (w == nid)
+        for (int k = 0; k < A - NS; ++k) v[c] |= ((unsigned)y[perm[k]] & 0xFFu) << (8 * k);
+    }
+    reinterpret_cast<int4 *>(tile)[(size_t)g * TE + slot] = make_int4(v[0], v[1], v[2], v[3]);
+  }
+  reinterpret_cast<double *>(tile + (size_t)ng * 4 * TE)[slot] = N;
+}
+
 // one candidate out of a quad tile: values in kernel order (PK: only the non-constant ones + the packed word), N
 template <int A, int NS, bool PK>
 struct Pcg2Cand {
@@ -82,7 +170,7 @@ struct Pcg2Cand {
 template <int A, int NS, bool PK, bool ID16>
 __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *tile, int slot) {
   static_assert(PK || !ID16, "16-bit values only in the packed tiles");
-  constexpr int NV = qtile_nv(A, NS, PK, ID16), NG = qtile_groups(NV);
+  constexpr int NG = Pcg2Format{0, PK, ID16, false}.groups(A, NS);  // the layout depends on PK and ID16 only
   int v[NG * 4];
   const int4 *q = reinterpret_cast<const int4 *>(tile);
 #pragma unroll
@@ -173,7 +261,7 @@ __device__ __forceinline__ bool pcg2_half_hit(unsigned k, unsigned c2) {
   return hit != 0;
 }
 
-// Paired tables (pcg2_paired): the weights of one candidate for the warp's records whose bit is set in `recs`, in w[0]
+// Paired tables (Pcg2Format::paired): the weights of one candidate for the warp's records whose bit is set in `recs`, in w[0]
 // and w[1]; each is the product pcg2_weight forms, factor for factor in the same order.  Per (candidate, attribute):
 // one PRMT spreads the 16-bit code over both halves of a word, c2 = {code, code}; ONE key load at slot code & 31
 // serves both records, whose hits are the halves of k ^ c2 that are zero (pcg2_half_hit); one value address serves
@@ -210,35 +298,21 @@ __device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc
   }
 }
 
-// Records per consumer warp.  With 2, a lane fetches its candidate once and scores it for both records: half the
-// tile loads and half the tile traffic through shared memory per (record, candidate) pair, two independent
-// dependency chains per warp; the price is registers (96 instead of 72: 2 CTAs per SM instead of 3) and twice the
-// per-record tables in shared memory -- so it is used for the 32-slot instantiations with up to 8 non-constant
-// attributes (faster at A = 10, NS = 6; three records per warp spill).  Every shape has LINK_WARPS consumer warps:
-// ONE CTA of 16 consumer warps per SM was slower than two CTAs of 8 (one ring per SM: every warp waits for the
-// slowest at each stage).
-__host__ __device__ constexpr int pcg2_rpw(int HC, int NS) { return (HC == 32 && NS >= 1 && NS <= 8) ? 2 : 1; }
-// 3 CTAs per SM (72 registers) only where one record per warp fits them: few non-constant attributes
-__host__ __device__ constexpr int pcg2_ctas_per_sm(int HC, int NS) { return (pcg2_rpw(HC, NS) >= 2 || NS > 6) ? 2 : 3; }
-// the two records of a warp share paired key tables (PAIR_KEYS) when every code fits 16 bits
-__host__ __device__ constexpr bool pcg2_paired(int HC, int NS, bool ID16, bool SC) {
-  return ID16 && SC && pcg2_rpw(HC, NS) == 2;
-}
 // bytes of one consumer warp's hash tables (H = the table size of the model)
-__host__ __device__ inline int pcg2_warp_tab_bytes(int H, int NS, bool paired) {
-  return paired ? NS * PAIR_ATTR_BYTES : pcg2_rpw(H == 32 ? 32 : 0, NS) * (NS > 0 ? NS : 1) * pcg2_tab_bytes(H);
+__host__ __device__ inline int pcg2_warp_tab_bytes(Pcg2Format f, int NS, int H) {
+  return f.paired(NS) ? NS * PAIR_ATTR_BYTES : f.rpw(NS) * (NS > 0 ? NS : 1) * pcg2_tab_bytes(H);
 }
 
 template <int A, int NS, int HC, bool PK, bool ID16, bool SC>
-__global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS)) k_link_pcg2(LinkParams p) {
+__global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16, SC}.ctas_per_sm(NS)) k_link_pcg2(LinkParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ int s_cta;
   if (sweep_dead(p.ctl)) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int NV = qtile_nv(A, NS, PK, ID16);
-  constexpr int TW = qtile_words(NV) * TE;
+  constexpr Pcg2Format FMT{HC, PK, ID16, SC};
+  constexpr int TW = FMT.words(A, NS) * TE;
   constexpr int NC = A - NS;
-  constexpr int RPW = pcg2_rpw(HC, NS);
+  constexpr int RPW = FMT.rpw(NS);
   constexpr int WARPS = LINK_WARPS;           // consumer warps; warp WARPS is the producer
   constexpr int PCG2_RECS = WARPS * RPW;      // records per work item (= per "CTA" of cta_ptr)
   TileRing rg;
@@ -247,9 +321,11 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
   rg.empty = rg.full + LINK_STAGES;
   rg.tw = TW;
   static_assert(2 * LINK_STAGES * 8 <= 128, "barrier area");
-  constexpr bool PAIR = pcg2_paired(HC, NS, ID16, SC);
+  constexpr bool PAIR = FMT.paired(NS);
   const int tabrec = (NS > 0 ? NS : 1) * pcg2_tab_bytes(HC ? HC : p.hslots);  // bytes of one record's hash tables
-  const int wtab = pcg2_warp_tab_bytes(HC ? HC : p.hslots, NS, PAIR);         // ... of one warp's
+  // ... of one warp's.  HC = 0: the records per warp of this stride come from p.hslots at run time (1 in every launch);
+  // a compile-time 1 moves ptxas's spills and cost 1.2 % at A = 11, NS = 5 (H100 SXM, 700 W)
+  const int wtab = pcg2_warp_tab_bytes(HC ? FMT : Pcg2Format{Pcg2Format::hc_of(p.hslots)}, NS, HC ? HC : p.hslots);
   char *tab0 = reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 + (size_t)warp * wtab;
   // PK: products of the matching constant attributes, by match mask, 16 entries per record
   double *ctab0 = reinterpret_cast<double *>(reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 +
@@ -448,52 +524,43 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, pcg2_ctas_per_sm(HC, NS
   }
 }
 
-inline size_t pcg2_smem_bytes(int A, int NS, int H, bool PK, bool id16, bool sc) {
-  const int HC = H == 32 ? 32 : 0;
-  const size_t recs = (size_t)LINK_WARPS * pcg2_rpw(HC, NS);
-  return (size_t)LINK_STAGES * qtile_words(qtile_nv(A, NS, PK, id16)) * TE * 4 + 128 +
-         (size_t)LINK_WARPS * pcg2_warp_tab_bytes(H, NS, pcg2_paired(HC, NS, id16, sc)) + recs * 16 * sizeof(double);
+// dynamic shared memory of one CTA (H = the table size of the model)
+inline size_t pcg2_smem_bytes(Pcg2Format f, int A, int NS, int H) {
+  return (size_t)LINK_STAGES * f.words(A, NS) * TE * 4 + 128 + (size_t)LINK_WARPS * pcg2_warp_tab_bytes(f, NS, H) +
+         (size_t)LINK_WARPS * f.rpw(NS) * 16 * sizeof(double);
 }
 
-// launch k_link_pcg2<A, NS, HC> for a runtime NS in [0, A]; HC = 32 (compile-time table size) when the model's
-// tables have 32 slots, else 0 (size read from the parameters); returns cudaError_t as int
-template <int A, int NS, int HC, bool PK, bool ID16, bool SC = false>
-int pcg2_launch_one(int grid, cudaStream_t stream, const LinkParams &lp, size_t *configured) {
-  const size_t smem = pcg2_smem_bytes(A, NS, lp.hslots, PK, ID16, SC);
+// k_link_pcg2<A, NS, ...> of format f for a runtime NS in [0, A] (nullptr: none); the `if constexpr` guards only keep
+// out the formats pcg2_format never gives this shape (packed constants need 1..4 of them, slot codes NS >= 1)
+using Pcg2Kernel = void (*)(LinkParams);
+template <int A, int NS>
+Pcg2Kernel pcg2_kernel(int ns, Pcg2Format f) {
+  if (ns != NS) {
+    if constexpr (NS > 0) return pcg2_kernel<A, NS - 1>(ns, f);
+    return nullptr;
+  }
+  if constexpr (A - NS >= 1 && A - NS <= 4) {
+    if constexpr (NS >= 1) {
+      if (f.sc) return f.id16 ? k_link_pcg2<A, NS, 32, true, true, true> : k_link_pcg2<A, NS, 32, true, false, true>;
+    }
+    if (f.pk) return f.id16 ? k_link_pcg2<A, NS, 32, true, true, false> : k_link_pcg2<A, NS, 32, true, false, false>;
+  }
+  return f.hc ? k_link_pcg2<A, NS, 32, false, false, false> : k_link_pcg2<A, NS, 0, false, false, false>;
+}
+
+// launch kernel k on `grid` CTAs with `smem` bytes of dynamic shared memory; lp == nullptr: load the kernel without
+// running it (see preload_kernels in dbl_engine.cu); returns cudaError_t as int
+inline int pcg2_launch(Pcg2Kernel k, size_t smem, const LinkParams *lp, int grid, cudaStream_t stream,
+                       size_t *configured) {
+  if (!k) return (int)cudaErrorInvalidValue;
   // the opt-in is per device: the cache belongs to the context (one model shape = one instantiation per context)
   if (*configured < smem) {
-    cudaError_t e = cudaFuncSetAttribute(k_link_pcg2<A, NS, HC, PK, ID16, SC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     *configured = smem;
   }
-  if (grid <= 0) {  // load the kernel without running it (see preload_kernels in dbl_engine.cu)
-    cudaFuncAttributes fa;
-    return (int)cudaFuncGetAttributes(&fa, k_link_pcg2<A, NS, HC, PK, ID16, SC>);
-  }
-  k_link_pcg2<A, NS, HC, PK, ID16, SC><<<grid, (LINK_WARPS + 1) * 32, smem, stream>>>(lp);
+  cudaFuncAttributes fa;
+  if (!lp) return (int)cudaFuncGetAttributes(&fa, k);
+  k<<<grid, (LINK_WARPS + 1) * 32, smem, stream>>>(*lp);
   return (int)cudaGetLastError();
 }
-
-template <int A, int NS>
-struct Pcg2Launch {
-  static int go(int ns, int grid, cudaStream_t stream, const LinkParams &lp, size_t *cfg) {
-    if (ns == NS) {
-      // byte-packed constant attributes: 1..4 of them, every vocabulary <= 255, 32-slot tables (lp.qtile_pk);
-      // 16-bit non-constant values when every non-constant vocabulary (SC: every slot code) fits (lp.qtile_id16);
-      // slot codes when every non-constant attribute has them (lp.qtile_sc)
-      if constexpr (A - NS >= 1 && A - NS <= 4) {
-        if constexpr (NS >= 1) {
-          if (lp.qtile_pk && lp.qtile_sc)
-            return lp.qtile_id16 ? pcg2_launch_one<A, NS, 32, true, true, true>(grid, stream, lp, cfg)
-                                 : pcg2_launch_one<A, NS, 32, true, false, true>(grid, stream, lp, cfg);
-        }
-        if (lp.qtile_pk) return lp.qtile_id16 ? pcg2_launch_one<A, NS, 32, true, true>(grid, stream, lp, cfg)
-                                              : pcg2_launch_one<A, NS, 32, true, false>(grid, stream, lp, cfg);
-      }
-      return lp.hslots == 32 ? pcg2_launch_one<A, NS, 32, false, false>(grid, stream, lp, cfg)
-                             : pcg2_launch_one<A, NS, 0, false, false>(grid, stream, lp, cfg);
-    }
-    if constexpr (NS > 0) return Pcg2Launch<A, NS - 1>::go(ns, grid, stream, lp, cfg);
-    return (int)cudaErrorInvalidValue;
-  }
-};

@@ -10,7 +10,8 @@ non-constant attributes) reaches each of them: the constant at kernel position N
 records miss every string value, every constant value or exactly one string value.  One block of an odd number of
 records: the last warp has one record, and the block spans several 128-entity tiles.
 
-Each case first asserts the kernel and the tile format it gets (GibbsEngine.link_tile_format), then after every sweep
+Each case first asserts the kernel and the tile format it gets (GibbsEngine.link_tile_format), before the engine has a
+state and after, then after every sweep
 from the initial state and from a random one: the state equals the oracle's and every record's link mass equals the
 oracle's, bit for bit; on the first sweep from the random state the masses also match the literal GU conditionals.
 The four high-code cases give the last non-constant attribute a 40 000-value vocabulary, so that codes >= 2^15 (the
@@ -157,12 +158,16 @@ def test_link_shape_against_oracle(oracle, monkeypatch, case):
     beta = [1000.0] * A
     seed = 41
     eng = D.GibbsEngine(p_idx, alpha, beta, None, seed, F)
+    # the kernel and its tile format follow from the model alone: already decided before the first state
+    kernel = f"k_link_pcg2<A={A},NS={n_str},HC=32,PK={int(pk)}>"
+    assert eng.link_kernel("PCG-II") == kernel
+    assert eng.link_tile_format("PCG-II") == expected_format(n_str, fmt)
     eng.init_state(x, file)
     eng.set_partitioner(D.KDTreePartitioner(0, []).fit(eng.download_state()["y"]))
     assert eng.num_partitions == 1
     eng.set_link_mass_capture(True)
     # routing first: the case tests what it says it tests
-    assert eng.link_kernel("PCG-II") == f"k_link_pcg2<A={A},NS={n_str},HC=32,PK={int(pk)}>"
+    assert eng.link_kernel("PCG-II") == kernel
     assert eng.link_tile_format("PCG-II") == expected_format(n_str, fmt)
 
     m0 = O.Model(o_idx, alpha, beta, None, seed, F)
