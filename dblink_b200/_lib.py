@@ -12,6 +12,7 @@ OK, ERR_INVALID, ERR_CUDA, ERR_ZERO_MASS, ERR_STATE = 0, -1, -2, -3, -4
 PCG_I, PCG_II, GIBBS, GIBBS_SEQ = 0, 1, 2, 3
 SAMPLERS = {"PCG-I": PCG_I, "PCG-II": PCG_II, "Gibbs": GIBBS, "Gibbs-Sequential": GIBBS_SEQ}  # ProjectStep.scala:35
 MAX_ATTRS = 32
+SIM_CONSTANT, SIM_LEVENSHTEIN, SIM_JARO_WINKLER = 0, 1, 2  # DBL_SIM_*
 
 i32p = C.POINTER(C.c_int32)
 i64p = C.POINTER(C.c_int64)

@@ -43,16 +43,69 @@ int host_levenshtein(const char *a, int la, const char *b, int lb) {
   return prev[lb];
 }
 
-double host_similarity_from_distance(int dist, int la, int lb, double threshold, double max_sim) {
+double host_levenshtein_unit(int dist, int la, int lb) {
   const int total = la + lb;
   double unit = 1.0;                        // SimilarityFn.scala:86-90
   if (total > 0) {
     const double d = (double)dist;
     unit = 1.0 - 2.0 * d / ((double)total + d);
   }
-  const double factor = max_sim / (max_sim - threshold);  // :63
+  return unit;
+}
+
+// Jaro-Winkler counts by the greedy scan: each a[i], left to right, takes the first unmatched b[j] with
+// |i - j| <= w = max(0, max(la, lb) / 2 - 1) and a[i] == b[j] (m matches); h = matched positions k whose k-th matched
+// bytes of a and b differ; l = common prefix, at most 4.  (m, h) are symmetric in (a, b), which the GPU path relies on.
+void host_jaro_winkler_counts(const char *a, int la, const char *b, int lb, int &m, int &h, int &l) {
+  m = h = l = 0;
+  if (la == 0 || lb == 0) return;
+  const int w = std::max(0, std::max(la, lb) / 2 - 1);
+  char buf[2][256];
+  std::vector<char> big;
+  char *ma = buf[0], *mb = buf[1];
+  if (la > 256 || lb > 256) { big.resize((size_t)la + lb); ma = big.data(); mb = big.data() + la; }
+  std::memset(ma, 0, la);
+  std::memset(mb, 0, lb);
+  for (int i = 0; i < la; ++i)
+    for (int j = std::max(0, i - w); j < std::min(lb, i + w + 1); ++j)
+      if (!mb[j] && a[i] == b[j]) { ma[i] = mb[j] = 1; ++m; break; }
+  for (int i = 0, j = 0; i < la; ++i) {
+    if (!ma[i]) continue;
+    while (!mb[j]) ++j;
+    if (a[i] != b[j]) ++h;
+    ++j;
+  }
+  while (l < 4 && l < la && l < lb && a[l] == b[l]) ++l;
+}
+
+double host_jaro_winkler_unit(int m, int h, int l, int la, int lb) {
+  if (la == 0 && lb == 0) return 1.0;
+  if (m == 0) return 0.0;
+  const double jaro = ((double)m / la + (double)m / lb + ((double)m - 0.5 * h) / m) / 3.0;
+  return jaro + (0.1 * l) * (1.0 - jaro);  // this TU is compiled with -ffp-contract=off: no FMA here
+}
+
+double host_similarity_from_unit(double unit, double threshold, double max_sim) {
+  const double factor = max_sim / (max_sim - threshold);  // SimilarityFn.scala:63
   const double s = factor * (max_sim * unit - threshold);  // :66
   return s > 0.0 ? s : 0.0;
+}
+
+// unit similarity of a pair under similarity 1 (Levenshtein) or 2 (Jaro-Winkler)
+static double host_unit_similarity(int similarity, const char *a, int la, const char *b, int lb) {
+  if (similarity == DBL_SIM_JARO_WINKLER) {
+    int m, h, l;
+    host_jaro_winkler_counts(a, la, b, lb, m, h, l);
+    return host_jaro_winkler_unit(m, h, l, la, lb);
+  }
+  return host_levenshtein_unit(host_levenshtein(a, la, b, lb), la, lb);
+}
+
+// unit similarity from the integer a device kernel reports for a pair: the edit distance, or m | h << 8 | l << 16
+static double host_unit_from_code(int similarity, int code, int la, int lb) {
+  if (similarity == DBL_SIM_JARO_WINKLER)
+    return host_jaro_winkler_unit(code & 255, (code >> 8) & 255, code >> 16, la, lb);
+  return host_levenshtein_unit(code, la, lb);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -246,11 +299,12 @@ void dbl_index::build_slot_codes() {
 extern "C" int dbl_index_build(dbl_index **out, const char *const *values, const double *weights, int32_t V,
                                int similarity, double threshold, double max_sim, int32_t kmax) {
   if (!out || !values || !weights || V <= 0 || kmax < 0) return DBL_ERR_INVALID;  // "index cannot be empty" :111
-  if (similarity != 0 && !(max_sim > 0.0 && threshold >= 0.0 && threshold < max_sim))
+  if (similarity < DBL_SIM_CONSTANT || similarity > DBL_SIM_JARO_WINKLER) return DBL_ERR_INVALID;
+  if (similarity != DBL_SIM_CONSTANT && !(max_sim > 0.0 && threshold >= 0.0 && threshold < max_sim))
     return DBL_ERR_INVALID;  // SimilarityFn.scala:59-61
   auto *ix = new dbl_index();
   ix->V = V;
-  ix->is_const = (similarity == 0);
+  ix->is_const = (similarity == DBL_SIM_CONSTANT);
   ix->kmax = kmax;
   std::vector<int> order(V);
   std::iota(order.begin(), order.end(), 0);
@@ -273,16 +327,20 @@ extern "C" int dbl_index_build(dbl_index **out, const char *const *values, const
     const char *env = std::getenv("DBL_INDEX_GPU");  // "0" = host only, "1" = GPU whenever possible
     const bool want_gpu = env ? (env[0] == '1') : (V >= 2048);
     if (want_gpu) {
-      // integer distances of the candidate pairs on the GPU, identical double arithmetic afterwards
-      std::vector<int> ci, cj, cd;
-      if (gpu_levenshtein_candidates(ix->values, threshold, max_sim, ci, cj, cd)) {
-        for (int r = 0; r < V; ++r) {  // the diagonal: distance 0
-          const double e = std::exp(host_similarity_from_distance(0, len[r], len[r], threshold, max_sim));
+      // integer codes of the candidate pairs on the GPU (edit distance, or Jaro-Winkler counts), identical double
+      // arithmetic afterwards
+      std::vector<int> ci, cj, cc;
+      if (gpu_similarity_candidates(similarity, ix->values, threshold, max_sim, ci, cj, cc)) {
+        for (int r = 0; r < V; ++r) {  // the diagonal: distance 0; m = |v|, h = 0, l = min(4, |v|)
+          const int code = similarity == DBL_SIM_JARO_WINKLER ? len[r] | std::min(4, len[r]) << 16 : 0;
+          const double e =
+              std::exp(host_similarity_from_unit(host_unit_from_code(similarity, code, len[r], len[r]), threshold, max_sim));
           if (e > 1.0) rows[r].emplace_back(r, e);
         }
         for (size_t k = 0; k < ci.size(); ++k) {
           const int i = ci[k], j = cj[k];
-          const double e = std::exp(host_similarity_from_distance(cd[k], len[i], len[j], threshold, max_sim));
+          const double e =
+              std::exp(host_similarity_from_unit(host_unit_from_code(similarity, cc[k], len[i], len[j]), threshold, max_sim));
           if (e > 1.0) { rows[i].emplace_back(j, e); rows[j].emplace_back(i, e); }
         }
         for (int r = 0; r < V; ++r) std::sort(rows[r].begin(), rows[r].end());
@@ -298,8 +356,8 @@ extern "C" int dbl_index_build(dbl_index **out, const char *const *values, const
           for (int r = i; r < std::min(V, i + 16); ++r) {
             auto &row = rows[r];
             for (int c = 0; c < V; ++c) {
-              const int d = host_levenshtein(ix->values[r].data(), len[r], ix->values[c].data(), len[c]);
-              const double e = std::exp(host_similarity_from_distance(d, len[r], len[c], threshold, max_sim));
+              const double u = host_unit_similarity(similarity, ix->values[r].data(), len[r], ix->values[c].data(), len[c]);
+              const double e = std::exp(host_similarity_from_unit(u, threshold, max_sim));
               if (e > 1.0) row.emplace_back(c, e);
             }
           }
@@ -328,9 +386,10 @@ extern "C" int dbl_index_build(dbl_index **out, const char *const *values, const
 extern "C" int dbl_index_from_tables(dbl_index **out, int32_t V, int similarity, const double *probs,
                                      const int32_t *rowptr, const int32_t *col, const double *expsim, int32_t kmax) {
   if (!out || !probs || V <= 0 || kmax < 0) return DBL_ERR_INVALID;
+  if (similarity < DBL_SIM_CONSTANT || similarity > DBL_SIM_JARO_WINKLER) return DBL_ERR_INVALID;
   auto *ix = new dbl_index();
   ix->V = V;
-  ix->is_const = (similarity == 0);
+  ix->is_const = (similarity == DBL_SIM_CONSTANT);
   ix->kmax = kmax;
   ix->probs.assign(probs, probs + V);
   ix->rowptr.assign(V + 1, 0);
@@ -377,9 +436,10 @@ extern "C" double dbl_index_exp_sim(const dbl_index *ix, int32_t v1, int32_t v2)
   return (it != e && *it == v2) ? ix->expsim[it - ix->col.begin()] : 1.0;  // getOrElse(valueId2, 1.0), :185
 }
 extern "C" double dbl_similarity(int similarity, const char *a, const char *b, double threshold, double max_sim) {
-  if (similarity == 0) return 0.0;  // ConstantSimilarityFn, SimilarityFn.scala:50
+  if (similarity < DBL_SIM_CONSTANT || similarity > DBL_SIM_JARO_WINKLER) return std::numeric_limits<double>::quiet_NaN();
+  if (similarity == DBL_SIM_CONSTANT) return 0.0;  // ConstantSimilarityFn, SimilarityFn.scala:50
   const int la = (int)std::strlen(a), lb = (int)std::strlen(b);
-  return host_similarity_from_distance(host_levenshtein(a, la, b, lb), la, lb, threshold, max_sim);
+  return host_similarity_from_unit(host_unit_similarity(similarity, a, la, b, lb), threshold, max_sim);
 }
 
 // ---------------------------------------------------------------------------------------------------

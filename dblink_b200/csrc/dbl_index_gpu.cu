@@ -1,12 +1,14 @@
 // AttributeIndex construction on the GPU (the step before the sweep; AttributeIndex.scala:107-245):
-//   * all-pairs thresholded Levenshtein (computeSimValueIndex, :219-231: V^2 pairs, keep exp(sim) > 1);
+//   * all-pairs thresholded Levenshtein or Jaro-Winkler (computeSimValueIndex, :219-231: V^2 pairs, keep
+//     exp(sim) > 1);
 //   * the similarity normalisations n_a(v) (computeSimNormalizations, :234-245) and the base pmfs / cdfs
 //     B_k, k = 0..kmax (getSimNormDist, :197-216).
 //
-// Everything stays bit-identical to the host loops: the device computes only the INTEGER edit distance of the pairs
-// that can possibly have a positive truncated similarity (the host turns (distance, lengths) into sim and exp(sim)
-// with the same double arithmetic as the host-only path), and the normalisation / pmf kernels run the host's
-// sequential sums unchanged, one independent sum per thread (this TU is compiled with -fmad=false like the rest).
+// Everything stays bit-identical to the host loops: the device computes only INTEGERS -- the edit distance, or the
+// Jaro-Winkler counts (m, h, l) -- of the pairs that can possibly have a positive truncated similarity (the host
+// turns (integers, lengths) into sim and exp(sim) with the same double arithmetic as the host-only path), and the
+// normalisation / pmf kernels run the host's sequential sums unchanged, one independent sum per thread (this TU is
+// compiled with -fmad=false like the rest).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -29,6 +31,17 @@ constexpr int LEV_TEXTS = 256;  // texts per CTA (32 per warp)
 //   of 5 per DP cell.
 // Only pairs j > i are produced (the matrix is symmetric), and only those whose distance can give a positive
 // truncated similarity: sim > 0  <=>  d < (|a| + |b|) (1 - t) / (1 + t), t = threshold / maxSimilarity.
+// Peq[c][lane] = bit set of the positions of byte c in pattern i0 + lane (all zero for lanes past V)
+__device__ __forceinline__ void load_patterns(unsigned long long *peq, int V, const unsigned char *__restrict__ strs,
+                                              int i, int m) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int k = threadIdx.x; k < 256 * 32; k += blockDim.x) peq[k] = 0ull;
+  __syncthreads();
+  if (warp == 0 && i < V)
+    for (int q = 0; q < m; ++q) peq[(int)strs[(size_t)i * MAXL + q] * 32 + lane] |= 1ull << q;
+  __syncthreads();
+}
+
 __global__ void __launch_bounds__(LEV_WARPS * 32) k_lev_tiles(int V, const unsigned char *__restrict__ strs,
                                                               const int *__restrict__ lens, double ratio,
                                                               unsigned long long cap,
@@ -39,13 +52,9 @@ __global__ void __launch_bounds__(LEV_WARPS * 32) k_lev_tiles(int V, const unsig
   const int j0 = blockIdx.x * LEV_TEXTS;
   if (j0 + LEV_TEXTS <= i0) return;  // whole text tile at or below the diagonal
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int k = threadIdx.x; k < 256 * 32; k += blockDim.x) peq[k] = 0ull;
-  __syncthreads();
   const int i = i0 + lane;
   const int m = (i < V) ? lens[i] : 0;
-  if (warp == 0 && i < V)
-    for (int q = 0; q < m; ++q) peq[(int)strs[(size_t)i * MAXL + q] * 32 + lane] |= 1ull << q;
-  __syncthreads();
+  load_patterns(peq, V, strs, i, m);
   const unsigned long long top = m > 0 ? 1ull << (m - 1) : 0ull;
   for (int jj = warp; jj < LEV_TEXTS; jj += LEV_WARPS) {
     const int j = j0 + jj;
@@ -75,6 +84,77 @@ __global__ void __launch_bounds__(LEV_WARPS * 32) k_lev_tiles(int V, const unsig
         if (slot < cap) out[slot] = make_int4(i, j, d, 0);
       }
     }
+  }
+}
+
+// Slack of the device's Jaro-Winkler filters against t = threshold / maxSimilarity: the host keeps a pair only when
+// maxSimilarity * unit > threshold, and the device's double estimates are within a few ulps of the host's, so a pair
+// the filters drop has unit < t - 1e-9 and a truncated similarity of exactly 0.
+constexpr double JW_SLACK = 1e-9;
+
+// Jaro-Winkler counts in the k_lev_tiles layout (lane = pattern a = string i, one text b = string j per warp
+// iteration, Peq in shared memory).  The greedy scan runs over the TEXT: each byte b[q] takes the lowest unmatched
+// pattern position in the window [q - w, q + w] holding the same byte (Peq & window & ~flagP); flagT records the
+// matched text positions.  This is the host's scan with a and b swapped; the counts (m, h) are symmetric in (a, b),
+// so they are the host's counts of (i, j) and (j, i) alike.  h pairs the k-th set bits of flagP and flagT: pattern
+// position ip holds b[jp] iff bit ip of Peq[b[jp]] is set.  l = the first q < 4 where bit q of Peq[b[q]] is clear.
+// The pair is skipped before the scan when even m = min(la, lb), h = 0, l = 4 cannot pass t (jaro <= (2 + min/max)/3),
+// and after it when its own estimate cannot; the host recomputes the exact double from (m, h, l).
+__global__ void __launch_bounds__(LEV_WARPS * 32) k_jw_tiles(int V, const unsigned char *__restrict__ strs,
+                                                             const int *__restrict__ lens, double t,
+                                                             unsigned long long cap,
+                                                             unsigned long long *__restrict__ count,
+                                                             int4 *__restrict__ out) {
+  extern __shared__ unsigned long long peq[];  // [256][32]
+  const int i0 = blockIdx.y * 32;
+  const int j0 = blockIdx.x * LEV_TEXTS;
+  if (j0 + LEV_TEXTS <= i0) return;  // whole text tile at or below the diagonal
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int i = i0 + lane;
+  const int la = (i < V) ? lens[i] : 0;
+  load_patterns(peq, V, strs, i, la);
+  const double cut = t - JW_SLACK;
+  for (int jj = warp; jj < LEV_TEXTS; jj += LEV_WARPS) {
+    const int j = j0 + jj;
+    if (j >= V) break;
+    if (i >= V || j <= i) continue;
+    const int lb = lens[j];
+    const unsigned char *T = strs + (size_t)j * MAXL;  // every lane reads the same bytes (broadcast from L1)
+    const int lo = min(la, lb), hi = max(la, lb);
+    if (hi > 0) {
+      const double jb = (2.0 + (double)lo / hi) / 3.0;
+      if (jb + 0.4 * (1.0 - jb) < cut) continue;
+    }
+    const int w = max(0, hi / 2 - 1);
+    unsigned long long fp = 0ull, ft = 0ull;
+    int l = 0;
+    bool prefix = true;
+    for (int q = 0; q < lb; ++q) {
+      const unsigned long long Eq = peq[(int)T[q] * 32 + lane];
+      if (q < 4 && prefix) {
+        if ((Eq >> q) & 1ull) ++l;
+        else prefix = false;
+      }
+      const unsigned long long win = (~0ull << max(0, q - w)) & ((2ull << min(q + w, 63)) - 1ull);
+      const unsigned long long cand = Eq & win & ~fp;
+      if (cand) {
+        fp |= cand & (0ull - cand);
+        ft |= 1ull << q;
+      }
+    }
+    const int m = __popcll(fp);
+    if (m == 0 && hi > 0) continue;  // unit 0; two empty strings (unit 1) leave with code 0
+    int h = 0;
+    for (unsigned long long p = fp, s = ft; p; p &= p - 1, s &= s - 1) {
+      const int ip = __ffsll((long long)p) - 1, jp = __ffsll((long long)s) - 1;
+      h += (int)(~(peq[(int)T[jp] * 32 + lane] >> ip) & 1ull);
+    }
+    if (m > 0) {
+      const double jaro = ((double)m / la + (double)m / lb + ((double)m - 0.5 * h) / m) / 3.0;
+      if (jaro + 0.1 * l * (1.0 - jaro) < cut) continue;
+    }
+    const unsigned long long slot = atomicAdd(count, 1ull);
+    if (slot < cap) out[slot] = make_int4(i, j, m | h << 8 | l << 16, 0);
   }
 }
 
@@ -131,10 +211,11 @@ struct Dev {
 };
 }  // namespace
 
-// Fills `out` with (i, j>i, distance) for every pair that may have a positive similarity.  Returns false when the
-// GPU path is not applicable (no device, strings too long) -- the caller then uses the host loop.
-bool gpu_levenshtein_candidates(const std::vector<std::string> &values, double threshold, double max_sim,
-                                std::vector<int> &oi, std::vector<int> &oj, std::vector<int> &od) {
+// Fills (oi, oj, oc) with (i, j>i, code) for every pair that may have a positive similarity: code = the edit distance
+// (similarity 1, k_lev_tiles) or m | h << 8 | l << 16 (similarity 2, k_jw_tiles).  Returns false when the GPU path is
+// not applicable (no device, strings too long) -- the caller then uses the host loop.
+bool gpu_similarity_candidates(int similarity, const std::vector<std::string> &values, double threshold,
+                               double max_sim, std::vector<int> &oi, std::vector<int> &oj, std::vector<int> &oc) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return false; }
   const int V = (int)values.size();
@@ -147,7 +228,10 @@ bool gpu_levenshtein_candidates(const std::vector<std::string> &values, double t
     std::memcpy(&h_strs[(size_t)v * MAXL], values[v].data(), values[v].size());
   }
   const double t = threshold / max_sim;
-  const double ratio = (1.0 - t) / (1.0 + t);
+  // both kernels take one double: Levenshtein the distance ratio of its length bound, Jaro-Winkler t itself
+  const bool jw = similarity == DBL_SIM_JARO_WINKLER;
+  const auto kernel = jw ? k_jw_tiles : k_lev_tiles;
+  const double param = jw ? t : (1.0 - t) / (1.0 + t);
   Dev d_strs, d_lens, d_count;
   if (!d_strs.alloc(h_strs.size()) || !d_lens.alloc(sizeof(int) * V) || !d_count.alloc(sizeof(unsigned long long))) {
     cudaGetLastError();
@@ -156,7 +240,7 @@ bool gpu_levenshtein_candidates(const std::vector<std::string> &values, double t
   cudaMemcpy(d_strs.p, h_strs.data(), h_strs.size(), cudaMemcpyHostToDevice);
   cudaMemcpy(d_lens.p, h_lens.data(), sizeof(int) * V, cudaMemcpyHostToDevice);
   const size_t smem = 256 * 32 * sizeof(unsigned long long);
-  if (cudaFuncSetAttribute(k_lev_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
     cudaGetLastError();
     return false;
   }
@@ -168,16 +252,16 @@ bool gpu_levenshtein_candidates(const std::vector<std::string> &values, double t
     // 2-D grid of tiles: x = text tiles (no 65 535 limit on this axis), y = pattern tiles of 32 (V <= 2 097 120)
     const dim3 grid((unsigned)((V + LEV_TEXTS - 1) / LEV_TEXTS), (unsigned)((V + 31) / 32));
     if (grid.y > 65535u) break;
-    k_lev_tiles<<<grid, LEV_WARPS * 32, smem>>>(V, (const unsigned char *)d_strs.p, (const int *)d_lens.p, ratio, cap,
-                                                (unsigned long long *)d_count.p, (int4 *)d_out.p);
+    kernel<<<grid, LEV_WARPS * 32, smem>>>(V, (const unsigned char *)d_strs.p, (const int *)d_lens.p, param, cap,
+                                           (unsigned long long *)d_count.p, (int4 *)d_out.p);
     unsigned long long n = 0;
     if (cudaMemcpy(&n, d_count.p, sizeof(n), cudaMemcpyDeviceToHost) != cudaSuccess) break;
     if (n <= cap) {
       std::vector<int4> h((size_t)n);
       if (n) cudaMemcpy(h.data(), d_out.p, sizeof(int4) * n, cudaMemcpyDeviceToHost);
       // the order in which pairs were appended depends on scheduling; the caller sorts the rows
-      oi.resize(n); oj.resize(n); od.resize(n);
-      for (size_t k = 0; k < n; ++k) { oi[k] = h[k].x; oj[k] = h[k].y; od[k] = h[k].z; }
+      oi.resize(n); oj.resize(n); oc.resize(n);
+      for (size_t k = 0; k < n; ++k) { oi[k] = h[k].x; oj[k] = h[k].y; oc[k] = h[k].z; }
       return true;
     }
     cap = n + 1024;

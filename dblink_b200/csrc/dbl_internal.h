@@ -243,12 +243,17 @@ struct dbl_kdtree {
 void host_draw_theta(int A, int F, const double *alpha, const double *beta, uint64_t seed, const int64_t *agg_dist,
                      const int64_t *file_sizes, uint32_t iter, double *theta_out);
 int host_levenshtein(const char *a, int la, const char *b, int lb);
-// GPU all-pairs candidate distances for the attribute index (dbl_index_gpu.cu); false = not applicable
-bool gpu_levenshtein_candidates(const std::vector<std::string> &values, double threshold, double max_sim,
-                                std::vector<int> &oi, std::vector<int> &oj, std::vector<int> &od);
+void host_jaro_winkler_counts(const char *a, int la, const char *b, int lb, int &m, int &h, int &l);
+// GPU all-pairs candidates for the attribute index (dbl_index_gpu.cu): (i, j > i, code) with code = the edit
+// distance (similarity 1) or m | h << 8 | l << 16 (similarity 2, Jaro-Winkler counts); false = not applicable
+bool gpu_similarity_candidates(int similarity, const std::vector<std::string> &values, double threshold,
+                               double max_sim, std::vector<int> &oi, std::vector<int> &oj, std::vector<int> &oc);
 // norm / invnorm / pk / cdf on the device (dbl_index_gpu.cu), same values as the host loops; false = not applicable
 bool gpu_index_tables(int V, int kmax, bool is_const, const std::vector<double> &probs,
                       const std::vector<int32_t> &rowptr, const std::vector<int32_t> &col,
                       const std::vector<double> &expsim, std::vector<double> &norm, std::vector<double> &invnorm,
                       std::vector<double> &pk, std::vector<double> &cdf);
-double host_similarity_from_distance(int dist, int la, int lb, double threshold, double max_sim);
+// unit similarities and the truncation of SimilarityFn.scala:65-70 (dbl_host.cpp, compiled without FP contraction)
+double host_levenshtein_unit(int dist, int la, int lb);
+double host_jaro_winkler_unit(int m, int h, int l, int la, int lb);
+double host_similarity_from_unit(double unit, double threshold, double max_sim);

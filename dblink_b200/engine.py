@@ -46,6 +46,12 @@ def _check(rc, what, ctx=None):
     raise DblinkError(f"{what}: error {rc} {msg}")
 
 
+SIMILARITY_KINDS = {"constant": _lib.SIM_CONSTANT, "levenshtein": _lib.SIM_LEVENSHTEIN,
+                    "jaro-winkler": _lib.SIM_JARO_WINKLER}
+SIMILARITY_FNS = {"ConstantSimilarityFn": _lib.SIM_CONSTANT, "LevenshteinSimilarityFn": _lib.SIM_LEVENSHTEIN,
+                  "JaroWinklerSimilarityFn": _lib.SIM_JARO_WINKLER}
+
+
 class AttributeIndex:
     """Index of one attribute domain (AttributeIndex.scala:39-104)."""
 
@@ -60,15 +66,18 @@ class AttributeIndex:
     @classmethod
     def build(cls, values_weights, similarity="constant", threshold=7.0, max_similarity=10.0,
               expected_max_cluster_size=10):
-        """AttributeIndex.apply (AttributeIndex.scala:107-127).  similarity: 'constant' | 'levenshtein'."""
+        """AttributeIndex.apply (AttributeIndex.scala:107-127).  similarity: 'constant' | 'levenshtein' |
+        'jaro-winkler'."""
         if not values_weights:
             raise ValueError("index cannot be empty")  # AttributeIndex.scala:111
+        if similarity not in SIMILARITY_KINDS:
+            raise ValueError(f"unsupported similarity {similarity!r}")
         L = _lib.load()
         vals = list(values_weights.keys())
         arr = (C.c_char_p * len(vals))(*[v.encode() for v in vals])
         w = _f64([values_weights[v] for v in vals])
         h = C.c_void_p()
-        sim = 0 if similarity == "constant" else 1
+        sim = SIMILARITY_KINDS[similarity]
         _check(L.dbl_index_build(C.byref(h), arr, _p(w, _lib.f64p), len(vals), sim, threshold, max_similarity,
                                  expected_max_cluster_size), "AttributeIndex.build")
         return cls(h, sim == 0)
@@ -150,14 +159,17 @@ class AttributeIndex:
 
 
 def similarity(a, b, name="LevenshteinSimilarityFn", threshold=7.0, max_similarity=10.0):
-    """SimilarityFn.getSimilarity (SimilarityFn.scala:50-98)."""
+    """SimilarityFn.getSimilarity (SimilarityFn.scala:50-98); name: 'ConstantSimilarityFn' |
+    'LevenshteinSimilarityFn' | 'JaroWinklerSimilarityFn'."""
+    if name not in SIMILARITY_FNS:
+        raise ValueError(f"unsupported similarity function {name}")
     if name == "ConstantSimilarityFn":
         return 0.0
     if not (max_similarity > 0.0):
         raise ValueError("`maxSimilarity` must be positive")
     if not (0.0 <= threshold < max_similarity):
         raise ValueError("`threshold` must be in the interval [0, maxSimilarity)")
-    return _lib.load().dbl_similarity(1, a.encode(), b.encode(), threshold, max_similarity)
+    return _lib.load().dbl_similarity(SIMILARITY_FNS[name], a.encode(), b.encode(), threshold, max_similarity)
 
 
 class KDTreePartitioner:

@@ -59,8 +59,8 @@ class Project:
             sf = c["similarityFunction"]
             if sf["name"] == "ConstantSimilarityFn":
                 fn = SimilarityFn("ConstantSimilarityFn")
-            elif sf["name"] == "LevenshteinSimilarityFn":
-                fn = SimilarityFn("LevenshteinSimilarityFn", float(sf["parameters"]["threshold"]),
+            elif sf["name"] in ("LevenshteinSimilarityFn", "JaroWinklerSimilarityFn"):
+                fn = SimilarityFn(sf["name"], float(sf["parameters"]["threshold"]),
                                   float(sf["parameters"]["maxSimilarity"]))
             else:
                 raise hocon.ConfigError("similarityFunction.name: unsupported value")
@@ -85,7 +85,7 @@ class Project:
         def sim(fn):
             if fn.name == "ConstantSimilarityFn":
                 return "ConstantSimilarityFn"
-            return f"LevenshteinSimilarityFn(threshold={fn.threshold}, maxSimilarity={fn.max_similarity})"
+            return f"{fn.name}(threshold={fn.threshold}, maxSimilarity={fn.max_similarity})"
 
         L = ["Data settings", "-------------", f"  * Using data files located at '{self.data_path}'",
              f"  * The record identifier attribute is '{self.rec_id_attribute}'",

@@ -10,18 +10,23 @@ from typing import List, Optional
 
 import numpy as np
 
-from .engine import AttributeIndex
+from .engine import SIMILARITY_FNS, AttributeIndex
+
+# the AttributeIndex.build kind of each similarity function
+_INDEX_KIND = {"ConstantSimilarityFn": "constant", "LevenshteinSimilarityFn": "levenshtein",
+               "JaroWinklerSimilarityFn": "jaro-winkler"}
 
 
 @dataclass
 class SimilarityFn:
-    """SimilarityFn.scala:50-107."""
+    """SimilarityFn.scala:50-107, plus JaroWinklerSimilarityFn: the Jaro-Winkler unit similarity of two strings
+    (bytes, prefix scale 0.1) under the same threshold / maxSimilarity truncation as LevenshteinSimilarityFn."""
     name: str = "ConstantSimilarityFn"
     threshold: float = 7.0
     max_similarity: float = 10.0
 
     def __post_init__(self):
-        if self.name not in ("ConstantSimilarityFn", "LevenshteinSimilarityFn"):
+        if self.name not in SIMILARITY_FNS:
             raise ValueError(f"unsupported similarity function {self.name}")
         if self.name != "ConstantSimilarityFn":
             if not self.max_similarity > 0.0:
@@ -32,6 +37,11 @@ class SimilarityFn:
     @property
     def is_constant(self):
         return self.name == "ConstantSimilarityFn"
+
+    @property
+    def index_kind(self):
+        """the `similarity` argument of AttributeIndex.build"""
+        return _INDEX_KIND[self.name]
 
 
 @dataclass
@@ -90,8 +100,8 @@ class RecordsCache:
         for a, attr in enumerate(attributes):
             vw = {k: float(v) for k, v in counts[a].items()}
             sf = attr.similarity_fn
-            indexes.append(AttributeIndex.build(vw, "constant" if sf.is_constant else "levenshtein", sf.threshold,
-                                                sf.max_similarity, expected_max_cluster_size))
+            indexes.append(AttributeIndex.build(vw, sf.index_kind, sf.threshold, sf.max_similarity,
+                                                expected_max_cluster_size))
         fids = sorted(fsz.keys())
         return cls(attributes, indexes, fids, [fsz[f] for f in fids], dict(missing))
 
@@ -187,9 +197,8 @@ def build_cache_from_columns(columns, files, attributes: List[Attribute], expect
         ci = np.where(valid, np.nan_to_num(codes, nan=0).astype(np.int64), 0)
         cnt = np.bincount(ci[valid], minlength=len(vals))
         sf = attr.similarity_fn
-        ix = AttributeIndex.build({v: float(c) for v, c in zip(vals, cnt) if c > 0},
-                                  "constant" if sf.is_constant else "levenshtein", sf.threshold, sf.max_similarity,
-                                  expected_max_cluster_size)
+        ix = AttributeIndex.build({v: float(c) for v, c in zip(vals, cnt) if c > 0}, sf.index_kind, sf.threshold,
+                                  sf.max_similarity, expected_max_cluster_size)
         lut = np.array([ix.value_idx_of(v) if c > 0 else -1 for v, c in zip(vals, cnt)] + [-1], np.int32)
         x[:, a] = np.where(valid, lut[ci], -1)
         indexes.append(ix)

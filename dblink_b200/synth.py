@@ -150,9 +150,8 @@ def build_encoded(enc, expected_max_cluster_size=10):
         cnt = np.bincount(c[c >= 0], minlength=len(vocab))
         used = np.flatnonzero(cnt)
         sf = attr.similarity_fn
-        ix = AttributeIndex.build({vocab[i]: float(cnt[i]) for i in used},
-                                  "constant" if sf.is_constant else "levenshtein", sf.threshold, sf.max_similarity,
-                                  expected_max_cluster_size)
+        ix = AttributeIndex.build({vocab[i]: float(cnt[i]) for i in used}, sf.index_kind, sf.threshold,
+                                  sf.max_similarity, expected_max_cluster_size)
         lut = np.full(len(vocab) + 1, -1, np.int32)
         for i in used:
             lut[i] = ix.value_idx_of(vocab[i])

@@ -34,6 +34,12 @@ extern "C" {
 
 #define DBL_MAX_ATTRS 32
 
+/* similarity functions of an attribute (SimilarityFn.scala:50-107, plus Jaro-Winkler) */
+#define DBL_SIM_CONSTANT 0     /* ConstantSimilarityFn                                                          */
+#define DBL_SIM_LEVENSHTEIN 1  /* LevenshteinSimilarityFn: unit = 1 - 2 d / (|a| + |b| + d)                     */
+#define DBL_SIM_JARO_WINKLER 2 /* JaroWinklerSimilarityFn: Jaro-Winkler over bytes, prefix scale 0.1, common
+                                  prefix capped at 4, no boost threshold; same truncation as Levenshtein         */
+
 typedef struct dbl_index dbl_index;   /* AttributeIndex  (AttributeIndex.scala:39-104)                          */
 typedef struct dbl_kdtree dbl_kdtree; /* KDTreePartitioner / MutableBST (partitioning/KDTreePartitioner.scala)  */
 typedef struct dbl_ctx dbl_ctx;       /* State + broadcast RecordsCache/PartitionFunction (State.scala:56-68)   */
@@ -43,11 +49,15 @@ typedef struct dbl_ctx dbl_ctx;       /* State + broadcast RecordsCache/Partitio
  * order, empirical pmf, sparse exp(similarity) rows (computeSimValueIndex :219-231), normalisations
  * (computeSimNormalizations :234-245), cached base pmfs k=0..kmax (getSimNormDist :197-216,
  * RecordsCache.scala:112-113).  similarity: 0 = ConstantSimilarityFn, 1 = LevenshteinSimilarityFn
- * (SimilarityFn.scala:50-107).  `values` need not be sorted; `weights` are the value counts.
+ * (SimilarityFn.scala:50-107), 2 = JaroWinklerSimilarityFn (DBL_SIM_*); any other value is DBL_ERR_INVALID.
+ * For 1 and 2 a pair is in the sparse rows when exp(sim) > 1, sim = the truncation of SimilarityFn.scala:65-70
+ * applied to the unit similarity.  `values` need not be sorted; `weights` are the value counts.
  * ------------------------------------------------------------------------------------------------- */
 int dbl_index_build(dbl_index **out, const char *const *values, const double *weights, int32_t num_values,
                     int similarity, double threshold, double max_similarity, int32_t kmax);
-/* Same object from pre-computed tables (phi = weight/total as in AttributeIndex.scala:114-115). */
+/* Same object from pre-computed tables (phi = weight/total as in AttributeIndex.scala:114-115).  similarity 0 =
+ * constant (no rows); 1 or 2 = non-constant, the rows given (both kinds give the same kind of tables); any other
+ * value is DBL_ERR_INVALID. */
 int dbl_index_from_tables(dbl_index **out, int32_t num_values, int similarity, const double *probs,
                           const int32_t *rowptr, const int32_t *col, const double *expsim, int32_t kmax);
 void dbl_index_free(dbl_index *);
@@ -66,7 +76,8 @@ const char *dbl_index_value(const dbl_index *, int32_t value_id);
 int dbl_index_tables(const dbl_index *, double *phi /*probabilityOf*/, double *norm /*simNormalizationOf*/,
                      int32_t *rowptr, int32_t *col, double *expsim /*simValuesOf*/);
 double dbl_index_exp_sim(const dbl_index *, int32_t v1, int32_t v2); /* expSimOf; NaN when out of range        */
-/* SimilarityFn.getSimilarity (SimilarityFn.scala:65-70, 84-96) */
+/* SimilarityFn.getSimilarity (SimilarityFn.scala:65-70, 84-96); similarity as in dbl_index_build (2 = Jaro-Winkler
+ * unit similarity under the same truncation); NaN for an unknown similarity */
 double dbl_similarity(int similarity, const char *a, const char *b, double threshold, double max_similarity);
 
 /* ---------------------------------------------------------------------------------------------------
