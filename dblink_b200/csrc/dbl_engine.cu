@@ -861,14 +861,20 @@ __global__ void k_mark_rec_owned(int64_t R, const int *__restrict__ link, const 
   if (r < R) rec_owned[r] = ent_owned[link[r]];
 }
 
-// ---- (1) peer-to-peer exchange: the data plane of a sharded dbl_sweep ---------------------------------------
-// Every rank owns one communication buffer (cudaMalloc, exported with cudaIpc, mapped by every peer over
-// NVLink/NVSwitch).  The kernels that decide which clusters leave write the messages STRAIGHT into the destination
-// rank's receive buffer (slot from a system-scope atomic on the destination's cursor), the partial summary goes into
-// a slot of every peer, one flag barrier follows, then every rank unpacks what it received and reduces the summary
-// slots in rank order.  No host round trip, no separate pack / count / send / receive steps.  Receive buffers have
-// room for EVERY entity and record (an entity moves at most once per sweep), and everything is double buffered by
-// barrier parity, so a fast rank can run ahead by one sweep without overwriting what a slow one still reads.
+// ---- the cluster messages of a sharded sweep -------------------------------------------------------------------
+// One set of kernels writes and applies the messages for both transports; they differ only in where the messages go
+// (MsgOut) and where the received ones are (MsgIn), two tables indexed by barrier parity:
+// * peer to peer (dbl_sweep on a connected context): every rank owns one communication buffer (cudaMalloc, exported
+//   with cudaIpc, mapped by every peer over NVLink/NVSwitch).  k_move_* write the messages STRAIGHT into the
+//   destination rank's receive buffer (slot from a system-scope atomic on the destination's cursor), the partial
+//   summary goes into a slot of every peer, one flag barrier follows, then every rank unpacks what it received and
+//   reduces the summary slots in rank order.  No host round trip.  Receive buffers have room for EVERY entity and
+//   record (an entity moves at most once per sweep), and everything is double buffered by barrier parity, so a fast
+//   rank can run ahead by one sweep without overwriting what a slow one still reads.  dbl_comm_import fills the
+//   tables once; the parity is picked on the device, so captured sweeps replay.
+// * host-mediated (dbl_sweep_begin / dbl_exchange_pack / dbl_exchange_unpack / dbl_sweep_end): k_move_* write into
+//   the caller's send buffers, rank d's messages at the offset of the counts before d, with cursors of this context;
+//   k_unpack_* read the caller's receive buffers.  Both parities point at the same buffers.
 constexpr int MAX_WORLD = 16;
 struct CommDev {
   int rank, world, A, nws;  // nws = summary words per slot (partial summary + status)
@@ -876,37 +882,43 @@ struct CommDev {
   unsigned char *base[MAX_WORLD];  // communication buffer of every rank (own buffer at [rank])
   size_t off_cursor, off_slots, off_ent, off_rec;
   __device__ __forceinline__ unsigned long long *arrive(int d) const { return reinterpret_cast<unsigned long long *>(base[d]); }
-  __device__ __forceinline__ unsigned long long *cursor(int d, int par) const {
+  __host__ __device__ __forceinline__ unsigned long long *cursor(int d, int par) const {
     return reinterpret_cast<unsigned long long *>(base[d] + off_cursor) + 2 * par;
   }
   __device__ __forceinline__ long long *slot(int d, int par, int src) const {
     return reinterpret_cast<long long *>(base[d] + off_slots) + ((size_t)par * world + src) * nws;
   }
-  __device__ __forceinline__ int *recv_ent(int d, int par) const {
-    return reinterpret_cast<int *>(base[d] + off_ent) + (size_t)par * cap_e * (A + 1);
-  }
-  __device__ __forceinline__ int *recv_rec(int d, int par) const {
-    return reinterpret_cast<int *>(base[d] + off_rec) + (size_t)par * cap_r * 3;
-  }
+  int *recv_ent(int d, int par) const { return reinterpret_cast<int *>(base[d] + off_ent) + (size_t)par * cap_e * (A + 1); }
+  int *recv_rec(int d, int par) const { return reinterpret_cast<int *>(base[d] + off_rec) + (size_t)par * cap_r * 3; }
 };
 __device__ __forceinline__ int comm_parity(const long long *ctl) { return (int)((ctl[CTL_EPOCH] + 1) & 1); }
 
-// slot in rank d's buffer for every lane that has a message for d: one system-scope atomic per destination and warp.
+// where the messages for destination rank d go, by parity
+struct MsgOut {
+  int *ent[MAX_WORLD][2], *rec[MAX_WORLD][2];
+  unsigned long long *cursor[MAX_WORLD][2];  // cursor pair: [0] entities, [1] records
+};
+// where the messages this rank received are, by parity
+struct MsgIn {
+  const int *ent[2], *rec[2];
+  const unsigned long long *count[2];  // count pair: [0] entities, [1] records
+};
+
+// slot in rank d's area for every lane that has a message for d: one system-scope atomic per destination and warp.
 // Every lane of the warp calls it (d < 0: nothing to send).
-__device__ __forceinline__ long long remote_slot(unsigned long long *const *cursors_unused, const CommDev &c, int par,
-                                                 int which, int d) {
-  (void)cursors_unused;
+__device__ __forceinline__ long long dest_slot(const MsgOut &o, int par, int which, int d) {
   const int lane = threadIdx.x & 31;
   const unsigned grp = __match_any_sync(FULL, d);
   const int leader = __ffs(grp) - 1;
   unsigned long long basev = 0;
-  if (d >= 0 && lane == leader) basev = atomicAdd_system(c.cursor(d, par) + which, (unsigned long long)__popc(grp));
+  if (d >= 0 && lane == leader) basev = atomicAdd_system(o.cursor[d][par] + which, (unsigned long long)__popc(grp));
   basev = __shfl_sync(FULL, basev, leader);
   return (long long)basev + __popc(grp & ((1u << lane) - 1u));
 }
 
 struct MoveParams {
-  CommDev c;
+  int rank;
+  MsgOut out;
   long long *ctl;
   int A;
   const int *ent_sorted, *rec_sorted;
@@ -927,12 +939,12 @@ __global__ void __launch_bounds__(256) k_move_ent(MoveParams p) {
     if (i < n) {
       e = p.ent_sorted[i];
       const int o = p.owner[p.blk[e]];
-      if (o != p.c.rank) d = o;
+      if (o != p.rank) d = o;
       p.ent_dest[e] = d;
     }
-    const long long slot = remote_slot(nullptr, p.c, par, 0, d);
+    const long long slot = dest_slot(p.out, par, 0, d);
     if (d >= 0) {
-      int *m = p.c.recv_ent(d, par) + slot * (p.A + 1);
+      int *m = p.out.ent[d][par] + slot * (p.A + 1);
       m[0] = (int)e;
       for (int a = 0; a < p.A; ++a) m[1 + a] = p.y[e * p.A + a];
       p.ent_owned[e] = 0;
@@ -954,9 +966,9 @@ __global__ void __launch_bounds__(256) k_move_rec(MoveParams p) {
       r = p.rec_sorted[i];
       d = p.ent_dest[p.link[r]];
     }
-    const long long slot = remote_slot(nullptr, p.c, par, 1, d);
+    const long long slot = dest_slot(p.out, par, 1, d);
     if (d >= 0) {
-      int *m = p.c.recv_rec(d, par) + slot * 3;
+      int *m = p.out.rec[d][par] + slot * 3;
       m[0] = (int)r; m[1] = p.link[r]; m[2] = (int)p.zmask[r];
       p.rec_owned[r] = 0;
       ++sent;
@@ -1003,7 +1015,7 @@ __global__ void __launch_bounds__(256) k_publish_barrier(CommDev c, long long *c
 // what the peers wrote for this rank (parity of the barrier just passed)
 __device__ __forceinline__ int done_parity(const long long *ctl) { return (int)(ctl[CTL_EPOCH] & 1); }
 struct UnpackParams {
-  CommDev c;
+  MsgIn in;
   const long long *ctl;
   int A;
   const AttrDev *attrs;
@@ -1013,11 +1025,11 @@ struct UnpackParams {
   unsigned *zmask;
   unsigned char *ent_owned, *rec_owned;
 };
-__global__ void __launch_bounds__(256) k_unpack_ent_p2p(UnpackParams p) {
+__global__ void __launch_bounds__(256) k_unpack_ent(UnpackParams p) {
   if (p.ctl[CTL_STATUS] & ST_PEER_TIMEOUT) return;
   const int par = done_parity(p.ctl);
-  const int64_t n = (int64_t) * reinterpret_cast<volatile unsigned long long *>(p.c.cursor(p.c.rank, par));
-  const int *buf = p.c.recv_ent(p.c.rank, par);
+  const int64_t n = (int64_t) * reinterpret_cast<const volatile unsigned long long *>(p.in.count[par]);
+  const int *buf = p.in.ent[par];
   GRID_STRIDE(i, n) {
     const int *m = buf + i * (p.A + 1);
     const int64_t e = m[0];
@@ -1032,11 +1044,11 @@ __global__ void __launch_bounds__(256) k_unpack_ent_p2p(UnpackParams p) {
     p.ent_owned[e] = 1;
   }
 }
-__global__ void __launch_bounds__(256) k_unpack_rec_p2p(UnpackParams p) {
+__global__ void __launch_bounds__(256) k_unpack_rec(UnpackParams p) {
   if (p.ctl[CTL_STATUS] & ST_PEER_TIMEOUT) return;
   const int par = done_parity(p.ctl);
-  const int64_t n = (int64_t) * reinterpret_cast<volatile unsigned long long *>(p.c.cursor(p.c.rank, par) + 1);
-  const int *buf = p.c.recv_rec(p.c.rank, par);
+  const int64_t n = (int64_t) * reinterpret_cast<const volatile unsigned long long *>(p.in.count[par] + 1);
+  const int *buf = p.in.rec[par];
   GRID_STRIDE(i, n) {
     const int *m = buf + i * 3;
     const int64_t r = m[0];
@@ -1119,80 +1131,6 @@ __global__ void k_lpt(int P, int world, int ent_slot, int rec_slot, const long l
     for (int b = 0; b < P; ++b) owner[b] = cand[b];
     ctl[CTL_REPLACED] += 1;
   }
-}
-
-// ---- (2) host-mediated exchange (multi-node / no peer access): counts to the host, messages packed into caller
-// buffers, the host moves them (e.g. NCCL all-to-all) and hands back what arrived -----------------------------------
-__global__ void k_move_count_ent(int64_t E, const int *__restrict__ blk, const int *__restrict__ owner, int rank,
-                                 const unsigned char *__restrict__ ent_owned, int *__restrict__ ent_dest,
-                                 unsigned long long *__restrict__ cnt) {
-  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= E) return;
-  int d = -1;
-  if (ent_owned[e]) {
-    const int o = owner[blk[e]];
-    if (o != rank) { d = o; atomicAdd(&cnt[o], 1ull); }
-  }
-  ent_dest[e] = d;
-}
-__global__ void k_move_count_rec(int64_t R, const int *__restrict__ link, const unsigned char *__restrict__ rec_owned,
-                                 const int *__restrict__ ent_dest, unsigned long long *__restrict__ cnt) {
-  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= R || !rec_owned[r]) return;
-  const int d = ent_dest[link[r]];
-  if (d >= 0) atomicAdd(&cnt[d], 1ull);
-}
-__global__ void k_move_pack_ent(int64_t E, int A, const int *__restrict__ y, const int *__restrict__ ent_dest,
-                                unsigned char *__restrict__ ent_owned, unsigned long long *__restrict__ cursor,
-                                int *__restrict__ buf) {
-  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= E) return;
-  const int d = ent_owned[e] ? ent_dest[e] : -1;
-  if (d < 0) return;
-  const unsigned long long slot = atomicAdd(&cursor[d], 1ull);
-  int *m = buf + slot * (A + 1);
-  m[0] = (int)e;
-  for (int a = 0; a < A; ++a) m[1 + a] = y[e * A + a];
-  ent_owned[e] = 0;
-}
-__global__ void k_move_pack_rec(int64_t R, const int *__restrict__ link, const unsigned *__restrict__ zmask,
-                                const int *__restrict__ ent_dest, unsigned char *__restrict__ rec_owned,
-                                unsigned long long *__restrict__ cursor, int *__restrict__ buf) {
-  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= R || !rec_owned[r]) return;
-  const int d = ent_dest[link[r]];
-  if (d < 0) return;
-  const unsigned long long slot = atomicAdd(&cursor[d], 1ull);
-  int *m = buf + slot * 3;
-  m[0] = (int)r; m[1] = link[r]; m[2] = (int)zmask[r];
-  rec_owned[r] = 0;
-}
-__global__ void k_unpack_ent(int64_t n, int A, const int *__restrict__ buf, const AttrDev *__restrict__ attrs,
-                             TreeDev tree, int *__restrict__ y, double *__restrict__ entN, int *__restrict__ blk,
-                             unsigned char *__restrict__ ent_owned) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int *m = buf + i * (A + 1);
-  const int64_t e = m[0];
-  double nn = 1.0;
-  for (int a = 0; a < A; ++a) {
-    const int v = m[1 + a];
-    y[e * A + a] = v;
-    if (!attrs[a].is_const) nn = nn * attrs[a].norm[v];
-  }
-  entN[e] = nn;
-  blk[e] = tree.n_nodes > 0 ? tree_leaf(tree, m + 1) : 0;
-  ent_owned[e] = 1;
-}
-__global__ void k_unpack_rec(int64_t n, const int *__restrict__ buf, int *__restrict__ link,
-                             unsigned *__restrict__ zmask, unsigned char *__restrict__ rec_owned) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int *m = buf + i * 3;
-  const int64_t r = m[0];
-  link[r] = m[1];
-  zmask[r] = (unsigned)m[2];
-  rec_owned[r] = 1;
 }
 
 // ---- read-out of a sharded state --------------------------------------------------------------------------
@@ -1376,8 +1314,9 @@ struct dbl_ctx {
   std::vector<int> owner_h;  // P entries; default: everything owned by this rank
   DevBuf<int> owner, ent_dest, ent_key, link_key;
   DevBuf<unsigned char> ent_owned, rec_owned;
-  DevBuf<unsigned long long> move_cnt;  // host-mediated exchange: [2*world] counts then [2*world] cursors
-  std::vector<int64_t> h_move_ent, h_move_rec;
+  // host-mediated exchange: [world] cursor pairs of the sent messages, then the pair of received counts
+  DevBuf<unsigned long long> move_cnt;
+  std::vector<int64_t> h_move_ent, h_move_rec;  // messages per destination, from the block histograms
   bool in_sweep = false, in_block_sweep = false;
   int block_sampler = 0;
   std::vector<char> block_done;
@@ -1388,6 +1327,8 @@ struct dbl_ctx {
   DevBuf<unsigned char> comm_buf;
   size_t comm_bytes = 0;
   CommDev comm{};
+  MsgOut p2p_out{};  // the mapped receive buffers and cursors (dbl_comm_import)
+  MsgIn p2p_in{};
   bool comm_ready = false;
   std::vector<void *> ipc_opened;
   DevBuf<int> lpt_scratch;
@@ -1783,7 +1724,7 @@ static int alloc_state(dbl_ctx *ctx, int64_t R, int64_t E) {
   CUDA_TRY(ctx->ent_dest.alloc(E));
   CUDA_TRY(ctx->ent_key.alloc(E));
   CUDA_TRY(ctx->link_key.alloc(R));
-  CUDA_TRY(ctx->move_cnt.alloc(4 * (size_t)ctx->world));
+  CUDA_TRY(ctx->move_cnt.alloc(2 * (size_t)ctx->world + 2));
   const int64_t M = std::max(R, E);
   CUDA_TRY(ctx->iota.alloc(M));
   k_iota<<<grid_for(M, 256), 256, 0, ctx->stream>>>(M, ctx->iota.p);
@@ -2504,23 +2445,35 @@ static int update_owned(dbl_ctx *ctx, int sampler) {
   return refresh_summary(ctx, true);
 }
 
-// (5) the shuffle (GU:144) + the global summary (SummaryAccumulators.scala:54-63), peer to peer
-static int exchange_p2p(dbl_ctx *ctx) {
+// the messages of the clusters whose new block belongs to another rank, written through `out` by the rank that owned
+// them and applied from `in` by the one that receives them (either transport).  max_*: the most messages `in` can hold.
+static void launch_move(dbl_ctx *ctx, const MsgOut &out) {
   MoveParams mp;
-  mp.c = ctx->comm; mp.ctl = ctx->ctl(); mp.A = ctx->A; mp.ent_sorted = ctx->ent_sorted.p; mp.rec_sorted = ctx->rec_sorted.p;
+  mp.rank = ctx->rank; mp.out = out; mp.ctl = ctx->ctl(); mp.A = ctx->A;
+  mp.ent_sorted = ctx->ent_sorted.p; mp.rec_sorted = ctx->rec_sorted.p;
   mp.blk = ctx->blk.p; mp.owner = ctx->owner.p; mp.link = ctx->link.p; mp.y = ctx->y.p; mp.zmask = ctx->zmask.p;
   mp.ent_dest = ctx->ent_dest.p; mp.ent_owned = ctx->ent_owned.p; mp.rec_owned = ctx->rec_owned.p;
   k_move_ent<<<grid_rows(ctx, ctx->E, 256), 256, 0, ctx->stream>>>(mp);
   k_move_rec<<<grid_rows(ctx, ctx->R, 256), 256, 0, ctx->stream>>>(mp);
-  k_publish_barrier<<<1, 256, 0, ctx->stream>>>(ctx->comm, ctx->ctl(), ctx->part(), ctx->nw, ctx->barrier_timeout_cycles);
+  ctx->launches += 2;
+}
+static void launch_unpack(dbl_ctx *ctx, const MsgIn &in, int64_t max_ent, int64_t max_rec) {
   UnpackParams up;
-  up.c = ctx->comm; up.ctl = ctx->ctl(); up.A = ctx->A; up.attrs = ctx->attrs.p; up.tree = ctx->tree; up.y = ctx->y.p;
+  up.in = in; up.ctl = ctx->ctl(); up.A = ctx->A; up.attrs = ctx->attrs.p; up.tree = ctx->tree; up.y = ctx->y.p;
   up.blk = ctx->blk.p; up.link = ctx->link.p; up.entN = ctx->entN.p; up.zmask = ctx->zmask.p;
   up.ent_owned = ctx->ent_owned.p; up.rec_owned = ctx->rec_owned.p;
-  k_unpack_ent_p2p<<<grid_rows(ctx, ctx->E, 256), 256, 0, ctx->stream>>>(up);
-  k_unpack_rec_p2p<<<grid_rows(ctx, ctx->R, 256), 256, 0, ctx->stream>>>(up);
+  k_unpack_ent<<<grid_rows(ctx, max_ent, 256), 256, 0, ctx->stream>>>(up);
+  k_unpack_rec<<<grid_rows(ctx, max_rec, 256), 256, 0, ctx->stream>>>(up);
+  ctx->launches += 2;
+}
+
+// (5) the shuffle (GU:144) + the global summary (SummaryAccumulators.scala:54-63), peer to peer
+static int exchange_p2p(dbl_ctx *ctx) {
+  launch_move(ctx, ctx->p2p_out);
+  k_publish_barrier<<<1, 256, 0, ctx->stream>>>(ctx->comm, ctx->ctl(), ctx->part(), ctx->nw, ctx->barrier_timeout_cycles);
+  launch_unpack(ctx, ctx->p2p_in, ctx->E, ctx->R);
   k_reduce_peers<<<1, 256, 0, ctx->stream>>>(ctx->comm, ctx->ctl(), ctx->nw, ctx->ll_slot(), ctx->glob());
-  ctx->launches += 6;
+  ctx->launches += 2;
   if (ctx->rebalance_period > 0 && ctx->P <= 1024) {
     k_lpt<<<1, 32, 0, ctx->stream>>>(ctx->P, ctx->world, ctx->blk_ent_slot(), ctx->blk_rec_slot(), ctx->glob(), ctx->ctl(),
                                      ctx->rebalance_period, ctx->rebalance_threshold, ctx->owner.p, ctx->lpt_scratch.p,
@@ -2794,7 +2747,7 @@ static int preload_kernels(dbl_ctx *ctx) {
 #define DBL_LOAD(k) CUDA_TRY(cudaFuncGetAttributes(&fa, k))
   DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_tiles); DBL_LOAD(k_build_qtiles); DBL_LOAD(k_values<VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
   DBL_LOAD(k_reduce_local); DBL_LOAD(k_finish); DBL_LOAD(k_move_ent); DBL_LOAD(k_move_rec); DBL_LOAD(k_publish_barrier);
-  DBL_LOAD(k_unpack_ent_p2p); DBL_LOAD(k_unpack_rec_p2p); DBL_LOAD(k_reduce_peers); DBL_LOAD(k_lpt);
+  DBL_LOAD(k_unpack_ent); DBL_LOAD(k_unpack_rec); DBL_LOAD(k_reduce_peers); DBL_LOAD(k_lpt);
   DBL_LOAD(k_link_generic); DBL_LOAD(k_link_match); DBL_LOAD(k_link_pruned); DBL_LOAD(k_state_hash);
   DBL_LOAD(k_gather_ent); DBL_LOAD(k_gather_rec); DBL_LOAD(k_export_ent); DBL_LOAD(k_export_rec);
   DBL_LOAD(k_inv_ids<unsigned>); DBL_LOAD(k_inv_ids<unsigned long long>); DBL_LOAD(k_inv_value_ptr32);
@@ -2892,6 +2845,17 @@ extern "C" int dbl_comm_import(dbl_ctx *ctx, const void *blobs, int32_t world) {
       ctx->comm.base[r] = static_cast<unsigned char *>(p);
     }
   }
+  const CommDev &c = ctx->comm;
+  for (int par = 0; par < 2; ++par) {
+    for (int d = 0; d < world; ++d) {
+      ctx->p2p_out.ent[d][par] = c.recv_ent(d, par);
+      ctx->p2p_out.rec[d][par] = c.recv_rec(d, par);
+      ctx->p2p_out.cursor[d][par] = c.cursor(d, par);
+    }
+    ctx->p2p_in.ent[par] = c.recv_ent(ctx->rank, par);
+    ctx->p2p_in.rec[par] = c.recv_rec(ctx->rank, par);
+    ctx->p2p_in.count[par] = c.cursor(ctx->rank, par);
+  }
   ctx->drop_graphs();
   if (ctx->has_state) { int rc = preload_kernels(ctx); if (rc) return rc; }
   ctx->comm_ready = true;
@@ -2920,24 +2884,22 @@ extern "C" int dbl_sweep_begin(dbl_ctx *ctx, int sampler, int64_t *ent_counts, i
   rc = update_owned(ctx, sampler);
   if (rc) return rc;
   const int W = ctx->world;
-  CUDA_TRY(cudaMemsetAsync(ctx->move_cnt.p, 0, sizeof(unsigned long long) * 4 * W, ctx->stream));
-  k_move_count_ent<<<grid_for(ctx->E, 256), 256, 0, ctx->stream>>>(ctx->E, ctx->blk.p, ctx->owner.p, ctx->rank,
-                                                                  ctx->ent_owned.p, ctx->ent_dest.p, ctx->move_cnt.p);
-  k_move_count_rec<<<grid_for(ctx->R, 256), 256, 0, ctx->stream>>>(ctx->R, ctx->link.p, ctx->rec_owned.p,
-                                                                  ctx->ent_dest.p, ctx->move_cnt.p + W);
-  ctx->launches += 2;
-  std::vector<unsigned long long> h(2 * W);
-  CUDA_TRY(cudaMemcpyAsync(h.data(), ctx->move_cnt.p, sizeof(unsigned long long) * 2 * W, cudaMemcpyDeviceToHost, ctx->stream));
+  std::vector<int> owner(ctx->P);  // the device's table: dbl_set_block_owners(ctx, NULL) does not update owner_h
+  CUDA_TRY(cudaMemcpyAsync(owner.data(), ctx->owner.p, sizeof(int) * ctx->P, cudaMemcpyDeviceToHost, ctx->stream));
   rc = snapshot(ctx);  // also the partial summary of the shard (dbl_partial_summary) and the sweep's status
+  // messages to rank d = the owned entities / records whose new block d owns: the block histograms of the summary.
+  // An abandoned sweep sends nothing, but the caller still runs the collective calls of the sweep.
   ctx->h_move_ent.assign(W, 0);
   ctx->h_move_rec.assign(W, 0);
-  for (int d = 0; d < W; ++d) {
-    ent_counts[d] = ctx->h_move_ent[d] = (int64_t)h[d];
-    rec_counts[d] = ctx->h_move_rec[d] = (int64_t)h[W + d];
+  if (!rc) {
+    for (int b = 0; b < ctx->P; ++b) {
+      const int d = owner[b];
+      if (d == ctx->rank) continue;
+      ctx->h_move_ent[d] += ctx->h_part()[ctx->blk_ent_slot() + b];
+      ctx->h_move_rec[d] += ctx->h_part()[ctx->blk_rec_slot() + b];
+    }
   }
-  if (rc) {  // abandoned: nothing leaves this rank, but the caller still runs the collective calls of the sweep
-    for (int d = 0; d < W; ++d) ent_counts[d] = rec_counts[d] = ctx->h_move_ent[d] = ctx->h_move_rec[d] = 0;
-  }
+  for (int d = 0; d < W; ++d) { ent_counts[d] = ctx->h_move_ent[d]; rec_counts[d] = ctx->h_move_rec[d]; }
   ctx->in_sweep = true;
   return rc;
 }
@@ -2948,26 +2910,38 @@ extern "C" int dbl_exchange_pack(dbl_ctx *ctx, void *ent_buf_dev, void *rec_buf_
   if (!ctx->in_sweep) { ctx->set_error("dbl_exchange_pack outside a sweep"); return DBL_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(ctx->device));
   const int W = ctx->world;
-  std::vector<unsigned long long> cur(2 * W);
-  unsigned long long oe = 0, orc = 0;
-  for (int d = 0; d < W; ++d) { cur[d] = oe; oe += ctx->h_move_ent[d]; cur[W + d] = orc; orc += ctx->h_move_rec[d]; }
-  CUDA_TRY(cudaMemcpyAsync(ctx->move_cnt.p + 2 * W, cur.data(), sizeof(unsigned long long) * 2 * W, cudaMemcpyHostToDevice,
-                           ctx->stream));
-  if (orc > 0) {
-    if (!rec_buf_dev) return DBL_ERR_INVALID;
-    k_move_pack_rec<<<grid_for(ctx->R, 256), 256, 0, ctx->stream>>>(ctx->R, ctx->link.p, ctx->zmask.p, ctx->ent_dest.p,
-                                                                   ctx->rec_owned.p, ctx->move_cnt.p + 3 * W,
-                                                                   (int *)rec_buf_dev);
+  int64_t oe = 0, orc = 0;
+  for (int d = 0; d < W; ++d) { oe += ctx->h_move_ent[d]; orc += ctx->h_move_rec[d]; }
+  if ((oe > 0 && !ent_buf_dev) || (orc > 0 && !rec_buf_dev)) return DBL_ERR_INVALID;
+  if (oe + orc == 0) return DBL_OK;  // also every abandoned sweep: nothing may leave this rank
+  // rank d's messages follow those of the ranks before it; the cursors are this context's
+  MsgOut out{};
+  oe = orc = 0;
+  for (int d = 0; d < W; ++d) {
+    for (int par = 0; par < 2; ++par) {
+      out.ent[d][par] = static_cast<int *>(ent_buf_dev) + oe * (ctx->A + 1);
+      out.rec[d][par] = static_cast<int *>(rec_buf_dev) + orc * 3;
+      out.cursor[d][par] = ctx->move_cnt.p + 2 * d;
+    }
+    oe += ctx->h_move_ent[d];
+    orc += ctx->h_move_rec[d];
   }
-  if (oe > 0) {
-    if (!ent_buf_dev) return DBL_ERR_INVALID;
-    k_move_pack_ent<<<grid_for(ctx->E, 256), 256, 0, ctx->stream>>>(ctx->E, ctx->A, ctx->y.p, ctx->ent_dest.p,
-                                                                   ctx->ent_owned.p, ctx->move_cnt.p + 2 * W,
-                                                                   (int *)ent_buf_dev);
-  }
-  ctx->launches += 2;
+  CUDA_TRY(cudaMemsetAsync(ctx->move_cnt.p, 0, sizeof(unsigned long long) * 2 * W, ctx->stream));
+  launch_move(ctx, out);
   CUDA_TRY(cudaGetLastError());
+  std::vector<unsigned long long> cur(2 * W);
+  CUDA_TRY(cudaMemcpyAsync(cur.data(), ctx->move_cnt.p, sizeof(unsigned long long) * 2 * W, cudaMemcpyDeviceToHost,
+                           ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // the host moves the buffers with NCCL on its own stream
+  // the buffers were sized by the counts of dbl_sweep_begin: the messages written must be exactly those
+  for (int d = 0; d < W; ++d)
+    if ((int64_t)cur[2 * d] != ctx->h_move_ent[d] || (int64_t)cur[2 * d + 1] != ctx->h_move_rec[d]) {
+      ctx->has_state = false;
+      ctx->set_error("dbl_exchange_pack: " + std::to_string(cur[2 * d]) + " entity / " + std::to_string(cur[2 * d + 1]) +
+                     " record messages for rank " + std::to_string(d) + ", but dbl_sweep_begin counted " +
+                     std::to_string(ctx->h_move_ent[d]) + " / " + std::to_string(ctx->h_move_rec[d]));
+      return DBL_ERR_STATE;
+    }
   return DBL_OK;
 }
 
@@ -2976,15 +2950,16 @@ extern "C" int dbl_exchange_unpack(dbl_ctx *ctx, const void *ent_buf_dev, int64_
   if (!ctx || n_ent < 0 || n_rec < 0) return DBL_ERR_INVALID;
   if (int rc1 = one_chain_only(ctx, "dbl_exchange_unpack")) return rc1;
   if (!ctx->in_sweep) { ctx->set_error("dbl_exchange_unpack outside a sweep"); return DBL_ERR_STATE; }
+  if ((n_ent > 0 && !ent_buf_dev) || (n_rec > 0 && !rec_buf_dev)) return DBL_ERR_INVALID;
+  if (n_ent + n_rec == 0) return DBL_OK;
   CUDA_TRY(cudaSetDevice(ctx->device));
-  if (n_ent > 0)
-    k_unpack_ent<<<grid_for(n_ent, 256), 256, 0, ctx->stream>>>(n_ent, ctx->A, (const int *)ent_buf_dev, ctx->attrs.p,
-                                                                ctx->tree, ctx->y.p, ctx->entN.p, ctx->blk.p,
-                                                                ctx->ent_owned.p);
-  if (n_rec > 0)
-    k_unpack_rec<<<grid_for(n_rec, 256), 256, 0, ctx->stream>>>(n_rec, (const int *)rec_buf_dev, ctx->link.p,
-                                                                ctx->zmask.p, ctx->rec_owned.p);
-  ctx->launches += 2;
+  unsigned long long *count = ctx->move_cnt.p + 2 * ctx->world;
+  const unsigned long long n[2] = {(unsigned long long)n_ent, (unsigned long long)n_rec};  // staging: alive until the sync
+  CUDA_TRY(cudaMemcpyAsync(count, n, sizeof(n), cudaMemcpyHostToDevice, ctx->stream));
+  const MsgIn in{{static_cast<const int *>(ent_buf_dev), static_cast<const int *>(ent_buf_dev)},
+                 {static_cast<const int *>(rec_buf_dev), static_cast<const int *>(rec_buf_dev)},
+                 {count, count}};
+  launch_unpack(ctx, in, n_ent, n_rec);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return DBL_OK;
