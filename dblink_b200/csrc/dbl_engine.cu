@@ -22,6 +22,7 @@
 #include <cstring>
 #include <cub/cub.cuh>
 #include <map>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -308,7 +309,7 @@ __global__ void k_block_scan(int P, const int *__restrict__ ent_ptr, const int *
     if (finish && !dead) ctl[CTL_ITER] += 1;
   }
 }
-// Tiled, block-sorted copies of the entity table, one thread per tile slot (padding slots of a block's last tile are
+// The tiled, block-sorted copy of the entity table, one thread per tile slot (padding slots of a block's last tile are
 // zeroed here: no memset of the whole table).
 struct TileSrc {
   int64_t n_slots;
@@ -332,24 +333,14 @@ struct TileSrc {
     return true;
   }
 };
-// attribute-major tiles { int32 y[A][TE]; f64 N[TE] } (k_link_generic / k_link_match / k_link_pruned)
-__global__ void k_build_tiles(TileSrc s, int *__restrict__ tiles) {
+// tiles of format f, NS non-constant attributes
+__global__ void k_build_entity_tiles(TileSrc s, Pcg2Format f, int NS, const AttrDev *__restrict__ attrs,
+                                     int *__restrict__ tiles) {
   int T, slot;
   const int *yrow;
   double N;
   if (!s.at((int64_t)blockIdx.x * blockDim.x + threadIdx.x, T, slot, yrow, N)) return;
-  int *tile = tiles + (size_t)T * tile_words(s.A);
-  for (int k = 0; k < s.A; ++k) tile[k * TE + slot] = yrow ? yrow[s.perm[k]] : 0;  // kernel order
-  reinterpret_cast<double *>(tile + (size_t)s.A * TE)[slot] = N;
-}
-// quad tiles of format f (k_link_pcg2), NS non-constant attributes
-__global__ void k_build_qtiles(TileSrc s, Pcg2Format f, int NS, const AttrDev *__restrict__ attrs,
-                               int *__restrict__ qtiles) {
-  int T, slot;
-  const int *yrow;
-  double N;
-  if (!s.at((int64_t)blockIdx.x * blockDim.x + threadIdx.x, T, slot, yrow, N)) return;
-  pcg2_store(f, s.A, NS, yrow, s.perm, attrs, qtiles + (size_t)T * f.words(s.A, NS) * TE, slot, N);
+  pcg2_store(f, s.A, NS, yrow, s.perm, attrs, tiles + (size_t)T * f.layout(s.A, NS).words(), slot, N);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1339,9 +1330,9 @@ struct dbl_ctx {
 
   // layout
   DevBuf<int> iota, blk_sorted, ent_sorted, rec_key, rec_key_sorted, rec_sorted;
-  DevBuf<int> ent_ptr, tile_ptr, rec_ptr, cta_ptr, cta_ptr2, cta_ptr3, tiles, qtiles;
+  DevBuf<int> ent_ptr, tile_ptr, rec_ptr, cta_ptr, cta_ptr2, cta_ptr3, tiles;
   DevBuf<double> lane_sums;  // k_link_pcg2 scratch: pass-1 lane sums per chunk of every resident warp
-  bool tiles_valid[2] = {false, false};  // attribute-major / quad tiles match the current layout
+  std::optional<Pcg2Format> tiles_fmt;  // the format `tiles` holds for the current layout; none: not built
   // inverted index of the block tables for the pruned PCG-I link kernel (built on demand, once per sweep): E * A ids,
   // unsigned or (inv_ids64) unsigned long long, with their candidate positions
   DevBuf<unsigned char> inv_ids_in, inv_ids;
@@ -1678,14 +1669,14 @@ static int alloc_blocks(dbl_ctx *ctx) {
   CUDA_TRY(ctx->cta_ptr3.alloc(P + 1));
   CUDA_TRY(ctx->lpt_scratch.alloc(2 * (size_t)P));
   CUDA_TRY(ctx->lpt_dscratch.alloc((size_t)P + MAX_WORLD));
+  // sized for the unpacked format: a packed one needs a constant attribute, so it has no more words per entity
   const size_t max_tiles = (size_t)(ctx->E / TE) + (size_t)P + 1;
-  CUDA_TRY(ctx->tiles.alloc(max_tiles * tile_words(ctx->A)));
+  CUDA_TRY(ctx->tiles.alloc(max_tiles * TileLayout::of(ctx->A).words()));
   // work item and grid of the persistent PCG-II kernel for this model shape (see Pcg2Format::rpw)
   ctx->pcg2_recs = LINK_WARPS * ctx->pcg2_fmt.rpw(ctx->n_str);
   ctx->pcg2_grid = ctx->sm_count * ctx->pcg2_fmt.ctas_per_sm(ctx->n_str);
   const size_t need = (size_t)ctx->pcg2_grid * ctx->pcg2_recs * 1024;
   if (ctx->lane_sums.n < need) CUDA_TRY(ctx->lane_sums.alloc(need));
-  CUDA_TRY(ctx->qtiles.alloc(max_tiles * ctx->pcg2_fmt.words(ctx->A, ctx->n_str) * TE));
   ctx->max_ctas = (int)((ctx->R + LINK_WARPS - 1) / LINK_WARPS) + P;
   return alloc_control(ctx);
 }
@@ -1783,7 +1774,7 @@ static int build_links_csr(dbl_ctx *ctx, bool commit_newlinks = false) {
   return DBL_OK;
 }
 
-// group entities and records by block (replaces the shuffle, GU:144); the tiled copies of the entity table are built
+// group entities and records by block (replaces the shuffle, GU:144); the tiled copy of the entity table is built
 // on demand by ensure_tiles().  end_of_sweep: this is the last step of a sweep -- the scan kernel also adopts the
 // partial summary as the global one (single rank) and counts the sweep.
 static int relayout(dbl_ctx *ctx, bool end_of_sweep = false) {
@@ -1808,24 +1799,22 @@ static int relayout(dbl_ctx *ctx, bool end_of_sweep = false) {
                                            end_of_sweep ? 1 : 0);
   ctx->launches += 9;
   ctx->inv_valid = false;
-  ctx->tiles_valid[0] = ctx->tiles_valid[1] = false;
+  ctx->tiles_fmt.reset();
   ctx->h_owned_ent = ctx->h_owned_rec = -1;  // changed on the device; snapshot() brings them back
   CUDA_TRY(cudaGetLastError());
   return DBL_OK;
 }
 
-// tiled copy of the block-sorted entity table in the format the coming link kernel reads (1: attribute-major, 2: quad)
-static int ensure_tiles(dbl_ctx *ctx, int fmt) {
-  if (ctx->tiles_valid[fmt - 1]) return DBL_OK;
+// tiled copy of the block-sorted entity table in format f, the one the coming link kernel reads; one buffer for
+// every format, rebuilt when it holds another
+static int ensure_tiles(dbl_ctx *ctx, Pcg2Format f) {
+  if (ctx->tiles_fmt == f) return DBL_OK;
   const int64_t n_slots = (int64_t)((size_t)(ctx->E / TE) + (size_t)ctx->P + 1) * TE;
   const TileSrc s{n_slots, ctx->A, ctx->P, ctx->y.p, ctx->ent_sorted.p, ctx->ent_ptr.p, ctx->tile_ptr.p,
                   ctx->perm_dev.p, ctx->entN.p};
-  if (fmt == 1) k_build_tiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(s, ctx->tiles.p);
-  else
-    k_build_qtiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(s, ctx->pcg2_fmt, ctx->n_str, ctx->attrs.p,
-                                                                    ctx->qtiles.p);
+  k_build_entity_tiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(s, f, ctx->n_str, ctx->attrs.p, ctx->tiles.p);
   ctx->launches += 1;
-  ctx->tiles_valid[fmt - 1] = true;
+  ctx->tiles_fmt = f;
   CUDA_TRY(cudaGetLastError());
   return DBL_OK;
 }
@@ -2332,7 +2321,6 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
   lp.theta = ctx->theta(); lp.ent_ptr = ctx->ent_ptr.p; lp.tile_ptr = ctx->tile_ptr.p; lp.rec_ptr = ctx->rec_ptr.p;
   lp.cta_ptr = ctx->cta_ptr.p; lp.ent_sorted = ctx->ent_sorted.p; lp.rec_sorted = ctx->rec_sorted.p;
   lp.tiles = ctx->tiles.p; lp.newlink = ctx->newlink.p;
-  lp.qtiles = ctx->qtiles.p;
   lp.work = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_WORK);
   lp.lane_sums = ctx->lane_sums.p;
   lp.status = reinterpret_cast<unsigned long long *>(ctx->ctl() + CTL_STATUS);
@@ -2353,13 +2341,13 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
     // persistent CTAs: a few per SM, each takes groups of LINK_WARPS records from the work counter until none is left
     // (k_theta zeroed the counter; the block-level API launches the kernel once per block after one k_theta)
     if (ctx->in_block_sweep) CUDA_TRY(cudaMemsetAsync(lp.work, 0, sizeof(unsigned long long), ctx->stream));
-    int rc = ensure_tiles(ctx, 2);
+    int rc = ensure_tiles(ctx, ctx->pcg2_fmt);
     if (rc) return rc;
     lp.cta_ptr = ctx->cta_ptr3.p;  // work items of PCG2_RECS records
     return dispatch_pcg2(ctx, &lp, std::min(ctx->max_ctas, ctx->pcg2_grid));
   }
   {
-    int rc = ensure_tiles(ctx, 1);  // every other link kernel reads the attribute-major tiles
+    int rc = ensure_tiles(ctx, Pcg2Format{});  // every other link kernel reads the unpacked format
     if (rc) return rc;
   }
   if (kernel == LINK_PRUNED) {  // pruned scoring through the inverted index
@@ -2388,7 +2376,7 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
     return DBL_OK;
   }
   if (kernel == LINK_MATCH) {
-    const size_t ring = (size_t)LINK_STAGES * tile_words(A) * 4 + 128;  // the tile ring of k_link_match
+    const size_t ring = (size_t)LINK_STAGES * TileLayout::of(A).words() * 4 + 128;  // the tile ring of k_link_match
     if (ctx->match_smem_cfg < ring) {
       CUDA_TRY(cudaFuncSetAttribute(k_link_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring));
       ctx->match_smem_cfg = ring;
@@ -2745,7 +2733,7 @@ extern "C" int dbl_set_rebalance(dbl_ctx *ctx, int32_t period, double threshold)
 static int preload_kernels(dbl_ctx *ctx) {
   cudaFuncAttributes fa;
 #define DBL_LOAD(k) CUDA_TRY(cudaFuncGetAttributes(&fa, k))
-  DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_tiles); DBL_LOAD(k_build_qtiles); DBL_LOAD(k_values<VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
+  DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_entity_tiles); DBL_LOAD(k_values<VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
   DBL_LOAD(k_reduce_local); DBL_LOAD(k_finish); DBL_LOAD(k_move_ent); DBL_LOAD(k_move_rec); DBL_LOAD(k_publish_barrier);
   DBL_LOAD(k_unpack_ent); DBL_LOAD(k_unpack_rec); DBL_LOAD(k_reduce_peers); DBL_LOAD(k_lpt);
   DBL_LOAD(k_link_generic); DBL_LOAD(k_link_match); DBL_LOAD(k_link_pruned); DBL_LOAD(k_state_hash);

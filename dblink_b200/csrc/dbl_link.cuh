@@ -11,6 +11,8 @@
 //   k_link_match    PCG-I / Gibbs: same tile pipeline; candidates must agree on every observed non-distorted
 //                   attribute, checked most-selective-first with a warp-wide early out.
 //   k_link_generic  any A <= 32 / any row length; tiles read through L1/L2.  Fallback only.
+// Every link kernel reads the same entity tiles (TileLayout); k_link_pcg2 reads the format its model gets
+// (Pcg2Format), the others the unpacked one.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -25,8 +27,21 @@ constexpr int LINK_STAGES = 4;   // tile ring depth
 constexpr int LINK_MAX_UNROLL_A = 16;
 constexpr unsigned FULL = 0xffffffffu;
 
-// int32 words per tile: A value rows (attribute-major), then the f64 row N(e)
-__host__ __device__ inline size_t tile_words(int A) { return (size_t)A * TE + 2 * TE; }
+// Entity tiles: the block-sorted entity table in tiles of TE entities.  The words of one entity sit in groups of
+// four, group-major ([group][slot][4] int32), so that a lane fetches a group with one 128-bit load (one conflict-free
+// load per lane in shared memory); the f64 row N(e) follows the groups (8 contiguous bytes per lane: a 64-bit load of
+// a word pair inside a 16-byte group would cost twice the wavefronts).  What the words hold is the tile format's
+// (Pcg2Format::nv); the unpacked format holds the A value ids in kernel order, zero padded to a whole group.
+struct TileLayout {
+  int ng;  // groups of four words per entity
+  __host__ __device__ static constexpr TileLayout of(int nv) { return {(nv + 3) / 4}; }  // nv words per entity
+  __host__ __device__ constexpr int entity_words() const { return ng * 4 + 2; }
+  __host__ __device__ constexpr int words() const { return entity_words() * TE; }  // int32 words per tile
+  // int4 index of group g of slot `slot`; int32 index of word w of slot `slot`
+  __host__ __device__ static constexpr int group(int g, int slot) { return g * TE + slot; }
+  __host__ __device__ static constexpr int word(int w, int slot) { return group(w >> 2, slot) * 4 + (w & 3); }
+  __host__ __device__ constexpr int n_word() const { return ng * 4 * TE; }  // int32 index where the row N starts
+};
 
 struct AttrDev {
   int V, is_const, kmax, hsize;
@@ -88,8 +103,7 @@ struct LinkParams {
   const unsigned *zmask;
   const double *theta;
   const int *ent_ptr, *tile_ptr, *rec_ptr, *cta_ptr, *ent_sorted, *rec_sorted;
-  const int *tiles;
-  const int *qtiles;         // quad tiles (k_link_pcg2)
+  const int *tiles;          // entity tiles (TileLayout) in the format the launched kernel reads
   unsigned long long *work;  // k_link_pcg2: next group of records to take (persistent CTAs); zeroed before the launch
   double *lane_sums;         // k_link_pcg2: scratch, [CTA][consumer warp][32 chunks][32 lanes] pass-1 lane sums
   int *newlink;
@@ -333,32 +347,34 @@ __device__ __forceinline__ bool rec_row_find(const RecAttr &c, int yv, double &e
   return false;
 }
 
-// protocol weight of one candidate; ycol points at attribute 0 of the candidate inside its tile (stride TE)
-__device__ __forceinline__ double generic_weight(const RecAttr *ra, int A, bool pcg2, const int *ycol, double N) {
+// protocol weight of the candidate in slot `slot` of an unpacked tile (A value ids in kernel order)
+__device__ __forceinline__ double generic_weight(const RecAttr *ra, int A, bool pcg2, const int *tile, int slot) {
+  const int *ys = tile + TileLayout::word(0, slot);  // word(a, slot) = word(0, slot) + word(a, 0): one live pointer
+  auto y = [&](int a) { return ys[TileLayout::word(a, 0)]; };
   double w;
   if (pcg2) {
     double c = 1.0;  // the constant attributes form their own product (a table look-up in k_link_pcg2)
     for (int a = 0; a < A; ++a)
-      if (ra[a].kind == 1 && ycol[a * TE] == ra[a].x) c = c * ra[a].rmatch;
-    w = N * c;
+      if (ra[a].kind == 1 && y(a) == ra[a].x) c = c * ra[a].rmatch;
+    w = reinterpret_cast<const double *>(tile + TileLayout::of(A).n_word())[slot] * c;  // N * c
     for (int a = 0; a < A; ++a) {  // non-constant attributes: one factor each, equal (multiplier) or similar (exp sim)
       if (ra[a].kind != 2) continue;
-      const int yv = ycol[a * TE];
+      const int yv = y(a);
       double e;
       if (yv == ra[a].x) w = w * ra[a].rmatch;
       else if (rec_row_find(ra[a], yv, e)) w = w * e;
     }
     for (int a = 0; a < A; ++a)
-      if (ra[a].kind == 3) w = w * ra[a].tab[ycol[a * TE]];
+      if (ra[a].kind == 3) w = w * ra[a].tab[y(a)];
   } else {
     for (int a = 0; a < A; ++a)
-      if (ra[a].kind == 4 && ycol[a * TE] != ra[a].x) return 0.0;
+      if (ra[a].kind == 4 && y(a) != ra[a].x) return 0.0;
     w = 1.0;
     for (int a = 0; a < A; ++a)
-      if (ra[a].kind == 2) w = w * ra[a].tab[ycol[a * TE]];
+      if (ra[a].kind == 2) w = w * ra[a].tab[y(a)];
     for (int a = 0; a < A; ++a) {
       double e;
-      if (ra[a].kind == 2 && rec_row_find(ra[a], ycol[a * TE], e)) w = w * e;
+      if (ra[a].kind == 2 && rec_row_find(ra[a], y(a), e)) w = w * e;
     }
   }
   return w;
@@ -393,14 +409,11 @@ __global__ void __launch_bounds__(LINK_WARPS * 32) k_link_generic(LinkParams p) 
   __syncwarp();
   const int n = p.ent_ptr[b + 1] - p.ent_ptr[b];
   const DrawGeom geo = draw_geom((n + TE - 1) / TE);
-  const size_t tw = tile_words(A);
+  const size_t tw = TileLayout::of(A).words();
   const int *tiles = p.tiles + (size_t)p.tile_ptr[b] * tw;
   auto wf = [&](int j) -> double {
     if (j >= n) return 0.0;
-    const int *tile = tiles + (size_t)(j / TE) * tw;
-    const int slot = j % TE;
-    const double N = reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot];
-    return generic_weight(ra, A, pcg2, tile + slot, N);
+    return generic_weight(ra, A, pcg2, tiles + (size_t)(j / TE) * tw, j % TE);
   };
   Checkpoints ck;
   double acc = 0.0;
@@ -470,7 +483,7 @@ __device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, un
 
 // Shared-memory ring of entity tiles filled by one producer warp; every consumer warp of the CTA reads every tile.
 struct TileRing {
-  int *tiles;          // LINK_STAGES * tile_words
+  int *tiles;          // LINK_STAGES tiles of tw words
   uint64_t *full;      // LINK_STAGES
   uint64_t *empty;     // LINK_STAGES
   int tw;              // words per tile
@@ -519,7 +532,7 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
   const int A = p.A;
   const int n = p.ent_ptr[b + 1] - p.ent_ptr[b];
   const int ntiles = p.tile_ptr[b + 1] - p.tile_ptr[b];
-  const int TW = (int)tile_words(A);
+  const int TW = TileLayout::of(A).words();
   TileRing rg;
   rg.tiles = reinterpret_cast<int *>(smem);
   rg.full = reinterpret_cast<uint64_t *>(smem + (size_t)LINK_STAGES * TW * 4);
@@ -560,7 +573,7 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
   const DrawGeom geo = draw_geom(ntiles);
   const int *mma = s_mm_attr[warp];
   const int *mmx = s_mm_x[warp];
-  const int off0 = nmm ? mma[0] * TE : 0;
+  const int a0 = nmm ? mma[0] : 0;
   const int x0 = nmm ? mmx[0] : 0;
 
   Checkpoints ck;
@@ -571,19 +584,18 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
     mbar_wait(&rg.full[s], (t / LINK_STAGES) & 1);
     if (active) {
       const int *tile = rg.tiles + (size_t)s * TW;
-      const double *tileN = reinterpret_cast<const double *>(tile + A * TE);
       const int valid = min(TE, n - t * TE);  // candidates in this tile (the last tile is zero padded)
 #pragma unroll
       for (int q = 0; q < TE / 32; ++q) {
         const int slot = q * 32 + lane;
         // the most selective must-match attribute decides almost every candidate: one load, one compare, one vote
-        bool ok = (slot < valid) && (nmm == 0 || tile[off0 + slot] == x0);
+        bool ok = (slot < valid) && (nmm == 0 || tile[TileLayout::word(a0, slot)] == x0);
         if (__any_sync(FULL, ok)) {
           for (int k = 1; k < nmm; ++k) {
-            ok = ok && (tile[mma[k] * TE + slot] == mmx[k]);
+            ok = ok && (tile[TileLayout::word(mma[k], slot)] == mmx[k]);
             if (!__any_sync(FULL, ok)) break;  // warp-uniform: nobody left after this attribute
           }
-          if (ok) acc = acc + generic_weight(ra, A, false, tile + slot, tileN[slot]);
+          if (ok) acc = acc + generic_weight(ra, A, false, tile, slot);
         }
       }
       if (++tile_in_chunk == geo.tpc || t + 1 == ntiles) {
@@ -598,9 +610,7 @@ __global__ void __launch_bounds__((MATCH_WARPS + 1) * 32) k_link_match(LinkParam
   if (!active || !check_mass(p, lane, r, ck.run)) return;
   auto wf = [&](int j) -> double {
     if (j >= n) return 0.0;
-    const int *tile = gtiles + (size_t)(j / TE) * TW;
-    const int slot = j % TE;
-    return generic_weight(ra, A, false, tile + slot, reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot]);
+    return generic_weight(ra, A, false, gtiles + (size_t)(j / TE) * TW, j % TE);
   };
   const U2 u = link_uniform(p, r);
   const int j = finish_draw(lane, n, geo, ck.Q, ck.run, u.u0, wf);
@@ -730,7 +740,7 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
   const int A = p.A;
   const int n = p.ent_ptr[b + 1] - p.ent_ptr[b];
   const int ntiles = p.tile_ptr[b + 1] - p.tile_ptr[b];
-  const size_t TW = tile_words(A);
+  const size_t TW = TileLayout::of(A).words();
   const int *gtiles = p.tiles + (size_t)p.tile_ptr[b] * TW;
   RecAttr *ra = s_ra[warp];
   int nmm = 0;
@@ -799,10 +809,10 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
     const int slot = j % TE;
     bool ok = true;
     for (int k = 0; k < nmm && ok; ++k)
-      if (mma[k] != best) ok = (tile[mma[k] * TE + slot] == mmx[k]);
+      if (mma[k] != best) ok = (tile[TileLayout::word(mma[k], slot)] == mmx[k]);
     if (!ok) return 0.0;
     if (!has_sim) return 1.0;  // GU:408-411: uniform over the candidates
-    return generic_weight(ra, A, false, tile + slot, reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot]);
+    return generic_weight(ra, A, false, tile, slot);
   };
 
   // ---- pass 1: lane sums per chunk from the survivors only
@@ -834,7 +844,7 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
       bool pass = false;
       if (idx < phi) {
         j = pp.inv_pos[idx];
-        pass = (gtiles[(size_t)(j / TE) * TW + a1 * TE + (j % TE)] == x1);
+        pass = (gtiles[(size_t)(j / TE) * TW + TileLayout::word(a1, j % TE)] == x1);
       }
       unsigned live = __ballot_sync(FULL, pass);
       while (live) {
@@ -844,10 +854,9 @@ __device__ __forceinline__ void pruned_record(const PrunedParams &pp, PrunedShar
         const int *tile = gtiles + (size_t)(ji / TE) * TW;
         const int slot = ji % TE;
         bool okl = true;
-        if (lane < nmm && mma[lane] != best) okl = (tile[mma[lane] * TE + slot] == mmx[lane]);
+        if (lane < nmm && mma[lane] != best) okl = (tile[TileLayout::word(mma[lane], slot)] == mmx[lane]);
         if (!__all_sync(FULL, okl)) continue;
-        const double wi = has_sim ? generic_weight(ra, A, false, tile + slot,
-                                                   reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot])
+        const double wi = has_sim ? generic_weight(ra, A, false, tile, slot)
                                   : 1.0;  // GU:408-411: uniform over the candidates
         if (wi > 0.0) add_survivor(ji, wi);
       }
@@ -963,7 +972,7 @@ __global__ void __launch_bounds__(HEAVY_WARPS * 32) k_link_heavy(PrunedParams pp
     const int b = pp.rec_key_sorted[ridx] >> pp.rec_key_shift;
     const int n = p.ent_ptr[b + 1] - p.ent_ptr[b];
     const int ntiles = p.tile_ptr[b + 1] - p.tile_ptr[b];
-    const size_t tw = tile_words(A);
+    const size_t tw = TileLayout::of(A).words();
     const int *tiles = p.tiles + (size_t)p.tile_ptr[b] * tw;
     __syncthreads();  // the previous record's tables and sums are no longer read
     if (warp == 0 && lane < A) {
@@ -975,9 +984,7 @@ __global__ void __launch_bounds__(HEAVY_WARPS * 32) k_link_heavy(PrunedParams pp
     const DrawGeom geo = draw_geom(ntiles);
     auto wf = [&](int j) -> double {
       if (j >= n) return 0.0;
-      const int *tile = tiles + (size_t)(j / TE) * tw;
-      const int slot = j % TE;
-      return generic_weight(s_ra, A, false, tile + slot, reinterpret_cast<const double *>(tile + (size_t)A * TE)[slot]);
+      return generic_weight(s_ra, A, false, tiles + (size_t)(j / TE) * tw, j % TE);
     };
     for (int c = warp; c < geo.nchunks; c += HEAVY_WARPS) {
       double acc = 0.0;

@@ -41,16 +41,15 @@ struct Pcg2Format {
   int hc;              // 32: the model's hash tables have 32 slots, a compile-time size; 0: p.hslots
   __host__ __device__ static constexpr int hc_of(int hslots) { return hslots == 32 ? 32 : 0; }
   bool pk, id16, sc;   // byte-packed constants; 16-bit non-constant values; slot codes in place of value ids
-  // "Quad tiles": the words a lane needs about ONE candidate sit in groups of four, group-major ([group][slot][4]
-  // int32), so that a warp fetches a group with one conflict-free 128-bit load per lane.  Words of an entity: nv
-  // values (pk: the NS non-constant values then the byte-packed constants; else all A values in kernel order) padded
-  // to a multiple of four; the f64 row N(e) follows the groups (8 contiguous bytes per lane: a 64-bit load of a word
-  // pair inside a 16-byte group would cost twice the wavefronts).  id16: the NS values are 16-bit, two per word
-  // (value 2i in the low half of word i), so A = 10 with 6 non-constant attributes needs one group instead of two.
-  // pcg2_store writes them, pcg2_load reads them.
+  // Words of an entity in the tiles (TileLayout): pk: the NS non-constant values then the byte-packed constants;
+  // else all A values in kernel order.  id16: the NS values are 16-bit, two per word (value 2i in the low half of
+  // word i), so A = 10 with 6 non-constant attributes needs one group instead of two.  pcg2_store writes them,
+  // pcg2_load reads them.
   __host__ __device__ constexpr int nv(int A, int NS) const { return pk ? (id16 ? (NS + 1) / 2 : NS) + 1 : A; }
-  __host__ __device__ constexpr int groups(int A, int NS) const { return (nv(A, NS) + 3) / 4; }
-  __host__ __device__ constexpr int words(int A, int NS) const { return groups(A, NS) * 4 + 2; }  // per entity
+  __host__ __device__ constexpr TileLayout layout(int A, int NS) const { return TileLayout::of(nv(A, NS)); }
+  __host__ __device__ constexpr bool operator==(Pcg2Format o) const {
+    return hc == o.hc && pk == o.pk && id16 == o.id16 && sc == o.sc;
+  }
   // Records per consumer warp.  With 2, a lane fetches its candidate once and scores it for both records: half the
   // tile loads and half the tile traffic through shared memory per (record, candidate) pair, two independent
   // dependency chains per warp; the price is registers (96 instead of 72: 2 CTAs per SM instead of 3) and twice the
@@ -133,18 +132,18 @@ __device__ __forceinline__ unsigned pcg2_const_offset(unsigned ypack, unsigned x
   return (eq * 0x00204081u) >> 25;
 }
 
-// One entity into slot `slot` of a quad tile of format f (pcg2_load reads it back).  y: the entity's values by
-// attribute id, nullptr for a padding slot (all zero); perm: kernel order.  Packed tiles: the non-constant values
-// (f.sc: their slot codes, AttrDev::pcode) at 32 or (f.id16) 16 bits, then the constants, one byte each.
+// One entity into slot `slot` of a tile of format f (pcg2_load reads it back).  y: the entity's values by attribute
+// id, nullptr for a padding slot (all zero); perm: kernel order.  Packed tiles: the non-constant values (f.sc: their
+// slot codes, AttrDev::pcode) at 32 or (f.id16) 16 bits, then the constants, one byte each.
 __device__ __forceinline__ void pcg2_store(Pcg2Format f, int A, int NS, const int *y, const int *perm,
                                            const AttrDev *attrs, int *tile, int slot, double N) {
-  const int ng = f.groups(A, NS);
+  const TileLayout tl = f.layout(A, NS);
   const int nid = f.id16 ? (NS + 1) / 2 : NS;  // words of non-constant values (packed tiles)
   auto ns_val = [&](int k) -> unsigned {       // value or slot code of kernel-order attribute k
     const int yv = y[perm[k]];
     return (unsigned)(f.sc ? attrs[perm[k]].pcode[yv] : yv);
   };
-  for (int g = 0; g < ng; ++g) {
+  for (int g = 0; g < tl.ng; ++g) {
     unsigned v[4] = {0u, 0u, 0u, 0u};
     for (int c = 0, w = 4 * g; c < 4 && y; ++c, ++w) {
       if (!f.pk) v[c] = w < A ? (unsigned)y[perm[w]] : 0u;
@@ -154,12 +153,12 @@ __device__ __forceinline__ void pcg2_store(Pcg2Format f, int A, int NS, const in
       else if (w == nid)
         for (int k = 0; k < A - NS; ++k) v[c] |= ((unsigned)y[perm[k]] & 0xFFu) << (8 * k);
     }
-    reinterpret_cast<int4 *>(tile)[(size_t)g * TE + slot] = make_int4(v[0], v[1], v[2], v[3]);
+    reinterpret_cast<int4 *>(tile)[TileLayout::group(g, slot)] = make_int4(v[0], v[1], v[2], v[3]);
   }
-  reinterpret_cast<double *>(tile + (size_t)ng * 4 * TE)[slot] = N;
+  reinterpret_cast<double *>(tile + tl.n_word())[slot] = N;
 }
 
-// one candidate out of a quad tile: values in kernel order (PK: only the non-constant ones + the packed word), N
+// one candidate out of a tile: values in kernel order (PK: only the non-constant ones + the packed word), N
 template <int A, int NS, bool PK>
 struct Pcg2Cand {
   int y[A];
@@ -170,12 +169,12 @@ struct Pcg2Cand {
 template <int A, int NS, bool PK, bool ID16>
 __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *tile, int slot) {
   static_assert(PK || !ID16, "16-bit values only in the packed tiles");
-  constexpr int NG = Pcg2Format{0, PK, ID16, false}.groups(A, NS);  // the layout depends on PK and ID16 only
-  int v[NG * 4];
+  constexpr TileLayout TL = Pcg2Format{0, PK, ID16, false}.layout(A, NS);  // the layout depends on PK and ID16 only
+  int v[TL.ng * 4];
   const int4 *q = reinterpret_cast<const int4 *>(tile);
 #pragma unroll
-  for (int g = 0; g < NG; ++g) {
-    const int4 t = q[g * TE + slot];
+  for (int g = 0; g < TL.ng; ++g) {
+    const int4 t = q[TileLayout::group(g, slot)];
     v[4 * g] = t.x; v[4 * g + 1] = t.y; v[4 * g + 2] = t.z; v[4 * g + 3] = t.w;
   }
   if constexpr (PK && ID16) {
@@ -193,7 +192,7 @@ __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *til
     for (int k = 0; k < A; ++k) c.y[k] = v[k];
     c.ypack = 0u;
   }
-  c.N = reinterpret_cast<const double *>(tile + NG * 4 * TE)[slot];
+  c.N = reinterpret_cast<const double *>(tile + TL.n_word())[slot];
 }
 
 // With skewed (Zipf-like) value frequencies some lane of the warp finds an equal or similar value on almost every
@@ -310,7 +309,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
   if (sweep_dead(p.ctl)) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr Pcg2Format FMT{HC, PK, ID16, SC};
-  constexpr int TW = FMT.words(A, NS) * TE;
+  constexpr int TW = FMT.layout(A, NS).words();
   constexpr int NC = A - NS;
   constexpr int RPW = FMT.rpw(NS);
   constexpr int WARPS = LINK_WARPS;           // consumer warps; warp WARPS is the producer
@@ -343,7 +342,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
     const int b = find_block(p, cta);
     const int n = p.ent_ptr[b + 1] - p.ent_ptr[b];
     const int ntiles = p.tile_ptr[b + 1] - p.tile_ptr[b];
-    const int *gtiles = p.qtiles + (size_t)p.tile_ptr[b] * TW;
+    const int *gtiles = p.tiles + (size_t)p.tile_ptr[b] * TW;
 
     if (warp == WARPS) {  // producer warp
       if (lane == 0) ring_produce<true>(rg, gtiles, ntiles, tbase);
@@ -526,7 +525,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
 
 // dynamic shared memory of one CTA (H = the table size of the model)
 inline size_t pcg2_smem_bytes(Pcg2Format f, int A, int NS, int H) {
-  return (size_t)LINK_STAGES * f.words(A, NS) * TE * 4 + 128 + (size_t)LINK_WARPS * pcg2_warp_tab_bytes(f, NS, H) +
+  return (size_t)LINK_STAGES * f.layout(A, NS).words() * 4 + 128 + (size_t)LINK_WARPS * pcg2_warp_tab_bytes(f, NS, H) +
          (size_t)LINK_WARPS * f.rpw(NS) * 16 * sizeof(double);
 }
 

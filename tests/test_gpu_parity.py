@@ -343,3 +343,34 @@ def test_pcg2_unpacked_constants_on_a_packable_model(oracle, monkeypatch):
         eng.sweep("PCG-II", 1)
         assert st.sweep(oracle.SAMPLERS["PCG-II"]) == 0
         assert_same_state(eng, st)
+
+
+def test_tile_formats_alternate_on_one_engine(oracle):
+    """One tile buffer serves every link kernel: k_link_pcg2 reads the packed slot-code format of this model,
+    k_link_pruned the unpacked one, so PCG-II and PCG-I sweeps on one engine overwrite each other's tiles.  Alternated
+    eagerly, through replayed graphs of several sweeps and block by block, they draw what the oracle draws."""
+    from dblink_b200 import synth
+
+    C = synth.SynthAttr
+    attrs = [C("c0", "constant", 5, 0.5), C("s0", "levenshtein", 40), C("c1", "constant", 9, 0.5),
+             C("s1", "levenshtein", 50), C("c2", "constant", 31, 0.5), C("s2", "levenshtein", 60)]
+    g = synth.generate(29, 900, attrs, dup=0.3, distortion=0.15, missing=0.08, n_files=2)
+    eng, rc, x, file = product_setup(g, 31, 1, (5,))
+    m, st, tree, ox, ofile = oracle_setup(oracle, g, 31, 1, (5,))
+    assert eng.link_kernel("PCG-II") == "k_link_pcg2<A=6,NS=3,HC=32,PK=1>"
+    assert eng.link_tile_format("PCG-II")["slot_codes"]
+    assert eng.link_kernel("PCG-I") == "k_link_pruned"
+    eng.set_link_mass_capture(True)
+    order = ("PCG-II", "PCG-I", "PCG-II")
+    for graph_mode, n in ((1, 1), (2, 3)):  # eager sweeps one by one; graphs forced on, several sweeps per call
+        eng.set_graph_mode(graph_mode)
+        for sampler in order:
+            eng.sweep(sampler, n)
+            assert st.sweep(oracle.SAMPLERS[sampler], n) == 0
+            assert_same_state(eng, st)
+            assert_same_mass(eng.link_mass(), st.last_link_mass(), f"graph mode {graph_mode}, {sampler}")
+    for sampler in order:
+        eng.sweep_by_block(sampler)
+        assert st.sweep(oracle.SAMPLERS[sampler]) == 0
+        assert_same_state(eng, st)
+    eng.close()
