@@ -119,6 +119,7 @@ SIGNATURES = {
     "dbl_link_mass": (C.c_int, [vp, f64p]),
     "dbl_index_hash_slots": (C.c_int32, [vp]),
     "dbl_index_slot_codes": (C.c_int, [vp, i32p]),
+    "dbl_index_pairs_on_device": (C.c_int32, [vp]),
     "dbl_set_graph_mode": (C.c_int, [vp, C.c_int]),
     "dbl_last_sweep_ms": (C.c_double, [vp]),
     "dbl_link_kernel_ms": (C.c_double, [vp, i64p]),

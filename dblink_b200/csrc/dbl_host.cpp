@@ -20,7 +20,39 @@
 // ---------------------------------------------------------------------------------------------------
 // SimilarityFn.scala:61-98
 // ---------------------------------------------------------------------------------------------------
-int host_levenshtein(const char *a, int la, const char *b, int lb) {
+// Strict UTF-8 (RFC 3629) to UTF-16 code units, the units a Java String holds: no overlong forms, no encoded
+// surrogates, nothing above U+10FFFF, no stray or missing continuation bytes.  The units are appended to out.
+// false = not valid UTF-8.
+bool host_utf8_to_utf16(const char *s, size_t n, std::u16string &out) {
+  const unsigned char *p = (const unsigned char *)s, *e = p + n;
+  while (p < e) {
+    uint32_t c = *p++;
+    int extra;
+    uint32_t lowest;
+    if (c < 0x80) { out.push_back((char16_t)c); continue; }
+    if (c >= 0xC2 && c <= 0xDF) { extra = 1; c &= 0x1F; lowest = 0x80; }
+    else if (c >= 0xE0 && c <= 0xEF) { extra = 2; c &= 0x0F; lowest = 0x800; }
+    else if (c >= 0xF0 && c <= 0xF4) { extra = 3; c &= 0x07; lowest = 0x10000; }
+    else return false;  // a continuation byte, C0 / C1 (always overlong) or F5..FF
+    if (e - p < extra) return false;
+    for (int k = 0; k < extra; ++k, ++p) {
+      if ((*p & 0xC0) != 0x80) return false;
+      c = c << 6 | (*p & 0x3F);
+    }
+    if (c < lowest || c > 0x10FFFF || (c >= 0xD800 && c <= 0xDFFF)) return false;
+    if (c < 0x10000) {
+      out.push_back((char16_t)c);
+    } else {
+      c -= 0x10000;
+      out.push_back((char16_t)(0xD800 + (c >> 10)));
+      out.push_back((char16_t)(0xDC00 + (c & 0x3FF)));
+    }
+  }
+  return true;
+}
+
+// commons-lang3 getLevenshteinDistance over UTF-16 code units (SimilarityFn.scala:95 compares with charAt)
+int host_levenshtein(const char16_t *a, int la, const char16_t *b, int lb) {
   if (la == 0) return lb;
   if (lb == 0) return la;
   // two-row DP on the shorter string
@@ -32,7 +64,7 @@ int host_levenshtein(const char *a, int la, const char *b, int lb) {
   for (int j = 0; j <= lb; ++j) prev[j] = j;
   for (int i = 1; i <= la; ++i) {
     cur[0] = i;
-    const char ca = a[i - 1];
+    const char16_t ca = a[i - 1];
     for (int j = 1; j <= lb; ++j) {
       const int sub = prev[j - 1] + (ca != b[j - 1] ? 1 : 0);
       const int del = prev[j] + 1, ins = cur[j - 1] + 1;
@@ -91,14 +123,39 @@ double host_similarity_from_unit(double unit, double threshold, double max_sim) 
   return s > 0.0 ? s : 0.0;
 }
 
-// unit similarity of a pair under similarity 1 (Levenshtein) or 2 (Jaro-Winkler)
-static double host_unit_similarity(int similarity, const char *a, int la, const char *b, int lb) {
-  if (similarity == DBL_SIM_JARO_WINKLER) {
-    int m, h, l;
-    host_jaro_winkler_counts(a, la, b, lb, m, h, l);
-    return host_jaro_winkler_unit(m, h, l, la, lb);
-  }
+// unit similarities of a pair: Levenshtein over UTF-16 code units, Jaro-Winkler over UTF-8 bytes
+static double host_levenshtein_unit_of(const char16_t *a, int la, const char16_t *b, int lb) {
   return host_levenshtein_unit(host_levenshtein(a, la, b, lb), la, lb);
+}
+static double host_jaro_winkler_unit_of(const std::string &a, const std::string &b) {
+  int m, h, l;
+  host_jaro_winkler_counts(a.data(), (int)a.size(), b.data(), (int)b.size(), m, h, l);
+  return host_jaro_winkler_unit(m, h, l, (int)a.size(), (int)b.size());
+}
+
+// The vocabulary's code units as byte symbols for the device kernel, which indexes its match masks by byte.  The edit
+// distance only asks whether two units are equal, so any one-to-one map keeps every distance: the identity when every
+// unit is below 256, otherwise a dense table of the distinct units.  false = more than 256 distinct units.
+static bool lev_byte_symbols(const std::u16string &units, const std::vector<size_t> &off,
+                             std::vector<std::string> &out) {
+  std::vector<uint8_t> seen(65536, 0), sym(65536, 0);
+  for (char16_t c : units) seen[c] = 1;
+  if (std::count(seen.begin() + 256, seen.end(), 1) == 0) {
+    for (int c = 0; c < 256; ++c) sym[c] = (uint8_t)c;
+  } else {
+    int n = 0;
+    for (int c = 0; c < 65536; ++c)
+      if (seen[c]) {
+        if (n == 256) return false;
+        sym[c] = (uint8_t)n++;
+      }
+  }
+  out.resize(off.size() - 1);
+  for (size_t v = 0; v + 1 < off.size(); ++v) {
+    out[v].resize(off[v + 1] - off[v]);
+    for (size_t q = off[v]; q < off[v + 1]; ++q) out[v][q - off[v]] = (char)sym[units[q]];
+  }
+  return true;
 }
 
 // unit similarity from the integer a device kernel reports for a pair: the edit distance, or m | h << 8 | l << 16
@@ -320,17 +377,38 @@ extern "C" int dbl_index_build(dbl_index **out, const char *const *values, const
   ix->rowptr.assign(V + 1, 0);
   if (!ix->is_const) {
     // all-pairs thresholded similarity (computeSimValueIndex, :219-231)
+    const bool lev = similarity == DBL_SIM_LEVENSHTEIN;
+    std::u16string units;               // Levenshtein: every value decoded once, value v = units[off[v] .. off[v+1])
+    std::vector<size_t> off(V + 1, 0);
+    bool ascii = true;                  // every value ASCII: its code units are its bytes
+    if (lev) {
+      size_t bytes = 0;
+      for (int i = 0; i < V; ++i) bytes += ix->values[i].size();
+      units.reserve(bytes);
+      for (int i = 0; i < V; ++i) {
+        if (!host_utf8_to_utf16(ix->values[i].data(), ix->values[i].size(), units)) {
+          delete ix;
+          return DBL_ERR_INVALID;
+        }
+        off[i + 1] = units.size();
+        ascii = ascii && off[i + 1] - off[i] == ix->values[i].size();
+      }
+    }
     std::vector<std::vector<std::pair<int32_t, double>>> rows(V);
-    std::vector<int> len(V);
-    for (int i = 0; i < V; ++i) len[i] = (int)ix->values[i].size();
+    std::vector<int> len(V);  // Levenshtein: code units (String.length); Jaro-Winkler: bytes
+    for (int i = 0; i < V; ++i) len[i] = lev ? (int)(off[i + 1] - off[i]) : (int)ix->values[i].size();
     bool done = false;
     const char *env = std::getenv("DBL_INDEX_GPU");  // "0" = host only, "1" = GPU whenever possible
     const bool want_gpu = env ? (env[0] == '1') : (V >= 2048);
     if (want_gpu) {
       // integer codes of the candidate pairs on the GPU (edit distance, or Jaro-Winkler counts), identical double
-      // arithmetic afterwards
+      // arithmetic afterwards.  Levenshtein hands the kernel one byte symbol per code unit (an ASCII vocabulary: its
+      // own bytes).
+      const bool mapped = lev && !ascii;
+      std::vector<std::string> symbols;
       std::vector<int> ci, cj, cc;
-      if (gpu_similarity_candidates(similarity, ix->values, threshold, max_sim, ci, cj, cc)) {
+      if ((!mapped || lev_byte_symbols(units, off, symbols)) &&
+          gpu_similarity_candidates(similarity, mapped ? symbols : ix->values, threshold, max_sim, ci, cj, cc)) {
         for (int r = 0; r < V; ++r) {  // the diagonal: distance 0; m = |v|, h = 0, l = min(4, |v|)
           const int code = similarity == DBL_SIM_JARO_WINKLER ? len[r] | std::min(4, len[r]) << 16 : 0;
           const double e =
@@ -345,6 +423,7 @@ extern "C" int dbl_index_build(dbl_index **out, const char *const *values, const
         }
         for (int r = 0; r < V; ++r) std::sort(rows[r].begin(), rows[r].end());
         done = true;
+        ix->pairs_on_device = true;
       }
     }
     if (!done) {
@@ -356,7 +435,8 @@ extern "C" int dbl_index_build(dbl_index **out, const char *const *values, const
           for (int r = i; r < std::min(V, i + 16); ++r) {
             auto &row = rows[r];
             for (int c = 0; c < V; ++c) {
-              const double u = host_unit_similarity(similarity, ix->values[r].data(), len[r], ix->values[c].data(), len[c]);
+              const double u = lev ? host_levenshtein_unit_of(&units[off[r]], len[r], &units[off[c]], len[c])
+                                   : host_jaro_winkler_unit_of(ix->values[r], ix->values[c]);
               const double e = std::exp(host_similarity_from_unit(u, threshold, max_sim));
               if (e > 1.0) row.emplace_back(c, e);
             }
@@ -407,6 +487,7 @@ extern "C" int dbl_index_from_tables(dbl_index **out, int32_t V, int similarity,
 extern "C" void dbl_index_free(dbl_index *ix) { delete ix; }
 extern "C" int32_t dbl_index_num_values(const dbl_index *ix) { return ix ? ix->V : 0; }
 extern "C" int32_t dbl_index_nnz(const dbl_index *ix) { return ix ? ix->rowptr[ix->V] : 0; }
+extern "C" int32_t dbl_index_pairs_on_device(const dbl_index *ix) { return ix && ix->pairs_on_device ? 1 : 0; }
 extern "C" int32_t dbl_index_value_id(const dbl_index *ix, const char *value) {
   if (!ix || !value || ix->values.empty()) return -1;
   auto it = std::lower_bound(ix->values.begin(), ix->values.end(), std::string(value));
@@ -438,8 +519,17 @@ extern "C" double dbl_index_exp_sim(const dbl_index *ix, int32_t v1, int32_t v2)
 extern "C" double dbl_similarity(int similarity, const char *a, const char *b, double threshold, double max_sim) {
   if (similarity < DBL_SIM_CONSTANT || similarity > DBL_SIM_JARO_WINKLER) return std::numeric_limits<double>::quiet_NaN();
   if (similarity == DBL_SIM_CONSTANT) return 0.0;  // ConstantSimilarityFn, SimilarityFn.scala:50
-  const int la = (int)std::strlen(a), lb = (int)std::strlen(b);
-  return host_similarity_from_unit(host_unit_similarity(similarity, a, la, b, lb), threshold, max_sim);
+  const std::string sa(a), sb(b);
+  double unit;
+  if (similarity == DBL_SIM_LEVENSHTEIN) {
+    std::u16string ua, ub;
+    if (!host_utf8_to_utf16(sa.data(), sa.size(), ua) || !host_utf8_to_utf16(sb.data(), sb.size(), ub))
+      return std::numeric_limits<double>::quiet_NaN();
+    unit = host_levenshtein_unit_of(ua.data(), (int)ua.size(), ub.data(), (int)ub.size());
+  } else {
+    unit = host_jaro_winkler_unit_of(sa, sb);
+  }
+  return host_similarity_from_unit(unit, threshold, max_sim);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -218,6 +218,7 @@ struct dbl_index {
   std::vector<double> expsim;
   std::vector<double> pk, cdf;      // (kmax+1) x V
   std::vector<double> logphi, lognorm;
+  bool pairs_on_device = false;    // dbl_index_build: the similarity pairs came from the device kernel
   // per-row perfect hash of the off-diagonal similar values (link kernel): slot = (uint32(v) * hmult[x]) >> hshift
   int32_t hsize = 0, hshift = 32;  // hsize == 0: no table (constant attribute, or rows too long)
   std::vector<uint32_t> hmult;     // V
@@ -242,10 +243,13 @@ struct dbl_kdtree {
 // theta draw (GU:305-320) -- host, libm
 void host_draw_theta(int A, int F, const double *alpha, const double *beta, uint64_t seed, const int64_t *agg_dist,
                      const int64_t *file_sizes, uint32_t iter, double *theta_out);
-int host_levenshtein(const char *a, int la, const char *b, int lb);
+// strict UTF-8 -> UTF-16 code units (false = invalid UTF-8) and the edit distance over code units
+bool host_utf8_to_utf16(const char *s, size_t n, std::u16string &out);
+int host_levenshtein(const char16_t *a, int la, const char16_t *b, int lb);
 void host_jaro_winkler_counts(const char *a, int la, const char *b, int lb, int &m, int &h, int &l);
 // GPU all-pairs candidates for the attribute index (dbl_index_gpu.cu): (i, j > i, code) with code = the edit
-// distance (similarity 1) or m | h << 8 | l << 16 (similarity 2, Jaro-Winkler counts); false = not applicable
+// distance (similarity 1) or m | h << 8 | l << 16 (similarity 2, Jaro-Winkler counts); false = not applicable.
+// values: for similarity 1 one byte symbol per UTF-16 code unit (dbl_index_build maps them), for 2 the UTF-8 bytes
 bool gpu_similarity_candidates(int similarity, const std::vector<std::string> &values, double threshold,
                                double max_sim, std::vector<int> &oi, std::vector<int> &oj, std::vector<int> &oc);
 // norm / invnorm / pk / cdf on the device (dbl_index_gpu.cu), same values as the host loops; false = not applicable

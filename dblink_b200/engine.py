@@ -126,6 +126,11 @@ class AttributeIndex:
         _check(rc, "AttributeIndex.slot_codes")
         return out
 
+    @property
+    def pairs_on_device(self):
+        """True when build() found the similarity pairs with the device kernel, False when the host loop did."""
+        return bool(_lib.load().dbl_index_pairs_on_device(self._h))
+
     def _require(self, v):
         if not 0 <= v < self.num_values:
             raise IndexError("valueId is not in the index")  # AttributeIndex.scala:137

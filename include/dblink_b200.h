@@ -36,7 +36,9 @@ extern "C" {
 
 /* similarity functions of an attribute (SimilarityFn.scala:50-107, plus Jaro-Winkler) */
 #define DBL_SIM_CONSTANT 0     /* ConstantSimilarityFn                                                          */
-#define DBL_SIM_LEVENSHTEIN 1  /* LevenshteinSimilarityFn: unit = 1 - 2 d / (|a| + |b| + d)                     */
+#define DBL_SIM_LEVENSHTEIN 1  /* LevenshteinSimilarityFn: unit = 1 - 2 d / (|a| + |b| + d), lengths and edit
+                                  distance in UTF-16 code units of the UTF-8 values, as String.length and
+                                  getLevenshteinDistance count them; invalid UTF-8 is refused                  */
 #define DBL_SIM_JARO_WINKLER 2 /* JaroWinklerSimilarityFn: Jaro-Winkler over bytes, prefix scale 0.1, common
                                   prefix capped at 4, no boost threshold; same truncation as Levenshtein         */
 
@@ -51,7 +53,9 @@ typedef struct dbl_ctx dbl_ctx;       /* State + broadcast RecordsCache/Partitio
  * RecordsCache.scala:112-113).  similarity: 0 = ConstantSimilarityFn, 1 = LevenshteinSimilarityFn
  * (SimilarityFn.scala:50-107), 2 = JaroWinklerSimilarityFn (DBL_SIM_*); any other value is DBL_ERR_INVALID.
  * For 1 and 2 a pair is in the sparse rows when exp(sim) > 1, sim = the truncation of SimilarityFn.scala:65-70
- * applied to the unit similarity.  `values` need not be sorted; `weights` are the value counts.
+ * applied to the unit similarity.  `values` need not be sorted; `weights` are the value counts.  Values are UTF-8;
+ * Levenshtein measures them in UTF-16 code units (a Java String's length and charAt), and with similarity 1 a value
+ * that is not valid UTF-8 (RFC 3629: no overlong forms, no surrogates, nothing above U+10FFFF) is DBL_ERR_INVALID.
  * ------------------------------------------------------------------------------------------------- */
 int dbl_index_build(dbl_index **out, const char *const *values, const double *weights, int32_t num_values,
                     int similarity, double threshold, double max_similarity, int32_t kmax);
@@ -70,6 +74,9 @@ int32_t dbl_index_hash_slots(const dbl_index *);
  * value the same slot in every row's table; DBL_ERR_STATE when the index has none (other table sizes, or values that
  * did not colour) */
 int dbl_index_slot_codes(const dbl_index *, int32_t *out);
+/* 1 when dbl_index_build found the index's similarity pairs with the device kernel, 0 when the host loop did (or the
+ * index is constant, or came from tables) */
+int32_t dbl_index_pairs_on_device(const dbl_index *);
 int32_t dbl_index_value_id(const dbl_index *, const char *value); /* valueIdxOf; -1 when absent              */
 const char *dbl_index_value(const dbl_index *, int32_t value_id);
 /* copies of the tables (arrays sized num_values, num_values+1, nnz, nnz); any pointer may be NULL */
@@ -77,7 +84,8 @@ int dbl_index_tables(const dbl_index *, double *phi /*probabilityOf*/, double *n
                      int32_t *rowptr, int32_t *col, double *expsim /*simValuesOf*/);
 double dbl_index_exp_sim(const dbl_index *, int32_t v1, int32_t v2); /* expSimOf; NaN when out of range        */
 /* SimilarityFn.getSimilarity (SimilarityFn.scala:65-70, 84-96); similarity as in dbl_index_build (2 = Jaro-Winkler
- * unit similarity under the same truncation); NaN for an unknown similarity */
+ * unit similarity under the same truncation); NaN for an unknown similarity, and for similarity 1 when a or b is not
+ * valid UTF-8 */
 double dbl_similarity(int similarity, const char *a, const char *b, double threshold, double max_similarity);
 
 /* ---------------------------------------------------------------------------------------------------

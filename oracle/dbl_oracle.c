@@ -60,9 +60,48 @@ void orc_uniform2(uint64_t seed, uint32_t phase, uint32_t iter, uint32_t id, uin
 /* Similarity function -- SimilarityFn.scala:61-98                                              */
 /* ------------------------------------------------------------------------------------------ */
 
-/* unit-cost Levenshtein distance (commons-lang3 StringUtils.getLevenshteinDistance, SimilarityFn.scala:22,95) */
-int orc_levenshtein(const char *a, const char *b) {
-  int la = (int)strlen(a), lb = (int)strlen(b);
+/* The reference measures Java Strings: a.length and charAt count UTF-16 code units.  utf8_units turns a UTF-8 value
+   into those units by the byte-sequence grammar of RFC 3629 section 4 (UTF8-1 .. UTF8-4): the lead byte fixes the
+   sequence length and the range of its second byte, which leaves out overlong forms, surrogates and everything above
+   U+10FFFF.  out needs room for strlen(s) units (a sequence never gives more units than bytes).  Returns the number of
+   units, or -1 when s is not valid UTF-8. */
+static int utf8_units(const char *s, uint16_t *out) {
+  const unsigned char *p = (const unsigned char *)s;
+  int n = 0;
+  while (*p) {
+    const unsigned b0 = p[0];
+    unsigned len, lo = 0x80, hi = 0xBF;
+    if (b0 <= 0x7F) { out[n++] = (uint16_t)b0; ++p; continue; }
+    if (b0 >= 0xC2 && b0 <= 0xDF) len = 2;
+    else if (b0 == 0xE0) { len = 3; lo = 0xA0; }
+    else if (b0 == 0xED) { len = 3; hi = 0x9F; }
+    else if (b0 >= 0xE1 && b0 <= 0xEF) len = 3;
+    else if (b0 == 0xF0) { len = 4; lo = 0x90; }
+    else if (b0 == 0xF4) { len = 4; hi = 0x8F; }
+    else if (b0 >= 0xF1 && b0 <= 0xF3) len = 4;
+    else return -1;
+    if (p[1] < lo || p[1] > hi) return -1; /* the terminating NUL fails here and below: no read past it */
+    for (unsigned k = 2; k < len; ++k)
+      if (p[k] < 0x80 || p[k] > 0xBF) return -1;
+    uint32_t cp = b0 & (0x7Fu >> len);
+    for (unsigned k = 1; k < len; ++k) cp = (cp << 6) | (p[k] & 0x3Fu);
+    p += len;
+    if (cp > 0xFFFF) {
+      cp -= 0x10000;
+      out[n++] = (uint16_t)(0xD800 | (cp >> 10));
+      out[n++] = (uint16_t)(0xDC00 | (cp & 0x3FF));
+    } else {
+      out[n++] = (uint16_t)cp;
+    }
+  }
+  return n;
+}
+
+static uint16_t *units_alloc(const char *s) { return (uint16_t *)malloc(sizeof(uint16_t) * (strlen(s) + 1)); }
+
+/* unit-cost Levenshtein distance over code units (commons-lang3 StringUtils.getLevenshteinDistance,
+   SimilarityFn.scala:22,95) */
+static int lev_units(const uint16_t *a, int la, const uint16_t *b, int lb) {
   if (la == 0) return lb;
   if (lb == 0) return la;
   int *row = (int *)malloc(sizeof(int) * (size_t)(lb + 1));
@@ -101,8 +140,22 @@ static double sim_from_distance(int dist, int la, int lb, double threshold, doub
   return trans > 0.0 ? trans : 0.0;
 }
 
+/* -1 when a or b is not valid UTF-8 */
+int orc_levenshtein(const char *a, const char *b) {
+  uint16_t *ua = units_alloc(a), *ub = units_alloc(b);
+  const int la = utf8_units(a, ua), lb = utf8_units(b, ub);
+  const int d = (la < 0 || lb < 0) ? -1 : lev_units(ua, la, ub, lb);
+  free(ua); free(ub);
+  return d;
+}
+
+/* NaN when a or b is not valid UTF-8 */
 double orc_lev_similarity(const char *a, const char *b, double threshold, double max_sim) {
-  return sim_from_distance(orc_levenshtein(a, b), (int)strlen(a), (int)strlen(b), threshold, max_sim);
+  uint16_t *ua = units_alloc(a), *ub = units_alloc(b);
+  const int la = utf8_units(a, ua), lb = utf8_units(b, ub);
+  const double s = (la < 0 || lb < 0) ? NAN : sim_from_distance(lev_units(ua, la, ub, lb), la, lb, threshold, max_sim);
+  free(ua); free(ub);
+  return s;
 }
 
 /* ------------------------------------------------------------------------------------------ */
@@ -175,15 +228,27 @@ orc_index *orc_index_build(const char *const *values, const double *weights, int
   free(sw);
   ix->rowptr = (int32_t *)calloc((size_t)V + 1, sizeof(int32_t));
   if (!is_const) {
-    /* AttributeIndex.scala:219-231: all pairs, keep exp(sim) > 1.0 */
+    /* AttributeIndex.scala:219-231: all pairs, keep exp(sim) > 1.0; lengths and distances in code units */
     int *len = (int *)malloc(sizeof(int) * (size_t)V);
-    for (int i = 0; i < V; ++i) len[i] = (int)strlen(ix->values[i]);
+    uint16_t **units = (uint16_t **)calloc((size_t)V, sizeof(uint16_t *));
+    int bad = 0;
+    for (int i = 0; i < V && !bad; ++i) {
+      units[i] = units_alloc(ix->values[i]);
+      len[i] = utf8_units(ix->values[i], units[i]);
+      bad = len[i] < 0;
+    }
+    if (bad) {
+      for (int i = 0; i < V; ++i) free(units[i]);
+      free(units); free(len);
+      orc_index_free(ix);
+      return NULL;
+    }
     size_t cap = (size_t)V * 8, nnz = 0;
     int32_t *ri = (int32_t *)malloc(sizeof(int32_t) * cap), *ci = (int32_t *)malloc(sizeof(int32_t) * cap);
     double *ev = (double *)malloc(sizeof(double) * cap);
     for (int i = 0; i < V; ++i)
       for (int j = i; j < V; ++j) {
-        int d = orc_levenshtein(ix->values[i], ix->values[j]);
+        int d = lev_units(units[i], len[i], units[j], len[j]);
         double e = exp(sim_from_distance(d, len[i], len[j], threshold, max_sim));
         if (e > 1.0) {
           if (nnz + 2 > cap) {
@@ -196,6 +261,8 @@ orc_index *orc_index_build(const char *const *values, const double *weights, int
           if (i != j) { ri[nnz] = j; ci[nnz] = i; ev[nnz] = e; ++nnz; }
         }
       }
+    for (int i = 0; i < V; ++i) free(units[i]);
+    free(units);
     free(len);
     for (size_t k = 0; k < nnz; ++k) ix->rowptr[ri[k] + 1]++;
     for (int i = 0; i < V; ++i) ix->rowptr[i + 1] += ix->rowptr[i];

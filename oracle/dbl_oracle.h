@@ -38,11 +38,13 @@ typedef struct orc_state orc_state;
 void orc_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]);
 void orc_uniform2(uint64_t seed, uint32_t phase, uint32_t iter, uint32_t id, uint32_t sub, double u[2]);
 
-/* ---- similarity function (SimilarityFn.scala:61-98) ---- */
+/* ---- similarity function (SimilarityFn.scala:61-98) ----
+   UTF-8 values measured in UTF-16 code units, as the reference's Java Strings are; -1 / NaN when a value is not
+   valid UTF-8 */
 int orc_levenshtein(const char *a, const char *b);
 double orc_lev_similarity(const char *a, const char *b, double threshold, double max_sim);
 
-/* ---- attribute index (AttributeIndex.scala:107-245) ---- */
+/* ---- attribute index (AttributeIndex.scala:107-245); NULL when a non-constant index has invalid UTF-8 ---- */
 orc_index *orc_index_build(const char *const *values, const double *weights, int V, int is_const,
                            double threshold, double max_sim, int kmax);
 void orc_index_free(orc_index *);

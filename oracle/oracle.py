@@ -183,6 +183,8 @@ class Index:
         arr = (C.c_char_p * len(vals))(*[v.encode() for v in vals])
         w = _f64([values_weights[v] for v in vals])
         h = lib().orc_index_build(arr, _p(w, c_dp), len(vals), int(is_const), threshold, max_sim, kmax)
+        if not h:
+            raise ValueError("orc_index_build refused the values (invalid UTF-8)")
         return cls(h)
 
     @classmethod

@@ -1,7 +1,8 @@
 """Literal Python restatement of JaroWinklerSimilarityFn and of the attribute-index rows it gives (test code only).
 
 The CPU oracle restates the reference, which has no Jaro-Winkler function; the Jaro-Winkler rows come from here and
-enter the oracle through orc_index_from_tables, which computes the normalisations and base pmfs as for any index."""
+enter the oracle through orc_index_from_tables, which computes the normalisations and base pmfs as for any index.
+index_rows / oracle_index take the similarity as an argument; lev_reference.py passes its Levenshtein."""
 import math
 
 import numpy as np
@@ -49,10 +50,10 @@ def similarity(a, b, threshold, max_sim):
     return s if s > 0.0 else 0.0
 
 
-def index_rows(values_weights, threshold, max_sim):
-    """AttributeIndex.scala:107-231 for Jaro-Winkler: value ids in byte order, probs = weight / total (total summed in
-    id order), all pairs kept when exp(sim) > 1 (pairs j >= i scored, mirrored: the counts are symmetric).
-    -> (values in id order, probs, rowptr, col, expsim)"""
+def index_rows(values_weights, threshold, max_sim, sim=similarity):
+    """AttributeIndex.scala:107-231 for a symmetric similarity `sim` (Jaro-Winkler by default): value ids in UTF-8 byte
+    order, probs = weight / total (total summed in id order), all pairs kept when exp(sim) > 1 (pairs j >= i scored,
+    mirrored).  -> (values in id order, probs, rowptr, col, expsim)"""
     vals = sorted(values_weights, key=lambda s: s.encode())
     total = 0.0
     for v in vals:
@@ -61,7 +62,7 @@ def index_rows(values_weights, threshold, max_sim):
     rows = [[] for _ in vals]
     for i, a in enumerate(vals):
         for j in range(i, len(vals)):
-            e = math.exp(similarity(a, vals[j], threshold, max_sim))
+            e = math.exp(sim(a, vals[j], threshold, max_sim))
             if e > 1.0:
                 rows[i].append((j, e))
                 if j != i:
@@ -73,7 +74,7 @@ def index_rows(values_weights, threshold, max_sim):
     return vals, probs, rowptr, col, expsim
 
 
-def oracle_index(O, values_weights, threshold, max_sim, kmax=10):
-    """-> (oracle Index built from the Jaro-Winkler rows, {value: id})"""
-    vals, probs, rowptr, col, expsim = index_rows(values_weights, threshold, max_sim)
+def oracle_index(O, values_weights, threshold, max_sim, kmax=10, sim=similarity):
+    """-> (oracle Index built from the rows of `sim` (Jaro-Winkler by default), {value: id})"""
+    vals, probs, rowptr, col, expsim = index_rows(values_weights, threshold, max_sim, sim)
     return O.Index.from_tables(probs, rowptr, col, expsim, False, kmax), {v: i for i, v in enumerate(vals)}
