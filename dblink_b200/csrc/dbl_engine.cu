@@ -207,26 +207,30 @@ __global__ void k_hist(int64_t n, const int *__restrict__ key, int *__restrict__
 // the link kernel (and its tile ring) advance at the same pace.  The order of records inside a block has no effect
 // on the draws (every record has its own counter-based stream).
 constexpr int REC_CLASS_BITS = 8;
-// cost class of a record (x is static): bits 7..6 = number of missing non-constant attributes (each one adds a
-// gather per candidate), bits 5..0 = expected number of similar-but-different candidate values per 32-candidate
-// step (how often the warp takes the rare multiply: equal or similar value), from the empirical value frequencies.
+// cost class of a record (x is static), from hq = the expected number of similar-but-different candidate values per
+// 32-candidate step (how often the warp takes the rare multiply: equal or similar value), from the empirical value
+// frequencies, in 0..63: a record without a missing non-constant value has class hq; one with a missing non-constant
+// value 64 + 4 lo + hq / 16, lo = the first non-constant attribute it misses (0..15, in attribute order), so that
+// records missing the same attribute share work items of k_link_pcg2 (whose producer stages the 1/n(y) columns the
+// work item's records miss, and whose warps skip the probes of an attribute both their records miss).
 __global__ void k_rec_class(int64_t R, int A, const AttrDev *__restrict__ attrs, const int *__restrict__ x,
                             unsigned char *__restrict__ cls) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= R) return;
-  int miss = 0;
+  int lo = -1;
   double h = 0.0;
-  for (int a = 0; a < A; ++a) {
+  for (int a = 0, q = 0; a < A; ++a) {
     const AttrDev &at = attrs[a];
     if (at.is_const) continue;
     const int xv = x[r * A + a];
-    if (xv < 0) { ++miss; continue; }
+    if (xv < 0) { if (lo < 0) lo = q; ++q; continue; }
+    ++q;
     h += at.probs[xv];  // an equal value takes the same path as a similar one (one table, see k_link_pcg2)
     for (int i = at.rowptr[xv]; i < at.rowptr[xv + 1]; ++i)
       if (at.col[i] != xv) h += at.probs[at.col[i]];
   }
   const int hq = min(63, (int)(h * 32.0 * 8.0));
-  cls[r] = (unsigned char)((min(miss, 3) << 6) | hq);
+  cls[r] = (unsigned char)(lo < 0 ? hq : 64 | (min(lo, 15) << 2) | (hq >> 4));
 }
 // block sort keys of the entities and of the records in one launch
 __global__ void k_block_keys(int64_t E, int64_t R, const int *__restrict__ blk, const int *__restrict__ link,
@@ -333,14 +337,21 @@ struct TileSrc {
     return true;
   }
 };
-// tiles of format f, NS non-constant attributes
+// tiles of format f, NS non-constant attributes; invn (k_link_pcg2, may be null): the 1/n(y) columns of every tile,
+// [tile][q][slot] (LinkParams::tile_invn), the invnorm of the entity's value of kernel-order attribute A - NS + q
+// (= scinvnorm of its slot code: the columns do not depend on the format)
 __global__ void k_build_entity_tiles(TileSrc s, Pcg2Format f, int NS, const AttrDev *__restrict__ attrs,
-                                     int *__restrict__ tiles) {
+                                     int *__restrict__ tiles, double *__restrict__ invn) {
   int T, slot;
   const int *yrow;
   double N;
   if (!s.at((int64_t)blockIdx.x * blockDim.x + threadIdx.x, T, slot, yrow, N)) return;
   pcg2_store(f, s.A, NS, yrow, s.perm, attrs, tiles + (size_t)T * f.layout(s.A, NS).words(), slot, N);
+  if (invn)
+    for (int q = 0; q < NS; ++q) {
+      const int a = s.perm[s.A - NS + q];
+      invn[((size_t)T * NS + q) * TE + slot] = yrow ? attrs[a].invnorm[yrow[a]] : 0.0;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -817,7 +828,11 @@ __global__ void k_validate(int64_t R, int64_t E, int A, int F, const AttrDev *__
       const int v = y[i * A + a];
       if (v < 0 || v >= attrs[a].V) bad |= 8;
     }
-  if (bad) atomicOr(flag, bad);
+  if (i < R)  // not an error: bit 4 = the record misses a non-constant value (k_link_pcg2 needs the 1/n(y) columns)
+    for (int a = 0; a < A; ++a)
+      if (!attrs[a].is_const && x[i * A + a] == -1) bad |= 16;
+  bad = __reduce_or_sync(FULL, bad);  // one atomic per warp (blocks of 256 threads: whole warps)
+  if (bad && (threadIdx.x & 31) == 0) atomicOr(flag, bad);
 }
 __global__ void k_pack_z(int64_t R, int A, const uint8_t *__restrict__ z, unsigned *__restrict__ zmask) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1333,6 +1348,10 @@ struct dbl_ctx {
   DevBuf<int> ent_ptr, tile_ptr, rec_ptr, cta_ptr, cta_ptr2, cta_ptr3, tiles;
   DevBuf<double> lane_sums;  // k_link_pcg2 scratch: pass-1 lane sums per chunk of every resident warp
   std::optional<Pcg2Format> tiles_fmt;  // the format `tiles` holds for the current layout; none: not built
+  // k_link_pcg2's 1/n(y) columns beside the tiles (LinkParams::tile_invn), allocated only when some record misses a
+  // non-constant value (rec_missing, found by k_validate at upload); tiles_invn: built with the current tiles
+  DevBuf<double> tile_invn;
+  bool rec_missing = false, tiles_invn = false;
   // inverted index of the block tables for the pruned PCG-I link kernel (built on demand, once per sweep): E * A ids,
   // unsigned or (inv_ids64) unsigned long long, with their candidate positions
   DevBuf<unsigned char> inv_ids_in, inv_ids;
@@ -1655,6 +1674,19 @@ extern "C" int64_t dbl_iteration(const dbl_ctx *ctx) { return ctx ? ctx->iterati
 extern "C" int64_t dbl_kernel_launches(const dbl_ctx *ctx) { return ctx ? ctx->launches : 0; }
 extern "C" const char *dbl_version(void) { return "dblink_b200 0.2 (sm_90a)"; }
 
+// the 1/n(y) columns of k_link_pcg2, as many tiles as `tiles` holds: only while some record misses a non-constant
+// value (48 MB at 1 M entities and 6 non-constant attributes)
+static int alloc_tile_invn(dbl_ctx *ctx) {
+  const size_t n = (ctx->rec_missing && ctx->n_str > 0 && ctx->P > 0)
+                       ? ((size_t)(ctx->E / TE) + (size_t)ctx->P + 1) * ctx->n_str * TE : 0;
+  if (n == ctx->tile_invn.n) return DBL_OK;
+  ctx->drop_graphs();  // captured sweeps hold the link parameters by value
+  ctx->tiles_fmt.reset();
+  if (n == 0) ctx->tile_invn.release();
+  else CUDA_TRY(ctx->tile_invn.alloc(n));
+  return DBL_OK;
+}
+
 static int alloc_blocks(dbl_ctx *ctx) {
   const int P = ctx->P;
   ctx->drop_graphs();  // captured sweeps hold the old buffers / tree
@@ -1672,6 +1704,7 @@ static int alloc_blocks(dbl_ctx *ctx) {
   // sized for the unpacked format: a packed one needs a constant attribute, so it has no more words per entity
   const size_t max_tiles = (size_t)(ctx->E / TE) + (size_t)P + 1;
   CUDA_TRY(ctx->tiles.alloc(max_tiles * TileLayout::of(ctx->A).words()));
+  if (int rc = alloc_tile_invn(ctx)) return rc;
   // work item and grid of the persistent PCG-II kernel for this model shape (see Pcg2Format::rpw)
   ctx->pcg2_recs = LINK_WARPS * ctx->pcg2_fmt.rpw(ctx->n_str);
   ctx->pcg2_grid = ctx->sm_count * ctx->pcg2_fmt.ctas_per_sm(ctx->n_str);
@@ -1806,15 +1839,18 @@ static int relayout(dbl_ctx *ctx, bool end_of_sweep = false) {
 }
 
 // tiled copy of the block-sorted entity table in format f, the one the coming link kernel reads; one buffer for
-// every format, rebuilt when it holds another
-static int ensure_tiles(dbl_ctx *ctx, Pcg2Format f) {
-  if (ctx->tiles_fmt == f) return DBL_OK;
+// every format, rebuilt when it holds another.  invn: with k_link_pcg2's 1/n(y) columns (when allocated)
+static int ensure_tiles(dbl_ctx *ctx, Pcg2Format f, bool invn = false) {
+  invn = invn && ctx->tile_invn.p;
+  if (ctx->tiles_fmt == f && ctx->tiles_invn == invn) return DBL_OK;
   const int64_t n_slots = (int64_t)((size_t)(ctx->E / TE) + (size_t)ctx->P + 1) * TE;
   const TileSrc s{n_slots, ctx->A, ctx->P, ctx->y.p, ctx->ent_sorted.p, ctx->ent_ptr.p, ctx->tile_ptr.p,
                   ctx->perm_dev.p, ctx->entN.p};
-  k_build_entity_tiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(s, f, ctx->n_str, ctx->attrs.p, ctx->tiles.p);
+  k_build_entity_tiles<<<grid_for(n_slots, 256), 256, 0, ctx->stream>>>(s, f, ctx->n_str, ctx->attrs.p, ctx->tiles.p,
+                                                                         invn ? ctx->tile_invn.p : nullptr);
   ctx->launches += 1;
   ctx->tiles_fmt = f;
+  ctx->tiles_invn = invn;
   CUDA_TRY(cudaGetLastError());
   return DBL_OK;
 }
@@ -1915,6 +1951,9 @@ static int finish_new_state(dbl_ctx *ctx, bool check_state, bool new_records) {
     CUDA_TRY(cudaMemcpyAsync(hc.data(), ctx->file_cnt.p, sizeof(int) * ctx->F, cudaMemcpyDeviceToHost, ctx->stream));
   }
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // nothing below may run on out-of-range ids
+  ctx->rec_missing = (bad & 16) != 0;
+  bad &= 15;
+  if (int rc = alloc_tile_invn(ctx)) return rc;
   if (bad) {
     ctx->has_state = false;
     ctx->set_error(bad & 1 ? "record value id out of range" : bad & 2 ? "file id out of range"
@@ -2286,7 +2325,7 @@ static int ensure_inverted_index(dbl_ctx *ctx) {
 
 static bool pcg2_kernel_fits(const dbl_ctx *ctx) {
   return ctx->hslots > 0 && ctx->A <= LINK_MAX_UNROLL_A &&
-         pcg2_smem_bytes(ctx->pcg2_fmt, ctx->A, ctx->n_str, ctx->hslots) <= 100 * 1024;
+         pcg2_smem_bytes(ctx->pcg2_fmt, ctx->A, ctx->n_str, ctx->hslots, false) <= 100 * 1024;
 }
 static int dispatch_pcg2(dbl_ctx *ctx, const LinkParams *lp, int grid = 0) {
   Pcg2Kernel k = nullptr;
@@ -2296,8 +2335,8 @@ static int dispatch_pcg2(dbl_ctx *ctx, const LinkParams *lp, int grid = 0) {
     DBL_CASE(9) DBL_CASE(10) DBL_CASE(11) DBL_CASE(12) DBL_CASE(13) DBL_CASE(14) DBL_CASE(15) DBL_CASE(16)
 #undef DBL_CASE
   }
-  const int rc = pcg2_launch(k, pcg2_smem_bytes(ctx->pcg2_fmt, ctx->A, ctx->n_str, ctx->hslots), lp, grid,
-                             ctx->stream, &ctx->pcg2_smem_cfg);
+  const size_t smem = pcg2_smem_bytes(ctx->pcg2_fmt, ctx->A, ctx->n_str, ctx->hslots, ctx->tile_invn.p != nullptr);
+  const int rc = pcg2_launch(k, smem, lp, grid, ctx->stream, &ctx->pcg2_smem_cfg);
   if (rc != 0) { ctx->set_error(std::string("k_link_pcg2 launch: ") + cudaGetErrorString((cudaError_t)rc)); return DBL_ERR_CUDA; }
   return DBL_OK;
 }
@@ -2341,8 +2380,9 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
     // persistent CTAs: a few per SM, each takes groups of LINK_WARPS records from the work counter until none is left
     // (k_theta zeroed the counter; the block-level API launches the kernel once per block after one k_theta)
     if (ctx->in_block_sweep) CUDA_TRY(cudaMemsetAsync(lp.work, 0, sizeof(unsigned long long), ctx->stream));
-    int rc = ensure_tiles(ctx, ctx->pcg2_fmt);
+    int rc = ensure_tiles(ctx, ctx->pcg2_fmt, true);
     if (rc) return rc;
+    lp.tile_invn = ctx->tile_invn.p;
     lp.cta_ptr = ctx->cta_ptr3.p;  // work items of PCG2_RECS records
     return dispatch_pcg2(ctx, &lp, std::min(ctx->max_ctas, ctx->pcg2_grid));
   }
@@ -3075,10 +3115,12 @@ extern "C" int dbl_state_hash(dbl_ctx *ctx, uint64_t *hash_out) {
 
 // which link kernel a sweep with this sampler launches: 0 k_link_generic, 1 k_link_match, 2 k_link_pruned,
 // 3 k_link_pcg2 plus the bits of the model's tile format (Pcg2Format::bits, decided by pcg2_format at model upload)
+// and +256 when the 1/n(y) columns travel with the tiles (some record misses a non-constant value)
 extern "C" int dbl_link_kernel(const dbl_ctx *ctx, int sampler) {
   if (!ctx || sampler < 0 || sampler > 3) return DBL_ERR_INVALID;
   const LinkKernel kernel = link_kernel(ctx, sampler);
-  return kernel == LINK_PCG2 ? LINK_PCG2 + ctx->pcg2_fmt.bits(ctx->n_str) : kernel;
+  if (kernel != LINK_PCG2) return kernel;
+  return LINK_PCG2 + ctx->pcg2_fmt.bits(ctx->n_str) + (ctx->tile_invn.p ? 256 : 0);
 }
 
 extern "C" int dbl_set_link_mode(dbl_ctx *ctx, int mode) {

@@ -104,6 +104,9 @@ struct LinkParams {
   const double *theta;
   const int *ent_ptr, *tile_ptr, *rec_ptr, *cta_ptr, *ent_sorted, *rec_sorted;
   const int *tiles;          // entity tiles (TileLayout) in the format the launched kernel reads
+  // k_link_pcg2: per tile, the 1/n(y) of each non-constant attribute of its entities, [tile][q][slot] f64 (q = kernel
+  // position - (A - NS), padding slots 0); nullptr when no record of the model misses a non-constant value
+  const double *tile_invn;
   unsigned long long *work;  // k_link_pcg2: next group of records to take (persistent CTAs); zeroed before the launch
   double *lane_sums;         // k_link_pcg2: scratch, [CTA][consumer warp][32 chunks][32 lanes] pass-1 lane sums
   int *newlink;
@@ -487,6 +490,11 @@ struct TileRing {
   uint64_t *full;      // LINK_STAGES
   uint64_t *empty;     // LINK_STAGES
   int tw;              // words per tile
+  // k_link_pcg2: LINK_STAGES x ncols f64 columns of TE entries beside the tiles ([stage][column][slot]), filled from
+  // the ncols columns per tile of gcols ([tile][column][slot]) that the producer's mask names; column q of a stage
+  // holds column q of its tile
+  double *cols = nullptr;
+  int ncols = 0;
 };
 
 __device__ __forceinline__ void ring_init(const TileRing &rg, int consumers) {
@@ -500,9 +508,11 @@ __device__ __forceinline__ void ring_init(const TileRing &rg, int consumers) {
 // RELAXED: the consumers are slow (PCG-II): let the producer sleep.  !RELAXED: the consumers drain tiles faster
 // than the producer can be woken (PCG-I): poll.
 // base = tiles this CTA has already streamed through the ring (persistent CTAs): stages and phases continue
+// cmask: the columns of gcols (rg.ncols per tile, see TileRing) to stage with each tile, bit q = column q; 0: tiles only
 template <bool RELAXED>
-__device__ __forceinline__ void ring_produce(const TileRing &rg, const int *gsrc, int ntiles, int base = 0) {
-  const unsigned bytes = (unsigned)rg.tw * 4u;
+__device__ __forceinline__ void ring_produce(const TileRing &rg, const int *gsrc, int ntiles, int base = 0,
+                                             const double *gcols = nullptr, unsigned cmask = 0u) {
+  const unsigned bytes = (unsigned)rg.tw * 4u + (unsigned)__popc(cmask) * (TE * 8u);
   for (int t = 0; t < ntiles; ++t) {
     const int g = base + t;
     const int s = g % LINK_STAGES;
@@ -511,7 +521,12 @@ __device__ __forceinline__ void ring_produce(const TileRing &rg, const int *gsrc
       else mbar_wait(&rg.empty[s], ((g / LINK_STAGES) - 1) & 1);
     }
     mbar_arrive_expect_tx(&rg.full[s], bytes);
-    tma_load_1d(rg.tiles + (size_t)s * rg.tw, gsrc + (size_t)t * rg.tw, bytes, &rg.full[s]);
+    tma_load_1d(rg.tiles + (size_t)s * rg.tw, gsrc + (size_t)t * rg.tw, (unsigned)rg.tw * 4u, &rg.full[s]);
+    for (unsigned m = cmask; m; m &= m - 1) {
+      const int q = __ffs(m) - 1;
+      tma_load_1d(rg.cols + ((size_t)s * rg.ncols + q) * TE, gcols + ((size_t)t * rg.ncols + q) * TE, TE * 8u,
+                  &rg.full[s]);
+    }
   }
 }
 

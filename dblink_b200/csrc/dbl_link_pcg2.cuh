@@ -26,8 +26,11 @@
 //    code & 31, computed once per (candidate, attribute) for both records of the warp (no per-record multiplier);
 //    with ID16 and SC the two records' tables are paired (PAIR_KEYS): one key word holds both records' 16-bit keys
 //    of a slot, so one key load and one value address serve both records;
-//  * records with a missing non-constant value multiply by 1/n(y): the two-record shapes keep the NS table pointers
-//    in registers for the whole work item (fetching them per step and attribute cost 15 % of the kernel at 1 M);
+//  * records with a missing non-constant value multiply by 1/n(y) of that attribute (their probe never hits): the
+//    1/n(y) of
+//    every tile entity travel with the tiles (LinkParams::tile_invn, one f64 column of TE per non-constant
+//    attribute), and the producer stages the columns its work item's records miss in the same ring stage as the
+//    tile, so that no pass-1 loop reads global memory;
 //  * lane l scores candidate 32*step + l; lane sums / chunk totals / draw as in DESIGN.md section 4.
 #pragma once
 #include <algorithm>
@@ -201,12 +204,14 @@ __device__ __forceinline__ void pcg2_load(Pcg2Cand<A, NS, PK> &c, const int *til
 // SC: the non-constant values are slot codes (AttrDev::pcode), whose low five bits are the slot in every record's
 // table: the slot of a probe does not depend on the record, so it is computed once for the warp's records, which need
 // no multipliers.
-// invnorm: the 1/n(y) tables of the non-constant attributes in kernel order (SC: indexed by code) when the caller
-// keeps them in registers; nullptr: read through p.attrs.
+// inv: the candidate's entry of its tile's first 1/n(y) column (LinkParams::tile_invn), column q at inv[q * TE]: in
+// pass 1 the column staged in shared memory with the tile, in pass 2 the one in global memory; read only for the
+// attributes the record misses.  Their probes stay: the record's table of such an attribute is empty, so the probe
+// never hits, and a warp-uniform skip per attribute cost more instructions per tile than the probes it saves (569
+// against 630 at A = 10, NS = 6, paired).
 template <int A, int NS, int HC, bool PK, bool SC, bool MISSING = true>
 __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS, SC> &rc, const LinkParams &p, const char *tab,
-                                              const double *ctab, const Pcg2Cand<A, NS, PK> &cd,
-                                              const double *const *invnorm = nullptr) {
+                                              const double *ctab, const Pcg2Cand<A, NS, PK> &cd, const double *inv) {
   static_assert(!SC || (PK && HC == 32), "slot codes only in the packed 32-slot tiles");
   const int hslots = HC ? HC : p.hslots;
   const int hshift = HC ? 27 : p.hshift;
@@ -240,9 +245,7 @@ __device__ __forceinline__ double pcg2_weight(const Pcg2Rec<A, NS, SC> &rc, cons
   if (MISSING && rc.mmask) {
 #pragma unroll
     for (int q = 0; q < NS; ++q)
-      if ((rc.mmask >> (A - NS + q)) & 1u)
-        w = w * (invnorm ? __ldg(invnorm[q] + y[A - NS + q])
-                         : (SC ? p.attrs[p.perm[A - NS + q]].scinvnorm : p.attrs[p.perm[A - NS + q]].invnorm)[y[A - NS + q]]);
+      if ((rc.mmask >> (A - NS + q)) & 1u) w = w * inv[q * TE];
   }
   return w;
 }
@@ -264,11 +267,11 @@ __device__ __forceinline__ bool pcg2_half_hit(unsigned k, unsigned c2) {
 // and w[1]; each is the product pcg2_weight forms, factor for factor in the same order.  Per (candidate, attribute):
 // one PRMT spreads the 16-bit code over both halves of a word, c2 = {code, code}; ONE key load at slot code & 31
 // serves both records, whose hits are the halves of k ^ c2 that are zero (pcg2_half_hit); one value address serves
-// both predicated value loads (record 1's values are PAIR_VALS bytes past record 0's).
+// both predicated value loads (record 1's values are PAIR_VALS bytes past record 0's).  inv: as in pcg2_weight.
 template <int A, int NS, bool MISSING = true>
-__device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc)[2], unsigned recs, const LinkParams &p,
+__device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc)[2], unsigned recs,
                                                  const char *tab, const double *ctab, const Pcg2Cand<A, NS, true> &cd,
-                                                 double (&w)[2], const double *const *invnorm = nullptr) {
+                                                 double (&w)[2], const double *inv) {
   static_assert(NS >= 1 && NS < A, "paired tables: packed constants and at least one non-constant attribute");
 #pragma unroll
   for (int ri = 0; ri < 2; ++ri)  // protocol 4.1: w = N * (product of the constant attributes' multipliers)
@@ -290,9 +293,7 @@ __device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc
       if (!((recs >> ri) & 1u) || !rc[ri].mmask) continue;
 #pragma unroll
       for (int q = 0; q < NS; ++q)
-        if ((rc[ri].mmask >> (A - NS + q)) & 1u)
-          w[ri] = w[ri] * (invnorm ? __ldg(invnorm[q] + cd.y[A - NS + q])
-                                   : p.attrs[p.perm[A - NS + q]].scinvnorm[cd.y[A - NS + q]]);
+        if ((rc[ri].mmask >> (A - NS + q)) & 1u) w[ri] = w[ri] * inv[q * TE];
     }
   }
 }
@@ -329,6 +330,10 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
   // PK: products of the matching constant attributes, by match mask, 16 entries per record
   double *ctab0 = reinterpret_cast<double *>(reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 +
                                             (size_t)WARPS * wtab) + warp * RPW * 16;
+  // the 1/n(y) columns of the staged tiles (only when p.tile_invn: see pcg2_smem_bytes)
+  rg.cols = reinterpret_cast<double *>(reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 +
+                                       (size_t)WARPS * wtab) + WARPS * RPW * 16;
+  rg.ncols = NS;
   ring_init(rg, WARPS);
   const int total_ctas = p.cta_ptr[p.P];
   int tbase = 0;  // tiles this CTA has streamed so far: stage and phase of the ring continue across work items
@@ -343,9 +348,20 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
     const int n = p.ent_ptr[b + 1] - p.ent_ptr[b];
     const int ntiles = p.tile_ptr[b + 1] - p.tile_ptr[b];
     const int *gtiles = p.tiles + (size_t)p.tile_ptr[b] * TW;
+    const double *gcols = p.tile_invn ? p.tile_invn + (size_t)p.tile_ptr[b] * NS * TE : nullptr;
+    const int rec0 = p.rec_ptr[b] + (cta - p.cta_ptr[b]) * PCG2_RECS;  // first record of the work item
 
     if (warp == WARPS) {  // producer warp
-      if (lane == 0) ring_produce<true>(rg, gtiles, ntiles, tbase);
+      // the columns to stage: the non-constant attributes that some record of the work item misses
+      unsigned cmask = 0u;
+      if (gcols && lane < PCG2_RECS && rec0 + lane < p.rec_ptr[b + 1]) {
+        const int r = p.rec_sorted[rec0 + lane];
+#pragma unroll
+        for (int q = 0; q < NS; ++q)
+          if (p.x[(int64_t)r * A + p.perm[A - NS + q]] < 0) cmask |= 1u << q;
+      }
+      cmask = __reduce_or_sync(FULL, cmask);
+      if (lane == 0) ring_produce<true>(rg, gtiles, ntiles, tbase, gcols, cmask);
       tbase += ntiles;
       continue;
     }
@@ -356,7 +372,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
     bool act[RPW];
 #pragma unroll
     for (int ri = 0; ri < RPW; ++ri) {
-      const int ridx = p.rec_ptr[b] + (cta - p.cta_ptr[b]) * PCG2_RECS + warp * RPW + ri;
+      const int ridx = rec0 + warp * RPW + ri;
       act[ri] = ridx < p.rec_ptr[b + 1];
       rr[ri] = act[ri] ? p.rec_sorted[ridx] : -1;
       const int r = rr[ri];
@@ -451,33 +467,27 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
     double *my_sums = p.lane_sums + ((size_t)blockIdx.x * WARPS + warp) * RPW * 1024;  // [record][chunk][lane]
     auto pass1 = [&](auto missing_tag) {
       constexpr bool MISSING = decltype(missing_tag)::value;
-      // the 1/n(y) tables of the non-constant attributes, loaded once instead of once per step and attribute
-      // (two-record shapes only: in the one-record shapes the NS pointers do not fit the register budget)
-      constexpr bool HOIST = MISSING && RPW == 2;
-      const double *invnorm[NS > 0 ? NS : 1];
-#pragma unroll
-      for (int q = 0; q < NS; ++q)
-        invnorm[q] = HOIST ? (SC ? p.attrs[p.perm[A - NS + q]].scinvnorm : p.attrs[p.perm[A - NS + q]].invnorm) : nullptr;
       for (int t = 0; t < ntiles; ++t) {
         const int g = tbase + t;
         const int s = g % LINK_STAGES;
         mbar_wait(&rg.full[s], (g / LINK_STAGES) & 1);
         if (act[0]) {  // (the second record of a warp is only there when the first is)
           const int *tile = rg.tiles + (size_t)s * TW;
+          const double *cols = rg.cols + (size_t)s * NS * TE + lane;  // the staged 1/n(y) columns (MISSING)
 #pragma unroll
           for (int q = 0; q < TE / 32; ++q) {
             Pcg2Cand<A, NS, PK> cd;
             pcg2_load<A, NS, PK, ID16>(cd, tile, q * 32 + lane);
             if constexpr (PAIR) {
               double w[2];
-              pcg2_weight_pair<A, NS, MISSING>(rc, 3u, p, tab0, ctab0, cd, w, invnorm);
+              pcg2_weight_pair<A, NS, MISSING>(rc, 3u, tab0, ctab0, cd, w, cols + q * 32);
               acc[0] = acc[0] + w[0];
               acc[1] = acc[1] + w[1];
             } else {
 #pragma unroll
               for (int ri = 0; ri < RPW; ++ri)
                 acc[ri] = acc[ri] + pcg2_weight<A, NS, HC, PK, SC, MISSING>(rc[ri], p, tab0 + ri * tabrec,
-                                                                          ctab0 + ri * 16, cd, HOIST ? invnorm : nullptr);
+                                                                          ctab0 + ri * 16, cd, cols + q * 32);
             }
           }
           if (++tile_in_chunk == geo.tpc || t + 1 == ntiles) {
@@ -508,12 +518,14 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
         if (j >= n) return 0.0;
         Pcg2Cand<A, NS, PK> cd;
         pcg2_load<A, NS, PK, ID16>(cd, gtiles + (size_t)(j / TE) * TW, j % TE);
+        // the candidate's 1/n(y) in global memory (read only when the record misses a value: then gcols is set)
+        const double *inv = gcols + (size_t)(j / TE) * NS * TE + j % TE;
         if constexpr (PAIR) {  // record ri's half of the paired tables
           double w[2];
-          pcg2_weight_pair<A, NS>(rc, 1u << ri, p, tab0, ctab0, cd, w);
+          pcg2_weight_pair<A, NS>(rc, 1u << ri, tab0, ctab0, cd, w, inv);
           return ri ? w[1] : w[0];
         } else {
-          return pcg2_weight<A, NS, HC, PK, SC>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd);
+          return pcg2_weight<A, NS, HC, PK, SC>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd, inv);
         }
       };
       const U2 u = link_uniform(p, r);
@@ -523,10 +535,11 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
   }
 }
 
-// dynamic shared memory of one CTA (H = the table size of the model)
-inline size_t pcg2_smem_bytes(Pcg2Format f, int A, int NS, int H) {
+// dynamic shared memory of one CTA (H = the table size of the model); invn: with the ring's 1/n(y) columns, NS per
+// stage (LinkParams::tile_invn set: some record misses a non-constant value)
+inline size_t pcg2_smem_bytes(Pcg2Format f, int A, int NS, int H, bool invn) {
   return (size_t)LINK_STAGES * f.layout(A, NS).words() * 4 + 128 + (size_t)LINK_WARPS * pcg2_warp_tab_bytes(f, NS, H) +
-         (size_t)LINK_WARPS * f.rpw(NS) * 16 * sizeof(double);
+         (size_t)LINK_WARPS * f.rpw(NS) * 16 * sizeof(double) + (invn ? (size_t)LINK_STAGES * NS * TE * sizeof(double) : 0);
 }
 
 // k_link_pcg2<A, NS, ...> of format f for a runtime NS in [0, A] (nullptr: none); the `if constexpr` guards only keep

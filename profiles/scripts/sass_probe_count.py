@@ -40,9 +40,10 @@ def tile_loops(ins):
         ops = [x[1] for x in body]
         if sum(o.startswith("SYNCS.PHASECHK") for o in ops) != 1 or not any(o.startswith("DMUL") for o in ops):
             continue
-        kind = "missing-value" if any(o.startswith("LDG") for o in ops) else "branch-free"
-        loops.append((kind, body))
-    return loops
+        loops.append(body)
+    # the loop with the fewest DMULs is the branch-free one; the missing-value loop adds the 1/n(y) multiplies
+    dmul = [sum(x[1].startswith("DMUL") for x in body) for body in loops]
+    return [("branch-free" if d == min(dmul) else "missing-value", body) for d, body in zip(dmul, loops)]
 
 
 def histogram(body):
