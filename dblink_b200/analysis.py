@@ -143,5 +143,30 @@ def format_cluster(ari):
             f" Adj. Rand index: {ari}\n=====================================\n")
 
 
+def _posterior_line(label, s, extra=""):
+    line = f" {label:<17}{s['mean']} (sd {s['sd']}, 95% interval [{s['q025']}, {s['q975']}], median {s['median']})"
+    if s["undefined"]:
+        line += f", undefined in {s['undefined']} samples"
+    return line + extra + "\n"
+
+
+def format_posterior_pairwise(summary, num_samples):
+    """The posterior-pairwise section: summary = analysis_arrays.posterior_summary over num_samples samples."""
+    return ("=====================================\n     Posterior pairwise metrics\n"
+            "-------------------------------------\n"
+            f" Samples:         {num_samples}\n" + _posterior_line("Precision:", summary["precision"])
+            + _posterior_line("Recall:", summary["recall"]) + _posterior_line("F1-score:", summary["f1score"])
+            + "=====================================\n")
+
+
+def format_posterior_cluster(summary, num_samples, true_num_clusters):
+    """The posterior-cluster section: summary = analysis_arrays.posterior_summary over num_samples samples."""
+    return ("=====================================\n      Posterior cluster metrics\n"
+            "-------------------------------------\n"
+            f" Samples:         {num_samples}\n" + _posterior_line("Adj. Rand index:", summary["adjRandIndex"])
+            + _posterior_line("Clusters:", summary["numClusters"], f" (true: {true_num_clusters})")
+            + "=====================================\n")
+
+
 def is_nan(x):
     return isinstance(x, float) and math.isnan(x)

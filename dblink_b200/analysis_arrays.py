@@ -281,20 +281,86 @@ def contingency(pred_labels, true_labels):
     return n, np.bincount(p), np.bincount(t)
 
 
-def pairwise_metrics(pred_labels, true_labels):
-    n, pn, tn = contingency(pred_labels, true_labels)
-    tp = int(_comb2(n).sum())
-    fp = int(_comb2(pn).sum()) - tp
-    fn = int(_comb2(tn).sum()) - tp
+PAIRWISE_KEYS = ("precision", "recall", "f1score", "TP", "FP", "FN")
+
+
+def metrics_from_counts(tp, pred_pairs, true_pairs, num_records):
+    """Pairwise precision / recall / F1 / TP / FP / FN and the adjusted Rand index (key adjRandIndex) of one clustering,
+    from its pair counts: tp = pairs put together by both clusterings, pred_pairs / true_pairs = pairs put together by
+    each.  Undefined values are NaN: precision without a predicted pair, recall without a true pair, F1 without either,
+    the adjusted Rand index with fewer than two records."""
+    tp, pc, tc = int(tp), int(pred_pairs), int(true_pairs)
+    fp, fn = pc - tp, tc - tp
     precision = tp / (tp + fp) if tp + fp else float("nan")
     recall = tp / (tp + fn) if tp + fn else float("nan")
     f1 = 2 * precision * recall / (precision + recall) if tp else (0.0 if (fp or fn) else float("nan"))
-    return {"precision": precision, "recall": recall, "f1score": f1, "TP": tp, "FP": fp, "FN": fn}
+    all_pairs = int(_comb2(num_records))
+    if all_pairs:
+        expected = pc * tc / all_pairs
+        max_index = (pc + tc) / 2.0
+        ari = (tp - expected) / (max_index - expected) if max_index != expected else 1.0
+    else:
+        ari = float("nan")
+    return {"precision": precision, "recall": recall, "f1score": f1, "TP": tp, "FP": fp, "FN": fn,
+            "adjRandIndex": ari}
+
+
+def _label_counts(pred_labels, true_labels):
+    n, pn, tn = contingency(pred_labels, true_labels)
+    return metrics_from_counts(_comb2(n).sum(), _comb2(pn).sum(), _comb2(tn).sum(), len(pred_labels))
+
+
+def pairwise_metrics(pred_labels, true_labels):
+    m = _label_counts(pred_labels, true_labels)
+    return {k: m[k] for k in PAIRWISE_KEYS}
 
 
 def adjusted_rand_index(pred_labels, true_labels):
-    n, pn, tn = contingency(pred_labels, true_labels)
-    total, pc, tc = int(_comb2(n).sum()), int(_comb2(pn).sum()), int(_comb2(tn).sum())
-    expected = pc * tc / int(_comb2(len(pred_labels)))
-    max_index = (pc + tc) / 2.0
-    return (total - expected) / (max_index - expected) if max_index != expected else 1.0
+    return _label_counts(pred_labels, true_labels)["adjRandIndex"]
+
+
+# ---- every sample against the ground truth ---------------------------------------------------------------
+def true_pairs(true_labels):
+    """The number of record pairs the ground truth puts together."""
+    return int(_comb2(np.unique(np.asarray(true_labels), return_counts=True)[1]).sum())
+
+
+def posterior_metric_counts(chain, truth):
+    """(tp, pred_pairs, num_clusters), int64[S]: per sample, the record pairs it shares with the ground truth
+    (truth[r] = true label of record index r), the pairs it puts together and its number of clusters."""
+    R = chain.num_records
+    truth = np.asarray(truth)
+    S = len(chain.samples)
+    out = [np.zeros(S, np.int64) for _ in range(3)]
+    for s, (mem, off, _) in enumerate(chain.samples):
+        if len(mem) != R:
+            raise ValueError("every sample must mention every record exactly once")
+        sizes = np.diff(off)
+        n, pn, _ = contingency(np.repeat(np.arange(len(sizes)), sizes), truth[mem])
+        out[0][s], out[1][s], out[2][s] = _comb2(n).sum(), _comb2(pn).sum(), len(pn)
+    return tuple(out)
+
+
+SAMPLE_METRICS = ("precision", "recall", "f1score", "adjRandIndex", "numClusters")
+
+
+def sample_metrics(tp, pred_pairs, num_clusters, truth):
+    """One dict per sample: metrics_from_counts of its counts, and numClusters."""
+    tc, R = true_pairs(truth), len(truth)
+    return [dict(metrics_from_counts(t, p, tc, R), numClusters=int(c)) for t, p, c in zip(tp, pred_pairs, num_clusters)]
+
+
+def posterior_summary(rows):
+    """For each of SAMPLE_METRICS over the samples (dicts of sample_metrics) where it is defined (not NaN): mean, sd
+    (ddof = 1; NaN below two values), the 2.5 %, 50 % and 97.5 % quantiles (np.quantile's default method), the number
+    of defined values n and of undefined ones."""
+    out = {}
+    for k in SAMPLE_METRICS:
+        v = np.asarray([r[k] for r in rows], np.float64)
+        d = v[~np.isnan(v)]
+        q = np.quantile(d, [0.025, 0.5, 0.975]) if len(d) else np.full(3, np.nan)
+        out[k] = {"mean": float(d.mean()) if len(d) else float("nan"),
+                  "sd": float(d.std(ddof=1)) if len(d) >= 2 else float("nan"),
+                  "q025": float(q[0]), "median": float(q[1]), "q975": float(q[2]),
+                  "n": len(d), "undefined": len(v) - len(d)}
+    return out

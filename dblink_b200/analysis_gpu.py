@@ -6,7 +6,9 @@ computes the same 64-bit cluster signatures (dbl_posterior.cu), the same per-rec
 earliest sample, and the same smallest-record-index labels.  The (S x R) signature matrix lives in device memory,
 filled one sample at a time; the host only turns each sample's (members, offsets) into a cluster label per record.
 The pairwise match counts equal analysis_arrays.pairwise_match_counts exactly: the device keeps the sorted table of
-(pair, count) and merges each sample's pairs into it.
+(pair, count) and merges each sample's pairs into it.  The per-sample counts against the ground truth equal
+analysis_arrays.posterior_metric_counts exactly: they are integers, counted on the device from one radix sort of
+(sample label, true label) per record.
 """
 import ctypes as C
 
@@ -153,3 +155,54 @@ def pairwise_match_counts(chain, max_pairs=MAX_PAIRS, min_count=1):
         return pairs.read(min_count)
     finally:
         pairs.close()
+
+
+class Evaluation:
+    """Owner of a dbl_eval handle: the ground truth goes in once, samples one at a time, read() gives the per-sample
+    counts."""
+
+    def __init__(self, num_records, truth, max_samples):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        self.num_records = int(num_records)
+        truth = np.ascontiguousarray(truth, np.int32)
+        if truth.shape != (self.num_records,):
+            raise ValueError("the ground truth needs one label per record")
+        _check(self._lib.dbl_eval_create(C.byref(self._h), self.num_records, truth.ctypes.data, int(max_samples)),
+               "dbl_eval_create")
+
+    def add_sample(self, cluster):
+        cluster = np.ascontiguousarray(cluster, np.int32)
+        if cluster.shape != (self.num_records,):
+            raise ValueError("a sample needs one cluster label per record")
+        _check(self._lib.dbl_eval_add_sample(self._h, cluster.ctypes.data), "dbl_eval_add_sample")
+
+    @property
+    def num_samples(self):
+        return self._lib.dbl_eval_num_samples(self._h)
+
+    def read(self):
+        """(tp, pred_pairs, num_clusters), int64[S]."""
+        out = [np.empty(self.num_samples, np.int64) for _ in range(3)]
+        _check(self._lib.dbl_eval_read(self._h, *(a.ctypes.data_as(_lib.i64p) for a in out)), "dbl_eval_read")
+        return tuple(out)
+
+    def close(self):
+        if self._h:
+            self._lib.dbl_eval_free(self._h)
+            self._h = C.c_void_p()
+
+
+def posterior_metric_counts(chain, truth):
+    """(tp, pred_pairs, num_clusters), identical to analysis_arrays.posterior_metric_counts(chain, truth)."""
+    R = chain.num_records
+    if R == 0 or not chain.samples:
+        return tuple(np.zeros(len(chain.samples), np.int64) for _ in range(3))
+    _, dense = np.unique(np.asarray(truth), return_inverse=True)  # any labels -> [0, number of entities)
+    ev = Evaluation(R, dense, len(chain.samples))
+    try:
+        for mem, off, _ in chain.samples:
+            ev.add_sample(sample_clusters(R, mem, off))
+        return ev.read()
+    finally:
+        ev.close()

@@ -16,6 +16,12 @@
 // unordered pair of records the number of samples in which they share a cluster.  The handle holds a sorted table of
 // (first << 32 | second, count) over the pairs seen so far; each sample's pairs are generated, sorted and merged into
 // it -- see dbl_pairs_add_sample.
+//
+// Every sample against the ground truth (dbl_eval_*, same numbers as analysis_arrays.posterior_metric_counts): per
+// sample the pair counts the pairwise metrics and the adjusted Rand index are made of -- tp = sum over the cells
+// (sample cluster, true entity) of C(n, 2), pred_pairs = sum over sample clusters of C(size, 2) -- and the number of
+// clusters, all in int64.  Each record becomes one key, sample label above true label; the keys are radix-sorted on
+// their 2 ceil(log2 R) bits, so cells and clusters are runs of the sorted keys -- see dbl_eval_add_sample.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -652,5 +658,160 @@ extern "C" int dbl_pairs_read(dbl_pairs *p, int32_t min_count, int32_t *first, i
   POST_TRY(cudaMemcpy(first, f.p, sizeof(int32_t) * n, cudaMemcpyDefault));
   POST_TRY(cudaMemcpy(second, s.p, sizeof(int32_t) * n, cudaMemcpyDefault));
   POST_TRY(cudaMemcpy(count, c.p, sizeof(int32_t) * n, cudaMemcpyDefault));
+  return DBL_OK;
+}
+
+// ---- every sample against the ground truth -------------------------------------------------------------------------
+namespace {
+// one key per record: its sample label above its true label, each in lab_bits bits
+__global__ void k_pack_labels(int64_t R, int lab_bits, const int32_t *__restrict__ cluster,
+                              const int32_t *__restrict__ truth, unsigned long long *__restrict__ key) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x)
+    key[r] = (unsigned long long)(uint32_t)cluster[r] << lab_bits | (uint32_t)truth[r];
+}
+
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Over the sorted keys: the last position of each run of equal keys (one cell of the contingency table) and of each
+// run of equal sample labels (one predicted cluster) finds its run's first position by binary search and adds
+// C(run length, 2); cluster runs are counted.  out = {tp, pred_pairs, num_clusters}, summed exactly in uint64.
+__global__ void k_eval_counts(int64_t R, int lab_bits, const unsigned long long *__restrict__ key,
+                              unsigned long long *__restrict__ tp, unsigned long long *__restrict__ pred_pairs,
+                              unsigned long long *__restrict__ num_clusters) {
+  unsigned long long cell = 0, pred = 0, clusters = 0;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long k = key[i];
+    const bool last = i == R - 1;
+    if (last || key[i + 1] != k) {
+      const unsigned long long n = (unsigned long long)(i + 1 - lower_bound_u64(key, i + 1, k));
+      cell += n * (n - 1) / 2;
+    }
+    const unsigned long long hi = k >> lab_bits;
+    if (last || (key[i + 1] >> lab_bits) != hi) {
+      const unsigned long long n = (unsigned long long)(i + 1 - lower_bound_u64(key, i + 1, hi << lab_bits));
+      pred += n * (n - 1) / 2;
+      ++clusters;
+    }
+  }
+  cell = warp_sum_u64(cell);
+  pred = warp_sum_u64(pred);
+  clusters = warp_sum_u64(clusters);
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(tp, cell);
+    atomicAdd(pred_pairs, pred);
+    atomicAdd(num_clusters, clusters);
+  }
+}
+}  // namespace
+
+struct dbl_eval {
+  int device = 0;
+  int64_t R = 0;
+  int32_t max_samples = 0, S = 0;
+  int lab_bits = 1;                // bits of a label in [0, R)
+  cudaStream_t stream = nullptr;
+  Buf truth, cluster, bad;         // true labels, the sample's labels, label check flag
+  Buf key_in, key_s;               // packed (sample label, true label) per record, unsorted and sorted
+  Buf tmp;                         // CUB temporary storage of the key sort
+  size_t tmp_bytes = 0;
+  Buf counts;                      // [3][max_samples] uint64: tp, pred_pairs, num_clusters per sample
+};
+
+// labels (host or device) into dst, then the range check; 1 in *bad when one is outside [0, R)
+static int upload_labels(int64_t R, const int32_t *labels, Buf &dst, Buf &flag, cudaStream_t st, int *bad) {
+  POST_TRY(cudaMemcpyAsync(dst.p, labels, sizeof(int32_t) * R, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemsetAsync(flag.p, 0, sizeof(int), st));
+  k_check_labels<<<grid_for(R), THREADS, 0, st>>>(R, dst.as<int32_t>(), flag.as<int>());
+  POST_TRY(cudaMemcpyAsync(bad, flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
+extern "C" int dbl_eval_create(dbl_eval **out, int64_t num_records, const int32_t *truth, int32_t max_samples) {
+  if (!out) return DBL_ERR_INVALID;
+  *out = nullptr;
+  if (num_records <= 0 || num_records > INT32_MAX || !truth || max_samples <= 0) return DBL_ERR_INVALID;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return DBL_ERR_CUDA; }
+  auto *p = new dbl_eval();
+  const int64_t R = num_records;
+  p->R = R;
+  p->max_samples = max_samples;
+  p->lab_bits = bits_for(R);
+  const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(unsigned long long) * (size_t)R;
+  int rc = DBL_OK, bad = 0;
+  if (cudaGetDevice(&p->device) != cudaSuccess ||
+      cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking) != cudaSuccess || p->truth.alloc(r4) != cudaSuccess ||
+      p->cluster.alloc(r4) != cudaSuccess || p->bad.alloc(sizeof(int)) != cudaSuccess ||
+      p->key_in.alloc(r8) != cudaSuccess || p->key_s.alloc(r8) != cudaSuccess ||
+      p->counts.alloc(3 * sizeof(unsigned long long) * (size_t)max_samples) != cudaSuccess ||
+      cub::DeviceRadixSort::SortKeys(nullptr, p->tmp_bytes, (const unsigned long long *)nullptr,
+                                     (unsigned long long *)nullptr, R, 0, 2 * p->lab_bits, p->stream) != cudaSuccess ||
+      p->tmp.alloc(p->tmp_bytes) != cudaSuccess)
+    rc = DBL_ERR_CUDA;
+  else
+    rc = upload_labels(R, truth, p->truth, p->bad, p->stream, &bad);
+  if (rc == DBL_OK && bad) rc = DBL_ERR_INVALID;
+  if (rc != DBL_OK) {
+    cudaGetLastError();
+    dbl_eval_free(p);
+    return rc;
+  }
+  *out = p;
+  return DBL_OK;
+}
+
+extern "C" void dbl_eval_free(dbl_eval *p) {
+  if (!p) return;
+  DeviceScope ds(p->device);
+  if (p->stream) {
+    cudaStreamSynchronize(p->stream);
+    cudaStreamDestroy(p->stream);
+  }
+  delete p;
+}
+
+extern "C" int32_t dbl_eval_num_samples(const dbl_eval *p) { return p ? p->S : 0; }
+
+// One sample: check the labels; pack (label, true label) per record into 2 lab_bits bits; radix-sort on those bits;
+// one pass over the sorted keys writes the sample's three counts into column S.  S moves only on success.
+extern "C" int dbl_eval_add_sample(dbl_eval *p, const int32_t *cluster) {
+  if (!p || !cluster || p->S >= p->max_samples) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  const int64_t R = p->R;
+  cudaStream_t st = p->stream;
+  int bad = 0;
+  const int rc = upload_labels(R, cluster, p->cluster, p->bad, st, &bad);
+  if (rc != DBL_OK) return rc;
+  if (bad) return DBL_ERR_INVALID;
+  k_pack_labels<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_bits, p->cluster.as<int32_t>(), p->truth.as<int32_t>(),
+                                                 p->key_in.as<unsigned long long>());
+  size_t tb = p->tmp_bytes;
+  POST_TRY(cub::DeviceRadixSort::SortKeys(p->tmp.p, tb, p->key_in.as<unsigned long long>(),
+                                          p->key_s.as<unsigned long long>(), R, 0, 2 * p->lab_bits, st));
+  unsigned long long *c = p->counts.as<unsigned long long>() + p->S;
+  const int32_t M = p->max_samples;
+  for (int j = 0; j < 3; ++j) POST_TRY(cudaMemsetAsync(c + (size_t)j * M, 0, sizeof(unsigned long long), st));
+  k_eval_counts<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_bits, p->key_s.as<unsigned long long>(), c, c + M,
+                                                 c + 2 * (size_t)M);
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  ++p->S;
+  return DBL_OK;
+}
+
+extern "C" int dbl_eval_read(dbl_eval *p, int64_t *tp, int64_t *pred_pairs, int64_t *num_clusters) {
+  if (!p || !tp || !pred_pairs || !num_clusters) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  const unsigned long long *c = p->counts.as<unsigned long long>();
+  const size_t M = (size_t)p->max_samples, bytes = sizeof(int64_t) * (size_t)p->S;
+  POST_TRY(cudaMemcpyAsync(tp, c, bytes, cudaMemcpyDeviceToHost, p->stream));
+  POST_TRY(cudaMemcpyAsync(pred_pairs, c + M, bytes, cudaMemcpyDeviceToHost, p->stream));
+  POST_TRY(cudaMemcpyAsync(num_clusters, c + 2 * M, bytes, cudaMemcpyDeviceToHost, p->stream));
+  POST_TRY(cudaStreamSynchronize(p->stream));
   return DBL_OK;
 }

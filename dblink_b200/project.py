@@ -15,7 +15,10 @@ from .engine import GibbsEngine, KDTreePartitioner
 from .records import (Attribute, RecordsCache, SimilarityFn, build_cache_from_columns, read_csv,  # noqa: F401
                       read_csv_columns)
 
-SUPPORTED_METRICS = ("pairwise", "cluster")  # ProjectStep.scala:36
+SMPC_METRICS = ("pairwise", "cluster")  # ProjectStep.scala:36
+# every sample at or after the cutoff against the ground truth: evaluation-samples.csv and a posterior summary
+POSTERIOR_METRICS = ("posterior-pairwise", "posterior-cluster")
+SUPPORTED_METRICS = SMPC_METRICS + POSTERIOR_METRICS
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics")
 
@@ -34,6 +37,14 @@ def pairwise_match_counts(chain, min_count=1):
     if _lib.load().dbl_device_count() > 0:
         return analysis_gpu.pairwise_match_counts(chain, min_count=min_count)
     return analysis_arrays.pairwise_match_counts(chain, min_count=min_count)
+
+
+def posterior_metric_counts(chain, truth):
+    """(tp, pred_pairs, num_clusters) of every sample of a ChainArrays against the ground truth: on the GPU when the
+    platform has one (analysis_gpu), else on the host (analysis_arrays).  Both give identical arrays."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.posterior_metric_counts(chain, truth)
+    return analysis_arrays.posterior_metric_counts(chain, truth)
 
 
 class Project:
@@ -130,11 +141,16 @@ class Project:
                 L.append(f"  * SummarizeStep: Calculating summary quantities {braces(prm['quantities'])} along the "
                          f"chain for iterations >= {prm['lower_iteration_cutoff']}")
             elif name == "evaluate":
-                if prm["use_existing_smpc"]:
-                    L.append(f"  * EvaluateStep: Evaluating saved sMPC clusters using {braces(prm['metrics'])} metrics")
-                else:
+                smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
+                post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
+                if smpc and prm["use_existing_smpc"]:
+                    L.append(f"  * EvaluateStep: Evaluating saved sMPC clusters using {braces(smpc)} metrics")
+                elif smpc:
                     L.append(f"  * EvaluateStep: Evaluating sMPC clusters (computed from the chain for iterations >= "
-                             f"{prm['lower_iteration_cutoff']}) using {braces(prm['metrics'])} metrics")
+                             f"{prm['lower_iteration_cutoff']}) using {braces(smpc)} metrics")
+                if post:
+                    L.append(f"  * EvaluateStep: Evaluating every sample of the chain for iterations >= "
+                             f"{prm['lower_iteration_cutoff']} using {braces(post)} metrics")
             else:
                 L.append("  * CopyFilesStep: Copying {" + ", ".join(prm["file_names"]) + "} to destination "
                          + prm["destination_path"])
@@ -335,22 +351,35 @@ class Project:
                 true_labels = self.true_labels()
                 if true_labels is None:
                     raise ValueError("Ground truth entity ids are required for evaluation")  # ProjectStep.scala:65
-                ch = self.read_chain(prm["lower_iteration_cutoff"])
-                smpc_path = os.path.join(self.output_path, "shared-most-probable-clusters.csv")
-                if prm["use_existing_smpc"] and os.path.exists(smpc_path):  # ProjectStep.scala EvaluateStep
-                    labels = self._read_smpc_labels(smpc_path, ch.record_ids)
-                else:
-                    labels = shared_most_probable_clusters(ch)
-                    self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
-                truth = true_labels(ch.record_ids)
-                text = []
-                for m in prm["metrics"]:
-                    if m == "pairwise":
-                        results["pairwise"] = analysis_arrays.pairwise_metrics(labels, truth)
-                        text.append(analysis.format_pairwise(results["pairwise"]))
+                cut = prm["lower_iteration_cutoff"]
+                text, ch = [], None
+                if any(m in SMPC_METRICS for m in prm["metrics"]):
+                    ch = self.read_chain(cut)
+                    smpc_path = os.path.join(self.output_path, "shared-most-probable-clusters.csv")
+                    if prm["use_existing_smpc"] and os.path.exists(smpc_path):  # ProjectStep.scala EvaluateStep
+                        labels = self._read_smpc_labels(smpc_path, ch.record_ids)
                     else:
-                        results["cluster"] = analysis_arrays.adjusted_rand_index(labels, truth)
-                        text.append(analysis.format_cluster(results["cluster"]))
+                        labels = shared_most_probable_clusters(ch)
+                        self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
+                    truth = true_labels(ch.record_ids)
+                    for m in prm["metrics"]:
+                        if m == "pairwise":
+                            results["pairwise"] = analysis_arrays.pairwise_metrics(labels, truth)
+                            text.append(analysis.format_pairwise(results["pairwise"]))
+                        elif m == "cluster":
+                            results["cluster"] = analysis_arrays.adjusted_rand_index(labels, truth)
+                            text.append(analysis.format_cluster(results["cluster"]))
+                if any(m in POSTERIOR_METRICS for m in prm["metrics"]):
+                    rows, true_clusters = self._evaluate_samples(cut, true_labels, ch)
+                    summary = analysis_arrays.posterior_summary(rows)
+                    for m in prm["metrics"]:
+                        if m == "posterior-pairwise":
+                            results[m] = {k: summary[k] for k in ("precision", "recall", "f1score")}
+                            text.append(analysis.format_posterior_pairwise(summary, len(rows)))
+                        elif m == "posterior-cluster":
+                            results[m] = {k: summary[k] for k in ("adjRandIndex", "numClusters")}
+                            results[m]["trueNumClusters"] = true_clusters
+                            text.append(analysis.format_posterior_cluster(summary, len(rows), true_clusters))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
             elif name == "copy-files":
@@ -372,6 +401,21 @@ class Project:
         if self.num_chains == 1:
             return analysis_arrays.read_chain_arrays(paths[0], lower_iteration_cutoff)
         return analysis_arrays.read_pooled_chain_arrays(paths, lower_iteration_cutoff)
+
+    def _evaluate_samples(self, lower_iteration_cutoff, true_labels, pooled=None):
+        """Every sample at or after the cutoff against the ground truth: each chain's evaluation-samples.csv in its
+        directory, and (the rows of all chains pooled chain-major, the true number of entities).  `pooled` is the
+        chain already read by read_chain, reused when there is one chain."""
+        rows, true_clusters = [], 0
+        for dr in self.chain_dirs():
+            ch = (pooled if pooled is not None and self.num_chains == 1 else
+                  analysis_arrays.read_chain_arrays(os.path.join(dr, "linkage-chain.parquet"), lower_iteration_cutoff))
+            truth = true_labels(ch.record_ids)
+            one = analysis_arrays.sample_metrics(*posterior_metric_counts(ch, truth), truth)
+            writers.save_evaluation_samples(ch.iterations, one, dr)
+            rows += one
+            true_clusters = len(np.unique(truth))
+        return rows, true_clusters
 
     @staticmethod
     def _read_smpc_labels(path, record_ids):

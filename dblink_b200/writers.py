@@ -5,6 +5,7 @@
   DiagnosticsWriter   diagnostics.csv with the header of DiagnosticsWriter.scala:39-45 and rows of :47-72
   save_cluster_size_distribution / save_partition_sizes   LinkageChain.scala:162-211
   save_pairwise_match_probabilities   pairwise-match-probabilities.csv: recordId1,recordId2,probability
+  save_evaluation_samples   evaluation-samples.csv: every sample's counts and metrics against the ground truth
 """
 import os
 import time
@@ -202,3 +203,16 @@ def save_pairwise_match_probabilities(first, second, count, num_samples, record_
                                                text.take(count[lo:lo + step]), pa.scalar(",", pa.large_string()))
             offs = np.frombuffer(rows.buffers()[1], np.int64)[rows.offset:rows.offset + len(rows) + 1]
             fh.write(memoryview(rows.buffers()[2])[offs[0]:offs[-1]])
+
+
+EVALUATION_SAMPLES_HEADER = "iteration,numClusters,TP,FP,FN,precision,recall,f1score,adjRandIndex"
+
+
+def save_evaluation_samples(iterations, rows, path):
+    """evaluation-samples.csv under `path`: one row per sample (rows = analysis_arrays.sample_metrics, in iteration
+    order); floats written with repr, so an undefined metric reads `nan`."""
+    with open(os.path.join(path, "evaluation-samples.csv"), "w") as fh:
+        fh.write(EVALUATION_SAMPLES_HEADER + "\n")
+        for it, r in zip(iterations, rows):
+            fh.write(f"{int(it)},{r['numClusters']},{r['TP']},{r['FP']},{r['FN']},{r['precision']!r},{r['recall']!r},"
+                     f"{r['f1score']!r},{r['adjRandIndex']!r}\n")

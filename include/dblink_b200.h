@@ -337,6 +337,31 @@ int32_t dbl_pairs_num_samples(const dbl_pairs *);
 int dbl_pairs_count(dbl_pairs *, int32_t min_count, int64_t *n_out);
 int dbl_pairs_read(dbl_pairs *, int32_t min_count, int32_t *first, int32_t *second, int32_t *count);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Every posterior sample against the ground truth: per sample, the integer counts its pairwise precision / recall /
+ * F1 and adjusted Rand index are made of, on the device that is current when dbl_eval_create() is called.  truth is
+ * one int32 label in [0, R) per record (records with equal labels are one true entity), host or device, uploaded once;
+ * samples are fed one at a time as cluster[R], as for dbl_posterior_*.  Per sample, counted in int64:
+ *   tp            sum over the cells (sample cluster, true entity) of C(n, 2): the pairs both put together
+ *   pred_pairs    sum over the sample's clusters of C(size, 2)
+ *   num_clusters  the number of distinct labels of the sample
+ * The true pairs sum C(true size, 2) and C(R, 2) do not depend on the sample and are left to the caller.
+ *   dbl_eval_add_sample  cluster may be a host or a device pointer (ready when the call is made); a label outside
+ *                        [0, R) or a sample beyond max_samples gives DBL_ERR_INVALID and adds nothing
+ *   dbl_eval_read        the S counts of each kind, in the order the samples were added, into host arrays;
+ *                        DBL_ERR_STATE before the first sample
+ * DBL_ERR_INVALID: num_records outside [1, 2^31 - 1], max_samples < 1, truth NULL or a true label outside [0, R) (no
+ * object is created).  DBL_ERR_CUDA: no device, or an allocation that fails (24 bytes per record, and the
+ * temporary storage of a radix sort of R 64-bit keys).
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct dbl_eval dbl_eval;
+int dbl_eval_create(dbl_eval **out, int64_t num_records, const int32_t *truth /* R, host or device */,
+                    int32_t max_samples);
+void dbl_eval_free(dbl_eval *);
+int dbl_eval_add_sample(dbl_eval *, const int32_t *cluster /* R, host or device */);
+int32_t dbl_eval_num_samples(const dbl_eval *);
+int dbl_eval_read(dbl_eval *, int64_t *tp, int64_t *pred_pairs, int64_t *num_clusters /* S entries each, host */);
+
 /* The protocol functions of the theta draw (DESIGN.md 4.5), exposed so that they can be checked without a GPU:
  * log / exp built from individually rounded binary64 operations, and updateDistProbs (GU:305-320) itself. */
 double dbl_det_log(double x);
