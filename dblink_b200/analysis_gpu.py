@@ -45,38 +45,66 @@ def sample_clusters(num_records, members, offsets):
     return cluster
 
 
-class Posterior:
-    """Owner of a dbl_posterior handle: samples go in one at a time, smpc() reads the summary."""
+class _Handle:
+    """Owner of one handle of dbl_posterior.cu, whose C functions are named <_prefix>_<name>: samples go in one at a
+    time, close() (or leaving a with block) frees it."""
 
-    def __init__(self, num_records, max_samples):
+    _prefix = None
+
+    def __init__(self, num_records, *create_args):
         self._lib = _lib.load()
         self._h = C.c_void_p()
         self.num_records = int(num_records)
-        _check(self._lib.dbl_posterior_create(C.byref(self._h), self.num_records, int(max_samples)),
-               "dbl_posterior_create")
+        self._call("create", C.byref(self._h), self.num_records, *create_args)
+
+    def _fn(self, name):
+        return getattr(self._lib, f"{self._prefix}_{name}")
+
+    def _call(self, name, *args):
+        _check(self._fn(name)(*args), f"{self._prefix}_{name}")
 
     def add_sample(self, cluster):
         cluster = np.ascontiguousarray(cluster, np.int32)
         if cluster.shape != (self.num_records,):
             raise ValueError("a sample needs one cluster label per record")
-        _check(self._lib.dbl_posterior_add_sample(self._h, cluster.ctypes.data), "dbl_posterior_add_sample")
+        self._call("add_sample", self._h, cluster.ctypes.data)
 
     @property
     def num_samples(self):
-        return self._lib.dbl_posterior_num_samples(self._h)
+        return self._fn("num_samples")(self._h)
+
+    def close(self):
+        if self._h:
+            self._fn("free")(self._h)
+            self._h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def _add_chain(handle, chain):
+    """Every sample of a ChainArrays into handle, in chain order."""
+    for mem, off, _ in chain.samples:
+        handle.add_sample(sample_clusters(handle.num_records, mem, off))
+
+
+class Posterior(_Handle):
+    """Owner of a dbl_posterior handle: samples go in one at a time, smpc() reads the summary."""
+
+    _prefix = "dbl_posterior"
+
+    def __init__(self, num_records, max_samples):
+        super().__init__(num_records, int(max_samples))
 
     def smpc(self):
         """(labels int64[R], freq float64[R])."""
         labels = np.empty(self.num_records, np.int32)
         freq = np.empty(self.num_records, np.float64)
-        _check(self._lib.dbl_posterior_smpc(self._h, labels.ctypes.data_as(_lib.i32p), freq.ctypes.data_as(_lib.f64p)),
-               "dbl_posterior_smpc")
+        self._call("smpc", self._h, labels.ctypes.data_as(_lib.i32p), freq.ctypes.data_as(_lib.f64p))
         return labels.astype(np.int64), freq
-
-    def close(self):
-        if self._h:
-            self._lib.dbl_posterior_free(self._h)
-            self._h = C.c_void_p()
 
 
 def most_probable_clusters(chain):
@@ -85,13 +113,9 @@ def most_probable_clusters(chain):
     R = chain.num_records
     if R == 0:
         return np.zeros(0, np.int64), np.zeros(0)
-    post = Posterior(R, len(chain.samples))
-    try:
-        for mem, off, _ in chain.samples:
-            post.add_sample(sample_clusters(R, mem, off))
+    with Posterior(R, len(chain.samples)) as post:
+        _add_chain(post, chain)
         return post.smpc()
-    finally:
-        post.close()
 
 
 def shared_most_probable_clusters(chain):
@@ -99,28 +123,17 @@ def shared_most_probable_clusters(chain):
     return most_probable_clusters(chain)[0]
 
 
-class Pairs:
+class Pairs(_Handle):
     """Owner of a dbl_pairs handle: samples go in one at a time, read() gives the pairwise match counts."""
 
+    _prefix = "dbl_pairs"
+
     def __init__(self, num_records, max_pairs=MAX_PAIRS):
-        self._lib = _lib.load()
-        self._h = C.c_void_p()
-        self.num_records = int(num_records)
-        _check(self._lib.dbl_pairs_create(C.byref(self._h), self.num_records, int(max_pairs)), "dbl_pairs_create")
-
-    def add_sample(self, cluster):
-        cluster = np.ascontiguousarray(cluster, np.int32)
-        if cluster.shape != (self.num_records,):
-            raise ValueError("a sample needs one cluster label per record")
-        _check(self._lib.dbl_pairs_add_sample(self._h, cluster.ctypes.data), "dbl_pairs_add_sample")
-
-    @property
-    def num_samples(self):
-        return self._lib.dbl_pairs_num_samples(self._h)
+        super().__init__(num_records, int(max_pairs))
 
     def count(self, min_count=1):
         n = C.c_int64()
-        _check(self._lib.dbl_pairs_count(self._h, int(min_count), C.byref(n)), "dbl_pairs_count")
+        self._call("count", self._h, int(min_count), C.byref(n))
         return n.value
 
     def read(self, min_count=1):
@@ -128,13 +141,8 @@ class Pairs:
         n = self.count(min_count)
         out = [np.empty(n, np.int32) for _ in range(3)]
         if n:
-            _check(self._lib.dbl_pairs_read(self._h, int(min_count), *(a.ctypes.data for a in out)), "dbl_pairs_read")
+            self._call("read", self._h, int(min_count), *(a.ctypes.data for a in out))
         return tuple(a.astype(np.int64) for a in out)
-
-    def close(self):
-        if self._h:
-            self._lib.dbl_pairs_free(self._h)
-            self._h = C.c_void_p()
 
 
 def pairwise_match_counts(chain, max_pairs=MAX_PAIRS, min_count=1):
@@ -142,55 +150,33 @@ def pairwise_match_counts(chain, max_pairs=MAX_PAIRS, min_count=1):
     R = chain.num_records
     if R == 0 or not chain.samples:
         return tuple(np.zeros(0, np.int64) for _ in range(3))
-    pairs = Pairs(R, max_pairs)
-    try:
-        for mem, off, _ in chain.samples:
-            cluster = sample_clusters(R, mem, off)  # the labels are valid, so DBL_ERR_INVALID below means the cap
-            try:
-                pairs.add_sample(cluster)
-            except DblinkError as e:
-                if e.status == _lib.ERR_INVALID:
-                    raise too_many_pairs(max_pairs) from e
-                raise
+    with Pairs(R, max_pairs) as pairs:
+        try:
+            _add_chain(pairs, chain)
+        except DblinkError as e:  # the labels are valid, so DBL_ERR_INVALID means the cap
+            if e.status == _lib.ERR_INVALID:
+                raise too_many_pairs(max_pairs) from e
+            raise
         return pairs.read(min_count)
-    finally:
-        pairs.close()
 
 
-class Evaluation:
+class Evaluation(_Handle):
     """Owner of a dbl_eval handle: the ground truth goes in once, samples one at a time, read() gives the per-sample
     counts."""
 
+    _prefix = "dbl_eval"
+
     def __init__(self, num_records, truth, max_samples):
-        self._lib = _lib.load()
-        self._h = C.c_void_p()
-        self.num_records = int(num_records)
         truth = np.ascontiguousarray(truth, np.int32)
-        if truth.shape != (self.num_records,):
+        if truth.shape != (int(num_records),):
             raise ValueError("the ground truth needs one label per record")
-        _check(self._lib.dbl_eval_create(C.byref(self._h), self.num_records, truth.ctypes.data, int(max_samples)),
-               "dbl_eval_create")
-
-    def add_sample(self, cluster):
-        cluster = np.ascontiguousarray(cluster, np.int32)
-        if cluster.shape != (self.num_records,):
-            raise ValueError("a sample needs one cluster label per record")
-        _check(self._lib.dbl_eval_add_sample(self._h, cluster.ctypes.data), "dbl_eval_add_sample")
-
-    @property
-    def num_samples(self):
-        return self._lib.dbl_eval_num_samples(self._h)
+        super().__init__(num_records, truth.ctypes.data, int(max_samples))
 
     def read(self):
         """(tp, pred_pairs, num_clusters), int64[S]."""
         out = [np.empty(self.num_samples, np.int64) for _ in range(3)]
-        _check(self._lib.dbl_eval_read(self._h, *(a.ctypes.data_as(_lib.i64p) for a in out)), "dbl_eval_read")
+        self._call("read", self._h, *(a.ctypes.data_as(_lib.i64p) for a in out))
         return tuple(out)
-
-    def close(self):
-        if self._h:
-            self._lib.dbl_eval_free(self._h)
-            self._h = C.c_void_p()
 
 
 def posterior_metric_counts(chain, truth):
@@ -199,10 +185,6 @@ def posterior_metric_counts(chain, truth):
     if R == 0 or not chain.samples:
         return tuple(np.zeros(len(chain.samples), np.int64) for _ in range(3))
     _, dense = np.unique(np.asarray(truth), return_inverse=True)  # any labels -> [0, number of entities)
-    ev = Evaluation(R, dense, len(chain.samples))
-    try:
-        for mem, off, _ in chain.samples:
-            ev.add_sample(sample_clusters(R, mem, off))
+    with Evaluation(R, dense, len(chain.samples)) as ev:
+        _add_chain(ev, chain)
         return ev.read()
-    finally:
-        ev.close()

@@ -119,8 +119,9 @@ __global__ void k_iota(int64_t n, int32_t *__restrict__ out) {
     out[i] = (int32_t)i;
 }
 
-// position of every run head of the sorted best signatures, 0 elsewhere (a max-scan then gives each element its head)
-__global__ void k_run_heads(int64_t n, const unsigned long long *__restrict__ keys, int32_t *__restrict__ head) {
+// position of every run head of sorted keys, 0 elsewhere (a max-scan then gives each position its run's start)
+template <class T>
+__global__ void k_run_heads(int64_t n, const T *__restrict__ keys, int32_t *__restrict__ head) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     head[i] = (i == 0 || keys[i] != keys[i - 1]) ? (int32_t)i : 0;
 }
@@ -136,10 +137,26 @@ struct MaxOp {
   __device__ __forceinline__ int32_t operator()(int32_t a, int32_t b) const { return a > b ? a : b; }
 };
 
+// A device buffer.  alloc() takes exactly what it is asked for; reserve() only grows: to at least twice its size, at
+// most `limit` bytes unless more is needed, and a new allocation replaces the old one only once it has succeeded.
 struct Buf {
   void *p = nullptr;
-  cudaError_t alloc(size_t bytes) { return cudaMalloc(&p, std::max<size_t>(bytes, 16)); }
+  size_t cap = 0;
   ~Buf() { if (p) cudaFree(p); }
+  cudaError_t alloc(size_t bytes) {
+    const cudaError_t e = cudaMalloc(&p, std::max<size_t>(bytes, 16));
+    if (e == cudaSuccess) cap = bytes;
+    return e;
+  }
+  cudaError_t reserve(size_t need, size_t limit = SIZE_MAX) {
+    if (need <= cap) return cudaSuccess;
+    Buf nb;
+    const cudaError_t e = nb.alloc(std::max(need, std::min(limit, cap > SIZE_MAX / 2 ? SIZE_MAX : 2 * cap)));
+    if (e != cudaSuccess) return e;
+    std::swap(p, nb.p);  // nb now frees the old buffer
+    std::swap(cap, nb.cap);
+    return cudaSuccess;
+  }
   template <class T> T *as() const { return (T *)p; }
 };
 
@@ -152,19 +169,6 @@ struct DeviceScope {
   }
   ~DeviceScope() { if (prev >= 0 && prev != dev) cudaSetDevice(prev); }
 };
-}  // namespace
-
-struct dbl_posterior {
-  int device = 0;
-  int64_t R = 0;
-  int32_t max_samples = 0, S = 0;
-  cudaStream_t stream = nullptr;
-  Buf sig;      // [R][max_samples] signatures
-  Buf cluster;  // R labels of the sample being added
-  Buf sum;      // R wrapping sums of mix64(record) per cluster
-  Buf size;     // R cluster sizes
-  Buf bad;      // label check flag
-};
 
 #define POST_TRY(expr)                   \
   do {                                   \
@@ -174,34 +178,30 @@ struct dbl_posterior {
     }                                    \
   } while (0)
 
-extern "C" int dbl_posterior_create(dbl_posterior **out, int64_t num_records, int32_t max_samples) {
-  if (!out) return DBL_ERR_INVALID;
-  *out = nullptr;
-  // a record's S samples are sorted in one block, so max_samples <= PAIR_BLOCK
-  if (num_records <= 0 || num_records > INT32_MAX || max_samples <= 0 || max_samples > PAIR_BLOCK)
-    return DBL_ERR_INVALID;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return DBL_ERR_CUDA; }
-  auto *p = new dbl_posterior();
-  p->R = num_records;
-  p->max_samples = max_samples;
-  int rc = DBL_OK;
-  if (cudaGetDevice(&p->device) != cudaSuccess || cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      p->sig.alloc(sizeof(unsigned long long) * (size_t)num_records * (size_t)max_samples) != cudaSuccess ||
-      p->cluster.alloc(sizeof(int32_t) * (size_t)num_records) != cudaSuccess ||
-      p->sum.alloc(sizeof(unsigned long long) * (size_t)num_records) != cudaSuccess ||
-      p->size.alloc(sizeof(unsigned int) * (size_t)num_records) != cudaSuccess || p->bad.alloc(sizeof(int)) != cudaSuccess)
-    rc = DBL_ERR_CUDA;  // no device, or the signature matrix does not fit
-  if (rc != DBL_OK) {
-    cudaGetLastError();
-    dbl_posterior_free(p);
-    return rc;
-  }
-  *out = p;
-  return DBL_OK;
-}
+// What every handle holds: its device, R, the number of samples added, its stream, the labels of the sample being
+// added and the label check flag.
+struct Handle {
+  int device = 0;
+  int64_t R = 0;
+  int32_t S = 0;
+  cudaStream_t stream = nullptr;
+  Buf cluster, bad;
 
-extern "C" void dbl_posterior_free(dbl_posterior *p) {
+  // R labels, host or device (unified addressing picks the copy direction), into dst, then the range check:
+  // DBL_ERR_INVALID when one is outside [0, R)
+  int take_labels(const int32_t *labels, Buf &dst) {
+    POST_TRY(cudaMemcpyAsync(dst.p, labels, sizeof(int32_t) * R, cudaMemcpyDefault, stream));
+    POST_TRY(cudaMemsetAsync(bad.p, 0, sizeof(int), stream));
+    k_check_labels<<<grid_for(R), THREADS, 0, stream>>>(R, dst.as<int32_t>(), bad.as<int>());
+    int flag = 0;
+    POST_TRY(cudaMemcpyAsync(&flag, bad.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    POST_TRY(cudaStreamSynchronize(stream));
+    return flag ? DBL_ERR_INVALID : DBL_OK;
+  }
+};
+
+template <class H>
+void free_handle(H *p) {
   if (!p) return;
   DeviceScope ds(p->device);
   if (p->stream) {
@@ -211,22 +211,85 @@ extern "C" void dbl_posterior_free(dbl_posterior *p) {
   delete p;  // Buf destructors free the device memory
 }
 
+// A create, once its own arguments are checked: a device must exist; the handle lives on the current one, with its
+// stream, sample labels and check flag, then init(p) allocates the rest.  On failure the half-built handle is freed.
+template <class H, class Init>
+int open_handle(H **out, int64_t num_records, Init init) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    return DBL_ERR_CUDA;
+  }
+  auto *p = new H();
+  p->R = num_records;
+  int rc = DBL_ERR_CUDA;
+  if (cudaGetDevice(&p->device) == cudaSuccess &&
+      cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking) == cudaSuccess &&
+      p->cluster.alloc(sizeof(int32_t) * (size_t)num_records) == cudaSuccess && p->bad.alloc(sizeof(int)) == cudaSuccess)
+    rc = init(p);
+  if (rc != DBL_OK) {
+    cudaGetLastError();
+    free_handle(p);
+    return rc;
+  }
+  *out = p;
+  return DBL_OK;
+}
+
+// Records grouped by key: a stable radix sort of (key, record) over bits [0, end_bit), then every sorted position's
+// run start, an inclusive max-scan of the run heads.  The sort is stable, so a run keeps its records in their order in
+// rec.  key_s, rec_s and start receive the n sorted keys, sorted records and run starts; head is n entries of scratch;
+// tmp grows to the temporary storage of the sort and the scan.
+template <class T>
+int group_by_key(int64_t n, int end_bit, const T *key, const int32_t *rec, T *key_s, int32_t *rec_s, int32_t *head,
+                 int32_t *start, Buf &tmp, cudaStream_t st) {
+  size_t tb_sort = 0, tb_scan = 0;
+  POST_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb_sort, key, key_s, rec, rec_s, n, 0, end_bit, st));
+  POST_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb_scan, head, start, MaxOp(), n, st));
+  POST_TRY(tmp.reserve(std::max(tb_sort, tb_scan)));
+  size_t tb = tmp.cap;
+  POST_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key, key_s, rec, rec_s, n, 0, end_bit, st));
+  k_run_heads<<<grid_for(n), THREADS, 0, st>>>(n, key_s, head);
+  tb = tmp.cap;
+  POST_TRY(cub::DeviceScan::InclusiveScan(tmp.p, tb, head, start, MaxOp(), n, st));
+  return DBL_OK;
+}
+}  // namespace
+
+struct dbl_posterior : Handle {
+  int32_t max_samples = 0;
+  Buf sig;   // [R][max_samples] signatures
+  Buf sum;   // R wrapping sums of mix64(record) per cluster
+  Buf size;  // R cluster sizes
+};
+
+extern "C" int dbl_posterior_create(dbl_posterior **out, int64_t num_records, int32_t max_samples) {
+  if (!out) return DBL_ERR_INVALID;
+  *out = nullptr;
+  // a record's S samples are sorted in one block, so max_samples <= PAIR_BLOCK
+  if (num_records <= 0 || num_records > INT32_MAX || max_samples <= 0 || max_samples > PAIR_BLOCK)
+    return DBL_ERR_INVALID;
+  return open_handle(out, num_records, [&](dbl_posterior *p) {
+    p->max_samples = max_samples;
+    if (p->sig.alloc(sizeof(unsigned long long) * (size_t)num_records * (size_t)max_samples) != cudaSuccess ||
+        p->sum.alloc(sizeof(unsigned long long) * (size_t)num_records) != cudaSuccess ||
+        p->size.alloc(sizeof(unsigned int) * (size_t)num_records) != cudaSuccess)
+      return DBL_ERR_CUDA;  // the signature matrix does not fit
+    return DBL_OK;
+  });
+}
+
+extern "C" void dbl_posterior_free(dbl_posterior *p) { free_handle(p); }
+
 extern "C" int32_t dbl_posterior_num_samples(const dbl_posterior *p) { return p ? p->S : 0; }
 
 extern "C" int dbl_posterior_add_sample(dbl_posterior *p, const int32_t *cluster) {
   if (!p || !cluster || p->S >= p->max_samples) return DBL_ERR_INVALID;
   DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(cluster, p->cluster); rc != DBL_OK) return rc;
   const int64_t R = p->R;
   cudaStream_t st = p->stream;
   const int32_t *c = p->cluster.as<int32_t>();
-  // host or device labels: unified addressing picks the copy direction
-  POST_TRY(cudaMemcpyAsync(p->cluster.p, cluster, sizeof(int32_t) * R, cudaMemcpyDefault, st));
-  POST_TRY(cudaMemsetAsync(p->bad.p, 0, sizeof(int), st));
-  k_check_labels<<<grid_for(R), THREADS, 0, st>>>(R, c, p->bad.as<int>());
-  int bad = 0;
-  POST_TRY(cudaMemcpyAsync(&bad, p->bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  POST_TRY(cudaStreamSynchronize(st));
-  if (bad) return DBL_ERR_INVALID;
   POST_TRY(cudaMemsetAsync(p->sum.p, 0, sizeof(unsigned long long) * R, st));
   POST_TRY(cudaMemsetAsync(p->size.p, 0, sizeof(unsigned int) * R, st));
   k_accumulate<<<grid_for(R), THREADS, 0, st>>>(R, c, p->sum.as<unsigned long long>(), p->size.as<unsigned int>());
@@ -280,30 +343,20 @@ extern "C" int dbl_posterior_smpc(dbl_posterior *p, int32_t *labels_out, double 
   }
   if (freq_out) POST_TRY(cudaMemcpy(freq_out, freq.p, sizeof(double) * R, cudaMemcpyDeviceToHost));
   if (!labels_out) return DBL_OK;
-  // group records by best signature: stable sort of (signature, record), run heads, max-scan, scatter
-  Buf rec_in, keys_s, rec_s, head, head_scan, labels, tmp;
+  // group records by best signature, then scatter each group's smallest record index to its records
+  Buf rec_in, keys_s, rec_s, head, start, labels, tmp;
   POST_TRY(rec_in.alloc(sizeof(int32_t) * R));
   POST_TRY(keys_s.alloc(sizeof(unsigned long long) * R));
   POST_TRY(rec_s.alloc(sizeof(int32_t) * R));
   POST_TRY(head.alloc(sizeof(int32_t) * R));
-  POST_TRY(head_scan.alloc(sizeof(int32_t) * R));
+  POST_TRY(start.alloc(sizeof(int32_t) * R));
   POST_TRY(labels.alloc(sizeof(int32_t) * R));
-  size_t tb_sort = 0, tb_scan = 0;
-  POST_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb_sort, (const unsigned long long *)nullptr,
-                                           (unsigned long long *)nullptr, (const int32_t *)nullptr, (int32_t *)nullptr,
-                                           (int)R, 0, 64, st));
-  POST_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb_scan, (const int32_t *)nullptr, (int32_t *)nullptr, MaxOp(),
-                                          (int)R, st));
-  POST_TRY(tmp.alloc(std::max(tb_sort, tb_scan)));
   k_iota<<<grid_for(R), THREADS, 0, st>>>(R, rec_in.as<int32_t>());
-  POST_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tb_sort, best.as<unsigned long long>(),
-                                           keys_s.as<unsigned long long>(), rec_in.as<int32_t>(), rec_s.as<int32_t>(),
-                                           (int)R, 0, 64, st));
-  k_run_heads<<<grid_for(R), THREADS, 0, st>>>(R, keys_s.as<unsigned long long>(), head.as<int32_t>());
-  POST_TRY(cub::DeviceScan::InclusiveScan(tmp.p, tb_scan, head.as<int32_t>(), head_scan.as<int32_t>(), MaxOp(), (int)R,
-                                          st));
-  k_scatter_labels<<<grid_for(R), THREADS, 0, st>>>(R, rec_s.as<int32_t>(), head_scan.as<int32_t>(),
-                                                    labels.as<int32_t>());
+  const int rc = group_by_key(R, 64, best.as<unsigned long long>(), rec_in.as<int32_t>(),
+                              keys_s.as<unsigned long long>(), rec_s.as<int32_t>(), head.as<int32_t>(),
+                              start.as<int32_t>(), tmp, st);
+  if (rc != DBL_OK) return rc;
+  k_scatter_labels<<<grid_for(R), THREADS, 0, st>>>(R, rec_s.as<int32_t>(), start.as<int32_t>(), labels.as<int32_t>());
   POST_TRY(cudaGetLastError());
   POST_TRY(cudaMemcpyAsync(labels_out, labels.p, sizeof(int32_t) * R, cudaMemcpyDeviceToHost, st));
   POST_TRY(cudaStreamSynchronize(st));
@@ -330,13 +383,6 @@ __device__ __forceinline__ int64_t lower_bound_u64(const unsigned long long *__r
     else hi = mid;
   }
   return lo;
-}
-
-// records sorted stably by label: position of every run head (cluster start), 0 elsewhere; a max-scan then gives
-// every position the start of its cluster
-__global__ void k_label_heads(int64_t R, const int32_t *__restrict__ lab, int32_t *__restrict__ head) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x)
-    head[i] = (i == 0 || lab[i] != lab[i - 1]) ? (int32_t)i : 0;
 }
 
 // the last position of each cluster writes the cluster's size at its first position
@@ -427,83 +473,42 @@ __global__ void k_scatter_pairs(int64_t H, const unsigned long long *__restrict_
     count[p] = cnt[i];
   }
 }
-
-// a device buffer that only grows: to at least twice its size, at most `limit` bytes unless more is needed.  A new
-// allocation replaces the old one only once it has succeeded.
-struct Grow {
-  Buf buf;
-  size_t cap = 0;
-  cudaError_t reserve(size_t need, size_t limit = SIZE_MAX) {
-    if (need <= cap) return cudaSuccess;
-    const size_t bytes = std::max(need, std::min(limit, cap > SIZE_MAX / 2 ? SIZE_MAX : 2 * cap));
-    Buf nb;
-    const cudaError_t e = nb.alloc(bytes);
-    if (e != cudaSuccess) return e;
-    std::swap(buf.p, nb.p);  // nb now frees the old buffer
-    cap = bytes;
-    return cudaSuccess;
-  }
-  template <class T> T *as() const { return buf.as<T>(); }
-};
 }  // namespace
 
-struct dbl_pairs {
-  int device = 0;
-  int64_t R = 0, max_pairs = 0, H = 0;  // H = distinct pairs held
-  int32_t S = 0;
+struct dbl_pairs : Handle {
+  int64_t max_pairs = 0, H = 0;         // H = distinct pairs held
   int lab_bits = 1, key_bits = 33;      // radix sort end bits of the labels and of the pair keys
-  cudaStream_t stream = nullptr;
-  Buf cluster, bad;                     // the sample's labels, label check flag
   Buf iota, lab_s, rec_s;               // record indices; labels and records sorted by label
   Buf head, start, size;                // run heads, cluster start per position, cluster size at its start
   Buf row, off;                         // int64 row lengths and their exclusive scan, R + 1 each
-  Grow key_in, key_s, is_new, rank;     // the sample's pair keys (unsorted, sorted) and their merge ranks
-  Grow tab_key[2], tab_cnt[2];          // held table (index cur) and the one the next sample merges into
+  Buf key_in, key_s, is_new, rank;      // grown on demand: the sample's pair keys (unsorted, sorted), merge ranks
+  Buf tab_key[2], tab_cnt[2];           // grown on demand: held table (index cur), the one the next sample merges into
   int cur = 0;
-  Grow tmp;                             // CUB temporary storage
+  Buf tmp;                              // CUB temporary storage, grown on demand
 };
 
 extern "C" int dbl_pairs_create(dbl_pairs **out, int64_t num_records, int64_t max_pairs) {
   if (!out) return DBL_ERR_INVALID;
   *out = nullptr;
   if (num_records <= 0 || num_records > INT32_MAX || max_pairs <= 0 || max_pairs > INT32_MAX) return DBL_ERR_INVALID;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return DBL_ERR_CUDA; }
-  auto *p = new dbl_pairs();
-  const int64_t R = num_records;
-  p->R = R;
-  p->max_pairs = max_pairs;
-  p->lab_bits = bits_for(R);
-  p->key_bits = 32 + bits_for(R);
-  const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(long long) * (size_t)(R + 1);
-  if (cudaGetDevice(&p->device) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking) != cudaSuccess || p->cluster.alloc(r4) != cudaSuccess ||
-      p->bad.alloc(sizeof(int)) != cudaSuccess || p->iota.alloc(r4) != cudaSuccess || p->lab_s.alloc(r4) != cudaSuccess ||
-      p->rec_s.alloc(r4) != cudaSuccess || p->head.alloc(r4) != cudaSuccess || p->start.alloc(r4) != cudaSuccess ||
-      p->size.alloc(r4) != cudaSuccess || p->row.alloc(r8) != cudaSuccess || p->off.alloc(r8) != cudaSuccess) {
-    cudaGetLastError();
-    dbl_pairs_free(p);
-    return DBL_ERR_CUDA;
-  }
-  k_iota<<<grid_for(R), THREADS, 0, p->stream>>>(R, p->iota.as<int32_t>());
-  if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(p->stream) != cudaSuccess) {
-    cudaGetLastError();
-    dbl_pairs_free(p);
-    return DBL_ERR_CUDA;
-  }
-  *out = p;
-  return DBL_OK;
+  return open_handle(out, num_records, [&](dbl_pairs *p) {
+    const int64_t R = num_records;
+    p->max_pairs = max_pairs;
+    p->lab_bits = bits_for(R);
+    p->key_bits = 32 + bits_for(R);
+    const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(long long) * (size_t)(R + 1);
+    if (p->iota.alloc(r4) != cudaSuccess || p->lab_s.alloc(r4) != cudaSuccess || p->rec_s.alloc(r4) != cudaSuccess ||
+        p->head.alloc(r4) != cudaSuccess || p->start.alloc(r4) != cudaSuccess || p->size.alloc(r4) != cudaSuccess ||
+        p->row.alloc(r8) != cudaSuccess || p->off.alloc(r8) != cudaSuccess)
+      return DBL_ERR_CUDA;
+    k_iota<<<grid_for(R), THREADS, 0, p->stream>>>(R, p->iota.as<int32_t>());
+    POST_TRY(cudaGetLastError());
+    POST_TRY(cudaStreamSynchronize(p->stream));
+    return DBL_OK;
+  });
 }
 
-extern "C" void dbl_pairs_free(dbl_pairs *p) {
-  if (!p) return;
-  DeviceScope ds(p->device);
-  if (p->stream) {
-    cudaStreamSynchronize(p->stream);
-    cudaStreamDestroy(p->stream);
-  }
-  delete p;
-}
+extern "C" void dbl_pairs_free(dbl_pairs *p) { free_handle(p); }
 
 extern "C" int32_t dbl_pairs_num_samples(const dbl_pairs *p) { return p ? p->S : 0; }
 
@@ -515,36 +520,23 @@ extern "C" int32_t dbl_pairs_num_samples(const dbl_pairs *p) { return p ? p->S :
 extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
   if (!p || !cluster || p->S == INT32_MAX) return DBL_ERR_INVALID;
   DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(cluster, p->cluster); rc != DBL_OK) return rc;
   const int64_t R = p->R, H = p->H;
   cudaStream_t st = p->stream;
-  POST_TRY(cudaMemcpyAsync(p->cluster.p, cluster, sizeof(int32_t) * R, cudaMemcpyDefault, st));
-  POST_TRY(cudaMemsetAsync(p->bad.p, 0, sizeof(int), st));
-  k_check_labels<<<grid_for(R), THREADS, 0, st>>>(R, p->cluster.as<int32_t>(), p->bad.as<int>());
-  int bad = 0;
-  POST_TRY(cudaMemcpyAsync(&bad, p->bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  POST_TRY(cudaStreamSynchronize(st));
-  if (bad) return DBL_ERR_INVALID;
 
-  // records grouped by label, ascending record index within a cluster
-  size_t tb_sort = 0, tb_max = 0, tb_sum = 0;
-  POST_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb_sort, (const int32_t *)nullptr, (int32_t *)nullptr,
-                                           (const int32_t *)nullptr, (int32_t *)nullptr, R, 0, p->lab_bits, st));
-  POST_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb_max, (const int32_t *)nullptr, (int32_t *)nullptr, MaxOp(), R, st));
-  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb_sum, (const long long *)nullptr, (long long *)nullptr, R + 1, st));
-  POST_TRY(p->tmp.reserve(std::max({tb_sort, tb_max, tb_sum})));
-  size_t tb = p->tmp.cap;
-  POST_TRY(cub::DeviceRadixSort::SortPairs(p->tmp.buf.p, tb, p->cluster.as<int32_t>(), p->lab_s.as<int32_t>(),
-                                           p->iota.as<int32_t>(), p->rec_s.as<int32_t>(), R, 0, p->lab_bits, st));
-  k_label_heads<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_s.as<int32_t>(), p->head.as<int32_t>());
-  tb = p->tmp.cap;
-  POST_TRY(cub::DeviceScan::InclusiveScan(p->tmp.buf.p, tb, p->head.as<int32_t>(), p->start.as<int32_t>(), MaxOp(), R,
-                                          st));
+  // records grouped by label, ascending record index within a cluster; tmp is grown before anything uses it
+  size_t tb = 0;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, p->row.as<long long>(), p->off.as<long long>(), R + 1, st));
+  POST_TRY(p->tmp.reserve(tb));
+  const int rc = group_by_key(R, p->lab_bits, p->cluster.as<int32_t>(), p->iota.as<int32_t>(), p->lab_s.as<int32_t>(),
+                              p->rec_s.as<int32_t>(), p->head.as<int32_t>(), p->start.as<int32_t>(), p->tmp, st);
+  if (rc != DBL_OK) return rc;
   k_cluster_sizes<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_s.as<int32_t>(), p->start.as<int32_t>(),
                                                    p->size.as<int32_t>());
   k_row_lengths<<<grid_for(R + 1), THREADS, 0, st>>>(R, p->start.as<int32_t>(), p->size.as<int32_t>(),
                                                      p->row.as<long long>());
   tb = p->tmp.cap;
-  POST_TRY(cub::DeviceScan::ExclusiveSum(p->tmp.buf.p, tb, p->row.as<long long>(), p->off.as<long long>(), R + 1, st));
+  POST_TRY(cub::DeviceScan::ExclusiveSum(p->tmp.p, tb, p->row.as<long long>(), p->off.as<long long>(), R + 1, st));
   long long n = 0;
   POST_TRY(cudaMemcpyAsync(&n, p->off.as<long long>() + R, sizeof(long long), cudaMemcpyDeviceToHost, st));
   POST_TRY(cudaGetLastError());
@@ -566,7 +558,7 @@ extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
                                             (unsigned long long *)nullptr, (int64_t)n, 0, p->key_bits, st));
     POST_TRY(p->tmp.reserve(tbk));
     tbk = p->tmp.cap;
-    POST_TRY(cub::DeviceRadixSort::SortKeys(p->tmp.buf.p, tbk, p->key_in.as<unsigned long long>(),
+    POST_TRY(cub::DeviceRadixSort::SortKeys(p->tmp.p, tbk, p->key_in.as<unsigned long long>(),
                                             p->key_s.as<unsigned long long>(), (int64_t)n, 0, p->key_bits, st));
   }
 
@@ -579,7 +571,7 @@ extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
                                          st));
   POST_TRY(p->tmp.reserve(tbr));
   tbr = p->tmp.cap;
-  POST_TRY(cub::DeviceScan::ExclusiveSum(p->tmp.buf.p, tbr, p->is_new.as<int32_t>(), p->rank.as<int32_t>(),
+  POST_TRY(cub::DeviceScan::ExclusiveSum(p->tmp.p, tbr, p->is_new.as<int32_t>(), p->rank.as<int32_t>(),
                                          (int64_t)n + 1, st));
   int32_t fresh = 0;
   POST_TRY(cudaMemcpyAsync(&fresh, p->rank.as<int32_t>() + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -707,72 +699,37 @@ __global__ void k_eval_counts(int64_t R, int lab_bits, const unsigned long long 
 }
 }  // namespace
 
-struct dbl_eval {
-  int device = 0;
-  int64_t R = 0;
-  int32_t max_samples = 0, S = 0;
+struct dbl_eval : Handle {
+  int32_t max_samples = 0;
   int lab_bits = 1;                // bits of a label in [0, R)
-  cudaStream_t stream = nullptr;
-  Buf truth, cluster, bad;         // true labels, the sample's labels, label check flag
+  Buf truth;                       // true labels
   Buf key_in, key_s;               // packed (sample label, true label) per record, unsorted and sorted
   Buf tmp;                         // CUB temporary storage of the key sort
-  size_t tmp_bytes = 0;
   Buf counts;                      // [3][max_samples] uint64: tp, pred_pairs, num_clusters per sample
 };
-
-// labels (host or device) into dst, then the range check; 1 in *bad when one is outside [0, R)
-static int upload_labels(int64_t R, const int32_t *labels, Buf &dst, Buf &flag, cudaStream_t st, int *bad) {
-  POST_TRY(cudaMemcpyAsync(dst.p, labels, sizeof(int32_t) * R, cudaMemcpyDefault, st));
-  POST_TRY(cudaMemsetAsync(flag.p, 0, sizeof(int), st));
-  k_check_labels<<<grid_for(R), THREADS, 0, st>>>(R, dst.as<int32_t>(), flag.as<int>());
-  POST_TRY(cudaMemcpyAsync(bad, flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  POST_TRY(cudaStreamSynchronize(st));
-  return DBL_OK;
-}
 
 extern "C" int dbl_eval_create(dbl_eval **out, int64_t num_records, const int32_t *truth, int32_t max_samples) {
   if (!out) return DBL_ERR_INVALID;
   *out = nullptr;
   if (num_records <= 0 || num_records > INT32_MAX || !truth || max_samples <= 0) return DBL_ERR_INVALID;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return DBL_ERR_CUDA; }
-  auto *p = new dbl_eval();
-  const int64_t R = num_records;
-  p->R = R;
-  p->max_samples = max_samples;
-  p->lab_bits = bits_for(R);
-  const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(unsigned long long) * (size_t)R;
-  int rc = DBL_OK, bad = 0;
-  if (cudaGetDevice(&p->device) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking) != cudaSuccess || p->truth.alloc(r4) != cudaSuccess ||
-      p->cluster.alloc(r4) != cudaSuccess || p->bad.alloc(sizeof(int)) != cudaSuccess ||
-      p->key_in.alloc(r8) != cudaSuccess || p->key_s.alloc(r8) != cudaSuccess ||
-      p->counts.alloc(3 * sizeof(unsigned long long) * (size_t)max_samples) != cudaSuccess ||
-      cub::DeviceRadixSort::SortKeys(nullptr, p->tmp_bytes, (const unsigned long long *)nullptr,
-                                     (unsigned long long *)nullptr, R, 0, 2 * p->lab_bits, p->stream) != cudaSuccess ||
-      p->tmp.alloc(p->tmp_bytes) != cudaSuccess)
-    rc = DBL_ERR_CUDA;
-  else
-    rc = upload_labels(R, truth, p->truth, p->bad, p->stream, &bad);
-  if (rc == DBL_OK && bad) rc = DBL_ERR_INVALID;
-  if (rc != DBL_OK) {
-    cudaGetLastError();
-    dbl_eval_free(p);
-    return rc;
-  }
-  *out = p;
-  return DBL_OK;
+  return open_handle(out, num_records, [&](dbl_eval *p) {
+    const int64_t R = num_records;
+    p->max_samples = max_samples;
+    p->lab_bits = bits_for(R);
+    const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(unsigned long long) * (size_t)R;
+    size_t tb = 0;
+    if (p->truth.alloc(r4) != cudaSuccess || p->key_in.alloc(r8) != cudaSuccess || p->key_s.alloc(r8) != cudaSuccess ||
+        p->counts.alloc(3 * sizeof(unsigned long long) * (size_t)max_samples) != cudaSuccess ||
+        cub::DeviceRadixSort::SortKeys(nullptr, tb, p->key_in.as<unsigned long long>(),
+                                       p->key_s.as<unsigned long long>(), R, 0, 2 * p->lab_bits,
+                                       p->stream) != cudaSuccess ||
+        p->tmp.alloc(tb) != cudaSuccess)
+      return DBL_ERR_CUDA;
+    return p->take_labels(truth, p->truth);
+  });
 }
 
-extern "C" void dbl_eval_free(dbl_eval *p) {
-  if (!p) return;
-  DeviceScope ds(p->device);
-  if (p->stream) {
-    cudaStreamSynchronize(p->stream);
-    cudaStreamDestroy(p->stream);
-  }
-  delete p;
-}
+extern "C" void dbl_eval_free(dbl_eval *p) { free_handle(p); }
 
 extern "C" int32_t dbl_eval_num_samples(const dbl_eval *p) { return p ? p->S : 0; }
 
@@ -781,15 +738,12 @@ extern "C" int32_t dbl_eval_num_samples(const dbl_eval *p) { return p ? p->S : 0
 extern "C" int dbl_eval_add_sample(dbl_eval *p, const int32_t *cluster) {
   if (!p || !cluster || p->S >= p->max_samples) return DBL_ERR_INVALID;
   DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(cluster, p->cluster); rc != DBL_OK) return rc;
   const int64_t R = p->R;
   cudaStream_t st = p->stream;
-  int bad = 0;
-  const int rc = upload_labels(R, cluster, p->cluster, p->bad, st, &bad);
-  if (rc != DBL_OK) return rc;
-  if (bad) return DBL_ERR_INVALID;
   k_pack_labels<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_bits, p->cluster.as<int32_t>(), p->truth.as<int32_t>(),
                                                  p->key_in.as<unsigned long long>());
-  size_t tb = p->tmp_bytes;
+  size_t tb = p->tmp.cap;
   POST_TRY(cub::DeviceRadixSort::SortKeys(p->tmp.p, tb, p->key_in.as<unsigned long long>(),
                                           p->key_s.as<unsigned long long>(), R, 0, 2 * p->lab_bits, st));
   unsigned long long *c = p->counts.as<unsigned long long>() + p->S;
