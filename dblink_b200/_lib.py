@@ -135,6 +135,7 @@ SIGNATURES = {
     "dbl_pairs_num_samples": (C.c_int32, [vp]),
     "dbl_pairs_count": (C.c_int, [vp, C.c_int32, i64p]),
     "dbl_pairs_read": (C.c_int, [vp, C.c_int32, vp, vp, vp]),
+    "dbl_pairs_score_sample": (C.c_int, [vp, vp, i64p, i64p]),
     "dbl_eval_create": (C.c_int, [C.POINTER(vp), C.c_int64, vp, C.c_int32]),
     "dbl_eval_free": (None, [vp]),
     "dbl_eval_add_sample": (C.c_int, [vp, vp]),

@@ -2,6 +2,7 @@
 
   most_probable_clusters / shared_most_probable_clusters  <- LinkageChain.scala:52-109
   pairwise_match_probabilities                            <- posterior probability that two records are one entity
+  binder_clusters                                         <- the sample of least posterior expected Binder loss
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
   pairwise_metrics                                        <- analysis/PairwiseMetrics.scala:44-63,
                                                              BinaryClassificationMetrics.scala:23-37
@@ -11,6 +12,7 @@ A linkage chain is a list of samples; a sample is (iteration, {partition_id: [cl
 collections of record ids (what linkage-chain.parquet stores, package.scala:94-96).
 """
 import collections
+import fractions
 import itertools
 import math
 
@@ -60,6 +62,29 @@ def pairwise_match_probabilities(chain):
             for a, b in itertools.combinations(c, 2):
                 count[frozenset((a, b))] += 1
     return {pair: k / n for pair, k in count.items()}
+
+
+def binder_clusters(chain, false_link_cost=0.5):
+    """The sample of least posterior expected Binder loss, by the definition: a pair linked in the sample costs
+    t (1 - p), a pair not linked costs (1 - t) p, summed over every pair of records, where t = false_link_cost and p
+    = the fraction of samples linking the pair.  Exact rational arithmetic; ties go to the earliest sample.  Returns
+    (position of the sample in the chain, its clusters as frozensets, every sample's loss as a float)."""
+    t = fractions.Fraction(false_link_cost)
+    S = len(chain)
+    clusters = [list(clusters_of_sample(s)) for s in chain]
+    records = sorted({r for cl in clusters for c in cl for r in c})
+    linked = [{frozenset(p) for c in cl for p in itertools.combinations(c, 2)} for cl in clusters]
+    count = collections.Counter(p for ls in linked for p in ls)
+    losses = []
+    for ls in linked:
+        loss = fractions.Fraction(0)
+        for a, b in itertools.combinations(records, 2):
+            pair = frozenset((a, b))
+            p = fractions.Fraction(count[pair], S)
+            loss += t * (1 - p) if pair in ls else (1 - t) * p
+        losses.append(loss)
+    best = min(range(S), key=lambda s: (losses[s], s))
+    return best, clusters[best], [float(x) for x in losses]
 
 
 def cluster_size_distribution(chain):
@@ -141,6 +166,25 @@ def format_cluster(ari):
     return ("=====================================\n          Cluster metrics            \n"
             "-------------------------------------\n"
             f" Adj. Rand index: {ari}\n=====================================\n")
+
+
+def _binder_estimate_line(iteration, chain, false_link_cost):
+    return f" Estimate:        sample at iteration {iteration} of chain {chain}, falseLinkCost {false_link_cost}\n"
+
+
+def format_binder_pairwise(m, iteration, chain, false_link_cost):
+    """The binder-pairwise section: m = pairwise metrics of the sample chosen at (iteration, chain)."""
+    return ("=====================================\n      Binder pairwise metrics\n"
+            "-------------------------------------\n" + _binder_estimate_line(iteration, chain, false_link_cost)
+            + f" Precision:      {m['precision']}\n Recall:         {m['recall']}\n F1-score:       {m['f1score']}\n"
+            "=====================================\n")
+
+
+def format_binder_cluster(ari, iteration, chain, false_link_cost):
+    """The binder-cluster section: ari = adjusted Rand index of the sample chosen at (iteration, chain)."""
+    return ("=====================================\n       Binder cluster metrics\n"
+            "-------------------------------------\n" + _binder_estimate_line(iteration, chain, false_link_cost)
+            + f" Adj. Rand index: {ari}\n=====================================\n")
 
 
 def _posterior_line(label, s, extra=""):

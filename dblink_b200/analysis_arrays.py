@@ -13,10 +13,12 @@ import numpy as np
 
 # ---- reading the chain -------------------------------------------------------------------------------
 class ChainArrays:
-    def __init__(self, record_ids, iterations, samples):
+    def __init__(self, record_ids, iterations, samples, chains=None):
         self.record_ids = record_ids  # pyarrow string array: index -> record id
         self.iterations = iterations  # int64[S], ascending
         self.samples = samples        # list of (members int32[n], offsets int64[nc+1], partition int32[nc])
+        # int64[S]: the chain each sample comes from (all 0 unless read_pooled_chain_arrays pooled several)
+        self.chains = np.zeros(len(samples), np.int64) if chains is None else np.asarray(chains, np.int64)
 
     @property
     def num_records(self):
@@ -71,7 +73,8 @@ def read_pooled_chain_arrays(paths, lower_iteration_cutoff=0):
     """The samples of several chains (one linkage-chain.parquet each) at or after the cutoff, pooled into ONE
     ChainArrays: chain-major, then by iteration (the order that defines the sMPC tie rule "earliest sample").  Every
     chain's ids are mapped through the first chain's record-id dictionary; chains that mention different records are
-    refused.  `iterations` is then ascending within each chain only."""
+    refused.  `iterations` is then ascending within each chain only; `chains` gives each sample's chain (its position
+    in `paths`)."""
     import pyarrow as pa
     import pyarrow.compute as pc
 
@@ -79,8 +82,8 @@ def read_pooled_chain_arrays(paths, lower_iteration_cutoff=0):
     if not chains:
         raise ValueError("no chains to pool")
     ids = chains[0].record_ids
-    its, samples = [], []
-    for ch in chains:
+    its, samples, which = [], [], []
+    for k, ch in enumerate(chains):
         if len(ch.record_ids) != len(ids):
             raise ValueError("the chains mention different records")
         pos = pc.index_in(ch.record_ids, value_set=ids)
@@ -90,8 +93,9 @@ def read_pooled_chain_arrays(paths, lower_iteration_cutoff=0):
         for mem, off, part in ch.samples:
             samples.append((remap[mem], off, part))
         its.append(ch.iterations)
+        which.append(np.full(len(ch.samples), k, np.int64))
     return ChainArrays(ids if len(ids) else pa.array([], pa.string()),
-                       np.concatenate(its) if its else np.zeros(0, np.int64), samples)
+                       np.concatenate(its) if its else np.zeros(0, np.int64), samples, np.concatenate(which))
 
 
 def sample_from_links(link, block_of_entity):
@@ -253,6 +257,65 @@ def pairwise_match_counts(chain, max_pairs=MAX_PAIRS, min_count=1):
     keep = cnt >= min_count
     keys, cnt = keys[keep], cnt[keep]
     return keys >> 32, keys & 0xFFFFFFFF, cnt
+
+
+def sample_labels(num_records, members, offsets):
+    """int64 labels[R] of one sample: every record labelled by the smallest record index of its cluster, as the sMPC
+    labels its groups (so labels_to_clusters orders both the same way)."""
+    members = np.asarray(members)
+    offsets = np.asarray(offsets, np.int64)
+    sizes = np.diff(offsets)
+    if len(members) != num_records or (sizes <= 0).any():
+        raise ValueError("every sample must mention every record exactly once")
+    labels = np.full(num_records, -1, np.int64)
+    if num_records:
+        labels[members] = np.repeat(np.minimum.reduceat(members, offsets[:-1]), sizes)
+    if (labels < 0).any():
+        raise ValueError("every sample must mention every record exactly once")
+    return labels
+
+
+# ---- the Binder-loss point estimate ---------------------------------------------------------------------
+# With count(i, j) = the samples in which records i and j share a cluster (p_ij = count / S) and t = the cost of a
+# false link (1 - t that of a missed link), the posterior expected Binder loss of a partition c is
+#   E[L(c)] = sum over pairs linked in c of t (1 - p_ij) + sum over pairs not linked in c of (1 - t) p_ij
+#           = ((1 - t) C + t S n(c) - K(c)) / S
+# where n(c) = the pairs c links, K(c) = the sum of count over them and C = the sum of all counts = sum of n over the
+# samples.  The estimate is the sample of least E[L] (Dahl's least-squares clustering at t = 1/2).
+
+def binder_counts(chain, max_pairs=MAX_PAIRS):
+    """(n, K), int64[S]: per sample the record pairs it puts together and the sum of their match counts over the
+    chain.  Raises ValueError as pairwise_match_counts does when the chain has more than max_pairs distinct pairs."""
+    first, second, count = pairwise_match_counts(chain, max_pairs)
+    keys = (first << 32) | second
+    S = len(chain.samples)
+    n, K = np.zeros(S, np.int64), np.zeros(S, np.int64)
+    for s, (mem, off, _) in enumerate(chain.samples):
+        k = sample_pair_keys(chain.num_records, mem, off)
+        pos = np.minimum(np.searchsorted(keys, k), max(len(keys) - 1, 0))
+        hit = keys[pos] == k if len(keys) else np.zeros(len(k), bool)
+        n[s], K[s] = len(k), int(count[pos[hit]].sum())
+    return n, K
+
+
+def binder_losses(n, K, false_link_cost):
+    """float64[S]: the posterior expected Binder loss ((1 - t) C + t S n - K) / S of every sample, t = false_link_cost,
+    C = sum of n."""
+    n, K = np.asarray(n, np.int64), np.asarray(K, np.int64)
+    S, C, t = len(n), int(n.sum()), float(false_link_cost)
+    return ((1.0 - t) * C + t * S * n.astype(np.float64) - K.astype(np.float64)) / S
+
+
+def binder_estimate(n, K, false_link_cost):
+    """The position of the sample of least expected Binder loss, ties going to the earliest.  t is a binary fraction
+    a / b, so the losses are compared exactly, as the integers a S n - b K (the rest of S E[L] b is the same for every
+    sample): two samples of equal loss tie whatever the rounding of binder_losses."""
+    a, b = float(false_link_cost).as_integer_ratio()
+    S = len(n)
+    if S == 0:
+        raise ValueError("the Binder-loss estimate needs at least one sample")
+    score = [a * S * int(x) - b * int(y) for x, y in zip(n, K)]
+    return min(range(S), key=lambda s: (score[s], s))
 
 
 def labels_to_clusters(labels, record_ids=None):

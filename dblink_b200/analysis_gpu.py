@@ -8,7 +8,8 @@ filled one sample at a time; the host only turns each sample's (members, offsets
 The pairwise match counts equal analysis_arrays.pairwise_match_counts exactly: the device keeps the sorted table of
 (pair, count) and merges each sample's pairs into it.  The per-sample counts against the ground truth equal
 analysis_arrays.posterior_metric_counts exactly: they are integers, counted on the device from one radix sort of
-(sample label, true label) per record.
+(sample label, true label) per record.  The Binder-loss counts (n, K) per sample equal analysis_arrays.binder_counts
+exactly: every sample goes into one pairs table, then every sample is scored against it.
 """
 import ctypes as C
 
@@ -144,6 +145,26 @@ class Pairs(_Handle):
             self._call("read", self._h, int(min_count), *(a.ctypes.data for a in out))
         return tuple(a.astype(np.int64) for a in out)
 
+    def score_sample(self, cluster):
+        """(n, K) of any labelling cluster[R] against the held table: the pairs it puts together and the sum of their
+        counts (0 for a pair the table does not hold).  The table does not change."""
+        cluster = np.ascontiguousarray(cluster, np.int32)
+        if cluster.shape != (self.num_records,):
+            raise ValueError("a sample needs one cluster label per record")
+        n, K = C.c_int64(), C.c_int64()
+        self._call("score_sample", self._h, cluster.ctypes.data, C.byref(n), C.byref(K))
+        return n.value, K.value
+
+
+def _add_pairs(pairs, chain, max_pairs):
+    """Every sample of a ChainArrays into a Pairs handle; the cap refusal as analysis_arrays raises it."""
+    try:
+        _add_chain(pairs, chain)
+    except DblinkError as e:  # the labels are valid, so DBL_ERR_INVALID means the cap
+        if e.status == _lib.ERR_INVALID:
+            raise too_many_pairs(max_pairs) from e
+        raise
+
 
 def pairwise_match_counts(chain, max_pairs=MAX_PAIRS, min_count=1):
     """(first, second, count), identical to analysis_arrays.pairwise_match_counts(chain, max_pairs, min_count)."""
@@ -151,13 +172,22 @@ def pairwise_match_counts(chain, max_pairs=MAX_PAIRS, min_count=1):
     if R == 0 or not chain.samples:
         return tuple(np.zeros(0, np.int64) for _ in range(3))
     with Pairs(R, max_pairs) as pairs:
-        try:
-            _add_chain(pairs, chain)
-        except DblinkError as e:  # the labels are valid, so DBL_ERR_INVALID means the cap
-            if e.status == _lib.ERR_INVALID:
-                raise too_many_pairs(max_pairs) from e
-            raise
+        _add_pairs(pairs, chain, max_pairs)
         return pairs.read(min_count)
+
+
+def binder_counts(chain, max_pairs=MAX_PAIRS):
+    """(n, K), int64[S], identical to analysis_arrays.binder_counts(chain, max_pairs): pass 1 adds every sample to one
+    handle, pass 2 scores every sample against the full table."""
+    R, S = chain.num_records, len(chain.samples)
+    n, K = np.zeros(S, np.int64), np.zeros(S, np.int64)
+    if R == 0 or S == 0:
+        return n, K
+    with Pairs(R, max_pairs) as pairs:
+        _add_pairs(pairs, chain, max_pairs)
+        for s, (mem, off, _) in enumerate(chain.samples):
+            n[s], K[s] = pairs.score_sample(sample_clusters(R, mem, off))
+    return n, K
 
 
 class Evaluation(_Handle):

@@ -15,7 +15,8 @@
 // Posterior pairwise match counts (dbl_pairs_*, same numbers as analysis_arrays.pairwise_match_counts): for every
 // unordered pair of records the number of samples in which they share a cluster.  The handle holds a sorted table of
 // (first << 32 | second, count) over the pairs seen so far; each sample's pairs are generated, sorted and merged into
-// it -- see dbl_pairs_add_sample.
+// it -- see dbl_pairs_add_sample.  dbl_pairs_score_sample generates the pairs of any labelling the same way and sums
+// their held counts (the Binder-loss estimate of analysis_arrays.binder_counts).
 //
 // Every sample against the ground truth (dbl_eval_*, same numbers as analysis_arrays.posterior_metric_counts): per
 // sample the pair counts the pairwise metrics and the adjusted Rand index are made of -- tp = sum over the cells
@@ -385,6 +386,11 @@ __device__ __forceinline__ int64_t lower_bound_u64(const unsigned long long *__r
   return lo;
 }
 
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  return v;
+}
+
 // the last position of each cluster writes the cluster's size at its first position
 __global__ void k_cluster_sizes(int64_t R, const int32_t *__restrict__ lab, const int32_t *__restrict__ start,
                                 int32_t *__restrict__ size_at_start) {
@@ -456,6 +462,22 @@ __global__ void k_merge_new(int64_t n, const unsigned long long *__restrict__ ke
   }
 }
 
+// the keys of one sample (in any order) looked up in the held table: the sum of the counts of those it holds, a key it
+// does not hold adding 0; summed per warp in uint64 and added with one atomic per warp, so the total is exact and
+// does not depend on the order
+__global__ void k_score_pairs(int64_t n, const unsigned long long *__restrict__ keys, int64_t H,
+                              const unsigned long long *__restrict__ held, const int32_t *__restrict__ hcnt,
+                              unsigned long long *__restrict__ sum) {
+  unsigned long long acc = 0;
+  for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long k = keys[j];
+    const int64_t b = lower_bound_u64(held, H, k);
+    if (b < H && held[b] == k) acc += (uint32_t)hcnt[b];
+  }
+  acc = warp_sum_u64(acc);
+  if ((threadIdx.x & 31) == 0 && acc) atomicAdd(sum, acc);
+}
+
 __global__ void k_flag_min_count(int64_t H, const int32_t *__restrict__ cnt, int32_t min_count,
                                  int32_t *__restrict__ flag) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= H; i += (int64_t)gridDim.x * blockDim.x)
@@ -485,6 +507,7 @@ struct dbl_pairs : Handle {
   Buf tab_key[2], tab_cnt[2];           // grown on demand: held table (index cur), the one the next sample merges into
   int cur = 0;
   Buf tmp;                              // CUB temporary storage, grown on demand
+  Buf score;                            // the uint64 count sum of dbl_pairs_score_sample
 };
 
 extern "C" int dbl_pairs_create(dbl_pairs **out, int64_t num_records, int64_t max_pairs) {
@@ -499,7 +522,8 @@ extern "C" int dbl_pairs_create(dbl_pairs **out, int64_t num_records, int64_t ma
     const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(long long) * (size_t)(R + 1);
     if (p->iota.alloc(r4) != cudaSuccess || p->lab_s.alloc(r4) != cudaSuccess || p->rec_s.alloc(r4) != cudaSuccess ||
         p->head.alloc(r4) != cudaSuccess || p->start.alloc(r4) != cudaSuccess || p->size.alloc(r4) != cudaSuccess ||
-        p->row.alloc(r8) != cudaSuccess || p->off.alloc(r8) != cudaSuccess)
+        p->row.alloc(r8) != cudaSuccess || p->off.alloc(r8) != cudaSuccess ||
+        p->score.alloc(sizeof(unsigned long long)) != cudaSuccess)
       return DBL_ERR_CUDA;
     k_iota<<<grid_for(R), THREADS, 0, p->stream>>>(R, p->iota.as<int32_t>());
     POST_TRY(cudaGetLastError());
@@ -512,16 +536,13 @@ extern "C" void dbl_pairs_free(dbl_pairs *p) { free_handle(p); }
 
 extern "C" int32_t dbl_pairs_num_samples(const dbl_pairs *p) { return p ? p->S : 0; }
 
-// One sample: check the labels; stable radix sort of (label, record); cluster starts and sizes; every position's row
-// of partners and its int64 offset, whose total is the sample's pair count sum k(k-1)/2; refuse before allocating
-// anything for the pairs if that count alone exceeds max_pairs; emit the keys; radix-sort them; merge them into the
-// spare table (a binary search per key on either side gives its place); commit by swapping tables only if the union
-// fits max_pairs.  A refusal or failure leaves the held table and S as they were.
-extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
-  if (!p || !cluster || p->S == INT32_MAX) return DBL_ERR_INVALID;
-  DeviceScope ds(p->device);
+// One sample's pair keys, unsorted, into key_in: check the labels; stable radix sort of (label, record); cluster
+// starts and sizes; every position's row of partners and its int64 offset, whose total *n_out is the sample's pair
+// count sum k(k-1)/2; refuse (DBL_ERR_INVALID) before allocating anything for the pairs if that count alone exceeds
+// max_pairs; emit the keys.  Neither the held table nor S changes.
+static int pairs_emit_sample(dbl_pairs *p, const int32_t *cluster, long long *n_out) {
   if (const int rc = p->take_labels(cluster, p->cluster); rc != DBL_OK) return rc;
-  const int64_t R = p->R, H = p->H;
+  const int64_t R = p->R;
   cudaStream_t st = p->stream;
 
   // records grouped by label, ascending record index within a cluster; tmp is grown before anything uses it
@@ -543,16 +564,33 @@ extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
   POST_TRY(cudaStreamSynchronize(st));
   if (n > p->max_pairs) return DBL_ERR_INVALID;  // this sample alone: nothing allocated for its pairs
 
+  const size_t cap8 = sizeof(unsigned long long) * (size_t)p->max_pairs;
+  POST_TRY(p->key_in.reserve(sizeof(unsigned long long) * (size_t)n, cap8));
+  if (n > 0)
+    k_emit_pairs<<<(int)std::min<int64_t>((R + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, 8192), THREADS, 0, st>>>(
+        R, p->rec_s.as<int32_t>(), p->off.as<long long>(), p->key_in.as<unsigned long long>());
+  *n_out = n;
+  return DBL_OK;
+}
+
+// One sample: its pair keys (pairs_emit_sample); radix-sort them; merge them into the spare table (a binary search per
+// key on either side gives its place); commit by swapping tables only if the union fits max_pairs.  A refusal or
+// failure leaves the held table and S as they were.
+extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
+  if (!p || !cluster || p->S == INT32_MAX) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  long long n = 0;
+  if (const int rc = pairs_emit_sample(p, cluster, &n); rc != DBL_OK) return rc;
+  const int64_t H = p->H;
+  cudaStream_t st = p->stream;
+
   // the sample's keys, sorted
   const size_t cap8 = sizeof(unsigned long long) * (size_t)p->max_pairs, cap4 = sizeof(int32_t) * (size_t)(p->max_pairs + 1);
-  POST_TRY(p->key_in.reserve(sizeof(unsigned long long) * (size_t)n, cap8));
   POST_TRY(p->key_s.reserve(sizeof(unsigned long long) * (size_t)n, cap8));
   POST_TRY(p->is_new.reserve(sizeof(int32_t) * (size_t)(n + 1), cap4));
   POST_TRY(p->rank.reserve(sizeof(int32_t) * (size_t)(n + 1), cap4));
   const unsigned long long *keys = p->key_s.as<unsigned long long>();
   if (n > 0) {
-    k_emit_pairs<<<(int)std::min<int64_t>((R + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, 8192), THREADS, 0, st>>>(
-        R, p->rec_s.as<int32_t>(), p->off.as<long long>(), p->key_in.as<unsigned long long>());
     size_t tbk = 0;
     POST_TRY(cub::DeviceRadixSort::SortKeys(nullptr, tbk, (const unsigned long long *)nullptr,
                                             (unsigned long long *)nullptr, (int64_t)n, 0, p->key_bits, st));
@@ -596,6 +634,31 @@ extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
   p->cur = nxt;
   p->H = H2;
   ++p->S;
+  return DBL_OK;
+}
+
+// One labelling scored against the held table: its pair keys (pairs_emit_sample), unsorted, each looked up in the
+// table by k_score_pairs.  n = its pair count, K = the sum of the held counts of its pairs.
+extern "C" int dbl_pairs_score_sample(dbl_pairs *p, const int32_t *cluster, int64_t *num_pairs_out,
+                                      int64_t *count_sum_out) {
+  if (!p || !cluster || !num_pairs_out || !count_sum_out) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  long long n = 0;
+  if (const int rc = pairs_emit_sample(p, cluster, &n); rc != DBL_OK) return rc;
+  const int64_t H = p->H;
+  cudaStream_t st = p->stream;
+  unsigned long long *sum = p->score.as<unsigned long long>(), K = 0;
+  POST_TRY(cudaMemsetAsync(sum, 0, sizeof(unsigned long long), st));
+  if (n > 0 && H > 0)
+    k_score_pairs<<<grid_for(n), THREADS, 0, st>>>(n, p->key_in.as<unsigned long long>(), H,
+                                                   p->tab_key[p->cur].as<unsigned long long>(),
+                                                   p->tab_cnt[p->cur].as<int32_t>(), sum);
+  POST_TRY(cudaMemcpyAsync(&K, sum, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  *num_pairs_out = n;
+  *count_sum_out = (int64_t)K;
   return DBL_OK;
 }
 
@@ -660,11 +723,6 @@ __global__ void k_pack_labels(int64_t R, int lab_bits, const int32_t *__restrict
                               const int32_t *__restrict__ truth, unsigned long long *__restrict__ key) {
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x)
     key[r] = (unsigned long long)(uint32_t)cluster[r] << lab_bits | (uint32_t)truth[r];
-}
-
-__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  return v;
 }
 
 // Over the sorted keys: the last position of each run of equal keys (one cell of the contingency table) and of each

@@ -18,9 +18,11 @@ from .records import (Attribute, RecordsCache, SimilarityFn, build_cache_from_co
 SMPC_METRICS = ("pairwise", "cluster")  # ProjectStep.scala:36
 # every sample at or after the cutoff against the ground truth: evaluation-samples.csv and a posterior summary
 POSTERIOR_METRICS = ("posterior-pairwise", "posterior-cluster")
-SUPPORTED_METRICS = SMPC_METRICS + POSTERIOR_METRICS
+# the sample of least posterior expected Binder loss (falseLinkCost = the cost of a false link) against the ground truth
+BINDER_METRICS = ("binder-pairwise", "binder-cluster")
+SUPPORTED_METRICS = SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
-                        "pairwise-match-probabilities", "convergence-diagnostics")
+                        "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters")
 
 
 def shared_most_probable_clusters(chain):
@@ -45,6 +47,33 @@ def posterior_metric_counts(chain, truth):
     if _lib.load().dbl_device_count() > 0:
         return analysis_gpu.posterior_metric_counts(chain, truth)
     return analysis_arrays.posterior_metric_counts(chain, truth)
+
+
+def binder_counts(chain):
+    """(n, K) of every sample of a ChainArrays, the pairs it links and the sum of their match counts: on the GPU when
+    the platform has one (analysis_gpu), else on the host (analysis_arrays).  Both give identical arrays."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.binder_counts(chain)
+    return analysis_arrays.binder_counts(chain)
+
+
+def binder_estimate(chain, false_link_cost):
+    """The sample of least posterior expected Binder loss of a ChainArrays: (its position, its labels, every sample's
+    linked pairs and expected loss)."""
+    if not chain.samples:
+        raise ValueError("the Binder-loss estimate needs at least one sample at or after lowerIterationCutoff")
+    n, K = binder_counts(chain)
+    s = analysis_arrays.binder_estimate(n, K, false_link_cost)
+    mem, off, _ = chain.samples[s]
+    return (s, analysis_arrays.sample_labels(chain.num_records, mem, off), n,
+            analysis_arrays.binder_losses(n, K, false_link_cost))
+
+
+def _false_link_cost(prm):
+    t = float(prm.get("falseLinkCost", 0.5))
+    if not 0.0 <= t <= 1.0:
+        raise ValueError("falseLinkCost must be in [0, 1].")
+    return t
 
 
 class Project:
@@ -140,6 +169,9 @@ class Project:
             elif name == "summarize":
                 L.append(f"  * SummarizeStep: Calculating summary quantities {braces(prm['quantities'])} along the "
                          f"chain for iterations >= {prm['lower_iteration_cutoff']}")
+                if "binder-clusters" in prm["quantities"]:
+                    L.append(f"  * SummarizeStep: binder-clusters is the sample of least posterior expected Binder "
+                             f"loss with falseLinkCost={prm['false_link_cost']}")
             elif name == "evaluate":
                 smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
                 post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
@@ -151,6 +183,11 @@ class Project:
                 if post:
                     L.append(f"  * EvaluateStep: Evaluating every sample of the chain for iterations >= "
                              f"{prm['lower_iteration_cutoff']} using {braces(post)} metrics")
+                binder = [m for m in prm["metrics"] if m in BINDER_METRICS]
+                if binder:
+                    L.append(f"  * EvaluateStep: Evaluating the sample of least posterior expected Binder loss "
+                             f"(falseLinkCost={prm['false_link_cost']}, iterations >= {prm['lower_iteration_cutoff']}) "
+                             f"using {braces(binder)} metrics")
             else:
                 L.append("  * CopyFilesStep: Copying {" + ", ".join(prm["file_names"]) + "} to destination "
                          + prm["destination_path"])
@@ -290,13 +327,15 @@ class Project:
                 if not 0.0 <= t <= 1.0:
                     raise ValueError("minMatchProbability must be in [0, 1].")
                 out.append(("summarize", dict(lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)),
-                                              quantities=q, min_match_probability=t)))
+                                              quantities=q, min_match_probability=t,
+                                              false_link_cost=_false_link_cost(prm))))
             elif name == "evaluate":
                 m = list(prm["metrics"])
                 if not m or any(x not in SUPPORTED_METRICS for x in m):
                     raise ValueError(f"metrics must be one of {SUPPORTED_METRICS}.")
                 out.append(("evaluate", dict(lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)), metrics=m,
-                                             use_existing_smpc=bool(prm.get("useExistingSMPC", False)))))
+                                             use_existing_smpc=bool(prm.get("useExistingSMPC", False)),
+                                             false_link_cost=_false_link_cost(prm))))
             elif name == "copy-files":
                 out.append(("copy-files", dict(file_names=list(prm["fileNames"]),
                                                destination_path=prm["destinationPath"],
@@ -344,6 +383,11 @@ class Project:
                         first, second, count = pairwise_match_counts(ch, min_count=analysis_arrays.min_match_count(t, S))
                         writers.save_pairwise_match_probabilities(first, second, count, S, ch.record_ids, t,
                                                                   self.output_path)
+                    elif q == "binder-clusters":
+                        s, labels, n, losses = binder_estimate(ch, prm["false_link_cost"])
+                        self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids),
+                                        "binder-clusters.csv")
+                        writers.save_binder_loss(ch.chains, ch.iterations, n, losses, self.output_path)
                     else:
                         labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
@@ -380,6 +424,19 @@ class Project:
                             results[m] = {k: summary[k] for k in ("adjRandIndex", "numClusters")}
                             results[m]["trueNumClusters"] = true_clusters
                             text.append(analysis.format_posterior_cluster(summary, len(rows), true_clusters))
+                if any(m in BINDER_METRICS for m in prm["metrics"]):
+                    ch = ch if ch is not None else self.read_chain(cut)
+                    t = prm["false_link_cost"]
+                    s, labels, _, _ = binder_estimate(ch, t)
+                    truth = true_labels(ch.record_ids)
+                    at = (int(ch.iterations[s]), int(ch.chains[s]), t)
+                    for m in prm["metrics"]:
+                        if m == "binder-pairwise":
+                            results[m] = analysis_arrays.pairwise_metrics(labels, truth)
+                            text.append(analysis.format_binder_pairwise(results[m], *at))
+                        elif m == "binder-cluster":
+                            results[m] = analysis_arrays.adjusted_rand_index(labels, truth)
+                            text.append(analysis.format_binder_cluster(results[m], *at))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
             elif name == "copy-files":
@@ -431,7 +488,8 @@ class Project:
             raise ValueError("shared-most-probable-clusters.csv does not cover every record of the chain")
         return labels
 
-    def _save_smpc(self, clusters):
-        with open(os.path.join(self.output_path, "shared-most-probable-clusters.csv"), "w") as fh:
+    def _save_smpc(self, clusters, file_name="shared-most-probable-clusters.csv"):
+        """Clusters (lists of record ids) under outputPath, one per line, ids sorted and joined by ", "."""
+        with open(os.path.join(self.output_path, file_name), "w") as fh:
             for c in clusters:
                 fh.write(", ".join(sorted(c)) + "\n")

@@ -6,6 +6,7 @@
   save_cluster_size_distribution / save_partition_sizes   LinkageChain.scala:162-211
   save_pairwise_match_probabilities   pairwise-match-probabilities.csv: recordId1,recordId2,probability
   save_evaluation_samples   evaluation-samples.csv: every sample's counts and metrics against the ground truth
+  save_binder_loss   binder-loss.csv: every sample's linked pairs and posterior expected Binder loss
 """
 import os
 import time
@@ -216,3 +217,15 @@ def save_evaluation_samples(iterations, rows, path):
         for it, r in zip(iterations, rows):
             fh.write(f"{int(it)},{r['numClusters']},{r['TP']},{r['FP']},{r['FN']},{r['precision']!r},{r['recall']!r},"
                      f"{r['f1score']!r},{r['adjRandIndex']!r}\n")
+
+
+BINDER_LOSS_HEADER = "chain,iteration,linkedPairs,expectedLoss"
+
+
+def save_binder_loss(chains, iterations, linked_pairs, losses, path):
+    """binder-loss.csv under `path`: one row per sample in pooled order (chain-major, then iteration), its record
+    pairs linked and its expected loss (analysis_arrays.binder_losses), written with repr."""
+    with open(os.path.join(path, "binder-loss.csv"), "w") as fh:
+        fh.write(BINDER_LOSS_HEADER + "\n")
+        for k, it, n, loss in zip(chains, iterations, linked_pairs, losses):
+            fh.write(f"{int(k)},{int(it)},{int(n)},{float(loss)!r}\n")

@@ -325,7 +325,14 @@ int dbl_posterior_smpc(dbl_posterior *, int32_t *labels_out /* R, may be NULL */
  *   dbl_pairs_count       the number of held pairs with count >= min_count
  *   dbl_pairs_read        those pairs, in ascending (first, second) order, first < second (record indices), with
  *                         their counts; the three arrays (dbl_pairs_count entries) may be host or device pointers
- *   count / read before the first sample give DBL_ERR_STATE.
+ *   dbl_pairs_score_sample  any labelling cluster[R] (host or device pointer, as for add_sample) against the held
+ *                         table: *num_pairs_out = n, the number of record pairs it puts together, and *count_sum_out =
+ *                         K, the sum of count(a, b) over those pairs (a pair the table does not hold counts 0), both
+ *                         int64.  The table and S do not change.  DBL_ERR_INVALID: a label outside [0, R), or n alone
+ *                         exceeding max_pairs (checked before anything is allocated for the pairs).  With
+ *                         t = the cost of a false link and 1 - t that of a missed link, the posterior expected Binder
+ *                         loss of the labelling is ((1 - t) C + t S n - K) / S, C = sum of all held counts.
+ *   count / read / score_sample before the first sample give DBL_ERR_STATE.
  * DBL_ERR_INVALID: num_records or max_pairs outside [1, 2^31 - 1].  DBL_ERR_CUDA: no device, or an allocation that
  * fails (the held table and the sample count stay as they were).
  * ------------------------------------------------------------------------------------------------- */
@@ -336,6 +343,8 @@ int dbl_pairs_add_sample(dbl_pairs *, const int32_t *cluster /* R, host or devic
 int32_t dbl_pairs_num_samples(const dbl_pairs *);
 int dbl_pairs_count(dbl_pairs *, int32_t min_count, int64_t *n_out);
 int dbl_pairs_read(dbl_pairs *, int32_t min_count, int32_t *first, int32_t *second, int32_t *count);
+int dbl_pairs_score_sample(dbl_pairs *, const int32_t *cluster /* R, host or device */, int64_t *num_pairs_out,
+                           int64_t *count_sum_out);
 
 /* ---------------------------------------------------------------------------------------------------
  * Every posterior sample against the ground truth: per sample, the integer counts its pairwise precision / recall /
