@@ -136,6 +136,8 @@ SIGNATURES = {
     "dbl_pairs_count": (C.c_int, [vp, C.c_int32, i64p]),
     "dbl_pairs_read": (C.c_int, [vp, C.c_int32, vp, vp, vp]),
     "dbl_pairs_score_sample": (C.c_int, [vp, vp, i64p, i64p]),
+    "dbl_pairs_binder_search": (C.c_int, [vp, C.c_int64, C.c_int64, vp, C.c_int32, vp, i32p, i32p, i64p, i64p, i64p,
+                                          i64p, i64p]),
     "dbl_eval_create": (C.c_int, [C.POINTER(vp), C.c_int64, vp, C.c_int32]),
     "dbl_eval_free": (None, [vp]),
     "dbl_eval_add_sample": (C.c_int, [vp, vp]),

@@ -3,6 +3,7 @@
   most_probable_clusters / shared_most_probable_clusters  <- LinkageChain.scala:52-109
   pairwise_match_probabilities                            <- posterior probability that two records are one entity
   binder_clusters                                         <- the sample of least posterior expected Binder loss
+  binder_search                                           <- single-record moves that lower the expected Binder loss
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
   pairwise_metrics                                        <- analysis/PairwiseMetrics.scala:44-63,
                                                              BinaryClassificationMetrics.scala:23-37
@@ -85,6 +86,81 @@ def binder_clusters(chain, false_link_cost=0.5):
         losses.append(loss)
     best = min(range(S), key=lambda s: (losses[s], s))
     return best, clusters[best], [float(x) for x in losses]
+
+
+def binder_search(chain, false_link_cost, starts, max_rounds=1000, records=None):
+    """Single-record moves from each start (a partition: clusters of ids) while they lower the posterior expected
+    Binder loss, by the definition, in exact rational arithmetic, with t = false_link_cost rounded as
+    analysis_arrays.search_cost rounds it.  `records` orders the record ids (a record's index is its position; default:
+    sorted).  One round: every record takes its best move to ANY other cluster or, out of a cluster of two or more, to a
+    singleton -- the least (change of loss, destination), a singleton counting as destination -1 and a cluster as its
+    smallest record index -- and proposes it if it lowers the loss; a proposal is applied if it is the least (change,
+    record index) among the proposals touching each cluster it touches (its source, and its destination unless that is
+    a singleton).  Returns (position of the chosen start: least loss, ties to the earlier; per start a dict with the
+    final clusters as frozensets, rounds = [(moves, change of linked pairs, change of count sum)], converged, n, K)."""
+    from .analysis_arrays import search_cost
+
+    t = fractions.Fraction(*search_cost(false_link_cost))
+    S = len(chain)
+    count = collections.Counter(p for s in chain for c in clusters_of_sample(s) for p in
+                                (frozenset(q) for q in itertools.combinations(c, 2)))
+    ids = sorted({r for s in chain for c in clusters_of_sample(s) for r in c}) if records is None else list(records)
+    index = {r: k for k, r in enumerate(ids)}
+
+    def pair_loss(i, j, linked):
+        p = fractions.Fraction(count[frozenset((i, j))], S)
+        return t * (1 - p) if linked else (1 - t) * p
+
+    def counts(cluster_of):
+        linked = [(i, j) for i, j in itertools.combinations(ids, 2) if cluster_of[i] == cluster_of[j]]
+        return len(linked), sum(count[frozenset(q)] for q in linked)
+
+    runs = []
+    for start in starts:
+        cluster_of = {r: frozenset(c) for c in start for r in c}
+        rounds, converged = [], False
+        while True:
+            label = {c: min(index[r] for r in c) for c in set(cluster_of.values())}
+            proposals = []
+            for i in ids:
+                A = cluster_of[i]
+                dests = [(label[X], X) for X in set(cluster_of.values()) if X != A]
+                if len(A) > 1:
+                    dests.append((-1, None))
+                best = None
+                for dest, X in dests:
+                    change = sum(pair_loss(i, j, j in (X or ())) - pair_loss(i, j, j in A) for j in ids if j != i)
+                    if best is None or (change, dest) < best[:2]:
+                        best = (change, dest, X)
+                if best is not None and best[0] < 0:
+                    proposals.append((best[0], index[i], i, A, best[2]))
+            if not proposals:
+                converged = True
+                break
+            if len(rounds) == max_rounds:
+                break
+            least = {}
+            for change, k, i, A, X in proposals:
+                for c in (A, X) if X is not None else (A,):
+                    least[c] = min(least.get(c, (change, k)), (change, k))
+            before = counts(cluster_of)
+            new = dict(cluster_of)
+            applied = 0
+            for change, k, i, A, X in proposals:
+                if all(least[c] == (change, k) for c in ((A, X) if X is not None else (A,))):
+                    applied += 1
+                    for r in A - {i}:
+                        new[r] = A - {i}
+                    joined = (X or frozenset()) | {i}
+                    for r in joined:
+                        new[r] = joined
+            cluster_of = new
+            after = counts(cluster_of)
+            rounds.append((applied, after[0] - before[0], after[1] - before[1]))
+        n, K = counts(cluster_of)
+        runs.append(dict(clusters=set(cluster_of.values()), rounds=rounds, converged=converged, n=n, K=K,
+                         loss=((1 - t) * sum(count.values()) + t * S * n - K) / S))
+    return min(range(len(runs)), key=lambda k: (runs[k]["loss"], k)), runs
 
 
 def cluster_size_distribution(chain):
@@ -184,6 +260,29 @@ def format_binder_cluster(ari, iteration, chain, false_link_cost):
     """The binder-cluster section: ari = adjusted Rand index of the sample chosen at (iteration, chain)."""
     return ("=====================================\n       Binder cluster metrics\n"
             "-------------------------------------\n" + _binder_estimate_line(iteration, chain, false_link_cost)
+            + f" Adj. Rand index: {ari}\n=====================================\n")
+
+
+def _binder_search_line(start, rounds, converged, false_link_cost, searched_cost):
+    return (f" Estimate:        search from the {start} start, {rounds} rounds, "
+            f"{'converged' if converged else 'not converged'}, falseLinkCost {false_link_cost} "
+            f"(searched at {searched_cost!r})\n")
+
+
+def format_binder_search_pairwise(m, start, rounds, converged, false_link_cost, searched_cost):
+    """The binder-search-pairwise section: m = pairwise metrics of the search result chosen from `start`."""
+    return ("=====================================\n   Binder search pairwise metrics\n"
+            "-------------------------------------\n"
+            + _binder_search_line(start, rounds, converged, false_link_cost, searched_cost)
+            + f" Precision:      {m['precision']}\n Recall:         {m['recall']}\n F1-score:       {m['f1score']}\n"
+            "=====================================\n")
+
+
+def format_binder_search_cluster(ari, start, rounds, converged, false_link_cost, searched_cost):
+    """The binder-search-cluster section: ari = adjusted Rand index of the search result chosen from `start`."""
+    return ("=====================================\n    Binder search cluster metrics\n"
+            "-------------------------------------\n"
+            + _binder_search_line(start, rounds, converged, false_link_cost, searched_cost)
             + f" Adj. Rand index: {ari}\n=====================================\n")
 
 

@@ -188,7 +188,13 @@ def shared_most_probable_clusters(chain):
     labelled by the smallest record index of the group."""
     sig = cluster_signatures(chain)
     best, _ = most_probable_signature(sig)
-    _, inv = np.unique(best, return_inverse=True)
+    return canonical_labels(best)
+
+
+def canonical_labels(keys):
+    """int64 labels[R]: records with equal keys grouped, each group labelled by its smallest record index."""
+    _, inv = np.unique(keys, return_inverse=True)
+    inv = inv.reshape(-1)
     rep = np.full(inv.max() + 1 if len(inv) else 0, np.iinfo(np.int64).max, np.int64)
     np.minimum.at(rep, inv, np.arange(len(inv)))
     return rep[inv].astype(np.int64)
@@ -301,8 +307,14 @@ def binder_counts(chain, max_pairs=MAX_PAIRS):
 def binder_losses(n, K, false_link_cost):
     """float64[S]: the posterior expected Binder loss ((1 - t) C + t S n - K) / S of every sample, t = false_link_cost,
     C = sum of n."""
-    n, K = np.asarray(n, np.int64), np.asarray(K, np.int64)
-    S, C, t = len(n), int(n.sum()), float(false_link_cost)
+    n = np.asarray(n, np.int64)
+    return expected_losses(n, K, int(n.sum()), len(n), false_link_cost)
+
+
+def expected_losses(n, K, C, S, false_link_cost):
+    """float64[]: the posterior expected Binder loss ((1 - t) C + t S n - K) / S of partitions with linked pairs n and
+    count sums K, against a chain of S samples whose counts sum to C."""
+    n, K, t = np.asarray(n, np.int64), np.asarray(K, np.int64), float(false_link_cost)
     return ((1.0 - t) * C + t * S * n.astype(np.float64) - K.astype(np.float64)) / S
 
 
@@ -316,6 +328,150 @@ def binder_estimate(n, K, false_link_cost):
         raise ValueError("the Binder-loss estimate needs at least one sample")
     score = [a * S * int(x) - b * int(y) for x, y in zip(n, K)]
     return min(range(S), key=lambda s: (score[s], s))
+
+
+# ---- a search beyond the samples: parallel single-record moves ---------------------------------------------
+# With t = a / b, S b E[L](c) = (b - a) C + J(c), J(c) = a S n(c) - b K(c).  Moving record i from its cluster A to a
+# cluster B changes J by  dJ = a S (|B| - |A| + 1) - b (w_B - w_A),  w_X = sum of count(i, j) over j in X \ {i}; a new
+# singleton is |B| = 0, w_B = 0.  A cluster holding none of i's partners is never better than the singleton, so the
+# candidates are the clusters of i's partners in the table and, when |A| > 1, a singleton.  One round:
+#   1. labels are canonical (smallest record index of the cluster);
+#   2. every record finds its least (dJ, destination), a singleton counting as destination -1, and proposes it if
+#      dJ < 0;
+#   3. a proposal touches its source cluster and, unless it goes to a singleton, its destination cluster; it is applied
+#      only if it has the least (dJ, i) among the proposals touching each cluster it touches.  Applied moves touch
+#      disjoint clusters, so their dJ add exactly, and the least proposal always wins, so J falls every round;
+#   4. relabel; log the moves and the sums of dn and dK.
+# The search stops when no record proposes a move (converged) or after max_rounds rounds.
+SEARCH_COST_BITS = 16          # t is rounded to a multiple of 2^-16 for the search, so a, b <= 2^16
+MAX_SEARCH_SIZE = 1 << 44      # S R below this keeps every dJ and every round's sum of dJ inside int64
+SEARCH_STARTS = ("binder-sample", "smpc")
+
+
+def search_cost(false_link_cost):
+    """(a, b): t rounded to the nearest multiple of 2^-16 (halves up) as a / b, b = 2^16.  Exact for 0, 1/4, 1/2, 3/4
+    and 1; 0.7 becomes 45875 / 65536."""
+    t = float(false_link_cost)
+    if not 0.0 <= t <= 1.0:
+        raise ValueError("falseLinkCost must be in [0, 1].")
+    b = 1 << SEARCH_COST_BITS
+    return int(math.floor(t * b + 0.5)), b
+
+
+def check_search_size(num_samples, num_records):
+    if int(num_samples) * int(num_records) >= MAX_SEARCH_SIZE:
+        raise ValueError(f"the Binder search needs samples x records < 2^44 (here {num_samples} x {num_records})")
+
+
+class SearchRun:
+    """One search: labels int64[R] (canonical) where it stopped; per round the moves applied and the sums of dn and
+    dK, int64[rounds]; whether it stopped because no record proposed a move; n and K of the result."""
+
+    def __init__(self, labels, moves, dn, dK, converged, n, K):
+        self.labels, self.converged, self.n, self.K = labels, bool(converged), int(n), int(K)
+        self.moves, self.dn, self.dK = (np.asarray(x, np.int64) for x in (moves, dn, dK))
+
+    @property
+    def rounds(self):
+        return len(self.moves)
+
+    def linked_pairs(self):
+        """int64[rounds + 1]: n of the start (round 0) and after every round."""
+        return self.n - int(self.dn.sum()) + np.r_[0, np.cumsum(self.dn)].astype(np.int64)
+
+    def count_sums(self):
+        """int64[rounds + 1]: K of the start (round 0) and after every round."""
+        return self.K - int(self.dK.sum()) + np.r_[0, np.cumsum(self.dK)].astype(np.int64)
+
+
+def search_result_counts(first, second, count, labels):
+    """(n, K) of a labelling: n from its cluster sizes, K = the counts of the held pairs whose records share a label."""
+    labels = np.asarray(labels, np.int64)
+    n = int(_comb2(np.bincount(labels)).sum()) if len(labels) else 0
+    return n, int(np.asarray(count, np.int64)[labels[first] == labels[second]].sum())
+
+
+def _run_starts(sorted_keys):
+    """Positions where a run of equal values starts."""
+    return np.flatnonzero(np.r_[True, sorted_keys[1:] != sorted_keys[:-1]]) if len(sorted_keys) else np.zeros(0, np.int64)
+
+
+def search_rounds(num_records, first, second, count, num_samples, start, a, b, max_rounds):
+    """The search from labels start[R] against the table (first, second, count) of a chain of num_samples samples,
+    t = a / b: a SearchRun."""
+    R, S = int(num_records), int(num_samples)
+    first, second, count = (np.asarray(x, np.int64) for x in (first, second, count))
+    src, dst, cnt = np.r_[first, second], np.r_[second, first], np.r_[count, count]
+    if np.shape(start) != (R,):
+        raise ValueError("a start needs one cluster label per record")
+    lab = canonical_labels(np.asarray(start, np.int64))
+    aS, big = a * S, np.iinfo(np.int64).max
+    moves, dn, dK, converged = [], [], [], False
+    while True:
+        size = np.bincount(lab, minlength=R).astype(np.int64)
+        # the sum of count per (record, partner label), in ascending (record, label) order
+        keys = src * R + lab[dst]
+        order = np.argsort(keys)
+        keys = keys[order]
+        runs = _run_starts(keys)
+        keys, w = keys[runs], np.add.reduceat(cnt[order], runs) if len(runs) else np.zeros(0, np.int64)
+        rec, X = keys // R, keys % R
+        own = X == lab[rec]
+        wA = np.zeros(R, np.int64)
+        wA[rec[own]] = w[own]
+        # candidates in ascending (record, destination) order: a record's singleton first, then its partner clusters
+        multi = np.flatnonzero(size[lab] > 1)
+        by = np.argsort(np.r_[2 * multi, 2 * rec[~own] + 1], kind="stable")
+        c_rec = np.r_[multi, rec[~own]][by]
+        c_dest = np.r_[np.full(len(multi), -1, np.int64), X[~own]][by]
+        c_dK = np.r_[-wA[multi], w[~own] - wA[rec[~own]]][by]
+        c_dn = np.where(c_dest >= 0, size[np.maximum(c_dest, 0)], 0) - size[lab[c_rec]] + 1
+        c_dJ = aS * c_dn - b * c_dK
+        # per record the first candidate of least dJ: the least (dJ, destination)
+        seg = _run_starts(c_rec)
+        least = np.repeat(np.minimum.reduceat(c_dJ, seg), np.diff(np.r_[seg, len(c_rec)])) if len(seg) else c_dJ
+        at = np.flatnonzero(c_dJ == least)
+        best = at[_run_starts(c_rec[at])]
+        best = best[c_dJ[best] < 0]
+        if not len(best):
+            converged = True
+            break
+        if len(moves) == max_rounds:
+            break
+        i, X, dJ = c_rec[best], c_dest[best], c_dJ[best]
+        A, to = lab[i], X >= 0
+        touched, t_dJ, t_i = np.r_[A, X[to]], np.r_[dJ, dJ[to]], np.r_[i, i[to]]
+        claim_dJ = np.full(R, big, np.int64)
+        np.minimum.at(claim_dJ, touched, t_dJ)
+        least = t_dJ == claim_dJ[touched]
+        claim_i = np.full(R, big, np.int64)
+        np.minimum.at(claim_i, touched[least], t_i[least])
+        win = (claim_dJ[A] == dJ) & (claim_i[A] == i)
+        win[to] &= (claim_dJ[X[to]] == dJ[to]) & (claim_i[X[to]] == i[to])
+        key = lab.copy()
+        key[i[win]] = np.where(to[win], X[win], R + i[win])
+        moves.append(int(win.sum()))
+        dn.append(int(c_dn[best][win].sum()))
+        dK.append(int(c_dK[best][win].sum()))
+        lab = canonical_labels(key)
+    n, K = search_result_counts(first, second, count, lab)
+    return SearchRun(lab, moves, dn, dK, converged, n, K)
+
+
+def search_choice(runs, num_samples, a, b):
+    """The position of the run of least J = a S n - b K, ties going to the earlier start."""
+    return min(range(len(runs)), key=lambda k: (a * num_samples * runs[k].n - b * runs[k].K, k))
+
+
+def binder_search(chain, false_link_cost, starts, max_rounds=1000, max_pairs=MAX_PAIRS):
+    """The search from each of starts (labels[R] each) against the chain's pairwise match counts, with t rounded by
+    search_cost: (the position of the chosen run, the SearchRuns)."""
+    R, S = chain.num_records, len(chain.samples)
+    check_search_size(S, R)
+    a, b = search_cost(false_link_cost)
+    first, second, count = pairwise_match_counts(chain, max_pairs)
+    runs = [search_rounds(R, first, second, count, S, st, a, b, max_rounds) for st in starts]
+    return search_choice(runs, S, a, b), runs
 
 
 def labels_to_clusters(labels, record_ids=None):

@@ -9,14 +9,17 @@ The pairwise match counts equal analysis_arrays.pairwise_match_counts exactly: t
 (pair, count) and merges each sample's pairs into it.  The per-sample counts against the ground truth equal
 analysis_arrays.posterior_metric_counts exactly: they are integers, counted on the device from one radix sort of
 (sample label, true label) per record.  The Binder-loss counts (n, K) per sample equal analysis_arrays.binder_counts
-exactly: every sample goes into one pairs table, then every sample is scored against it.
+exactly: every sample goes into one pairs table, then every sample is scored against it.  The Binder search
+(single-record moves from a start) equals analysis_arrays.binder_search exactly, in labels, round logs, n and K: the
+rule is in integers, and the device applies it to the same table.
 """
 import ctypes as C
 
 import numpy as np
 
 from . import _lib
-from .analysis_arrays import MAX_PAIRS, too_many_pairs
+from .analysis_arrays import (MAX_PAIRS, SearchRun, check_search_size, search_choice, search_cost,
+                              too_many_pairs)
 from .engine import DblinkError
 
 _STATUS = {_lib.ERR_INVALID: "invalid argument (bad size, label out of range, too many samples or pairs)",
@@ -155,6 +158,21 @@ class Pairs(_Handle):
         self._call("score_sample", self._h, cluster.ctypes.data, C.byref(n), C.byref(K))
         return n.value, K.value
 
+    def binder_search(self, a, b, start, max_rounds):
+        """The single-record-move search from labels start[R] against the held table at t = a / b: an
+        analysis_arrays.SearchRun.  The table does not change."""
+        start = np.ascontiguousarray(start, np.int32)
+        if start.shape != (self.num_records,):
+            raise ValueError("a start needs one cluster label per record")
+        max_rounds = int(max_rounds)
+        labels = np.empty(self.num_records, np.int32)
+        logs = [np.zeros(max(max_rounds, 0), np.int64) for _ in range(3)]
+        rounds, converged, n, K = C.c_int32(), C.c_int32(), C.c_int64(), C.c_int64()
+        self._call("binder_search", self._h, int(a), int(b), start.ctypes.data, max_rounds, labels.ctypes.data,
+                   C.byref(rounds), C.byref(converged), *(x.ctypes.data_as(_lib.i64p) for x in logs), C.byref(n),
+                   C.byref(K))
+        return SearchRun(labels.astype(np.int64), *(x[:rounds.value] for x in logs), converged.value, n.value, K.value)
+
 
 def _add_pairs(pairs, chain, max_pairs):
     """Every sample of a ChainArrays into a Pairs handle; the cap refusal as analysis_arrays raises it."""
@@ -188,6 +206,18 @@ def binder_counts(chain, max_pairs=MAX_PAIRS):
         for s, (mem, off, _) in enumerate(chain.samples):
             n[s], K[s] = pairs.score_sample(sample_clusters(R, mem, off))
     return n, K
+
+
+def binder_search(chain, false_link_cost, starts, max_rounds=1000, max_pairs=MAX_PAIRS):
+    """(chosen position, SearchRuns), identical to analysis_arrays.binder_search(chain, false_link_cost, starts,
+    max_rounds, max_pairs): pass 1 adds every sample to one handle, then the search runs from each start on it."""
+    R, S = chain.num_records, len(chain.samples)
+    check_search_size(S, R)
+    a, b = search_cost(false_link_cost)
+    with Pairs(R, max_pairs) as pairs:
+        _add_pairs(pairs, chain, max_pairs)
+        runs = [pairs.binder_search(a, b, st, max_rounds) for st in starts]
+    return search_choice(runs, S, a, b), runs
 
 
 class Evaluation(_Handle):

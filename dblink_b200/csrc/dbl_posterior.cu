@@ -716,6 +716,284 @@ extern "C" int dbl_pairs_read(dbl_pairs *p, int32_t min_count, int32_t *first, i
   return DBL_OK;
 }
 
+// ---- the Binder search: parallel single-record moves against the held table ----------------------------------------
+namespace {
+constexpr long long NO_MOVE = LLONG_MAX;
+
+__global__ void k_widen_labels(int64_t R, const int32_t *__restrict__ in, unsigned long long *__restrict__ out) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x)
+    out[r] = (uint32_t)in[r];
+}
+
+__global__ void k_label_sizes(int64_t R, const int32_t *__restrict__ lab, int32_t *__restrict__ size) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x)
+    atomicAdd(&size[lab[r]], 1);
+}
+
+// every held pair twice, once from each of its records: key = record << lab_bits | the partner's label, value = the
+// pair's count.  Sorted, a record's entries are one segment, grouped by partner label.
+__global__ void k_partner_keys(int64_t H, int lab_bits, const unsigned long long *__restrict__ held,
+                               const int32_t *__restrict__ hcnt, const int32_t *__restrict__ lab,
+                               unsigned long long *__restrict__ key, int32_t *__restrict__ val) {
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < 2 * H; e += (int64_t)gridDim.x * blockDim.x) {
+    const bool from_first = e < H;
+    const int64_t t = from_first ? e : e - H;
+    const unsigned long long k = held[t];
+    const uint32_t f = (uint32_t)(k >> 32), s = (uint32_t)(k & 0xffffffffull);
+    key[e] = (unsigned long long)(from_first ? f : s) << lab_bits | (uint32_t)lab[from_first ? s : f];
+    val[e] = hcnt[t];
+  }
+}
+
+// One record per thread over its segment of the sorted entries (found by binary search): w_A = the counts of its
+// partners in its own cluster A, then per partner cluster X (runs of equal labels, ascending) w_X and
+// dJ = aS (|X| - |A| + 1) - b (w_X - w_A); a singleton (|A| > 1) is dJ = aS (1 - |A|) + b w_A and is tried first as
+// destination -1, so a strict < keeps the least (dJ, destination).  A record with dJ < 0 proposes its move and claims
+// its source and destination clusters with atomicMin on dJ; proposals are counted into *num_props.
+__global__ void k_best_move(int64_t R, int lab_bits, int64_t n, const unsigned long long *__restrict__ key,
+                            const int32_t *__restrict__ val, const int32_t *__restrict__ lab,
+                            const int32_t *__restrict__ size, long long aS, long long b, long long *__restrict__ prop_dJ,
+                            int32_t *__restrict__ prop_dest, long long *__restrict__ prop_dK,
+                            long long *__restrict__ claim_dJ, unsigned long long *__restrict__ num_props) {
+  const unsigned long long mask = (1ull << lab_bits) - 1;
+  unsigned long long props = 0;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t lo = lower_bound_u64(key, n, (unsigned long long)r << lab_bits);
+    const int64_t hi = lower_bound_u64(key, n, (unsigned long long)(r + 1) << lab_bits);
+    const int32_t A = lab[r];
+    const long long sA = size[A];
+    long long wA = 0;
+    for (int64_t k = lo; k < hi; ++k)
+      if ((key[k] & mask) == (unsigned long long)A) wA += val[k];
+    long long best = NO_MOVE, best_dK = 0;
+    int32_t dest = INT_MAX;
+    if (sA > 1) {
+      best = aS * (1 - sA) + b * wA;
+      best_dK = -wA;
+      dest = -1;
+    }
+    long long w = 0;
+    for (int64_t k = lo; k < hi; ++k) {
+      const unsigned long long X = key[k] & mask;
+      w += val[k];
+      if (k + 1 == hi || (key[k + 1] & mask) != X) {
+        if (X != (unsigned long long)A) {
+          const long long dK = w - wA, dJ = aS * (size[X] - sA + 1) - b * dK;
+          if (dJ < best) {
+            best = dJ;
+            best_dK = dK;
+            dest = (int32_t)X;
+          }
+        }
+        w = 0;
+      }
+    }
+    const bool propose = best < 0;
+    prop_dJ[r] = propose ? best : NO_MOVE;
+    prop_dest[r] = dest;
+    prop_dK[r] = best_dK;
+    if (propose) {
+      atomicMin(&claim_dJ[A], best);
+      if (dest >= 0) atomicMin(&claim_dJ[dest], best);
+      ++props;
+    }
+  }
+  props = warp_sum_u64(props);
+  if ((threadIdx.x & 31) == 0 && props) atomicAdd(num_props, props);
+}
+
+// second stage of the claims: among the proposals of least dJ on a cluster, the least record index
+__global__ void k_claim_record(int64_t R, const int32_t *__restrict__ lab, const long long *__restrict__ prop_dJ,
+                               const int32_t *__restrict__ prop_dest, const long long *__restrict__ claim_dJ,
+                               unsigned int *__restrict__ claim_i) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x) {
+    const long long dJ = prop_dJ[r];
+    if (dJ == NO_MOVE) continue;
+    const int32_t A = lab[r], X = prop_dest[r];
+    if (claim_dJ[A] == dJ) atomicMin(&claim_i[A], (unsigned int)r);
+    if (X >= 0 && claim_dJ[X] == dJ) atomicMin(&claim_i[X], (unsigned int)r);
+  }
+}
+
+// A proposal that holds the claim of every cluster it touches moves its record: the record's group key becomes its
+// destination's label, or R + r for a singleton (a key no cluster has); every other record keeps its label.  The
+// round's moves, sum of dn = |X| - |A| + 1 and sum of dK go to stats[0..2], summed exactly in uint64.
+__global__ void k_apply_moves(int64_t R, const int32_t *__restrict__ lab, const int32_t *__restrict__ size,
+                              const long long *__restrict__ prop_dJ, const int32_t *__restrict__ prop_dest,
+                              const long long *__restrict__ prop_dK, const long long *__restrict__ claim_dJ,
+                              const unsigned int *__restrict__ claim_i, unsigned long long *__restrict__ gkey,
+                              unsigned long long *__restrict__ stats) {
+  unsigned long long moves = 0, dn = 0, dK = 0;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t A = lab[r];
+    unsigned long long k = (uint32_t)A;
+    const long long dJ = prop_dJ[r];
+    if (dJ != NO_MOVE) {
+      const int32_t X = prop_dest[r];
+      const bool win = claim_dJ[A] == dJ && claim_i[A] == (unsigned int)r &&
+                       (X < 0 || (claim_dJ[X] == dJ && claim_i[X] == (unsigned int)r));
+      if (win) {
+        k = X >= 0 ? (unsigned long long)X : (unsigned long long)(R + r);
+        ++moves;
+        dn += (unsigned long long)((X >= 0 ? (long long)size[X] : 0ll) - size[A] + 1);
+        dK += (unsigned long long)prop_dK[r];
+      }
+    }
+    gkey[r] = k;
+  }
+  moves = warp_sum_u64(moves);
+  dn = warp_sum_u64(dn);
+  dK = warp_sum_u64(dK);
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&stats[0], moves);
+    atomicAdd(&stats[1], dn);
+    atomicAdd(&stats[2], dK);
+  }
+}
+
+// n = sum over clusters of C(size, 2), K = the counts of the held pairs whose records share a label: out[0], out[1]
+__global__ void k_search_counts(int64_t R, const int32_t *__restrict__ size, int64_t H,
+                                const unsigned long long *__restrict__ held, const int32_t *__restrict__ hcnt,
+                                const int32_t *__restrict__ lab, unsigned long long *__restrict__ out) {
+  unsigned long long n = 0, K = 0;
+  const int64_t m = R > H ? R : H;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
+    if (i < R) n += (unsigned long long)size[i] * (unsigned long long)(size[i] - 1) / 2;
+    if (i < H) {
+      const unsigned long long k = held[i];
+      if (lab[k >> 32] == lab[k & 0xffffffffull]) K += (uint32_t)hcnt[i];
+    }
+  }
+  n = warp_sum_u64(n);
+  K = warp_sum_u64(K);
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&out[0], n);
+    atomicAdd(&out[1], K);
+  }
+}
+}  // namespace
+
+// The search: check the start labels (into the handle's sample-label buffer) and group them canonically; then rounds of
+// sizes, partner keys, their radix sort (2 lab_bits bits, double-buffered), best moves, the two-stage claims, the
+// moves, and the canonical relabel by group_by_key, until no record proposes or max_rounds rounds are done.  Every
+// buffer is the call's own (48 bytes per held pair and 56 per record, plus the handle's scratch and sort storage), so
+// the table and S never change, whatever the outcome.
+extern "C" int dbl_pairs_binder_search(dbl_pairs *p, int64_t a, int64_t b, const int32_t *start, int32_t max_rounds,
+                                       int32_t *labels_out, int32_t *rounds_out, int32_t *converged_out,
+                                       int64_t *moves, int64_t *dn, int64_t *dK, int64_t *n_out, int64_t *K_out) {
+  if (!p || !start || !labels_out || !rounds_out || !converged_out || !moves || !dn || !dK || !n_out || !K_out ||
+      max_rounds < 1 || b < 1 || b > (int64_t(1) << 16) || a < 0 || a > b)
+    return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  if ((int64_t)p->S * p->R >= (int64_t(1) << 44)) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(start, p->cluster); rc != DBL_OK) return rc;
+  const int64_t R = p->R, H = p->H, E = 2 * H;
+  const int bits = p->lab_bits, gbits = bits_for(2 * R);
+  cudaStream_t st = p->stream;
+  const unsigned long long *held = p->tab_key[p->cur].as<unsigned long long>();
+  const int32_t *hcnt = p->tab_cnt[p->cur].as<int32_t>();
+
+  const size_t e8 = sizeof(unsigned long long) * (size_t)E, e4 = sizeof(int32_t) * (size_t)E;
+  const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(long long) * (size_t)R;
+  Buf key[2], val[2], lab, size, gkey, gkey_s, prop_dJ, prop_dest, prop_dK, claim_dJ, claim_i, stats;
+  POST_TRY(key[0].alloc(e8));
+  POST_TRY(key[1].alloc(e8));
+  POST_TRY(val[0].alloc(e4));
+  POST_TRY(val[1].alloc(e4));
+  POST_TRY(lab.alloc(r4));
+  POST_TRY(size.alloc(r4));
+  POST_TRY(gkey.alloc(r8));
+  POST_TRY(gkey_s.alloc(r8));
+  POST_TRY(prop_dJ.alloc(r8));
+  POST_TRY(prop_dest.alloc(r4));
+  POST_TRY(prop_dK.alloc(r8));
+  POST_TRY(claim_dJ.alloc(r8));
+  POST_TRY(claim_i.alloc(r4));
+  POST_TRY(stats.alloc(4 * sizeof(unsigned long long)));
+  cub::DoubleBuffer<unsigned long long> kb(key[0].as<unsigned long long>(), key[1].as<unsigned long long>());
+  cub::DoubleBuffer<int32_t> vb(val[0].as<int32_t>(), val[1].as<int32_t>());
+  size_t tb = 0;
+  if (E > 0) {
+    POST_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, kb, vb, E, 0, 2 * bits, st));
+    POST_TRY(p->tmp.reserve(tb));
+  }
+  unsigned long long *st4 = stats.as<unsigned long long>();
+  int32_t *L = lab.as<int32_t>(), *Z = size.as<int32_t>();
+
+  // the labels of gkey, grouped; each record labelled by its group's smallest record index
+  auto relabel = [&]() {
+    const int rc = group_by_key(R, gbits, gkey.as<unsigned long long>(), p->iota.as<int32_t>(),
+                                gkey_s.as<unsigned long long>(), p->rec_s.as<int32_t>(), p->head.as<int32_t>(),
+                                p->start.as<int32_t>(), p->tmp, st);
+    if (rc == DBL_OK)
+      k_scatter_labels<<<grid_for(R), THREADS, 0, st>>>(R, p->rec_s.as<int32_t>(), p->start.as<int32_t>(), L);
+    return rc;
+  };
+  auto sizes = [&]() {
+    POST_TRY(cudaMemsetAsync(Z, 0, r4, st));
+    k_label_sizes<<<grid_for(R), THREADS, 0, st>>>(R, L, Z);
+    return DBL_OK;
+  };
+  k_widen_labels<<<grid_for(R), THREADS, 0, st>>>(R, p->cluster.as<int32_t>(), gkey.as<unsigned long long>());
+  if (const int rc = relabel(); rc != DBL_OK) return rc;
+
+  const long long aS = (long long)a * p->S;
+  int32_t rounds = 0, converged = 0;
+  for (;;) {
+    if (const int rc = sizes(); rc != DBL_OK) return rc;
+    if (E > 0) {
+      k_partner_keys<<<grid_for(E), THREADS, 0, st>>>(H, bits, held, hcnt, L, kb.Current(), vb.Current());
+      size_t tbs = p->tmp.cap;
+      POST_TRY(cub::DeviceRadixSort::SortPairs(p->tmp.p, tbs, kb, vb, E, 0, 2 * bits, st));
+    }
+    POST_TRY(cudaMemsetAsync(claim_dJ.p, 0x7f, r8, st));  // above every dJ < 0
+    POST_TRY(cudaMemsetAsync(claim_i.p, 0xff, r4, st));   // above every record index
+    POST_TRY(cudaMemsetAsync(st4, 0, 4 * sizeof(unsigned long long), st));
+    k_best_move<<<grid_for(R), THREADS, 0, st>>>(R, bits, E, kb.Current(), vb.Current(), L, Z, aS, b,
+                                                 prop_dJ.as<long long>(), prop_dest.as<int32_t>(),
+                                                 prop_dK.as<long long>(), claim_dJ.as<long long>(), st4 + 3);
+    k_claim_record<<<grid_for(R), THREADS, 0, st>>>(R, L, prop_dJ.as<long long>(), prop_dest.as<int32_t>(),
+                                                    claim_dJ.as<long long>(), claim_i.as<unsigned int>());
+    unsigned long long props = 0;
+    POST_TRY(cudaMemcpyAsync(&props, st4 + 3, sizeof(props), cudaMemcpyDeviceToHost, st));
+    POST_TRY(cudaGetLastError());
+    POST_TRY(cudaStreamSynchronize(st));
+    if (props == 0) {
+      converged = 1;
+      break;
+    }
+    if (rounds == max_rounds) break;
+    k_apply_moves<<<grid_for(R), THREADS, 0, st>>>(R, L, Z, prop_dJ.as<long long>(), prop_dest.as<int32_t>(),
+                                                   prop_dK.as<long long>(), claim_dJ.as<long long>(),
+                                                   claim_i.as<unsigned int>(), gkey.as<unsigned long long>(), st4);
+    if (const int rc = relabel(); rc != DBL_OK) return rc;
+    unsigned long long log[3];
+    POST_TRY(cudaMemcpyAsync(log, st4, sizeof(log), cudaMemcpyDeviceToHost, st));
+    POST_TRY(cudaGetLastError());
+    POST_TRY(cudaStreamSynchronize(st));
+    moves[rounds] = (int64_t)log[0];
+    dn[rounds] = (int64_t)log[1];
+    dK[rounds] = (int64_t)log[2];
+    ++rounds;
+  }
+
+  // n and K of the result, from its sizes and one pass over the held table
+  if (const int rc = sizes(); rc != DBL_OK) return rc;
+  POST_TRY(cudaMemsetAsync(st4, 0, 2 * sizeof(unsigned long long), st));
+  k_search_counts<<<grid_for(std::max(R, H)), THREADS, 0, st>>>(R, Z, H, held, hcnt, L, st4);
+  unsigned long long nk[2];
+  POST_TRY(cudaMemcpyAsync(nk, st4, sizeof(nk), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaMemcpyAsync(labels_out, L, r4, cudaMemcpyDefault, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  *rounds_out = rounds;
+  *converged_out = converged;
+  *n_out = (int64_t)nk[0];
+  *K_out = (int64_t)nk[1];
+  return DBL_OK;
+}
+
 // ---- every sample against the ground truth -------------------------------------------------------------------------
 namespace {
 // one key per record: its sample label above its true label, each in lab_bits bits

@@ -20,9 +20,12 @@ SMPC_METRICS = ("pairwise", "cluster")  # ProjectStep.scala:36
 POSTERIOR_METRICS = ("posterior-pairwise", "posterior-cluster")
 # the sample of least posterior expected Binder loss (falseLinkCost = the cost of a false link) against the ground truth
 BINDER_METRICS = ("binder-pairwise", "binder-cluster")
-SUPPORTED_METRICS = SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS
+# the least expected Binder loss found by single-record moves from the Binder sample and from the sMPC
+BINDER_SEARCH_METRICS = ("binder-search-pairwise", "binder-search-cluster")
+SUPPORTED_METRICS = SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_SEARCH_METRICS
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
-                        "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters")
+                        "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
+                        "binder-search-clusters")
 
 
 def shared_most_probable_clusters(chain):
@@ -67,6 +70,41 @@ def binder_estimate(chain, false_link_cost):
     mem, off, _ = chain.samples[s]
     return (s, analysis_arrays.sample_labels(chain.num_records, mem, off), n,
             analysis_arrays.binder_losses(n, K, false_link_cost))
+
+
+def binder_search(chain, false_link_cost, starts, max_rounds):
+    """(chosen position, SearchRuns) of the single-record-move search from each start: on the GPU when the platform
+    has one (analysis_gpu), else on the host (analysis_arrays).  Both give identical results."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.binder_search(chain, false_link_cost, starts, max_rounds)
+    return analysis_arrays.binder_search(chain, false_link_cost, starts, max_rounds)
+
+
+def binder_search_estimate(chain, false_link_cost, max_rounds):
+    """The search from the Binder sample and from the sMPC of a ChainArrays: (the chosen start's name, its SearchRun,
+    the rows of binder-search.csv: per start and round its name, the round, the moves, the linked pairs and the
+    expected loss at the given falseLinkCost; round 0 is the start)."""
+    _, labels, n, _ = binder_estimate(chain, false_link_cost)
+    best, runs = binder_search(chain, false_link_cost, [labels, shared_most_probable_clusters(chain)], max_rounds)
+    C, S = int(n.sum()), len(n)
+    rows = []
+    for name, run in zip(analysis_arrays.SEARCH_STARTS, runs):
+        linked = run.linked_pairs()
+        losses = analysis_arrays.expected_losses(linked, run.count_sums(), C, S, false_link_cost)
+        rows += [(name, r, m, k, loss) for r, (m, k, loss) in enumerate(zip(np.r_[0, run.moves], linked, losses))]
+    return analysis_arrays.SEARCH_STARTS[best], runs[best], rows
+
+
+def _searched_cost(false_link_cost):
+    a, b = analysis_arrays.search_cost(false_link_cost)
+    return a / b
+
+
+def _max_search_rounds(prm):
+    m = prm.get("maxSearchRounds", 1000)
+    if isinstance(m, bool) or not isinstance(m, int) or m < 1:
+        raise ValueError("maxSearchRounds must be a positive integer.")
+    return m
 
 
 def _false_link_cost(prm):
@@ -172,6 +210,12 @@ class Project:
                 if "binder-clusters" in prm["quantities"]:
                     L.append(f"  * SummarizeStep: binder-clusters is the sample of least posterior expected Binder "
                              f"loss with falseLinkCost={prm['false_link_cost']}")
+                if "binder-search-clusters" in prm["quantities"]:
+                    L.append(f"  * SummarizeStep: binder-search-clusters is the least posterior expected Binder loss "
+                             f"found by single-record moves from the Binder sample and the sMPC, with "
+                             f"falseLinkCost={prm['false_link_cost']} (searched at "
+                             f"{_searched_cost(prm['false_link_cost'])!r}) and "
+                             f"maxSearchRounds={prm['max_search_rounds']}")
             elif name == "evaluate":
                 smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
                 post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
@@ -188,6 +232,13 @@ class Project:
                     L.append(f"  * EvaluateStep: Evaluating the sample of least posterior expected Binder loss "
                              f"(falseLinkCost={prm['false_link_cost']}, iterations >= {prm['lower_iteration_cutoff']}) "
                              f"using {braces(binder)} metrics")
+                search = [m for m in prm["metrics"] if m in BINDER_SEARCH_METRICS]
+                if search:
+                    L.append(f"  * EvaluateStep: Evaluating the least posterior expected Binder loss found by "
+                             f"single-record moves from the Binder sample and the sMPC (falseLinkCost="
+                             f"{prm['false_link_cost']}, searched at {_searched_cost(prm['false_link_cost'])!r}, "
+                             f"maxSearchRounds={prm['max_search_rounds']}, iterations >= "
+                             f"{prm['lower_iteration_cutoff']}) using {braces(search)} metrics")
             else:
                 L.append("  * CopyFilesStep: Copying {" + ", ".join(prm["file_names"]) + "} to destination "
                          + prm["destination_path"])
@@ -328,14 +379,16 @@ class Project:
                     raise ValueError("minMatchProbability must be in [0, 1].")
                 out.append(("summarize", dict(lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)),
                                               quantities=q, min_match_probability=t,
-                                              false_link_cost=_false_link_cost(prm))))
+                                              false_link_cost=_false_link_cost(prm),
+                                              max_search_rounds=_max_search_rounds(prm))))
             elif name == "evaluate":
                 m = list(prm["metrics"])
                 if not m or any(x not in SUPPORTED_METRICS for x in m):
                     raise ValueError(f"metrics must be one of {SUPPORTED_METRICS}.")
                 out.append(("evaluate", dict(lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)), metrics=m,
                                              use_existing_smpc=bool(prm.get("useExistingSMPC", False)),
-                                             false_link_cost=_false_link_cost(prm))))
+                                             false_link_cost=_false_link_cost(prm),
+                                             max_search_rounds=_max_search_rounds(prm))))
             elif name == "copy-files":
                 out.append(("copy-files", dict(file_names=list(prm["fileNames"]),
                                                destination_path=prm["destinationPath"],
@@ -388,6 +441,11 @@ class Project:
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids),
                                         "binder-clusters.csv")
                         writers.save_binder_loss(ch.chains, ch.iterations, n, losses, self.output_path)
+                    elif q == "binder-search-clusters":
+                        _, run, rows = binder_search_estimate(ch, prm["false_link_cost"], prm["max_search_rounds"])
+                        self._save_smpc(analysis_arrays.labels_to_clusters(run.labels, ch.record_ids),
+                                        "binder-search-clusters.csv")
+                        writers.save_binder_search(rows, self.output_path)
                     else:
                         labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
@@ -437,6 +495,19 @@ class Project:
                         elif m == "binder-cluster":
                             results[m] = analysis_arrays.adjusted_rand_index(labels, truth)
                             text.append(analysis.format_binder_cluster(results[m], *at))
+                if any(m in BINDER_SEARCH_METRICS for m in prm["metrics"]):
+                    ch = ch if ch is not None else self.read_chain(cut)
+                    t = prm["false_link_cost"]
+                    start, run, _ = binder_search_estimate(ch, t, prm["max_search_rounds"])
+                    truth = true_labels(ch.record_ids)
+                    at = (start, run.rounds, run.converged, t, _searched_cost(t))
+                    for m in prm["metrics"]:
+                        if m == "binder-search-pairwise":
+                            results[m] = analysis_arrays.pairwise_metrics(run.labels, truth)
+                            text.append(analysis.format_binder_search_pairwise(results[m], *at))
+                        elif m == "binder-search-cluster":
+                            results[m] = analysis_arrays.adjusted_rand_index(run.labels, truth)
+                            text.append(analysis.format_binder_search_cluster(results[m], *at))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
             elif name == "copy-files":

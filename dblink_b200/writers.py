@@ -7,6 +7,7 @@
   save_pairwise_match_probabilities   pairwise-match-probabilities.csv: recordId1,recordId2,probability
   save_evaluation_samples   evaluation-samples.csv: every sample's counts and metrics against the ground truth
   save_binder_loss   binder-loss.csv: every sample's linked pairs and posterior expected Binder loss
+  save_binder_search   binder-search.csv: every round of the Binder search from each start
 """
 import os
 import time
@@ -229,3 +230,15 @@ def save_binder_loss(chains, iterations, linked_pairs, losses, path):
         fh.write(BINDER_LOSS_HEADER + "\n")
         for k, it, n, loss in zip(chains, iterations, linked_pairs, losses):
             fh.write(f"{int(k)},{int(it)},{int(n)},{float(loss)!r}\n")
+
+
+BINDER_SEARCH_HEADER = "start,round,moves,linkedPairs,expectedLoss"
+
+
+def save_binder_search(rows, path):
+    """binder-search.csv under `path`: rows (start name, round, moves, linked pairs, expected loss) as
+    project.binder_search_estimate gives them, round 0 being the start; the loss written with repr."""
+    with open(os.path.join(path, "binder-search.csv"), "w") as fh:
+        fh.write(BINDER_SEARCH_HEADER + "\n")
+        for start, r, moves, n, loss in rows:
+            fh.write(f"{start},{int(r)},{int(moves)},{int(n)},{float(loss)!r}\n")

@@ -332,7 +332,21 @@ int dbl_posterior_smpc(dbl_posterior *, int32_t *labels_out /* R, may be NULL */
  *                         exceeding max_pairs (checked before anything is allocated for the pairs).  With
  *                         t = the cost of a false link and 1 - t that of a missed link, the posterior expected Binder
  *                         loss of the labelling is ((1 - t) C + t S n - K) / S, C = sum of all held counts.
- *   count / read / score_sample before the first sample give DBL_ERR_STATE.
+ *   dbl_pairs_binder_search  single-record moves from the labelling start[R] (host or device pointer, any labels in
+ *                         [0, R)) while they lower J = a S n - b K, i.e. the expected Binder loss at t = a / b, against
+ *                         the held table.  A round: every record's least (dJ, destination) over its partners' clusters
+ *                         and, out of a cluster of two or more, a singleton (destination -1; a cluster counts as its
+ *                         smallest record index), proposed if dJ < 0; a proposal is applied if it holds the least
+ *                         (dJ, record) among the proposals touching each cluster it touches (its source, and its
+ *                         destination unless a singleton).  The search stops when no record proposes (*converged_out
+ *                         = 1) or after max_rounds rounds (0).  Per round moves / dn / dK (host, max_rounds entries
+ *                         each, *rounds_out written): the moves applied and the sums of their changes of n and K.
+ *                         labels_out (R, host or device): each record labelled by the smallest record index of its
+ *                         cluster.  *n_out = sum over clusters of C(size, 2), *K_out = the sum of the held counts of the
+ *                         pairs it links, so a result is never refused by max_pairs.  The table and S do not change.
+ *                         DBL_ERR_INVALID: a NULL pointer, max_rounds < 1, not 0 <= a <= b <= 2^16, S R >= 2^44, a
+ *                         start label outside [0, R).  Memory: 48 bytes per held pair and 56 per record, for the call.
+ *   count / read / score_sample / binder_search before the first sample give DBL_ERR_STATE.
  * DBL_ERR_INVALID: num_records or max_pairs outside [1, 2^31 - 1].  DBL_ERR_CUDA: no device, or an allocation that
  * fails (the held table and the sample count stay as they were).
  * ------------------------------------------------------------------------------------------------- */
@@ -345,6 +359,10 @@ int dbl_pairs_count(dbl_pairs *, int32_t min_count, int64_t *n_out);
 int dbl_pairs_read(dbl_pairs *, int32_t min_count, int32_t *first, int32_t *second, int32_t *count);
 int dbl_pairs_score_sample(dbl_pairs *, const int32_t *cluster /* R, host or device */, int64_t *num_pairs_out,
                            int64_t *count_sum_out);
+int dbl_pairs_binder_search(dbl_pairs *, int64_t a, int64_t b, const int32_t *start /* R, host or device */,
+                            int32_t max_rounds, int32_t *labels_out /* R */, int32_t *rounds_out,
+                            int32_t *converged_out, int64_t *moves, int64_t *dn, int64_t *dK /* max_rounds each, host */,
+                            int64_t *n_out, int64_t *K_out);
 
 /* ---------------------------------------------------------------------------------------------------
  * Every posterior sample against the ground truth: per sample, the integer counts its pairwise precision / recall /
