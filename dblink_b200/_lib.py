@@ -143,6 +143,12 @@ SIGNATURES = {
     "dbl_eval_add_sample": (C.c_int, [vp, vp]),
     "dbl_eval_num_samples": (C.c_int32, [vp]),
     "dbl_eval_read": (C.c_int, [vp, i64p, i64p, i64p]),
+    "dbl_vi_create": (C.c_int, [C.POINTER(vp), C.c_int64, C.c_int32]),
+    "dbl_vi_free": (None, [vp]),
+    "dbl_vi_add_sample": (C.c_int, [vp, vp]),
+    "dbl_vi_num_samples": (C.c_int32, [vp]),
+    "dbl_vi_set_batch_keys": (C.c_int, [vp, C.c_int64]),
+    "dbl_vi_cross": (C.c_int, [vp, C.c_int64, vp]),
     "dbl_version": (C.c_char_p, []),
 }
 

@@ -4,6 +4,8 @@
   pairwise_match_probabilities                            <- posterior probability that two records are one entity
   binder_clusters                                         <- the sample of least posterior expected Binder loss
   binder_search                                           <- single-record moves that lower the expected Binder loss
+  vi_clusters                                             <- the sample of least posterior expected variation of
+                                                             information
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
   pairwise_metrics                                        <- analysis/PairwiseMetrics.scala:44-63,
                                                              BinaryClassificationMetrics.scala:23-37
@@ -163,6 +165,35 @@ def binder_search(chain, false_link_cost, starts, max_rounds=1000, records=None)
     return min(range(len(runs)), key=lambda k: (runs[k]["loss"], k)), runs
 
 
+def vi_clusters(chain):
+    """The sample of least posterior expected variation of information, by the definition: VI(c, c') = H(c) + H(c')
+    - 2 I(c, c') in bits, with H(c) = - sum over clusters x of p log2 p, p = |x| / R, and I(c, c') = sum over the
+    non-empty cells x ^ y of p_xy log2(p_xy / (p_x p_y)); the expected VI of a sample is the mean of its VI against
+    every sample.  Floats; ties go to the earliest sample.  Returns (position of the sample in the chain, its clusters
+    as frozensets, every sample's expected VI)."""
+    S = len(chain)
+    clusters = [list(clusters_of_sample(s)) for s in chain]
+    R = len({r for cl in clusters for c in cl for r in c})
+
+    def entropy(cl):
+        return -sum(len(x) / R * math.log2(len(x) / R) for x in cl)
+
+    def mutual_information(a, b):
+        total = 0.0
+        for x in a:
+            for y in b:
+                n = len(x & y)
+                if n:
+                    total += n / R * math.log2(n * R / (len(x) * len(y)))
+        return total
+
+    H = [entropy(cl) for cl in clusters]
+    losses = [sum(H[t] + H[s] - 2 * mutual_information(clusters[t], clusters[s]) for s in range(S)) / S
+              for t in range(S)]
+    best = min(range(S), key=lambda s: (losses[s], s))
+    return best, clusters[best], losses
+
+
 def cluster_size_distribution(chain):
     """iteration -> {cluster size: count} (LinkageChain.scala:137-154)."""
     out = {}
@@ -283,6 +314,25 @@ def format_binder_search_cluster(ari, start, rounds, converged, false_link_cost,
     return ("=====================================\n    Binder search cluster metrics\n"
             "-------------------------------------\n"
             + _binder_search_line(start, rounds, converged, false_link_cost, searched_cost)
+            + f" Adj. Rand index: {ari}\n=====================================\n")
+
+
+def _vi_estimate_line(iteration, chain, expected_vi):
+    return f" Estimate:        sample at iteration {iteration} of chain {chain}, expected VI {expected_vi!r}\n"
+
+
+def format_vi_pairwise(m, iteration, chain, expected_vi):
+    """The vi-pairwise section: m = pairwise metrics of the sample chosen at (iteration, chain)."""
+    return ("=====================================\n        VI pairwise metrics\n"
+            "-------------------------------------\n" + _vi_estimate_line(iteration, chain, expected_vi)
+            + f" Precision:      {m['precision']}\n Recall:         {m['recall']}\n F1-score:       {m['f1score']}\n"
+            "=====================================\n")
+
+
+def format_vi_cluster(ari, iteration, chain, expected_vi):
+    """The vi-cluster section: ari = adjusted Rand index of the sample chosen at (iteration, chain)."""
+    return ("=====================================\n         VI cluster metrics\n"
+            "-------------------------------------\n" + _vi_estimate_line(iteration, chain, expected_vi)
             + f" Adj. Rand index: {ari}\n=====================================\n")
 
 

@@ -474,6 +474,81 @@ def binder_search(chain, false_link_cost, starts, max_rounds=1000, max_pairs=MAX
     return search_choice(runs, S, a, b), runs
 
 
+# ---- the variation-of-information point estimate -----------------------------------------------------------
+# With A(c) = sum over the blocks of c of n log2 n, the variation of information of two partitions of R records is
+#   VI(c, c') = (A(c) + A(c') - 2 A(c ^ c')) / R,   c ^ c' = the non-empty cells (cluster of c, cluster of c'),
+# and the posterior expected VI of sample t against the S samples is E_t = (1/S) sum_s VI(C_t, C_s).  In integers:
+#   g_s[n] = the clusters of n records in sample s,  G_t[n] = sum over s != t of the cells of n records in C_t ^ C_s,
+#   D_t[n] = (S - 2) g_t[n] + sum_s g_s[n] - 2 G_t[n],  E_t = sum over n >= 2 of D_t[n] n log2 n / (R S)
+# (n log2 n is 0 at n = 0, 1, so those entries stay 0).  The estimate is the sample of least E_t, ties going to the
+# earliest.  A cell is never larger than its clusters, so every histogram has width M + 1, M = the largest cluster.
+MAX_VI_ENTRIES = 1 << 28  # S x (M + 1) histogram entries (the GPU's int64 matrix: 2 GB at the cap)
+
+
+def vi_width(chain):
+    """M + 1, M = the largest cluster of any sample of the chain (1 without records); ValueError when the S x (M + 1)
+    histograms would exceed MAX_VI_ENTRIES."""
+    S = len(chain.samples)
+    M = max((int(np.diff(off).max()) for _, off, _ in chain.samples if len(off) > 1), default=0)
+    if S * (M + 1) > MAX_VI_ENTRIES:
+        raise ValueError(f"the VI histograms need {S} x {M + 1} entries, more than {MAX_VI_ENTRIES}")
+    return M + 1
+
+
+def vi_cluster_histograms(chain, width):
+    """g, int64[S, width]: per sample the number of clusters of each size n >= 2 (entries 0 and 1 are 0)."""
+    g = np.zeros((len(chain.samples), width), np.int64)
+    for s, (_, off, _) in enumerate(chain.samples):
+        g[s] = np.bincount(np.diff(off), minlength=width)[:width]
+    g[:, :2] = 0
+    return g
+
+
+def vi_cross_histograms(chain):
+    """G, int64[S, M + 1]: per sample t and cell size n >= 2, the number of cells of n records in C_t ^ C_s summed
+    over the samples s != t.  Each pair t < s is counted once and added to both rows; only the records in clusters of
+    two or more of C_t can be in a cell of two or more.  ValueError as vi_width raises it."""
+    R, S = chain.num_records, len(chain.samples)
+    width = vi_width(chain)
+    G = np.zeros((S, width), np.int64)
+    labels = [sample_labels(R, mem, off) for mem, off, _ in chain.samples]
+    for t in range(S):
+        big = np.flatnonzero(np.bincount(labels[t], minlength=R)[labels[t]] >= 2)
+        if not len(big):
+            continue
+        hi = labels[t][big] * R
+        for s in range(t + 1, S):
+            _, n = np.unique(hi + labels[s][big], return_counts=True)
+            h = np.bincount(n[n >= 2], minlength=width)
+            G[t] += h
+            G[s] += h
+    return G
+
+
+def vi_losses(g, G, num_records):
+    """float64[S]: the posterior expected VI of every sample, from the cluster histograms g and the cell histograms G
+    (int64[S, width] each): E_t = fsum over n >= 2 of float(D_t[n]) (n log2 n), divided by R S.  fsum is correctly
+    rounded and does not depend on the order, so equal integers give equal losses."""
+    g, G = np.asarray(g, np.int64), np.asarray(G, np.int64)
+    S, width = G.shape
+    if num_records == 0:
+        return np.zeros(S)
+    D = (S - 2) * g + g.sum(axis=0) - 2 * G
+    weight = np.array([0.0, 0.0] + [n * math.log2(n) for n in range(2, width)])[:width]
+    out = np.zeros(S)
+    for t in range(S):
+        nz = np.flatnonzero(D[t])
+        out[t] = math.fsum(D[t, nz].astype(np.float64) * weight[nz]) / (num_records * S)
+    return out
+
+
+def vi_estimate(losses):
+    """The position of the sample of least expected VI, ties going to the earliest."""
+    if len(losses) == 0:
+        raise ValueError("the VI estimate needs at least one sample")
+    return min(range(len(losses)), key=lambda s: (losses[s], s))
+
+
 def labels_to_clusters(labels, record_ids=None):
     """labels -> list of clusters (arrays of record indices, or lists of ids when record_ids is given)."""
     order = np.argsort(labels, kind="stable")

@@ -11,7 +11,9 @@ analysis_arrays.posterior_metric_counts exactly: they are integers, counted on t
 (sample label, true label) per record.  The Binder-loss counts (n, K) per sample equal analysis_arrays.binder_counts
 exactly: every sample goes into one pairs table, then every sample is scored against it.  The Binder search
 (single-record moves from a start) equals analysis_arrays.binder_search exactly, in labels, round logs, n and K: the
-rule is in integers, and the device applies it to the same table.
+rule is in integers, and the device applies it to the same table.  The cell histograms of the variation-of-information
+estimate equal analysis_arrays.vi_cross_histograms exactly: they are integers, counted on the device from radix-sorted
+(sample, label, label) keys of every pair of held samples.
 """
 import ctypes as C
 
@@ -19,7 +21,7 @@ import numpy as np
 
 from . import _lib
 from .analysis_arrays import (MAX_PAIRS, SearchRun, check_search_size, search_choice, search_cost,
-                              too_many_pairs)
+                              too_many_pairs, vi_width)
 from .engine import DblinkError
 
 _STATUS = {_lib.ERR_INVALID: "invalid argument (bad size, label out of range, too many samples or pairs)",
@@ -248,3 +250,36 @@ def posterior_metric_counts(chain, truth):
     with Evaluation(R, dense, len(chain.samples)) as ev:
         _add_chain(ev, chain)
         return ev.read()
+
+
+class VI(_Handle):
+    """Owner of a dbl_vi handle: samples go in one at a time, cross() gives the cell histograms G."""
+
+    _prefix = "dbl_vi"
+
+    def __init__(self, num_records, max_samples):
+        super().__init__(num_records, int(max_samples))
+
+    def set_batch_keys(self, max_keys):
+        """The keys one sort of cross() may hold: bounds its memory, not its result."""
+        self._call("set_batch_keys", self._h, int(max_keys))
+
+    def cross(self, width):
+        """G, int64[S, width]: per sample t and cell size n >= 2, the cells of n records in C_t ^ C_s over s != t."""
+        G = np.empty((self.num_samples, int(width)), np.int64)
+        self._call("cross", self._h, int(width), G.ctypes.data)
+        return G
+
+
+def vi_cross_histograms(chain, batch_keys=None):
+    """G, int64[S, M + 1], identical to analysis_arrays.vi_cross_histograms(chain), refusals included; batch_keys
+    bounds the keys of one device sort (VI.set_batch_keys)."""
+    R, S = chain.num_records, len(chain.samples)
+    width = vi_width(chain)
+    if R == 0 or S == 0:
+        return np.zeros((S, width), np.int64)
+    with VI(R, S) as vi:
+        if batch_keys is not None:
+            vi.set_batch_keys(batch_keys)
+        _add_chain(vi, chain)
+        return vi.cross(width)

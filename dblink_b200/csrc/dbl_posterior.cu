@@ -23,6 +23,11 @@
 // (sample cluster, true entity) of C(n, 2), pred_pairs = sum over sample clusters of C(size, 2) -- and the number of
 // clusters, all in int64.  Each record becomes one key, sample label above true label; the keys are radix-sorted on
 // their 2 ceil(log2 R) bits, so cells and clusters are runs of the sorted keys -- see dbl_eval_add_sample.
+//
+// Cell histograms of every pair of held samples (dbl_vi_*, same numbers as analysis_arrays.vi_cross_histograms): for
+// every sample t and cell size n >= 2, the number of cells of n records in C_t ^ C_s summed over the other samples s,
+// in int64 -- the integers the posterior expected variation of information is made of.  Cells are runs of radix-sorted
+// (s, label in C_t, label in C_s) keys over the records in C_t's clusters of two or more -- see dbl_vi_cross.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -1103,5 +1108,235 @@ extern "C" int dbl_eval_read(dbl_eval *p, int64_t *tp, int64_t *pred_pairs, int6
   POST_TRY(cudaMemcpyAsync(pred_pairs, c + M, bytes, cudaMemcpyDeviceToHost, p->stream));
   POST_TRY(cudaMemcpyAsync(num_clusters, c + 2 * M, bytes, cudaMemcpyDeviceToHost, p->stream));
   POST_TRY(cudaStreamSynchronize(p->stream));
+  return DBL_OK;
+}
+
+// ---- the variation-of-information estimate: cell histograms of every pair of held samples -------------------------
+namespace {
+constexpr int VI_SMEM_BINS = 64;  // cell sizes below this are summed per block in shared memory for row t
+
+// every record's cluster size, then the largest into *max_size
+__global__ void k_max_size(int64_t R, const int32_t *__restrict__ size, int32_t *__restrict__ max_size) {
+  int32_t m = 0;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x)
+    m = max(m, size[r]);
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(max_size, m);
+}
+
+// 1 for a record in a cluster of two or more of C_t (only those can be in a cell of two or more); entry R is 0, so an
+// exclusive scan gives every flagged record its place and ends with their number
+__global__ void k_flag_big(int64_t R, const int32_t *__restrict__ lab, const int32_t *__restrict__ size,
+                           int32_t *__restrict__ flag) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r <= R; r += (int64_t)gridDim.x * blockDim.x)
+    flag[r] = r < R && size[lab[r]] >= 2;
+}
+
+__global__ void k_scatter_flagged(int64_t R, const int32_t *__restrict__ flag, const int32_t *__restrict__ pos,
+                                  int32_t *__restrict__ sel) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x)
+    if (flag[r]) sel[pos[r]] = (int32_t)r;
+}
+
+// one key per (sample s0 + i, selected record): i << 2 lab_bits | label in C_t << lab_bits | label in C_s; the
+// selected records are in ascending index, so a sample's labels are read in order
+__global__ void k_vi_keys(int64_t nsel, int32_t B, int lab_bits, int64_t R, const int32_t *__restrict__ sel,
+                          const int32_t *__restrict__ lab_t, const int32_t *__restrict__ rows,
+                          unsigned long long *__restrict__ key) {
+  for (int32_t i = blockIdx.y; i < B; i += gridDim.y) {
+    const int32_t *lab_s = rows + (int64_t)i * R;
+    const unsigned long long hi = (unsigned long long)i << (2 * lab_bits);
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < nsel; k += (int64_t)gridDim.x * blockDim.x) {
+      const int32_t r = sel[k];
+      key[(int64_t)i * nsel + k] = hi | (unsigned long long)(uint32_t)lab_t[r] << lab_bits | (uint32_t)lab_s[r];
+    }
+  }
+}
+
+// the length of the run of sorted keys that ends at i (key[i] == k): gallop back from i, then a binary search
+__device__ __forceinline__ int64_t run_length(const unsigned long long *__restrict__ key, int64_t i,
+                                              unsigned long long k) {
+  int64_t known = i, step = 1, lo = 0;  // key[known] == k
+  for (;;) {
+    const int64_t j = i - step;
+    if (j < 0) break;
+    if (key[j] != k) {
+      lo = j + 1;
+      break;
+    }
+    known = j;
+    step <<= 1;
+  }
+  return i + 1 - (lo + lower_bound_u64(key + lo, known - lo, k));
+}
+
+// Over the sorted keys of one batch: the last position of each run of n >= 2 equal keys (a cell of C_t ^ C_s) adds 1
+// to G[t][n] and to G[s][n].  A warp's lanes take 32 consecutive positions; lanes with equal (s, n), or equal n for
+// row t, are summed by __match_any_sync and add once, row t's small n into a shared-memory histogram first.
+__global__ void k_vi_cells(int64_t n, int hi_shift, const unsigned long long *__restrict__ key, int32_t s0, int32_t t,
+                           int64_t width, unsigned long long *__restrict__ G) {
+  __shared__ unsigned long long hist[VI_SMEM_BINS];
+  for (int j = threadIdx.x; j < VI_SMEM_BINS; j += blockDim.x) hist[j] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  unsigned long long *Gt = G + (int64_t)t * width;
+  for (int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31); base < n;
+       base += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t i = base + lane;
+    int64_t len = 0;
+    unsigned long long k = 0;
+    if (i < n) {
+      k = key[i];
+      if (i > 0 && key[i - 1] == k && (i == n - 1 || key[i + 1] != k)) len = run_length(key, i, k);
+    }
+    const unsigned emit = __ballot_sync(0xffffffffu, len >= 2);
+    if (len >= 2) {
+      const int64_t s = s0 + (int64_t)(k >> hi_shift);
+      const unsigned by_s = __match_any_sync(emit, (unsigned long long)s << 32 | (unsigned long long)len);
+      if (lane == __ffs(by_s) - 1) atomicAdd(&G[s * width + len], (unsigned long long)__popc(by_s));
+      const unsigned by_n = __match_any_sync(emit, (unsigned long long)len);
+      if (lane == __ffs(by_n) - 1) {
+        if (len < VI_SMEM_BINS) atomicAdd(&hist[len], (unsigned long long)__popc(by_n));
+        else atomicAdd(&Gt[len], (unsigned long long)__popc(by_n));
+      }
+    }
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < VI_SMEM_BINS && j < width; j += blockDim.x)
+    if (hist[j]) atomicAdd(&Gt[j], hist[j]);
+}
+}  // namespace
+
+struct dbl_vi : Handle {
+  int32_t max_samples = 0;
+  int lab_bits = 1;                       // bits of a label in [0, R)
+  int32_t max_size = 0;                   // M, the largest cluster of any held sample
+  int64_t batch_keys = PAIR_BLOCK;        // keys of one batch of samples s (at least the selected records of one)
+  Buf rows;                               // [max_samples][R] held labels
+  Buf size, peak;                         // cluster sizes of one sample; its largest (int32)
+};
+
+extern "C" int dbl_vi_create(dbl_vi **out, int64_t num_records, int32_t max_samples) {
+  if (!out) return DBL_ERR_INVALID;
+  *out = nullptr;
+  if (num_records <= 0 || num_records > INT32_MAX || max_samples <= 0) return DBL_ERR_INVALID;
+  return open_handle(out, num_records, [&](dbl_vi *p) {
+    const int64_t R = num_records;
+    p->max_samples = max_samples;
+    p->lab_bits = bits_for(R);
+    const size_t r4 = sizeof(int32_t) * (size_t)R;
+    if (p->rows.alloc(r4 * (size_t)max_samples) != cudaSuccess || p->size.alloc(r4) != cudaSuccess ||
+        p->peak.alloc(sizeof(int32_t)) != cudaSuccess)
+      return DBL_ERR_CUDA;  // the held label matrix does not fit
+    return DBL_OK;
+  });
+}
+
+extern "C" void dbl_vi_free(dbl_vi *p) { free_handle(p); }
+
+extern "C" int32_t dbl_vi_num_samples(const dbl_vi *p) { return p ? p->S : 0; }
+
+extern "C" int dbl_vi_set_batch_keys(dbl_vi *p, int64_t max_keys) {
+  if (!p || max_keys < 1) return DBL_ERR_INVALID;
+  p->batch_keys = max_keys;
+  return DBL_OK;
+}
+
+// One sample: check the labels; its largest cluster; append it as row S.  S and M move only on success.
+extern "C" int dbl_vi_add_sample(dbl_vi *p, const int32_t *cluster) {
+  if (!p || !cluster || p->S >= p->max_samples) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(cluster, p->cluster); rc != DBL_OK) return rc;
+  const int64_t R = p->R;
+  cudaStream_t st = p->stream;
+  int32_t *Z = p->size.as<int32_t>();
+  POST_TRY(cudaMemsetAsync(Z, 0, sizeof(int32_t) * R, st));
+  POST_TRY(cudaMemsetAsync(p->peak.p, 0, sizeof(int32_t), st));
+  k_label_sizes<<<grid_for(R), THREADS, 0, st>>>(R, p->cluster.as<int32_t>(), Z);
+  k_max_size<<<grid_for(R), THREADS, 0, st>>>(R, Z, p->peak.as<int32_t>());
+  POST_TRY(cudaMemcpyAsync(p->rows.as<int32_t>() + (size_t)p->S * R, p->cluster.p, sizeof(int32_t) * R,
+                           cudaMemcpyDeviceToDevice, st));
+  int32_t m = 0;
+  POST_TRY(cudaMemcpyAsync(&m, p->peak.p, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  p->max_size = std::max(p->max_size, m);
+  ++p->S;
+  return DBL_OK;
+}
+
+// G[t][n] = sum over s != t of the cells of n >= 2 records in C_t ^ C_s, each unordered pair {t, s} counted once and
+// added to both rows.  For every t: the sizes of C_t and its n_t records in clusters of two or more, in ascending index
+// (flags, an exclusive scan, a scatter); then the samples s > t in batches of B, B n_t <= max(batch_keys, n_t) keys
+// that fit 64 bits; per batch the keys (k_vi_keys), one radix sort over their 2 lab_bits + bits_for(B) bits, and one
+// pass (k_vi_cells) over the sorted keys.  The held samples never change.
+extern "C" int dbl_vi_cross(dbl_vi *p, int64_t width, int64_t *G_out) {
+  if (!p || !G_out) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  if (width < (int64_t)p->max_size + 1 || width > INT64_MAX / 8 / p->S) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  const int64_t R = p->R;
+  const int32_t S = p->S;
+  const int b = p->lab_bits;
+  cudaStream_t st = p->stream;
+  const size_t gbytes = sizeof(unsigned long long) * (size_t)S * (size_t)width;
+  Buf G, flag, pos, sel, key[2], tmp;
+  POST_TRY(G.alloc(gbytes));
+  POST_TRY(cudaMemsetAsync(G.p, 0, gbytes, st));
+  if (S > 1) {
+    POST_TRY(flag.alloc(sizeof(int32_t) * (size_t)(R + 1)));
+    POST_TRY(pos.alloc(sizeof(int32_t) * (size_t)(R + 1)));
+    POST_TRY(sel.alloc(sizeof(int32_t) * (size_t)R));
+    const int32_t *rows = p->rows.as<int32_t>();
+    int32_t *Z = p->size.as<int32_t>();
+    size_t tb_scan = 0;
+    POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb_scan, (const int32_t *)nullptr, (int32_t *)nullptr, R + 1, st));
+    // the batch width in samples allowed by 64-bit keys: bits_for(B) <= 64 - 2 b
+    const int64_t B_bits = (64 - 2 * b) >= 31 ? INT32_MAX : (int64_t(1) << (64 - 2 * b));
+    // the key buffers grow on demand, never past the largest batch this call can make
+    const int64_t most_keys = std::min<int64_t>(std::max<int64_t>(p->batch_keys, R), R * (int64_t)(S - 1));
+    const size_t key_limit = sizeof(unsigned long long) * (size_t)most_keys;
+    for (int32_t t = 0; t + 1 < S; ++t) {
+      const int32_t *lab_t = rows + (size_t)t * R;
+      POST_TRY(cudaMemsetAsync(Z, 0, sizeof(int32_t) * R, st));
+      k_label_sizes<<<grid_for(R), THREADS, 0, st>>>(R, lab_t, Z);
+      k_flag_big<<<grid_for(R + 1), THREADS, 0, st>>>(R, lab_t, Z, flag.as<int32_t>());
+      POST_TRY(tmp.reserve(tb_scan));
+      size_t tb = tmp.cap;
+      POST_TRY(cub::DeviceScan::ExclusiveSum(tmp.p, tb, flag.as<int32_t>(), pos.as<int32_t>(), R + 1, st));
+      k_scatter_flagged<<<grid_for(R), THREADS, 0, st>>>(R, flag.as<int32_t>(), pos.as<int32_t>(), sel.as<int32_t>());
+      int32_t nsel = 0;
+      POST_TRY(cudaMemcpyAsync(&nsel, pos.as<int32_t>() + R, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+      POST_TRY(cudaGetLastError());
+      POST_TRY(cudaStreamSynchronize(st));
+      if (nsel == 0) continue;  // C_t is all singletons: every cell with it is a singleton
+      const int64_t B_max = std::min<int64_t>({(int64_t)S - 1 - t, std::max<int64_t>(1, p->batch_keys / nsel),
+                                               B_bits});
+      for (int32_t s0 = t + 1; s0 < S; s0 += (int32_t)B_max) {
+        const int32_t B = (int32_t)std::min<int64_t>(B_max, S - s0);
+        const int64_t n = (int64_t)B * nsel;
+        const int end_bit = 2 * b + bits_for(B);
+        POST_TRY(key[0].reserve(sizeof(unsigned long long) * (size_t)n, key_limit));
+        POST_TRY(key[1].reserve(sizeof(unsigned long long) * (size_t)n, key_limit));
+        cub::DoubleBuffer<unsigned long long> kb(key[0].as<unsigned long long>(), key[1].as<unsigned long long>());
+        const dim3 grid((unsigned)std::min<int64_t>((nsel + THREADS - 1) / THREADS, 1024),
+                        (unsigned)std::min<int32_t>(B, 65535));
+        k_vi_keys<<<grid, THREADS, 0, st>>>(nsel, B, b, R, sel.as<int32_t>(), lab_t, rows + (size_t)s0 * R,
+                                            kb.Current());
+        size_t tbs = 0;
+        POST_TRY(cub::DeviceRadixSort::SortKeys(nullptr, tbs, kb, n, 0, end_bit, st));
+        POST_TRY(tmp.reserve(tbs));
+        tbs = tmp.cap;
+        POST_TRY(cub::DeviceRadixSort::SortKeys(tmp.p, tbs, kb, n, 0, end_bit, st));
+        k_vi_cells<<<grid_for(n), THREADS, 0, st>>>(n, 2 * b, kb.Current(), s0, t, width,
+                                                    G.as<unsigned long long>());
+        POST_TRY(cudaGetLastError());
+      }
+    }
+  }
+  // host or device output: unified addressing picks the copy direction
+  POST_TRY(cudaMemcpyAsync(G_out, G.p, gbytes, cudaMemcpyDefault, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
   return DBL_OK;
 }

@@ -22,10 +22,12 @@ POSTERIOR_METRICS = ("posterior-pairwise", "posterior-cluster")
 BINDER_METRICS = ("binder-pairwise", "binder-cluster")
 # the least expected Binder loss found by single-record moves from the Binder sample and from the sMPC
 BINDER_SEARCH_METRICS = ("binder-search-pairwise", "binder-search-cluster")
-SUPPORTED_METRICS = SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_SEARCH_METRICS
+# the sample of least posterior expected variation of information against the ground truth
+VI_METRICS = ("vi-pairwise", "vi-cluster")
+SUPPORTED_METRICS = SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_SEARCH_METRICS + VI_METRICS
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
-                        "binder-search-clusters")
+                        "binder-search-clusters", "vi-clusters")
 
 
 def shared_most_probable_clusters(chain):
@@ -93,6 +95,28 @@ def binder_search_estimate(chain, false_link_cost, max_rounds):
         losses = analysis_arrays.expected_losses(linked, run.count_sums(), C, S, false_link_cost)
         rows += [(name, r, m, k, loss) for r, (m, k, loss) in enumerate(zip(np.r_[0, run.moves], linked, losses))]
     return analysis_arrays.SEARCH_STARTS[best], runs[best], rows
+
+
+def vi_cross_histograms(chain):
+    """G of a ChainArrays, the cell histograms of every sample against the others: on the GPU when the platform has
+    one (analysis_gpu), else on the host (analysis_arrays).  Both give identical arrays."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.vi_cross_histograms(chain)
+    return analysis_arrays.vi_cross_histograms(chain)
+
+
+def vi_estimate(chain):
+    """The sample of least posterior expected variation of information of a ChainArrays: (its position, its labels,
+    every sample's number of clusters and expected VI)."""
+    if not chain.samples:
+        raise ValueError("the VI estimate needs at least one sample at or after lowerIterationCutoff")
+    G = vi_cross_histograms(chain)
+    g = analysis_arrays.vi_cluster_histograms(chain, G.shape[1])
+    losses = analysis_arrays.vi_losses(g, G, chain.num_records)
+    s = analysis_arrays.vi_estimate(losses)
+    mem, off, _ = chain.samples[s]
+    return (s, analysis_arrays.sample_labels(chain.num_records, mem, off),
+            np.array([len(off) - 1 for _, off, _ in chain.samples], np.int64), losses)
 
 
 def _searched_cost(false_link_cost):
@@ -216,6 +240,9 @@ class Project:
                              f"falseLinkCost={prm['false_link_cost']} (searched at "
                              f"{_searched_cost(prm['false_link_cost'])!r}) and "
                              f"maxSearchRounds={prm['max_search_rounds']}")
+                if "vi-clusters" in prm["quantities"]:
+                    L.append("  * SummarizeStep: vi-clusters is the sample of least posterior expected variation of "
+                             "information")
             elif name == "evaluate":
                 smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
                 post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
@@ -239,6 +266,10 @@ class Project:
                              f"{prm['false_link_cost']}, searched at {_searched_cost(prm['false_link_cost'])!r}, "
                              f"maxSearchRounds={prm['max_search_rounds']}, iterations >= "
                              f"{prm['lower_iteration_cutoff']}) using {braces(search)} metrics")
+                vi = [m for m in prm["metrics"] if m in VI_METRICS]
+                if vi:
+                    L.append(f"  * EvaluateStep: Evaluating the sample of least posterior expected variation of "
+                             f"information (iterations >= {prm['lower_iteration_cutoff']}) using {braces(vi)} metrics")
             else:
                 L.append("  * CopyFilesStep: Copying {" + ", ".join(prm["file_names"]) + "} to destination "
                          + prm["destination_path"])
@@ -446,6 +477,10 @@ class Project:
                         self._save_smpc(analysis_arrays.labels_to_clusters(run.labels, ch.record_ids),
                                         "binder-search-clusters.csv")
                         writers.save_binder_search(rows, self.output_path)
+                    elif q == "vi-clusters":
+                        _, labels, num_clusters, losses = vi_estimate(ch)
+                        self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids), "vi-clusters.csv")
+                        writers.save_vi_loss(ch.chains, ch.iterations, num_clusters, losses, self.output_path)
                     else:
                         labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
@@ -508,6 +543,18 @@ class Project:
                         elif m == "binder-search-cluster":
                             results[m] = analysis_arrays.adjusted_rand_index(run.labels, truth)
                             text.append(analysis.format_binder_search_cluster(results[m], *at))
+                if any(m in VI_METRICS for m in prm["metrics"]):
+                    ch = ch if ch is not None else self.read_chain(cut)
+                    s, labels, _, losses = vi_estimate(ch)
+                    truth = true_labels(ch.record_ids)
+                    at = (int(ch.iterations[s]), int(ch.chains[s]), float(losses[s]))
+                    for m in prm["metrics"]:
+                        if m == "vi-pairwise":
+                            results[m] = analysis_arrays.pairwise_metrics(labels, truth)
+                            text.append(analysis.format_vi_pairwise(results[m], *at))
+                        elif m == "vi-cluster":
+                            results[m] = analysis_arrays.adjusted_rand_index(labels, truth)
+                            text.append(analysis.format_vi_cluster(results[m], *at))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
             elif name == "copy-files":

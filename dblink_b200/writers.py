@@ -8,6 +8,7 @@
   save_evaluation_samples   evaluation-samples.csv: every sample's counts and metrics against the ground truth
   save_binder_loss   binder-loss.csv: every sample's linked pairs and posterior expected Binder loss
   save_binder_search   binder-search.csv: every round of the Binder search from each start
+  save_vi_loss   vi-loss.csv: every sample's number of clusters and posterior expected variation of information
 """
 import os
 import time
@@ -242,3 +243,15 @@ def save_binder_search(rows, path):
         fh.write(BINDER_SEARCH_HEADER + "\n")
         for start, r, moves, n, loss in rows:
             fh.write(f"{start},{int(r)},{int(moves)},{int(n)},{float(loss)!r}\n")
+
+
+VI_LOSS_HEADER = "chain,iteration,numClusters,expectedLoss"
+
+
+def save_vi_loss(chains, iterations, num_clusters, losses, path):
+    """vi-loss.csv under `path`: one row per sample in pooled order (chain-major, then iteration), its number of
+    clusters and its expected variation of information (analysis_arrays.vi_losses), written with repr."""
+    with open(os.path.join(path, "vi-loss.csv"), "w") as fh:
+        fh.write(VI_LOSS_HEADER + "\n")
+        for k, it, n, loss in zip(chains, iterations, num_clusters, losses):
+            fh.write(f"{int(k)},{int(it)},{int(n)},{float(loss)!r}\n")

@@ -389,6 +389,38 @@ int dbl_eval_add_sample(dbl_eval *, const int32_t *cluster /* R, host or device 
 int32_t dbl_eval_num_samples(const dbl_eval *);
 int dbl_eval_read(dbl_eval *, int64_t *tp, int64_t *pred_pairs, int64_t *num_clusters /* S entries each, host */);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Cell histograms for the posterior expected variation of information (VI) of every sample, on the device that is
+ * current when dbl_vi_create() is called.  Samples are fed one at a time as cluster[R], as for dbl_posterior_*, and
+ * held as an int32 [max_samples][R] device matrix allocated up front (4 R max_samples bytes).  For held samples
+ * C_0 .. C_{S-1} and n >= 2:
+ *   G[t][n] = sum over s != t of the number of cells (non-empty intersections of a cluster of C_t and one of C_s) of
+ *             exactly n records, int64; G[t][0] = G[t][1] = 0.
+ * With g_s[n] = the clusters of n records in sample s and D_t[n] = (S - 2) g_t[n] + sum_s g_s[n] - 2 G[t][n], the
+ * expected VI of sample t against the S samples is sum over n of D_t[n] n log2 n / (R S); that sum is the caller's.
+ *   dbl_vi_add_sample  cluster may be a host or a device pointer (ready when the call is made); a label outside
+ *                      [0, R) or a sample beyond max_samples gives DBL_ERR_INVALID and adds nothing.  The handle
+ *                      tracks M, the largest cluster of any held sample.
+ *   dbl_vi_set_batch_keys  the keys one sort may hold (default 2^26; at least the records of one sample's clusters of
+ *                      two or more are always taken together); DBL_ERR_INVALID below 1.  It bounds the memory of
+ *                      dbl_vi_cross and does not change its result.
+ *   dbl_vi_cross       G as S x width int64 (row-major, host or device pointer).  DBL_ERR_INVALID: width < M + 1 or
+ *                      S width 8 bytes past INT64_MAX; DBL_ERR_STATE before the first sample.  Memory, the call's own
+ *                      and freed on return: 8 S width bytes, 12 per record, and two buffers of 8 bytes per sorted key
+ *                      (at most max(batch keys, R)) plus the sort's temporary storage.  The held samples do not
+ *                      change, whatever the outcome.  The work is S (S - 1) / 2 sorts of the records in clusters of
+ *                      two or more, batched over samples.
+ * DBL_ERR_INVALID: num_records outside [1, 2^31 - 1] or max_samples < 1.  DBL_ERR_CUDA: no device, or the held label
+ * matrix (or a buffer of dbl_vi_cross) does not fit on it.
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct dbl_vi dbl_vi;
+int dbl_vi_create(dbl_vi **out, int64_t num_records, int32_t max_samples);
+void dbl_vi_free(dbl_vi *);
+int dbl_vi_add_sample(dbl_vi *, const int32_t *cluster /* R, host or device */);
+int32_t dbl_vi_num_samples(const dbl_vi *);
+int dbl_vi_set_batch_keys(dbl_vi *, int64_t max_keys);
+int dbl_vi_cross(dbl_vi *, int64_t width, int64_t *G_out /* S x width */);
+
 /* The protocol functions of the theta draw (DESIGN.md 4.5), exposed so that they can be checked without a GPU:
  * log / exp built from individually rounded binary64 operations, and updateDistProbs (GU:305-320) itself. */
 double dbl_det_log(double x);
