@@ -56,6 +56,7 @@ SIGNATURES = {
     "dbl_index_value_id": (C.c_int32, [vp, C.c_char_p]),
     "dbl_index_value": (C.c_char_p, [vp, C.c_int32]),
     "dbl_index_tables": (C.c_int, [vp, f64p, f64p, i32p, i32p, f64p]),
+    "dbl_index_base_tables": (C.c_int, [vp, i32p, f64p, f64p, f64p, f64p, f64p]),
     "dbl_index_exp_sim": (C.c_double, [vp, C.c_int32, C.c_int32]),
     "dbl_similarity": (C.c_double, [C.c_int, C.c_char_p, C.c_char_p, C.c_double, C.c_double]),
     "dbl_kdtree_fit": (C.c_int, [C.POINTER(vp), i32p, C.c_int64, C.c_int32, C.c_int32, i32p, C.c_int32]),

@@ -16,6 +16,8 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <cfloat>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -30,6 +32,7 @@
 #define DBL_ENGINE_TU 1
 #include "dbl_link.cuh"
 #include "dbl_link_pcg2.cuh"
+#include "dbl_scale.h"
 
 #define CUDA_TRY(expr)                                                                          \
   do {                                                                                          \
@@ -411,11 +414,12 @@ struct ValParams {
   const double *theta;
   const int *ent_rec_ptr, *rec_by_ent;
   int *y;
+  long long *far_list;  // (entity, attribute) rows e * A + a whose draw k_values_rescaled makes; count in ctl[CTL_FAR]
 };
 
 struct BaseDist {
   const AttrDev *at;
-  int k;
+  int k, sc, ez;  // sc: the uncached weights are rescaled, zk = Z_k * 2^(-512 ez)
   const double *pk, *cdf;
   double zk;
 };
@@ -425,10 +429,14 @@ __device__ __forceinline__ double base_weight(const AttrDev &at, int k, int v) {
     for (int i = 0; i < k; ++i) w = w * at.norm[v];
   return w;
 }
+// RS: the uncached weights may need rescaling (DESIGN.md section 4.7).  Never for k <= 1 (Z_0 = 1, Z_1 >= min n(v)),
+// so the draws of isolated entities and single-record clusters compile without it
+template <bool RS>
 __device__ void base_init(BaseDist &b, const AttrDev &at, int k) {
   b.at = &at;
   if (at.is_const) k = 0;
   b.k = k;
+  b.sc = 0;
   if (k <= at.kmax) {
     b.pk = at.pk + (size_t)k * at.V;
     b.cdf = at.cdf + (size_t)k * at.V;
@@ -437,17 +445,33 @@ __device__ void base_init(BaseDist &b, const AttrDev &at, int k) {
     b.pk = nullptr; b.cdf = nullptr;
     double z = 0.0;
     for (int v = 0; v < at.V; ++v) z += base_weight(at, k, v);
+    if (RS) {
+      b.sc = !(z >= BASE_Z_MIN);  // as base_row: the weights underflow, rescale them
+      if (b.sc) z = base_z_sc(at.V, at.probs, at.norm, at.is_const, k, b.ez);
+    }
     b.zk = z;
   }
 }
-__device__ __forceinline__ double base_prob(const BaseDist &b, int v) {
-  return b.pk ? b.pk[v] : base_weight(*b.at, b.k, v) / b.zk;
+// uncached weight of v at the scale of zk
+template <bool RS>
+__device__ __forceinline__ double base_w(const BaseDist &b, int v) {
+  if (RS && b.sc) {
+    int e;
+    const double w = base_weight_sc(b.at->probs, b.at->norm, b.at->is_const, b.k, v, e);
+    return sc_down(w, e - b.ez);
+  }
+  return base_weight(*b.at, b.k, v);
 }
+template <bool RS>
+__device__ __forceinline__ double base_prob(const BaseDist &b, int v) {
+  return b.pk ? b.pk[v] : base_w<RS>(b, v) / b.zk;
+}
+template <bool RS>
 __device__ int base_draw(const BaseDist &b, double u) {
   if (b.cdf) return invcdf(b.cdf, b.at->V, u);
   double c = 0.0;
   for (int v = 0; v < b.at->V; ++v) {
-    c += base_weight(*b.at, b.k, v) / b.zk;
+    c += base_w<RS>(b, v) / b.zk;
     if (c > u) return v;
   }
   return b.at->V - 1;
@@ -480,123 +504,19 @@ __device__ __forceinline__ bool in_support(const ValParams &p, const AttrDev &at
   return row_find(at, xr, v, e);
 }
 
-// new value of attribute a of entity e.  UB > 1: the loop over the similarity row of a single linked record fetches
-// UB candidates at a time (independent loads, same sums in the same order): for problems too small to fill the GPU
-// the kernel's time is the longest dependent-load chain of one thread, not throughput
-template <int UB>
-__device__ int value_update(const ValParams &p, uint32_t iter, int64_t e, int a) {
-  const AttrDev &at = p.attrs[a];
-  const bool collapsed = (p.sampler == DBL_PCG_I || p.sampler == DBL_PCG_II);
-  const U2 u = chain_uniform2(p.seed, p.cm.seeds, p.cm.ents, PH_VALUE, iter, e, (uint32_t)a);
-  const int lo = p.ent_rec_ptr[e], hi = p.ent_rec_ptr[e + 1];
+// the value draw of an entity with two or more linked records (first-appearance enumeration of the support, two
+// passes).  Plain weights W(v) = B_k(v) (G(v) - 1); SC: every weight carried as W * 2^(512 e) (DESIGN.md section
+// 4.7): t(v) = B_k(v) Z_k (G(v) - 1), the walk in units of the largest scale E, Z_k only in the mixture test.  The
+// plain form returns VALUE_FAR when the total leaves the double range (G overflows for clusters of about 709 / ln g
+// agreeing records, and 0 * inf is NaN where B_k(v) underflowed as well); k_values_rescaled then draws with SC.
+// RS: the base distribution may be rescaled (base_init<RS>).
+constexpr int VALUE_FAR = -2;
+template <bool SC, bool RS>
+__device__ __forceinline__ int cluster_draw(const ValParams &p, const AttrDev &at, int a, int lo, int hi, bool collapsed,
+                                            const BaseDist &b, U2 u) {
   const int *rec = p.rec_by_ent;
-
-  int k = 0;
-  for (int i = lo; i < hi; ++i) k += (p.x[(int64_t)rec[i] * p.A + a] >= 0);
-  BaseDist b;
-  if (k == 0) {  // GU:588-589
-    base_init(b, at, 0);
-    return base_draw(b, u.u1);
-  }
-  if (!collapsed) {
-    for (int i = lo; i < hi; ++i) {  // GU:619-630
-      const int r = rec[i];
-      const int xr = p.x[(int64_t)r * p.A + a];
-      if (xr >= 0 && !((p.zmask[r] >> a) & 1u)) return xr;
-    }
-    if (at.is_const) {  // GU:633-634
-      base_init(b, at, 0);
-      return base_draw(b, u.u1);
-    }
-  }
-  base_init(b, at, k);  // GU:584-586
   double total = 0.0, target = 0.0, cum = 0.0;
-  int picked = -1, last_pos = -1;
-  if (hi - lo == 1) {
-    // one linked record (most entities): the candidate values are the record's own similarity row, so the factors
-    // come straight from that row (no searches, no first-appearance check); same operations as the general path
-    const int r = rec[lo];
-    const int xr = p.x[(int64_t)r * p.A + a];  // observed (k == 1)
-    const int q0 = at.is_const ? 0 : at.rowptr[xr];
-    const int nv = at.is_const ? 1 : (at.rowptr[xr + 1] - q0);
-    double extra = 0.0;  // what the collapsed update adds to the factor of v == x (GU:553,557,560)
-    if (collapsed) {
-      const double th = p.theta[a * p.F + p.file[r]];
-      extra = at.is_const ? (1.0 / th - 1.0) / at.phi[xr] : (1.0 / th - 1.0) / (at.phi[xr] * at.norm[xr]);
-    }
-    auto weight = [&](int q, int &v) -> double {
-      double G = 1.0;
-      if (at.is_const) {
-        v = xr;
-        if (collapsed) G = G * (1.0 + extra);
-      } else {
-        v = at.col[q0 + q];
-        const double ex = at.expsim[q0 + q];
-        G = G * ((collapsed && v == xr) ? ex + extra : ex);
-      }
-      return base_prob(b, v) * (G - 1.0);  // GU:567 / 724
-    };
-    if constexpr (UB > 1) {
-      // same weights, same order of the sums; the loads of UB consecutive candidates are issued together
-      auto batch = [&](int q, int (&v)[UB], double (&W)[UB]) {
-        double ex[UB], bp[UB];
-#pragma unroll
-        for (int i = 0; i < UB; ++i) {
-          const int qq = min(q + i, nv - 1);
-          v[i] = at.is_const ? xr : at.col[q0 + qq];
-          ex[i] = at.is_const ? 0.0 : at.expsim[q0 + qq];
-        }
-#pragma unroll
-        for (int i = 0; i < UB; ++i) bp[i] = base_prob(b, v[i]);
-#pragma unroll
-        for (int i = 0; i < UB; ++i) {
-          double G = 1.0;
-          if (at.is_const) { if (collapsed) G = G * (1.0 + extra); }
-          else G = G * ((collapsed && v[i] == xr) ? ex[i] + extra : ex[i]);
-          W[i] = bp[i] * (G - 1.0);
-        }
-      };
-      for (int q = 0; q < nv; q += UB) {
-        int v[UB];
-        double W[UB];
-        batch(q, v, W);
-#pragma unroll
-        for (int i = 0; i < UB; ++i)
-          if (q + i < nv) total += W[i];
-      }
-      if (u.u0 < 1.0 / (1.0 + total)) return base_draw(b, u.u1);  // GU:593-594
-      target = u.u1 * total;
-      for (int q = 0; q < nv && picked < 0; q += UB) {
-        int v[UB];
-        double W[UB];
-        batch(q, v, W);
-#pragma unroll
-        for (int i = 0; i < UB; ++i)
-          if (q + i < nv && picked < 0) {
-            cum += W[i];
-            if (W[i] > 0.0) last_pos = v[i];
-            if (cum > target) picked = v[i];
-          }
-      }
-    } else {
-      for (int q = 0; q < nv; ++q) {
-        int v;
-        total += weight(q, v);
-      }
-      if (u.u0 < 1.0 / (1.0 + total)) return base_draw(b, u.u1);  // GU:593-594
-      target = u.u1 * total;
-      for (int q = 0; q < nv && picked < 0; ++q) {
-        int v;
-        const double W = weight(q, v);
-        cum += W;
-        if (W > 0.0) last_pos = v;
-        if (cum > target) picked = v;
-      }
-    }
-    if (picked < 0) picked = last_pos;
-    if (picked < 0) picked = base_draw(b, u.u1);
-    return picked;
-  }
+  int picked = -1, last_pos = -1, E = INT_MIN;
   for (int pass = 0; pass < 2; ++pass) {
     for (int i = lo; i < hi; ++i) {
       const int r = rec[i];
@@ -619,6 +539,7 @@ __device__ int value_update(const ValParams &p, uint32_t iter, int64_t e, int a)
         }
         if (seen) continue;
         double G = 1.0;
+        int eg = 0;
         for (int j = i; j < hi; ++j) {
           const int rj = rec[j];
           const int xj = p.x[(int64_t)rj * p.A + a];
@@ -637,11 +558,29 @@ __device__ int value_update(const ValParams &p, uint32_t iter, int64_t e, int a)
             G = G * g;
           } else if (g_factor(p, at, a, rj, collapsed, v, g)) {
             G = G * g;
+          } else {
+            continue;
           }
+          if (SC && G > SC_UP) { G = G * SC_DN; ++eg; }
         }
-        const double W = base_prob(b, v) * (G - 1.0);  // GU:567 / 724
+        double W;
+        int ew = 0;
+        if (!SC) {
+          W = base_prob<RS>(b, v) * (G - 1.0);  // GU:567 / 724
+        } else {  // G - 1 == G at eg > 0: 2^-512 is below half an ulp of G >= 1
+          int eb;
+          W = base_weight_sc(at.probs, at.norm, at.is_const, b.k, v, eb) * (eg ? G : G - 1.0);
+          ew = eb + eg;
+          if (pass == 1) W = sc_down(W, ew - E);
+        }
         if (pass == 0) {
-          total += W;
+          if (!SC) {
+            total += W;
+          } else if (W > 0.0) {
+            if (E == INT_MIN) E = ew;
+            if (ew > E) { total = sc_down(total, E - ew); E = ew; }
+            total += sc_down(W, ew - E);
+          }
         } else {
           cum += W;
           if (W > 0.0) last_pos = v;
@@ -650,13 +589,143 @@ __device__ int value_update(const ValParams &p, uint32_t iter, int64_t e, int a)
       }
     }
     if (pass == 0) {
-      if (u.u0 < 1.0 / (1.0 + total)) return base_draw(b, u.u1);  // GU:593-594
+      if (!SC && !(total <= DBL_MAX)) return VALUE_FAR;
+      double mix = total;  // the plain total of the mixture test GU:593-594
+      if (SC && E != INT_MIN) {
+        int ez;
+        mix = total / base_z_sc(at.V, at.probs, at.norm, at.is_const, b.k, ez);
+        for (int d = E - ez; d > 0; --d) mix = mix * SC_UP;
+        mix = sc_down(mix, E - ez);
+      }
+      if (u.u0 < 1.0 / (1.0 + mix)) return base_draw<RS>(b, u.u1);  // GU:593-594
       target = u.u1 * total;
     }
   }
   if (picked < 0) picked = last_pos;
-  if (picked < 0) picked = base_draw(b, u.u1);
+  if (picked < 0) picked = base_draw<RS>(b, u.u1);
   return picked;
+}
+
+// new value of attribute a of entity e.  UB > 1: the loop over the similarity row of a single linked record fetches
+// UB candidates at a time (independent loads, same sums in the same order): for problems too small to fill the GPU
+// the kernel's time is the longest dependent-load chain of one thread, not throughput
+template <int UB>
+__device__ int value_update(const ValParams &p, uint32_t iter, int64_t e, int a) {
+  const AttrDev &at = p.attrs[a];
+  const bool collapsed = (p.sampler == DBL_PCG_I || p.sampler == DBL_PCG_II);
+  const U2 u = chain_uniform2(p.seed, p.cm.seeds, p.cm.ents, PH_VALUE, iter, e, (uint32_t)a);
+  const int lo = p.ent_rec_ptr[e], hi = p.ent_rec_ptr[e + 1];
+  const int *rec = p.rec_by_ent;
+
+  int k = 0;
+  for (int i = lo; i < hi; ++i) k += (p.x[(int64_t)rec[i] * p.A + a] >= 0);
+  BaseDist b;
+  if (k == 0) {  // GU:588-589
+    base_init<false>(b, at, 0);
+    return base_draw<false>(b, u.u1);
+  }
+  if (!collapsed) {
+    for (int i = lo; i < hi; ++i) {  // GU:619-630
+      const int r = rec[i];
+      const int xr = p.x[(int64_t)r * p.A + a];
+      if (xr >= 0 && !((p.zmask[r] >> a) & 1u)) return xr;
+    }
+    if (at.is_const) {  // GU:633-634
+      base_init<false>(b, at, 0);
+      return base_draw<false>(b, u.u1);
+    }
+  }
+  double total = 0.0, target = 0.0, cum = 0.0;
+  int picked = -1, last_pos = -1;
+  if (hi - lo == 1) {
+    base_init<false>(b, at, k);  // GU:584-586
+    // one linked record (most entities): the candidate values are the record's own similarity row, so the factors
+    // come straight from that row (no searches, no first-appearance check); same operations as the general path
+    const int r = rec[lo];
+    const int xr = p.x[(int64_t)r * p.A + a];  // observed (k == 1)
+    const int q0 = at.is_const ? 0 : at.rowptr[xr];
+    const int nv = at.is_const ? 1 : (at.rowptr[xr + 1] - q0);
+    double extra = 0.0;  // what the collapsed update adds to the factor of v == x (GU:553,557,560)
+    if (collapsed) {
+      const double th = p.theta[a * p.F + p.file[r]];
+      extra = at.is_const ? (1.0 / th - 1.0) / at.phi[xr] : (1.0 / th - 1.0) / (at.phi[xr] * at.norm[xr]);
+    }
+    auto weight = [&](int q, int &v) -> double {
+      double G = 1.0;
+      if (at.is_const) {
+        v = xr;
+        if (collapsed) G = G * (1.0 + extra);
+      } else {
+        v = at.col[q0 + q];
+        const double ex = at.expsim[q0 + q];
+        G = G * ((collapsed && v == xr) ? ex + extra : ex);
+      }
+      return base_prob<false>(b, v) * (G - 1.0);  // GU:567 / 724
+    };
+    if constexpr (UB > 1) {
+      // same weights, same order of the sums; the loads of UB consecutive candidates are issued together
+      auto batch = [&](int q, int (&v)[UB], double (&W)[UB]) {
+        double ex[UB], bp[UB];
+#pragma unroll
+        for (int i = 0; i < UB; ++i) {
+          const int qq = min(q + i, nv - 1);
+          v[i] = at.is_const ? xr : at.col[q0 + qq];
+          ex[i] = at.is_const ? 0.0 : at.expsim[q0 + qq];
+        }
+#pragma unroll
+        for (int i = 0; i < UB; ++i) bp[i] = base_prob<false>(b, v[i]);
+#pragma unroll
+        for (int i = 0; i < UB; ++i) {
+          double G = 1.0;
+          if (at.is_const) { if (collapsed) G = G * (1.0 + extra); }
+          else G = G * ((collapsed && v[i] == xr) ? ex[i] + extra : ex[i]);
+          W[i] = bp[i] * (G - 1.0);
+        }
+      };
+      for (int q = 0; q < nv; q += UB) {
+        int v[UB];
+        double W[UB];
+        batch(q, v, W);
+#pragma unroll
+        for (int i = 0; i < UB; ++i)
+          if (q + i < nv) total += W[i];
+      }
+      if (u.u0 < 1.0 / (1.0 + total)) return base_draw<false>(b, u.u1);  // GU:593-594
+      target = u.u1 * total;
+      for (int q = 0; q < nv && picked < 0; q += UB) {
+        int v[UB];
+        double W[UB];
+        batch(q, v, W);
+#pragma unroll
+        for (int i = 0; i < UB; ++i)
+          if (q + i < nv && picked < 0) {
+            cum += W[i];
+            if (W[i] > 0.0) last_pos = v[i];
+            if (cum > target) picked = v[i];
+          }
+      }
+    } else {
+      for (int q = 0; q < nv; ++q) {
+        int v;
+        total += weight(q, v);
+      }
+      if (u.u0 < 1.0 / (1.0 + total)) return base_draw<false>(b, u.u1);  // GU:593-594
+      target = u.u1 * total;
+      for (int q = 0; q < nv && picked < 0; ++q) {
+        int v;
+        const double W = weight(q, v);
+        cum += W;
+        if (W > 0.0) last_pos = v;
+        if (cum > target) picked = v;
+      }
+    }
+    if (picked < 0) picked = last_pos;
+    if (picked < 0) picked = base_draw<false>(b, u.u1);
+    return picked;
+  }
+  base_init<false>(b, at, k);  // GU:584-586
+  if (!b.pk && !(b.zk >= BASE_Z_MIN)) return VALUE_FAR;  // the uncached weights underflow: k_values_rescaled draws
+  return cluster_draw<false, false>(p, at, a, lo, hi, collapsed, b, u);  // VALUE_FAR: k_values_rescaled draws
 }
 
 template <int UB>
@@ -669,8 +738,37 @@ __global__ void __launch_bounds__(128) k_values(ValParams p) {
     const int64_t e = p.rows.row(t / p.A);
     if (e < 0) continue;
     const int a = (int)(t % p.A);
-    p.y[e * p.A + a] = value_update<UB>(p, iter, e, a);
+    const int v = value_update<UB>(p, iter, e, a);
+    if (v != VALUE_FAR) p.y[e * p.A + a] = v;
+    else p.far_list[atomicAdd(reinterpret_cast<unsigned long long *>(const_cast<long long *>(p.rows.ctl) + CTL_FAR), 1ull)] = e * p.A + a;
   }
+}
+// the draws k_values left because their weights leave the double range, as the oracle makes them: rescaled base
+// weights, then rescaled perturbation weights when the plain total still leaves the range.  A kernel of
+// its own: inlined into k_values the rare rescaled draw costs every common draw registers.  One CTA: usually there
+// are none, and the kernel reads the count, zeroes it and returns.
+__global__ void __launch_bounds__(128) k_values_rescaled(ValParams p) {
+  long long *cnt = const_cast<long long *>(p.rows.ctl) + CTL_FAR;
+  const int64_t n = *cnt;
+  if (!p.rows.dead()) {
+    const uint32_t iter = (uint32_t)(p.rows.ctl[CTL_ITER] + 1);
+    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+      const int64_t e = p.far_list[i] / p.A;
+      const int a = (int)(p.far_list[i] % p.A);
+      const AttrDev &at = p.attrs[a];
+      const U2 u = chain_uniform2(p.seed, p.cm.seeds, p.cm.ents, PH_VALUE, iter, e, (uint32_t)a);
+      const int lo = p.ent_rec_ptr[e], hi = p.ent_rec_ptr[e + 1];
+      int k = 0;
+      for (int j = lo; j < hi; ++j) k += (p.x[(int64_t)p.rec_by_ent[j] * p.A + a] >= 0);
+      const bool collapsed = (p.sampler == DBL_PCG_I || p.sampler == DBL_PCG_II);
+      BaseDist b;
+      base_init<true>(b, at, k);
+      const int v = cluster_draw<false, true>(p, at, a, lo, hi, collapsed, b, u);
+      p.y[e * p.A + a] = v != VALUE_FAR ? v : cluster_draw<true, true>(p, at, a, lo, hi, collapsed, b, u);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *cnt = 0;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1357,6 +1455,7 @@ struct dbl_ctx {
   DevBuf<unsigned char> inv_ids_in, inv_ids;
   bool inv_ids64 = false;
   DevBuf<int> inv_pos_in, inv_pos, inv_vptr, heavy_list;
+  DevBuf<long long> far_list;  // k_values -> k_values_rescaled
   InvDense inv_dense;
   bool inv_use_dense = false;  // inv_vptr holds the dense pointer table
   DevBuf<unsigned char> inv_tmp;
@@ -2465,10 +2564,13 @@ static int update_owned(dbl_ctx *ctx, int sampler) {
   vp.A = A; vp.F = F; vp.sampler = sampler; vp.seed = ctx->seed; vp.cm = ctx->chain_map(); vp.rows = rows_prefix(ctx, true);
   vp.attrs = ctx->attrs.p; vp.x = ctx->x.p; vp.file = ctx->file.p; vp.zmask = ctx->zmask.p; vp.theta = ctx->theta();
   vp.ent_rec_ptr = ctx->ent_rec_ptr.p; vp.rec_by_ent = ctx->rec_by_ent.p; vp.y = ctx->y.p;
+  if (ctx->far_list.n != (size_t)(ctx->E * A)) CUDA_TRY(ctx->far_list.alloc((size_t)(ctx->E * A)));
+  vp.far_list = ctx->far_list.p;
   // latency-bound sizes (the grid does not fill the GPU a few times over): the variant with batched loads
   if (ctx->E * A <= (int64_t)ctx->sm_count * 2048 * 4) k_values<8><<<grid_rows(ctx, ctx->E * A, 128), 128, 0, ctx->stream>>>(vp);
   else k_values<VALUES_UB_LARGE><<<grid_rows(ctx, ctx->E * A, 128), 128, 0, ctx->stream>>>(vp);
-  ctx->launches += 1;
+  k_values_rescaled<<<1, 128, 0, ctx->stream>>>(vp);
+  ctx->launches += 2;
   // (4) N(e), new block ids, distortions, partial summary
   return refresh_summary(ctx, true);
 }
@@ -2773,7 +2875,7 @@ extern "C" int dbl_set_rebalance(dbl_ctx *ctx, int32_t period, double threshold)
 static int preload_kernels(dbl_ctx *ctx) {
   cudaFuncAttributes fa;
 #define DBL_LOAD(k) CUDA_TRY(cudaFuncGetAttributes(&fa, k))
-  DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_entity_tiles); DBL_LOAD(k_values<VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
+  DBL_LOAD(k_theta); DBL_LOAD(k_link_heavy); DBL_LOAD(k_commit_link_keys); DBL_LOAD(k_build_entity_tiles); DBL_LOAD(k_values<VALUES_UB_LARGE>); DBL_LOAD(k_values<8>); DBL_LOAD(k_values_rescaled); DBL_LOAD(k_entity_post); DBL_LOAD(k_dist);
   DBL_LOAD(k_reduce_local); DBL_LOAD(k_finish); DBL_LOAD(k_move_ent); DBL_LOAD(k_move_rec); DBL_LOAD(k_publish_barrier);
   DBL_LOAD(k_unpack_ent); DBL_LOAD(k_unpack_rec); DBL_LOAD(k_reduce_peers); DBL_LOAD(k_lpt);
   DBL_LOAD(k_link_generic); DBL_LOAD(k_link_match); DBL_LOAD(k_link_pruned); DBL_LOAD(k_state_hash);

@@ -16,6 +16,7 @@
 #include <tuple>
 
 #include "dbl_internal.h"
+#include "dbl_scale.h"
 
 // ---------------------------------------------------------------------------------------------------
 // SimilarityFn.scala:61-98
@@ -192,27 +193,10 @@ void dbl_index::finish() {
         norm[v] = 1.0 / acc;
       }
     }
-    // base pmfs: weight_k(v) = probs(v) * norm(v)^k by k successive multiplications (DESIGN.md), normalised
-    // like DiscreteDist does (random/IndexNonUniformDiscreteDist.scala:66-88); cdf = running sum.
     pk.assign((size_t)(kmax + 1) * V, 0.0);
     cdf.assign((size_t)(kmax + 1) * V, 0.0);
-    for (int k = 0; k <= kmax; ++k) {
-      double *p = pk.data() + (size_t)k * V, *c = cdf.data() + (size_t)k * V;
-      double z = 0.0;
-      for (int v = 0; v < V; ++v) {
-        double w = probs[v];
-        if (!is_const)
-          for (int i = 0; i < k; ++i) w = w * norm[v];
-        p[v] = w;
-        z += w;
-      }
-      double run = 0.0;
-      for (int v = 0; v < V; ++v) {
-        p[v] = p[v] / z;
-        run += p[v];
-        c[v] = run;
-      }
-    }
+    for (int k = 0; k <= kmax; ++k)
+      base_row(V, probs.data(), norm.data(), is_const, k, pk.data() + (size_t)k * V, cdf.data() + (size_t)k * V);
   }
   phi.assign(pk.begin(), pk.begin() + V);
   logphi.resize(V);
@@ -506,6 +490,17 @@ extern "C" int dbl_index_tables(const dbl_index *ix, double *phi, double *norm, 
   if (rowptr) std::copy(ix->rowptr.begin(), ix->rowptr.end(), rowptr);
   if (col) std::copy(ix->col.begin(), ix->col.end(), col);
   if (expsim) std::copy(ix->expsim.begin(), ix->expsim.end(), expsim);
+  return DBL_OK;
+}
+extern "C" int dbl_index_base_tables(const dbl_index *ix, int32_t *kmax, double *invnorm, double *logphi,
+                                     double *lognorm, double *pk, double *cdf) {
+  if (!ix) return DBL_ERR_INVALID;
+  if (kmax) *kmax = ix->kmax;
+  if (invnorm) std::copy(ix->invnorm.begin(), ix->invnorm.end(), invnorm);
+  if (logphi) std::copy(ix->logphi.begin(), ix->logphi.end(), logphi);
+  if (lognorm) std::copy(ix->lognorm.begin(), ix->lognorm.end(), lognorm);
+  if (pk) std::copy(ix->pk.begin(), ix->pk.end(), pk);
+  if (cdf) std::copy(ix->cdf.begin(), ix->cdf.end(), cdf);
   return DBL_OK;
 }
 extern "C" double dbl_index_exp_sim(const dbl_index *ix, int32_t v1, int32_t v2) {

@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "dbl_internal.h"
+#include "dbl_scale.h"
 
 namespace {
 constexpr int MAXL = 64;        // longest string the bit-parallel kernel takes (one 64-bit word per column)
@@ -182,26 +183,12 @@ __global__ void k_sim_norms(int V, const double *__restrict__ probs, const int *
 }
 
 // getSimNormDist (AttributeIndex.scala:197-216): B_k(v) = probs(v) n(v)^k / Z_k for k = 0..kmax, and the running sums
-// the inverse-cdf draws use; sequential sums as on the host, one k per thread
+// the inverse-cdf draws use; sequential sums as on the host (base_row), one k per thread
 __global__ void k_base_pmfs(int V, int kmax, int is_const, const double *__restrict__ probs,
                             const double *__restrict__ norm, double *__restrict__ pk, double *__restrict__ cdf) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k > kmax) return;
-  double *p = pk + (size_t)k * V, *c = cdf + (size_t)k * V;
-  double z = 0.0;
-  for (int v = 0; v < V; ++v) {
-    double w = probs[v];
-    if (!is_const)
-      for (int i = 0; i < k; ++i) w = w * norm[v];
-    p[v] = w;
-    z += w;
-  }
-  double run = 0.0;
-  for (int v = 0; v < V; ++v) {
-    p[v] = p[v] / z;
-    run += p[v];
-    c[v] = run;
-  }
+  base_row(V, probs, norm, is_const != 0, k, pk + (size_t)k * V, cdf + (size_t)k * V);
 }
 
 struct Dev {

@@ -111,9 +111,18 @@ class AttributeIndex:
         rowptr = np.zeros(V + 1, np.int32)
         col = np.zeros(max(nnz, 1), np.int32)
         es = np.zeros(max(nnz, 1))
-        _check(_lib.load().dbl_index_tables(self._h, _p(phi, _lib.f64p), _p(norm, _lib.f64p), _p(rowptr, _lib.i32p),
-                                            _p(col, _lib.i32p), _p(es, _lib.f64p)), "AttributeIndex.tables")
-        return {"phi": phi, "norm": norm, "rowptr": rowptr, "col": col[:nnz], "expsim": es[:nnz]}
+        L = _lib.load()
+        _check(L.dbl_index_tables(self._h, _p(phi, _lib.f64p), _p(norm, _lib.f64p), _p(rowptr, _lib.i32p),
+                                    _p(col, _lib.i32p), _p(es, _lib.f64p)), "AttributeIndex.tables")
+        kmax = C.c_int32(0)
+        _check(L.dbl_index_base_tables(self._h, C.byref(kmax), None, None, None, None, None), "AttributeIndex.tables")
+        invnorm, logphi, lognorm = np.zeros(V), np.zeros(V), np.zeros(V)
+        pk, cdf = np.zeros((kmax.value + 1, V)), np.zeros((kmax.value + 1, V))
+        _check(L.dbl_index_base_tables(self._h, None, _p(invnorm, _lib.f64p), _p(logphi, _lib.f64p),
+                                       _p(lognorm, _lib.f64p), _p(pk, _lib.f64p), _p(cdf, _lib.f64p)),
+               "AttributeIndex.tables")
+        return {"phi": phi, "norm": norm, "rowptr": rowptr, "col": col[:nnz], "expsim": es[:nnz], "invnorm": invnorm,
+                "logphi": logphi, "lognorm": lognorm, "pk": pk, "cdf": cdf}
 
     @property
     def slot_codes(self):

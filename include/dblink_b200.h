@@ -82,6 +82,10 @@ const char *dbl_index_value(const dbl_index *, int32_t value_id);
 /* copies of the tables (arrays sized num_values, num_values+1, nnz, nnz); any pointer may be NULL */
 int dbl_index_tables(const dbl_index *, double *phi /*probabilityOf*/, double *norm /*simNormalizationOf*/,
                      int32_t *rowptr, int32_t *col, double *expsim /*simValuesOf*/);
+/* the derived tables: *kmax, then invnorm = 1/n(v), logphi, lognorm (num_values each) and the cached base pmfs pk and
+ * their running sums cdf ((kmax+1) x num_values, row k = B_k); any pointer may be NULL */
+int dbl_index_base_tables(const dbl_index *, int32_t *kmax, double *invnorm, double *logphi, double *lognorm, double *pk,
+                          double *cdf);
 double dbl_index_exp_sim(const dbl_index *, int32_t v1, int32_t v2); /* expSimOf; NaN when out of range        */
 /* SimilarityFn.getSimilarity (SimilarityFn.scala:65-70, 84-96); similarity as in dbl_index_build (2 = Jaro-Winkler
  * unit similarity under the same truncation); NaN for an unknown similarity, and for similarity 1 when a or b is not

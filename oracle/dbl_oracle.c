@@ -12,6 +12,8 @@
 #include "dbl_oracle.h"
 #include "dbl_oracle_priv.h"
 
+#include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <pthread.h>
 #include <stdio.h>
@@ -166,6 +168,45 @@ double orc_lev_similarity(const char *a, const char *b, double threshold, double
 typedef struct { const char *s; double w; } sw_pair;
 static int cmp_sw(const void *a, const void *b) { return strcmp(((const sw_pair *)a)->s, ((const sw_pair *)b)->s); }
 
+/* Exact power-of-two rescaling (DESIGN.md section 4.7).  A weight that may leave the double range is carried as
+   w * 2^(512 e): w stays normal and every step is one of the protocol's roundings or an exact scaling, so while the
+   plain arithmetic stays normal both give the same bits. */
+#define SC_UP 0x1p512
+#define SC_DN 0x1p-512
+#define BASE_Z_MIN 0x1p-969 /* DBL_MIN * 2^53: a base row whose plain Z_k falls below it is built rescaled */
+
+/* probs(v) n(v)^k as w * 2^(512 e): the k multiplications of the plain weight, w brought back above 2^-512 after
+   each (n(v) > 2^-510 keeps the product normal) */
+static double base_weight_sc(const orc_index *ix, int k, int v, int *e) {
+  double w = ix->probs[v];
+  int ex = 0;
+  if (!ix->is_const)
+    for (int i = 0; i < k; ++i) {
+      w = w * ix->norm[v];
+      if (w < SC_DN) { w = w * SC_UP; --ex; }
+    }
+  *e = ex;
+  return w;
+}
+/* w * 2^(512 d) for d <= 0 */
+static double sc_down(double w, int d) {
+  for (; d < 0 && w != 0.0; ++d) w = w * SC_DN;
+  return w;
+}
+/* Z_k = sum_v probs(v) n(v)^k as z * 2^(512 ez): id order, the sum kept at the scale of the largest weight so far */
+static double base_z_sc(const orc_index *ix, int k, int *ez) {
+  int E;
+  double z = base_weight_sc(ix, k, 0, &E);
+  for (int v = 1; v < ix->V; ++v) {
+    int e;
+    const double w = base_weight_sc(ix, k, v, &e);
+    if (e > E) { z = sc_down(z, E - e); E = e; }
+    z += sc_down(w, e - E);
+  }
+  *ez = E;
+  return z;
+}
+
 static void index_finish(orc_index *ix) {
   int V = ix->V;
   /* norms: AttributeIndex.scala:234-245 (uses `probs`, not the renormalised distribution) */
@@ -197,6 +238,15 @@ static void index_finish(orc_index *ix) {
         for (int i = 0; i < k; ++i) w = w * ix->norm[v];
       pk[v] = w;
       z += w;
+    }
+    if (!(z >= BASE_Z_MIN)) { /* the weights underflow: the same row from the rescaled weights */
+      int E;
+      z = base_z_sc(ix, k, &E);
+      for (int v = 0; v < V; ++v) {
+        int e;
+        const double w = base_weight_sc(ix, k, v, &e);
+        pk[v] = sc_down(w, e - E);
+      }
     }
     double c = 0.0;
     for (int v = 0; v < V; ++v) {
@@ -1084,7 +1134,7 @@ void orc_link_weights(const orc_state *s, int64_t r, int sampler, const int32_t 
 
 /* base pmf entry and cdf for power k (getSimNormDist, AttributeIndex.scala:197-206); beyond kmax the
    table is evaluated on the fly with the same arithmetic as index_finish */
-typedef struct { const orc_index *ix; int k; double zk; const double *pk, *cdf; } base_dist;
+typedef struct { const orc_index *ix; int k, sc, ez; double zk; const double *pk, *cdf; } base_dist;
 
 static double base_weight(const orc_index *ix, int k, int v) {
   double w = ix->probs[v];
@@ -1095,19 +1145,29 @@ static void base_init(base_dist *b, const orc_index *ix, int k) {
   b->ix = ix;
   if (ix->is_const) k = 0;
   b->k = k;
+  b->sc = 0;
   if (k <= ix->kmax) { b->pk = ix->pk + (size_t)k * ix->V; b->cdf = ix->cdf + (size_t)k * ix->V; b->zk = 0.0; }
   else {
     b->pk = NULL; b->cdf = NULL;
     double z = 0.0;
     for (int v = 0; v < ix->V; ++v) z += base_weight(ix, k, v);
+    b->sc = !(z >= BASE_Z_MIN); /* as index_finish: the weights underflow, rescale them */
+    if (b->sc) z = base_z_sc(ix, k, &b->ez);
     b->zk = z;
   }
 }
-static double base_prob(const base_dist *b, int v) { return b->pk ? b->pk[v] : base_weight(b->ix, b->k, v) / b->zk; }
+/* uncached weight of v at the scale of zk */
+static double base_w(const base_dist *b, int v) {
+  if (!b->sc) return base_weight(b->ix, b->k, v);
+  int e;
+  const double w = base_weight_sc(b->ix, b->k, v, &e);
+  return sc_down(w, e - b->ez);
+}
+static double base_prob(const base_dist *b, int v) { return b->pk ? b->pk[v] : base_w(b, v) / b->zk; }
 static int base_draw(const base_dist *b, double u) {
   if (b->cdf) return orc_invcdf(b->cdf, b->ix->V, u);
   double c = 0.0;
-  for (int v = 0; v < b->ix->V; ++v) { c += base_weight(b->ix, b->k, v) / b->zk; if (c > u) return v; }
+  for (int v = 0; v < b->ix->V; ++v) { c += base_w(b, v) / b->zk; if (c > u) return v; }
   return b->ix->V - 1;
 }
 
@@ -1170,8 +1230,12 @@ static int value_draw(const orc_state *s, const int64_t *lrec, int64_t nl, int a
     if (ix->is_const) { base_init(&b, ix, 0); result = base_draw(&b, u1); free(obs); return result; } /* GU:633-634 */
   }
   base_init(&b, ix, (int)k); /* GU:584-586 */
+  /* Plain weights W(v) = B_k(v) (G(v) - 1).  When their total leaves the double range (G overflows for clusters of
+     about 709 / ln g agreeing records, and 0 * inf is NaN where B_k(v) underflowed as well), pass 0 is redone with every weight carried
+     as W * 2^(512 e) (DESIGN.md section 4.7): t(v) = B_k(v) Z_k (G(v) - 1) and the walk in units of the largest
+     scale E; Z_k only enters the mixture test. */
   double total = 0.0;
-  int picked = -1, last_pos = -1;
+  int picked = -1, last_pos = -1, sc = 0, E = INT_MIN;
   double target = 0.0, cum = 0.0;
   for (int pass = 0; pass < 2; ++pass) {
     for (int64_t i = 0; i < k; ++i) {
@@ -1183,11 +1247,31 @@ static int value_draw(const orc_state *s, const int64_t *lrec, int64_t nl, int a
         int seen = 0;
         for (int64_t j = 0; j < i && !seen; ++j) seen = in_support(s, obs[j], a, v);
         if (seen) continue;
-        double G = 1.0;
-        for (int64_t j = i; j < k; ++j) { double g; if (g_factor(s, obs[j], a, collapsed, v, &g)) G = G * g; }
-        double W = base_prob(&b, v) * (G - 1.0); /* GU:567 / 724 */
-        if (pass == 0) total += W;
-        else {
+        double G = 1.0, W;
+        int eg = 0, ew = 0;
+        for (int64_t j = i; j < k; ++j) {
+          double g;
+          if (g_factor(s, obs[j], a, collapsed, v, &g)) {
+            G = G * g;
+            if (sc && G > SC_UP) { G = G * SC_DN; ++eg; }
+          }
+        }
+        if (!sc) {
+          W = base_prob(&b, v) * (G - 1.0); /* GU:567 / 724 */
+        } else { /* G - 1 == G at eg > 0: 2^-512 is below half an ulp of G >= 1 */
+          int eb;
+          W = base_weight_sc(ix, b.k, v, &eb) * (eg ? G : G - 1.0);
+          ew = eb + eg;
+          if (pass == 1) W = sc_down(W, ew - E);
+        }
+        if (pass == 0) {
+          if (!sc) total += W;
+          else if (W > 0.0) {
+            if (E == INT_MIN) E = ew;
+            if (ew > E) { total = sc_down(total, E - ew); E = ew; }
+            total += sc_down(W, ew - E);
+          }
+        } else {
           cum += W;
           if (W > 0.0) last_pos = v;
           if (picked < 0 && cum > target) picked = v;
@@ -1195,7 +1279,15 @@ static int value_draw(const orc_state *s, const int64_t *lrec, int64_t nl, int a
       }
     }
     if (pass == 0) {
-      if (u0 < 1.0 / (1.0 + total)) { result = base_draw(&b, u1); free(obs); return result; } /* GU:593-594 */
+      if (!sc && !(total <= DBL_MAX)) { sc = 1; total = 0.0; pass = -1; continue; }
+      double mix = total; /* the plain total of the mixture test GU:593-594 */
+      if (sc && E != INT_MIN) {
+        int ez;
+        mix = total / base_z_sc(ix, b.k, &ez);
+        for (int d = E - ez; d > 0; --d) mix = mix * SC_UP;
+        mix = sc_down(mix, E - ez);
+      }
+      if (u0 < 1.0 / (1.0 + mix)) { result = base_draw(&b, u1); free(obs); return result; } /* GU:593-594 */
       target = u1 * total;
     }
   }
@@ -1214,7 +1306,8 @@ int orc_value_draw(const orc_state *s, int64_t e, int a, int sampler, double u0,
 }
 
 /* literal full-domain conditional for distribution tests.  PCG-*: p(v) ~ B_k(v) prod_r g_r(v), i.e. the
-   mixture of GU:593-597 written out; Gibbs: GU:619-643; Gibbs-Sequential: GU:661-695. */
+   mixture of GU:593-597 written out; Gibbs: GU:619-643; Gibbs-Sequential: GU:661-695.  Summed in logarithms and
+   normalised through the largest term, so clusters whose B_k underflows or whose prod g overflows stay exact. */
 void orc_ref_value_pmf(const orc_state *s, int64_t e, int a, int sampler, double *pmf) {
   const orc_model *m = s->m;
   const orc_index *ix = m->idx[a];
@@ -1227,23 +1320,25 @@ void orc_ref_value_pmf(const orc_state *s, int64_t e, int a, int sampler, double
   for (int64_t i = 0; i < nl; ++i) if (s->x[rec[ptr[e] + i] * A + a] >= 0) obs[k++] = rec[ptr[e] + i];
   int forced = -1;
   if (!collapsed) for (int64_t i = 0; i < k && forced < 0; ++i) if (!s->z[obs[i] * A + a]) forced = s->x[obs[i] * A + a];
-  double z = 0.0;
+  double top = -INFINITY, z = 0.0;
   for (int v = 0; v < V; ++v) {
-    double p;
-    if (forced >= 0) p = (v == forced) ? 1.0 : 0.0;
-    else if (k == 0 || (!collapsed && ix->is_const)) p = ix->phi[v];
+    double lp;
+    if (forced >= 0) lp = (v == forced) ? 0.0 : -INFINITY;
+    else if (k == 0 || (!collapsed && ix->is_const)) lp = log(ix->phi[v]);
     else if (sampler == ORC_GIBBS_SEQ) {
-      p = ix->phi[v];
+      lp = log(ix->phi[v]);
       for (int64_t i = 0; i < k; ++i) { /* GU:689 */
         int32_t xr = s->x[obs[i] * A + a];
-        p *= orc_index_exp_sim_of(ix, xr, v) * ix->norm[v] * ix->phi[xr];
+        lp += log(orc_index_exp_sim_of(ix, xr, v)) + log(ix->norm[v]) + log(ix->phi[xr]);
       }
     } else {
-      p = ix->probs[v] * (ix->is_const ? 1.0 : pow(ix->norm[v], (double)k));
-      for (int64_t i = 0; i < k; ++i) { double g; if (g_factor(s, obs[i], a, collapsed, v, &g)) p *= g; }
+      lp = log(ix->probs[v]) + (ix->is_const ? 0.0 : (double)k * log(ix->norm[v]));
+      for (int64_t i = 0; i < k; ++i) { double g; if (g_factor(s, obs[i], a, collapsed, v, &g)) lp += log(g); }
     }
-    pmf[v] = p; z += p;
+    pmf[v] = lp;
+    if (lp > top) top = lp;
   }
+  for (int v = 0; v < V; ++v) { pmf[v] = exp(pmf[v] - top); z += pmf[v]; }
   for (int v = 0; v < V; ++v) pmf[v] /= z;
   free(obs); free(ptr); free(rec);
 }

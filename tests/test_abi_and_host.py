@@ -130,8 +130,10 @@ def test_records_cache_and_index_match_oracle(oracle):
     oi = oracle_indexes(oracle, g)
     for a in range(rc.num_attributes):
         t = rc.indexes[a].tables()
-        for k in ("phi", "norm", "rowptr", "col", "expsim"):
+        for k in ("phi", "norm", "rowptr", "col", "expsim", "invnorm", "pk", "cdf"):
             np.testing.assert_array_equal(t[k], getattr(oi[a], k))
+        np.testing.assert_allclose(t["logphi"], np.log(oi[a].phi), rtol=1e-15, atol=1e-300)
+        np.testing.assert_allclose(t["lognorm"], np.log(oi[a].norm), rtol=1e-15, atol=1e-300)
     x, file = rc.transform_records(g["values"], g["files"])
     assert x.shape == (1500, 4) and set(np.unique(file)) == {0, 1}
     assert rc.num_records == 1500 and sum(rc.file_sizes) == 1500
