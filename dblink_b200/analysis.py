@@ -6,6 +6,8 @@
   binder_search                                           <- single-record moves that lower the expected Binder loss
   vi_clusters                                             <- the sample of least posterior expected variation of
                                                              information
+  vi_search                                               <- single-record moves that lower the quantised expected
+                                                             variation of information
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
   pairwise_metrics                                        <- analysis/PairwiseMetrics.scala:44-63,
                                                              BinaryClassificationMetrics.scala:23-37
@@ -194,6 +196,76 @@ def vi_clusters(chain):
     return best, clusters[best], losses
 
 
+def vi_search(chain, starts, max_rounds=1000, records=None):
+    """Single-record moves from each start (a partition: clusters of ids) while they lower J_q, by the definition:
+    J_q(c) = S sum over clusters X of F_q(|X|) - 2 sum over the samples s and the non-empty cells x ^ y (x of c, y of
+    C_s) of F_q(|x ^ y|), F_q(n) = D_q[0] + ... + D_q[n - 1] with D_q = analysis_arrays.vi_search_table(R), in exact
+    integers.  `records` orders the record ids (a record's index is its position; default: sorted).  One round: every
+    record takes its best move to ANY other cluster or, out of a cluster of two or more, to a singleton -- the least
+    (change of J_q, destination), the change recomputed from scratch as J_q(after) - J_q(before), a singleton counting
+    as destination -1 and a cluster as its smallest record index -- and proposes it if it lowers J_q; a proposal is
+    applied if it is the least (change, record index) among the proposals touching each cluster it touches.  Returns
+    (position of the chosen start: least final J_q, ties to the earlier; per start a dict with the final clusters as
+    frozensets, rounds = [(moves, clusters after the round, change of J_q)], converged, J0 and J)."""
+    from .analysis_arrays import vi_search_table
+
+    S = len(chain)
+    samples = [list(clusters_of_sample(s)) for s in chain]
+    ids = sorted({r for cl in samples for c in cl for r in c}) if records is None else list(records)
+    index = {r: k for k, r in enumerate(ids)}
+    F = [0]
+    for d in vi_search_table(len(ids)).tolist():
+        F.append(F[-1] + d)
+
+    def J(parts):
+        total = S * sum(F[len(x)] for x in parts)
+        for cl in samples:
+            total -= 2 * sum(F[len(x & y)] for x in parts for y in cl if x & y)
+        return total
+
+    runs = []
+    for start in starts:
+        parts = {frozenset(c) for c in start}
+        rounds, converged, J0 = [], False, J(parts)
+        while True:
+            label = {c: min(index[r] for r in c) for c in parts}
+            base = J(parts)
+            proposals = []
+            for i in ids:
+                A = next(c for c in parts if i in c)
+                dests = [(label[X], X) for X in parts if X != A] + ([(-1, None)] if len(A) > 1 else [])
+                best = None
+                for dest, X in dests:
+                    moved = (parts - {A, X}) | ({A - {i}} if len(A) > 1 else set()) | {(X or frozenset()) | {i}}
+                    change = J(moved) - base
+                    if best is None or (change, dest) < best[:2]:
+                        best = (change, dest, X)
+                if best is not None and best[0] < 0:
+                    proposals.append((best[0], index[i], i, A, best[2]))
+            if not proposals:
+                converged = True
+                break
+            if len(rounds) == max_rounds:
+                break
+            least = {}
+            for change, k, i, A, X in proposals:
+                for c in (A, X) if X is not None else (A,):
+                    least[c] = min(least.get(c, (change, k)), (change, k))
+            new = set(parts)
+            applied = 0
+            for change, k, i, A, X in proposals:
+                if all(least[c] == (change, k) for c in ((A, X) if X is not None else (A,))):
+                    applied += 1
+                    new -= {A, X}
+                    if len(A) > 1:
+                        new.add(A - {i})
+                    new.add((X or frozenset()) | {i})
+            parts = new
+            rounds.append((applied, len(parts), J(parts) - base))
+        runs.append(dict(clusters=parts, rounds=rounds, converged=converged, J0=J0, J=J(parts)))
+    return min(range(len(runs)), key=lambda k: (runs[k]["J"], k)), runs
+
+
 def cluster_size_distribution(chain):
     """iteration -> {cluster size: count} (LinkageChain.scala:137-154)."""
     out = {}
@@ -333,6 +405,29 @@ def format_vi_cluster(ari, iteration, chain, expected_vi):
     """The vi-cluster section: ari = adjusted Rand index of the sample chosen at (iteration, chain)."""
     return ("=====================================\n         VI cluster metrics\n"
             "-------------------------------------\n" + _vi_estimate_line(iteration, chain, expected_vi)
+            + f" Adj. Rand index: {ari}\n=====================================\n")
+
+
+def _vi_search_lines(start, rounds, converged, exact):
+    return (f" Estimate:        search from the {start} start, {rounds} rounds, "
+            f"{'converged' if converged else 'not converged'}\n"
+            f" Expected VI:     vi-sample start {exact[0]!r}, smpc start {exact[1]!r}, from vi-sample {exact[2]!r}, "
+            f"from smpc {exact[3]!r}\n")
+
+
+def format_vi_search_pairwise(m, start, rounds, converged, exact):
+    """The vi-search-pairwise section: m = pairwise metrics of the search result chosen from `start`; exact = the
+    expected VI of the two starts and the two results (project.vi_search_estimate)."""
+    return ("=====================================\n     VI search pairwise metrics\n"
+            "-------------------------------------\n" + _vi_search_lines(start, rounds, converged, exact)
+            + f" Precision:      {m['precision']}\n Recall:         {m['recall']}\n F1-score:       {m['f1score']}\n"
+            "=====================================\n")
+
+
+def format_vi_search_cluster(ari, start, rounds, converged, exact):
+    """The vi-search-cluster section: ari = adjusted Rand index of the search result chosen from `start`."""
+    return ("=====================================\n      VI search cluster metrics\n"
+            "-------------------------------------\n" + _vi_search_lines(start, rounds, converged, exact)
             + f" Adj. Rand index: {ari}\n=====================================\n")
 
 

@@ -405,7 +405,7 @@ def search_rounds(num_records, first, second, count, num_samples, start, a, b, m
     if np.shape(start) != (R,):
         raise ValueError("a start needs one cluster label per record")
     lab = canonical_labels(np.asarray(start, np.int64))
-    aS, big = a * S, np.iinfo(np.int64).max
+    aS = a * S
     moves, dn, dK, converged = [], [], [], False
     while True:
         size = np.bincount(lab, minlength=R).astype(np.int64)
@@ -438,24 +438,32 @@ def search_rounds(num_records, first, second, count, num_samples, start, a, b, m
             break
         if len(moves) == max_rounds:
             break
-        i, X, dJ = c_rec[best], c_dest[best], c_dJ[best]
-        A, to = lab[i], X >= 0
-        touched, t_dJ, t_i = np.r_[A, X[to]], np.r_[dJ, dJ[to]], np.r_[i, i[to]]
-        claim_dJ = np.full(R, big, np.int64)
-        np.minimum.at(claim_dJ, touched, t_dJ)
-        least = t_dJ == claim_dJ[touched]
-        claim_i = np.full(R, big, np.int64)
-        np.minimum.at(claim_i, touched[least], t_i[least])
-        win = (claim_dJ[A] == dJ) & (claim_i[A] == i)
-        win[to] &= (claim_dJ[X[to]] == dJ[to]) & (claim_i[X[to]] == i[to])
-        key = lab.copy()
-        key[i[win]] = np.where(to[win], X[win], R + i[win])
+        win, lab = claim_moves(lab, c_rec[best], c_dest[best], c_dJ[best])
         moves.append(int(win.sum()))
         dn.append(int(c_dn[best][win].sum()))
         dK.append(int(c_dK[best][win].sum()))
-        lab = canonical_labels(key)
     n, K = search_result_counts(first, second, count, lab)
     return SearchRun(lab, moves, dn, dK, converged, n, K)
+
+
+def claim_moves(lab, i, X, dJ):
+    """One round's claims, shared by both searches: records i propose moving from their clusters lab[i] to X (-1: a
+    new singleton) with changes dJ < 0.  A proposal wins if it holds the least (dJ, i) among the proposals touching each
+    cluster it touches (its source, and its destination unless a singleton).  Returns (win mask, the canonical labels
+    after the winning moves)."""
+    R, big = len(lab), np.iinfo(np.int64).max
+    A, to = lab[i], X >= 0
+    touched, t_dJ, t_i = np.r_[A, X[to]], np.r_[dJ, dJ[to]], np.r_[i, i[to]]
+    claim_dJ = np.full(R, big, np.int64)
+    np.minimum.at(claim_dJ, touched, t_dJ)
+    least = t_dJ == claim_dJ[touched]
+    claim_i = np.full(R, big, np.int64)
+    np.minimum.at(claim_i, touched[least], t_i[least])
+    win = (claim_dJ[A] == dJ) & (claim_i[A] == i)
+    win[to] &= (claim_dJ[X[to]] == dJ[to]) & (claim_i[X[to]] == i[to])
+    key = lab.copy()
+    key[i[win]] = np.where(to[win], X[win], R + i[win])
+    return win, canonical_labels(key)
 
 
 def search_choice(runs, num_samples, a, b):
@@ -530,16 +538,41 @@ def vi_losses(g, G, num_records):
     (int64[S, width] each): E_t = fsum over n >= 2 of float(D_t[n]) (n log2 n), divided by R S.  fsum is correctly
     rounded and does not depend on the order, so equal integers give equal losses."""
     g, G = np.asarray(g, np.int64), np.asarray(G, np.int64)
-    S, width = G.shape
-    if num_records == 0:
-        return np.zeros(S)
-    D = (S - 2) * g + g.sum(axis=0) - 2 * G
-    weight = np.array([0.0, 0.0] + [n * math.log2(n) for n in range(2, width)])[:width]
-    out = np.zeros(S)
-    for t in range(S):
-        nz = np.flatnonzero(D[t])
-        out[t] = math.fsum(D[t, nz].astype(np.float64) * weight[nz]) / (num_records * S)
-    return out
+    S = G.shape[0]
+    g_sum = g.sum(axis=0)
+    # against every sample including itself, sample t has G[t] + g[t] cells of each size (C_t ^ C_t = C_t)
+    return np.array([vi_label_loss(g[t], G[t] + g[t], g_sum, S, num_records) for t in range(S)], np.float64)
+
+
+def vi_label_loss(g_c, G_c, g_sum, num_samples, num_records):
+    """The posterior expected VI of a labelling c against S samples, from integer histograms indexed by size n: g_c[n] =
+    the clusters of n records of c, G_c[n] = the cells of n >= 2 records of c ^ C_s summed over every sample s, g_sum[n]
+    = the clusters of n records summed over the samples.  D[n] = S g_c[n] + g_sum[n] - 2 G_c[n], E = fsum over n >= 2 of
+    float(D[n]) (n log2 n), divided by R S.  fsum is correctly rounded and does not depend on the order, so equal
+    integers give equal losses."""
+    S, R = int(num_samples), int(num_records)
+    if R == 0 or S == 0:
+        return 0.0
+    width = max(len(g_c), len(G_c), len(g_sum))
+    pad = lambda x: np.pad(np.asarray(x, np.int64), (0, width - len(x)))  # noqa: E731
+    D = S * pad(g_c) + pad(g_sum) - 2 * pad(G_c)
+    D[:2] = 0
+    nz = np.flatnonzero(D)
+    return math.fsum(D[nz].astype(np.float64) * np.array([n * math.log2(n) for n in nz.tolist()])) / (R * S)
+
+
+def vi_label_cells(chain, labels, width):
+    """G, int64[width]: the cells of n >= 2 records of labels ^ C_s summed over the samples s of the chain (width at
+    least M + 1, M = the largest cluster of any sample, as every cell lies inside one)."""
+    R = chain.num_records
+    labels = np.asarray(labels, np.int64)
+    G = np.zeros(int(width), np.int64)
+    for mem, off, _ in chain.samples:
+        lab_s = sample_labels(R, mem, off)
+        big = np.flatnonzero(np.bincount(lab_s, minlength=R)[lab_s] >= 2)
+        _, n = np.unique(lab_s[big] * R + labels[big], return_counts=True)
+        G += np.bincount(n[n >= 2], minlength=width)[:width]
+    return G
 
 
 def vi_estimate(losses):
@@ -547,6 +580,224 @@ def vi_estimate(losses):
     if len(losses) == 0:
         raise ValueError("the VI estimate needs at least one sample")
     return min(range(len(losses)), key=lambda s: (losses[s], s))
+
+
+# ---- the VI search: parallel single-record moves ----------------------------------------------------------------
+# With f(n) = n log2 n, A(x) = sum over the blocks of x of f(|block|) and samples C_1 .. C_S, R S E[VI](c) = S A(c) +
+# sum_s A(C_s) - 2 sum_s A(c ^ C_s).  The search works on the quantised table D_q[m] = round(2^Q (f(m + 1) - f(m))),
+# m = 0 .. R - 1, with F_q(n) = D_q[0] + ... + D_q[n - 1] in place of f, and lowers
+#   J_q(c) = S sum over clusters X of F_q(|X|) - 2 sum_s sum over the cells of c ^ C_s of F_q(n).
+# Moving record i from A (|A| = a) to B (|B| = beta; a new singleton is beta = 0) changes J_q by exactly
+#   dJ = S (D_q[beta] - D_q[a - 1]) - 2 (w_B - w_A),  w_B = sum_s D_q[|B ^ C_s(i)|],  w_A = sum_s D_q[|A ^ C_s(i)| - 1].
+# D_q[0] = 0 and D_q is non-decreasing, so a cluster sharing no sample cluster with i is never better than the
+# singleton: the candidates are the clusters of the records that share a sample cluster with i and, when a > 1, a
+# singleton; only samples where i is in a cluster of two or more add to w.  Moves that touch disjoint clusters of c
+# touch disjoint cells of every c ^ C_s, so the claims of the Binder search (claim_moves) apply unchanged, their dJ add
+# exactly and J_q falls every round.  The quantised expected VI E_q(c) = (J_q(c) + sum_s A_q(C_s)) / (2^Q R S) is
+# within 2^(1-Q) bits of E[VI](c): each F_q(n) is off f(n) 2^Q by at most n / 2.
+VI_SEARCH_BITS = 20             # Q
+MAX_VI_SEARCH_SQUARES = 1 << 28  # a sample's sum over its clusters of |K|^2: bounds its contributions to one round
+VI_SEARCH_STARTS = ("vi-sample", "smpc")
+
+
+def vi_search_table(num_records):
+    """D_q, int64[R]: round(2^Q (f(m + 1) - f(m))) for m = 0 .. R - 1, f(m + 1) - f(m) = log2(m + 1) + m log2(1 + 1/m)
+    evaluated without cancellation, halves rounded up."""
+    R = int(num_records)
+    d = np.zeros(R)
+    m = np.arange(1, R, dtype=np.float64)
+    d[1:] = np.log2(m + 1) + m * np.log1p(1.0 / m) / math.log(2)
+    return np.floor(d * float(1 << VI_SEARCH_BITS) + 0.5).astype(np.int64)
+
+
+def check_vi_search_size(num_samples, num_records):
+    """S R (ceil(log2 R) + 2) 2^(Q+2) < 2^63 keeps every dJ, round sum, J_q and sum_s A_q(C_s) inside int64."""
+    S, R = int(num_samples), int(num_records)
+    if S * R * ((max(R, 1) - 1).bit_length() + 2) << (VI_SEARCH_BITS + 2) >= 1 << 63:
+        raise ValueError(f"the VI search needs samples x records x (ceil(log2 records) + 2) x 2^22 < 2^63 "
+                         f"(here {S} x {R})")
+
+
+def check_vi_search_squares(squares):
+    """squares[s] = sum over the clusters of sample s of |K|^2; ValueError past MAX_VI_SEARCH_SQUARES."""
+    for s, q in enumerate(squares):
+        if int(q) > MAX_VI_SEARCH_SQUARES:
+            raise ValueError(f"the VI search refuses sample {s}: its clusters' squared sizes sum to {int(q)}, more "
+                             f"than {MAX_VI_SEARCH_SQUARES}")
+
+
+def vi_sample_squares(chain):
+    """int64[S]: per sample the sum over its clusters of |K|^2."""
+    return np.array([int((np.diff(off).astype(np.int64) ** 2).sum()) for _, off, _ in chain.samples], np.int64)
+
+
+def vi_search_prefix(table):
+    """F_q, int64[R + 1]: F_q(n) = D_q[0] + ... + D_q[n - 1]."""
+    return np.r_[0, np.cumsum(np.asarray(table, np.int64))].astype(np.int64)
+
+
+def vi_sample_sum(chain, table):
+    """sum over the samples and their clusters K of F_q(|K|): the J_q-independent part of R S 2^Q E_q."""
+    F = vi_search_prefix(table)
+    return sum(int(F[np.diff(off)].sum()) for _, off, _ in chain.samples)
+
+
+class VISearchRun:
+    """One VI search: labels int64[R] (canonical) where it stopped; per round the moves applied, the clusters after it
+    and the change of J_q, int64[rounds]; whether it stopped because no record proposed a move; J_q of the start."""
+
+    def __init__(self, labels, moves, clusters, dJ, converged, J0):
+        self.labels, self.converged, self.J0 = labels, bool(converged), int(J0)
+        self.moves, self.clusters, self.dJ = (np.asarray(x, np.int64) for x in (moves, clusters, dJ))
+
+    @property
+    def rounds(self):
+        return len(self.moves)
+
+    @property
+    def J(self):
+        return self.J0 + int(self.dJ.sum())
+
+    def objectives(self):
+        """[J_q of the start (round 0), then after every round], Python ints."""
+        return [self.J0 + int(x) for x in np.r_[0, np.cumsum(self.dJ)]]
+
+
+def vi_search_losses(objectives, sample_sum, num_samples, num_records):
+    """E_q = (J_q + sum_s A_q(C_s)) / (2^Q R S) for each J_q: one correctly rounded division of integers."""
+    den = (int(num_records) * int(num_samples)) << VI_SEARCH_BITS
+    return [(int(J) + int(sample_sum)) / den for J in objectives]
+
+
+def _vi_contributions(R, lab_s, big, lab, table):
+    """One sample's contributions to w: for each record i in a cluster K of two or more of the sample and each cell
+    (K, B) of m records, (i R + B, D_q[m]), or D_q[m - 1] for i's own cell; and the sum of F_q over the cells is left to
+    the caller through the cell sizes.  Returns (keys, values, cell sizes)."""
+    if not len(big):
+        return (np.zeros(0, np.int64),) * 3
+    key = lab_s[big] * R + lab[big]
+    order = np.argsort(key, kind="stable")
+    ks, rec = key[order], big[order]
+    cs = _run_starts(ks)
+    cn = np.diff(np.r_[cs, len(ks)])
+    cK, cB = ks[cs] // R, ks[cs] % R
+    ks_K = _run_starts(cK)                                # first cell of each sample cluster
+    nK = np.diff(np.r_[ks_K, len(cs)])                    # its number of cells
+    kidx = np.repeat(np.repeat(np.arange(len(ks_K)), nK), cn)  # per sorted record, its sample cluster
+    cnt = nK[kidx]
+    total = int(cnt.sum())
+    first = np.repeat(np.cumsum(cnt) - cnt, cnt)
+    j = np.arange(total) - first + np.repeat(ks_K[kidx], cnt)
+    i = np.repeat(rec, cnt)
+    B, m = cB[j], cn[j]
+    return i * R + B, table[m - (B == lab[i])], cn
+
+
+def vi_search_rounds(num_records, sample_labels_list, table, start, max_rounds):
+    """The VI search from labels start[R] against the samples (a list of int64 labels[R], one per sample) with the
+    table D_q: a VISearchRun."""
+    R, S = int(num_records), len(sample_labels_list)
+    table = np.asarray(table, np.int64)
+    if table.shape != (R,):
+        raise ValueError("the VI search table needs one entry per record")
+    if np.shape(start) != (R,):
+        raise ValueError("a start needs one cluster label per record")
+    F = vi_search_prefix(table)
+    bigs = [np.flatnonzero(np.bincount(ls, minlength=R)[ls] >= 2) for ls in sample_labels_list]
+    lab = canonical_labels(np.asarray(start, np.int64))
+    moves, clusters, dJs, converged, J0 = [], [], [], False, None
+    while True:
+        size = np.bincount(lab, minlength=R).astype(np.int64)
+        keys, vals, cell_F = [], [], 0
+        for ls, big in zip(sample_labels_list, bigs):
+            k, v, cn = _vi_contributions(R, ls, big, lab, table)
+            keys.append(k)
+            vals.append(v)
+            cell_F += int(F[cn].sum())
+        if J0 is None:
+            J0 = S * int(F[size].sum()) - 2 * cell_F
+        keys = np.concatenate(keys) if keys else np.zeros(0, np.int64)
+        vals = np.concatenate(vals) if vals else np.zeros(0, np.int64)
+        order = np.argsort(keys, kind="stable")
+        keys = keys[order]
+        runs = _run_starts(keys)
+        keys, w = keys[runs], np.add.reduceat(vals[order], runs) if len(runs) else np.zeros(0, np.int64)
+        rec, X = keys // R, keys % R
+        own = X == lab[rec]
+        wA = np.zeros(R, np.int64)
+        wA[rec[own]] = w[own]
+        a = size[lab]
+        dA = table[a - 1]
+        # candidates in ascending (record, destination) order: a record's singleton first, then its clusters
+        multi = np.flatnonzero(a > 1)
+        by = np.argsort(np.r_[2 * multi, 2 * rec[~own] + 1], kind="stable")
+        c_rec = np.r_[multi, rec[~own]][by]
+        c_dest = np.r_[np.full(len(multi), -1, np.int64), X[~own]][by]
+        r_o, x_o = rec[~own], X[~own]
+        c_dJ = np.r_[-S * dA[multi] + 2 * wA[multi],
+                     S * (table[size[x_o]] - dA[r_o]) - 2 * (w[~own] - wA[r_o])][by]
+        seg = _run_starts(c_rec)
+        least = np.repeat(np.minimum.reduceat(c_dJ, seg), np.diff(np.r_[seg, len(c_rec)])) if len(seg) else c_dJ
+        at = np.flatnonzero(c_dJ == least)
+        best = at[_run_starts(c_rec[at])]
+        best = best[c_dJ[best] < 0]
+        if not len(best):
+            converged = True
+            break
+        if len(moves) == max_rounds:
+            break
+        win, lab = claim_moves(lab, c_rec[best], c_dest[best], c_dJ[best])
+        moves.append(int(win.sum()))
+        clusters.append(int(len(np.unique(lab))))
+        dJs.append(int(c_dJ[best][win].sum()))
+    return VISearchRun(lab, moves, clusters, dJs, converged, J0)
+
+
+def vi_search_choice(runs):
+    """The position of the run of least final J_q, ties going to the earlier start."""
+    return min(range(len(runs)), key=lambda k: (runs[k].J, k))
+
+
+class VISamples:
+    """The held samples of a chain on the host, with the methods of analysis_gpu.VI: cross (the cell histograms of
+    every pair of samples), search (the VI search) and score (the cells of a labelling with every sample)."""
+
+    def __init__(self, chain):
+        self.chain = chain
+        self.num_records, self.num_samples = chain.num_records, len(chain.samples)
+        self._labels = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        pass
+
+    def labels(self):
+        if self._labels is None:
+            self._labels = [sample_labels(self.num_records, mem, off) for mem, off, _ in self.chain.samples]
+        return self._labels
+
+    def cross(self, width):
+        G = vi_cross_histograms(self.chain)
+        return np.pad(G, ((0, 0), (0, int(width) - G.shape[1])))
+
+    def search(self, table, start, max_rounds):
+        return vi_search_rounds(self.num_records, self.labels(), table, start, max_rounds)
+
+    def score(self, labels, width):
+        return vi_label_cells(self.chain, labels, width)
+
+
+def vi_search(chain, starts, max_rounds=1000):
+    """The VI search from each of starts (labels[R] each) against the chain's samples: (the position of the chosen run,
+    the VISearchRuns).  ValueError before any work for the size bound or a sample past the squares cap."""
+    R, S = chain.num_records, len(chain.samples)
+    check_vi_search_size(S, R)
+    check_vi_search_squares(vi_sample_squares(chain))
+    vi = VISamples(chain)
+    runs = [vi.search(vi_search_table(R), st, max_rounds) for st in starts]
+    return vi_search_choice(runs), runs
 
 
 def labels_to_clusters(labels, record_ids=None):

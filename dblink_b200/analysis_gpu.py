@@ -13,15 +13,18 @@ exactly: every sample goes into one pairs table, then every sample is scored aga
 (single-record moves from a start) equals analysis_arrays.binder_search exactly, in labels, round logs, n and K: the
 rule is in integers, and the device applies it to the same table.  The cell histograms of the variation-of-information
 estimate equal analysis_arrays.vi_cross_histograms exactly: they are integers, counted on the device from radix-sorted
-(sample, label, label) keys of every pair of held samples.
+(sample, label, label) keys of every pair of held samples.  The VI search (single-record moves on a quantised table)
+and the cells of any labelling with every held sample equal analysis_arrays.vi_search_rounds / vi_label_cells exactly,
+on the same handle.
 """
 import ctypes as C
 
 import numpy as np
 
 from . import _lib
-from .analysis_arrays import (MAX_PAIRS, SearchRun, check_search_size, search_choice, search_cost,
-                              too_many_pairs, vi_width)
+from .analysis_arrays import (MAX_PAIRS, SearchRun, VISearchRun, check_search_size, check_vi_search_size,
+                              check_vi_search_squares, search_choice, search_cost, too_many_pairs, vi_sample_squares,
+                              vi_search_choice, vi_search_table, vi_width)
 from .engine import DblinkError
 
 _STATUS = {_lib.ERR_INVALID: "invalid argument (bad size, label out of range, too many samples or pairs)",
@@ -269,6 +272,58 @@ class VI(_Handle):
         G = np.empty((self.num_samples, int(width)), np.int64)
         self._call("cross", self._h, int(width), G.ctypes.data)
         return G
+
+    def score(self, labels, width):
+        """G, int64[width]: the cells of n >= 2 records of labels ^ C_s summed over the held samples s."""
+        labels = np.ascontiguousarray(labels, np.int32)
+        if labels.shape != (self.num_records,):
+            raise ValueError("a labelling needs one cluster label per record")
+        G = np.empty(int(width), np.int64)
+        self._call("score", self._h, labels.ctypes.data, int(width), G.ctypes.data)
+        return G
+
+    def search(self, table, start, max_rounds):
+        """The VI search from labels start[R] with the table D_q (analysis_arrays.vi_search_table): an
+        analysis_arrays.VISearchRun.  The held samples do not change."""
+        table = np.ascontiguousarray(table, np.int64)
+        start = np.ascontiguousarray(start, np.int32)
+        if table.shape != (self.num_records,):
+            raise ValueError("the VI search table needs one entry per record")
+        if start.shape != (self.num_records,):
+            raise ValueError("a start needs one cluster label per record")
+        max_rounds = int(max_rounds)
+        labels = np.empty(self.num_records, np.int32)
+        logs = [np.zeros(max(max_rounds, 0), np.int64) for _ in range(3)]
+        rounds, converged, J0 = C.c_int32(), C.c_int32(), C.c_int64()
+        self._call("search", self._h, table.ctypes.data_as(_lib.i64p), start.ctypes.data, max_rounds,
+                   labels.ctypes.data, C.byref(rounds), C.byref(converged), *(x.ctypes.data_as(_lib.i64p) for x in logs),
+                   C.byref(J0))
+        return VISearchRun(labels.astype(np.int64), *(x[:rounds.value] for x in logs), converged.value, J0.value)
+
+
+def vi_samples(chain, batch_keys=None):
+    """A VI handle holding every sample of a ChainArrays (R > 0 and S > 0), with the methods of
+    analysis_arrays.VISamples."""
+    vi = VI(chain.num_records, len(chain.samples))
+    try:
+        if batch_keys is not None:
+            vi.set_batch_keys(batch_keys)
+        _add_chain(vi, chain)
+    except BaseException:
+        vi.close()
+        raise
+    return vi
+
+
+def vi_search(chain, starts, max_rounds=1000, batch_keys=None):
+    """(chosen position, VISearchRuns), identical to analysis_arrays.vi_search(chain, starts, max_rounds), refusals
+    included: every sample is added to one handle, then the search runs from each start on it."""
+    R, S = chain.num_records, len(chain.samples)
+    check_vi_search_size(S, R)
+    check_vi_search_squares(vi_sample_squares(chain))
+    with vi_samples(chain, batch_keys) as vi:
+        runs = [vi.search(vi_search_table(R), st, max_rounds) for st in starts]
+    return vi_search_choice(runs), runs
 
 
 def vi_cross_histograms(chain, batch_keys=None):

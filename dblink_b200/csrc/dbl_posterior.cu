@@ -28,12 +28,17 @@
 // every sample t and cell size n >= 2, the number of cells of n records in C_t ^ C_s summed over the other samples s,
 // in int64 -- the integers the posterior expected variation of information is made of.  Cells are runs of radix-sorted
 // (s, label in C_t, label in C_s) keys over the records in C_t's clusters of two or more -- see dbl_vi_cross.
+// On the same handle, the VI search (dbl_vi_search, same numbers as analysis_arrays.vi_search_rounds) and the cells of
+// any labelling with every held sample (dbl_vi_score, as analysis_arrays.vi_label_cells) share one cell pass over
+// radix-sorted (s, label in C_s, label in c) keys -- see vi_cell_batches.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <climits>
 #include <cstdint>
 #include <cub/cub.cuh>
+#include <new>
+#include <vector>
 
 #include "dbl_internal.h"
 
@@ -160,6 +165,18 @@ struct Buf {
     const cudaError_t e = nb.alloc(std::max(need, std::min(limit, cap > SIZE_MAX / 2 ? SIZE_MAX : 2 * cap)));
     if (e != cudaSuccess) return e;
     std::swap(p, nb.p);  // nb now frees the old buffer
+    std::swap(cap, nb.cap);
+    return cudaSuccess;
+  }
+  // reserve() that keeps the first `keep` bytes: copied on st, synchronised before the old buffer is freed
+  cudaError_t reserve_keep(size_t need, size_t keep, cudaStream_t st) {
+    if (need <= cap) return cudaSuccess;
+    Buf nb;
+    cudaError_t e = nb.alloc(std::max(need, cap > SIZE_MAX / 2 ? SIZE_MAX : 2 * cap));
+    if (e == cudaSuccess && keep) e = cudaMemcpyAsync(nb.p, p, keep, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && keep) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return e;
+    std::swap(p, nb.p);
     std::swap(cap, nb.cap);
     return cudaSuccess;
   }
@@ -822,13 +839,14 @@ __global__ void k_claim_record(int64_t R, const int32_t *__restrict__ lab, const
 
 // A proposal that holds the claim of every cluster it touches moves its record: the record's group key becomes its
 // destination's label, or R + r for a singleton (a key no cluster has); every other record keeps its label.  The
-// round's moves, sum of dn = |X| - |A| + 1 and sum of dK go to stats[0..2], summed exactly in uint64.
+// round's moves, sum of dn = |X| - |A| + 1 and sum of the proposals' int64 payloads (the Binder search's dK, the VI
+// search's dJ) go to stats[0..2], summed exactly in uint64.
 __global__ void k_apply_moves(int64_t R, const int32_t *__restrict__ lab, const int32_t *__restrict__ size,
                               const long long *__restrict__ prop_dJ, const int32_t *__restrict__ prop_dest,
-                              const long long *__restrict__ prop_dK, const long long *__restrict__ claim_dJ,
+                              const long long *__restrict__ payload, const long long *__restrict__ claim_dJ,
                               const unsigned int *__restrict__ claim_i, unsigned long long *__restrict__ gkey,
                               unsigned long long *__restrict__ stats) {
-  unsigned long long moves = 0, dn = 0, dK = 0;
+  unsigned long long moves = 0, dn = 0, sum = 0;
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x) {
     const int32_t A = lab[r];
     unsigned long long k = (uint32_t)A;
@@ -841,19 +859,30 @@ __global__ void k_apply_moves(int64_t R, const int32_t *__restrict__ lab, const 
         k = X >= 0 ? (unsigned long long)X : (unsigned long long)(R + r);
         ++moves;
         dn += (unsigned long long)((X >= 0 ? (long long)size[X] : 0ll) - size[A] + 1);
-        dK += (unsigned long long)prop_dK[r];
+        sum += (unsigned long long)payload[r];
       }
     }
     gkey[r] = k;
   }
   moves = warp_sum_u64(moves);
   dn = warp_sum_u64(dn);
-  dK = warp_sum_u64(dK);
+  sum = warp_sum_u64(sum);
   if ((threadIdx.x & 31) == 0) {
     atomicAdd(&stats[0], moves);
     atomicAdd(&stats[1], dn);
-    atomicAdd(&stats[2], dK);
+    atomicAdd(&stats[2], sum);
   }
+}
+
+// The labels after a round's moves: records grouped by their group key gkey (gbits bits), each labelled by its group's
+// smallest record index into L.  gkey_s, rec_s, head and start are R entries of scratch each; tmp grows as the sort
+// and scan need.
+int canonical_relabel(int64_t R, int gbits, const unsigned long long *gkey, const int32_t *iota,
+                      unsigned long long *gkey_s, int32_t *rec_s, int32_t *head, int32_t *start, int32_t *L, Buf &tmp,
+                      cudaStream_t st) {
+  const int rc = group_by_key(R, gbits, gkey, iota, gkey_s, rec_s, head, start, tmp, st);
+  if (rc == DBL_OK) k_scatter_labels<<<grid_for(R), THREADS, 0, st>>>(R, rec_s, start, L);
+  return rc;
 }
 
 // n = sum over clusters of C(size, 2), K = the counts of the held pairs whose records share a label: out[0], out[1]
@@ -928,12 +957,9 @@ extern "C" int dbl_pairs_binder_search(dbl_pairs *p, int64_t a, int64_t b, const
 
   // the labels of gkey, grouped; each record labelled by its group's smallest record index
   auto relabel = [&]() {
-    const int rc = group_by_key(R, gbits, gkey.as<unsigned long long>(), p->iota.as<int32_t>(),
-                                gkey_s.as<unsigned long long>(), p->rec_s.as<int32_t>(), p->head.as<int32_t>(),
-                                p->start.as<int32_t>(), p->tmp, st);
-    if (rc == DBL_OK)
-      k_scatter_labels<<<grid_for(R), THREADS, 0, st>>>(R, p->rec_s.as<int32_t>(), p->start.as<int32_t>(), L);
-    return rc;
+    return canonical_relabel(R, gbits, gkey.as<unsigned long long>(), p->iota.as<int32_t>(),
+                             gkey_s.as<unsigned long long>(), p->rec_s.as<int32_t>(), p->head.as<int32_t>(),
+                             p->start.as<int32_t>(), L, p->tmp, st);
   };
   auto sizes = [&]() {
     POST_TRY(cudaMemsetAsync(Z, 0, r4, st));
@@ -1207,13 +1233,39 @@ __global__ void k_vi_cells(int64_t n, int hi_shift, const unsigned long long *__
 }
 }  // namespace
 
+namespace {
+// out[0] = the sum over the clusters of a sample of |K|^2 (= sum over records of their cluster's size), out[1] = its
+// records in clusters of two or more (the keys it gives a cell pass)
+__global__ void k_sample_stats(int64_t R, const int32_t *__restrict__ lab, const int32_t *__restrict__ size,
+                               unsigned long long *__restrict__ out) {
+  unsigned long long q = 0, big = 0;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t k = size[lab[r]];
+    q += (unsigned long long)k;
+    big += k >= 2;
+  }
+  q = warp_sum_u64(q);
+  big = warp_sum_u64(big);
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&out[0], q);
+    atomicAdd(&out[1], big);
+  }
+}
+
+struct SampleStats {
+  int64_t squares;  // sum over the sample's clusters of |K|^2: bounds its contributions to a round of the VI search
+  int64_t keys;     // its records in clusters of two or more: its keys in a cell pass
+};
+}  // namespace
+
 struct dbl_vi : Handle {
   int32_t max_samples = 0;
   int lab_bits = 1;                       // bits of a label in [0, R)
   int32_t max_size = 0;                   // M, the largest cluster of any held sample
   int64_t batch_keys = PAIR_BLOCK;        // keys of one batch of samples s (at least the selected records of one)
   Buf rows;                               // [max_samples][R] held labels
-  Buf size, peak;                         // cluster sizes of one sample; its largest (int32)
+  Buf size, peak, sq;                     // cluster sizes of one sample; its largest (int32); its SampleStats
+  std::vector<SampleStats> stats;         // per held sample
 };
 
 extern "C" int dbl_vi_create(dbl_vi **out, int64_t num_records, int32_t max_samples) {
@@ -1226,7 +1278,7 @@ extern "C" int dbl_vi_create(dbl_vi **out, int64_t num_records, int32_t max_samp
     p->lab_bits = bits_for(R);
     const size_t r4 = sizeof(int32_t) * (size_t)R;
     if (p->rows.alloc(r4 * (size_t)max_samples) != cudaSuccess || p->size.alloc(r4) != cudaSuccess ||
-        p->peak.alloc(sizeof(int32_t)) != cudaSuccess)
+        p->peak.alloc(sizeof(int32_t)) != cudaSuccess || p->sq.alloc(2 * sizeof(unsigned long long)) != cudaSuccess)
       return DBL_ERR_CUDA;  // the held label matrix does not fit
     return DBL_OK;
   });
@@ -1242,7 +1294,8 @@ extern "C" int dbl_vi_set_batch_keys(dbl_vi *p, int64_t max_keys) {
   return DBL_OK;
 }
 
-// One sample: check the labels; its largest cluster; append it as row S.  S and M move only on success.
+// One sample: check the labels; its largest cluster, its sum of squared cluster sizes and its records in clusters of two
+// or more; append it as row S.  S, M and the per-sample counts move only on success.
 extern "C" int dbl_vi_add_sample(dbl_vi *p, const int32_t *cluster) {
   if (!p || !cluster || p->S >= p->max_samples) return DBL_ERR_INVALID;
   DeviceScope ds(p->device);
@@ -1252,14 +1305,23 @@ extern "C" int dbl_vi_add_sample(dbl_vi *p, const int32_t *cluster) {
   int32_t *Z = p->size.as<int32_t>();
   POST_TRY(cudaMemsetAsync(Z, 0, sizeof(int32_t) * R, st));
   POST_TRY(cudaMemsetAsync(p->peak.p, 0, sizeof(int32_t), st));
+  POST_TRY(cudaMemsetAsync(p->sq.p, 0, 2 * sizeof(unsigned long long), st));
   k_label_sizes<<<grid_for(R), THREADS, 0, st>>>(R, p->cluster.as<int32_t>(), Z);
   k_max_size<<<grid_for(R), THREADS, 0, st>>>(R, Z, p->peak.as<int32_t>());
+  k_sample_stats<<<grid_for(R), THREADS, 0, st>>>(R, p->cluster.as<int32_t>(), Z, p->sq.as<unsigned long long>());
   POST_TRY(cudaMemcpyAsync(p->rows.as<int32_t>() + (size_t)p->S * R, p->cluster.p, sizeof(int32_t) * R,
                            cudaMemcpyDeviceToDevice, st));
   int32_t m = 0;
+  unsigned long long q[2] = {0, 0};
   POST_TRY(cudaMemcpyAsync(&m, p->peak.p, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaMemcpyAsync(q, p->sq.p, sizeof(q), cudaMemcpyDeviceToHost, st));
   POST_TRY(cudaGetLastError());
   POST_TRY(cudaStreamSynchronize(st));
+  try {
+    p->stats.push_back({(int64_t)q[0], (int64_t)q[1]});
+  } catch (const std::bad_alloc &) {
+    return DBL_ERR_CUDA;  // nothing has moved
+  }
   p->max_size = std::max(p->max_size, m);
   ++p->S;
   return DBL_OK;
@@ -1338,5 +1400,463 @@ extern "C" int dbl_vi_cross(dbl_vi *p, int64_t width, int64_t *G_out) {
   POST_TRY(cudaMemcpyAsync(G_out, G.p, gbytes, cudaMemcpyDefault, st));
   POST_TRY(cudaGetLastError());
   POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
+// ---- the VI search and the expected VI of any labelling: cells of c ^ C_s over every held sample --------------------
+namespace {
+constexpr int64_t VI_MAX_SQUARES = int64_t(1) << 28;  // a sample's sum over clusters of |K|^2 the search accepts
+
+// one key per selected record r of sample s0 + sl: sl << 2 lab_bits | label in C_s << lab_bits | label in c, with r
+__global__ void k_vis_keys(int64_t nsel, const int32_t *__restrict__ sel, const int32_t *__restrict__ lab_s,
+                           const int32_t *__restrict__ L, int32_t sl, int lab_bits, unsigned long long *__restrict__ key,
+                           int32_t *__restrict__ rec) {
+  const unsigned long long hi = (unsigned long long)sl << (2 * lab_bits);
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < nsel; k += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t r = sel[k];
+    key[k] = hi | (unsigned long long)(uint32_t)lab_s[r] << lab_bits | (uint32_t)L[r];
+    rec[k] = r;
+  }
+}
+
+__global__ void k_cell_heads(int64_t n, const unsigned long long *__restrict__ key, int32_t *__restrict__ head) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    head[i] = i == 0 || key[i] != key[i - 1];
+}
+
+// cell c (0-based, in sorted order) starts at cpos[c]; cpos[number of cells] = n
+__global__ void k_cell_pos(int64_t n, const int32_t *__restrict__ head, const int32_t *__restrict__ crank,
+                           int32_t *__restrict__ cpos) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    if (head[i]) cpos[crank[i] - 1] = (int32_t)i;
+    if (i == n - 1) cpos[crank[i]] = (int32_t)n;
+  }
+}
+
+// cells of n >= 2 records counted into G[n] (n < width, as every cell is inside a cluster of at most M records)
+__global__ void k_cell_hist(int64_t ncell, const int32_t *__restrict__ cpos, unsigned long long *__restrict__ G) {
+  for (int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; c < ncell; c += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t m = cpos[c + 1] - cpos[c];
+    if (m >= 2) atomicAdd(&G[m], 1ull);
+  }
+}
+
+// sum over cells of F_q(n) into *out
+__global__ void k_cell_F(int64_t ncell, const int32_t *__restrict__ cpos, const long long *__restrict__ F,
+                         unsigned long long *__restrict__ out) {
+  unsigned long long acc = 0;
+  for (int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; c < ncell; c += (int64_t)gridDim.x * blockDim.x)
+    acc += (unsigned long long)F[cpos[c + 1] - cpos[c]];
+  acc = warp_sum_u64(acc);
+  if ((threadIdx.x & 31) == 0 && acc) atomicAdd(out, acc);
+}
+
+// sum over clusters of F_q(|X|), and the number of clusters: out[0], out[1]
+__global__ void k_size_stats(int64_t R, const int32_t *__restrict__ size, const long long *__restrict__ F,
+                             unsigned long long *__restrict__ out) {
+  unsigned long long f = 0, k = 0;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x) {
+    f += (unsigned long long)F[size[r]];
+    k += size[r] > 0;
+  }
+  f = warp_sum_u64(f);
+  k = warp_sum_u64(k);
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&out[0], f);
+    atomicAdd(&out[1], k);
+  }
+}
+
+// the cells of the sample cluster K holding sorted position i: [first cell, its number of cells)
+__device__ __forceinline__ void cluster_cells(const unsigned long long *__restrict__ key, int64_t n, int lab_bits,
+                                              const int32_t *__restrict__ crank, int64_t i, int32_t *first,
+                                              int32_t *count) {
+  const unsigned long long K = key[i] >> lab_bits;
+  const int64_t lo = lower_bound_u64(key, n, K << lab_bits), hi = lower_bound_u64(key, n, (K + 1) << lab_bits);
+  *first = crank[lo] - 1;
+  *count = crank[hi - 1] - crank[lo] + 1;
+}
+
+// per sorted position, the number of cells of its sample cluster (its contributions); entry n is 0
+__global__ void k_vis_count(int64_t n, int lab_bits, const unsigned long long *__restrict__ key,
+                            const int32_t *__restrict__ crank, long long *__restrict__ cnt) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= n; i += (int64_t)gridDim.x * blockDim.x) {
+    int32_t first = 0, count = 0;
+    if (i < n) cluster_cells(key, n, lab_bits, crank, i, &first, &count);
+    cnt[i] = count;
+  }
+}
+
+// One warp per sorted position (record i, in sample cluster K) writes, at its int64 offset, one contribution per cell
+// (K, B) of m records: key i << lab_bits | B, value D_q[m] for B != c(i), D_q[m - 1] for i's own cell.
+__global__ void k_vis_emit(int64_t n, int lab_bits, const unsigned long long *__restrict__ key,
+                           const int32_t *__restrict__ rec, const int32_t *__restrict__ crank,
+                           const int32_t *__restrict__ cpos, const long long *__restrict__ off,
+                           const int32_t *__restrict__ L, const long long *__restrict__ Dq,
+                           unsigned long long *__restrict__ ckey, long long *__restrict__ cval) {
+  const int lane = threadIdx.x & 31;
+  const unsigned long long mask = (1ull << lab_bits) - 1;
+  const int64_t nwarps = (int64_t)gridDim.x * WARPS_PER_BLOCK;
+  for (int64_t w = blockIdx.x * (int64_t)WARPS_PER_BLOCK + (threadIdx.x >> 5); w < n; w += nwarps) {
+    int32_t first = 0, count = 0;
+    cluster_cells(key, n, lab_bits, crank, w, &first, &count);
+    const int32_t i = rec[w];
+    const unsigned long long A = (uint32_t)L[i], hi = (unsigned long long)(uint32_t)i << lab_bits;
+    const long long o = off[w];
+    for (int32_t j = lane; j < count; j += 32) {
+      const int32_t s = cpos[first + j], m = cpos[first + j + 1] - s;
+      const unsigned long long B = key[s] & mask;
+      ckey[o + j] = hi | B;
+      cval[o + j] = Dq[B == A ? m - 1 : m];
+    }
+  }
+}
+
+// One record per thread over its segment of the reduced (record << lab_bits | cluster, w) table: w_A of its own
+// cluster A, then per cluster B (ascending) dJ = S (D_q[|B|] - D_q[a - 1]) - 2 (w_B - w_A); the singleton (a > 1) is
+// dJ = -S D_q[a - 1] + 2 w_A and is tried first as destination -1, so a strict < keeps the least (dJ, destination).
+// A record with dJ < 0 proposes its move and claims its source and destination with atomicMin on dJ.
+__global__ void k_vis_best_move(int64_t R, int lab_bits, int64_t n, const unsigned long long *__restrict__ key,
+                                const long long *__restrict__ w, const int32_t *__restrict__ lab,
+                                const int32_t *__restrict__ size, const long long *__restrict__ Dq, long long S,
+                                long long *__restrict__ prop_dJ, int32_t *__restrict__ prop_dest,
+                                long long *__restrict__ claim_dJ, unsigned long long *__restrict__ num_props) {
+  const unsigned long long mask = (1ull << lab_bits) - 1;
+  unsigned long long props = 0;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t lo = lower_bound_u64(key, n, (unsigned long long)r << lab_bits);
+    const int64_t hi = lower_bound_u64(key, n, (unsigned long long)(r + 1) << lab_bits);
+    const int32_t A = lab[r];
+    const long long a = size[A], dA = Dq[a - 1];
+    long long wA = 0;
+    for (int64_t k = lo; k < hi; ++k)
+      if ((key[k] & mask) == (unsigned long long)A) wA = w[k];
+    long long best = NO_MOVE;
+    int32_t dest = INT_MAX;
+    if (a > 1) {
+      best = -S * dA + 2 * wA;
+      dest = -1;
+    }
+    for (int64_t k = lo; k < hi; ++k) {
+      const unsigned long long X = key[k] & mask;
+      if (X == (unsigned long long)A) continue;
+      const long long dJ = S * (Dq[size[X]] - dA) - 2 * (w[k] - wA);
+      if (dJ < best) {
+        best = dJ;
+        dest = (int32_t)X;
+      }
+    }
+    const bool propose = best < 0;
+    prop_dJ[r] = propose ? best : NO_MOVE;
+    prop_dest[r] = dest;
+    if (propose) {
+      atomicMin(&claim_dJ[A], best);
+      if (dest >= 0) atomicMin(&claim_dJ[dest], best);
+      ++props;
+    }
+  }
+  props = warp_sum_u64(props);
+  if ((threadIdx.x & 31) == 0 && props) atomicAdd(num_props, props);
+}
+
+// The cells of a labelling L (int32 [R], device, labels in [0, R)) with every held sample, batch by batch.  Each sample
+// has a weight, its keys (the score) or its sum of |K|^2 (the search, which bounds its contributions); a batch takes
+// samples while their weights stay within max(batch_keys, that of its first sample), their keys within INT32_MAX and
+// its key bits within 63.  Per sample the records in its clusters of two or more (flags, an exclusive scan, a scatter)
+// give one key each (k_vis_keys), so the key buffers hold the batch's keys and no more; the batch's (key, record) pairs
+// are radix-sorted, and the cells are their runs of equal keys: cell ranks (an inclusive scan of the heads) and cell
+// starts.  on_batch(n, ncell) sees the sorted keys in key.Current(), their records in rec.Current(), the ranks in
+// crank and the starts in cpos.
+struct CellPass {
+  Buf key[2], rec[2], head, crank, cpos, flag, pos, sel, tmp;
+  cub::DoubleBuffer<unsigned long long> kb;
+  cub::DoubleBuffer<int32_t> rb;
+};
+
+template <class OnBatch>
+int vi_cell_batches(dbl_vi *p, const int32_t *L, int64_t SampleStats::*weight, CellPass &c, OnBatch on_batch) {
+  const int64_t R = p->R;
+  const int32_t S = p->S;
+  const int b = p->lab_bits;
+  cudaStream_t st = p->stream;
+  const int32_t *rows = p->rows.as<int32_t>();
+  int32_t *Z = p->size.as<int32_t>();
+  POST_TRY(c.flag.reserve(sizeof(int32_t) * (size_t)(R + 1)));
+  POST_TRY(c.pos.reserve(sizeof(int32_t) * (size_t)(R + 1)));
+  POST_TRY(c.sel.reserve(sizeof(int32_t) * (size_t)R));
+  size_t tb_scan = 0;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb_scan, (const int32_t *)nullptr, (int32_t *)nullptr, R + 1, st));
+  for (int32_t s0 = 0; s0 < S;) {
+    const std::vector<SampleStats> &ss = p->stats;
+    const int64_t limit = std::max(p->batch_keys, ss[s0].*weight);
+    int32_t s1 = s0 + 1;
+    int64_t w = ss[s0].*weight, keys = ss[s0].keys;  // keys <= R <= INT32_MAX
+    while (s1 < S && w + ss[s1].*weight <= limit && keys + ss[s1].keys <= INT32_MAX &&
+           2 * b + bits_for((int64_t)s1 - s0 + 1) <= 63) {
+      w += ss[s1].*weight;
+      keys += ss[s1++].keys;
+    }
+    const int32_t B = s1 - s0;
+    POST_TRY(c.key[0].reserve(sizeof(unsigned long long) * (size_t)keys));
+    POST_TRY(c.key[1].reserve(sizeof(unsigned long long) * (size_t)keys));
+    POST_TRY(c.rec[0].reserve(sizeof(int32_t) * (size_t)keys));
+    POST_TRY(c.rec[1].reserve(sizeof(int32_t) * (size_t)keys));
+    c.kb = cub::DoubleBuffer<unsigned long long>(c.key[0].as<unsigned long long>(), c.key[1].as<unsigned long long>());
+    c.rb = cub::DoubleBuffer<int32_t>(c.rec[0].as<int32_t>(), c.rec[1].as<int32_t>());
+    int64_t n = 0;
+    for (int32_t s = s0; s < s1; ++s) {
+      const int32_t *lab_s = rows + (size_t)s * R;
+      POST_TRY(cudaMemsetAsync(Z, 0, sizeof(int32_t) * R, st));
+      k_label_sizes<<<grid_for(R), THREADS, 0, st>>>(R, lab_s, Z);
+      k_flag_big<<<grid_for(R + 1), THREADS, 0, st>>>(R, lab_s, Z, c.flag.as<int32_t>());
+      POST_TRY(c.tmp.reserve(tb_scan));
+      size_t tb = c.tmp.cap;
+      POST_TRY(cub::DeviceScan::ExclusiveSum(c.tmp.p, tb, c.flag.as<int32_t>(), c.pos.as<int32_t>(), R + 1, st));
+      k_scatter_flagged<<<grid_for(R), THREADS, 0, st>>>(R, c.flag.as<int32_t>(), c.pos.as<int32_t>(),
+                                                         c.sel.as<int32_t>());
+      const int64_t nsel = ss[s].keys;  // what the scan selects, counted when the sample was added
+      if (nsel > 0)
+        k_vis_keys<<<grid_for(nsel), THREADS, 0, st>>>(nsel, c.sel.as<int32_t>(), lab_s, L, s - s0, b,
+                                                       c.kb.Current() + n, c.rb.Current() + n);
+      n += nsel;
+    }
+    POST_TRY(cudaGetLastError());
+    s0 = s1;
+    if (n == 0) continue;  // every sample of the batch is all singletons: every cell with them is a singleton
+    const int end_bit = 2 * b + bits_for(B);
+    POST_TRY(c.head.reserve(sizeof(int32_t) * (size_t)n));
+    POST_TRY(c.crank.reserve(sizeof(int32_t) * (size_t)n));
+    POST_TRY(c.cpos.reserve(sizeof(int32_t) * (size_t)(n + 1)));
+    size_t tbs = 0, tbc = 0;
+    POST_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tbs, c.kb, c.rb, n, 0, end_bit, st));
+    POST_TRY(cub::DeviceScan::InclusiveSum(nullptr, tbc, (const int32_t *)nullptr, (int32_t *)nullptr, n, st));
+    POST_TRY(c.tmp.reserve(std::max(tbs, tbc)));
+    tbs = c.tmp.cap;
+    POST_TRY(cub::DeviceRadixSort::SortPairs(c.tmp.p, tbs, c.kb, c.rb, n, 0, end_bit, st));
+    k_cell_heads<<<grid_for(n), THREADS, 0, st>>>(n, c.kb.Current(), c.head.as<int32_t>());
+    tbc = c.tmp.cap;
+    POST_TRY(cub::DeviceScan::InclusiveSum(c.tmp.p, tbc, c.head.as<int32_t>(), c.crank.as<int32_t>(), n, st));
+    k_cell_pos<<<grid_for(n), THREADS, 0, st>>>(n, c.head.as<int32_t>(), c.crank.as<int32_t>(), c.cpos.as<int32_t>());
+    int32_t ncell = 0;
+    POST_TRY(cudaMemcpyAsync(&ncell, c.crank.as<int32_t>() + n - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    POST_TRY(cudaGetLastError());
+    POST_TRY(cudaStreamSynchronize(st));
+    if (const int rc = on_batch(n, (int64_t)ncell); rc != DBL_OK) return rc;
+  }
+  return DBL_OK;
+}
+}  // namespace
+
+// G[n] = the cells of n >= 2 records of labels ^ C_s summed over the held samples s, from the cell pass of the search.
+extern "C" int dbl_vi_score(dbl_vi *p, const int32_t *labels, int64_t width, int64_t *G_out) {
+  if (!p || !labels || !G_out) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  if (width < (int64_t)p->max_size + 1 || width > INT64_MAX / 8) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(labels, p->cluster); rc != DBL_OK) return rc;
+  cudaStream_t st = p->stream;
+  const size_t gbytes = sizeof(unsigned long long) * (size_t)width;
+  Buf G;
+  CellPass c;
+  POST_TRY(G.alloc(gbytes));
+  POST_TRY(cudaMemsetAsync(G.p, 0, gbytes, st));
+  const int rc = vi_cell_batches(p, p->cluster.as<int32_t>(), &SampleStats::keys, c, [&](int64_t, int64_t ncell) {
+    k_cell_hist<<<grid_for(ncell), THREADS, 0, st>>>(ncell, c.cpos.as<int32_t>(), G.as<unsigned long long>());
+    return DBL_OK;
+  });
+  if (rc != DBL_OK) return rc;
+  POST_TRY(cudaMemcpyAsync(G_out, G.p, gbytes, cudaMemcpyDefault, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
+// The search: check the table and the bounds; take and canonically group the start; then rounds of sizes, the cell
+// pass with every sample's contributions (k_vis_count, an int64 scan, k_vis_emit), each batch's contributions sorted
+// with the running table and reduced by key into it, best moves, the two-stage claims, the moves and the canonical
+// relabel of the Binder search, until no record proposes or max_rounds rounds are done.  The first round's cell pass
+// also sums F_q over the cells, which with the sizes gives J_q of the start.  Every buffer is the call's own.
+extern "C" int dbl_vi_search(dbl_vi *p, const int64_t *step, const int32_t *start, int32_t max_rounds,
+                             int32_t *labels_out, int32_t *rounds_out, int32_t *converged_out, int64_t *moves,
+                             int64_t *clusters, int64_t *dJ, int64_t *J0_out) {
+  if (!p || !step || !start || !labels_out || !rounds_out || !converged_out || !moves || !clusters || !dJ || !J0_out ||
+      max_rounds < 1)
+    return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  const int64_t R = p->R;
+  const int32_t S = p->S;
+  if (step[0] != 0) return DBL_ERR_INVALID;
+  for (int64_t m = 1; m < R; ++m)
+    if (step[m] < step[m - 1]) return DBL_ERR_INVALID;
+  // every J_q, dJ and round sum is within 4 S R D_q[R - 1] in magnitude
+  if ((unsigned __int128)S * (unsigned __int128)R * (unsigned __int128)step[R - 1] >= ((unsigned __int128)1 << 61))
+    return DBL_ERR_INVALID;
+  for (int32_t s = 0; s < S; ++s)
+    if (p->stats[s].squares > VI_MAX_SQUARES) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(start, p->cluster); rc != DBL_OK) return rc;
+  const int b = p->lab_bits, gbits = bits_for(2 * R);
+  cudaStream_t st = p->stream;
+
+  const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(long long) * (size_t)R;
+  Buf Dq, F, iota, lab, size, gkey, gkey_s, rec_s, head, start_b, prop_dJ, prop_dest, claim_dJ, claim_i, stats;
+  Buf cnt, off, ck[2], cv[2], nruns;
+  CellPass c;
+  POST_TRY(Dq.alloc(r8));
+  POST_TRY(F.alloc(sizeof(long long) * (size_t)(R + 1)));
+  POST_TRY(iota.alloc(r4));
+  POST_TRY(lab.alloc(r4));
+  POST_TRY(size.alloc(r4));
+  POST_TRY(gkey.alloc(r8));
+  POST_TRY(gkey_s.alloc(r8));
+  POST_TRY(rec_s.alloc(r4));
+  POST_TRY(head.alloc(r4));
+  POST_TRY(start_b.alloc(r4));
+  POST_TRY(prop_dJ.alloc(r8));
+  POST_TRY(prop_dest.alloc(r4));
+  POST_TRY(claim_dJ.alloc(r8));
+  POST_TRY(claim_i.alloc(r4));
+  POST_TRY(stats.alloc(8 * sizeof(unsigned long long)));
+  POST_TRY(nruns.alloc(sizeof(long long)));
+  {
+    // F_q(n) = sum over m < n of D_q[m], exact in int64 by the bound above
+    std::vector<long long> f;
+    try {
+      f.resize((size_t)R + 1);
+    } catch (const std::bad_alloc &) {
+      return DBL_ERR_CUDA;
+    }
+    f[0] = 0;
+    for (int64_t m = 0; m < R; ++m) f[m + 1] = f[m] + step[m];
+    POST_TRY(cudaMemcpyAsync(Dq.p, step, r8, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(F.p, f.data(), sizeof(long long) * (size_t)(R + 1), cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaStreamSynchronize(st));
+  }
+  unsigned long long *st8 = stats.as<unsigned long long>();
+  int32_t *L = lab.as<int32_t>(), *Z = size.as<int32_t>();
+  const long long *dq = Dq.as<long long>();
+  k_iota<<<grid_for(R), THREADS, 0, st>>>(R, iota.as<int32_t>());
+  auto relabel = [&]() {
+    return canonical_relabel(R, gbits, gkey.as<unsigned long long>(), iota.as<int32_t>(),
+                             gkey_s.as<unsigned long long>(), rec_s.as<int32_t>(), head.as<int32_t>(),
+                             start_b.as<int32_t>(), L, c.tmp, st);
+  };
+  // sizes of L, then sum of F_q over its clusters and its number of clusters into st8[4], st8[5]
+  auto sizes = [&]() {
+    POST_TRY(cudaMemsetAsync(Z, 0, r4, st));
+    POST_TRY(cudaMemsetAsync(st8 + 4, 0, 2 * sizeof(unsigned long long), st));
+    k_label_sizes<<<grid_for(R), THREADS, 0, st>>>(R, L, Z);
+    k_size_stats<<<grid_for(R), THREADS, 0, st>>>(R, Z, F.as<long long>(), st8 + 4);
+    return DBL_OK;
+  };
+  k_widen_labels<<<grid_for(R), THREADS, 0, st>>>(R, p->cluster.as<int32_t>(), gkey.as<unsigned long long>());
+  if (const int rc = relabel(); rc != DBL_OK) return rc;
+  if (const int rc = sizes(); rc != DBL_OK) return rc;
+  POST_TRY(cudaMemsetAsync(st8 + 6, 0, sizeof(unsigned long long), st));  // sum of F_q over the start's cells
+
+  int32_t rounds = 0, converged = 0;
+  long long J0 = 0;
+  for (;;) {
+    // every sample's contributions, reduced into (record << b | cluster, w) in ck/cv[cur], acc_n entries
+    int cur = 0;
+    int64_t acc_n = 0;
+    const bool first_round = rounds == 0;
+    const int rc = vi_cell_batches(p, L, &SampleStats::squares, c, [&](int64_t n, int64_t ncell) {
+      if (first_round)
+        k_cell_F<<<grid_for(ncell), THREADS, 0, st>>>(ncell, c.cpos.as<int32_t>(), F.as<long long>(), st8 + 6);
+      POST_TRY(cnt.reserve(sizeof(long long) * (size_t)(n + 1)));
+      POST_TRY(off.reserve(sizeof(long long) * (size_t)(n + 1)));
+      k_vis_count<<<grid_for(n + 1), THREADS, 0, st>>>(n, b, c.kb.Current(), c.crank.as<int32_t>(),
+                                                        cnt.as<long long>());
+      size_t tb = 0;
+      POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.as<long long>(), off.as<long long>(), n + 1, st));
+      POST_TRY(c.tmp.reserve(tb));
+      tb = c.tmp.cap;
+      POST_TRY(cub::DeviceScan::ExclusiveSum(c.tmp.p, tb, cnt.as<long long>(), off.as<long long>(), n + 1, st));
+      long long nc = 0;
+      POST_TRY(cudaMemcpyAsync(&nc, off.as<long long>() + n, sizeof(long long), cudaMemcpyDeviceToHost, st));
+      POST_TRY(cudaStreamSynchronize(st));
+      const int64_t total = acc_n + nc;
+      // both sides hold the running table and the batch's contributions; side cur keeps its running table
+      const size_t need = sizeof(long long) * (size_t)total, keep = sizeof(long long) * (size_t)acc_n;
+      POST_TRY(ck[cur].reserve_keep(need, keep, st));
+      POST_TRY(cv[cur].reserve_keep(need, keep, st));
+      POST_TRY(ck[cur ^ 1].reserve(need));
+      POST_TRY(cv[cur ^ 1].reserve(need));
+      k_vis_emit<<<(int)std::min<int64_t>((n + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, 8192), THREADS, 0, st>>>(
+          n, b, c.kb.Current(), c.rb.Current(), c.crank.as<int32_t>(), c.cpos.as<int32_t>(), off.as<long long>(), L,
+          dq, ck[cur].as<unsigned long long>() + acc_n, cv[cur].as<long long>() + acc_n);
+      // the running table and the batch's contributions, sorted and reduced by key into the other side
+      cub::DoubleBuffer<unsigned long long> kk(ck[cur].as<unsigned long long>(), ck[cur ^ 1].as<unsigned long long>());
+      cub::DoubleBuffer<long long> vv(cv[cur].as<long long>(), cv[cur ^ 1].as<long long>());
+      size_t tbs = 0, tbr = 0;
+      POST_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tbs, kk, vv, total, 0, 2 * b, st));
+      POST_TRY(c.tmp.reserve(tbs));
+      tbs = c.tmp.cap;
+      POST_TRY(cub::DeviceRadixSort::SortPairs(c.tmp.p, tbs, kk, vv, total, 0, 2 * b, st));
+      const int sorted = kk.Current() == ck[cur].as<unsigned long long>() ? cur : cur ^ 1;
+      const int other = sorted ^ 1;
+      POST_TRY(cub::DeviceReduce::ReduceByKey(nullptr, tbr, ck[sorted].as<unsigned long long>(),
+                                              ck[other].as<unsigned long long>(), cv[sorted].as<long long>(),
+                                              cv[other].as<long long>(), nruns.as<long long>(), cub::Sum(), total,
+                                              st));
+      POST_TRY(c.tmp.reserve(tbr));
+      tbr = c.tmp.cap;
+      POST_TRY(cub::DeviceReduce::ReduceByKey(c.tmp.p, tbr, ck[sorted].as<unsigned long long>(),
+                                              ck[other].as<unsigned long long>(), cv[sorted].as<long long>(),
+                                              cv[other].as<long long>(), nruns.as<long long>(), cub::Sum(), total,
+                                              st));
+      long long runs = 0;
+      POST_TRY(cudaMemcpyAsync(&runs, nruns.p, sizeof(long long), cudaMemcpyDeviceToHost, st));
+      POST_TRY(cudaGetLastError());
+      POST_TRY(cudaStreamSynchronize(st));
+      cur = other;
+      acc_n = runs;
+      return DBL_OK;
+    });
+    if (rc != DBL_OK) return rc;
+    if (first_round) {
+      unsigned long long f[3];
+      POST_TRY(cudaMemcpyAsync(f, st8 + 4, sizeof(f), cudaMemcpyDeviceToHost, st));
+      POST_TRY(cudaStreamSynchronize(st));
+      J0 = (long long)S * (long long)f[0] - 2 * (long long)f[2];
+    }
+    POST_TRY(cudaMemsetAsync(claim_dJ.p, 0x7f, r8, st));  // above every dJ < 0
+    POST_TRY(cudaMemsetAsync(claim_i.p, 0xff, r4, st));   // above every record index
+    POST_TRY(cudaMemsetAsync(st8, 0, 4 * sizeof(unsigned long long), st));
+    k_vis_best_move<<<grid_for(R), THREADS, 0, st>>>(R, b, acc_n, ck[cur].as<unsigned long long>(),
+                                                     cv[cur].as<long long>(), L, Z, dq, S, prop_dJ.as<long long>(),
+                                                     prop_dest.as<int32_t>(), claim_dJ.as<long long>(), st8 + 3);
+    k_claim_record<<<grid_for(R), THREADS, 0, st>>>(R, L, prop_dJ.as<long long>(), prop_dest.as<int32_t>(),
+                                                    claim_dJ.as<long long>(), claim_i.as<unsigned int>());
+    unsigned long long props = 0;
+    POST_TRY(cudaMemcpyAsync(&props, st8 + 3, sizeof(props), cudaMemcpyDeviceToHost, st));
+    POST_TRY(cudaGetLastError());
+    POST_TRY(cudaStreamSynchronize(st));
+    if (props == 0) {
+      converged = 1;
+      break;
+    }
+    if (rounds == max_rounds) break;
+    k_apply_moves<<<grid_for(R), THREADS, 0, st>>>(R, L, Z, prop_dJ.as<long long>(), prop_dest.as<int32_t>(),
+                                                   prop_dJ.as<long long>(), claim_dJ.as<long long>(),
+                                                   claim_i.as<unsigned int>(), gkey.as<unsigned long long>(), st8);
+    if (const int rc2 = relabel(); rc2 != DBL_OK) return rc2;
+    if (const int rc2 = sizes(); rc2 != DBL_OK) return rc2;
+    unsigned long long log[6];
+    POST_TRY(cudaMemcpyAsync(log, st8, sizeof(log), cudaMemcpyDeviceToHost, st));
+    POST_TRY(cudaGetLastError());
+    POST_TRY(cudaStreamSynchronize(st));
+    moves[rounds] = (int64_t)log[0];
+    dJ[rounds] = (int64_t)log[2];
+    clusters[rounds] = (int64_t)log[5];
+    ++rounds;
+  }
+  POST_TRY(cudaMemcpyAsync(labels_out, L, r4, cudaMemcpyDefault, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  *rounds_out = rounds;
+  *converged_out = converged;
+  *J0_out = (int64_t)J0;
   return DBL_OK;
 }

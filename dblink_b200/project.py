@@ -24,10 +24,13 @@ BINDER_METRICS = ("binder-pairwise", "binder-cluster")
 BINDER_SEARCH_METRICS = ("binder-search-pairwise", "binder-search-cluster")
 # the sample of least posterior expected variation of information against the ground truth
 VI_METRICS = ("vi-pairwise", "vi-cluster")
-SUPPORTED_METRICS = SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_SEARCH_METRICS + VI_METRICS
+# the least expected variation of information found by single-record moves from the VI sample and from the sMPC
+VI_SEARCH_METRICS = ("vi-search-pairwise", "vi-search-cluster")
+SUPPORTED_METRICS = (SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_SEARCH_METRICS + VI_METRICS
+                     + VI_SEARCH_METRICS)
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
-                        "binder-search-clusters", "vi-clusters")
+                        "binder-search-clusters", "vi-clusters", "vi-search-clusters")
 
 
 def shared_most_probable_clusters(chain):
@@ -117,6 +120,46 @@ def vi_estimate(chain):
     mem, off, _ = chain.samples[s]
     return (s, analysis_arrays.sample_labels(chain.num_records, mem, off),
             np.array([len(off) - 1 for _, off, _ in chain.samples], np.int64), losses)
+
+
+def vi_samples(chain):
+    """Every sample of a ChainArrays held once for the VI search path: an analysis_gpu.VI handle when the platform has
+    a device, else analysis_arrays.VISamples.  Both give identical results."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.vi_samples(chain)
+    return analysis_arrays.VISamples(chain)
+
+
+def vi_search_estimate(chain, max_rounds):
+    """The VI search from the VI sample and from the sMPC of a ChainArrays, on one set of held samples that also gives
+    the cross histograms and the scores: (the chosen start's name, its VISearchRun, the rows of vi-search.csv -- per
+    start and round its name, the round, the moves, the clusters and the quantised expected VI E_q; round 0 is the
+    start -- and the exact expected VI of [vi-sample start, smpc start, vi-sample result, smpc result])."""
+    if not chain.samples:
+        raise ValueError("the VI search needs at least one sample at or after lowerIterationCutoff")
+    R, S = chain.num_records, len(chain.samples)
+    width = analysis_arrays.vi_width(chain)
+    analysis_arrays.check_vi_search_size(S, R)
+    analysis_arrays.check_vi_search_squares(analysis_arrays.vi_sample_squares(chain))
+    smpc = shared_most_probable_clusters(chain)
+    table = analysis_arrays.vi_search_table(R)
+    g = analysis_arrays.vi_cluster_histograms(chain, width)
+    g_sum = g.sum(axis=0)
+    with vi_samples(chain) as vi:
+        s = analysis_arrays.vi_estimate(analysis_arrays.vi_losses(g, vi.cross(width), R))
+        mem, off, _ = chain.samples[s]
+        starts = [analysis_arrays.sample_labels(R, mem, off), smpc]
+        runs = [vi.search(table, st, max_rounds) for st in starts]
+        exact = [analysis_arrays.vi_label_loss(np.bincount(np.bincount(lab)), vi.score(lab, width), g_sum, S, R)
+                 for lab in starts + [r.labels for r in runs]]
+    best = analysis_arrays.vi_search_choice(runs)
+    sample_sum = analysis_arrays.vi_sample_sum(chain, table)
+    rows = []
+    for name, st, run in zip(analysis_arrays.VI_SEARCH_STARTS, starts, runs):
+        losses = analysis_arrays.vi_search_losses(run.objectives(), sample_sum, S, R)
+        counts = [len(np.unique(st))] + run.clusters.tolist()
+        rows += [(name, r, m, k, loss) for r, (m, k, loss) in enumerate(zip([0] + run.moves.tolist(), counts, losses))]
+    return analysis_arrays.VI_SEARCH_STARTS[best], runs[best], rows, exact
 
 
 def _searched_cost(false_link_cost):
@@ -243,6 +286,10 @@ class Project:
                 if "vi-clusters" in prm["quantities"]:
                     L.append("  * SummarizeStep: vi-clusters is the sample of least posterior expected variation of "
                              "information")
+                if "vi-search-clusters" in prm["quantities"]:
+                    L.append(f"  * SummarizeStep: vi-search-clusters is the least posterior expected variation of "
+                             f"information found by single-record moves from the VI sample and the sMPC, with "
+                             f"maxSearchRounds={prm['max_search_rounds']}")
             elif name == "evaluate":
                 smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
                 post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
@@ -270,6 +317,12 @@ class Project:
                 if vi:
                     L.append(f"  * EvaluateStep: Evaluating the sample of least posterior expected variation of "
                              f"information (iterations >= {prm['lower_iteration_cutoff']}) using {braces(vi)} metrics")
+                vi_search = [m for m in prm["metrics"] if m in VI_SEARCH_METRICS]
+                if vi_search:
+                    L.append(f"  * EvaluateStep: Evaluating the least posterior expected variation of information "
+                             f"found by single-record moves from the VI sample and the sMPC (maxSearchRounds="
+                             f"{prm['max_search_rounds']}, iterations >= {prm['lower_iteration_cutoff']}) using "
+                             f"{braces(vi_search)} metrics")
             else:
                 L.append("  * CopyFilesStep: Copying {" + ", ".join(prm["file_names"]) + "} to destination "
                          + prm["destination_path"])
@@ -481,6 +534,11 @@ class Project:
                         _, labels, num_clusters, losses = vi_estimate(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids), "vi-clusters.csv")
                         writers.save_vi_loss(ch.chains, ch.iterations, num_clusters, losses, self.output_path)
+                    elif q == "vi-search-clusters":
+                        _, run, rows, _ = vi_search_estimate(ch, prm["max_search_rounds"])
+                        self._save_smpc(analysis_arrays.labels_to_clusters(run.labels, ch.record_ids),
+                                        "vi-search-clusters.csv")
+                        writers.save_vi_search(rows, self.output_path)
                     else:
                         labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
@@ -555,6 +613,18 @@ class Project:
                         elif m == "vi-cluster":
                             results[m] = analysis_arrays.adjusted_rand_index(labels, truth)
                             text.append(analysis.format_vi_cluster(results[m], *at))
+                if any(m in VI_SEARCH_METRICS for m in prm["metrics"]):
+                    ch = ch if ch is not None else self.read_chain(cut)
+                    start, run, _, exact = vi_search_estimate(ch, prm["max_search_rounds"])
+                    truth = true_labels(ch.record_ids)
+                    at = (start, run.rounds, run.converged, exact)
+                    for m in prm["metrics"]:
+                        if m == "vi-search-pairwise":
+                            results[m] = analysis_arrays.pairwise_metrics(run.labels, truth)
+                            text.append(analysis.format_vi_search_pairwise(results[m], *at))
+                        elif m == "vi-search-cluster":
+                            results[m] = analysis_arrays.adjusted_rand_index(run.labels, truth)
+                            text.append(analysis.format_vi_search_cluster(results[m], *at))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
             elif name == "copy-files":

@@ -255,3 +255,15 @@ def save_vi_loss(chains, iterations, num_clusters, losses, path):
         fh.write(VI_LOSS_HEADER + "\n")
         for k, it, n, loss in zip(chains, iterations, num_clusters, losses):
             fh.write(f"{int(k)},{int(it)},{int(n)},{float(loss)!r}\n")
+
+
+VI_SEARCH_HEADER = "start,round,moves,numClusters,expectedLoss"
+
+
+def save_vi_search(rows, path):
+    """vi-search.csv under `path`: rows (start name, round, moves, clusters, quantised expected VI) as
+    project.vi_search_estimate gives them, round 0 being the start; the loss written with repr."""
+    with open(os.path.join(path, "vi-search.csv"), "w") as fh:
+        fh.write(VI_SEARCH_HEADER + "\n")
+        for start, r, moves, k, loss in rows:
+            fh.write(f"{start},{int(r)},{int(moves)},{int(k)},{float(loss)!r}\n")

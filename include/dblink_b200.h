@@ -414,8 +414,42 @@ int dbl_eval_read(dbl_eval *, int64_t *tp, int64_t *pred_pairs, int64_t *num_clu
  *                      (at most max(batch keys, R)) plus the sort's temporary storage.  The held samples do not
  *                      change, whatever the outcome.  The work is S (S - 1) / 2 sorts of the records in clusters of
  *                      two or more, batched over samples.
+ *   dbl_vi_score       any labelling c = labels[R] (host or device pointer, labels in [0, R)) against the held samples:
+ *                      G_out[n] (width int64, host or device) = sum over s of the cells of n >= 2 records of c ^ C_s;
+ *                      G_out[0] = G_out[1] = 0.  With g_c[n] = the clusters of n records of c, the expected VI of c is
+ *                      sum over n of (S g_c[n] + sum_s g_s[n] - 2 G[n]) n log2 n / (R S).  DBL_ERR_INVALID: width
+ *                      < M + 1, a label outside [0, R).  It runs the search's cell pass (below) once, its batches
+ *                      taking samples while their keys (records in clusters of two or more) stay within
+ *                      max(batch keys, one sample's), with no cap on cluster sizes.  Memory, the call's own: 8 width
+ *                      bytes, 12 per record, 36 per key of the largest batch (at most max(batch keys, R)) and the
+ *                      sorts' temporary storage.
+ *   dbl_vi_search      single-record moves from the labelling start[R] (host or device pointer, labels in [0, R)) while
+ *                      they lower J_q(c) = S sum over clusters X of F(|X|) - 2 sum_s sum over cells of c ^ C_s of F(n),
+ *                      F(n) = step[0] + ... + step[n - 1].  step (R int64, host) is D_q[m] = round(2^20 (f(m + 1) -
+ *                      f(m))), f(n) = n log2 n, so that J_q / (2^20 R S) is the expected VI up to a constant; it must
+ *                      have step[0] = 0 and be non-decreasing.  Moving record i from A (|A| = a) to B changes J_q by
+ *                      S (step[|B|] - step[a - 1]) - 2 (w_B - w_A), w_X = sum over s of step[|X ^ C_s(i)|] for B and
+ *                      of step[|A ^ C_s(i)| - 1] for A; a singleton is |B| = 0, w_B = 0.  The rounds and claims are
+ *                      those of dbl_pairs_binder_search: every record's least (dJ, destination) over the clusters
+ *                      sharing a sample cluster with it and, out of a cluster of two or more, a singleton (-1), proposed
+ *                      if dJ < 0, applied if it holds the least (dJ, record) on every cluster it touches.  It stops when
+ *                      no record proposes (*converged_out = 1) or after max_rounds rounds (0).  Per round moves /
+ *                      clusters / dJ (host, max_rounds entries each, *rounds_out written): the moves applied, the
+ *                      clusters after the round and the change of J_q; *J0_out = J_q of the start.  labels_out (R, host
+ *                      or device): each record labelled by the smallest record index of its cluster.  A round sorts
+ *                      one key per record in a cluster of two or more of each sample, batched over samples as
+ *                      dbl_vi_score does, except that a batch takes samples while their sums of |K|^2 stay within
+ *                      max(batch keys, that of its first sample); it emits one contribution per key and cell of its
+ *                      sample cluster (at most sum |K|^2 per sample), and sorts and reduces them by (record, cluster).
+ *                      DBL_ERR_INVALID: a NULL pointer, max_rounds < 1, step[0] != 0 or step decreasing, S R step[R-1]
+ *                      >= 2^61 (which keeps every J_q and dJ inside int64), a held sample whose sum over its clusters of
+ *                      |K|^2 exceeds 2^28, a start label outside [0, R) -- all before any device work.  Memory, the
+ *                      call's own: 92 bytes per record, 52 per key of the largest batch (at most the batch's sum of
+ *                      |K|^2), 32 per entry of the batch's contributions plus the running (record, cluster) table, and
+ *                      the sorts' temporary storage.
+ *   dbl_vi_score / dbl_vi_search before the first sample give DBL_ERR_STATE; neither changes the held samples.
  * DBL_ERR_INVALID: num_records outside [1, 2^31 - 1] or max_samples < 1.  DBL_ERR_CUDA: no device, or the held label
- * matrix (or a buffer of dbl_vi_cross) does not fit on it.
+ * matrix (or a buffer of dbl_vi_cross, dbl_vi_score or dbl_vi_search) does not fit on it.
  * ------------------------------------------------------------------------------------------------- */
 typedef struct dbl_vi dbl_vi;
 int dbl_vi_create(dbl_vi **out, int64_t num_records, int32_t max_samples);
@@ -424,6 +458,10 @@ int dbl_vi_add_sample(dbl_vi *, const int32_t *cluster /* R, host or device */);
 int32_t dbl_vi_num_samples(const dbl_vi *);
 int dbl_vi_set_batch_keys(dbl_vi *, int64_t max_keys);
 int dbl_vi_cross(dbl_vi *, int64_t width, int64_t *G_out /* S x width */);
+int dbl_vi_score(dbl_vi *, const int32_t *labels /* R, host or device */, int64_t width, int64_t *G_out /* width */);
+int dbl_vi_search(dbl_vi *, const int64_t *step /* R, host */, const int32_t *start /* R, host or device */,
+                  int32_t max_rounds, int32_t *labels_out /* R */, int32_t *rounds_out, int32_t *converged_out,
+                  int64_t *moves, int64_t *clusters, int64_t *dJ /* max_rounds each, host */, int64_t *J0_out);
 
 /* The protocol functions of the theta draw (DESIGN.md 4.5), exposed so that they can be checked without a GPU:
  * log / exp built from individually rounded binary64 operations, and updateDistProbs (GU:305-320) itself. */
