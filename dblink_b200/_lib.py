@@ -151,6 +151,7 @@ SIGNATURES = {
     "dbl_vi_set_batch_keys": (C.c_int, [vp, C.c_int64]),
     "dbl_vi_cross": (C.c_int, [vp, C.c_int64, vp]),
     "dbl_vi_score": (C.c_int, [vp, vp, C.c_int64, vp]),
+    "dbl_vi_score_samples": (C.c_int, [vp, vp, C.c_int64, vp]),
     "dbl_vi_search": (C.c_int, [vp, i64p, vp, C.c_int32, vp, i32p, i32p, i64p, i64p, i64p, i64p]),
     "dbl_version": (C.c_char_p, []),
 }

@@ -8,6 +8,7 @@
                                                              information
   vi_search                                               <- single-record moves that lower the quantised expected
                                                              variation of information
+  credible_ball                                           <- the samples within a VI or Binder radius of an estimate
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
   pairwise_metrics                                        <- analysis/PairwiseMetrics.scala:44-63,
                                                              BinaryClassificationMetrics.scala:23-37
@@ -266,6 +267,53 @@ def vi_search(chain, starts, max_rounds=1000, records=None):
     return min(range(len(runs)), key=lambda k: (runs[k]["J"], k)), runs
 
 
+def credible_ball(chain, center, level):
+    """The credible ball around a partition `center` (clusters of ids), by the definitions (Wade and Ghahramani 2018):
+    the distance of every sample from the center, VI(c, C_s) = H(c) + H(C_s) - 2 I(c, C_s) in bits as vi_clusters
+    computes it, and the Binder distance, the record pairs one of them links and the other does not, by enumerating
+    every pair; k = ceil(level S) with level the fraction its repr spells; the radius is the k-th smallest distance and
+    the ball every sample within it.  The bounds are samples in the ball: vertical-upper the farthest from the center,
+    horizontal-upper the farthest of those with the fewest clusters, horizontal-lower the farthest of those with the
+    most clusters, each the earliest sample when several qualify; ties = how many qualify.  Entropies carry rounding, so
+    VI distances within 1e-12 of each other count as equal (each is ranked as the smallest of its run of such values).
+    Returns {"vi" | "binder": dict(distances, radius, in_ball, bounds = {bound: (sample position, ties)})}."""
+    samples = [list(clusters_of_sample(s)) for s in chain]
+    center = [frozenset(c) for c in center]
+    S = len(samples)
+    R = sum(len(c) for c in center)
+
+    def entropy(cl):
+        return -sum(len(x) / R * math.log2(len(x) / R) for x in cl)
+
+    def mutual_information(a, b):
+        return sum(len(x & y) / R * math.log2(len(x & y) * R / (len(x) * len(y))) for x in a for y in b if x & y)
+
+    def pairs(cl):
+        return {frozenset(p) for c in cl for p in itertools.combinations(c, 2)}
+
+    k = math.ceil(fractions.Fraction(repr(float(level))) * S)
+    num_clusters = [len(cl) for cl in samples]
+    out = {}
+    for name, dist in (("vi", lambda cl: entropy(center) + entropy(cl) - 2 * mutual_information(center, cl)),
+                       ("binder", lambda cl: len(pairs(center) ^ pairs(cl)))):
+        raw = [dist(cl) for cl in samples]
+        d = list(raw)
+        if name == "vi":
+            for a, b in zip(sorted(range(S), key=lambda s: raw[s]), sorted(range(S), key=lambda s: raw[s])[1:]):
+                if raw[b] - d[a] <= 1e-12:
+                    d[b] = d[a]
+        radius = sorted(d)[k - 1]
+        ball = [s for s in range(S) if d[s] <= radius]
+        farthest = lambda among: [s for s in among if d[s] == max(d[t] for t in among)]  # noqa: E731
+        fewest = [s for s in ball if num_clusters[s] == min(num_clusters[t] for t in ball)]
+        most = [s for s in ball if num_clusters[s] == max(num_clusters[t] for t in ball)]
+        bounds = {bound: (tied[0], len(tied)) for bound, tied in (("vertical-upper", farthest(ball)),
+                                                                   ("horizontal-upper", farthest(fewest)),
+                                                                   ("horizontal-lower", farthest(most)))}
+        out[name] = dict(distances=raw, radius=radius, in_ball=[d[s] <= radius for s in range(S)], bounds=bounds)
+    return out
+
+
 def cluster_size_distribution(chain):
     """iteration -> {cluster size: count} (LinkageChain.scala:137-154)."""
     out = {}
@@ -429,6 +477,21 @@ def format_vi_search_cluster(ari, start, rounds, converged, exact):
     return ("=====================================\n      VI search cluster metrics\n"
             "-------------------------------------\n" + _vi_search_lines(start, rounds, converged, exact)
             + f" Adj. Rand index: {ari}\n=====================================\n")
+
+
+def format_credible_ball(res):
+    """The credible-ball section: res = the center, the level, the samples and per distance the truth's distance from
+    the center, the radius, whether the truth lies in the ball and the samples in it (project.py)."""
+    def line(label, r, unit):
+        where = "inside" if r["truthInBall"] else "outside"
+        return (f" {label:<17}truth at {r['truthDistance']!r}{unit} from the center, radius {r['radius']!r}, {where} "
+                f"the ball of {r['samplesInBall']} samples\n")
+
+    return ("=====================================\n           Credible ball\n"
+            "-------------------------------------\n"
+            f" Center:          {res['center']}, level {res['level']!r}, {res['samples']} samples\n"
+            + line("VI:", res["vi"], " bits") + line("Binder:", res["binder"], " pairs")
+            + "=====================================\n")
 
 
 def _posterior_line(label, s, extra=""):

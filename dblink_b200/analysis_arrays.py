@@ -5,6 +5,7 @@ A sample is held as (members, offsets, partition_of_cluster): `members` = record
 dictionary) of all clusters back to back, `offsets[c]:offsets[c+1]` = cluster c.  The simple set-based functions in
 analysis.py stay as the readable restatement; tests compare the two on random chains.
 """
+import fractions
 import math
 import os
 
@@ -561,18 +562,24 @@ def vi_label_loss(g_c, G_c, g_sum, num_samples, num_records):
     return math.fsum(D[nz].astype(np.float64) * np.array([n * math.log2(n) for n in nz.tolist()])) / (R * S)
 
 
-def vi_label_cells(chain, labels, width):
-    """G, int64[width]: the cells of n >= 2 records of labels ^ C_s summed over the samples s of the chain (width at
-    least M + 1, M = the largest cluster of any sample, as every cell lies inside one)."""
+def vi_sample_cells(chain, labels, width):
+    """G, int64[S, width]: per sample s the cells of n >= 2 records of labels ^ C_s (width at least M + 1, M = the
+    largest cluster of any sample, as every cell lies inside one)."""
     R = chain.num_records
     labels = np.asarray(labels, np.int64)
-    G = np.zeros(int(width), np.int64)
-    for mem, off, _ in chain.samples:
+    G = np.zeros((len(chain.samples), int(width)), np.int64)
+    for s, (mem, off, _) in enumerate(chain.samples):
         lab_s = sample_labels(R, mem, off)
         big = np.flatnonzero(np.bincount(lab_s, minlength=R)[lab_s] >= 2)
         _, n = np.unique(lab_s[big] * R + labels[big], return_counts=True)
-        G += np.bincount(n[n >= 2], minlength=width)[:width]
+        G[s] = np.bincount(n[n >= 2], minlength=width)[:width]
     return G
+
+
+def vi_label_cells(chain, labels, width):
+    """G, int64[width]: the cells of n >= 2 records of labels ^ C_s summed over the samples s of the chain: the row sum
+    of vi_sample_cells."""
+    return vi_sample_cells(chain, labels, width).sum(axis=0)
 
 
 def vi_estimate(losses):
@@ -580,6 +587,68 @@ def vi_estimate(losses):
     if len(losses) == 0:
         raise ValueError("the VI estimate needs at least one sample")
     return min(range(len(losses)), key=lambda s: (losses[s], s))
+
+
+# ---- the credible ball around a point estimate (Wade and Ghahramani 2018, section 4) --------------------------------
+# Per sample s and cell size n, with g_x[n] = the clusters of n records of x and G_s[n] = the cells of n >= 2 records of
+# c ^ C_s: D_s[n] = g_c[n] + g_s[n] - 2 G_s[n].  Then VI(c, C_s) = sum over n of D_s[n] n log2 n / R bits, and the
+# Binder distance, the record pairs one of c, C_s links and the other does not, is sum over n of D_s[n] n (n - 1) / 2,
+# exact in int64.  The ball of level p holds every sample within the radius, the k-th smallest distance, k = ceil(p S)
+# (an exact fraction of repr(p)); ties at the radius are inside.  Its bounds are samples in the ball: the farthest from
+# c (vertical upper), the farthest of those with the fewest clusters (horizontal upper) and the farthest of those with
+# the most clusters (horizontal lower); ties go to the earliest sample in pooled order.
+CREDIBLE_BALL_BOUNDS = ("vertical-upper", "horizontal-upper", "horizontal-lower")
+CREDIBLE_BALL_DISTANCES = ("vi", "binder")
+
+
+def credible_ball_distances(g_c, g, G_rows, num_records):
+    """(vi float64[S], binder int64[S]): the distances of a labelling c from every sample, from integer histograms
+    indexed by size n: g_c[n] = the clusters of n records of c, g[s][n] those of sample s, G_rows[s][n] = the cells of
+    n >= 2 records of c ^ C_s.  The VI is fsum over n >= 2 of float(D_s[n]) (n log2 n), divided by R: correctly rounded
+    and order-free, so equal integers give equal distances."""
+    g_c, g, G = np.asarray(g_c, np.int64), np.asarray(g, np.int64), np.asarray(G_rows, np.int64)
+    S, R = G.shape[0], int(num_records)
+    width = max(len(g_c), g.shape[1], G.shape[1])
+    D = (np.pad(g_c, (0, width - len(g_c)))[None, :] + np.pad(g, ((0, 0), (0, width - g.shape[1])))
+         - 2 * np.pad(G, ((0, 0), (0, width - G.shape[1]))))
+    D[:, :2] = 0
+    n = np.arange(width, dtype=np.int64)
+    binder = (D * (n * (n - 1) // 2)).sum(axis=1) if S else np.zeros(0, np.int64)
+    f = np.array([k * math.log2(k) if k >= 2 else 0.0 for k in range(width)])
+    vi = np.zeros(S, np.float64)
+    for s in range(S):
+        nz = np.flatnonzero(D[s])
+        vi[s] = math.fsum(D[s, nz].astype(np.float64) * f[nz]) / R if R else 0.0
+    return vi, binder.astype(np.int64)
+
+
+def credible_level_rank(level, num_samples):
+    """k = ceil(level S), exact: level is taken as the fraction its repr spells (0.7 is 7/10, so 0.7 x 10 gives 7)."""
+    level = float(level)
+    if not 0.0 < level <= 1.0:
+        raise ValueError("credibleLevel must be in (0, 1].")
+    return math.ceil(fractions.Fraction(repr(level)) * int(num_samples))
+
+
+def credible_ball(distances, num_clusters, level):
+    """The credible ball of one distance: (radius, in-ball bool[S], {bound: (sample position, ties)}).  ties counts the
+    samples of the ball that equal the chosen one in what the bound ranks them by."""
+    d = np.asarray(distances)
+    k = np.asarray(num_clusters, np.int64)
+    S = len(d)
+    if S == 0:
+        raise ValueError("the credible ball needs at least one sample")
+    radius = np.sort(d, kind="stable")[credible_level_rank(level, S) - 1].item()
+    inside = d <= radius
+    members = np.flatnonzero(inside).tolist()
+    rank = {"vertical-upper": lambda s: (-d[s],),
+            "horizontal-upper": lambda s: (k[s], -d[s]),
+            "horizontal-lower": lambda s: (-k[s], -d[s])}
+    bounds = {}
+    for name in CREDIBLE_BALL_BOUNDS:
+        best = min(members, key=lambda s: (rank[name](s), s))
+        bounds[name] = (best, sum(rank[name](s) == rank[name](best) for s in members))
+    return radius, inside, bounds
 
 
 # ---- the VI search: parallel single-record moves ----------------------------------------------------------------
@@ -760,7 +829,8 @@ def vi_search_choice(runs):
 
 class VISamples:
     """The held samples of a chain on the host, with the methods of analysis_gpu.VI: cross (the cell histograms of
-    every pair of samples), search (the VI search) and score (the cells of a labelling with every sample)."""
+    every pair of samples), search (the VI search), score (the cells of a labelling with every sample) and
+    score_samples (those cells per sample)."""
 
     def __init__(self, chain):
         self.chain = chain
@@ -787,6 +857,9 @@ class VISamples:
 
     def score(self, labels, width):
         return vi_label_cells(self.chain, labels, width)
+
+    def score_samples(self, labels, width):
+        return vi_sample_cells(self.chain, labels, width)
 
 
 def vi_search(chain, starts, max_rounds=1000):

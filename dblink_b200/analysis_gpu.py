@@ -14,8 +14,8 @@ exactly: every sample goes into one pairs table, then every sample is scored aga
 rule is in integers, and the device applies it to the same table.  The cell histograms of the variation-of-information
 estimate equal analysis_arrays.vi_cross_histograms exactly: they are integers, counted on the device from radix-sorted
 (sample, label, label) keys of every pair of held samples.  The VI search (single-record moves on a quantised table)
-and the cells of any labelling with every held sample equal analysis_arrays.vi_search_rounds / vi_label_cells exactly,
-on the same handle.
+and the cells of any labelling with every held sample, summed or per sample, equal analysis_arrays.vi_search_rounds /
+vi_label_cells / vi_sample_cells exactly, on the same handle.
 """
 import ctypes as C
 
@@ -280,6 +280,15 @@ class VI(_Handle):
             raise ValueError("a labelling needs one cluster label per record")
         G = np.empty(int(width), np.int64)
         self._call("score", self._h, labels.ctypes.data, int(width), G.ctypes.data)
+        return G
+
+    def score_samples(self, labels, width):
+        """G, int64[S, width]: per held sample s the cells of n >= 2 records of labels ^ C_s."""
+        labels = np.ascontiguousarray(labels, np.int32)
+        if labels.shape != (self.num_records,):
+            raise ValueError("a labelling needs one cluster label per record")
+        G = np.empty((self.num_samples, int(width)), np.int64)
+        self._call("score_samples", self._h, labels.ctypes.data, int(width), G.ctypes.data)
         return G
 
     def search(self, table, start, max_rounds):

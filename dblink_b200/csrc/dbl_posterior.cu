@@ -30,7 +30,8 @@
 // (s, label in C_t, label in C_s) keys over the records in C_t's clusters of two or more -- see dbl_vi_cross.
 // On the same handle, the VI search (dbl_vi_search, same numbers as analysis_arrays.vi_search_rounds) and the cells of
 // any labelling with every held sample (dbl_vi_score, as analysis_arrays.vi_label_cells) share one cell pass over
-// radix-sorted (s, label in C_s, label in c) keys -- see vi_cell_batches.
+// radix-sorted (s, label in C_s, label in c) keys -- see vi_cell_batches; dbl_vi_score_samples keeps the cells of
+// each sample apart (as analysis_arrays.vi_sample_cells), for the credible ball around a point estimate.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -1441,6 +1442,31 @@ __global__ void k_cell_hist(int64_t ncell, const int32_t *__restrict__ cpos, uns
   }
 }
 
+// Per sample: each cell of n >= 2 records counted into G[s][n], s = s0 + (its first key >> hi_shift).  Cells are in key
+// order, sample then cluster, so a warp's cells mostly share a row and a small n; lanes with equal (s, n) are summed by
+// __match_any_sync and add once.
+__global__ void k_cell_rows(int64_t ncell, int hi_shift, const unsigned long long *__restrict__ key,
+                            const int32_t *__restrict__ cpos, int32_t s0, int64_t width,
+                            unsigned long long *__restrict__ G) {
+  const int lane = threadIdx.x & 31;
+  for (int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31); base < ncell;
+       base += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t c = base + lane;
+    int32_t m = 0;
+    int64_t s = 0;
+    if (c < ncell) {
+      const int32_t first = cpos[c];
+      m = cpos[c + 1] - first;
+      s = s0 + (int64_t)(key[first] >> hi_shift);
+    }
+    const unsigned emit = __ballot_sync(0xffffffffu, m >= 2);
+    if (m >= 2) {
+      const unsigned same = __match_any_sync(emit, (unsigned long long)s << 32 | (unsigned long long)(uint32_t)m);
+      if (lane == __ffs(same) - 1) atomicAdd(&G[s * width + m], (unsigned long long)__popc(same));
+    }
+  }
+}
+
 // sum over cells of F_q(n) into *out
 __global__ void k_cell_F(int64_t ncell, const int32_t *__restrict__ cpos, const long long *__restrict__ F,
                          unsigned long long *__restrict__ out) {
@@ -1565,8 +1591,8 @@ __global__ void k_vis_best_move(int64_t R, int lab_bits, int64_t n, const unsign
 // its key bits within 63.  Per sample the records in its clusters of two or more (flags, an exclusive scan, a scatter)
 // give one key each (k_vis_keys), so the key buffers hold the batch's keys and no more; the batch's (key, record) pairs
 // are radix-sorted, and the cells are their runs of equal keys: cell ranks (an inclusive scan of the heads) and cell
-// starts.  on_batch(n, ncell) sees the sorted keys in key.Current(), their records in rec.Current(), the ranks in
-// crank and the starts in cpos.
+// starts.  on_batch(s0, n, ncell) sees the batch's first sample s0, the sorted keys in key.Current(), their records in
+// rec.Current(), the ranks in crank and the starts in cpos.
 struct CellPass {
   Buf key[2], rec[2], head, crank, cpos, flag, pos, sel, tmp;
   cub::DoubleBuffer<unsigned long long> kb;
@@ -1621,6 +1647,7 @@ int vi_cell_batches(dbl_vi *p, const int32_t *L, int64_t SampleStats::*weight, C
       n += nsel;
     }
     POST_TRY(cudaGetLastError());
+    const int32_t first = s0;
     s0 = s1;
     if (n == 0) continue;  // every sample of the batch is all singletons: every cell with them is a singleton
     const int end_bit = 2 * b + bits_for(B);
@@ -1641,7 +1668,7 @@ int vi_cell_batches(dbl_vi *p, const int32_t *L, int64_t SampleStats::*weight, C
     POST_TRY(cudaMemcpyAsync(&ncell, c.crank.as<int32_t>() + n - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     POST_TRY(cudaGetLastError());
     POST_TRY(cudaStreamSynchronize(st));
-    if (const int rc = on_batch(n, (int64_t)ncell); rc != DBL_OK) return rc;
+    if (const int rc = on_batch(first, n, (int64_t)ncell); rc != DBL_OK) return rc;
   }
   return DBL_OK;
 }
@@ -1660,10 +1687,39 @@ extern "C" int dbl_vi_score(dbl_vi *p, const int32_t *labels, int64_t width, int
   CellPass c;
   POST_TRY(G.alloc(gbytes));
   POST_TRY(cudaMemsetAsync(G.p, 0, gbytes, st));
-  const int rc = vi_cell_batches(p, p->cluster.as<int32_t>(), &SampleStats::keys, c, [&](int64_t, int64_t ncell) {
+  const int rc = vi_cell_batches(p, p->cluster.as<int32_t>(), &SampleStats::keys, c, [&](int32_t, int64_t, int64_t ncell) {
     k_cell_hist<<<grid_for(ncell), THREADS, 0, st>>>(ncell, c.cpos.as<int32_t>(), G.as<unsigned long long>());
     return DBL_OK;
   });
+  if (rc != DBL_OK) return rc;
+  POST_TRY(cudaMemcpyAsync(G_out, G.p, gbytes, cudaMemcpyDefault, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
+// G[s][n] = the cells of n >= 2 records of labels ^ C_s, one row per held sample: the score's cell pass, each batch's
+// cells counted into the rows of their samples (k_cell_rows).
+extern "C" int dbl_vi_score_samples(dbl_vi *p, const int32_t *labels, int64_t width, int64_t *G_out) {
+  if (!p || !labels || !G_out) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  if (width < (int64_t)p->max_size + 1 || width > INT64_MAX / 8 / p->S) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(labels, p->cluster); rc != DBL_OK) return rc;
+  cudaStream_t st = p->stream;
+  const int hi_shift = 2 * p->lab_bits;
+  const size_t gbytes = sizeof(unsigned long long) * (size_t)p->S * (size_t)width;
+  Buf G;
+  CellPass c;
+  POST_TRY(G.alloc(gbytes));
+  POST_TRY(cudaMemsetAsync(G.p, 0, gbytes, st));
+  const int rc = vi_cell_batches(p, p->cluster.as<int32_t>(), &SampleStats::keys, c,
+                                 [&](int32_t s0, int64_t, int64_t ncell) {
+                                   k_cell_rows<<<grid_for(ncell), THREADS, 0, st>>>(
+                                       ncell, hi_shift, c.kb.Current(), c.cpos.as<int32_t>(), s0, width,
+                                       G.as<unsigned long long>());
+                                   return DBL_OK;
+                                 });
   if (rc != DBL_OK) return rc;
   POST_TRY(cudaMemcpyAsync(G_out, G.p, gbytes, cudaMemcpyDefault, st));
   POST_TRY(cudaGetLastError());
@@ -1761,7 +1817,7 @@ extern "C" int dbl_vi_search(dbl_vi *p, const int64_t *step, const int32_t *star
     int cur = 0;
     int64_t acc_n = 0;
     const bool first_round = rounds == 0;
-    const int rc = vi_cell_batches(p, L, &SampleStats::squares, c, [&](int64_t n, int64_t ncell) {
+    const int rc = vi_cell_batches(p, L, &SampleStats::squares, c, [&](int32_t, int64_t n, int64_t ncell) {
       if (first_round)
         k_cell_F<<<grid_for(ncell), THREADS, 0, st>>>(ncell, c.cpos.as<int32_t>(), F.as<long long>(), st8 + 6);
       POST_TRY(cnt.reserve(sizeof(long long) * (size_t)(n + 1)));

@@ -26,11 +26,16 @@ BINDER_SEARCH_METRICS = ("binder-search-pairwise", "binder-search-cluster")
 VI_METRICS = ("vi-pairwise", "vi-cluster")
 # the least expected variation of information found by single-record moves from the VI sample and from the sMPC
 VI_SEARCH_METRICS = ("vi-search-pairwise", "vi-search-cluster")
+# whether the ground truth lies in the credible ball around a point estimate, in VI and in Binder distance
+CREDIBLE_BALL_METRICS = ("credible-ball",)
 SUPPORTED_METRICS = (SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_SEARCH_METRICS + VI_METRICS
-                     + VI_SEARCH_METRICS)
+                     + VI_SEARCH_METRICS + CREDIBLE_BALL_METRICS)
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
-                        "binder-search-clusters", "vi-clusters", "vi-search-clusters")
+                        "binder-search-clusters", "vi-clusters", "vi-search-clusters", "credible-ball")
+# the point estimates a credible ball may be centred on
+CREDIBLE_BALL_CENTERS = ("shared-most-probable-clusters", "binder-clusters", "binder-search-clusters", "vi-clusters",
+                         "vi-search-clusters")
 
 
 def shared_most_probable_clusters(chain):
@@ -162,6 +167,89 @@ def vi_search_estimate(chain, max_rounds):
     return analysis_arrays.VI_SEARCH_STARTS[best], runs[best], rows, exact
 
 
+def credible_ball_center(chain, center, false_link_cost, max_rounds):
+    """The labels of the point estimate `center` (one of CREDIBLE_BALL_CENTERS) of a ChainArrays, computed as its own
+    summarize quantity computes it."""
+    if center == "shared-most-probable-clusters":
+        return shared_most_probable_clusters(chain)
+    if center == "binder-clusters":
+        return binder_estimate(chain, false_link_cost)[1]
+    if center == "binder-search-clusters":
+        return binder_search_estimate(chain, false_link_cost, max_rounds)[1].labels
+    if center == "vi-clusters":
+        return vi_estimate(chain)[1]
+    if center == "vi-search-clusters":
+        return vi_search_estimate(chain, max_rounds)[1].labels
+    raise ValueError(f"credibleBallCenter must be one of {CREDIBLE_BALL_CENTERS}.")
+
+
+def credible_ball_estimate(chain, center, level, false_link_cost, max_rounds):
+    """The credible ball of a ChainArrays around the estimate `center`: (its labels, every sample's number of clusters,
+    {"vi" | "binder": (every sample's distance from the center, radius, in-ball mask, bounds)}), the bounds as
+    analysis_arrays.credible_ball gives them.  The cells of the center with every sample come from one set of held
+    samples (GPU or host)."""
+    if not chain.samples:
+        raise ValueError("the credible ball needs at least one sample at or after lowerIterationCutoff")
+    R = chain.num_records
+    labels = np.asarray(credible_ball_center(chain, center, false_link_cost, max_rounds), np.int64)
+    width = analysis_arrays.vi_width(chain)
+    g = analysis_arrays.vi_cluster_histograms(chain, width)
+    with vi_samples(chain) as vi:
+        G = vi.score_samples(labels, width)
+    distances = analysis_arrays.credible_ball_distances(np.bincount(np.bincount(labels)), g, G, R)
+    num_clusters = np.array([len(off) - 1 for _, off, _ in chain.samples], np.int64)
+    balls = {name: (d,) + analysis_arrays.credible_ball(d, num_clusters, level)
+             for name, d in zip(analysis_arrays.CREDIBLE_BALL_DISTANCES, distances)}
+    return labels, num_clusters, balls
+
+
+def credible_ball_truth(labels, truth):
+    """(VI, Binder distance) of the ground truth from the labelling `labels`: one contingency table of the two, through
+    analysis_arrays.credible_ball_distances."""
+    labels, truth = np.asarray(labels, np.int64), np.unique(np.asarray(truth), return_inverse=True)[1].astype(np.int64)
+    R = len(labels)
+    _, n = np.unique(labels * max(R, 1) + truth, return_counts=True)
+    sizes = np.bincount(np.bincount(truth))
+    cells = np.bincount(n[n >= 2], minlength=len(sizes))
+    vi, binder = analysis_arrays.credible_ball_distances(np.bincount(np.bincount(labels)), sizes[None, :],
+                                                         cells[None, :], R)
+    return float(vi[0]), int(binder[0])
+
+
+def _credible_ball_rows(chain, center, level, balls):
+    """The rows of credible-ball.csv: per distance and bound, (distance, bound, center, level, radius, samples in the
+    ball, samples, chain, iteration, clusters, distance to the center, ties) of the bound's sample."""
+    rows = []
+    S = len(chain.samples)
+    for name, (d, radius, inside, bounds) in balls.items():
+        for bound in analysis_arrays.CREDIBLE_BALL_BOUNDS:
+            s, ties = bounds[bound]
+            rows.append((name, bound, center, level, radius, int(inside.sum()), S, int(chain.chains[s]),
+                         int(chain.iterations[s]), len(chain.samples[s][1]) - 1, d[s].item(), ties))
+    return rows
+
+
+def _credible_ball_settings(prm):
+    """The settings a credible ball's center is computed with, for run.txt."""
+    center = prm["credible_ball_center"]
+    out = f"credibleBallCenter={center}"
+    if center.startswith("binder"):
+        out += f", falseLinkCost={prm['false_link_cost']}"
+    if center.endswith("search-clusters"):
+        out += f", maxSearchRounds={prm['max_search_rounds']}"
+    return out + f", credibleLevel={prm['credible_level']}"
+
+
+def _credible_ball_params(prm):
+    center = prm.get("credibleBallCenter", "vi-search-clusters")
+    if center not in CREDIBLE_BALL_CENTERS:
+        raise ValueError(f"credibleBallCenter must be one of {CREDIBLE_BALL_CENTERS}.")
+    level = prm.get("credibleLevel", 0.95)
+    if isinstance(level, bool) or not isinstance(level, (int, float)) or not 0.0 < float(level) <= 1.0:
+        raise ValueError("credibleLevel must be in (0, 1].")
+    return dict(credible_ball_center=center, credible_level=float(level))
+
+
 def _searched_cost(false_link_cost):
     a, b = analysis_arrays.search_cost(false_link_cost)
     return a / b
@@ -290,6 +378,10 @@ class Project:
                     L.append(f"  * SummarizeStep: vi-search-clusters is the least posterior expected variation of "
                              f"information found by single-record moves from the VI sample and the sMPC, with "
                              f"maxSearchRounds={prm['max_search_rounds']}")
+                if "credible-ball" in prm["quantities"]:
+                    L.append(f"  * SummarizeStep: credible-ball is the smallest ball around a point estimate, in "
+                             f"variation of information and in Binder distance, that holds a share of the samples, "
+                             f"with {_credible_ball_settings(prm)}")
             elif name == "evaluate":
                 smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
                 post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
@@ -323,6 +415,11 @@ class Project:
                              f"found by single-record moves from the VI sample and the sMPC (maxSearchRounds="
                              f"{prm['max_search_rounds']}, iterations >= {prm['lower_iteration_cutoff']}) using "
                              f"{braces(vi_search)} metrics")
+                ball = [m for m in prm["metrics"] if m in CREDIBLE_BALL_METRICS]
+                if ball:
+                    L.append(f"  * EvaluateStep: Evaluating whether the ground truth lies in the credible ball around a "
+                             f"point estimate ({_credible_ball_settings(prm)}, iterations >= "
+                             f"{prm['lower_iteration_cutoff']}) using {braces(ball)} metrics")
             else:
                 L.append("  * CopyFilesStep: Copying {" + ", ".join(prm["file_names"]) + "} to destination "
                          + prm["destination_path"])
@@ -464,7 +561,8 @@ class Project:
                 out.append(("summarize", dict(lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)),
                                               quantities=q, min_match_probability=t,
                                               false_link_cost=_false_link_cost(prm),
-                                              max_search_rounds=_max_search_rounds(prm))))
+                                              max_search_rounds=_max_search_rounds(prm),
+                                              **_credible_ball_params(prm))))
             elif name == "evaluate":
                 m = list(prm["metrics"])
                 if not m or any(x not in SUPPORTED_METRICS for x in m):
@@ -472,7 +570,8 @@ class Project:
                 out.append(("evaluate", dict(lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)), metrics=m,
                                              use_existing_smpc=bool(prm.get("useExistingSMPC", False)),
                                              false_link_cost=_false_link_cost(prm),
-                                             max_search_rounds=_max_search_rounds(prm))))
+                                             max_search_rounds=_max_search_rounds(prm),
+                                             **_credible_ball_params(prm))))
             elif name == "copy-files":
                 out.append(("copy-files", dict(file_names=list(prm["fileNames"]),
                                                destination_path=prm["destinationPath"],
@@ -539,6 +638,19 @@ class Project:
                         self._save_smpc(analysis_arrays.labels_to_clusters(run.labels, ch.record_ids),
                                         "vi-search-clusters.csv")
                         writers.save_vi_search(rows, self.output_path)
+                    elif q == "credible-ball":
+                        center, level = prm["credible_ball_center"], prm["credible_level"]
+                        _, num_clusters, balls = credible_ball_estimate(ch, center, level, prm["false_link_cost"],
+                                                                        prm["max_search_rounds"])
+                        writers.save_credible_ball_samples(ch.chains, ch.iterations, num_clusters, balls["vi"][0],
+                                                           balls["binder"][0], self.output_path)
+                        rows = _credible_ball_rows(ch, center, level, balls)
+                        writers.save_credible_ball(rows, self.output_path)
+                        for name, bound, *_ in rows:
+                            mem, off, _ = ch.samples[balls[name][3][bound][0]]
+                            self._save_smpc(analysis_arrays.labels_to_clusters(
+                                analysis_arrays.sample_labels(ch.num_records, mem, off), ch.record_ids),
+                                f"credible-ball-{name}-{bound}.csv")
                     else:
                         labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
@@ -625,6 +737,19 @@ class Project:
                         elif m == "vi-search-cluster":
                             results[m] = analysis_arrays.adjusted_rand_index(run.labels, truth)
                             text.append(analysis.format_vi_search_cluster(results[m], *at))
+                if any(m in CREDIBLE_BALL_METRICS for m in prm["metrics"]):
+                    ch = ch if ch is not None else self.read_chain(cut)
+                    center, level = prm["credible_ball_center"], prm["credible_level"]
+                    labels, _, balls = credible_ball_estimate(ch, center, level, prm["false_link_cost"],
+                                                              prm["max_search_rounds"])
+                    truth = credible_ball_truth(labels, true_labels(ch.record_ids))
+                    res = dict(center=center, level=level, samples=len(ch.samples))
+                    for name, t in zip(analysis_arrays.CREDIBLE_BALL_DISTANCES, truth):
+                        _, radius, inside, _ = balls[name]
+                        res[name] = dict(truthDistance=t, radius=radius, truthInBall=t <= radius,
+                                         samplesInBall=int(inside.sum()))
+                    results["credible-ball"] = res
+                    text.append(analysis.format_credible_ball(res))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
             elif name == "copy-files":

@@ -267,3 +267,29 @@ def save_vi_search(rows, path):
         fh.write(VI_SEARCH_HEADER + "\n")
         for start, r, moves, k, loss in rows:
             fh.write(f"{start},{int(r)},{int(moves)},{int(k)},{float(loss)!r}\n")
+
+
+CREDIBLE_BALL_SAMPLES_HEADER = "chain,iteration,numClusters,viDistance,binderDistance"
+
+
+def save_credible_ball_samples(chains, iterations, num_clusters, vi, binder, path):
+    """credible-ball-samples.csv under `path`: one row per sample in pooled order (chain-major, then iteration), its
+    number of clusters and its VI (written with repr) and Binder distance from the center of the ball."""
+    with open(os.path.join(path, "credible-ball-samples.csv"), "w") as fh:
+        fh.write(CREDIBLE_BALL_SAMPLES_HEADER + "\n")
+        for k, it, n, v, b in zip(chains, iterations, num_clusters, vi, binder):
+            fh.write(f"{int(k)},{int(it)},{int(n)},{float(v)!r},{int(b)}\n")
+
+
+CREDIBLE_BALL_HEADER = ("distance,bound,center,level,radius,samplesInBall,samples,chain,iteration,numClusters,"
+                        "distanceToCenter,ties")
+
+
+def save_credible_ball(rows, path):
+    """credible-ball.csv under `path`: rows (distance, bound, center, level, radius, samples in the ball, samples,
+    chain, iteration, clusters, distance to the center, ties) as project.py gives them, one per distance and bound;
+    floats written with repr."""
+    with open(os.path.join(path, "credible-ball.csv"), "w") as fh:
+        fh.write(CREDIBLE_BALL_HEADER + "\n")
+        for row in rows:
+            fh.write(",".join(repr(x) if isinstance(x, float) else str(x) for x in row) + "\n")

@@ -423,6 +423,15 @@ int dbl_eval_read(dbl_eval *, int64_t *tp, int64_t *pred_pairs, int64_t *num_clu
  *                      max(batch keys, one sample's), with no cap on cluster sizes.  Memory, the call's own: 8 width
  *                      bytes, 12 per record, 36 per key of the largest batch (at most max(batch keys, R)) and the
  *                      sorts' temporary storage.
+ *   dbl_vi_score_samples  the same cells kept per sample: G_out[s][n] (S x width int64, row-major, host or device) =
+ *                      the cells of n >= 2 records of c ^ C_s; G_out[s][0] = G_out[s][1] = 0, and row s sums to
+ *                      dbl_vi_score's G_out.  With g_x[n] = the clusters of n records of x and D_s[n] = g_c[n] + g_s[n]
+ *                      - 2 G_out[s][n], VI(c, C_s) = sum over n of D_s[n] n log2 n / R bits and the pairs one of c, C_s
+ *                      links and the other does not number sum over n of D_s[n] n (n - 1) / 2 -- the distances of a
+ *                      credible ball around c.  DBL_ERR_INVALID: a NULL pointer, width < M + 1, S width 8 bytes past
+ *                      INT64_MAX, a label outside [0, R).  The cell pass and its batches are dbl_vi_score's; each
+ *                      batch's cells are counted into the rows of their samples.  Memory, the call's own: 8 S width
+ *                      bytes plus that of dbl_vi_score.
  *   dbl_vi_search      single-record moves from the labelling start[R] (host or device pointer, labels in [0, R)) while
  *                      they lower J_q(c) = S sum over clusters X of F(|X|) - 2 sum_s sum over cells of c ^ C_s of F(n),
  *                      F(n) = step[0] + ... + step[n - 1].  step (R int64, host) is D_q[m] = round(2^20 (f(m + 1) -
@@ -447,9 +456,10 @@ int dbl_eval_read(dbl_eval *, int64_t *tp, int64_t *pred_pairs, int64_t *num_clu
  *                      call's own: 92 bytes per record, 52 per key of the largest batch (at most the batch's sum of
  *                      |K|^2), 32 per entry of the batch's contributions plus the running (record, cluster) table, and
  *                      the sorts' temporary storage.
- *   dbl_vi_score / dbl_vi_search before the first sample give DBL_ERR_STATE; neither changes the held samples.
+ *   dbl_vi_score, dbl_vi_score_samples and dbl_vi_search before the first sample give DBL_ERR_STATE; none changes the
+ *   held samples.
  * DBL_ERR_INVALID: num_records outside [1, 2^31 - 1] or max_samples < 1.  DBL_ERR_CUDA: no device, or the held label
- * matrix (or a buffer of dbl_vi_cross, dbl_vi_score or dbl_vi_search) does not fit on it.
+ * matrix (or a buffer of dbl_vi_cross, dbl_vi_score, dbl_vi_score_samples or dbl_vi_search) does not fit on it.
  * ------------------------------------------------------------------------------------------------- */
 typedef struct dbl_vi dbl_vi;
 int dbl_vi_create(dbl_vi **out, int64_t num_records, int32_t max_samples);
@@ -459,6 +469,8 @@ int32_t dbl_vi_num_samples(const dbl_vi *);
 int dbl_vi_set_batch_keys(dbl_vi *, int64_t max_keys);
 int dbl_vi_cross(dbl_vi *, int64_t width, int64_t *G_out /* S x width */);
 int dbl_vi_score(dbl_vi *, const int32_t *labels /* R, host or device */, int64_t width, int64_t *G_out /* width */);
+int dbl_vi_score_samples(dbl_vi *, const int32_t *labels /* R, host or device */, int64_t width,
+                         int64_t *G_out /* S x width */);
 int dbl_vi_search(dbl_vi *, const int64_t *step /* R, host */, const int32_t *start /* R, host or device */,
                   int32_t max_rounds, int32_t *labels_out /* R */, int32_t *rounds_out, int32_t *converged_out,
                   int64_t *moves, int64_t *clusters, int64_t *dJ /* max_rounds each, host */, int64_t *J0_out);
