@@ -1316,6 +1316,13 @@ __global__ void __launch_bounds__(256) k_state_hash(RowSet ents, RowSet recs, in
 // ---------------------------------------------------------------------------------------------------
 // host-side context
 // ---------------------------------------------------------------------------------------------------
+// cudaFree synchronises the whole device.  Several ranks may share one device, and while a sharded sweep is being
+// enqueued (the first one after a state of another size reallocates buffers) a peer's k_publish_barrier may already
+// spin, waiting for kernels this rank has not launched yet: the free would wait for the barrier and the barrier for
+// the free until it times out.  dbl_sweep_async of a sharded context parks the buffers it replaces here instead; the
+// context frees them when it enqueues no sweep (state upload, dbl_comm_export, destruction).
+static thread_local std::vector<void *> *t_deferred_free = nullptr;
+
 template <typename T>
 struct DevBuf {
   T *p = nullptr;
@@ -1325,7 +1332,13 @@ struct DevBuf {
     n = count;
     return cudaMalloc((void **)&p, std::max<size_t>(count, 1) * sizeof(T));
   }
-  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
+  void release() {
+    if (p) {
+      if (t_deferred_free) t_deferred_free->push_back(p);
+      else cudaFree(p);
+    }
+    p = nullptr; n = 0;
+  }
   ~DevBuf() { release(); }
 };
 
@@ -1506,6 +1519,11 @@ struct dbl_ctx {
     }
     graphs.clear();
     graph_warm.clear();
+  }
+  std::vector<void *> deferred_free;  // buffers a sharded sweep replaced (t_deferred_free)
+  void free_deferred() {
+    for (void *q : deferred_free) cudaFree(q);
+    deferred_free.clear();
   }
 
   void set_error(const std::string &s) { err = s; }
@@ -1757,6 +1775,7 @@ extern "C" void dbl_ctx_destroy(dbl_ctx *ctx) {
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
   comm_close(ctx);
   ctx->drop_graphs();
+  ctx->free_deferred();
   for (auto &pe : ctx->pending_events) for (cudaEvent_t e : pe.e) cudaEventDestroy(e);
   for (auto &pe : ctx->event_pool) for (cudaEvent_t e : pe.e) cudaEventDestroy(e);
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
@@ -2175,6 +2194,7 @@ static int state_init(dbl_ctx *ctx, int64_t R, const int32_t *x, const int32_t *
 extern "C" int dbl_state_init(dbl_ctx *ctx, int64_t R, const int32_t *x, const int32_t *file, int64_t pop) {
   if (!ctx || !x || !file) return DBL_ERR_INVALID;
   CUDA_TRY(cudaSetDevice(ctx->device));
+  ctx->free_deferred();
   int rc = set_chains(ctx, 1, nullptr);
   if (rc) return rc;
   return state_init(ctx, R, x, file, pop);
@@ -2218,6 +2238,7 @@ extern "C" int dbl_state_upload(dbl_ctx *ctx, int64_t R, int64_t E, const int32_
     return DBL_ERR_STATE;
   }
   CUDA_TRY(cudaSetDevice(ctx->device));
+  ctx->free_deferred();
   int rc = set_chains(ctx, 1, nullptr);
   if (rc) return rc;
   return state_upload(ctx, R, E, x, file, z, link, y, theta, iteration);
@@ -2471,6 +2492,9 @@ static int launch_link(dbl_ctx *ctx, int sampler) {
       CUDA_TRY(ctx->link_mass.alloc((size_t)ctx->R));
       CUDA_TRY(cudaMemsetAsync(ctx->link_mass.p, 0, sizeof(double) * (size_t)ctx->R, ctx->stream));
     }
+    // a shard scores only the records it owns; every other entry keeps the all-ones pattern, a NaN no kernel stores
+    if (ctx->world > 1)
+      CUDA_TRY(cudaMemsetAsync(ctx->link_mass.p, 0xFF, sizeof(double) * (size_t)ctx->R, ctx->stream));
     lp.link_mass = ctx->link_mass.p;
   }
   lp.hslots = ctx->hslots; lp.hshift = ctx->hshift;
@@ -2714,7 +2738,10 @@ extern "C" int dbl_sweep_async(dbl_ctx *ctx, int sampler, int32_t n_sweeps) {
   CUDA_TRY(cudaSetDevice(ctx->device));
   if (!ctx->async_open) CUDA_TRY(cudaEventRecord(ctx->ev0, ctx->stream));
   ctx->async_open = true;
-  return run_sweeps(ctx, sampler, n_sweeps);
+  t_deferred_free = ctx->world > 1 ? &ctx->deferred_free : nullptr;
+  rc = run_sweeps(ctx, sampler, n_sweeps);
+  t_deferred_free = nullptr;
+  return rc;
 }
 
 extern "C" int dbl_set_graph_mode(dbl_ctx *ctx, int mode) {
@@ -2908,6 +2935,7 @@ extern "C" int dbl_comm_export(dbl_ctx *ctx, void *blob_out) {
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   comm_close(ctx);
   ctx->drop_graphs();
+  ctx->free_deferred();
   CommDev &c = ctx->comm;
   memset(&c, 0, sizeof(c));
   c.rank = ctx->rank; c.world = ctx->world; c.A = ctx->A; c.nws = ctx->nw + 1;
@@ -3234,7 +3262,6 @@ extern "C" int dbl_set_link_mode(dbl_ctx *ctx, int mode) {
 
 extern "C" int dbl_set_link_mass_capture(dbl_ctx *ctx, int on) {
   if (!ctx) return DBL_ERR_INVALID;
-  if (ctx->world > 1) { ctx->set_error("link-mass capture needs an unsharded context"); return DBL_ERR_STATE; }
   ctx->drop_graphs();  // captured sweeps hold the link parameters by value
   ctx->link_mass_on = on != 0;
   if (!ctx->link_mass_on) ctx->link_mass.release();
@@ -3243,7 +3270,6 @@ extern "C" int dbl_set_link_mass_capture(dbl_ctx *ctx, int on) {
 
 extern "C" int dbl_link_mass(dbl_ctx *ctx, double *mass_out) {
   if (!ctx || !mass_out) return DBL_ERR_INVALID;
-  if (ctx->world > 1) { ctx->set_error("link-mass capture needs an unsharded context"); return DBL_ERR_STATE; }
   if (!ctx->has_state) { ctx->set_error("no state"); return DBL_ERR_STATE; }
   if (!ctx->link_mass_on || ctx->link_mass.n != (size_t)ctx->R) {
     ctx->set_error("dbl_link_mass: no sweep has run with the capture on (dbl_set_link_mass_capture)");

@@ -99,6 +99,22 @@ def merge_owned(parts, R, E, A):
     return {"y": y, "block": blk, "link": link, "z": z}
 
 
+LINK_MASS_UNSCORED = np.uint64(0xFFFFFFFFFFFFFFFF)  # dbl_link_mass on a shard: a record another rank scored
+
+
+def merge_link_mass(parts):
+    """R totals from the ranks' `dbl_link_mass` arrays, each holding the totals of the records its rank scored and
+    the all-ones bit pattern everywhere else.  Raises unless exactly one rank scored each record."""
+    bits = np.stack([np.asarray(p, np.float64).view(np.uint64) for p in parts])
+    scored = bits != LINK_MASS_UNSCORED
+    n = scored.sum(axis=0)
+    bad = np.flatnonzero(n != 1)
+    if bad.size:
+        raise RuntimeError(f"link masses: {bad.size} records not scored by exactly one rank "
+                           f"(record {bad[0]}: {n[bad[0]]} ranks)")
+    return bits[scored.argmax(axis=0), np.arange(bits.shape[1])].view(np.float64)
+
+
 def sum_hashes(dist, he, hr, device, torch):
     """Sum of the ranks' row fingerprints mod 2^64 (two's-complement int64 addition wraps the same way)."""
     t = torch.from_numpy(np.array([he, hr], np.uint64).view(np.int64).copy()).to(device)
@@ -434,11 +450,16 @@ class LocalShards:
         self.set_owners(owner)
         self.connect()
 
-    def upload_state(self, x, file_ids, z, link, y, theta, iteration=0):
-        owner = self.block_owners()
+    def upload_state(self, x, file_ids, z, link, y, theta, iteration=0, owner=None):
+        """owner = the block -> rank table to carve the shards with (default: the current one).  A state of another
+        shape closes the communication buffers (they are sized by the state): the ranks connect again."""
+        owner = self.block_owners() if owner is None else owner
         for e in self.engines:
             e.upload_state(x, file_ids, z, link, y, theta, iteration)
         self.set_owners(owner)
+        e0 = self.engines[0]
+        if (e0.num_records, e0.num_entities) != self._connected_shape:
+            self.connect()
 
     def set_owners(self, owner):
         owner = np.ascontiguousarray(owner, dtype=np.int32)
@@ -464,9 +485,19 @@ class LocalShards:
             blobs += bytes(blob)
         for e in self.engines:
             _check(L.dbl_comm_import(e._h, blobs, self.world), "comm_import", e._h)
+        self._connected_shape = (self.engines[0].num_records, self.engines[0].num_entities)
 
     def sweep(self, sampler="PCG-I", n=1):
         self._each(lambda r, e: e.sweep(sampler, n))
+
+    def set_link_mass_capture(self, on=True):
+        """Checking aid: every rank's link kernels store the total mass of each record they score."""
+        for e in self.engines:
+            e.set_link_mass_capture(on)
+
+    def link_mass(self):
+        """float64[R]: the total mass of each record's link categorical in the last sweep, from the rank that scored it."""
+        return merge_link_mass([e.link_mass() for e in self.engines])
 
     @property
     def iteration(self):

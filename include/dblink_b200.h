@@ -249,6 +249,8 @@ int dbl_state_hash(dbl_ctx *, uint64_t *hash_out /*2*/);
  *                     (CUDA IPC handle); the host layer all-gathers the blobs with whatever it has (sockets, MPI,
  *                     torch.distributed, Spark's driver) -- this is the only thing it ever moves
  *   dbl_comm_import   maps every peer's buffer over NVLink / NVSwitch
+ *   The receive buffers are sized by the state at dbl_comm_export: a state of another shape (other R or E) closes
+ *   them, and dbl_sweep returns DBL_ERR_STATE until every rank has exported and imported again.
  *   dbl_sweep / dbl_sweep_async then run the whole transition on the device: clusters whose new block belongs to
  *   another rank are written straight into that rank's receive buffer by the kernel that finds them, the partial
  *   summaries go into a slot of every peer, one flag barrier per sweep, theta is drawn redundantly on every rank.
@@ -499,7 +501,9 @@ int dbl_link_kernel(const dbl_ctx *, int sampler);
  * mass of each record's categorical -- the sum of its protocol weights over the block, the number the draw tests for
  * zero / non-finite -- into a device array of R entries, from the link phase of the sweep that ran last.  Toggling
  * drops captured sweep graphs.  dbl_link_mass copies the R totals (record order) to the host; DBL_ERR_STATE before a
- * sweep with the capture on.  Both return DBL_ERR_STATE on a sharded context. */
+ * sweep with the capture on.  On a sharded context the array keeps its R global entries: before each sweep's link
+ * phase it is filled with the all-ones bit pattern (a NaN no kernel stores), so afterwards a rank holds the totals
+ * of the records it scored and that pattern everywhere else; exactly one rank scores each record. */
 int dbl_set_link_mass_capture(dbl_ctx *, int on);
 int dbl_link_mass(dbl_ctx *, double *mass_out /*R*/);
 /* How dbl_sweep / dbl_sweep_async enqueue several sweeps: 0 = automatic (problems small enough to be bound by kernel

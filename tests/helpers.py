@@ -48,13 +48,20 @@ def oracle_setup(O, g, seed, levels=0, attr_ids=(), pop=0, kmax=10):
     x, file, F = encode(idx, g)
     alpha = [a.alpha for a in g["attributes"]]
     beta = [a.beta for a in g["attributes"]]
+    m, s, tree = oracle_model_setup(O, idx, alpha, beta, seed, F, x, file, levels, attr_ids, pop)
+    return m, s, tree, x, file
+
+
+def oracle_model_setup(O, idx, alpha, beta, seed, F, x, file, levels=0, attr_ids=(), pop=0):
+    """oracle_setup from oracle indexes and encoded records: the k-d tree is fitted on the initial state, as the
+    product's engines and shards fit theirs -> (model_with_tree, state at iteration 0, tree)"""
     m0 = O.Model(idx, alpha, beta, None, seed, F)
     s0 = O.State.init(m0, x, file, pop)
     tree = O.KDTree.fit(s0.y, levels, list(attr_ids))
     m = O.Model(idx, alpha, beta, tree, seed, F)
     s = O.State.from_arrays(m, x, file, s0.z, s0.link, s0.y, s0.theta, 0)
     s._keep = (m0, s0)
-    return m, s, tree, x, file
+    return m, s, tree
 
 
 def product_setup(g, seed, levels=0, attr_ids=(), pop=0, kmax=10):

@@ -36,6 +36,31 @@ def test_lpt_assign():
     assert lpt_assign([], 4).shape == (0,)
 
 
+def test_merge_link_mass():
+    """each record's total comes from the one rank that scored it; a record scored by no rank or by two is refused"""
+    import numpy as np
+
+    from dblink_b200.distributed import LINK_MASS_UNSCORED, merge_link_mass
+
+    want = np.array([0.5, 3.0, 1e-300, 0.0, np.inf, 7.25])
+    owner = np.array([0, 2, 1, 1, 0, 2])
+    unscored = np.full(len(want), LINK_MASS_UNSCORED).view(np.float64)
+    parts = [np.where(owner == r, want, unscored) for r in range(3)]
+    got = merge_link_mass(parts)
+    assert (got.view(np.uint64) == want.view(np.uint64)).all()
+    # a NaN a kernel stores is a total, not the marker of a record another rank scored
+    parts[0][0] = np.nan
+    assert np.isnan(merge_link_mass(parts)[0])
+    lost = [p.copy() for p in parts]
+    lost[1][2] = unscored[0]
+    with pytest.raises(RuntimeError, match="1 records"):
+        merge_link_mass(lost)
+    twice = [p.copy() for p in parts]
+    twice[0][3] = 2.0
+    with pytest.raises(RuntimeError, match="record 3: 2 ranks"):
+        merge_link_mass(twice)
+
+
 @pytest.mark.gpu
 def test_sharded_chain_matches_oracle():
     import torch

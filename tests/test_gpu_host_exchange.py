@@ -16,16 +16,20 @@ pytestmark = pytest.mark.gpu
 
 def make(world, g, seed, levels, split):
     import dblink_b200 as D
-    from dblink_b200 import _lib
-    from dblink_b200.distributed import lpt_assign
-    from dblink_b200.engine import _check, _p
 
     rc = D.RecordsCache.build(g["values"], g["files"], g["attributes"])
     x, file = rc.transform_records(g["values"], g["files"])
     alpha = [a.alpha for a in g["attributes"]]
     beta = [a.beta for a in g["attributes"]]
-    engines = [D.GibbsEngine(rc.indexes, alpha, beta, None, seed, len(rc.file_ids), rank=r, world_size=world)
-               for r in range(world)]
+    return make_engines(world, rc.indexes, alpha, beta, seed, len(rc.file_ids), x, file, levels, split), x, file
+
+
+def make_engines(world, indexes, alpha, beta, seed, F, x, file, levels, split):
+    """One context per rank from the initial state of the records, k-d blocks fitted on it, placed by LPT."""
+    import dblink_b200 as D
+    from dblink_b200.distributed import lpt_assign
+
+    engines = [D.GibbsEngine(indexes, alpha, beta, None, seed, F, rank=r, world_size=world) for r in range(world)]
     for e in engines:
         e.init_state(x, file)
     y0 = engines[0].download_state()["y"]
@@ -34,10 +38,17 @@ def make(world, g, seed, levels, split):
     link, blk = engines[0].links()
     P = engines[0].num_partitions
     cost = np.bincount(blk, minlength=P).astype(np.float64) * np.bincount(blk[link], minlength=P)
-    owner = np.ascontiguousarray(lpt_assign(cost, world), dtype=np.int32)
+    set_owners(engines, lpt_assign(cost, world))
+    return engines
+
+
+def set_owners(engines, owner):
+    from dblink_b200 import _lib
+    from dblink_b200.engine import _check, _p
+
+    owner = np.ascontiguousarray(owner, dtype=np.int32)
     for e in engines:
         _check(_lib.load().dbl_set_block_owners(e._h, _p(owner, _lib.i32p)), "set_block_owners", e._h)
-    return engines, x, file
 
 
 def host_sweep(engines, sampler):

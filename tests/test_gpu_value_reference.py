@@ -51,10 +51,13 @@ def test_index_tables_device_host_and_oracle(oracle, monkeypatch, similarity):
                     np.testing.assert_array_equal(host[k], getattr(ix, k), err_msg=f"{what} {k} (oracle)")
 
 
-def crafted_setup(oracle, pad=0, sizes=None, seeds=(99,)):
+def crafted_setup(oracle, pad=0, sizes=None, seeds=(99,), initial_tree=False):
     """engine + oracle models of the crafted attributes and a state holding every crafted cluster; pad isolated
-    entities whose constant value (t) puts them in a block of their own"""
+    entities whose constant value (t) puts them in a block of their own.  initial_tree: fit the k-d tree on the
+    initial state of the records instead (as sharded chains do; the pad entities then share a block with clusters)"""
     import dblink_b200 as D
+
+    from helpers import oracle_model_setup
 
     specs, picks = crafted_specs(oracle)
     kw = {} if sizes is None else {"sizes": sizes}
@@ -68,9 +71,16 @@ def crafted_setup(oracle, pad=0, sizes=None, seeds=(99,)):
     oix = [oracle.Index.build(vw, const, 7.0, 10.0, kmax) for vw, const, kmax in specs]
     dix = [D.AttributeIndex.build(vw, "constant" if const else "levenshtein", 7.0, 10.0, kmax)
            for vw, const, kmax in specs]
-    tree = oracle.KDTree.fit(y, 1, [3])
-    part = D.KDTreePartitioner(1, [3]).fit(y)
-    models = [oracle.Model(oix, [1.0] * A, [4.0] * A, tree, s, F) for s in seeds]
+    if initial_tree:
+        setups = [oracle_model_setup(oracle, oix, [1.0] * A, [4.0] * A, s, F, x, file, 1, [3]) for s in seeds]
+        models = [m for m, _, _ in setups]
+        for m, s0, _ in setups:
+            m._keep = s0
+        part = D.KDTreePartitioner(1, [3]).fit(setups[0][1].y)
+    else:
+        tree = oracle.KDTree.fit(y, 1, [3])
+        part = D.KDTreePartitioner(1, [3]).fit(y)
+        models = [oracle.Model(oix, [1.0] * A, [4.0] * A, tree, s, F) for s in seeds]
     return dix, part, models, (x, file, z, link, y, theta), info
 
 
