@@ -153,6 +153,11 @@ SIGNATURES = {
     "dbl_vi_score": (C.c_int, [vp, vp, C.c_int64, vp]),
     "dbl_vi_score_samples": (C.c_int, [vp, vp, C.c_int64, vp]),
     "dbl_vi_search": (C.c_int, [vp, i64p, vp, C.c_int32, vp, i32p, i32p, i64p, i64p, i64p, i64p]),
+    "dbl_values_create": (C.c_int, [C.POINTER(vp), C.c_int64, vp, C.c_int32, C.c_int32]),
+    "dbl_values_free": (None, [vp]),
+    "dbl_values_add_sample": (C.c_int, [vp, vp]),
+    "dbl_values_num_samples": (C.c_int32, [vp]),
+    "dbl_values_modes": (C.c_int, [vp, vp, vp]),
     "dbl_version": (C.c_char_p, []),
 }
 

@@ -9,6 +9,8 @@
   vi_search                                               <- single-record moves that lower the quantised expected
                                                              variation of information
   credible_ball                                           <- the samples within a VI or Binder radius of an estimate
+  entity_value_counts / entity_value_modes                <- the posterior of the entity values of an estimate's
+                                                             clusters
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
   pairwise_metrics                                        <- analysis/PairwiseMetrics.scala:44-63,
                                                              BinaryClassificationMetrics.scala:23-37
@@ -521,3 +523,29 @@ def format_posterior_cluster(summary, num_samples, true_num_clusters):
 
 def is_nan(x):
     return isinstance(x, float) and math.isnan(x)
+
+
+def entity_value_counts(chain, values, center):
+    """The entity-value counts of the point estimate `center` (a list of sets of record ids; cluster k = center[k]),
+    restated with dicts: chain = [(iteration, {partition: [cluster of ids]})], values[s][a] = {frozenset of a cluster
+    of sample s: the value of its entity for attribute a}.  Returns {(k, a, v): the number of (sample, record of
+    center[k]) whose entity has value v}."""
+    counts = collections.Counter()
+    for (_, parts), vals in zip(chain, values):
+        where = {r: frozenset(c) for cl in parts.values() for c in cl for r in c}
+        for k, c in enumerate(center):
+            for a, va in enumerate(vals):
+                for r in c:
+                    counts[(k, a, va[where[r]])] += 1
+    return dict(counts)
+
+
+def entity_value_modes(counts, num_clusters, num_attributes):
+    """{(k, a): (mode, count)} from entity_value_counts: the value of largest count, ties to the smallest value."""
+    out = {}
+    for (k, a, v), n in counts.items():
+        best = out.get((k, a))
+        if best is None or n > best[1] or (n == best[1] and v < best[0]):
+            out[(k, a)] = (v, n)
+    assert len(out) == num_clusters * num_attributes
+    return out

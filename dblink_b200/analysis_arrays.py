@@ -26,6 +26,22 @@ class ChainArrays:
         return len(self.record_ids)
 
 
+def chain_files(path):
+    """(partition id, file name, file path) of every file of a chain written hive-partitioned by partitionId, in the
+    order the readers take them: partitionId= directories sorted by name (as strings, so 10 comes before 2), then
+    their files by name."""
+    for d in sorted(os.listdir(path)):
+        if not d.startswith("partitionId="):
+            continue
+        for f in sorted(os.listdir(os.path.join(path, d))):
+            yield int(d.split("=")[1]), f, os.path.join(path, d, f)
+
+
+def kept_clusters(sizes):
+    """The clusters of a linkage-chain row that a ChainArrays sample keeps: the non-empty ones."""
+    return np.asarray(sizes) > 0
+
+
 def read_chain_arrays(path, lower_iteration_cutoff=0):
     """linkage-chain.parquet (hive-partitioned by partitionId) -> ChainArrays, through Arrow only."""
     import pyarrow as pa
@@ -33,17 +49,13 @@ def read_chain_arrays(path, lower_iteration_cutoff=0):
     import pyarrow.parquet as pq
 
     rows = {}  # iteration -> list of (pid, ListArray of clusters)
-    for d in sorted(os.listdir(path)):
-        if not d.startswith("partitionId="):
-            continue
-        pid = int(d.split("=")[1])
-        for f in sorted(os.listdir(os.path.join(path, d))):
-            t = pq.ParquetFile(os.path.join(path, d, f)).read()
-            its = t.column("iteration").to_numpy()
-            ls = t.column("linkageStructure").combine_chunks()
-            for i, it in enumerate(its):
-                if it >= lower_iteration_cutoff:
-                    rows.setdefault(int(it), []).append((pid, ls[i].values))  # list<string> of that row
+    for pid, _, f in chain_files(path):
+        t = pq.ParquetFile(f).read()
+        its = t.column("iteration").to_numpy()
+        ls = t.column("linkageStructure").combine_chunks()
+        for i, it in enumerate(its):
+            if it >= lower_iteration_cutoff:
+                rows.setdefault(int(it), []).append((pid, ls[i].values))  # list<string> of that row
     its = sorted(rows)
     if not its:
         return ChainArrays(pa.array([], pa.string()), np.zeros(0, np.int64), [])
@@ -63,7 +75,7 @@ def read_chain_arrays(path, lower_iteration_cutoff=0):
             sizes.append(sz)
             part.append(np.full(len(sz), pid, np.int32))
         sizes = np.concatenate(sizes) if sizes else np.zeros(0, np.int64)
-        keep = sizes > 0
+        keep = kept_clusters(sizes)
         samples.append((np.concatenate(mem) if mem else np.zeros(0, np.int32),
                         np.r_[0, np.cumsum(sizes[keep])].astype(np.int64),
                         (np.concatenate(part) if part else np.zeros(0, np.int32))[keep]))
@@ -982,3 +994,201 @@ def posterior_summary(rows):
                   "q025": float(q[0]), "median": float(q[1]), "q975": float(q[2]),
                   "n": len(d), "undefined": len(v) - len(d)}
     return out
+
+
+# ---- the posterior of the entity values of a point estimate's clusters ------------------------------------------
+# For a point estimate with clusters c (canonical labels 0 .. C-1), a matching attribute and its value v:
+#   count(c, v) = sum over samples s and records r of c of 1[y_s(link_s(r)) = v]
+# so count / (|c| S) is the probability that the entity a uniformly chosen record of c links to has value v, and the
+# counts of c sum to |c| S.  The mode of c is the v of largest count, ties going to the smallest value id (the first
+# value in byte order).
+ENTITY_VALUES_CHAIN = "entity-values-chain.parquet"
+
+
+def _no_entity_values(iteration):
+    return ValueError(f"the sample at iteration {iteration} has no entity values (it was recorded with "
+                      f"saveEntityValues off): raise lowerIterationCutoff past it, or sample again with "
+                      f"saveEntityValues on")
+
+
+def _entity_value_index(chain_dir):
+    """iteration -> the name of the files of entity-values-chain.parquet under chain_dir holding it."""
+    import pyarrow.parquet as pq
+
+    path = os.path.join(chain_dir, ENTITY_VALUES_CHAIN)
+    index = {}
+    if os.path.isdir(path):
+        for _, name, f in chain_files(path):
+            for it in pq.read_table(f, columns=["iteration"]).column("iteration").to_numpy():
+                index.setdefault(int(it), name)
+    return index
+
+
+def _entity_value_group(chain_dir, name, attribute_names):
+    """The rows of the files called `name` of a chain directory, one flush of its two writers: (the cluster sizes of
+    each linkage row, the attribute value lists of each entity-values row), both keyed by (iteration, partition id)
+    and in chain_files order."""
+    import pyarrow.parquet as pq
+
+    sizes, values = {}, {}
+    for pid, f_name, f in chain_files(os.path.join(chain_dir, "linkage-chain.parquet")):
+        if f_name == name:
+            t = pq.ParquetFile(f).read()
+            ls = t.column("linkageStructure").combine_chunks()
+            for i, it in enumerate(t.column("iteration").to_numpy()):
+                sizes[(int(it), pid)] = np.diff(ls[i].values.offsets.to_numpy())
+    for pid, f_name, f in chain_files(os.path.join(chain_dir, ENTITY_VALUES_CHAIN)):
+        if f_name == name:
+            t = pq.ParquetFile(f).read()
+            cols = [t.column(a).combine_chunks() for a in attribute_names]
+            for i, it in enumerate(t.column("iteration").to_numpy()):
+                values[(int(it), pid)] = [c[i].values for c in cols]
+    return sizes, values
+
+
+def read_entity_values(chain_dirs, chain, attribute_names, attribute_values):
+    """Yields, for every sample of `chain` in order, int32[A][R]: the value id, per matching attribute, of the entity
+    each record links to.  chain = read_chain_arrays of chain_dirs[0]'s linkage chain, or read_pooled_chain_arrays of
+    every chain directory's (chain.chains[s] = the directory of sample s).  The values come from each directory's
+    entity-values-chain.parquet, walked as read_chain_arrays walks the linkage chain (chain_files) with the same kept
+    clusters; attribute_values[a] = the pyarrow string array of attribute a's values in value-id order.  One flush of
+    files is read at a time, so no more than a write buffer of samples is held.  Raises ValueError for a row whose
+    lists do not have one entry per cluster of its linkage row, a value the attribute lacks, or a sample without
+    entity values."""
+    import pyarrow as pa
+    import pyarrow.compute as pc
+
+    A, R = len(attribute_names), chain.num_records
+    indexes, loaded, group = {}, None, None
+    for s, (it, k) in enumerate(zip(chain.iterations, chain.chains)):
+        it, k = int(it), int(k)
+        if k not in indexes:
+            indexes[k] = _entity_value_index(chain_dirs[k])
+        name = indexes[k].get(it)
+        if name is None:
+            raise _no_entity_values(it)
+        if loaded != (k, name):
+            loaded, group = (k, name), _entity_value_group(chain_dirs[k], name, attribute_names)
+        sizes, values = group
+        mem, off, _ = chain.samples[s]
+        cols = [[] for _ in range(A)]
+        rows_of = [key for key in sizes if key[0] == it]
+        if {key for key in values if key[0] == it} != set(rows_of):
+            # files of one name that are not one flush of the two writers, e.g. values left by another chain
+            raise ValueError(f"entity-values-chain.parquet, iteration {it}, files {name}: the partitions do not match "
+                             f"those of linkage-chain.parquet")
+        for key in rows_of:
+            row = values[key]
+            if any(len(v) != len(sizes[key]) for v in row):
+                raise ValueError(f"entity-values-chain.parquet, iteration {it}, partition {key[1]}: the value lists "
+                                 f"do not have one entry per cluster of the linkage row ({len(sizes[key])})")
+            keep = pa.array(kept_clusters(sizes[key]))
+            for a in range(A):
+                cols[a].append(row[a].filter(keep))
+        out = np.empty((A, R), np.int32)
+        for a in range(A):
+            got = pa.concat_arrays(cols[a]) if cols[a] else pa.array([], pa.string())
+            if len(got) != len(off) - 1:
+                raise ValueError(f"entity-values-chain.parquet, iteration {it}: {len(got)} values of "
+                                 f"'{attribute_names[a]}' for {len(off) - 1} clusters")
+            ids = pc.index_in(got, value_set=attribute_values[a])
+            if ids.null_count:
+                bad = got.filter(pc.is_null(ids))[0].as_py()
+                raise ValueError(f"entity-values-chain.parquet, iteration {it}: '{attribute_names[a]}' has the value "
+                                 f"{bad!r}, which its index lacks")
+            out[a, mem] = np.repeat(ids.to_numpy(zero_copy_only=False).astype(np.int32), np.diff(off))
+        yield out
+
+
+class EntityValueCounts:
+    """count(c, v) of one attribute over the samples added, for the clusters of labels[R] in [0, C): the integers of
+    the dbl_values handle (analysis_gpu.EntityValues), held as a sorted table of keys c V + v and int64 counts."""
+
+    def __init__(self, labels, num_clusters, num_values):
+        self.labels = np.asarray(labels, np.int64)
+        self.num_clusters, self.num_values = int(num_clusters), int(num_values)
+        if len(self.labels) and (self.labels.min() < 0 or self.labels.max() >= self.num_clusters):
+            raise ValueError("a cluster label outside [0, num_clusters)")
+        self.keys, self.counts = np.zeros(0, np.int64), np.zeros(0, np.int64)
+        self.num_samples = 0
+
+    def add_sample(self, values):
+        values = np.asarray(values, np.int64)
+        if values.shape != self.labels.shape:
+            raise ValueError("a sample needs one value per record")
+        if len(values) and (values.min() < 0 or values.max() >= self.num_values):
+            raise ValueError("a value outside [0, num_values)")
+        k, n = np.unique(self.labels * self.num_values + values, return_counts=True)
+        self.keys, inv = np.unique(np.r_[self.keys, k], return_inverse=True)
+        counts = np.zeros(len(self.keys), np.int64)
+        np.add.at(counts, inv, np.r_[self.counts, n.astype(np.int64)])
+        self.counts = counts
+        self.num_samples += 1
+
+    def table(self):
+        """(cluster, value, count), int64, in ascending (cluster, value) order."""
+        return self.keys // self.num_values, self.keys % self.num_values, self.counts.copy()
+
+    def modes(self):
+        """(mode int32[C], count int64[C]): per cluster the value of largest count, ties to the smallest value; -1
+        and 0 for a label no record has."""
+        if not self.num_samples:
+            raise ValueError("no sample added")
+        cl, v, n = self.table()
+        by = np.lexsort((v, -n, cl))
+        lead = by[np.r_[True, cl[by][1:] != cl[by][:-1]]] if len(by) else by
+        mode, count = np.full(self.num_clusters, -1, np.int32), np.zeros(self.num_clusters, np.int64)
+        mode[cl[lead]], count[cl[lead]] = v[lead], n[lead]
+        return mode, count
+
+    def close(self):
+        pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def canonical_clusters(labels):
+    """int64 labels 0 .. C-1 of any labelling, cluster k being the k-th group of labels_to_clusters(labels)."""
+    return np.unique(np.asarray(labels), return_inverse=True)[1].reshape(-1).astype(np.int64)
+
+
+def entity_value_modes(labels, value_samples, num_values, counter=EntityValueCounts):
+    """(modes int32[A][C], counts int64[A][C], S) of the canonical labels[R] (0 .. C-1) over the samples of
+    value_samples, an iterable of int32[A][R] (read_entity_values) consumed once: one counter per attribute (of
+    num_values[a] values), all alive while the samples stream through.  counter = EntityValueCounts on the host,
+    analysis_gpu.EntityValues on the device; both give the same integers."""
+    import contextlib
+
+    labels = np.asarray(labels, np.int64)
+    C = int(labels.max()) + 1 if len(labels) else 0
+    with contextlib.ExitStack() as stack:
+        handles = [stack.enter_context(counter(labels, C, V)) for V in num_values]
+        S = 0
+        for vals in value_samples:
+            for h, v in zip(handles, vals):
+                h.add_sample(v)
+            S += 1
+        if S == 0:
+            raise ValueError("the entity values need at least one sample at or after lowerIterationCutoff")
+        out = [h.modes() for h in handles]
+    return (np.array([m for m, _ in out], np.int32).reshape(len(out), C),
+            np.array([n for _, n in out], np.int64).reshape(len(out), C), S)
+
+
+def entity_value_rows(labels, modes, counts, num_samples, attribute_values):
+    """The rows of entity-values.csv from the integers: per cluster k of the canonical labels, (k, its size, then per
+    attribute its mode's value string and repr(count / (size S)))."""
+    sizes = np.bincount(np.asarray(labels, np.int64), minlength=modes.shape[1])
+    strings = [np.asarray(v.to_pylist() if hasattr(v, "to_pylist") else list(v), dtype=object)
+               for v in attribute_values]
+    rows = []
+    for k, size in enumerate(sizes.tolist()):
+        row = [k, size]
+        for a in range(len(strings)):
+            row += [strings[a][modes[a, k]], repr(int(counts[a, k]) / (size * num_samples))]
+        rows.append(row)
+    return rows

@@ -15,13 +15,16 @@ rule is in integers, and the device applies it to the same table.  The cell hist
 estimate equal analysis_arrays.vi_cross_histograms exactly: they are integers, counted on the device from radix-sorted
 (sample, label, label) keys of every pair of held samples.  The VI search (single-record moves on a quantised table)
 and the cells of any labelling with every held sample, summed or per sample, equal analysis_arrays.vi_search_rounds /
-vi_label_cells / vi_sample_cells exactly, on the same handle.
+vi_label_cells / vi_sample_cells exactly, on the same handle.  The entity-value counts of a point estimate's clusters
+equal analysis_arrays.EntityValueCounts exactly: the device keeps the sorted table of (cluster, value) keys and int64
+counts per attribute and merges each sample's run-length-encoded keys into it; the modes are a segmented arg-max.
 """
 import ctypes as C
 
 import numpy as np
 
 from . import _lib
+from . import analysis_arrays
 from .analysis_arrays import (MAX_PAIRS, SearchRun, VISearchRun, check_search_size, check_vi_search_size,
                               check_vi_search_squares, search_choice, search_cost, too_many_pairs, vi_sample_squares,
                               vi_search_choice, vi_search_table, vi_width)
@@ -347,3 +350,33 @@ def vi_cross_histograms(chain, batch_keys=None):
             vi.set_batch_keys(batch_keys)
         _add_chain(vi, chain)
         return vi.cross(width)
+
+
+class EntityValues(_Handle):
+    """Owner of a dbl_values handle, one attribute: the estimate's labels go in once, each sample's value per record
+    one at a time, modes() reads every cluster's mode and its count."""
+
+    _prefix = "dbl_values"
+
+    def __init__(self, labels, num_clusters, num_values):
+        labels = np.ascontiguousarray(labels, np.int32)
+        super().__init__(len(labels), labels.ctypes.data, int(num_clusters), int(num_values))
+        self.num_clusters = int(num_clusters)
+
+    def add_sample(self, values):
+        values = np.ascontiguousarray(values, np.int32)
+        if values.shape != (self.num_records,):
+            raise ValueError("a sample needs one value per record")
+        self._call("add_sample", self._h, values.ctypes.data)
+
+    def modes(self):
+        """(mode int32[C], count int64[C]), as analysis_arrays.EntityValueCounts.modes."""
+        mode, count = np.empty(self.num_clusters, np.int32), np.empty(self.num_clusters, np.int64)
+        self._call("modes", self._h, mode.ctypes.data, count.ctypes.data)
+        return mode, count
+
+
+def entity_value_modes(labels, value_samples, num_values):
+    """(modes, counts, S), identical to analysis_arrays.entity_value_modes(labels, value_samples, num_values): one
+    handle per attribute, all alive while the samples stream through."""
+    return analysis_arrays.entity_value_modes(labels, value_samples, num_values, EntityValues)

@@ -32,6 +32,12 @@
 // any labelling with every held sample (dbl_vi_score, as analysis_arrays.vi_label_cells) share one cell pass over
 // radix-sorted (s, label in C_s, label in c) keys -- see vi_cell_batches; dbl_vi_score_samples keeps the cells of
 // each sample apart (as analysis_arrays.vi_sample_cells), for the credible ball around a point estimate.
+//
+// Entity values per cluster of a point estimate (dbl_values_*, same numbers as analysis_arrays.EntityValueCounts): for
+// one attribute, count(c, v) = the (sample, record of c) pairs whose entity has value v, in int64.  The handle holds a
+// sorted table of (c << bits(V) | v, count); each sample's keys are radix-sorted, run-length encoded and merged into
+// it by the merge kernels of dbl_pairs, with the run lengths as counts -- see dbl_values_add_sample.  The modes are a
+// segmented arg-max over the table (dbl_values_modes).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -57,10 +63,10 @@ __device__ __forceinline__ unsigned long long mix64(unsigned long long x) {  // 
 
 int grid_for(int64_t n) { return (int)std::min<int64_t>((n + THREADS - 1) / THREADS, 4096); }
 
-// any label outside [0, R) raises the flag; runs before anything indexes by label
-__global__ void k_check_labels(int64_t R, const int32_t *__restrict__ cluster, int *__restrict__ bad) {
+// any of the R labels outside [0, bound) raises the flag; runs before anything indexes by label
+__global__ void k_check_labels(int64_t R, int64_t bound, const int32_t *__restrict__ cluster, int *__restrict__ bad) {
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x)
-    if (cluster[r] < 0 || (int64_t)cluster[r] >= R) *bad = 1;
+    if (cluster[r] < 0 || (int64_t)cluster[r] >= bound) *bad = 1;
 }
 
 __global__ void k_accumulate(int64_t R, const int32_t *__restrict__ cluster, unsigned long long *__restrict__ sum,
@@ -212,11 +218,11 @@ struct Handle {
   Buf cluster, bad;
 
   // R labels, host or device (unified addressing picks the copy direction), into dst, then the range check:
-  // DBL_ERR_INVALID when one is outside [0, R)
-  int take_labels(const int32_t *labels, Buf &dst) {
+  // DBL_ERR_INVALID when one is outside [0, bound), bound = R unless given
+  int take_labels(const int32_t *labels, Buf &dst, int64_t bound = -1) {
     POST_TRY(cudaMemcpyAsync(dst.p, labels, sizeof(int32_t) * R, cudaMemcpyDefault, stream));
     POST_TRY(cudaMemsetAsync(bad.p, 0, sizeof(int), stream));
-    k_check_labels<<<grid_for(R), THREADS, 0, stream>>>(R, dst.as<int32_t>(), bad.as<int>());
+    k_check_labels<<<grid_for(R), THREADS, 0, stream>>>(R, bound < 0 ? R : bound, dst.as<int32_t>(), bad.as<int>());
     int flag = 0;
     POST_TRY(cudaMemcpyAsync(&flag, bad.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
     POST_TRY(cudaStreamSynchronize(stream));
@@ -459,29 +465,35 @@ __global__ void k_probe_new(int64_t n, const unsigned long long *__restrict__ ke
   }
 }
 
-// merge, held side: an entry moves up by the number of new keys below it, and counts one more if the sample has it
-__global__ void k_merge_held(int64_t H, const unsigned long long *__restrict__ held, const int32_t *__restrict__ hcnt,
-                             int64_t n, const unsigned long long *__restrict__ keys, const int32_t *__restrict__ rank,
-                             unsigned long long *__restrict__ out_key, int32_t *__restrict__ out_cnt) {
+// merge, held side: an entry moves up by the number of new keys below it, and counts add[lb] more (1 when add is
+// null) if the sample has it.  Cnt is int32 for the pairs table, int64 for the entity-value table.
+template <class Cnt>
+__global__ void k_merge_held(int64_t H, const unsigned long long *__restrict__ held, const Cnt *__restrict__ hcnt,
+                             int64_t n, const unsigned long long *__restrict__ keys, const int32_t *__restrict__ add,
+                             const int32_t *__restrict__ rank, unsigned long long *__restrict__ out_key,
+                             Cnt *__restrict__ out_cnt) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < H; i += (int64_t)gridDim.x * blockDim.x) {
     const unsigned long long k = held[i];
     const int64_t lb = lower_bound_u64(keys, n, k);
     const int64_t pos = i + rank[lb];
     out_key[pos] = k;
-    out_cnt[pos] = hcnt[i] + (lb < n && keys[lb] == k);
+    out_cnt[pos] = hcnt[i] + (lb < n && keys[lb] == k ? (add ? (Cnt)add[lb] : (Cnt)1) : (Cnt)0);
   }
 }
 
-// merge, sample side: a new key lands after the held entries below it and the new keys before it, with count 1
-__global__ void k_merge_new(int64_t n, const unsigned long long *__restrict__ keys, const int32_t *__restrict__ is_new,
-                            const int32_t *__restrict__ rank, int64_t H, const unsigned long long *__restrict__ held,
-                            unsigned long long *__restrict__ out_key, int32_t *__restrict__ out_cnt) {
+// merge, sample side: a new key lands after the held entries below it and the new keys before it, with count add[j]
+// (1 when add is null)
+template <class Cnt>
+__global__ void k_merge_new(int64_t n, const unsigned long long *__restrict__ keys, const int32_t *__restrict__ add,
+                            const int32_t *__restrict__ is_new, const int32_t *__restrict__ rank, int64_t H,
+                            const unsigned long long *__restrict__ held, unsigned long long *__restrict__ out_key,
+                            Cnt *__restrict__ out_cnt) {
   for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
     if (!is_new[j]) continue;
     const unsigned long long k = keys[j];
     const int64_t pos = lower_bound_u64(held, H, k) + rank[j];
     out_key[pos] = k;
-    out_cnt[pos] = 1;
+    out_cnt[pos] = add ? (Cnt)add[j] : (Cnt)1;
   }
 }
 
@@ -517,6 +529,43 @@ __global__ void k_scatter_pairs(int64_t H, const unsigned long long *__restrict_
     second[p] = (int32_t)(key[i] & 0xffffffffull);
     count[p] = cnt[i];
   }
+}
+
+// The n sorted distinct keys of a sample against a held sorted table of H keys: is_new[j] = 1 for a key the table
+// lacks, rank = the exclusive scan of is_new over n + 1 entries, *fresh_out = the number of new keys.  is_new and rank
+// must hold n + 1 entries; tmp grows to the scan's temporary storage.
+int probe_new_keys(int64_t n, const unsigned long long *keys, int64_t H, const unsigned long long *held, Buf &is_new,
+                   Buf &rank, Buf &tmp, cudaStream_t st, int64_t *fresh_out) {
+  k_probe_new<<<grid_for(n + 1), THREADS, 0, st>>>(n, keys, H, held, is_new.as<int32_t>());
+  size_t tbr = 0;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tbr, (const int32_t *)nullptr, (int32_t *)nullptr, (int64_t)n + 1,
+                                         st));
+  POST_TRY(tmp.reserve(tbr));
+  tbr = tmp.cap;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(tmp.p, tbr, is_new.as<int32_t>(), rank.as<int32_t>(), (int64_t)n + 1, st));
+  int32_t fresh = 0;
+  POST_TRY(cudaMemcpyAsync(&fresh, rank.as<int32_t>() + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  *fresh_out = fresh;
+  return DBL_OK;
+}
+
+// The union of the held table (held, hcnt; H entries) and the probed sample keys (probe_new_keys), each sample key
+// counting add[j] (1 when add is null), into (out_key, out_cnt), H + fresh entries; synchronised.
+template <class Cnt>
+int merge_keys(int64_t H, const unsigned long long *held, const Cnt *hcnt, int64_t n, const unsigned long long *keys,
+               const int32_t *add, const Buf &is_new, const Buf &rank, unsigned long long *out_key, Cnt *out_cnt,
+               cudaStream_t st) {
+  if (H > 0)
+    k_merge_held<Cnt><<<grid_for(H), THREADS, 0, st>>>(H, held, hcnt, n, keys, add, rank.as<int32_t>(), out_key,
+                                                       out_cnt);
+  if (n > 0)
+    k_merge_new<Cnt><<<grid_for(n), THREADS, 0, st>>>(n, keys, add, is_new.as<int32_t>(), rank.as<int32_t>(), H, held,
+                                                      out_key, out_cnt);
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
 }
 }  // namespace
 
@@ -626,18 +675,8 @@ extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
   // which keys are new, and their ranks among the new ones
   const unsigned long long *held = p->tab_key[p->cur].as<unsigned long long>();
   const int32_t *hcnt = p->tab_cnt[p->cur].as<int32_t>();
-  k_probe_new<<<grid_for(n + 1), THREADS, 0, st>>>(n, keys, H, held, p->is_new.as<int32_t>());
-  size_t tbr = 0;
-  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tbr, (const int32_t *)nullptr, (int32_t *)nullptr, (int64_t)n + 1,
-                                         st));
-  POST_TRY(p->tmp.reserve(tbr));
-  tbr = p->tmp.cap;
-  POST_TRY(cub::DeviceScan::ExclusiveSum(p->tmp.p, tbr, p->is_new.as<int32_t>(), p->rank.as<int32_t>(),
-                                         (int64_t)n + 1, st));
-  int32_t fresh = 0;
-  POST_TRY(cudaMemcpyAsync(&fresh, p->rank.as<int32_t>() + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  POST_TRY(cudaGetLastError());
-  POST_TRY(cudaStreamSynchronize(st));
+  int64_t fresh = 0;
+  if (const int rc = probe_new_keys(n, keys, H, held, p->is_new, p->rank, p->tmp, st, &fresh); rc != DBL_OK) return rc;
   const int64_t H2 = H + fresh;
   if (H2 > p->max_pairs) return DBL_ERR_INVALID;  // the union does not fit: the held table stays as it is
 
@@ -645,15 +684,10 @@ extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
   const int nxt = p->cur ^ 1;
   POST_TRY(p->tab_key[nxt].reserve(sizeof(unsigned long long) * (size_t)H2, cap8));
   POST_TRY(p->tab_cnt[nxt].reserve(sizeof(int32_t) * (size_t)H2, sizeof(int32_t) * (size_t)p->max_pairs));
-  unsigned long long *ok = p->tab_key[nxt].as<unsigned long long>();
-  int32_t *oc = p->tab_cnt[nxt].as<int32_t>();
-  if (H > 0)
-    k_merge_held<<<grid_for(H), THREADS, 0, st>>>(H, held, hcnt, n, keys, p->rank.as<int32_t>(), ok, oc);
-  if (n > 0)
-    k_merge_new<<<grid_for(n), THREADS, 0, st>>>(n, keys, p->is_new.as<int32_t>(), p->rank.as<int32_t>(), H, held, ok,
-                                                 oc);
-  POST_TRY(cudaGetLastError());
-  POST_TRY(cudaStreamSynchronize(st));
+  if (const int rc = merge_keys<int32_t>(H, held, hcnt, n, keys, nullptr, p->is_new, p->rank,
+                                         p->tab_key[nxt].as<unsigned long long>(), p->tab_cnt[nxt].as<int32_t>(), st);
+      rc != DBL_OK)
+    return rc;
   p->cur = nxt;
   p->H = H2;
   ++p->S;
@@ -1914,5 +1948,183 @@ extern "C" int dbl_vi_search(dbl_vi *p, const int64_t *step, const int32_t *star
   *rounds_out = rounds;
   *converged_out = converged;
   *J0_out = (int64_t)J0;
+  return DBL_OK;
+}
+
+// ---- entity values per cluster of a point estimate -----------------------------------------------------------------
+namespace {
+// one key per record: its cluster label above the value of the entity it links to in this sample
+__global__ void k_value_keys(int64_t R, int val_bits, const int32_t *__restrict__ label,
+                             const int32_t *__restrict__ value, unsigned long long *__restrict__ key) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < R; r += (int64_t)gridDim.x * blockDim.x)
+    key[r] = (unsigned long long)(uint32_t)label[r] << val_bits | (uint32_t)value[r];
+}
+
+// Segmented arg-max over the held table, pass 1: best[c] = the largest count of label c.  The table is sorted by key,
+// so the entries of a label are contiguous and a warp's lanes hold runs of equal labels: a segmented shuffle reduction
+// leaves each run's largest count at its first lane, which adds one atomic.  A label of many entries costs one atomic
+// per warp it spans.
+__global__ void k_mode_count(int64_t H, int val_bits, const unsigned long long *__restrict__ key,
+                             const long long *__restrict__ cnt, unsigned long long *__restrict__ best) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * WARPS_PER_BLOCK;
+  for (int64_t base = (blockIdx.x * (int64_t)WARPS_PER_BLOCK + (threadIdx.x >> 5)) * 32; base < H; base += nwarps * 32) {
+    const int64_t i = base + lane;
+    const bool valid = i < H;
+    const long long lab = valid ? (long long)(key[i] >> val_bits) : -1 - lane;  // a tail lane matches no one
+    long long c = valid ? cnt[i] : 0;
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long ol = __shfl_down_sync(0xffffffffu, lab, o), oc = __shfl_down_sync(0xffffffffu, c, o);
+      if (lane + o < 32 && ol == lab && oc > c) c = oc;
+    }
+    const long long prev = __shfl_up_sync(0xffffffffu, lab, 1);
+    if (valid && (lane == 0 || prev != lab)) atomicMax(&best[lab], (unsigned long long)c);
+  }
+}
+
+// pass 2: first[c] = the first table position of label c whose count is best[c], i.e. its smallest such value; the
+// lanes of a warp with equal labels and the best count elect their lowest lane, which adds one atomic
+__global__ void k_mode_first(int64_t H, int val_bits, const unsigned long long *__restrict__ key,
+                             const long long *__restrict__ cnt, const unsigned long long *__restrict__ best,
+                             unsigned long long *__restrict__ first) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * WARPS_PER_BLOCK;
+  for (int64_t base = (blockIdx.x * (int64_t)WARPS_PER_BLOCK + (threadIdx.x >> 5)) * 32; base < H; base += nwarps * 32) {
+    const int64_t i = base + lane;
+    const unsigned long long lab = i < H ? key[i] >> val_bits : 0ull;
+    const bool hit = i < H && (unsigned long long)cnt[i] == best[lab];
+    const unsigned peers = __match_any_sync(0xffffffffu, hit ? lab : ~0ull);
+    if (hit && lane == __ffs(peers) - 1) atomicMin(&first[lab], (unsigned long long)i);
+  }
+}
+
+// per label its mode (the value of its first best position, -1 when the label has no record) and the mode's count
+__global__ void k_mode_out(int64_t C, unsigned long long mask, const unsigned long long *__restrict__ key,
+                           const unsigned long long *__restrict__ best, const unsigned long long *__restrict__ first,
+                           int32_t *__restrict__ mode, long long *__restrict__ count) {
+  for (int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; c < C; c += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long f = first[c];
+    mode[c] = f == ~0ull ? -1 : (int32_t)(key[f] & mask);
+    count[c] = (long long)best[c];
+  }
+}
+}  // namespace
+
+struct dbl_values : Handle {
+  int32_t C = 0, V = 0;
+  int val_bits = 1, key_bits = 2;       // bits of a value in [0, V); radix sort end bit of the keys
+  int64_t H = 0;                        // distinct (label, value) keys held
+  Buf labels;                           // R labels in [0, C); Handle::cluster receives each sample's values
+  Buf key_in, key_s, uniq;              // R keys each: unsorted, sorted, distinct
+  Buf runs, nruns;                      // R int32 run lengths of the distinct keys; their number
+  Buf is_new, rank;                     // R + 1 each: merge flags and ranks
+  Buf tab_key[2], tab_cnt[2];           // grown on demand: held table (index cur), the one the next sample merges into
+  int cur = 0;
+  Buf tmp;                              // CUB temporary storage, grown on demand
+};
+
+extern "C" int dbl_values_create(dbl_values **out, int64_t num_records, const int32_t *labels, int32_t num_clusters,
+                                 int32_t num_values) {
+  if (!out) return DBL_ERR_INVALID;
+  *out = nullptr;
+  if (num_records <= 0 || num_records > INT32_MAX || !labels || num_clusters <= 0 || num_values <= 0)
+    return DBL_ERR_INVALID;
+  return open_handle(out, num_records, [&](dbl_values *p) {
+    const int64_t R = num_records;
+    p->C = num_clusters;
+    p->V = num_values;
+    p->val_bits = bits_for(num_values);
+    p->key_bits = bits_for(num_clusters) + p->val_bits;
+    const size_t r4 = sizeof(int32_t) * (size_t)R, r8 = sizeof(unsigned long long) * (size_t)R;
+    if (p->labels.alloc(r4) != cudaSuccess || p->key_in.alloc(r8) != cudaSuccess || p->key_s.alloc(r8) != cudaSuccess ||
+        p->uniq.alloc(r8) != cudaSuccess || p->runs.alloc(r4) != cudaSuccess ||
+        p->nruns.alloc(sizeof(int64_t)) != cudaSuccess || p->is_new.alloc(r4 + sizeof(int32_t)) != cudaSuccess ||
+        p->rank.alloc(r4 + sizeof(int32_t)) != cudaSuccess)
+      return DBL_ERR_CUDA;
+    return p->take_labels(labels, p->labels, num_clusters);
+  });
+}
+
+extern "C" void dbl_values_free(dbl_values *p) { free_handle(p); }
+
+extern "C" int32_t dbl_values_num_samples(const dbl_values *p) { return p ? p->S : 0; }
+
+// One sample: check the values; key (label << val_bits | value) per record; radix-sort on key_bits bits; run-length
+// encode into (distinct key, records); merge those into the spare table with their run lengths as counts, then commit
+// by swapping tables.  A refusal or failure leaves the held table and S as they were.
+extern "C" int dbl_values_add_sample(dbl_values *p, const int32_t *values) {
+  if (!p || !values || p->S == INT32_MAX) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(values, p->cluster, p->V); rc != DBL_OK) return rc;
+  const int64_t R = p->R, H = p->H;
+  cudaStream_t st = p->stream;
+  k_value_keys<<<grid_for(R), THREADS, 0, st>>>(R, p->val_bits, p->labels.as<int32_t>(), p->cluster.as<int32_t>(),
+                                                p->key_in.as<unsigned long long>());
+  size_t tb_sort = 0, tb_rle = 0;
+  unsigned long long *ks = p->key_s.as<unsigned long long>(), *uniq = p->uniq.as<unsigned long long>();
+  POST_TRY(cub::DeviceRadixSort::SortKeys(nullptr, tb_sort, p->key_in.as<unsigned long long>(), ks, R, 0, p->key_bits,
+                                          st));
+  POST_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, tb_rle, ks, uniq, p->runs.as<int32_t>(),
+                                              p->nruns.as<int64_t>(), R, st));
+  POST_TRY(p->tmp.reserve(std::max(tb_sort, tb_rle)));
+  size_t tb = p->tmp.cap;
+  POST_TRY(cub::DeviceRadixSort::SortKeys(p->tmp.p, tb, p->key_in.as<unsigned long long>(), ks, R, 0, p->key_bits,
+                                          st));
+  tb = p->tmp.cap;
+  POST_TRY(cub::DeviceRunLengthEncode::Encode(p->tmp.p, tb, ks, uniq, p->runs.as<int32_t>(), p->nruns.as<int64_t>(),
+                                              R, st));
+  int64_t n = 0;
+  POST_TRY(cudaMemcpyAsync(&n, p->nruns.p, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+
+  const unsigned long long *held = p->tab_key[p->cur].as<unsigned long long>();
+  const long long *hcnt = p->tab_cnt[p->cur].as<long long>();
+  int64_t fresh = 0;
+  if (const int rc = probe_new_keys(n, uniq, H, held, p->is_new, p->rank, p->tmp, st, &fresh); rc != DBL_OK) return rc;
+  const int64_t H2 = H + fresh;
+  const int nxt = p->cur ^ 1;
+  POST_TRY(p->tab_key[nxt].reserve(sizeof(unsigned long long) * (size_t)H2));
+  POST_TRY(p->tab_cnt[nxt].reserve(sizeof(long long) * (size_t)H2));
+  if (const int rc = merge_keys<long long>(H, held, hcnt, n, uniq, p->runs.as<int32_t>(), p->is_new, p->rank,
+                                           p->tab_key[nxt].as<unsigned long long>(), p->tab_cnt[nxt].as<long long>(),
+                                           st);
+      rc != DBL_OK)
+    return rc;
+  p->cur = nxt;
+  p->H = H2;
+  ++p->S;
+  return DBL_OK;
+}
+
+// Per label the value of largest count, ties to the smallest value: k_mode_count, then k_mode_first, over the held
+// table; a label without records gets mode -1 and count 0.  The table and S do not change.
+extern "C" int dbl_values_modes(dbl_values *p, int32_t *mode_out, int64_t *count_out) {
+  if (!p || !mode_out || !count_out) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  const int64_t C = p->C, H = p->H;
+  cudaStream_t st = p->stream;
+  Buf best, first, mode, count;
+  POST_TRY(best.alloc(sizeof(unsigned long long) * C));
+  POST_TRY(first.alloc(sizeof(unsigned long long) * C));
+  POST_TRY(mode.alloc(sizeof(int32_t) * C));
+  POST_TRY(count.alloc(sizeof(long long) * C));
+  POST_TRY(cudaMemsetAsync(best.p, 0, sizeof(unsigned long long) * C, st));
+  POST_TRY(cudaMemsetAsync(first.p, 0xff, sizeof(unsigned long long) * C, st));
+  const unsigned long long *key = p->tab_key[p->cur].as<unsigned long long>();
+  const long long *cnt = p->tab_cnt[p->cur].as<long long>();
+  const int warp_grid = (int)std::min<int64_t>((H + THREADS - 1) / THREADS, 8192);
+  k_mode_count<<<warp_grid, THREADS, 0, st>>>(H, p->val_bits, key, cnt, best.as<unsigned long long>());
+  k_mode_first<<<warp_grid, THREADS, 0, st>>>(H, p->val_bits, key, cnt, best.as<unsigned long long>(),
+                                              first.as<unsigned long long>());
+  k_mode_out<<<grid_for(C), THREADS, 0, st>>>(C, (1ull << p->val_bits) - 1, key, best.as<unsigned long long>(),
+                                              first.as<unsigned long long>(), mode.as<int32_t>(),
+                                              count.as<long long>());
+  POST_TRY(cudaGetLastError());
+  // host or device outputs: unified addressing picks the copy direction
+  POST_TRY(cudaMemcpyAsync(mode_out, mode.p, sizeof(int32_t) * C, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(count_out, count.p, sizeof(int64_t) * C, cudaMemcpyDefault, st));
+  POST_TRY(cudaStreamSynchronize(st));
   return DBL_OK;
 }

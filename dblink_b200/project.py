@@ -32,7 +32,8 @@ SUPPORTED_METRICS = (SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_
                      + VI_SEARCH_METRICS + CREDIBLE_BALL_METRICS)
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
-                        "binder-search-clusters", "vi-clusters", "vi-search-clusters", "credible-ball")
+                        "binder-search-clusters", "vi-clusters", "vi-search-clusters", "credible-ball",
+                        "entity-values")
 # the point estimates a credible ball may be centred on
 CREDIBLE_BALL_CENTERS = ("shared-most-probable-clusters", "binder-clusters", "binder-search-clusters", "vi-clusters",
                          "vi-search-clusters")
@@ -167,6 +168,14 @@ def vi_search_estimate(chain, max_rounds):
     return analysis_arrays.VI_SEARCH_STARTS[best], runs[best], rows, exact
 
 
+def entity_value_modes(labels, value_samples, num_values):
+    """(modes, counts, S) of the entity values of the clusters of labels over the samples of value_samples: on the
+    GPU when the platform has one (analysis_gpu), else on the host (analysis_arrays).  Both give identical arrays."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.entity_value_modes(labels, value_samples, num_values)
+    return analysis_arrays.entity_value_modes(labels, value_samples, num_values)
+
+
 def credible_ball_center(chain, center, false_link_cost, max_rounds):
     """The labels of the point estimate `center` (one of CREDIBLE_BALL_CENTERS) of a ChainArrays, computed as its own
     summarize quantity computes it."""
@@ -229,15 +238,22 @@ def _credible_ball_rows(chain, center, level, balls):
     return rows
 
 
-def _credible_ball_settings(prm):
-    """The settings a credible ball's center is computed with, for run.txt."""
-    center = prm["credible_ball_center"]
-    out = f"credibleBallCenter={center}"
+def _center_settings(prm, key, name):
+    """The settings the point estimate prm[key] is computed with, for run.txt: `name`=center, then the settings that
+    apply to it."""
+    center = prm[key]
+    out = f"{name}={center}"
     if center.startswith("binder"):
         out += f", falseLinkCost={prm['false_link_cost']}"
     if center.endswith("search-clusters"):
         out += f", maxSearchRounds={prm['max_search_rounds']}"
-    return out + f", credibleLevel={prm['credible_level']}"
+    return out
+
+
+def _credible_ball_settings(prm):
+    """The settings a credible ball's center is computed with, for run.txt."""
+    return (_center_settings(prm, "credible_ball_center", "credibleBallCenter")
+            + f", credibleLevel={prm['credible_level']}")
 
 
 def _credible_ball_params(prm):
@@ -248,6 +264,22 @@ def _credible_ball_params(prm):
     if isinstance(level, bool) or not isinstance(level, (int, float)) or not 0.0 < float(level) <= 1.0:
         raise ValueError("credibleLevel must be in (0, 1].")
     return dict(credible_ball_center=center, credible_level=float(level))
+
+
+def _entity_values_center(prm):
+    center = prm.get("entityValuesCenter", "shared-most-probable-clusters")
+    if center not in CREDIBLE_BALL_CENTERS:
+        raise ValueError(f"entityValuesCenter must be one of {CREDIBLE_BALL_CENTERS}.")
+    return center
+
+
+def _save_entity_values(prm):
+    """{"save_entity_values": True} when the sample step records entity values, else nothing: a step without the
+    option keeps the parameters it always had."""
+    save = prm.get("saveEntityValues", False)
+    if not isinstance(save, bool):
+        raise ValueError("saveEntityValues must be a boolean.")
+    return {"save_entity_values": True} if save else {}
 
 
 def _searched_cost(false_link_cost):
@@ -358,7 +390,9 @@ class Project:
                 src = "saved state" if prm["resume"] else "new initial state"
                 L.append(f"  * SampleStep: Evolving the chain from {src} with sampleSize={prm['sample_size']}, "
                          f"burninInterval={prm['burnin_interval']}, thinningInterval={prm['thinning_interval']} and "
-                         f"sampler={prm['sampler']}")
+                         f"sampler={prm['sampler']}"
+                         + (", saving every sample's entity values (saveEntityValues=true)"
+                            if prm.get("save_entity_values") else ""))
             elif name == "summarize":
                 L.append(f"  * SummarizeStep: Calculating summary quantities {braces(prm['quantities'])} along the "
                          f"chain for iterations >= {prm['lower_iteration_cutoff']}")
@@ -382,6 +416,10 @@ class Project:
                     L.append(f"  * SummarizeStep: credible-ball is the smallest ball around a point estimate, in "
                              f"variation of information and in Binder distance, that holds a share of the samples, "
                              f"with {_credible_ball_settings(prm)}")
+                if "entity-values" in prm["quantities"]:
+                    L.append(f"  * SummarizeStep: entity-values is the most probable value of each attribute of the "
+                             f"entity of each cluster of a point estimate, from the entity values saved with the "
+                             f"samples, with {_center_settings(prm, 'entity_values_center', 'entityValuesCenter')}")
             elif name == "evaluate":
                 smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
                 post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
@@ -547,7 +585,8 @@ class Project:
                 out.append(("sample", dict(sample_size=int(prm["sampleSize"]),
                                            burnin_interval=int(prm.get("burninInterval", 0)),
                                            thinning_interval=int(prm.get("thinningInterval", 1)),
-                                           resume=bool(prm.get("resume", True)), sampler=prm.get("sampler", "PCG-I"))))
+                                           resume=bool(prm.get("resume", True)), sampler=prm.get("sampler", "PCG-I"),
+                                           **_save_entity_values(prm))))
             elif name == "summarize":
                 q = list(prm["quantities"])
                 if not q or any(x not in SUPPORTED_QUANTITIES for x in q):
@@ -562,6 +601,7 @@ class Project:
                                               quantities=q, min_match_probability=t,
                                               false_link_cost=_false_link_cost(prm),
                                               max_search_rounds=_max_search_rounds(prm),
+                                              entity_values_center=_entity_values_center(prm),
                                               **_credible_ball_params(prm))))
             elif name == "evaluate":
                 m = list(prm["metrics"])
@@ -594,7 +634,8 @@ class Project:
                 log(f"SampleStep: sampleSize={prm['sample_size']} burninInterval={prm['burnin_interval']} "
                     f"thinningInterval={prm['thinning_interval']} sampler={prm['sampler']}")
                 chain.sample(eng, d["rec_ids"], [a.name for a in self.matching_attributes], prm["sample_size"],
-                             self.output_path, prm["burnin_interval"], prm["thinning_interval"], sampler=prm["sampler"])
+                             self.output_path, prm["burnin_interval"], prm["thinning_interval"], sampler=prm["sampler"],
+                             entity_values=self.attribute_values() if prm.get("save_entity_values") else None)
                 self.save_state(eng)  # Sampler.scala:120
             elif name == "summarize":
                 # array implementations (analysis_arrays): same quantities as analysis.py, no loop over clusters
@@ -651,6 +692,8 @@ class Project:
                             self._save_smpc(analysis_arrays.labels_to_clusters(
                                 analysis_arrays.sample_labels(ch.num_records, mem, off), ch.record_ids),
                                 f"credible-ball-{name}-{bound}.csv")
+                    elif q == "entity-values":
+                        self._summarize_entity_values(ch, prm)
                     else:
                         labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
@@ -771,6 +814,27 @@ class Project:
         if self.num_chains == 1:
             return analysis_arrays.read_chain_arrays(paths[0], lower_iteration_cutoff)
         return analysis_arrays.read_pooled_chain_arrays(paths, lower_iteration_cutoff)
+
+    def attribute_values(self):
+        """Per matching attribute, the pyarrow string array of its values in value-id order (the strcmp order of the
+        values, dbl_host.cpp)."""
+        import pyarrow as pa
+
+        return [pa.array([ix.value_of(v) for v in range(ix.num_values)], pa.string())
+                for ix in self.load()["cache"].indexes]
+
+    def _summarize_entity_values(self, ch, prm):
+        """entity-values-clusters.csv (the center, line k = cluster k) and entity-values.csv (every cluster's most
+        probable value of each attribute), from the entity values saved with the samples of ch."""
+        labels = analysis_arrays.canonical_clusters(credible_ball_center(ch, prm["entity_values_center"],
+                                                                         prm["false_link_cost"],
+                                                                         prm["max_search_rounds"]))
+        names, values = [a.name for a in self.matching_attributes], self.attribute_values()
+        samples = analysis_arrays.read_entity_values(self.chain_dirs(), ch, names, values)
+        modes, counts, S = entity_value_modes(labels, samples, [len(v) for v in values])
+        self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids), "entity-values-clusters.csv")
+        writers.save_entity_values(names, analysis_arrays.entity_value_rows(labels, modes, counts, S, values),
+                                   self.output_path)
 
     def _evaluate_samples(self, lower_iteration_cutoff, true_labels, pooled=None):
         """Every sample at or after the cutoff against the ground truth: each chain's evaluation-samples.csv in its

@@ -1,13 +1,15 @@
 """Chain driver: Sampler.sample (Sampler.scala:51-124) over a GibbsEngine / ShardedGibbs."""
 import os
+import shutil
 
-from .writers import DiagnosticsWriter, LinkageChainWriter, linkage_structure_arrow
+from .writers import (DiagnosticsWriter, EntityValuesChainWriter, LinkageChainWriter, cluster_layout,
+                      entity_values_arrow, linkage_structure_arrow)
 
 SUPPORTED_SAMPLERS = ("PCG-I", "PCG-II", "Gibbs", "Gibbs-Sequential")  # ProjectStep.scala:35
 
 
 def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin_interval=0, thinning_interval=1,
-           write_buffer_size=10, sampler="PCG-I", population_size=None, on_sample=None):
+           write_buffer_size=10, sampler="PCG-I", population_size=None, on_sample=None, entity_values=None):
     """Generates `sample_size` posterior samples by successively applying the transition operator; writes
     linkage-chain.parquet and diagnostics.csv under output_path.  Returns the number of sweeps performed.
     on_sample(summary, parts) sees every recorded sample; parts = {partition id: pyarrow ListArray of clusters}
@@ -15,7 +17,14 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
 
     An engine holding K > 1 chains (GibbsEngine.init_chains / upload_chains) writes chain k's linkage-chain.parquet
     and diagnostics.csv under output_path/chain-<k>/, from one download of every chain's links per recorded sample;
-    on_sample then sees every chain's sample, chain-major."""
+    on_sample then sees every chain's sample, chain-major.
+
+    entity_values: None, or per matching attribute its value strings in value-id order.  Given, each chain directory
+    also gets entity-values-chain.parquet (writers.EntityValuesChainWriter), the value of every cluster's entity at
+    every recorded sample; y comes from download_state (one chain), download_chains (K > 1) or, on a sharded engine,
+    its download_state of y, block and link (a collective; rank 0 writes).  Not given, a new (not continued) chain
+    removes the entity-values-chain.parquet an earlier chain left in its directory: the linkage chain it described
+    is replaced."""
     if sample_size <= 0:
         raise ValueError("`sampleSize` must be positive.")            # Sampler.scala:61
     if burnin_interval < 0:
@@ -34,30 +43,52 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
     pop = population_size if population_size is not None else engine.num_entities
     K = getattr(engine, "num_chains", 1)
     dirs = [output_path] if K == 1 else [os.path.join(output_path, f"chain-{k}") for k in range(K)]
-    lw = dw = ids = None
+    lw = dw = ew = ids = None
     if writer:
-        lw, dw = [], []
+        lw, dw, ew = [], [], []
         for d in dirs:
             os.makedirs(d, exist_ok=True)
             lw.append(LinkageChainWriter(os.path.join(d, "linkage-chain.parquet"), write_buffer_size, continue_chain))
             dw.append(DiagnosticsWriter(os.path.join(d, "diagnostics.csv"), attribute_names, continue_chain))
+            ev_path = os.path.join(d, "entity-values-chain.parquet")
+            if entity_values is not None:
+                ew.append(EntityValuesChainWriter(ev_path, attribute_names, write_buffer_size, continue_chain,
+                                                  lw[-1].file_no))
+            elif not continue_chain and os.path.isdir(ev_path):
+                # a new chain without entity values: the values of an earlier chain in this directory would describe
+                # other linkage rows under the same iterations and file names, so they go with that chain
+                shutil.rmtree(ev_path)
 
         import pyarrow as pa
 
         ids = pa.array([str(r) for r in record_ids], pa.string())
+        values = None if entity_values is None else [
+            v if isinstance(v, pa.Array) else pa.array(list(v), pa.string()) for v in entity_values]
 
     def record():
-        if K == 1:
+        y = [None] * K
+        if K == 1 and entity_values is None:
             link, blk = engine.links()  # sharded: a collective, every rank takes part
             samples = [(link, blk, engine.summary())]
+        elif K == 1:
+            # sharded (it has a rank): a collective over the arrays named, every rank takes part
+            st = (engine.download_state(keys=("y", "block", "link")) if hasattr(engine, "rank") else
+                  engine.download_state())
+            samples, y = [(st["link"], st["block"], engine.summary())], [st["y"]]
         else:
-            st = engine.download_chains(links_only=True)
+            st = engine.download_chains(links_only=entity_values is None)
             samples = [(st[k]["link"], st[k]["block"], engine.chain_summary(k)) for k in range(K)]
+            if entity_values is not None:
+                y = [st[k]["y"] for k in range(K)]
         if not writer:
             return
         for k, (link, blk, s) in enumerate(samples):
-            parts = linkage_structure_arrow(link, blk, ids)  # {partition id: ListArray of clusters}
+            # one cluster order for both files
+            layout = cluster_layout(link, blk) if entity_values is not None else None
+            parts = linkage_structure_arrow(link, blk, ids, layout)  # {partition id: ListArray of clusters}
             lw[k].append(s["iteration"], parts)
+            if entity_values is not None:
+                ew[k].append(s["iteration"], entity_values_arrow(link, blk, y[k], values, layout))
             dw[k].write_row(s, pop)
             if on_sample:
                 on_sample(s, parts)
@@ -78,6 +109,6 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
         record()
         count += 1
     if writer:
-        for w in lw + dw:
+        for w in lw + ew + dw:
             w.close()
     return done

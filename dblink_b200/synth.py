@@ -80,18 +80,22 @@ def config_attrs(config: int) -> List[SynthAttr]:
 
 def generate_encoded(seed, n_records, attrs: List[SynthAttr], dup=0.10, distortion=0.05, missing=0.01, n_files=1):
     """Array form: per attribute a vocabulary (list of strings) and a code per record (-1 = missing).
-    -> dict(vocabs=[A][*] str, codes=int32[R, A], files=int32[R], ent_ids=int64[R], attributes=[Attribute])."""
+    -> dict(vocabs=[A][*] str, codes=int32[R, A], files=int32[R], ent_ids=int64[R], attributes=[Attribute],
+    ent_values=int32[E, A]): ent_values[e] = the codes of entity e's true values, the values its records carry when
+    not distorted (no random draw of its own: the other keys are those of the same seed without it)."""
     rng = np.random.default_rng(seed)
     R = int(n_records)
     n_ent = max(1, int(round(R * (1.0 - dup))))
     ent_of = np.concatenate([np.arange(n_ent), rng.integers(0, n_ent, R - n_ent)])
     rng.shuffle(ent_of)
     vocabs, codes = [], np.empty((R, len(attrs)), np.int32)
+    ent_values = np.empty((n_ent, len(attrs)), np.int32)
     for a, sa in enumerate(attrs):
         if sa.kind == "constant":
             vocab = [f"{i:03d}" for i in range(sa.vocab)]
             p = _zipf_probs(sa.vocab, sa.zipf)
             ent_val = rng.choice(sa.vocab, n_ent, p=p)
+            ent_values[:, a] = ent_val
             val = ent_val[ent_of]
             dist = rng.random(R) < distortion
             val = np.where(dist, rng.choice(sa.vocab, R, p=p), val)
@@ -101,6 +105,7 @@ def generate_encoded(seed, n_records, attrs: List[SynthAttr], dup=0.10, distorti
             n_base = len(base_idx)
             p = _zipf_probs(n_base, sa.zipf)
             ent_base = rng.choice(n_base, n_ent, p=p)
+            ent_values[:, a] = base_idx[ent_base]
             rec_base = ent_base[ent_of]
             first = base_idx[rec_base]
             count = np.r_[base_idx[1:], len(vocab)][rec_base] - first
@@ -116,7 +121,8 @@ def generate_encoded(seed, n_records, attrs: List[SynthAttr], dup=0.10, distorti
                   else SimilarityFn("LevenshteinSimilarityFn", 7.0, 10.0), alpha=10.0, beta=1000.0)
         for sa in attrs
     ]
-    return {"vocabs": vocabs, "codes": codes, "files": files, "ent_ids": ent_of, "attributes": attributes}
+    return {"vocabs": vocabs, "codes": codes, "files": files, "ent_ids": ent_of, "attributes": attributes,
+            "ent_values": ent_values}
 
 
 def generate(seed, n_records, attrs: List[SynthAttr], dup=0.10, distortion=0.05, missing=0.01, n_files=1):

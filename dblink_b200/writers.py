@@ -2,6 +2,8 @@
 
   LinkageChainWriter  linkage-chain.parquet, hive-partitioned by partitionId, columns iteration:int64,
                       linkageStructure:list<list<string>> (package.scala:94-96, util/BufferedRDDWriter.scala:44-50)
+  EntityValuesChainWriter   entity-values-chain.parquet: the value of every cluster's entity, aligned with the linkage
+                      chain's rows and clusters
   DiagnosticsWriter   diagnostics.csv with the header of DiagnosticsWriter.scala:39-45 and rows of :47-72
   save_cluster_size_distribution / save_partition_sizes   LinkageChain.scala:162-211
   save_pairwise_match_probabilities   pairwise-match-probabilities.csv: recordId1,recordId2,probability
@@ -9,6 +11,7 @@
   save_binder_loss   binder-loss.csv: every sample's linked pairs and posterior expected Binder loss
   save_binder_search   binder-search.csv: every round of the Binder search from each start
   save_vi_loss   vi-loss.csv: every sample's number of clusters and posterior expected variation of information
+  save_entity_values   entity-values.csv: every cluster's most probable value of each attribute and its probability
 """
 import os
 import time
@@ -30,36 +33,66 @@ def linkage_structure(link, block_of_entity, record_ids):
     return parts
 
 
-def linkage_structure_arrow(link, block_of_entity, record_ids):
-    """The same structure without Python loops over clusters: partition id -> pyarrow ListArray (list<string>), one
-    entry per non-isolated entity, clusters in ascending entity id, records of a cluster in ascending record index.
-    `record_ids` = a pyarrow string array (or anything pa.array accepts).  At 1M records this takes ~0.2 s where
-    the list-of-lists form takes seconds, so a recorded sample costs about as much as the sweeps between samples."""
-    import pyarrow as pa
-
+def cluster_layout(link, block_of_entity):
+    """The order clusters are written in, shared by linkage-chain.parquet and entity-values-chain.parquet: records
+    sorted by block, then entity, then record index.  Returns (order, cstart, cend, centity, parts): order = the
+    records in that order, cluster k = order[cstart[k]:cend[k]] of entity centity[k], and parts = [(partition id,
+    first cluster, end cluster)] over the partitions that hold clusters, in ascending partition id."""
     link = np.asarray(link)
     R = len(link)
-    ids = record_ids if isinstance(record_ids, pa.Array) else pa.array([str(r) for r in record_ids], pa.string())
     rec_blk = np.asarray(block_of_entity)[link]
     order = np.lexsort((link, rec_blk))  # stable: by block, then entity, then record index
     sl, sb = link[order], rec_blk[order]
     cstart = np.flatnonzero(np.r_[True, sl[1:] != sl[:-1]]) if R else np.zeros(0, np.int64)
     cend = np.r_[cstart[1:], R]
-    cblk = sb[cstart]
-    values = ids.take(pa.array(order, pa.int64()))
-    blocks, first = np.unique(cblk, return_index=True)
+    blocks, first = np.unique(sb[cstart], return_index=True)
     last = np.r_[first[1:], len(cstart)]
-    parts = {}
-    for b, f, e in zip(blocks, first, last):  # one iteration per partition
-        lo, hi = int(cstart[f]), int(cend[e - 1])
-        offs = np.r_[cstart[f:e], hi] - lo
-        parts[int(b)] = pa.ListArray.from_arrays(pa.array(offs, pa.int32()), values.slice(lo, hi - lo))
-    # a partition that holds only isolated entities still has a row, with an empty linkage structure
-    # (State.getLinkageStructure maps over every partition, State.scala:102-112)
+    return order, cstart, cend, sl[cstart], [(int(b), int(f), int(e)) for b, f, e in zip(blocks, first, last)]
+
+
+def _empty_partitions(parts, block_of_entity, empty):
+    """A partition that holds only isolated entities still has a row, with an empty linkage structure
+    (State.getLinkageStructure maps over every partition, State.scala:102-112)."""
     for b in np.unique(np.asarray(block_of_entity)):
         if int(b) not in parts:
-            parts[int(b)] = pa.ListArray.from_arrays(pa.array([0], pa.int32()), pa.array([], pa.string()))
+            parts[int(b)] = empty()
     return parts
+
+
+def linkage_structure_arrow(link, block_of_entity, record_ids, layout=None):
+    """The same structure without Python loops over clusters: partition id -> pyarrow ListArray (list<string>), one
+    entry per non-isolated entity, clusters in ascending entity id, records of a cluster in ascending record index.
+    `record_ids` = a pyarrow string array (or anything pa.array accepts).  At 1M records this takes ~0.2 s where
+    the list-of-lists form takes seconds, so a recorded sample costs about as much as the sweeps between samples.
+    `layout` = cluster_layout(link, block_of_entity) when the caller already has it."""
+    import pyarrow as pa
+
+    ids = record_ids if isinstance(record_ids, pa.Array) else pa.array([str(r) for r in record_ids], pa.string())
+    order, cstart, cend, _, parts_of = layout if layout is not None else cluster_layout(link, block_of_entity)
+    values = ids.take(pa.array(order, pa.int64()))
+    parts = {}
+    for b, f, e in parts_of:  # one iteration per partition
+        lo, hi = int(cstart[f]), int(cend[e - 1])
+        offs = np.r_[cstart[f:e], hi] - lo
+        parts[b] = pa.ListArray.from_arrays(pa.array(offs, pa.int32()), values.slice(lo, hi - lo))
+    return _empty_partitions(parts, block_of_entity,
+                             lambda: pa.ListArray.from_arrays(pa.array([0], pa.int32()), pa.array([], pa.string())))
+
+
+def entity_values_arrow(link, block_of_entity, y, value_strings, layout=None):
+    """Partition id -> [one pyarrow string array per matching attribute]: entry k of attribute a is the value of the
+    entity of cluster k of the same partition in linkage_structure_arrow(link, block_of_entity, ...) -- non-isolated
+    entities only, in the same order.  y = int32[E][A] entity value ids; value_strings[a] = attribute a's values in
+    value-id order (a pyarrow string array or anything pa.array accepts).  `layout` = cluster_layout(link,
+    block_of_entity) when the caller already has it: the sample step computes it once for both files."""
+    import pyarrow as pa
+
+    y = np.asarray(y)
+    vals = [v if isinstance(v, pa.Array) else pa.array(list(v), pa.string()) for v in value_strings]
+    _, _, _, centity, parts_of = layout if layout is not None else cluster_layout(link, block_of_entity)
+    parts = {b: [vals[a].take(pa.array(y[centity[f:e], a], pa.int64())) for a in range(len(vals))]
+             for b, f, e in parts_of}
+    return _empty_partitions(parts, block_of_entity, lambda: [pa.array([], pa.string()) for _ in vals])
 
 
 class LinkageChainWriter:
@@ -107,6 +140,58 @@ class LinkageChainWriter:
                               pa.list_(pa.list_(pa.string())))
             tbl = pa.Table.from_arrays([its, ls], schema=self.schema)
             pq.write_table(tbl, os.path.join(d, f"part-{self.file_no:05d}.parquet"))
+        self.file_no += 1
+        self.buf = []
+
+    close = flush
+
+
+class EntityValuesChainWriter:
+    """entity-values-chain.parquet, hive-partitioned by partitionId like linkage-chain.parquet, columns
+    iteration:int64 and one list<string> per matching attribute, named after it (rows from entity_values_arrow).  It
+    flushes in lockstep with the chain's LinkageChainWriter: the same buffer size, and file numbers starting at
+    `file_no`, the linkage writer's, so the rows of one flush land in files of the same name in both."""
+
+    def __init__(self, path, attribute_names, write_buffer_size, append, file_no):
+        import pyarrow as pa
+
+        self.pa = pa
+        self.path = path
+        self.names = list(attribute_names)
+        self.buf = []
+        self.n = write_buffer_size
+        self.file_no = file_no
+        self.schema = pa.schema([("iteration", pa.int64())] + [(a, pa.list_(pa.string())) for a in self.names])
+        if os.path.exists(path) and not append:
+            import shutil
+
+            shutil.rmtree(path)
+        os.makedirs(path, exist_ok=True)
+
+    def append(self, iteration, parts):
+        self.buf.append((iteration, parts))
+        if len(self.buf) >= self.n:
+            self.flush()
+
+    def flush(self):
+        import pyarrow.parquet as pq
+
+        if not self.buf:
+            return
+        pa = self.pa
+        by_part = {}
+        for it, parts in self.buf:
+            for pid, cols in parts.items():
+                by_part.setdefault(pid, []).append((it, cols))
+        for pid, rows in by_part.items():
+            d = os.path.join(self.path, f"partitionId={pid}")
+            os.makedirs(d, exist_ok=True)
+            offs = pa.array(np.r_[0, np.cumsum([len(r[1][0]) if r[1] else 0 for r in rows])], pa.int32())
+            cols = [pa.array([r[0] for r in rows], pa.int64())]
+            for a in range(len(self.names)):
+                cols.append(pa.ListArray.from_arrays(offs, pa.concat_arrays([r[1][a] for r in rows])))
+            pq.write_table(pa.Table.from_arrays(cols, schema=self.schema),
+                           os.path.join(d, f"part-{self.file_no:05d}.parquet"))
         self.file_no += 1
         self.buf = []
 
@@ -293,3 +378,14 @@ def save_credible_ball(rows, path):
         fh.write(CREDIBLE_BALL_HEADER + "\n")
         for row in rows:
             fh.write(",".join(repr(x) if isinstance(x, float) else str(x) for x in row) + "\n")
+
+
+def save_entity_values(attribute_names, rows, path):
+    """entity-values.csv under `path`: header cluster,size,<attr>,<attr>Probability,... (matching attributes in config
+    order), then rows as analysis_arrays.entity_value_rows gives them, CSV-quoted where a value needs it."""
+    import csv
+
+    with open(os.path.join(path, "entity-values.csv"), "w", newline="") as fh:
+        out = csv.writer(fh, lineterminator="\n")
+        out.writerow(["cluster", "size"] + [x for a in attribute_names for x in (a, a + "Probability")])
+        out.writerows(rows)

@@ -477,6 +477,34 @@ int dbl_vi_search(dbl_vi *, const int64_t *step /* R, host */, const int32_t *st
                   int32_t max_rounds, int32_t *labels_out /* R */, int32_t *rounds_out, int32_t *converged_out,
                   int64_t *moves, int64_t *clusters, int64_t *dJ /* max_rounds each, host */, int64_t *J0_out);
 
+/* ---------------------------------------------------------------------------------------------------
+ * The posterior of the entity values of a point estimate's clusters, one attribute per object, on the device that is
+ * current when dbl_values_create() is called.  labels (R int32 in [0, C), host or device, uploaded once) gives each
+ * record its cluster c of the estimate; samples are fed one at a time as values[R], the value id in [0, V) of the
+ * entity record r links to in that sample, for this attribute.  With S samples added:
+ *   count(c, v) = sum over samples s and records r of c of 1[values_s[r] = v], int64; sum over v = |c| S.
+ * The object holds a sorted table of (c << bits(V) | v, int64 count) over the keys seen so far (16 bytes each, twice:
+ * the table and the one the next sample merges into; they grow on demand).
+ *   dbl_values_add_sample  values may be a host or a device pointer (ready when the call is made); one key per record,
+ *                      radix-sorted over bits(C) + bits(V) bits, run-length encoded and merged into the table with the
+ *                      run lengths as counts (the merge kernels of dbl_pairs).  DBL_ERR_INVALID, adding nothing: a NULL
+ *                      pointer, a value outside [0, V), S reaching INT32_MAX
+ *   dbl_values_modes   per cluster c its mode (the v of largest count(c, v), ties to the smallest v; -1 for a label no
+ *                      record has) into mode_out[C] and that count into count_out[C], host or device pointers; a
+ *                      segmented arg-max over the held table.  DBL_ERR_INVALID: a NULL pointer; DBL_ERR_STATE before
+ *                      the first sample.  The table and S do not change.
+ * DBL_ERR_INVALID: a NULL pointer, num_records outside [1, 2^31 - 1], num_clusters or num_values below 1, or a label
+ * outside [0, C) (no object is created).  DBL_ERR_CUDA: no device, or an allocation that fails (44 bytes per record
+ * up front; the held table and the sample count stay as they were).  Every refusal leaves the object usable.
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct dbl_values dbl_values;
+int dbl_values_create(dbl_values **out, int64_t num_records, const int32_t *labels /* R, host or device, in [0, C) */,
+                      int32_t num_clusters, int32_t num_values);
+void dbl_values_free(dbl_values *);
+int dbl_values_add_sample(dbl_values *, const int32_t *values /* R, host or device, in [0, V) */);
+int32_t dbl_values_num_samples(const dbl_values *);
+int dbl_values_modes(dbl_values *, int32_t *mode_out /* C */, int64_t *count_out /* C */);
+
 /* The protocol functions of the theta draw (DESIGN.md 4.5), exposed so that they can be checked without a GPU:
  * log / exp built from individually rounded binary64 operations, and updateDistProbs (GU:305-320) itself. */
 double dbl_det_log(double x);
