@@ -139,6 +139,9 @@ SIGNATURES = {
     "dbl_pairs_score_sample": (C.c_int, [vp, vp, i64p, i64p]),
     "dbl_pairs_binder_search": (C.c_int, [vp, C.c_int64, C.c_int64, vp, C.c_int32, vp, i32p, i32p, i64p, i64p, i64p,
                                           i64p, i64p]),
+    "dbl_pairs_trace_begin": (C.c_int, [vp, C.c_int32]),
+    "dbl_pairs_trace_sample": (C.c_int, [vp, vp, C.c_int32]),
+    "dbl_pairs_mixing": (C.c_int, [vp, C.c_int32, C.c_int32, i32p, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]),
     "dbl_eval_create": (C.c_int, [C.POINTER(vp), C.c_int64, vp, C.c_int32]),
     "dbl_eval_free": (None, [vp]),
     "dbl_eval_add_sample": (C.c_int, [vp, vp]),

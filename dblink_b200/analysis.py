@@ -72,6 +72,62 @@ def pairwise_match_probabilities(chain):
     return {pair: k / n for pair, k in count.items()}
 
 
+def pairwise_match_diagnostics(chains):
+    """chains: K lists of samples, each sample the set of record pairs (frozensets) it puts in one cluster.  For every
+    pair linked in some sample, its 0/1 draws, each chain cut to the shortest chain's n draws and split into halves
+    [0, N) and [n - N, n), N = n // 2 -> (linked draws, least and largest per-chain count, max_t, split-R̂, ESS), by
+    the definitions of Vehtari, Gelman, Simpson, Carpenter & Bürkner (2021) in exact fractions: biased autocovariances
+    of each half, W = mean within-half variance, B / N = variance of the half means, var+ = (N - 1) / N W + B / N,
+    R̂ = sqrt(var+ / W), rho[0] = 1 and rho[t] = 1 - (W - mean autocovariance at lag t) / var+, then Geyer's initial
+    positive sequence, initial monotone sequence and truncated estimator, ESS = M N / max(tau, 1 / log10(M N))."""
+    F = fractions.Fraction
+    n = min(len(ch) for ch in chains)
+    N, M = n // 2, 2 * len(chains)
+    pairs = {p for ch in chains for s in ch for p in s}
+    floor = 1.0 / math.log10(M * N)
+    out = {}
+    for pair in pairs:
+        per_chain = [[int(pair in s) for s in ch[:n]] for ch in chains]
+        halves = [x[:N] for x in per_chain] + [x[n - N:] for x in per_chain]
+        means = [F(sum(h), N) for h in halves]
+        acov = [[F(sum((h[t] - mu) * (h[t + tau] - mu) for t in range(N - tau)), N) for tau in range(N)]
+                for h, mu in zip(halves, means)]
+        W = sum(a[0] * F(N, N - 1) for a in acov) / M
+        grand = sum(means) / M
+        B_over_N = sum((mu - grand) ** 2 for mu in means) / (M - 1)
+        var_plus = F(N - 1, N) * W + B_over_N
+        count = sum(sum(h) for h in halves)
+        chain_counts = [sum(x[:N]) + sum(x[n - N:]) for x in per_chain]
+        if var_plus == 0:
+            out[pair] = (count, min(chain_counts), max(chain_counts), 0, float("nan"), float("nan"))
+            continue
+        rhat = math.sqrt(var_plus / W) if W > 0 else float("inf")
+        rho = [F(1)] + [1 - (W - sum(a[tau] for a in acov) / M) / var_plus for tau in range(1, N)]
+        # Geyer's initial positive sequence
+        rho_p = [F(0)] * N
+        t = 0
+        even, odd = rho[0], rho[1]
+        rho_p[0], rho_p[1] = even, odd
+        while t < N - 5 and even + odd > 0:
+            t += 2
+            even, odd = rho[t], rho[t + 1]
+            if even + odd >= 0:
+                rho_p[t], rho_p[t + 1] = even, odd
+        max_t = t
+        if even > 0:
+            rho_p[max_t] = even
+        # initial monotone sequence
+        t = 2
+        while t <= max_t - 2:
+            if rho_p[t] + rho_p[t + 1] > rho_p[t - 2] + rho_p[t - 1]:
+                rho_p[t] = rho_p[t + 1] = (rho_p[t - 2] + rho_p[t - 1]) / 2
+            t += 2
+        tau_hat = -1 + 2 * sum(rho_p[:max_t]) + rho_p[max_t]
+        ess = float(F(M * N) / tau_hat) if tau_hat > floor else M * N / floor
+        out[pair] = (count, min(chain_counts), max(chain_counts), max_t, rhat, ess)
+    return out
+
+
 def binder_clusters(chain, false_link_cost=0.5):
     """The sample of least posterior expected Binder loss, by the definition: a pair linked in the sample costs
     t (1 - p), a pair not linked costs (1 - t) p, summed over every pair of records, where t = false_link_cost and p

@@ -294,6 +294,188 @@ def sample_labels(num_records, members, offsets):
     return labels
 
 
+# ---- per-pair MCMC diagnostics of the match probabilities ------------------------------------------------
+# For a pair, x_s = 1[the two records share a cluster in sample s].  Each of K chains, cut to the first n draws (n =
+# the shortest chain's), gives two halves [0, N) and [n - N, n), N = n // 2: M = 2K halves, as convergence.split_rhat
+# splits them.  With c_m the linked draws of half m, per lag tau in [0, N) the integers
+#   L_m[tau] = sum_{t < N - tau} x_t x_{t + tau},  h_m[tau] = sum_{t < N - tau} x_t,  g_m[tau] = sum_{t >= tau} x_t,
+#   Q_m[tau] = N^2 L - N c (h + g) + (N - tau) c^2 = N^3 x the half's biased autocovariance at lag tau,
+# A = sum_m Q_m, Bn = M sum c_m^2 - (sum c_m)^2, V = (M - 1)(N - 1) A[0] + N (N - 1) Bn and Wn = (M - 1) N A[0]
+# (var+ and W of Vehtari et al. 2021, scaled by M (M - 1) N^3 (N - 1)) give split-R̂ = sqrt(V / Wn) and, from
+# u[tau] = 2 (V - Wn + (M - 1)(N - 1) A[tau]) (u[0] = 2 V, so rho[tau] = u[tau] / 2V), the effective sample size by
+# Geyer's initial positive and initial monotone sequences.  Every comparison is on int64 u, and the monotone step keeps
+# each pair sum at the running minimum of the pair sums before it, so one pass over the lags suffices.
+MAX_TRACE_WORDS = 1 << 31    # uint32 words of the GPU's bit trace, [ceil(S / 32)][held pairs]
+MIXING_SIZE_BOUND = 1 << 30  # M N^2 below this keeps every integer above inside int64 (M^2 N^4 < 2^60)
+MIN_DRAWS = 4                # convergence.MIN_DRAWS
+
+
+def chain_draws(chain):
+    """(starts int32[K], n) of a pooled ChainArrays: chain k's draws are pooled positions starts[k] .. starts[k] + n - 1,
+    n = the shortest chain's number of samples.  The one place that decides which draws the diagnostics use."""
+    chains = np.asarray(chain.chains, np.int64)
+    K = int(chains.max()) + 1 if len(chains) else 1
+    counts = np.bincount(chains, minlength=K)
+    if len(chains) and (np.diff(chains) < 0).any():
+        raise ValueError("the pooled samples are not chain-major")
+    n = int(counts.min())
+    if n < MIN_DRAWS:
+        raise ValueError(f"pairwise-match-diagnostics needs at least {MIN_DRAWS} draws per chain after the cutoff")
+    return np.r_[0, np.cumsum(counts)[:-1]].astype(np.int32), n
+
+
+def check_mixing_size(num_chains, draws):
+    M, N = 2 * int(num_chains), int(draws) // 2
+    if M * N * N >= MIXING_SIZE_BOUND:
+        raise ValueError(f"pairwise-match-diagnostics needs M N^2 < 2^30: {M} half-chains of {N} draws")
+
+
+def check_trace_size(num_samples, num_pairs):
+    words = -(-int(num_samples) // 32) * int(num_pairs)
+    if words > MAX_TRACE_WORDS:
+        raise ValueError(f"the match trace needs {words} words, more than {MAX_TRACE_WORDS}")
+
+
+def ess_floor(num_chains, draws):
+    """1 / log10(M N), the least autocorrelation time the ESS divides by."""
+    return 1.0 / math.log10(2 * int(num_chains) * (int(draws) // 2))
+
+
+def pairwise_match_trace(chain, keys):
+    """bool[len(keys), S]: x[i, s] = 1 when the pair keys[i] (first << 32 | second, sorted) shares a cluster in pooled
+    sample s."""
+    keys = np.asarray(keys, np.int64)
+    x = np.zeros((len(keys), len(chain.samples)), bool)
+    if len(keys) == 0:
+        return x
+    for s, (mem, off, _) in enumerate(chain.samples):
+        k = sample_pair_keys(chain.num_records, mem, off)
+        pos = np.minimum(np.searchsorted(keys, k), len(keys) - 1)
+        hit = keys[pos] == k
+        x[pos[hit], s] = True
+    return x
+
+
+def pack_trace(x):
+    """bool[H, P] -> uint32[ceil(P / 32), H], the GPU's word-major bit trace (bit p % 32 of word p // 32)."""
+    H, P = x.shape
+    W = -(-P // 32)
+    pad = np.zeros((H, 32 * W), bool)
+    pad[:, :P] = x
+    return np.packbits(pad.reshape(H, W, 4, 8), axis=-1, bitorder="little").reshape(H, W * 4).view("<u4").T.copy()
+
+
+class MatchMixing:
+    """Per pair, int64 arrays count (linked draws of the 2 K N used), chain_min / chain_max (the least and largest of
+    one chain's), max_t (the lag where the initial positive sequence truncates) and float64 rhat, ess; with M halves
+    of N = draws // 2 draws from each chain's first `draws`."""
+
+    def __init__(self, count, chain_min, chain_max, max_t, rhat, ess, M, draws):
+        self.count, self.chain_min, self.chain_max, self.max_t = count, chain_min, chain_max, max_t
+        self.rhat, self.ess, self.M, self.draws, self.N = rhat, ess, M, draws, draws // 2
+
+
+def mixing_from_trace(x, starts, n, floor):
+    """The diagnostics of every row of a bool trace x[H, P] over the chains starts[k] .. starts[k] + n - 1: a
+    MatchMixing, equal bit for bit to dbl_pairs_mixing.  The per-lag integers are taken vectorised over the pairs, one
+    lag pair at a time, while any pair's sequence has not truncated."""
+    starts = [int(s) for s in starts]
+    K, n = len(starts), int(n)
+    N, M = n // 2, 2 * len(starts)
+    check_mixing_size(K, n)
+    H = x.shape[0]
+    halves = [np.ascontiguousarray(x[:, s + o:s + o + N], np.uint8) for s in starts for o in (0, n - N)]
+    c = np.stack([h.sum(1, dtype=np.int64) for h in halves]).reshape(M, H)  # [M, H]
+    chain_c = c[0::2] + c[1::2]                                    # halves of one chain are adjacent
+    S1, S2 = c.sum(0), (c * c).sum(0)
+    A0 = sum(N * c[m] - c[m] * c[m] for m in range(M)) * N         # Q_m[0] = N (N c - c^2)
+    V = (M - 1) * (N - 1) * A0 + N * (N - 1) * (M * S2 - S1 * S1)
+    Wn = (M - 1) * N * A0
+
+    def u_at(tau, rows):
+        if tau == 0:
+            return 2 * V[rows]
+        A = np.zeros(len(rows), np.int64)
+        for m, h in enumerate(halves):
+            hm = h[rows]
+            L = (hm[:, :N - tau] & hm[:, tau:]).sum(1, dtype=np.int64)
+            hh, gg = hm[:, :N - tau].sum(1, dtype=np.int64), hm[:, tau:].sum(1, dtype=np.int64)
+            cm = c[m, rows]
+            A += N * N * L - N * cm * (hh + gg) + (N - tau) * cm * cm
+        return 2 * (V[rows] - Wn[rows] + (M - 1) * (N - 1) * A)
+
+    max_t = np.zeros(H, np.int64)
+    acc = np.zeros(H, np.float64)
+    last = np.zeros(H, np.int64)
+    live = np.flatnonzero(V != 0)
+    even, odd = u_at(0, live), u_at(1, live)
+    P = even + odd
+    cur = P.copy()                                                 # the pair sum after the monotone step
+    t = 0
+    while len(live):
+        stop = ~((t < N - 5) & (P > 0))
+        done = live[stop]
+        max_t[done] = t
+        last[done] = np.where((P[stop] >= 0) | (even[stop] > 0), even[stop], 0)
+        keep = ~stop
+        live, cur = live[keep], cur[keep]
+        if not len(live):
+            break
+        acc[live] = acc[live] + cur.astype(np.float64)            # the pair before max_t, in ascending lag order
+        t += 2
+        even, odd = u_at(t, live), u_at(t + 1, live)
+        P = even + odd
+        cur = np.minimum(P, cur)
+    rhat = np.full(H, np.nan)
+    ess = np.full(H, np.nan)
+    pos = V != 0
+    with np.errstate(divide="ignore"):
+        rhat[pos] = np.sqrt(V[pos].astype(np.float64) / Wn[pos].astype(np.float64))
+    num = (acc + acc) + last.astype(np.float64)
+    tau_hat = -1.0 + num[pos] / (2 * V[pos]).astype(np.float64)
+    ess[pos] = np.float64(M * N) / np.where(tau_hat > floor, tau_hat, floor)
+    return MatchMixing(S1, chain_c.min(0), chain_c.max(0), max_t, rhat, ess, M, n)
+
+
+def mcse(count, num_draws, ess):
+    """Monte Carlo standard error of a probability count / num_draws with effective sample size ess:
+    sqrt(count (D - count) / (D (D - 1)) / ess), D = num_draws."""
+    count = np.asarray(count, np.int64)
+    D = int(num_draws)
+    var = (count * (D - count)).astype(np.float64) / float(D * (D - 1))
+    with np.errstate(invalid="ignore"):
+        return np.sqrt(var / np.asarray(ess, np.float64))
+
+
+def match_diagnostics_summary(mix, num_chains, draws):
+    """The (quantity, value) rows of pairwise-match-diagnostics-summary.csv over the pairs of a MatchMixing: the pairs
+    with R̂ above 1.01 and 1.1 (inf included), with R̂ = inf and with R̂ undefined (NaN), the least and the median of
+    the defined ESS, and the pairs with ESS below 100 per chain."""
+    K = int(num_chains)
+    rhat, ess = np.asarray(mix.rhat), np.asarray(mix.ess)
+    defined = ess[~np.isnan(ess)]
+    return [("numChains", K), ("drawsPerChain", int(draws)), ("pairs", len(rhat)),
+            ("pairsRhatAbove1.01", int((rhat > 1.01).sum())), ("pairsRhatAbove1.1", int((rhat > 1.1).sum())),
+            ("pairsRhatInf", int(np.isinf(rhat).sum())), ("pairsRhatUndefined", int(np.isnan(rhat).sum())),
+            ("minEss", float(defined.min()) if len(defined) else float("nan")),
+            ("medianEss", float(np.median(defined)) if len(defined) else float("nan")),
+            ("pairsEssBelow100PerChain", int((defined < 100 * K).sum()))]
+
+
+def pairwise_match_diagnostics(chain, min_count=1, max_pairs=MAX_PAIRS):
+    """(first, second, count, MatchMixing) over the pairs with count >= min_count (pairwise_match_counts' rows, count
+    over every pooled sample), the diagnostics over the draws chain_draws picks.  Raises ValueError for fewer than
+    MIN_DRAWS draws per chain, M N^2 >= 2^30 or a trace of more than MAX_TRACE_WORDS words."""
+    starts, n = chain_draws(chain)
+    check_mixing_size(len(starts), n)
+    first, second, count = pairwise_match_counts(chain, max_pairs)
+    check_trace_size(len(chain.samples), len(first))
+    keep = count >= min_count
+    first, second, count = first[keep], second[keep], count[keep]
+    x = pairwise_match_trace(chain, (first << 32) | second)
+    return first, second, count, mixing_from_trace(x, starts, n, ess_floor(len(starts), n))
+
+
 # ---- the Binder-loss point estimate ---------------------------------------------------------------------
 # With count(i, j) = the samples in which records i and j share a cluster (p_ij = count / S) and t = the cost of a
 # false link (1 - t that of a missed link), the posterior expected Binder loss of a partition c is

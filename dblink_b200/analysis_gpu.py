@@ -18,6 +18,8 @@ and the cells of any labelling with every held sample, summed or per sample, equ
 vi_label_cells / vi_sample_cells exactly, on the same handle.  The entity-value counts of a point estimate's clusters
 equal analysis_arrays.EntityValueCounts exactly: the device keeps the sorted table of (cluster, value) keys and int64
 counts per attribute and merges each sample's run-length-encoded keys into it; the modes are a segmented arg-max.
+The per-pair split-R̂ and ESS equal analysis_arrays.pairwise_match_diagnostics bit for bit: a bit trace per held pair,
+then integer lag statistics and the same rounded double operations per pair on the device.
 """
 import ctypes as C
 
@@ -181,6 +183,28 @@ class Pairs(_Handle):
                    C.byref(K))
         return SearchRun(labels.astype(np.int64), *(x[:rounds.value] for x in logs), converged.value, n.value, K.value)
 
+    def trace_begin(self, num_positions):
+        """A zeroed bit trace of num_positions bits per held pair (dropped by the next add_sample)."""
+        self._call("trace_begin", self._h, int(num_positions))
+
+    def trace_sample(self, cluster, position):
+        """Sets bit `position` of every held pair that labelling cluster[R] puts together."""
+        cluster = np.ascontiguousarray(cluster, np.int32)
+        if cluster.shape != (self.num_records,):
+            raise ValueError("a sample needs one cluster label per record")
+        self._call("trace_sample", self._h, cluster.ctypes.data, int(position))
+
+    def mixing(self, min_count, starts, draws, floor):
+        """An analysis_arrays.MatchMixing of the held pairs with count >= min_count, in read() order, over the chains
+        of `draws` trace positions from starts[k]."""
+        starts = np.ascontiguousarray(starts, np.int32)
+        n = self.count(min_count)
+        i32 = [np.empty(n, np.int32) for _ in range(4)]
+        f64 = [np.empty(n, np.float64) for _ in range(2)]
+        self._call("mixing", self._h, int(min_count), len(starts), starts.ctypes.data_as(_lib.i32p), int(draws),
+                   float(floor), *(a.ctypes.data for a in i32 + f64))
+        return analysis_arrays.MatchMixing(*(a.astype(np.int64) for a in i32), *f64, 2 * len(starts), int(draws))
+
 
 def _add_pairs(pairs, chain, max_pairs):
     """Every sample of a ChainArrays into a Pairs handle; the cap refusal as analysis_arrays raises it."""
@@ -214,6 +238,24 @@ def binder_counts(chain, max_pairs=MAX_PAIRS):
         for s, (mem, off, _) in enumerate(chain.samples):
             n[s], K[s] = pairs.score_sample(sample_clusters(R, mem, off))
     return n, K
+
+
+def pairwise_match_diagnostics(chain, min_count=1, max_pairs=MAX_PAIRS):
+    """(first, second, count, MatchMixing), identical to analysis_arrays.pairwise_match_diagnostics(chain, min_count,
+    max_pairs), refusals included: pass 1 adds every sample to one handle, the trace pass marks every pooled sample's
+    held pairs, then one mixing call."""
+    starts, n = analysis_arrays.chain_draws(chain)
+    analysis_arrays.check_mixing_size(len(starts), n)
+    R, S = chain.num_records, len(chain.samples)
+    with Pairs(R, max_pairs) as pairs:
+        _add_pairs(pairs, chain, max_pairs)
+        analysis_arrays.check_trace_size(S, pairs.count())
+        pairs.trace_begin(S)
+        for s, (mem, off, _) in enumerate(chain.samples):
+            pairs.trace_sample(sample_clusters(R, mem, off), s)
+        first, second, count = pairs.read(min_count)
+        mix = pairs.mixing(min_count, starts, n, analysis_arrays.ess_floor(len(starts), n))
+    return first, second, count, mix
 
 
 def binder_search(chain, false_link_cost, starts, max_rounds=1000, max_pairs=MAX_PAIRS):

@@ -187,6 +187,11 @@ struct Buf {
     std::swap(cap, nb.cap);
     return cudaSuccess;
   }
+  void reset() {
+    if (p) cudaFree(p);
+    p = nullptr;
+    cap = 0;
+  }
   template <class T> T *as() const { return (T *)p; }
 };
 
@@ -580,6 +585,8 @@ struct dbl_pairs : Handle {
   int cur = 0;
   Buf tmp;                              // CUB temporary storage, grown on demand
   Buf score;                            // the uint64 count sum of dbl_pairs_score_sample
+  Buf trace;                            // dbl_pairs_trace_begin: [ceil(P / 32)][H] uint32 bits, word-major
+  int32_t trace_P = 0;                  // its positions P; 0 = no trace
 };
 
 extern "C" int dbl_pairs_create(dbl_pairs **out, int64_t num_records, int64_t max_pairs) {
@@ -691,6 +698,8 @@ extern "C" int dbl_pairs_add_sample(dbl_pairs *p, const int32_t *cluster) {
   p->cur = nxt;
   p->H = H2;
   ++p->S;
+  p->trace.reset();  // its rows were the old table's pairs
+  p->trace_P = 0;
   return DBL_OK;
 }
 
@@ -770,6 +779,222 @@ extern "C" int dbl_pairs_read(dbl_pairs *p, int32_t min_count, int32_t *first, i
   POST_TRY(cudaMemcpy(first, f.p, sizeof(int32_t) * n, cudaMemcpyDefault));
   POST_TRY(cudaMemcpy(second, s.p, sizeof(int32_t) * n, cudaMemcpyDefault));
   POST_TRY(cudaMemcpy(count, c.p, sizeof(int32_t) * n, cudaMemcpyDefault));
+  return DBL_OK;
+}
+
+// ---- per-pair MCMC diagnostics: split-R̂ and effective sample size of every held pair's link indicator -------------
+// A bit trace holds x_s(pair) = 1[the pair shares a cluster in sample s] for every held pair and pooled position s,
+// word-major ([ceil(P / 32)][H] uint32), filled one sample at a time by looking its pair keys up in the held table.
+// dbl_pairs_mixing splits each of K chains (n draws from a start position) into two halves of N = n / 2 draws and
+// computes, per pair, in int64 (see analysis_arrays.pairwise_match_diagnostics for the definitions):
+//   L_m[tau] = sum_{t < N - tau} x_t x_{t + tau},  h_m[tau] = sum_{t < N - tau} x_t,  g_m[tau] = sum_{t >= tau} x_t,
+//   Q_m[tau] = N^2 L - N c_m (h + g) + (N - tau) c_m^2  (N^3 x the half's biased autocovariance),  A = sum_m Q_m,
+//   V = (M - 1)(N - 1) A[0] + N (N - 1) (M sum c_m^2 - (sum c_m)^2),  Wn = (M - 1) N A[0],
+//   u[0] = 2 V,  u[tau] = 2 (V - Wn + (M - 1)(N - 1) A[tau]),
+// R̂ = sqrt(V / Wn), and Geyer's initial positive and monotone sequences over the lag pairs of u, streamed: the
+// monotone sequence makes each pair sum the running minimum of those before it.  Every integer fits int64 when
+// M N^2 < 2^30 (so M^2 N^4 < 2^60).
+namespace {
+constexpr int64_t MAX_TRACE_WORDS = int64_t(1) << 31;
+constexpr int64_t MIXING_SIZE_BOUND = int64_t(1) << 30;  // M N^2 below this
+
+// every key of one sample found in the held table sets bit `pos` of that pair's row; keys it does not hold are ignored
+__global__ void k_mark_pairs(int64_t n, const unsigned long long *__restrict__ keys, int64_t H,
+                             const unsigned long long *__restrict__ held, int32_t pos, uint32_t *__restrict__ trace) {
+  uint32_t *row = trace + (int64_t)(pos >> 5) * H;
+  const uint32_t bit = 1u << (pos & 31);
+  for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long k = keys[j];
+    const int64_t b = lower_bound_u64(held, H, k);
+    if (b < H && held[b] == k) atomicOr(row + b, bit);
+  }
+}
+
+// the low `k` bits set (none for k <= 0, all for k >= 32)
+__device__ __forceinline__ uint32_t low_bits(int64_t k) {
+  return k <= 0 ? 0u : k >= 32 ? 0xffffffffu : (1u << k) - 1u;
+}
+
+// bits s .. s + 31 of pair h's row (positions at or past the trace's end read 0)
+__device__ __forceinline__ uint32_t trace_bits(const uint32_t *__restrict__ trace, int64_t H, int64_t W, int64_t h,
+                                               int64_t s) {
+  const int64_t w = s >> 5;
+  const uint32_t lo = w < W ? trace[w * H + h] : 0u, hi = w + 1 < W ? trace[(w + 1) * H + h] : 0u;
+  return __funnelshift_r(lo, hi, (uint32_t)(s & 31));
+}
+
+// One warp per held pair with count >= min_count, written at out[pos[h]].  The lanes take 32 lags at a time; each lane
+// walks the 2K halves once per batch, so the halves' counts come with every batch.  The Geyer pass runs on every lane
+// (the lag values are shuffled to all), and the warp stops as soon as the sequence truncates.
+__global__ void k_pair_mixing(int64_t H, const int32_t *__restrict__ flag, const int32_t *__restrict__ pos,
+                              const uint32_t *__restrict__ trace, int64_t W, int32_t K,
+                              const int32_t *__restrict__ starts, int32_t n, double ess_floor,
+                              int32_t *__restrict__ c_out, int32_t *__restrict__ cmin_out,
+                              int32_t *__restrict__ cmax_out, int32_t *__restrict__ maxt_out,
+                              double *__restrict__ rhat_out, double *__restrict__ ess_out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * WARPS_PER_BLOCK;
+  const int64_t N = n / 2, M = 2 * (int64_t)K, nw = (N + 31) / 32;
+  for (int64_t h = blockIdx.x * (int64_t)WARPS_PER_BLOCK + (threadIdx.x >> 5); h < H; h += nwarps) {
+    if (!flag[h]) continue;
+    long long V = 0, Wn = 0, acc_even = 0, run_min = 0, cur = 0, sum_c = 0;
+    int32_t cmin = INT32_MAX, cmax = 0;
+    int64_t t = 0;
+    double acc = 0.0;
+    bool stop = false;
+    for (int64_t base = 0; !stop; base += 32) {
+      const int64_t tau = base + lane;
+      long long A = 0, S1 = 0, S2 = 0;
+      for (int32_t k = 0; k < K; ++k) {
+        int32_t chain_c = 0;
+        for (int half = 0; half < 2; ++half) {
+          const int64_t s0 = (int64_t)starts[k] + (half ? n - N : 0);
+          long long L = 0, hh = 0, gg = 0, c = 0;
+          for (int64_t i = 0; i < nw; ++i) {
+            const uint32_t x = trace_bits(trace, H, W, h, s0 + 32 * i) & low_bits(N - 32 * i);
+            const uint32_t y = trace_bits(trace, H, W, h, s0 + tau + 32 * i);
+            const uint32_t mk = low_bits(N - tau - 32 * i);
+            L += __popc(x & y & mk);
+            hh += __popc(x & mk);
+            gg += __popc(y & mk);
+            c += __popc(x);
+          }
+          A += N * N * L - N * c * (hh + gg) + (N - tau) * c * c;
+          S1 += c;
+          S2 += c * c;
+          chain_c += (int32_t)c;
+        }
+        cmin = min(cmin, chain_c);
+        cmax = max(cmax, chain_c);
+      }
+      if (base == 0) {
+        const long long A0 = __shfl_sync(0xffffffffu, A, 0);
+        V = (M - 1) * (N - 1) * A0 + N * (N - 1) * (M * S2 - S1 * S1);
+        Wn = (M - 1) * N * A0;
+        sum_c = S1;
+        if (V == 0) break;
+      }
+      const long long u = tau == 0 ? 2 * V : 2 * (V - Wn + (M - 1) * (N - 1) * A);
+      // the lag pairs of this batch, in order, until the sequence truncates
+      for (int j = 0; j < 32 && !stop; j += 2) {
+        const long long even = __shfl_sync(0xffffffffu, u, j), odd = __shfl_sync(0xffffffffu, u, j + 1);
+        const long long P = even + odd;
+        if (base + j == 0) {
+          run_min = cur = P;
+        } else {
+          acc = __dadd_rn(acc, __ll2double_rn(cur));  // the previous pair lies before max_t
+          t = base + j;
+          cur = min(P, run_min);
+          run_min = cur;
+        }
+        if (!(t < N - 5 && P > 0)) {
+          stop = true;
+          acc_even = (P >= 0 || even > 0) ? even : 0;
+        }
+      }
+    }
+    if (lane == 0) {
+      const int64_t o = pos[h];
+      c_out[o] = (int32_t)sum_c;
+      cmin_out[o] = cmin;
+      cmax_out[o] = cmax;
+      if (V == 0) {
+        maxt_out[o] = 0;
+        rhat_out[o] = __longlong_as_double(0x7ff8000000000000ll);  // NaN
+        ess_out[o] = __longlong_as_double(0x7ff8000000000000ll);
+      } else {
+        maxt_out[o] = (int32_t)t;
+        rhat_out[o] = Wn > 0 ? __dsqrt_rn(__ddiv_rn(__ll2double_rn(V), __ll2double_rn(Wn)))
+                             : __longlong_as_double(0x7ff0000000000000ll);  // +inf
+        const double num = __dadd_rn(__dadd_rn(acc, acc), __ll2double_rn(acc_even));
+        const double tau_hat = __dadd_rn(-1.0, __ddiv_rn(num, __ll2double_rn(2 * V)));
+        ess_out[o] = __ddiv_rn(__ll2double_rn(M * N), tau_hat > ess_floor ? tau_hat : ess_floor);
+      }
+    }
+  }
+}
+}  // namespace
+
+// A zeroed trace of num_positions bits per held pair; replaces any earlier one.
+extern "C" int dbl_pairs_trace_begin(dbl_pairs *p, int32_t num_positions) {
+  if (!p || num_positions < 1) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  const int64_t W = ((int64_t)num_positions + 31) / 32;
+  if (p->H > 0 && W > MAX_TRACE_WORDS / p->H) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  p->trace.reset();
+  p->trace_P = 0;
+  const size_t bytes = sizeof(uint32_t) * (size_t)(W * p->H);
+  POST_TRY(p->trace.alloc(bytes));
+  POST_TRY(cudaMemsetAsync(p->trace.p, 0, bytes, p->stream));
+  POST_TRY(cudaStreamSynchronize(p->stream));
+  p->trace_P = num_positions;
+  return DBL_OK;
+}
+
+// One labelling's pairs (pairs_emit_sample) set bit `position` of the held pairs among them.
+extern "C" int dbl_pairs_trace_sample(dbl_pairs *p, const int32_t *cluster, int32_t position) {
+  if (!p || !cluster) return DBL_ERR_INVALID;
+  if (p->trace_P == 0) return DBL_ERR_STATE;
+  if (position < 0 || position >= p->trace_P) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  long long n = 0;
+  if (const int rc = pairs_emit_sample(p, cluster, &n); rc != DBL_OK) return rc;
+  cudaStream_t st = p->stream;
+  if (n > 0 && p->H > 0)
+    k_mark_pairs<<<grid_for(n), THREADS, 0, st>>>(n, p->key_in.as<unsigned long long>(), p->H,
+                                                  p->tab_key[p->cur].as<unsigned long long>(), position,
+                                                  p->trace.as<uint32_t>());
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
+// split-R̂ and ESS of every held pair with count >= min_count, in dbl_pairs_read order.
+extern "C" int dbl_pairs_mixing(dbl_pairs *p, int32_t min_count, int32_t num_chains, const int32_t *chain_starts,
+                                int32_t draws, double ess_floor, int32_t *count_out, int32_t *chain_min_out,
+                                int32_t *chain_max_out, int32_t *max_t_out, double *rhat_out, double *ess_out) {
+  if (!p || !chain_starts || !count_out || !chain_min_out || !chain_max_out || !max_t_out || !rhat_out || !ess_out)
+    return DBL_ERR_INVALID;
+  if (p->trace_P == 0) return DBL_ERR_STATE;
+  const int64_t N = draws / 2, M = 2 * (int64_t)num_chains;
+  // N <= 2^15 keeps M N^2 inside int64 for any K
+  if (num_chains < 1 || N < 2 || N > 32768 || M * N * N >= MIXING_SIZE_BOUND) return DBL_ERR_INVALID;
+  for (int32_t k = 0; k < num_chains; ++k)
+    if (chain_starts[k] < 0 || (int64_t)chain_starts[k] + draws > p->trace_P) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  const int64_t H = p->H, W = ((int64_t)p->trace_P + 31) / 32;
+  cudaStream_t st = p->stream;
+  Buf flag, pos, tmp, starts;
+  POST_TRY(flag.alloc(sizeof(int32_t) * (H + 1)));
+  POST_TRY(pos.alloc(sizeof(int32_t) * (H + 1)));
+  POST_TRY(starts.alloc(sizeof(int32_t) * num_chains));
+  POST_TRY(cudaMemcpyAsync(starts.p, chain_starts, sizeof(int32_t) * num_chains, cudaMemcpyHostToDevice, st));
+  size_t tb = 0;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, (const int32_t *)nullptr, (int32_t *)nullptr, H + 1, st));
+  POST_TRY(tmp.alloc(tb));
+  k_flag_min_count<<<grid_for(H + 1), THREADS, 0, st>>>(H, p->tab_cnt[p->cur].as<int32_t>(), min_count,
+                                                        flag.as<int32_t>());
+  POST_TRY(cub::DeviceScan::ExclusiveSum(tmp.p, tb, flag.as<int32_t>(), pos.as<int32_t>(), H + 1, st));
+  int32_t sel = 0;
+  POST_TRY(cudaMemcpyAsync(&sel, pos.as<int32_t>() + H, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  if (sel == 0) return DBL_OK;
+  Buf out4[4], out8[2];
+  for (Buf &b : out4) POST_TRY(b.alloc(sizeof(int32_t) * (size_t)sel));
+  for (Buf &b : out8) POST_TRY(b.alloc(sizeof(double) * (size_t)sel));
+  k_pair_mixing<<<(int)std::min<int64_t>((H + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, 8192), THREADS, 0, st>>>(
+      H, flag.as<int32_t>(), pos.as<int32_t>(), p->trace.as<uint32_t>(), W, num_chains, starts.as<int32_t>(), draws,
+      ess_floor, out4[0].as<int32_t>(), out4[1].as<int32_t>(), out4[2].as<int32_t>(), out4[3].as<int32_t>(),
+      out8[0].as<double>(), out8[1].as<double>());
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  // host or device outputs: unified addressing picks the copy direction
+  int32_t *o4[4] = {count_out, chain_min_out, chain_max_out, max_t_out};
+  double *o8[2] = {rhat_out, ess_out};
+  for (int i = 0; i < 4; ++i) POST_TRY(cudaMemcpy(o4[i], out4[i].p, sizeof(int32_t) * (size_t)sel, cudaMemcpyDefault));
+  for (int i = 0; i < 2; ++i) POST_TRY(cudaMemcpy(o8[i], out8[i].p, sizeof(double) * (size_t)sel, cudaMemcpyDefault));
   return DBL_OK;
 }
 

@@ -33,7 +33,7 @@ SUPPORTED_METRICS = (SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
                         "binder-search-clusters", "vi-clusters", "vi-search-clusters", "credible-ball",
-                        "entity-values")
+                        "entity-values", "pairwise-match-diagnostics")
 # the point estimates a credible ball may be centred on
 CREDIBLE_BALL_CENTERS = ("shared-most-probable-clusters", "binder-clusters", "binder-search-clusters", "vi-clusters",
                          "vi-search-clusters")
@@ -53,6 +53,15 @@ def pairwise_match_counts(chain, min_count=1):
     if _lib.load().dbl_device_count() > 0:
         return analysis_gpu.pairwise_match_counts(chain, min_count=min_count)
     return analysis_arrays.pairwise_match_counts(chain, min_count=min_count)
+
+
+def pairwise_match_diagnostics(chain, min_count=1):
+    """(first, second, count, MatchMixing) of a ChainArrays, the pairs that share a cluster in at least min_count
+    samples and their split-R̂ and ESS: on the GPU when the platform has one (analysis_gpu), else on the host
+    (analysis_arrays).  Both give identical arrays."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.pairwise_match_diagnostics(chain, min_count=min_count)
+    return analysis_arrays.pairwise_match_diagnostics(chain, min_count=min_count)
 
 
 def posterior_metric_counts(chain, truth):
@@ -416,6 +425,10 @@ class Project:
                     L.append(f"  * SummarizeStep: credible-ball is the smallest ball around a point estimate, in "
                              f"variation of information and in Binder distance, that holds a share of the samples, "
                              f"with {_credible_ball_settings(prm)}")
+                if "pairwise-match-diagnostics" in prm["quantities"]:
+                    L.append(f"  * SummarizeStep: pairwise-match-diagnostics gives split-R̂, effective sample size and "
+                             f"Monte Carlo standard error of every pair's link indicator, for the pairs of "
+                             f"minMatchProbability={prm['min_match_probability']!r}")
                 if "entity-values" in prm["quantities"]:
                     L.append(f"  * SummarizeStep: entity-values is the most probable value of each attribute of the "
                              f"entity of each cluster of a point estimate, from the entity values saved with the "
@@ -660,6 +673,15 @@ class Project:
                         first, second, count = pairwise_match_counts(ch, min_count=analysis_arrays.min_match_count(t, S))
                         writers.save_pairwise_match_probabilities(first, second, count, S, ch.record_ids, t,
                                                                   self.output_path)
+                    elif q == "pairwise-match-diagnostics":
+                        S, t = len(ch.samples), prm["min_match_probability"]
+                        first, second, count, mix = pairwise_match_diagnostics(
+                            ch, min_count=analysis_arrays.min_match_count(t, S))
+                        mcse = analysis_arrays.mcse(mix.count, mix.M * mix.N, mix.ess)
+                        writers.save_pairwise_match_diagnostics(first, second, count, S, mix, mcse, ch.record_ids,
+                                                                self.output_path)
+                        writers.save_pairwise_match_diagnostics_summary(
+                            analysis_arrays.match_diagnostics_summary(mix, mix.M // 2, mix.draws), self.output_path)
                     elif q == "binder-clusters":
                         s, labels, n, losses = binder_estimate(ch, prm["false_link_cost"])
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids),

@@ -257,6 +257,60 @@ def save_partition_sizes(sizes, path):
             fh.write(str(it) + "," + ",".join(str(sizes[it].get(p, 0)) for p in pids) + "\n")
 
 
+def pair_row_order(first, second, count, record_ids):
+    """The row order of pairwise-match-probabilities.csv: (ids as a large_string Arrow array, r1, r2, order), where
+    r1[i] < r2[i] in record-id code-point order and `order` sorts the pairs by count descending, then r1, then r2
+    (r1, r2 already in that order)."""
+    import pyarrow as pa
+    import pyarrow.compute as pc
+
+    first, second, count = np.asarray(first), np.asarray(second), np.asarray(count, np.int64)
+    ids = record_ids if isinstance(record_ids, pa.Array) else pa.array([str(r) for r in record_ids], pa.string())
+    ids = ids.cast(pa.large_string())
+    rank = np.empty(len(ids), np.int64)
+    rank[pc.sort_indices(ids).to_numpy()] = np.arange(len(ids))  # UTF-8 byte order = code-point order
+    swap = rank[first] > rank[second]
+    r1, r2 = np.where(swap, second, first), np.where(swap, first, second)
+    order = np.lexsort((rank[r2], rank[r1], -count))
+    return ids, r1[order], r2[order], order
+
+
+PAIRWISE_MATCH_DIAGNOSTICS_HEADER = ("recordId1,recordId2,probability,minChainProbability,maxChainProbability,splitRhat,"
+                                     "ess,mcse")
+
+
+def save_pairwise_match_diagnostics(first, second, count, num_samples, mix, mcse, record_ids, path):
+    """pairwise-match-diagnostics.csv under `path`: the rows of pairwise-match-probabilities.csv (the same pairs,
+    order and probability text, count / num_samples), each with its least and largest per-chain probability over the
+    2N draws of a chain the diagnostics use, split-R̂, ESS and MCSE (mix = an analysis_arrays.MatchMixing), written
+    with repr."""
+    S = int(num_samples)
+    with open(os.path.join(path, "pairwise-match-diagnostics.csv"), "w") as fh:
+        fh.write(PAIRWISE_MATCH_DIAGNOSTICS_HEADER + "\n")
+        if len(count) == 0:
+            return
+        ids, r1, r2, order = pair_row_order(first, second, count, record_ids)
+        ids = ids.to_pylist()
+        D = 2 * mix.N
+        count = np.asarray(count, np.int64)[order]
+        cols = [mix.chain_min[order], mix.chain_max[order], mix.rhat[order], mix.ess[order], np.asarray(mcse)[order]]
+        step = 1 << 16
+        for lo in range(0, len(order), step):
+            fh.write("".join(f"{ids[a]},{ids[b]},{c / S!r},{lo_c / D!r},{hi_c / D!r},{float(rh)!r},{float(e)!r},"
+                             f"{float(m)!r}\n"
+                             for a, b, c, lo_c, hi_c, rh, e, m in zip(r1[lo:lo + step], r2[lo:lo + step],
+                                                                     count[lo:lo + step].tolist(),
+                                                                     *(x[lo:lo + step].tolist() for x in cols))))
+
+
+def save_pairwise_match_diagnostics_summary(rows, path):
+    """pairwise-match-diagnostics-summary.csv under `path`: (quantity, value) rows, floats written with repr."""
+    with open(os.path.join(path, "pairwise-match-diagnostics-summary.csv"), "w") as fh:
+        fh.write("quantity,value\n")
+        for q, v in rows:
+            fh.write(f"{q},{v!r}\n")
+
+
 def save_pairwise_match_probabilities(first, second, count, num_samples, record_ids, threshold, path):
     """pairwise-match-probabilities.csv under `path`: header recordId1,recordId2,probability, then one row per pair
     with count / S >= threshold (float64; the row's text parses back to exactly count / S).  In a row recordId1 <
@@ -274,15 +328,8 @@ def save_pairwise_match_probabilities(first, second, count, num_samples, record_
             return
         count = np.asarray(count, np.int64)
         keep = count >= min_match_count(threshold, S)
-        first, second, count = np.asarray(first)[keep], np.asarray(second)[keep], count[keep]
-        ids = record_ids if isinstance(record_ids, pa.Array) else pa.array([str(r) for r in record_ids], pa.string())
-        ids = ids.cast(pa.large_string())
-        rank = np.empty(len(ids), np.int64)
-        rank[pc.sort_indices(ids).to_numpy()] = np.arange(len(ids))  # UTF-8 byte order = code-point order
-        swap = rank[first] > rank[second]
-        r1, r2 = np.where(swap, second, first), np.where(swap, first, second)
-        order = np.lexsort((rank[r2], rank[r1], -count))
-        r1, r2, count = r1[order], r2[order], count[order]
+        ids, r1, r2, order = pair_row_order(np.asarray(first)[keep], np.asarray(second)[keep], count[keep], record_ids)
+        count = count[keep][order]
         # repr: the shortest text that parses back to the same float64; one per possible count
         text = pa.array([repr(c / S) + "\n" for c in range(S + 1)], pa.large_string())
         step = 1 << 20

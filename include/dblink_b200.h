@@ -353,6 +353,28 @@ int dbl_posterior_smpc(dbl_posterior *, int32_t *labels_out /* R, may be NULL */
  *                         DBL_ERR_INVALID: a NULL pointer, max_rounds < 1, not 0 <= a <= b <= 2^16, S R >= 2^44, a
  *                         start label outside [0, R).  Memory: 48 bytes per held pair and 56 per record, for the call.
  *   count / read / score_sample / binder_search before the first sample give DBL_ERR_STATE.
+ *   dbl_pairs_trace_begin  a zeroed bit trace of num_positions bits per held pair, word-major ([ceil(P / 32)][H]
+ *                         uint32, bit p of pair h = bit p % 32 of word (p / 32) H + h), replacing any earlier trace.
+ *                         DBL_ERR_STATE before the first sample; DBL_ERR_INVALID: num_positions < 1, or more than 2^31
+ *                         words.  A later dbl_pairs_add_sample changes the held pairs, so it drops the trace.
+ *   dbl_pairs_trace_sample  any labelling cluster[R] (host or device pointer): sets bit `position` of every held pair
+ *                         it puts together; pairs the table does not hold are ignored, repeating a position changes
+ *                         nothing.  DBL_ERR_STATE: no trace; DBL_ERR_INVALID: position outside [0, P), a label outside
+ *                         [0, R), or its pairs alone exceeding max_pairs.  The table and S do not change.
+ *   dbl_pairs_mixing      per held pair with count >= min_count, in dbl_pairs_read order (dbl_pairs_count entries per
+ *                         output, host or device pointers): the standard MCMC diagnostics of its link indicator over K
+ *                         chains of `draws` = n trace positions from chain_starts[k] (host, K entries), each split
+ *                         into halves [0, N) and [n - N, n), N = n / 2, M = 2K halves:
+ *                           count_out      the linked draws over the 2 K N used draws
+ *                           chain_min_out / chain_max_out  the least and largest count of one chain over its 2N
+ *                           max_t_out      the lag where Geyer's initial positive sequence truncates
+ *                           rhat_out       split-R̂ = sqrt(var+ / W) (+inf when W = 0 < var+, NaN when var+ = 0)
+ *                           ess_out        M N / max(tau, ess_floor), tau = the integrated autocorrelation time by
+ *                                          Geyer's initial positive and monotone sequences (Vehtari et al. 2021);
+ *                                          NaN when var+ = 0
+ *                         computed in int64 and rounded doubles exactly as analysis_arrays.pairwise_match_diagnostics
+ *                         computes them.  DBL_ERR_STATE: no trace; DBL_ERR_INVALID: a NULL pointer, K < 1, N < 2,
+ *                         M N^2 >= 2^30, or a chain range outside [0, P).  Neither the table nor the trace changes.
  * DBL_ERR_INVALID: num_records or max_pairs outside [1, 2^31 - 1].  DBL_ERR_CUDA: no device, or an allocation that
  * fails (the held table and the sample count stay as they were).
  * ------------------------------------------------------------------------------------------------- */
@@ -369,6 +391,11 @@ int dbl_pairs_binder_search(dbl_pairs *, int64_t a, int64_t b, const int32_t *st
                             int32_t max_rounds, int32_t *labels_out /* R */, int32_t *rounds_out,
                             int32_t *converged_out, int64_t *moves, int64_t *dn, int64_t *dK /* max_rounds each, host */,
                             int64_t *n_out, int64_t *K_out);
+int dbl_pairs_trace_begin(dbl_pairs *, int32_t num_positions);
+int dbl_pairs_trace_sample(dbl_pairs *, const int32_t *cluster /* R, host or device */, int32_t position);
+int dbl_pairs_mixing(dbl_pairs *, int32_t min_count, int32_t num_chains, const int32_t *chain_starts /* K, host */,
+                     int32_t draws, double ess_floor, int32_t *count_out, int32_t *chain_min_out,
+                     int32_t *chain_max_out, int32_t *max_t_out, double *rhat_out, double *ess_out);
 
 /* ---------------------------------------------------------------------------------------------------
  * Every posterior sample against the ground truth: per sample, the integer counts its pairwise precision / recall /
