@@ -130,6 +130,7 @@ SIGNATURES = {
     "dbl_posterior_add_sample": (C.c_int, [vp, vp]),
     "dbl_posterior_num_samples": (C.c_int32, [vp]),
     "dbl_posterior_smpc": (C.c_int, [vp, i32p, f64p]),
+    "dbl_posterior_cluster_counts": (C.c_int, [vp, vp, C.c_int32, vp]),
     "dbl_pairs_create": (C.c_int, [C.POINTER(vp), C.c_int64, C.c_int64]),
     "dbl_pairs_free": (None, [vp]),
     "dbl_pairs_add_sample": (C.c_int, [vp, vp]),
@@ -142,6 +143,7 @@ SIGNATURES = {
     "dbl_pairs_trace_begin": (C.c_int, [vp, C.c_int32]),
     "dbl_pairs_trace_sample": (C.c_int, [vp, vp, C.c_int32]),
     "dbl_pairs_mixing": (C.c_int, [vp, C.c_int32, C.c_int32, i32p, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]),
+    "dbl_pairs_record_links": (C.c_int, [vp, vp, C.c_int32, vp, vp, vp, vp, vp, vp]),
     "dbl_eval_create": (C.c_int, [C.POINTER(vp), C.c_int64, vp, C.c_int32]),
     "dbl_eval_free": (None, [vp]),
     "dbl_eval_add_sample": (C.c_int, [vp, vp]),

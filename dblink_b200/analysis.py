@@ -9,6 +9,8 @@
   vi_search                                               <- single-record moves that lower the quantised expected
                                                              variation of information
   credible_ball                                           <- the samples within a VI or Binder radius of an estimate
+  clerical_review                                         <- each record's and cluster's expected false and missed
+                                                             links against an estimate, for a review queue
   entity_value_counts / entity_value_modes                <- the posterior of the entity values of an estimate's
                                                              clusters
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
@@ -372,6 +374,49 @@ def credible_ball(chain, center, level):
     return out
 
 
+def clerical_review(chain, center, false_link_cost, records):
+    """The clerical review of a point estimate by the definitions, with sets and Fractions: center = a list of sets of
+    record ids (cluster k = center[k]), records = the record ids in index order (the tie rules go by index), t =
+    false_link_cost, p(i, j) = the fraction of samples linking i and j.  Per record id i: W = the sum over the other
+    records of the samples linking them to i, I = the same over its cluster, FL = the sum over its cluster's other
+    records of 1 - p, ML = the sum over the records outside its cluster of p, A = the samples holding its cluster as
+    a cluster, and its strongest outside partner (largest p > 0, ties to the smaller index; None) with its count.  Per
+    cluster: size, probability (A / S), FL = half the members' FL, ML = the members' ML, loss = t FL + (1 - t) ML,
+    weakest = the least p over its pairs (None for a singleton), strongest = (inside id, outside id, p) of largest
+    p > 0, ties to the smaller inside then outside index (None).  Returns (records, clusters, review order: by loss
+    highest first, ties to the smaller k)."""
+    F = fractions.Fraction
+    t, S = F(false_link_cost), len(chain)
+    samples = [set(clusters_of_sample(s)) for s in chain]
+    count = collections.Counter(frozenset(p) for cl in samples for c in cl for p in itertools.combinations(c, 2))
+    index = {r: i for i, r in enumerate(records)}
+    center = [frozenset(c) for c in center]
+    cluster_of = {r: c for c in center for r in c}
+    recs = {}
+    for i in records:
+        mine = cluster_of[i]
+        n = {j: count[frozenset((i, j))] for j in records if j != i}
+        outside = [(n[j], j) for j in records if j not in mine and n[j] > 0]
+        best = min(outside, key=lambda x: (-x[0], index[x[1]])) if outside else (0, None)
+        recs[i] = dict(W=sum(n.values()), I=sum(n[j] for j in mine if j != i),
+                       FL=sum((1 - F(n[j], S) for j in mine if j != i), F(0)),
+                       ML=sum((F(n[j], S) for j in records if j not in mine), F(0)),
+                       A=sum(1 for cl in samples if mine in cl), partner=best[1], partner_count=best[0])
+    clusters = []
+    for c in center:
+        fl, ml = sum(recs[i]["FL"] for i in c) / 2, sum(recs[i]["ML"] for i in c)
+        links = [(count[frozenset((i, j))], i, j) for i in c for j in records
+                 if j not in c and count[frozenset((i, j))] > 0]
+        top = min(links, key=lambda x: (-x[0], index[x[1]], index[x[2]])) if links else None
+        clusters.append(dict(size=len(c), probability=F(sum(1 for cl in samples if c in cl), S), FL=fl, ML=ml,
+                             loss=t * fl + (1 - t) * ml,
+                             weakest=min(F(count[frozenset(p)], S) for p in itertools.combinations(c, 2))
+                             if len(c) > 1 else None,
+                             strongest=None if top is None else (top[1], top[2], F(top[0], S))))
+    order = sorted(range(len(center)), key=lambda k: (-clusters[k]["loss"], k))
+    return recs, clusters, order
+
+
 def cluster_size_distribution(chain):
     """iteration -> {cluster size: count} (LinkageChain.scala:137-154)."""
     out = {}
@@ -605,3 +650,18 @@ def entity_value_modes(counts, num_clusters, num_attributes):
             out[(k, a)] = (v, n)
     assert len(out) == num_clusters * num_attributes
     return out
+
+
+def format_clerical_review(res):
+    """The clerical-review section: res = the center, the clusters, the erroneous ones, the shares of them found in the
+    first 1 %, 5 % and 10 % of the review queue and of the queue by cluster probability, and the queue's normalised
+    area under the found-curve (analysis_arrays.clerical_review_evaluation)."""
+    def shares(x):
+        return f"{x[0]!r} in the first 1%, {x[1]!r} in 5%, {x[2]!r} in 10%"
+
+    return ("=====================================\n          Clerical review\n"
+            "-------------------------------------\n"
+            f" Center:          {res['center']}, {res['clusters']} clusters, {res['erroneous']} not a true entity\n"
+            f" Review queue:    found {shares(res['found'])}, area {res['area']!r}\n"
+            f" By probability:  found {shares(res['baseline'])}\n"
+            "=====================================\n")

@@ -1374,3 +1374,201 @@ def entity_value_rows(labels, modes, counts, num_samples, attribute_values):
             row += [strings[a][modes[a, k]], repr(int(counts[a, k]) / (size * num_samples))]
         rows.append(row)
     return rows
+
+
+# ---- clerical review of a point estimate ---------------------------------------------------------------
+# With count(i, j) the pair table of S samples and c a point estimate with canonical labels 0 .. C-1 (record i in
+# cluster c(i) of n(i) records), per record, in integers:
+#   W(i) = sum over j != i of count(i, j) = sum over the samples of (|C_s(i)| - 1),
+#   I(i) = the same sum over the j in c(i),
+#   S FL(i) = S (n(i) - 1) - I(i)   (S x the expected false links: partners in c that a sample does not link),
+#   S ML(i) = W(i) - I(i)           (S x the expected missed links: partners a sample links that c does not),
+#   A(i) = the samples in which i's cluster equals c(i) as a set (the cluster signatures of the sMPC).
+# Per cluster k: S FL_k = sum of S FL(i) / 2 (the sum is even), S ML_k = sum of S ML(i); the review order is by the
+# expected loss t FL_k + (1 - t) ML_k, highest first, ties to the smaller k, compared exactly with t = a / b.  Since
+# sum over k of S FL_k = S n(c) - K(c) and sum of S ML_k = 2 (C - K(c)), the sum over k of t FL_k + (1 - t) ML_k / 2 is
+# the expected Binder loss of c.
+REVIEW_SHARES = (1, 5, 10)  # the first 1 %, 5 % and 10 % of a review queue, in the evaluation
+
+
+def check_canonical(labels, num_clusters):
+    """Raise ValueError unless labels lie in [0, num_clusters) and every cluster holds a record."""
+    labels = np.asarray(labels, np.int64)
+    C = int(num_clusters)
+    if len(labels) and (labels.min() < 0 or labels.max() >= C):
+        raise ValueError("a cluster label outside [0, num_clusters)")
+    if C < 1 or C > max(len(labels), 1) or (np.bincount(labels, minlength=C) == 0).any():
+        raise ValueError("the labels are not canonical: a cluster in [0, num_clusters) holds no record")
+
+
+class RecordLinks:
+    """The integers of dbl_pairs_record_links, int64: per record W, I, the strongest partner outside its cluster (-1
+    when there is none) and its count; per cluster the held pairs inside it and their least count (0 when none)."""
+
+    def __init__(self, W, I, partner, partner_count, inner, least):  # noqa: E741
+        self.W, self.I, self.partner, self.partner_count, self.inner, self.least = (
+            np.asarray(x, np.int64) for x in (W, I, partner, partner_count, inner, least))
+
+
+def record_links(first, second, count, labels, num_clusters):
+    """RecordLinks of the canonical labels[R] (0 .. C-1) against the pair table (first, second, count)
+    (pairwise_match_counts): the same integers as analysis_gpu.record_links.  Strongest outside partner: the largest
+    count, ties to the smallest partner index."""
+    labels = np.asarray(labels, np.int64)
+    R, C = len(labels), int(num_clusters)
+    check_canonical(labels, C)
+    first, second, count = (np.asarray(x, np.int64) for x in (first, second, count))
+    W, I = np.zeros(R, np.int64), np.zeros(R, np.int64)  # noqa: E741
+    np.add.at(W, first, count)
+    np.add.at(W, second, count)
+    same = labels[first] == labels[second]
+    np.add.at(I, first[same], count[same])
+    np.add.at(I, second[same], count[same])
+    inner = np.bincount(labels[first[same]], minlength=C).astype(np.int64)
+    least = np.full(C, np.iinfo(np.int64).max, np.int64)
+    np.minimum.at(least, labels[first[same]], count[same])
+    least[inner == 0] = 0
+    a, b = np.r_[first[~same], second[~same]], np.r_[second[~same], first[~same]]
+    n = np.r_[count[~same], count[~same]]
+    by = np.lexsort((b, -n, a))
+    lead = by[np.r_[True, a[by][1:] != a[by][:-1]]] if len(by) else by
+    partner, partner_count = np.full(R, -1, np.int64), np.zeros(R, np.int64)
+    partner[a[lead]], partner_count[a[lead]] = b[lead], n[lead]
+    return RecordLinks(W, I, partner, partner_count, inner, least)
+
+
+def cluster_appearances(chain, labels):
+    """A, int64[R]: for the canonical labels[R], the samples of a ChainArrays in which each record's cluster equals
+    its cluster in labels as a set, by the cluster signatures of the sMPC (cluster_signatures): the same integers as
+    analysis_gpu.cluster_appearances."""
+    labels = np.asarray(labels, np.int64)
+    R = chain.num_records
+    if len(labels) != R:
+        raise ValueError("the labels need one cluster label per record")
+    C = int(labels.max()) + 1 if R else 0
+    check_canonical(labels, C)
+    center = ChainArrays(chain.record_ids, np.zeros(1, np.int64), [sample_from_links(labels, np.zeros(C, np.int32))])
+    return (cluster_signatures(chain) == cluster_signatures(center)[0]).sum(axis=0).astype(np.int64)
+
+
+class ClericalReview:
+    """The review of a point estimate with canonical labels[R] (0 .. C-1) over S samples, in integers: per record
+    S FL, S ML and A; per cluster size, A, S FL, S ML, the least internal count (-1 for a singleton), the strongest
+    outside link (inside record, outside record, count; -1, -1, 0 when there is none) and the review order."""
+
+    def __init__(self, links, appearances, labels, num_samples, false_link_cost):
+        labels = np.asarray(labels, np.int64)
+        S, C = int(num_samples), len(links.inner)
+        check_canonical(labels, C)
+        self.labels, self.num_samples, self.false_link_cost = labels, S, float(false_link_cost)
+        self.size = np.bincount(labels, minlength=C).astype(np.int64)
+        self.record_fl = S * (self.size[labels] - 1) - links.I
+        self.record_ml = links.W - links.I
+        self.record_appearances = np.asarray(appearances, np.int64)
+        self.partner, self.partner_count = links.partner, links.partner_count
+        self.appearances = np.zeros(C, np.int64)
+        self.appearances[labels] = self.record_appearances
+        fl2, self.ml = np.zeros(C, np.int64), np.zeros(C, np.int64)
+        np.add.at(fl2, labels, self.record_fl)
+        np.add.at(self.ml, labels, self.record_ml)
+        if (fl2 % 2).any():
+            raise ValueError("the false links of a cluster do not add up to an even number")
+        self.fl = fl2 // 2
+        self.weakest = np.where(self.size == 1, -1, np.where(links.inner == _comb2(self.size), links.least, 0))
+        # strongest outside link: over the members' own strongest partners, the largest count, ties to the smaller
+        # inside record, then to the smaller outside record (each member's partner is already its smallest of the count)
+        has = np.flatnonzero(self.partner >= 0)
+        by = has[np.lexsort((self.partner[has], has, -self.partner_count[has], labels[has]))]
+        lead = by[np.r_[True, labels[by][1:] != labels[by][:-1]]] if len(by) else by
+        self.inside, self.outside = np.full(C, -1, np.int64), np.full(C, -1, np.int64)
+        self.outside_count = np.zeros(C, np.int64)
+        self.inside[labels[lead]], self.outside[labels[lead]] = lead, self.partner[lead]
+        self.outside_count[labels[lead]] = self.partner_count[lead]
+        self.order = review_order(self.fl, self.ml, false_link_cost)
+
+    def losses(self):
+        """Per cluster t FL_k + (1 - t) ML_k as the float nearest the exact value."""
+        a, b = float(self.false_link_cost).as_integer_ratio()
+        return [float(fractions.Fraction(a * f + (b - a) * m, b * self.num_samples))
+                for f, m in zip(self.fl.tolist(), self.ml.tolist())]
+
+
+def review_order(fl, ml, false_link_cost):
+    """int64[C]: the clusters by expected loss t FL_k + (1 - t) ML_k, highest first, ties to the smaller k, compared
+    exactly: t = a / b and the integers a S FL_k + (b - a) S ML_k in Python integers (they may pass int64)."""
+    a, b = float(false_link_cost).as_integer_ratio()
+    score = [a * f + (b - a) * m for f, m in zip(np.asarray(fl).tolist(), np.asarray(ml).tolist())]
+    return np.array(sorted(range(len(score)), key=lambda k: (-score[k], k)), np.int64)
+
+
+def _ids(record_ids):
+    return [str(r) for r in (record_ids.to_pylist() if hasattr(record_ids, "to_pylist") else record_ids)]
+
+
+def clerical_review_rows(review, record_ids):
+    """The rows of clerical-review.csv: per cluster in review order (rank from 1, cluster, size, cluster probability,
+    expected false links, expected missed links, expected loss, weakest internal link probability, strongest outside
+    link's inside and outside record ids and probability); an empty field where a cluster has no such link."""
+    ids, S = _ids(record_ids), review.num_samples
+    losses = review.losses()
+    rows = []
+    for rank, k in enumerate(review.order.tolist(), 1):
+        w, i = int(review.weakest[k]), int(review.inside[k])
+        rows.append([rank, k, int(review.size[k]), repr(int(review.appearances[k]) / S), repr(int(review.fl[k]) / S),
+                     repr(int(review.ml[k]) / S), repr(losses[k]), "" if w < 0 else repr(w / S),
+                     "" if i < 0 else ids[i], "" if i < 0 else ids[int(review.outside[k])],
+                     "" if i < 0 else repr(int(review.outside_count[k]) / S)])
+    return rows
+
+
+def clerical_review_record_rows(review, record_ids):
+    """The rows of clerical-review-records.csv: per record in chain record order (record id, cluster, cluster
+    probability, expected false links, expected missed links, strongest outside record id and its probability)."""
+    ids, S = _ids(record_ids), review.num_samples
+    rows = []
+    for r, (k, a, f, m, j, n) in enumerate(zip(review.labels.tolist(), review.record_appearances.tolist(),
+                                                review.record_fl.tolist(), review.record_ml.tolist(),
+                                                review.partner.tolist(), review.partner_count.tolist())):
+        rows.append([ids[r], k, repr(a / S), repr(f / S), repr(m / S), "" if j < 0 else ids[j],
+                     "" if j < 0 else repr(n / S)])
+    return rows
+
+
+def erroneous_clusters(labels, truth):
+    """bool[C]: the clusters of the canonical labels that are not exactly one true entity."""
+    labels = np.asarray(labels, np.int64)
+    truth = np.unique(np.asarray(truth), return_inverse=True)[1].reshape(-1).astype(np.int64)
+    C, T = (int(labels.max()) + 1 if len(labels) else 0), (int(truth.max()) + 1 if len(truth) else 1)
+    cells, n = np.unique(labels * T + truth, return_counts=True)
+    cl, tr = cells // T, cells % T
+    cells_of = np.bincount(cl, minlength=C)
+    single = cells_of[cl] == 1
+    correct = np.zeros(C, bool)
+    correct[cl[single]] = n[single] == np.bincount(truth, minlength=T)[tr[single]]
+    return ~correct
+
+
+def _found_shares(found, erroneous):
+    """The share of the erroneous clusters in the first ceil(p C / 100) of a queue, p in REVIEW_SHARES (NaN when
+    there is none)."""
+    C = len(found)
+    return [found[-(-p * C // 100) - 1] / erroneous if erroneous else float("nan") for p in REVIEW_SHARES]
+
+
+def clerical_review_evaluation(review, truth):
+    """How well the review order finds the clusters that are not exactly a true entity: (rows of
+    clerical-review-evaluation.csv -- per queue position its rank, cluster, whether it is erroneous and the erroneous
+    clusters found so far -- and a summary dict: clusters, erroneous, the shares found in the first 1 %, 5 % and 10 %
+    of the queue, the normalised area under the found-curve and the same shares for the queue by cluster probability
+    alone, lowest first, ties to the smaller cluster).  The area is (sum of found(r) - worst) / (best - worst): the
+    share of (erroneous, correct) cluster pairs the queue puts in that order; NaN when every or no cluster is
+    erroneous."""
+    err = erroneous_clusters(review.labels, truth)
+    C, E = len(err), int(err.sum())
+    found = np.cumsum(err[review.order]).tolist()
+    rows = [[r + 1, k, int(err[k]), f] for r, (k, f) in enumerate(zip(review.order.tolist(), found))]
+    area = (float(fractions.Fraction(sum(found) - E * (E + 1) // 2, E * (C - E))) if 0 < E < C else float("nan"))
+    by_probability = np.lexsort((np.arange(C), review.appearances))
+    summary = dict(clusters=C, erroneous=E, found=_found_shares(found, E), area=area,
+                   baseline=_found_shares(np.cumsum(err[by_probability]).tolist(), E))
+    return rows, summary

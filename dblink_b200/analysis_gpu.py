@@ -19,7 +19,9 @@ vi_label_cells / vi_sample_cells exactly, on the same handle.  The entity-value 
 equal analysis_arrays.EntityValueCounts exactly: the device keeps the sorted table of (cluster, value) keys and int64
 counts per attribute and merges each sample's run-length-encoded keys into it; the modes are a segmented arg-max.
 The per-pair split-R̂ and ESS equal analysis_arrays.pairwise_match_diagnostics bit for bit: a bit trace per held pair,
-then integer lag statistics and the same rounded double operations per pair on the device.
+then integer lag statistics and the same rounded double operations per pair on the device.  The links of every record
+against a point estimate and the appearances of its clusters, for clerical review, equal analysis_arrays.record_links
+and cluster_appearances exactly: integer atomics over the held pair table, and the sMPC's signatures compared.
 """
 import ctypes as C
 
@@ -120,6 +122,16 @@ class Posterior(_Handle):
         self._call("smpc", self._h, labels.ctypes.data_as(_lib.i32p), freq.ctypes.data_as(_lib.f64p))
         return labels.astype(np.int64), freq
 
+    def cluster_counts(self, labels, num_clusters):
+        """A, int64[R]: for labels[R] canonical in [0, num_clusters), the held samples in which each record's cluster
+        equals its cluster in labels as a set."""
+        labels = np.ascontiguousarray(labels, np.int32)
+        if labels.shape != (self.num_records,):
+            raise ValueError("the labels need one cluster label per record")
+        count = np.empty(self.num_records, np.int32)
+        self._call("cluster_counts", self._h, labels.ctypes.data, int(num_clusters), count.ctypes.data)
+        return count.astype(np.int64)
+
 
 def most_probable_clusters(chain):
     """(labels, freq) of a ChainArrays: labels = the sMPC labels (the smallest record index of each group of records
@@ -205,6 +217,19 @@ class Pairs(_Handle):
                    float(floor), *(a.ctypes.data for a in i32 + f64))
         return analysis_arrays.MatchMixing(*(a.astype(np.int64) for a in i32), *f64, 2 * len(starts), int(draws))
 
+    def record_links(self, labels, num_clusters):
+        """An analysis_arrays.RecordLinks of labels[R], canonical in [0, num_clusters), against the held table.  The
+        table does not change."""
+        labels = np.ascontiguousarray(labels, np.int32)
+        if labels.shape != (self.num_records,):
+            raise ValueError("the labels need one cluster label per record")
+        R, C = self.num_records, int(num_clusters)
+        W, I, inner = np.empty(R, np.int64), np.empty(R, np.int64), np.empty(max(C, 0), np.int64)  # noqa: E741
+        partner, partner_count, least = np.empty(R, np.int32), np.empty(R, np.int32), np.empty(max(C, 0), np.int32)
+        self._call("record_links", self._h, labels.ctypes.data, C,
+                   *(a.ctypes.data for a in (W, I, partner, partner_count, inner, least)))
+        return analysis_arrays.RecordLinks(W, I, partner, partner_count, inner, least)
+
 
 def _add_pairs(pairs, chain, max_pairs):
     """Every sample of a ChainArrays into a Pairs handle; the cap refusal as analysis_arrays raises it."""
@@ -256,6 +281,26 @@ def pairwise_match_diagnostics(chain, min_count=1, max_pairs=MAX_PAIRS):
         first, second, count = pairs.read(min_count)
         mix = pairs.mixing(min_count, starts, n, analysis_arrays.ess_floor(len(starts), n))
     return first, second, count, mix
+
+
+def record_links(chain, labels, max_pairs=MAX_PAIRS):
+    """RecordLinks of the canonical labels[R] (0 .. C-1), identical to analysis_arrays.record_links(
+    *analysis_arrays.pairwise_match_counts(chain, max_pairs), labels, C): every sample goes into one handle, then one
+    pass over its table."""
+    labels = np.asarray(labels, np.int64)
+    R = chain.num_records
+    with Pairs(R, max_pairs) as pairs:
+        _add_pairs(pairs, chain, max_pairs)
+        return pairs.record_links(labels, int(labels.max()) + 1)
+
+
+def cluster_appearances(chain, labels):
+    """A, int64[R], identical to analysis_arrays.cluster_appearances(chain, labels): every sample's signatures go
+    into one dbl_posterior handle, then every record's row is compared with the signature of its cluster in labels."""
+    labels = np.asarray(labels, np.int64)
+    with Posterior(chain.num_records, len(chain.samples)) as post:
+        _add_chain(post, chain)
+        return post.cluster_counts(labels, int(labels.max()) + 1)
 
 
 def binder_search(chain, false_link_cost, starts, max_rounds=1000, max_pairs=MAX_PAIRS):

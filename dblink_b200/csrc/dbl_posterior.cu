@@ -38,6 +38,12 @@
 // sorted table of (c << bits(V) | v, count); each sample's keys are radix-sorted, run-length encoded and merged into
 // it by the merge kernels of dbl_pairs, with the run lengths as counts -- see dbl_values_add_sample.  The modes are a
 // segmented arg-max over the table (dbl_values_modes).
+//
+// Clerical review of a point estimate (same integers as analysis_arrays.record_links / cluster_appearances): per
+// record W, I and its strongest partner outside its cluster, per cluster its held internal pairs and their least
+// count, by one pass over the held pair table (dbl_pairs_record_links); per record the samples holding its cluster of
+// the estimate, by comparing its row of the sMPC signature matrix with the estimate's own signatures
+// (dbl_posterior_cluster_counts).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -53,6 +59,7 @@ namespace {
 // (signature, sample) pairs sorted per record block: bounds the block's temporaries (~2 GB) whatever R and S are
 constexpr int64_t PAIR_BLOCK = int64_t(1) << 26;
 constexpr int THREADS = 256;
+constexpr int WARPS_PER_BLOCK = THREADS / 32;
 
 __device__ __forceinline__ unsigned long long mix64(unsigned long long x) {  // splitmix64 finaliser
   x += 0x9E3779B97F4A7C15ull;
@@ -398,10 +405,67 @@ extern "C" int dbl_posterior_smpc(dbl_posterior *p, int32_t *labels_out, double 
   return DBL_OK;
 }
 
+// ---- how often each cluster of a labelling appears in the samples -------------------------------------------------
+namespace {
+// any of the C clusters without a record raises the flag (the labels are then not canonical for C)
+template <class T>
+__global__ void k_flag_empty(int64_t C, const T *__restrict__ size, int *__restrict__ bad) {
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < C; k += (int64_t)gridDim.x * blockDim.x)
+    if (size[k] == 0) *bad = 1;
+}
+
+// one warp per record: the samples whose signature of the record equals the center's, over its row of the
+// record-major signature matrix (32 consecutive samples per load)
+__global__ void k_match_center(int64_t R, int32_t stride, int32_t S, const unsigned long long *__restrict__ sig,
+                               const unsigned long long *__restrict__ center, int32_t *__restrict__ count) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * WARPS_PER_BLOCK;
+  for (int64_t r = blockIdx.x * (int64_t)WARPS_PER_BLOCK + (threadIdx.x >> 5); r < R; r += nwarps) {
+    const unsigned long long c = center[r], *row = sig + r * stride;
+    int32_t n = 0;
+    for (int32_t s = lane; s - lane < S; s += 32) n += __popc(__ballot_sync(0xffffffffu, s < S && row[s] == c));
+    if (lane == 0) count[r] = n;
+  }
+}
+}  // namespace
+
+// The labels (canonical for C) into the handle's label buffer and their cluster sizes by k_accumulate, which refuse
+// a label outside [0, C) and an empty cluster; the center's signatures by k_signatures as one column of an R x 1
+// matrix; then every record's row of the signature matrix against them.
+extern "C" int dbl_posterior_cluster_counts(dbl_posterior *p, const int32_t *labels, int32_t num_clusters,
+                                            int32_t *count_out) {
+  if (!p || !labels || !count_out || num_clusters < 1 || num_clusters > p->R) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(labels, p->cluster, num_clusters); rc != DBL_OK) return rc;
+  const int64_t R = p->R, C = num_clusters;
+  cudaStream_t st = p->stream;
+  const int32_t *c = p->cluster.as<int32_t>();
+  unsigned long long *sum = p->sum.as<unsigned long long>();
+  unsigned int *size = p->size.as<unsigned int>();
+  POST_TRY(cudaMemsetAsync(sum, 0, sizeof(unsigned long long) * R, st));
+  POST_TRY(cudaMemsetAsync(size, 0, sizeof(unsigned int) * R, st));
+  k_accumulate<<<grid_for(R), THREADS, 0, st>>>(R, c, sum, size);
+  k_flag_empty<<<grid_for(C), THREADS, 0, st>>>(C, size, p->bad.as<int>());  // bad is 0 after take_labels
+  int flag = 0;
+  POST_TRY(cudaMemcpyAsync(&flag, p->bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  if (flag) return DBL_ERR_INVALID;
+  Buf center, count;
+  POST_TRY(center.alloc(sizeof(unsigned long long) * R));
+  POST_TRY(count.alloc(sizeof(int32_t) * R));
+  k_signatures<<<grid_for(R), THREADS, 0, st>>>(R, 1, 0, c, sum, size, center.as<unsigned long long>());
+  k_match_center<<<(int)std::min<int64_t>((R + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, 8192), THREADS, 0, st>>>(
+      R, p->max_samples, p->S, p->sig.as<unsigned long long>(), center.as<unsigned long long>(), count.as<int32_t>());
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaMemcpyAsync(count_out, count.p, sizeof(int32_t) * R, cudaMemcpyDefault, st));
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
 // ---- posterior pairwise match counts -------------------------------------------------------------------------------
 namespace {
-constexpr int WARPS_PER_BLOCK = THREADS / 32;
-
 // bits needed to hold every value in [0, n)
 int bits_for(int64_t n) {
   int b = 1;
@@ -1282,6 +1346,151 @@ extern "C" int dbl_pairs_binder_search(dbl_pairs *p, int64_t a, int64_t b, const
   *converged_out = converged;
   *n_out = (int64_t)nk[0];
   *K_out = (int64_t)nk[1];
+  return DBL_OK;
+}
+
+// ---- every record's links against a labelling, for clerical review ------------------------------------------------
+namespace {
+// Per held pair (f, s, n), f < s: W of both records += n; when lab[f] == lab[s], I of both += n and the cluster gets
+// one more held internal pair and min= n as its least count; otherwise each record's strongest outside partner
+// max= n << 32 | (0xFFFFFFFF - partner), so ties go to the smaller partner.  The table is sorted by f, so the lanes
+// of a warp mostly share f: f's updates are reduced over each run of equal f in the warp (a segmented shuffle
+// reduction) and applied once by the run's first lane; s's go straight to atomics.  Every update is an integer
+// atomic, so the result does not depend on their order.
+__global__ void k_record_links(int64_t H, const unsigned long long *__restrict__ held, const int32_t *__restrict__ hcnt,
+                               const int32_t *__restrict__ lab, unsigned long long *__restrict__ W,
+                               unsigned long long *__restrict__ I, unsigned long long *__restrict__ best,
+                               unsigned long long *__restrict__ inner, unsigned int *__restrict__ least) {
+  const int lane = threadIdx.x & 31;
+  for (int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31); base < H;
+       base += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t e = base + lane;
+    uint32_t f = 0xffffffffu;  // no record: R <= 2^31 - 1
+    int32_t L = 0;
+    unsigned long long w = 0, in = 0, top = 0, pairs = 0;
+    unsigned int lo = 0xffffffffu;
+    if (e < H) {
+      const unsigned long long k = held[e];
+      f = (uint32_t)(k >> 32);
+      const uint32_t s = (uint32_t)(k & 0xffffffffull), n = (uint32_t)hcnt[e];
+      L = lab[f];
+      w = n;
+      atomicAdd(&W[s], w);
+      if (L == lab[s]) {
+        in = n;
+        pairs = 1;
+        lo = n;
+        atomicAdd(&I[s], in);
+      } else {
+        top = (unsigned long long)n << 32 | (0xffffffffu - s);
+        atomicMax(&best[s], (unsigned long long)n << 32 | (0xffffffffu - f));
+      }
+    }
+    const uint32_t prev = __shfl_up_sync(0xffffffffu, f, 1);
+    const bool head = lane == 0 || prev != f;
+    const unsigned later = __ballot_sync(0xffffffffu, head) & ~((2u << lane) - 1u);  // lane 31: 2u << 31 == 0
+    const int end = later ? __ffs(later) - 1 : 32;  // one past the last lane of this lane's run
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long w2 = __shfl_down_sync(0xffffffffu, w, o), in2 = __shfl_down_sync(0xffffffffu, in, o);
+      const unsigned long long top2 = __shfl_down_sync(0xffffffffu, top, o);
+      const unsigned long long pairs2 = __shfl_down_sync(0xffffffffu, pairs, o);
+      const unsigned int lo2 = __shfl_down_sync(0xffffffffu, lo, o);
+      if (lane + o < end) {
+        w += w2;
+        in += in2;
+        top = top2 > top ? top2 : top;
+        pairs += pairs2;
+        lo = lo2 < lo ? lo2 : lo;
+      }
+    }
+    if (head && e < H) {
+      atomicAdd(&W[f], w);
+      if (in) atomicAdd(&I[f], in);
+      if (top) atomicMax(&best[f], top);
+      if (pairs) {
+        atomicAdd(&inner[L], pairs);
+        atomicMin(&least[L], lo);
+      }
+    }
+  }
+}
+
+// the packed partners as (partner, count), -1 and 0 for none; the least internal count, 0 for a cluster without one
+__global__ void k_links_out(int64_t R, int64_t C, const unsigned long long *__restrict__ best,
+                            const unsigned long long *__restrict__ inner, const unsigned int *__restrict__ least,
+                            int32_t *__restrict__ partner, int32_t *__restrict__ partner_count,
+                            int32_t *__restrict__ least_out) {
+  const int64_t m = R > C ? R : C;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
+    if (i < R) {
+      const unsigned long long b = best[i];
+      partner[i] = b ? (int32_t)(0xffffffffu - (uint32_t)(b & 0xffffffffull)) : -1;
+      partner_count[i] = (int32_t)(b >> 32);
+    }
+    if (i < C) least_out[i] = inner[i] ? (int32_t)least[i] : 0;
+  }
+}
+}  // namespace
+
+// The labels (canonical for C) into the handle's label buffer, checked for range and for an empty cluster before
+// anything else; then one pass of k_record_links over the held table.  The table and S do not change.
+extern "C" int dbl_pairs_record_links(dbl_pairs *p, const int32_t *labels, int32_t num_clusters, int64_t *W_out,
+                                      int64_t *I_out, int32_t *partner_out, int32_t *partner_count_out,
+                                      int64_t *inner_out, int32_t *least_out) {
+  if (!p || !labels || !W_out || !I_out || !partner_out || !partner_count_out || !inner_out || !least_out ||
+      num_clusters < 1 || num_clusters > p->R)
+    return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(labels, p->cluster, num_clusters); rc != DBL_OK) return rc;
+  const int64_t R = p->R, C = num_clusters, H = p->H;
+  cudaStream_t st = p->stream;
+  const int32_t *L = p->cluster.as<int32_t>();
+  int32_t *size = p->size.as<int32_t>();
+  POST_TRY(cudaMemsetAsync(size, 0, sizeof(int32_t) * C, st));
+  k_label_sizes<<<grid_for(R), THREADS, 0, st>>>(R, L, size);
+  k_flag_empty<<<grid_for(C), THREADS, 0, st>>>(C, size, p->bad.as<int>());  // bad is 0 after take_labels
+  int flag = 0;
+  POST_TRY(cudaMemcpyAsync(&flag, p->bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  if (flag) return DBL_ERR_INVALID;
+
+  const size_t r8 = sizeof(unsigned long long) * (size_t)R, r4 = sizeof(int32_t) * (size_t)R;
+  const size_t c8 = sizeof(unsigned long long) * (size_t)C, c4 = sizeof(int32_t) * (size_t)C;
+  Buf W, I, best, inner, least, partner, pcount, lout;
+  POST_TRY(W.alloc(r8));
+  POST_TRY(I.alloc(r8));
+  POST_TRY(best.alloc(r8));
+  POST_TRY(inner.alloc(c8));
+  POST_TRY(least.alloc(c4));
+  POST_TRY(partner.alloc(r4));
+  POST_TRY(pcount.alloc(r4));
+  POST_TRY(lout.alloc(c4));
+  POST_TRY(cudaMemsetAsync(W.p, 0, r8, st));
+  POST_TRY(cudaMemsetAsync(I.p, 0, r8, st));
+  POST_TRY(cudaMemsetAsync(best.p, 0, r8, st));
+  POST_TRY(cudaMemsetAsync(inner.p, 0, c8, st));
+  POST_TRY(cudaMemsetAsync(least.p, 0xff, c4, st));
+  if (H > 0)
+    k_record_links<<<grid_for(H), THREADS, 0, st>>>(H, p->tab_key[p->cur].as<unsigned long long>(),
+                                                    p->tab_cnt[p->cur].as<int32_t>(), L,
+                                                    W.as<unsigned long long>(), I.as<unsigned long long>(),
+                                                    best.as<unsigned long long>(), inner.as<unsigned long long>(),
+                                                    least.as<unsigned int>());
+  k_links_out<<<grid_for(std::max(R, C)), THREADS, 0, st>>>(R, C, best.as<unsigned long long>(),
+                                                          inner.as<unsigned long long>(), least.as<unsigned int>(),
+                                                          partner.as<int32_t>(), pcount.as<int32_t>(),
+                                                          lout.as<int32_t>());
+  POST_TRY(cudaGetLastError());
+  // host or device outputs: unified addressing picks the copy direction
+  POST_TRY(cudaMemcpyAsync(W_out, W.p, r8, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(I_out, I.p, r8, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(partner_out, partner.p, r4, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(partner_count_out, pcount.p, r4, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(inner_out, inner.p, c8, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(least_out, lout.p, c4, cudaMemcpyDefault, st));
+  POST_TRY(cudaStreamSynchronize(st));
   return DBL_OK;
 }
 

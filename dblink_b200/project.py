@@ -28,12 +28,14 @@ VI_METRICS = ("vi-pairwise", "vi-cluster")
 VI_SEARCH_METRICS = ("vi-search-pairwise", "vi-search-cluster")
 # whether the ground truth lies in the credible ball around a point estimate, in VI and in Binder distance
 CREDIBLE_BALL_METRICS = ("credible-ball",)
+# how well the clerical review queue of a point estimate finds its clusters that are not exactly a true entity
+CLERICAL_REVIEW_METRICS = ("clerical-review",)
 SUPPORTED_METRICS = (SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_SEARCH_METRICS + VI_METRICS
-                     + VI_SEARCH_METRICS + CREDIBLE_BALL_METRICS)
+                     + VI_SEARCH_METRICS + CREDIBLE_BALL_METRICS + CLERICAL_REVIEW_METRICS)
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
                         "binder-search-clusters", "vi-clusters", "vi-search-clusters", "credible-ball",
-                        "entity-values", "pairwise-match-diagnostics")
+                        "entity-values", "pairwise-match-diagnostics", "clerical-review")
 # the point estimates a credible ball may be centred on
 CREDIBLE_BALL_CENTERS = ("shared-most-probable-clusters", "binder-clusters", "binder-search-clusters", "vi-clusters",
                          "vi-search-clusters")
@@ -201,6 +203,34 @@ def credible_ball_center(chain, center, false_link_cost, max_rounds):
     raise ValueError(f"credibleBallCenter must be one of {CREDIBLE_BALL_CENTERS}.")
 
 
+def record_links(chain, labels):
+    """analysis_arrays.RecordLinks of the canonical labels[R] against the pair table of a ChainArrays: on the GPU when
+    the platform has one (analysis_gpu), else on the host (analysis_arrays).  Both give identical integers."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.record_links(chain, labels)
+    first, second, count = analysis_arrays.pairwise_match_counts(chain)
+    return analysis_arrays.record_links(first, second, count, labels, int(np.max(labels)) + 1)
+
+
+def cluster_appearances(chain, labels):
+    """A, int64[R]: the samples of a ChainArrays in which each record's cluster is its cluster in the canonical
+    labels[R]: on the GPU when the platform has one (analysis_gpu), else on the host (analysis_arrays).  Both give
+    identical integers."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.cluster_appearances(chain, labels)
+    return analysis_arrays.cluster_appearances(chain, labels)
+
+
+def clerical_review_estimate(chain, center, false_link_cost, max_rounds):
+    """The analysis_arrays.ClericalReview of the point estimate `center` (one of CREDIBLE_BALL_CENTERS) of a
+    ChainArrays, its clusters numbered canonically, ranked at falseLinkCost = false_link_cost."""
+    if not chain.samples:
+        raise ValueError("the clerical review needs at least one sample at or after lowerIterationCutoff")
+    labels = analysis_arrays.canonical_clusters(credible_ball_center(chain, center, false_link_cost, max_rounds))
+    return analysis_arrays.ClericalReview(record_links(chain, labels), cluster_appearances(chain, labels), labels,
+                                          len(chain.samples), false_link_cost)
+
+
 def credible_ball_estimate(chain, center, level, false_link_cost, max_rounds):
     """The credible ball of a ChainArrays around the estimate `center`: (its labels, every sample's number of clusters,
     {"vi" | "binder": (every sample's distance from the center, radius, in-ball mask, bounds)}), the bounds as
@@ -280,6 +310,20 @@ def _entity_values_center(prm):
     if center not in CREDIBLE_BALL_CENTERS:
         raise ValueError(f"entityValuesCenter must be one of {CREDIBLE_BALL_CENTERS}.")
     return center
+
+
+def _clerical_review_center(prm):
+    center = prm.get("clericalReviewCenter", "shared-most-probable-clusters")
+    if center not in CREDIBLE_BALL_CENTERS:
+        raise ValueError(f"clericalReviewCenter must be one of {CREDIBLE_BALL_CENTERS}.")
+    return center
+
+
+def _clerical_review_settings(prm):
+    """The settings a clerical review is computed with, for run.txt: its center's, then the cost of a false link the
+    queue is ranked at."""
+    return (_center_settings(prm, "clerical_review_center", "clericalReviewCenter")
+            + f", ranked at falseLinkCost={prm['false_link_cost']}")
 
 
 def _save_entity_values(prm):
@@ -433,6 +477,9 @@ class Project:
                     L.append(f"  * SummarizeStep: entity-values is the most probable value of each attribute of the "
                              f"entity of each cluster of a point estimate, from the entity values saved with the "
                              f"samples, with {_center_settings(prm, 'entity_values_center', 'entityValuesCenter')}")
+                if "clerical-review" in prm["quantities"]:
+                    L.append(f"  * SummarizeStep: clerical-review ranks the clusters of a point estimate by their "
+                             f"expected false and missed links, with {_clerical_review_settings(prm)}")
             elif name == "evaluate":
                 smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
                 post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
@@ -471,6 +518,11 @@ class Project:
                     L.append(f"  * EvaluateStep: Evaluating whether the ground truth lies in the credible ball around a "
                              f"point estimate ({_credible_ball_settings(prm)}, iterations >= "
                              f"{prm['lower_iteration_cutoff']}) using {braces(ball)} metrics")
+                review = [m for m in prm["metrics"] if m in CLERICAL_REVIEW_METRICS]
+                if review:
+                    L.append(f"  * EvaluateStep: Evaluating how soon the clerical review queue of a point estimate "
+                             f"reaches its clusters that are not a true entity ({_clerical_review_settings(prm)}, "
+                             f"iterations >= {prm['lower_iteration_cutoff']}) using {braces(review)} metrics")
             else:
                 L.append("  * CopyFilesStep: Copying {" + ", ".join(prm["file_names"]) + "} to destination "
                          + prm["destination_path"])
@@ -615,6 +667,7 @@ class Project:
                                               false_link_cost=_false_link_cost(prm),
                                               max_search_rounds=_max_search_rounds(prm),
                                               entity_values_center=_entity_values_center(prm),
+                                              clerical_review_center=_clerical_review_center(prm),
                                               **_credible_ball_params(prm))))
             elif name == "evaluate":
                 m = list(prm["metrics"])
@@ -624,6 +677,7 @@ class Project:
                                              use_existing_smpc=bool(prm.get("useExistingSMPC", False)),
                                              false_link_cost=_false_link_cost(prm),
                                              max_search_rounds=_max_search_rounds(prm),
+                                             clerical_review_center=_clerical_review_center(prm),
                                              **_credible_ball_params(prm))))
             elif name == "copy-files":
                 out.append(("copy-files", dict(file_names=list(prm["fileNames"]),
@@ -716,6 +770,15 @@ class Project:
                                 f"credible-ball-{name}-{bound}.csv")
                     elif q == "entity-values":
                         self._summarize_entity_values(ch, prm)
+                    elif q == "clerical-review":
+                        review = clerical_review_estimate(ch, prm["clerical_review_center"], prm["false_link_cost"],
+                                                          prm["max_search_rounds"])
+                        self._save_smpc(analysis_arrays.labels_to_clusters(review.labels, ch.record_ids),
+                                        "clerical-review-clusters.csv")
+                        writers.save_clerical_review(analysis_arrays.clerical_review_rows(review, ch.record_ids),
+                                                     self.output_path)
+                        writers.save_clerical_review_records(
+                            analysis_arrays.clerical_review_record_rows(review, ch.record_ids), self.output_path)
                     else:
                         labels = shared_most_probable_clusters(ch)
                         self._save_smpc(analysis_arrays.labels_to_clusters(labels, ch.record_ids))
@@ -815,6 +878,15 @@ class Project:
                                          samplesInBall=int(inside.sum()))
                     results["credible-ball"] = res
                     text.append(analysis.format_credible_ball(res))
+                if any(m in CLERICAL_REVIEW_METRICS for m in prm["metrics"]):
+                    ch = ch if ch is not None else self.read_chain(cut)
+                    center = prm["clerical_review_center"]
+                    review = clerical_review_estimate(ch, center, prm["false_link_cost"], prm["max_search_rounds"])
+                    rows, res = analysis_arrays.clerical_review_evaluation(review, true_labels(ch.record_ids))
+                    writers.save_clerical_review_evaluation(rows, self.output_path)
+                    res["center"] = center
+                    results["clerical-review"] = res
+                    text.append(analysis.format_clerical_review(res))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
             elif name == "copy-files":

@@ -436,3 +436,38 @@ def save_entity_values(attribute_names, rows, path):
         out = csv.writer(fh, lineterminator="\n")
         out.writerow(["cluster", "size"] + [x for a in attribute_names for x in (a, a + "Probability")])
         out.writerows(rows)
+
+
+CLERICAL_REVIEW_HEADER = ("rank", "cluster", "size", "clusterProbability", "expectedFalseLinks", "expectedMissedLinks",
+                          "expectedLoss", "weakestInternalLinkProbability", "strongestLinkInsideRecordId",
+                          "strongestLinkOutsideRecordId", "strongestOutsideLinkProbability")
+CLERICAL_REVIEW_RECORDS_HEADER = ("recordId", "cluster", "clusterProbability", "expectedFalseLinks",
+                                  "expectedMissedLinks", "strongestOutsideRecordId", "strongestOutsideLinkProbability")
+CLERICAL_REVIEW_EVALUATION_HEADER = ("rank", "cluster", "erroneous", "erroneousFound")
+
+
+def _save_csv(path, name, header, rows):
+    import csv
+
+    with open(os.path.join(path, name), "w", newline="") as fh:
+        out = csv.writer(fh, lineterminator="\n")
+        out.writerow(header)
+        out.writerows(rows)
+
+
+def save_clerical_review(rows, path):
+    """clerical-review.csv under `path`: one row per cluster of the point estimate in review order, as
+    analysis_arrays.clerical_review_rows gives them, CSV-quoted where a record id needs it."""
+    _save_csv(path, "clerical-review.csv", CLERICAL_REVIEW_HEADER, rows)
+
+
+def save_clerical_review_records(rows, path):
+    """clerical-review-records.csv under `path`: one row per record in chain record order, as
+    analysis_arrays.clerical_review_record_rows gives them."""
+    _save_csv(path, "clerical-review-records.csv", CLERICAL_REVIEW_RECORDS_HEADER, rows)
+
+
+def save_clerical_review_evaluation(rows, path):
+    """clerical-review-evaluation.csv under `path`: per position of the review queue its cluster, whether it is not
+    exactly a true entity (1) and the erroneous clusters found up to it."""
+    _save_csv(path, "clerical-review-evaluation.csv", CLERICAL_REVIEW_EVALUATION_HEADER, rows)

@@ -307,6 +307,11 @@ int dbl_owned_masks(dbl_ctx *, uint8_t *ent_owned, uint8_t *rec_owned);
  *                             sample) and its frequency count / S (freq_out); records grouped by that signature, each
  *                             labelled by the smallest record index of its group (labels_out); either may be NULL;
  *                             DBL_ERR_STATE before the first sample
+ *   dbl_posterior_cluster_counts  for labels[R] (host or device) in [0, C), every cluster holding a record, A(i) per
+ *                             record (count_out, R, host or device): the samples in which i's cluster is, as a set, its
+ *                             cluster in labels -- the same signatures compared, so up to 2^-64 collisions.
+ *                             DBL_ERR_INVALID: a NULL pointer, C outside [1, R], a label outside [0, C) or an empty
+ *                             cluster; DBL_ERR_STATE before the first sample.  The samples do not change.
  * DBL_ERR_CUDA: no device, or the signature matrix (8 R max_samples bytes) does not fit on it.
  * ------------------------------------------------------------------------------------------------- */
 typedef struct dbl_posterior dbl_posterior;
@@ -315,6 +320,8 @@ void dbl_posterior_free(dbl_posterior *);
 int dbl_posterior_add_sample(dbl_posterior *, const int32_t *cluster /* R, host or device */);
 int32_t dbl_posterior_num_samples(const dbl_posterior *);
 int dbl_posterior_smpc(dbl_posterior *, int32_t *labels_out /* R, may be NULL */, double *freq_out /* R, may be NULL */);
+int dbl_posterior_cluster_counts(dbl_posterior *, const int32_t *labels /* R, host or device */, int32_t num_clusters,
+                                 int32_t *count_out /* R, host or device */);
 
 /* ---------------------------------------------------------------------------------------------------
  * Posterior pairwise match probabilities: for every unordered pair of records {a, b} that share a cluster in at least
@@ -375,6 +382,14 @@ int dbl_posterior_smpc(dbl_posterior *, int32_t *labels_out /* R, may be NULL */
  *                         computed in int64 and rounded doubles exactly as analysis_arrays.pairwise_match_diagnostics
  *                         computes them.  DBL_ERR_STATE: no trace; DBL_ERR_INVALID: a NULL pointer, K < 1, N < 2,
  *                         M N^2 >= 2^30, or a chain range outside [0, P).  Neither the table nor the trace changes.
+ *   dbl_pairs_record_links  for labels[R] (host or device) in [0, C), every cluster holding a record, against the
+ *                         held table, in int64 unless said: per record i, W = sum of count(i, j) over its partners j and
+ *                         I = the same over the partners sharing its label; its strongest partner outside its label
+ *                         (largest count, ties to the smaller j; -1 and 0 when there is none) and that count, int32;
+ *                         per cluster, the held pairs inside it and their least count (int32, 0 when none is held).
+ *                         Outputs: R, R, R, R, C, C entries, host or device pointers.  DBL_ERR_INVALID: a NULL pointer,
+ *                         C outside [1, R], a label outside [0, C) or an empty cluster; DBL_ERR_STATE before the first
+ *                         sample.  The table and S do not change.  Memory: 40 bytes per record and 20 per cluster.
  * DBL_ERR_INVALID: num_records or max_pairs outside [1, 2^31 - 1].  DBL_ERR_CUDA: no device, or an allocation that
  * fails (the held table and the sample count stay as they were).
  * ------------------------------------------------------------------------------------------------- */
@@ -396,6 +411,9 @@ int dbl_pairs_trace_sample(dbl_pairs *, const int32_t *cluster /* R, host or dev
 int dbl_pairs_mixing(dbl_pairs *, int32_t min_count, int32_t num_chains, const int32_t *chain_starts /* K, host */,
                      int32_t draws, double ess_floor, int32_t *count_out, int32_t *chain_min_out,
                      int32_t *chain_max_out, int32_t *max_t_out, double *rhat_out, double *ess_out);
+int dbl_pairs_record_links(dbl_pairs *, const int32_t *labels /* R, host or device */, int32_t num_clusters,
+                           int64_t *W_out, int64_t *I_out, int32_t *partner_out, int32_t *partner_count_out,
+                           int64_t *inner_out /* C */, int32_t *least_out /* C */);
 
 /* ---------------------------------------------------------------------------------------------------
  * Every posterior sample against the ground truth: per sample, the integer counts its pairwise precision / recall /
