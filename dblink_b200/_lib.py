@@ -163,6 +163,14 @@ SIGNATURES = {
     "dbl_values_add_sample": (C.c_int, [vp, vp]),
     "dbl_values_num_samples": (C.c_int32, [vp]),
     "dbl_values_modes": (C.c_int, [vp, vp, vp]),
+    "dbl_query_create": (C.c_int, [C.POINTER(vp), C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, i32p, f64p,
+                                   i32p, i32p, f64p, f64p, i64p, i32p, f64p, C.c_double, C.c_int64]),
+    "dbl_query_free": (None, [vp]),
+    "dbl_query_num_samples": (C.c_int32, [vp]),
+    "dbl_query_add_sample": (C.c_int, [vp, vp, C.c_int32, vp, f64p]),
+    "dbl_query_score_sample": (C.c_int, [vp, vp, C.c_int32, vp, f64p]),
+    "dbl_query_num_candidates": (C.c_int, [vp, i64p]),
+    "dbl_query_read": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "dbl_version": (C.c_char_p, []),
 }
 

@@ -665,3 +665,54 @@ def format_clerical_review(res):
             f" Review queue:    found {shares(res['found'])}, area {res['area']!r}\n"
             f" By probability:  found {shares(res['baseline'])}\n"
             "=====================================\n")
+
+
+def query_link_probabilities(queries, samples, tables, constant, population_size):
+    """The posterior predictive of new records, restated literally with dicts and Python floats for small chains.
+    queries = [(file, {attribute: value id})] (missing attributes left out); samples = [(clusters, values, theta)]
+    with clusters = lists of record indices, values[k] = the entity values of cluster k, theta[a][f]; tables[a] =
+    AttributeIndex.tables() of attribute a.  Per sample, w(q, k) = prod over the observed a of (1 - theta) [x = y] +
+    theta psi(x) norm(y) expsim(x, y) (expsim = 1 off x's row; norm = expsim = 1 when constant), m(q) = prod over the
+    observed a of psi(x) ((1 - theta) + theta sigma(x)), sigma(x) = sum over y of psi(y) norm(y) expsim(x, y) (1 when
+    constant), Z = sum_k w + (M - K) m.  Returns ({(q, r): p}, [p_new], [ESS]) over every pair, no threshold."""
+    def expsim(a, x, y):
+        t = tables[a]
+        for j in range(t["rowptr"][x], t["rowptr"][x + 1]):
+            if t["col"][j] == y:
+                return float(t["expsim"][j])
+        return 1.0
+
+    def norm(a, y):
+        return 1.0 if constant[a] else float(tables[a]["norm"][y])
+
+    def sigma(a, x):
+        if constant[a]:
+            return 1.0
+        return sum(float(tables[a]["phi"][y]) * norm(a, y) * expsim(a, x, y) for y in range(len(tables[a]["phi"])))
+
+    M = population_size
+    num, den, den2, new = {}, [0.0] * len(queries), [0.0] * len(queries), [0.0] * len(queries)
+    for clusters, values, theta in samples:
+        K = len(clusters)
+        for q, (f, obs) in enumerate(queries):
+            w = []
+            for k in range(K):
+                wk = 1.0
+                for a, x in obs.items():
+                    th, y = float(theta[a][f]), int(values[k][a])
+                    wk *= (1.0 - th) * (1.0 if x == y else 0.0) + th * float(tables[a]["phi"][x]) * norm(a, y) * \
+                        expsim(a, x, y)
+                w.append(wk)
+            m = 1.0
+            for a, x in obs.items():
+                th = float(theta[a][f])
+                m *= float(tables[a]["phi"][x]) * ((1.0 - th) + th * sigma(a, x))
+            Z = sum(w) + (M - K) * m
+            for k, members in enumerate(clusters):
+                for r in members:
+                    num[(q, r)] = num.get((q, r), 0.0) + w[k]
+            den[q] += Z
+            den2[q] += Z * Z
+            new[q] += (M - K) * m
+    p = {key: v / den[key[0]] for key, v in num.items()}
+    return p, [new[q] / den[q] for q in range(len(queries))], [den[q] ** 2 / den2[q] for q in range(len(queries))]

@@ -1572,3 +1572,369 @@ def clerical_review_evaluation(review, truth):
     summary = dict(clusters=C, erroneous=E, found=_found_shares(found, E), area=area,
                    baseline=_found_shares(np.cumsum(err[by_probability]).tolist(), E))
     return rows, summary
+
+
+# ---- new records linked to a finished chain ----------------------------------------------------------------------
+# A query record has value ids x_qa in the data's vocabularies (-1 = missing, or a value the data never holds) and a
+# file f(q).  For a sample with clusters k of entity values y_ka and distortion probabilities theta_af, the collapsed
+# PCG-II link weight of q against cluster k is w(q, k) = prod over the observed a of
+#   g(y) = (1 - theta) [x = y] + theta psi(x) norm(y) expsim(x, y)     (norm(y) = 1/n(y), expsim = 1 off x's sparse row;
+#                                                                       norm = expsim = 1 for a constant attribute)
+# and an entity no record links to has expected weight m(q) = prod over the observed a of h = psi(x) ((1 - theta) +
+# theta sigma(x)), sigma(x) = sum_y psi(y) norm(y) expsim(x, y) (1 for a constant attribute).  With M the population
+# size and K the sample's clusters, Z(q) = sum_k w(q, k) + (M - K) m(q).  Weights are carried relative to m:
+# rho(q, k) = w / m = prod_a r(y), r = c0 [x = y] + c1 norm(y) expsim(x, y), c0 = (1 - theta) / h, c1 = theta psi(x) / h,
+# so log w = log m + log rho and log Z = log m + log(sum_k rho + M - K).  Over the samples s, with L_q = max_s log Z_s
+# and Z~ = exp(log Z - L_q):
+#   p(q, r) = sum_s w_s(q, c_s(r)) / sum_s Z_s(q),  p_new(q) = sum_s (M - K_s) m_s(q) / sum_s Z_s(q),
+#   ESS(q) = (sum_s Z_s)^2 / sum_s Z_s^2.
+# p(q, r) >= t needs some sample with w_s >= t Z_s: pass 1 collects those (q, r) as candidates (at most floor(1/t)
+# clusters per query and sample), pass 2 sums w over every sample for the candidates only.
+MAX_QUERY_CANDIDATES = MAX_PAIRS
+QUERY_BLOCK = 1 << 22  # query x cluster entries of one dense block of the numpy scan
+
+
+class QueryTables:
+    """The per-query tables, built once from the attribute indexes: x int32[Q][A] (-1 = missing or unseen), file
+    int32[Q], psi and sigma float64[Q][A], the hit rows (x's sparse row: value ids ascending and their expsim) as
+    hit_offsets int64[Q A + 1], hit_values, hit_expsim, and per attribute its norm table (ones when constant).
+    tables[a] = AttributeIndex.tables() of attribute a; constant[a] = whether it is constant."""
+
+    def __init__(self, x, file, tables, constant, num_files):
+        x = np.array(x, np.int32, ndmin=2)
+        Q, A = x.shape
+        self.x, self.file = x, np.asarray(file, np.int32).reshape(Q)
+        self.num_files = int(num_files)
+        self.num_values = np.array([len(t["phi"]) for t in tables], np.int32)
+        if len(tables) != A or len(constant) != A:
+            raise ValueError("one table per matching attribute")
+        if Q and (self.file.min() < 0 or self.file.max() >= self.num_files):
+            raise ValueError("a query's file is not one of the data's files")
+        if ((x < -1) | (x >= self.num_values[None, :])).any():
+            raise ValueError("a query value id is outside its attribute's index")
+        self.norm = [np.ones(len(t["phi"])) if c else np.asarray(t["norm"], np.float64) for t, c in zip(tables, constant)]
+        self.psi, self.sigma = np.zeros((Q, A)), np.ones((Q, A))
+        rows = []  # (q, a) -> (values, expsim)
+        for a, (t, c) in enumerate(zip(tables, constant)):
+            obs = x[:, a] >= 0
+            self.psi[obs, a] = np.asarray(t["phi"])[x[obs, a]]
+            if c:
+                continue
+            base = float(np.dot(t["phi"], self.norm[a]))
+            for v in np.unique(x[obs, a]):
+                lo, hi = t["rowptr"][v], t["rowptr"][v + 1]
+                cols, es = np.asarray(t["col"][lo:hi]), np.asarray(t["expsim"][lo:hi])
+                keep = es != 1.0
+                rows.append((a, int(v), cols[keep], es[keep]))
+                self.sigma[x[:, a] == v, a] = base + float(np.dot(t["phi"][cols] * self.norm[a][cols], es - 1.0))
+        row_of = {(a, v): (cols, es) for a, v, cols, es in rows}
+        lens = np.zeros(Q * A, np.int64)
+        for q, a in zip(*np.nonzero(x >= 0)):
+            if (a, int(x[q, a])) in row_of:
+                lens[q * A + a] = len(row_of[(a, int(x[q, a]))][0])
+        self.hit_offsets = np.r_[0, np.cumsum(lens)].astype(np.int64)
+        self.hit_values = np.zeros(int(self.hit_offsets[-1]), np.int32)
+        self.hit_expsim = np.zeros(int(self.hit_offsets[-1]))
+        for i in np.flatnonzero(lens):
+            q, a = divmod(int(i), A)
+            cols, es = row_of[(a, int(x[q, a]))]
+            lo = self.hit_offsets[i]
+            order = np.argsort(cols, kind="stable")
+            self.hit_values[lo:lo + len(cols)] = cols[order]
+            self.hit_expsim[lo:lo + len(cols)] = es[order]
+
+    @property
+    def num_queries(self):
+        return self.x.shape[0]
+
+    @property
+    def num_attributes(self):
+        return self.x.shape[1]
+
+    def hits(self, q, a):
+        lo, hi = self.hit_offsets[q * self.num_attributes + a], self.hit_offsets[q * self.num_attributes + a + 1]
+        return self.hit_values[lo:hi], self.hit_expsim[lo:hi]
+
+
+def query_coefficients(tab, theta):
+    """(c0, c1 float64[Q][A], log m float64[Q]) of one sample's theta[A][F]; c0 = c1 = 0 where x is not observed."""
+    theta = np.asarray(theta, np.float64).reshape(tab.num_attributes, tab.num_files)
+    th = theta[np.arange(tab.num_attributes)[None, :], tab.file[:, None]]
+    obs = tab.x >= 0
+    with np.errstate(divide="ignore", invalid="ignore"):
+        h = tab.psi * ((1.0 - th) + th * tab.sigma)
+        c0 = np.where(obs, (1.0 - th) / h, 0.0)
+        c1 = np.where(obs, th * tab.psi / h, 0.0)
+        logm = np.zeros(tab.num_queries)
+        for a in range(tab.num_attributes):  # attribute order, as on the device
+            logm += np.where(obs[:, a], np.log(np.where(obs[:, a], h[:, a], 1.0)), 0.0)
+    return c0, c1, logm
+
+
+def query_rho(tab, coef, values, qs):
+    """rho(q, k) float64[len(qs)][K] of the queries qs against the K rows of values int32[K][A]: the product over the
+    observed attributes, in attribute order, of c0 [x = y] + c1 norm(y) expsim(x, y)."""
+    c0, c1, _ = coef
+    values = np.asarray(values)
+    qs = np.asarray(qs, np.int64)
+    rho = np.ones((len(qs), len(values)))
+    for a in range(tab.num_attributes):
+        x = tab.x[qs, a]
+        obs = x >= 0
+        if not obs.any():
+            continue
+        y = values[:, a]
+        t = c1[qs, a][:, None] * tab.norm[a][y][None, :]
+        lens = tab.hit_offsets[qs * tab.num_attributes + a + 1] - tab.hit_offsets[qs * tab.num_attributes + a]
+        if lens.any():
+            E = np.ones((len(qs), tab.num_values[a]))
+            for i in np.flatnonzero(lens):
+                cols, es = tab.hits(int(qs[i]), a)
+                E[i, cols] = es
+            t = t * E[:, y]
+        r = np.where(y[None, :] == x[:, None], c0[qs, a][:, None], 0.0) + t
+        rho *= np.where(obs[:, None], r, 1.0)
+    return rho
+
+
+def _attribute_hit_keys(tab, a):
+    """Attribute a's hits of every query as sorted keys q V_a + y, with their expsim."""
+    A, Q, V = tab.num_attributes, tab.num_queries, int(tab.num_values[a])
+    starts = tab.hit_offsets[np.arange(Q) * A + a]
+    n = tab.hit_offsets[np.arange(Q) * A + a + 1] - starts
+    idx = np.repeat(starts, n) + (np.arange(n.sum()) - np.repeat(np.cumsum(n) - n, n))
+    return np.repeat(np.arange(Q, dtype=np.int64), n) * V + tab.hit_values[idx], tab.hit_expsim[idx]
+
+
+def query_pair_rho(tab, coef, values, q, k):
+    """rho(q[i], k[i]) for pairs (query, cluster): as query_rho, one entry per pair."""
+    c0, c1, _ = coef
+    q, k = np.asarray(q, np.int64), np.asarray(k, np.int64)
+    values = np.asarray(values)
+    rho = np.ones(len(q))
+    for a in range(tab.num_attributes):
+        x = tab.x[q, a]
+        y = values[k, a].astype(np.int64)
+        t = c1[q, a] * tab.norm[a][y]
+        keys, es = _attribute_hit_keys(tab, a)
+        if len(keys):
+            want = q * int(tab.num_values[a]) + y
+            pos = np.minimum(np.searchsorted(keys, want), len(keys) - 1)
+            t = np.where(keys[pos] == want, t * es[pos], t)
+        rho *= np.where(x >= 0, np.where(y == x, c0[q, a], 0.0) + t, 1.0)
+    return rho
+
+
+def _check_min_link_probability(t):
+    if isinstance(t, bool) or not isinstance(t, (int, float)) or not 0.0 < float(t) <= 1.0:
+        raise ValueError("minLinkProbability must be in (0, 1].")
+    return float(t)
+
+
+def check_query_sample(tab, labels, values, theta, num_records, population_size):
+    """The refusals of both passes for one sample: (labels int64[R] in [0, K), values int32[K][A], theta[A][F])."""
+    labels, values = np.asarray(labels), np.asarray(values)
+    theta = np.asarray(theta, np.float64)
+    K = len(values)
+    if labels.shape != (num_records,) or values.ndim != 2 or values.shape[1] != tab.num_attributes:
+        raise ValueError("a sample needs one cluster label per record and one value row per cluster")
+    if K < 1 or K > population_size:
+        raise ValueError(f"a sample has {K} clusters, more than the population size {population_size}"
+                         if K else "a sample has no clusters")
+    if labels.min() < 0 or labels.max() >= K or (np.bincount(labels, minlength=K) == 0).any():
+        raise ValueError("a sample's cluster labels must cover [0, K) exactly")
+    if ((values < 0) | (values >= tab.num_values[None, :])).any():
+        raise ValueError("an entity value id is outside its attribute's index")
+    if theta.size != tab.num_attributes * tab.num_files or not ((theta >= 0.0) & (theta <= 1.0)).all():
+        raise ValueError("distortion probabilities must be [A][F] values in [0, 1]")
+
+
+class QueryResult:
+    """What both passes give: the candidates (query, record) in (query, record) order with their sums, and per query
+    L_q, sum Z~, sum Z~^2, the new-entity sum and every sample's log Z ([S][Q])."""
+
+    def __init__(self, query, record, sums, scale, zsum, zsq, fresh, logz):
+        self.query, self.record, self.sums = np.asarray(query, np.int64), np.asarray(record, np.int64), sums
+        self.scale, self.zsum, self.zsq, self.fresh, self.logz = scale, zsum, zsq, fresh, logz
+
+    @property
+    def probability(self):
+        return self.sums / self.zsum[self.query]
+
+    @property
+    def new_entity_probability(self):
+        return self.fresh / self.zsum
+
+    @property
+    def effective_samples(self):
+        return self.zsum * self.zsum / self.zsq
+
+
+class QueryScores:
+    """The numpy path of the two passes (analysis_gpu.Query is the device's): add_sample for every sample (pass 1),
+    then score_sample for the same samples in the same order (pass 2), then read()."""
+
+    def __init__(self, tables, num_records, population_size, min_link_probability,
+                 max_candidates=MAX_QUERY_CANDIDATES):
+        self.tab, self.R, self.M = tables, int(num_records), int(population_size)
+        self.t = _check_min_link_probability(min_link_probability)
+        self.max_candidates = int(max_candidates)
+        self.logz, self.logm, self.kcount = [], [], []
+        self.keys = np.zeros(0, np.int64)
+        self.S2, self.sums, self.scale = 0, None, None
+
+    @property
+    def num_samples(self):
+        return len(self.logz)
+
+    def add_sample(self, labels, values, theta):
+        if self.S2:
+            raise ValueError("pass 2 has begun")
+        check_query_sample(self.tab, labels, values, theta, self.R, self.M)
+        labels, values = np.asarray(labels, np.int64), np.asarray(values)
+        tab, K, Q = self.tab, len(values), self.tab.num_queries
+        coef = query_coefficients(tab, theta)
+        step = max(1, QUERY_BLOCK // max(K, 1))
+        total = np.zeros(Q)
+        emitted = []
+        for lo in range(0, Q, step):
+            qs = np.arange(lo, min(Q, lo + step))
+            rho = query_rho(tab, coef, values, qs)
+            s = rho.sum(axis=1) + (self.M - K)
+            total[qs] = s
+            qi, ki = np.nonzero(rho >= self.t * s[:, None])
+            emitted.append((qs[qi], ki))
+        with np.errstate(divide="ignore"):
+            logz = coef[2] + np.log(total)
+        q = np.concatenate([e[0] for e in emitted]).astype(np.int64)
+        k = np.concatenate([e[1] for e in emitted]).astype(np.int64)
+        order = np.argsort(labels, kind="stable")
+        start = np.searchsorted(labels[order], np.arange(K))
+        size = np.bincount(labels, minlength=K)
+        n = size[k]
+        rec = order[np.repeat(start[k], n) + (np.arange(n.sum()) - np.repeat(np.cumsum(n) - n, n))]
+        new = np.union1d(self.keys, (np.repeat(q, n) << 32) | rec)
+        if len(new) > self.max_candidates:
+            raise ValueError(f"more than {self.max_candidates} candidate (query, record) pairs: raise "
+                             f"minLinkProbability")
+        self.keys = new
+        self.logz.append(logz)
+        self.logm.append(coef[2])
+        self.kcount.append(K)
+
+    def score_sample(self, labels, values, theta):
+        if self.S2 >= self.num_samples:
+            raise ValueError("pass 2 has more samples than pass 1")
+        if len(values) != self.kcount[self.S2]:
+            raise ValueError("pass 2 must score the samples of pass 1, in the same order")
+        check_query_sample(self.tab, labels, values, theta, self.R, self.M)
+        if self.S2 == 0:
+            self.scale = np.max(np.asarray(self.logz), axis=0)
+            self.sums = np.zeros(len(self.keys))
+        labels = np.asarray(labels, np.int64)
+        coef = query_coefficients(self.tab, theta)
+        q, r = self.keys >> 32, self.keys & 0xffffffff
+        with np.errstate(divide="ignore"):
+            self.sums += np.exp(coef[2][q] + np.log(query_pair_rho(self.tab, coef, values, q, labels[r])) -
+                                self.scale[q])
+        self.S2 += 1
+
+    def read(self):
+        if self.num_samples == 0 or self.S2 != self.num_samples:
+            raise ValueError("pass 2 must score every sample of pass 1 before the results are read")
+        logz, logm = np.asarray(self.logz), np.asarray(self.logm)
+        zt = np.exp(logz - self.scale[None, :])
+        un = self.M - np.asarray(self.kcount, np.int64)
+        with np.errstate(divide="ignore"):
+            fresh = np.where(un[:, None] > 0, np.exp(np.log(np.maximum(un, 1))[:, None] + logm - self.scale[None, :]),
+                             0.0)
+        zsum, zsq, fsum = np.zeros(len(self.scale)), np.zeros(len(self.scale)), np.zeros(len(self.scale))
+        for s in range(len(zt)):  # sample order, as on the device
+            zsum += zt[s]
+            zsq += zt[s] * zt[s]
+            fsum += fresh[s]
+        return QueryResult(self.keys >> 32, self.keys & 0xffffffff, self.sums, self.scale, zsum, zsq, fsum, logz)
+
+
+def query_sample_arrays(num_records, members, offsets, values):
+    """(labels int64[R] in [0, K), cluster values int32[K][A]) of one sample: members / offsets of the chain and the
+    per-record values int32[A][R] read_entity_values gives."""
+    members = np.asarray(members)
+    sizes = np.diff(np.asarray(offsets, np.int64))
+    labels = np.full(num_records, -1, np.int64)
+    labels[members] = np.repeat(np.arange(len(sizes)), sizes)
+    return labels, np.ascontiguousarray(np.asarray(values)[:, members[np.asarray(offsets[:-1], np.int64)]].T,
+                                        np.int32)
+
+
+def link_queries(tables, samples, num_records, population_size, min_link_probability, scorer=QueryScores):
+    """Both passes over the samples: samples() yields (labels, values[K][A], theta[A][F]) per sample, the same each time
+    it is called; scorer = QueryScores or analysis_gpu.Query.  Returns the QueryResult."""
+    if scorer is QueryScores:
+        qs = scorer(tables, num_records, population_size, min_link_probability)
+        return _two_passes(qs, samples)
+    with scorer(tables, num_records, population_size, min_link_probability) as qs:
+        return _two_passes(qs, samples)
+
+
+def _two_passes(qs, samples):
+    for s in samples():
+        qs.add_sample(*s)
+    if qs.num_samples == 0:
+        raise ValueError("linking records needs at least one sample at or after lowerIterationCutoff")
+    for s in samples():
+        qs.score_sample(*s)
+    return qs.read()
+
+
+def query_link_rows(result, min_link_probability, data_position):
+    """The reported pairs: (query, record, p) with p >= t, in query order, then p descending, then the record's data
+    position (data_position[r] = its row in the data file)."""
+    p = result.probability
+    keep = p >= min_link_probability
+    q, r, p = result.query[keep], result.record[keep], p[keep]
+    order = np.lexsort((np.asarray(data_position)[r], -p, q))
+    return q[order], r[order], p[order]
+
+
+def read_distortion_probabilities(chain_dirs, chain, num_attributes, num_files):
+    """float64[S][A][F]: theta of every sample of `chain` (pooled as read_entity_values takes it), from each chain
+    directory's distortion-probabilities-chain.csv.  Raises ValueError for a sample past the cutoff without a row, or
+    a file whose columns are not A F."""
+    import csv
+
+    rows = {}
+    out = np.empty((len(chain.samples), num_attributes, num_files))
+    for s, (it, k) in enumerate(zip(chain.iterations, chain.chains)):
+        k = int(k)
+        if k not in rows:
+            rows[k] = {}
+            path = os.path.join(chain_dirs[k], "distortion-probabilities-chain.csv")
+            if os.path.exists(path):
+                with open(path, newline="") as fh:
+                    rd = csv.reader(fh)
+                    head = next(rd, None)
+                    if head is None or len(head) != 1 + num_attributes * num_files:
+                        raise ValueError(f"{path}: expected iteration and {num_attributes * num_files} columns")
+                    for row in rd:
+                        rows[k][int(row[0])] = [float(v) for v in row[1:]]
+        got = rows[k].get(int(it))
+        if got is None:
+            raise ValueError(f"the sample at iteration {int(it)} has no distortion probabilities (it was recorded with "
+                             f"saveDistortionProbabilities off): raise lowerIterationCutoff past it, or sample again "
+                             f"with saveDistortionProbabilities on")
+        out[s] = np.asarray(got).reshape(num_attributes, num_files)
+    return out
+
+
+def distortion_summary(theta):
+    """Per (attribute, file), attribute-major: (mean, sd, 2.5 %, 50 %, 97.5 % quantiles) of theta[S][A][F] over the
+    samples (numpy quantile, default method; sd with ddof 0) and S."""
+    theta = np.asarray(theta, np.float64)
+    S = theta.shape[0]
+    if S == 0:
+        raise ValueError("distortion-probabilities needs at least one sample at or after lowerIterationCutoff")
+    flat = theta.reshape(S, -1)
+    q = np.quantile(flat, [0.025, 0.5, 0.975], axis=0)
+    return [(float(flat[:, j].mean()), float(flat[:, j].std()), float(q[0, j]), float(q[1, j]), float(q[2, j]), S)
+            for j in range(flat.shape[1])]

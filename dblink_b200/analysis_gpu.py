@@ -467,3 +467,73 @@ def entity_value_modes(labels, value_samples, num_values):
     """(modes, counts, S), identical to analysis_arrays.entity_value_modes(labels, value_samples, num_values): one
     handle per attribute, all alive while the samples stream through."""
     return analysis_arrays.entity_value_modes(labels, value_samples, num_values, EntityValues)
+
+
+class Query(_Handle):
+    """Owner of a dbl_query handle: the query tables (analysis_arrays.QueryTables) go in once; add_sample for every
+    sample (pass 1), score_sample for the same samples in the same order (pass 2), read() gives the
+    analysis_arrays.QueryResult.  Labels and values may be numpy arrays or device pointers (int)."""
+
+    _prefix = "dbl_query"
+
+    def __init__(self, tables, num_records, population_size, min_link_probability,
+                 max_candidates=analysis_arrays.MAX_QUERY_CANDIDATES):
+        t = analysis_arrays._check_min_link_probability(min_link_probability)
+        tab = tables
+        self._keep = [np.ascontiguousarray(tab.num_values, np.int32),
+                      np.ascontiguousarray(np.concatenate(tab.norm), np.float64),
+                      np.ascontiguousarray(tab.file, np.int32), np.ascontiguousarray(tab.x, np.int32),
+                      np.ascontiguousarray(tab.psi, np.float64), np.ascontiguousarray(tab.sigma, np.float64),
+                      np.ascontiguousarray(tab.hit_offsets, np.int64),
+                      np.ascontiguousarray(np.r_[tab.hit_values, 0], np.int32),
+                      np.ascontiguousarray(np.r_[tab.hit_expsim, 0.0], np.float64)]
+        ptrs = [_lib.i32p, _lib.f64p, _lib.i32p, _lib.i32p, _lib.f64p, _lib.f64p, _lib.i64p, _lib.i32p, _lib.f64p]
+        self.tab, self.Q, self.A = tab, tab.num_queries, tab.num_attributes
+        super().__init__(num_records, int(population_size), self.Q, self.A, int(tab.num_files),
+                         *[a.ctypes.data_as(p) for a, p in zip(self._keep, ptrs)], t, int(max_candidates))
+
+    def _sample(self, name, labels, values, theta):
+        theta = np.ascontiguousarray(theta, np.float64)
+        if theta.size != self.A * self.tab.num_files:
+            raise ValueError("distortion probabilities must be [A][F]")
+        if isinstance(labels, int):
+            lab = labels
+        else:
+            labels = np.ascontiguousarray(labels, np.int32)
+            if labels.shape != (self.num_records,):
+                raise ValueError("a sample needs one cluster label per record")
+            lab = labels.ctypes.data
+        if isinstance(values, tuple):  # (device pointer, K)
+            val, K = values
+        else:
+            values = np.ascontiguousarray(values, np.int32)
+            if values.ndim != 2 or values.shape[1] != self.A:
+                raise ValueError("a sample needs one value row of A ids per cluster")
+            val, K = values.ctypes.data, len(values)
+        self._call(name, self._h, lab, int(K), val, theta.ctypes.data_as(_lib.f64p))
+
+    def add_sample(self, labels, values, theta):
+        self._sample("add_sample", labels, values, theta)
+
+    def score_sample(self, labels, values, theta):
+        self._sample("score_sample", labels, values, theta)
+
+    def num_candidates(self):
+        n = C.c_int64(0)
+        self._call("num_candidates", self._h, C.byref(n))
+        return n.value
+
+    def read(self):
+        H, Q, S = self.num_candidates(), self.Q, self.num_samples
+        q, r = np.zeros(H, np.int32), np.zeros(H, np.int32)
+        sums = np.zeros(H)
+        scale, zsum, zsq, fresh = (np.zeros(Q) for _ in range(4))
+        logz = np.zeros((S, Q))
+        self._call("read", self._h, q.ctypes.data, r.ctypes.data, sums.ctypes.data, scale.ctypes.data,
+                   zsum.ctypes.data, zsq.ctypes.data, fresh.ctypes.data, logz.ctypes.data)
+        return analysis_arrays.QueryResult(q, r, sums, scale, zsum, zsq, fresh, logz)
+
+
+def link_queries(tables, samples, num_records, population_size, min_link_probability):
+    """analysis_arrays.link_queries on the device."""
+    return analysis_arrays.link_queries(tables, samples, num_records, population_size, min_link_probability, Query)

@@ -2562,3 +2562,619 @@ extern "C" int dbl_values_modes(dbl_values *p, int32_t *mode_out, int64_t *count
   POST_TRY(cudaStreamSynchronize(st));
   return DBL_OK;
 }
+
+// ---- new records linked to a finished chain: the posterior predictive of each query record's entity --------------
+// For query q (value ids x_qa, -1 = missing, file f(q)) and a sample with clusters k of entity values y_ka and
+// distortion probabilities theta_af, the collapsed PCG-II link weight against cluster k is w(q, k) = prod over the
+// observed a of g_qa(y_ka), g = (1 - theta) [x = y] + theta psi(x) norm(y) expsim(x, y), and the expected weight of an
+// entity no record links to is m(q) = prod over the observed a of h_qa, h = psi(x) ((1 - theta) + theta sigma(x)).
+// Every weight is carried relative to m: rho(q, k) = prod_a r_qa(y), r = g / h = c0 [x = y] + c1 norm(y) expsim(x, y)
+// with c0 = (1 - theta) / h and c1 = theta psi(x) / h, so a product of 32 factors stays in range whatever the
+// attributes' probabilities.  log Z(q) = log m(q) + log(sum_k rho(q, k) + M - K).
+//   pass 1 (dbl_query_add_sample): k_query_scan sums rho over a chunk of clusters per query -- a block holds 128
+//     queries' coefficients and hit masks in shared memory and streams tiles of the clusters' value rows and norms;
+//     the chunks' partial sums are added in chunk order (k_query_logz), so the bits do not depend on the schedule.  A
+//     second scan emits the clusters with rho >= t (sum rho + M - K), i.e. w >= t Z; their records become candidate
+//     keys q << 32 | r, merged into the held sorted set by the merge kernels of dbl_pairs.
+//   pass 2 (dbl_query_score_sample): one thread per held candidate adds exp(log w - L_q), L_q = max_s log Z_s(q).
+// A query's hits for attribute a are the sparse row of x (the value ids y with expsim(x, y) != 1), sorted; a 64-bit
+// mask of hashed hit ids in shared memory skips the search of the row for almost every y that is not a hit.
+namespace {
+constexpr int QUERY_THREADS = 128;  // queries per scan block
+constexpr int QUERY_TILE = 64;      // clusters per shared-memory tile
+
+__device__ __forceinline__ unsigned long long hit_bit(int32_t y) {
+  return 1ull << ((uint32_t)y * 0x9E3779B1u >> 26);
+}
+
+// expsim(x, y) of a query attribute: its sorted hit row [lo, hi), 1 off the row
+__device__ __forceinline__ double hit_value(const int32_t *__restrict__ col, const double *__restrict__ val,
+                                            long long lo, long long hi, int32_t y) {
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    const int32_t c = col[mid];
+    if (c == y) return val[mid];
+    if (c < y) lo = mid + 1;
+    else hi = mid;
+  }
+  return 1.0;
+}
+
+// one sample's coefficients, one thread per query: c0, c1 per observed attribute, log m(q)
+__global__ void k_query_coef(int32_t Q, int32_t A, int32_t F, const int32_t *__restrict__ file,
+                             const int32_t *__restrict__ x, const double *__restrict__ psi,
+                             const double *__restrict__ sigma, const double *__restrict__ theta, double *__restrict__ c0,
+                             double *__restrict__ c1, double *__restrict__ logm) {
+  for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < Q; q += (int64_t)gridDim.x * blockDim.x) {
+    double lm = 0.0;
+    for (int a = 0; a < A; ++a) {
+      const int64_t i = q * A + a;
+      if (x[i] < 0) {
+        c0[i] = 0.0;
+        c1[i] = 0.0;
+        continue;
+      }
+      const double th = theta[a * F + file[q]];
+      const double h = psi[i] * ((1.0 - th) + th * sigma[i]);
+      c0[i] = (1.0 - th) / h;
+      c1[i] = th * psi[i] / h;
+      lm += log(h);
+    }
+    logm[q] = lm;
+  }
+}
+
+// value ids of the K clusters in [0, V_a)
+__global__ void k_query_check_values(int64_t n, int32_t A, const int32_t *__restrict__ y,
+                                     const int32_t *__restrict__ nv, int *__restrict__ bad) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t v = y[i];
+    if (v < 0 || v >= nv[i % A]) *bad = 1;
+  }
+}
+
+// rho = prod_a r_qa(y_a) over the observed attributes, in attribute order
+__device__ __forceinline__ double query_rho(int32_t A, const int32_t *ys, const double *nrm, const int32_t *sx,
+                                            const double *sc0, const double *sc1, const unsigned long long *smask,
+                                            int stride, int64_t qa0, const long long *__restrict__ hoff,
+                                            const int32_t *__restrict__ hcol, const double *__restrict__ hval) {
+  double rho = 1.0;
+  for (int a = 0; a < A; ++a) {
+    const int32_t xv = sx[a * stride];
+    if (xv < 0) continue;
+    const int32_t y = ys[a];
+    double t = sc1[a * stride] * nrm[a];
+    if (smask[a * stride] & hit_bit(y)) t = t * hit_value(hcol, hval, hoff[qa0 + a], hoff[qa0 + a + 1], y);
+    rho = rho * ((y == xv ? sc0[a * stride] : 0.0) + t);
+  }
+  return rho;
+}
+
+// Pass-1 scan of clusters [chunk lo, hi) for the block's 128 queries.  EMIT = false: partial[chunk][q] = the sum of
+// rho in cluster order.  EMIT = true: every (q, k) with rho >= thr[q] is appended to out (q << 32 | k) while it fits.
+template <bool EMIT>
+__global__ void __launch_bounds__(QUERY_THREADS) k_query_scan(
+    int32_t Q, int32_t A, int64_t K, int64_t chunk, const int32_t *__restrict__ y, const int32_t *__restrict__ voff,
+    const double *__restrict__ norm, const int32_t *__restrict__ x, const double *__restrict__ c0,
+    const double *__restrict__ c1, const unsigned long long *__restrict__ mask, const long long *__restrict__ hoff,
+    const int32_t *__restrict__ hcol, const double *__restrict__ hval, double *__restrict__ partial,
+    const double *__restrict__ thr, unsigned long long *__restrict__ out, unsigned long long *__restrict__ count,
+    unsigned long long cap) {
+  extern __shared__ double smem[];
+  double *sc0 = smem, *sc1 = sc0 + A * QUERY_THREADS;
+  unsigned long long *smask = (unsigned long long *)(sc1 + A * QUERY_THREADS);
+  double *tnrm = (double *)(smask + A * QUERY_THREADS);
+  int32_t *sx = (int32_t *)(tnrm + A * QUERY_TILE), *ty = sx + A * QUERY_THREADS;
+  const int tx = threadIdx.x;
+  const int64_t q = (int64_t)blockIdx.x * QUERY_THREADS + tx;
+  const bool live = q < Q;
+  for (int a = 0; a < A; ++a) {
+    const int64_t i = q * A + a;
+    sx[a * QUERY_THREADS + tx] = live ? x[i] : -1;
+    sc0[a * QUERY_THREADS + tx] = live ? c0[i] : 0.0;
+    sc1[a * QUERY_THREADS + tx] = live ? c1[i] : 0.0;
+    smask[a * QUERY_THREADS + tx] = live ? mask[i] : 0ull;
+  }
+  const int64_t lo = (int64_t)blockIdx.y * chunk, hi = K < lo + chunk ? K : lo + chunk;
+  const double t_q = EMIT && live ? thr[q] : 0.0;
+  double sum = 0.0;
+  for (int64_t k0 = lo; k0 < hi; k0 += QUERY_TILE) {
+    const int n = (int)(hi - k0 < QUERY_TILE ? hi - k0 : QUERY_TILE);
+    __syncthreads();
+    for (int j = tx; j < n * A; j += QUERY_THREADS) {
+      const int a = j % A;
+      const int32_t v = y[k0 * A + j];
+      ty[j] = v;
+      tnrm[j] = norm[voff[a] + v];
+    }
+    __syncthreads();
+    if (!live) continue;
+    for (int j = 0; j < n; ++j) {
+      const double rho = query_rho(A, ty + j * A, tnrm + j * A, sx + tx, sc0 + tx, sc1 + tx, smask + tx,
+                                   QUERY_THREADS, q * A, hoff, hcol, hval);
+      if (EMIT) {
+        if (rho >= t_q) {
+          const unsigned long long at = atomicAdd(count, 1ull);
+          if (at < cap) out[at] = (unsigned long long)q << 32 | (unsigned long long)(k0 + j);
+        }
+      } else {
+        sum += rho;
+      }
+    }
+  }
+  if (!EMIT && live) partial[(int64_t)blockIdx.y * Q + q] = sum;
+}
+
+// per query: the chunks' sums in chunk order, log Z = log m + log(sum + M - K), and the emission threshold
+__global__ void k_query_logz(int32_t Q, int32_t chunks, const double *__restrict__ partial, double extra,
+                             const double *__restrict__ logm, double t, double *__restrict__ logz,
+                             double *__restrict__ thr) {
+  for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < Q; q += (int64_t)gridDim.x * blockDim.x) {
+    double s = 0.0;
+    for (int32_t c = 0; c < chunks; ++c) s += partial[(int64_t)c * Q + q];
+    s += extra;
+    logz[q] = logm[q] + log(s);
+    thr[q] = t * s;
+  }
+}
+
+// per cluster: its first position among the records sorted by label (then k_query_cluster_sizes: its size)
+__global__ void k_query_cluster_bounds(int64_t R, const int32_t *__restrict__ lab_s, int32_t *__restrict__ cstart) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t c = lab_s[i];
+    if (i == 0 || lab_s[i - 1] != c) cstart[c] = (int32_t)i;
+  }
+}
+
+__global__ void k_query_cluster_sizes(int64_t R, const int32_t *__restrict__ lab_s, const int32_t *__restrict__ cstart,
+                                      int32_t *__restrict__ csize) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t c = lab_s[i];
+    if (i == R - 1 || lab_s[i + 1] != c) csize[c] = (int32_t)(i - cstart[c] + 1);
+  }
+}
+
+__global__ void k_query_flag_empty(int64_t K, const int32_t *__restrict__ csize, int *__restrict__ bad) {
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < K; k += (int64_t)gridDim.x * blockDim.x)
+    if (csize[k] <= 0) *bad = 1;
+}
+
+// entry n is 0, so an exclusive scan over n + 1 entries ends with the number of candidate keys
+__global__ void k_query_emit_sizes(int64_t n, const unsigned long long *__restrict__ qk,
+                                   const int32_t *__restrict__ csize, long long *__restrict__ len) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= n; i += (int64_t)gridDim.x * blockDim.x)
+    len[i] = i < n ? csize[(uint32_t)(qk[i] & 0xffffffffull)] : 0;
+}
+
+// one warp per emitted (q, k): the keys q << 32 | r of the records of cluster k
+__global__ void k_query_emit_keys(int64_t n, const unsigned long long *__restrict__ qk,
+                                  const int32_t *__restrict__ cstart, const int32_t *__restrict__ rec_s,
+                                  const long long *__restrict__ off, unsigned long long *__restrict__ keys) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * WARPS_PER_BLOCK;
+  for (int64_t w = blockIdx.x * (int64_t)WARPS_PER_BLOCK + (threadIdx.x >> 5); w < n; w += nwarps) {
+    const unsigned long long hi = qk[w] & 0xffffffff00000000ull;
+    const int32_t k = (int32_t)(qk[w] & 0xffffffffull);
+    const long long o = off[w], m = off[w + 1] - o;
+    const int32_t *rec = rec_s + cstart[k];
+    for (long long j = lane; j < m; j += 32) keys[o + j] = hi | (uint32_t)rec[j];
+  }
+}
+
+// per query the largest log Z over the pass-1 samples
+__global__ void k_query_scale(int32_t Q, int32_t S, const double *__restrict__ logz, double *__restrict__ scale) {
+  for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < Q; q += (int64_t)gridDim.x * blockDim.x) {
+    double m = -INFINITY;
+    for (int32_t s = 0; s < S; ++s) m = fmax(m, logz[(int64_t)s * Q + q]);
+    scale[q] = m;
+  }
+}
+
+// pass 2, one thread per candidate: sum += exp(log m + log rho - L_q) of the record's cluster in this sample
+__global__ void k_query_score(int64_t H, int32_t A, const unsigned long long *__restrict__ key,
+                              const int32_t *__restrict__ label, const int32_t *__restrict__ y,
+                              const int32_t *__restrict__ voff, const double *__restrict__ norm,
+                              const int32_t *__restrict__ x, const double *__restrict__ c0,
+                              const double *__restrict__ c1, const unsigned long long *__restrict__ mask,
+                              const long long *__restrict__ hoff, const int32_t *__restrict__ hcol,
+                              const double *__restrict__ hval, const double *__restrict__ logm,
+                              const double *__restrict__ scale, double *__restrict__ sum) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < H; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t q = (int64_t)(key[i] >> 32);
+    const int32_t r = (int32_t)(key[i] & 0xffffffffull);
+    const int32_t *ys = y + (int64_t)label[r] * A;
+    const int64_t qa0 = q * A;
+    double rho = 1.0;
+    for (int a = 0; a < A; ++a) {
+      const int32_t xv = x[qa0 + a];
+      if (xv < 0) continue;
+      const int32_t v = ys[a];
+      double t = c1[qa0 + a] * norm[voff[a] + v];
+      if (mask[qa0 + a] & hit_bit(v)) t = t * hit_value(hcol, hval, hoff[qa0 + a], hoff[qa0 + a + 1], v);
+      rho = rho * ((v == xv ? c0[qa0 + a] : 0.0) + t);
+    }
+    sum[i] += exp(logm[q] + log(rho) - scale[q]);
+  }
+}
+
+__global__ void k_query_split(int64_t H, const unsigned long long *__restrict__ key, int32_t *__restrict__ query,
+                              int32_t *__restrict__ record) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < H; i += (int64_t)gridDim.x * blockDim.x) {
+    query[i] = (int32_t)(key[i] >> 32);
+    record[i] = (int32_t)(key[i] & 0xffffffffull);
+  }
+}
+
+// per query, in sample order: sum Z~, sum Z~^2 and the new-entity sum, Z~ = exp(log Z - L_q)
+__global__ void k_query_totals(int32_t Q, int32_t S, const double *__restrict__ logz, const double *__restrict__ logm,
+                               const long long *__restrict__ kcount, int64_t M, const double *__restrict__ scale,
+                               double *__restrict__ zsum, double *__restrict__ zsq, double *__restrict__ fresh) {
+  for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < Q; q += (int64_t)gridDim.x * blockDim.x) {
+    double a = 0.0, b = 0.0, c = 0.0;
+    for (int32_t s = 0; s < S; ++s) {
+      const double z = exp(logz[(int64_t)s * Q + q] - scale[q]);
+      a += z;
+      b += z * z;
+      const long long un = M - kcount[s];
+      if (un > 0) c += exp(log((double)un) + logm[(int64_t)s * Q + q] - scale[q]);
+    }
+    zsum[q] = a;
+    zsq[q] = b;
+    fresh[q] = c;
+  }
+}
+}  // namespace
+
+struct dbl_query : Handle {
+  int32_t Q = 0, A = 0, F = 0;
+  int64_t M = 0, max_candidates = 0;
+  double t = 0.0;
+  int64_t emit_cap = 0;                 // (q, k) pairs one sample may emit: Q (floor(1 / t) + 2), max_candidates
+  int q_bits = 1;                       // bits of a query index
+  Buf voff, nvals, norm;                // per attribute: offset into norm, V_a; norm(y) of every attribute
+  Buf file, x, psi, sigma, mask;        // per query / (query, attribute)
+  Buf hoff, hcol, hval;                 // hit rows: (Q A + 1) int64 offsets, their value ids and expsim
+  Buf c0, c1, logm1, thr, theta;        // one sample's coefficients, log m, emission thresholds and theta
+  Buf y;                                // one sample's cluster values [K][A]
+  Buf partial;                          // [chunks][Q] pass-1 sums
+  Buf logz, logm, kcount;               // per pass-1 sample: [S][Q] log Z, [S][Q] log m, K_s
+  int32_t S2 = 0;                       // pass-2 samples scored
+  Buf scale, sums;                      // L_q; per held candidate the pass-2 sum
+  Buf iota, lab_s, rec_s, head, start;  // records grouped by label
+  Buf cstart, csize;                    // per cluster
+  Buf emit, emit_n, len, off;           // emitted (q, k), their count, key counts and offsets
+  Buf key_in, key_s, is_new, rank;      // candidate keys of a sample, merge flags and ranks
+  Buf tab_key[2], tab_cnt[2];           // held candidate set (index cur) and the spare one
+  int cur = 0;
+  int64_t H = 0;
+  Buf tmp;
+};
+
+namespace {
+size_t query_smem(int32_t A) {
+  return (size_t)A * QUERY_THREADS * (3 * sizeof(double) + sizeof(int32_t)) +
+         (size_t)A * QUERY_TILE * (sizeof(double) + sizeof(int32_t));
+}
+
+// One sample's common steps: labels in [0, K), value ids in range, theta in [0, 1]; theta and the values uploaded;
+// the coefficients and log m of every query (into c0, c1, logm_out)
+int query_take_sample(dbl_query *p, const int32_t *labels, int32_t K, const int32_t *values, const double *theta,
+                      double *logm_out) {
+  if (K <= 0 || K > p->M || K > p->R) return DBL_ERR_INVALID;
+  const int A = p->A, F = p->F;
+  for (int i = 0; i < A * F; ++i)
+    if (!(theta[i] >= 0.0 && theta[i] <= 1.0)) return DBL_ERR_INVALID;
+  if (const int rc = p->take_labels(labels, p->cluster, K); rc != DBL_OK) return rc;
+  cudaStream_t st = p->stream;
+  const int64_t n = (int64_t)K * A;
+  POST_TRY(p->y.reserve(sizeof(int32_t) * (size_t)n));
+  POST_TRY(cudaMemcpyAsync(p->y.p, values, sizeof(int32_t) * n, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(p->theta.p, theta, sizeof(double) * A * F, cudaMemcpyHostToDevice, st));
+  POST_TRY(cudaMemsetAsync(p->bad.p, 0, sizeof(int), st));
+  k_query_check_values<<<grid_for(n), THREADS, 0, st>>>(n, A, p->y.as<int32_t>(), p->nvals.as<int32_t>(),
+                                                        p->bad.as<int>());
+  int flag = 0;
+  POST_TRY(cudaMemcpyAsync(&flag, p->bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaStreamSynchronize(st));
+  if (flag) return DBL_ERR_INVALID;
+  k_query_coef<<<grid_for(p->Q), THREADS, 0, st>>>(p->Q, A, F, p->file.as<int32_t>(), p->x.as<int32_t>(),
+                                                   p->psi.as<double>(), p->sigma.as<double>(), p->theta.as<double>(),
+                                                   p->c0.as<double>(), p->c1.as<double>(), logm_out);
+  POST_TRY(cudaGetLastError());
+  return DBL_OK;
+}
+}  // namespace
+
+extern "C" int dbl_query_create(dbl_query **out, int64_t num_records, int64_t population_size, int32_t num_queries,
+                                int32_t num_attrs, int32_t num_files, const int32_t *num_values, const double *norm,
+                                const int32_t *file, const int32_t *x, const double *psi, const double *sigma,
+                                const int64_t *hit_offsets, const int32_t *hit_values, const double *hit_expsim,
+                                double min_link_probability, int64_t max_candidates) {
+  if (!out) return DBL_ERR_INVALID;
+  *out = nullptr;
+  if (num_records <= 0 || num_records > INT32_MAX || population_size < 1 || num_queries <= 0 || num_attrs <= 0 ||
+      num_attrs > 32 || num_files <= 0 || !num_values || !norm || !file || !x || !psi || !sigma || !hit_offsets ||
+      !(min_link_probability > 0.0 && min_link_probability <= 1.0) || max_candidates <= 0 ||
+      max_candidates > INT32_MAX)
+    return DBL_ERR_INVALID;
+  const int64_t Q = num_queries, A = num_attrs, QA = Q * A, nh = hit_offsets[QA];
+  if (hit_offsets[0] != 0 || nh < 0 || (nh > 0 && (!hit_values || !hit_expsim))) return DBL_ERR_INVALID;
+  std::vector<int32_t> voff(A);
+  int64_t nv_total = 0;
+  for (int a = 0; a < A; ++a) {
+    if (num_values[a] <= 0) return DBL_ERR_INVALID;
+    voff[a] = (int32_t)nv_total;
+    nv_total += num_values[a];
+  }
+  if (nv_total > INT32_MAX) return DBL_ERR_INVALID;
+  for (int64_t q = 0; q < Q; ++q)
+    if (file[q] < 0 || file[q] >= num_files) return DBL_ERR_INVALID;
+  for (int64_t i = 0; i < QA; ++i) {
+    const int a = (int)(i % A);
+    if (x[i] < -1 || x[i] >= num_values[a] || hit_offsets[i] > hit_offsets[i + 1]) return DBL_ERR_INVALID;
+  }
+  std::vector<unsigned long long> mask(QA, 0ull);
+  for (int64_t i = 0; i < QA; ++i)
+    for (int64_t j = hit_offsets[i]; j < hit_offsets[i + 1]; ++j) {
+      const int32_t v = hit_values[j];
+      if (v < 0 || v >= num_values[i % A] || (j > hit_offsets[i] && hit_values[j - 1] >= v)) return DBL_ERR_INVALID;
+      mask[i] |= 1ull << ((uint32_t)v * 0x9E3779B1u >> 26);
+    }
+  return open_handle(out, num_records, [&](dbl_query *p) {
+    p->Q = num_queries;
+    p->A = num_attrs;
+    p->F = num_files;
+    p->M = population_size;
+    p->t = min_link_probability;
+    p->max_candidates = max_candidates;
+    // every emitted (q, k) adds at least one candidate key, so more than max_candidates is a refusal anyway
+    // clamped before the product: at most max_candidates (< 2^31) per query, so Q times it fits int64
+    const int64_t per_query = (int64_t)std::min(std::floor(1.0 / min_link_probability) + 2.0, (double)max_candidates);
+    p->emit_cap = std::min<int64_t>(Q * per_query, max_candidates);
+    p->q_bits = bits_for(Q);
+    const int64_t R = num_records;
+    const size_t r4 = sizeof(int32_t) * (size_t)R, qa8 = sizeof(double) * (size_t)QA;
+    if (p->voff.alloc(sizeof(int32_t) * A) != cudaSuccess || p->nvals.alloc(sizeof(int32_t) * A) != cudaSuccess ||
+        p->norm.alloc(sizeof(double) * nv_total) != cudaSuccess || p->file.alloc(sizeof(int32_t) * Q) != cudaSuccess ||
+        p->x.alloc(sizeof(int32_t) * QA) != cudaSuccess || p->psi.alloc(qa8) != cudaSuccess ||
+        p->sigma.alloc(qa8) != cudaSuccess || p->mask.alloc(qa8) != cudaSuccess ||
+        p->hoff.alloc(sizeof(long long) * (QA + 1)) != cudaSuccess ||
+        p->hcol.alloc(sizeof(int32_t) * std::max<int64_t>(nh, 1)) != cudaSuccess ||
+        p->hval.alloc(sizeof(double) * std::max<int64_t>(nh, 1)) != cudaSuccess || p->c0.alloc(qa8) != cudaSuccess ||
+        p->c1.alloc(qa8) != cudaSuccess || p->logm1.alloc(sizeof(double) * Q) != cudaSuccess ||
+        p->thr.alloc(sizeof(double) * Q) != cudaSuccess || p->theta.alloc(sizeof(double) * A * num_files) != cudaSuccess ||
+        p->scale.alloc(sizeof(double) * Q) != cudaSuccess || p->iota.alloc(r4) != cudaSuccess ||
+        p->lab_s.alloc(r4) != cudaSuccess || p->rec_s.alloc(r4) != cudaSuccess || p->head.alloc(r4) != cudaSuccess ||
+        p->start.alloc(r4) != cudaSuccess || p->cstart.alloc(r4) != cudaSuccess || p->csize.alloc(r4) != cudaSuccess ||
+        p->emit.alloc(sizeof(unsigned long long) * std::min<int64_t>(p->emit_cap, 4 * Q + 1024)) != cudaSuccess ||
+        p->emit_n.alloc(sizeof(unsigned long long)) != cudaSuccess)
+      return DBL_ERR_CUDA;
+    cudaStream_t st = p->stream;
+    POST_TRY(cudaMemcpyAsync(p->voff.p, voff.data(), sizeof(int32_t) * A, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(p->nvals.p, num_values, sizeof(int32_t) * A, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(p->norm.p, norm, sizeof(double) * nv_total, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(p->file.p, file, sizeof(int32_t) * Q, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(p->x.p, x, sizeof(int32_t) * QA, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(p->psi.p, psi, qa8, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(p->sigma.p, sigma, qa8, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(p->mask.p, mask.data(), qa8, cudaMemcpyHostToDevice, st));
+    POST_TRY(cudaMemcpyAsync(p->hoff.p, hit_offsets, sizeof(long long) * (QA + 1), cudaMemcpyHostToDevice, st));
+    if (nh > 0) {
+      POST_TRY(cudaMemcpyAsync(p->hcol.p, hit_values, sizeof(int32_t) * nh, cudaMemcpyHostToDevice, st));
+      POST_TRY(cudaMemcpyAsync(p->hval.p, hit_expsim, sizeof(double) * nh, cudaMemcpyHostToDevice, st));
+    }
+    // the largest any handle needs (32 attributes): a later handle with fewer attributes must not lower the limit an
+    // earlier one launches under
+    const int smem = (int)query_smem(32);
+    POST_TRY(cudaFuncSetAttribute(k_query_scan<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    POST_TRY(cudaFuncSetAttribute(k_query_scan<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    k_iota<<<grid_for(R), THREADS, 0, st>>>(R, p->iota.as<int32_t>());
+    POST_TRY(cudaGetLastError());
+    POST_TRY(cudaStreamSynchronize(st));
+    return DBL_OK;
+  });
+}
+
+extern "C" void dbl_query_free(dbl_query *p) { free_handle(p); }
+
+extern "C" int32_t dbl_query_num_samples(const dbl_query *p) { return p ? p->S : 0; }
+
+// Pass 1, one sample: coefficients; the scan's sums and log Z; the emitting scan; the emitted clusters' records as
+// candidate keys, radix-sorted and merged into the spare set; commit (set swap, log Z / log m / K kept, S + 1) only when
+// the union fits max_candidates.  A refusal or failure leaves the handle as it was.
+extern "C" int dbl_query_add_sample(dbl_query *p, const int32_t *labels, int32_t num_clusters, const int32_t *values,
+                                    const double *theta) {
+  if (!p || !labels || !values || !theta || p->S == INT32_MAX) return DBL_ERR_INVALID;
+  if (p->S2 > 0) return DBL_ERR_STATE;  // pass 2 has begun
+  DeviceScope ds(p->device);
+  const int64_t Q = p->Q, A = p->A, R = p->R, K = num_clusters, S = p->S;
+  cudaStream_t st = p->stream;
+  POST_TRY(p->logz.reserve_keep(sizeof(double) * Q * (S + 1), sizeof(double) * Q * S, st));
+  POST_TRY(p->logm.reserve_keep(sizeof(double) * Q * (S + 1), sizeof(double) * Q * S, st));
+  POST_TRY(p->kcount.reserve_keep(sizeof(long long) * (S + 1), sizeof(long long) * S, st));
+  double *logz_s = p->logz.as<double>() + Q * S, *logm_s = p->logm.as<double>() + Q * S;
+  if (const int rc = query_take_sample(p, labels, num_clusters, values, theta, logm_s); rc != DBL_OK) return rc;
+
+  // records grouped by cluster; every cluster must hold one
+  const int rc_g = group_by_key(R, bits_for(K), p->cluster.as<int32_t>(), p->iota.as<int32_t>(),
+                                p->lab_s.as<int32_t>(), p->rec_s.as<int32_t>(), p->head.as<int32_t>(),
+                                p->start.as<int32_t>(), p->tmp, st);
+  if (rc_g != DBL_OK) return rc_g;
+  POST_TRY(cudaMemsetAsync(p->csize.p, 0, sizeof(int32_t) * K, st));
+  k_query_cluster_bounds<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_s.as<int32_t>(), p->cstart.as<int32_t>());
+  k_query_cluster_sizes<<<grid_for(R), THREADS, 0, st>>>(R, p->lab_s.as<int32_t>(), p->cstart.as<int32_t>(),
+                                                         p->csize.as<int32_t>());
+  POST_TRY(cudaMemsetAsync(p->bad.p, 0, sizeof(int), st));
+  k_query_flag_empty<<<grid_for(K), THREADS, 0, st>>>(K, p->csize.as<int32_t>(), p->bad.as<int>());
+
+  // the scan: sums per chunk, then log Z and thresholds, then the emitting scan
+  const int64_t qtiles = (Q + QUERY_THREADS - 1) / QUERY_THREADS;
+  const int64_t tiles = (K + QUERY_TILE - 1) / QUERY_TILE;
+  const int64_t chunks = std::max<int64_t>(1, std::min<int64_t>(tiles, (2048 + qtiles - 1) / qtiles));
+  const int64_t chunk = ((tiles + chunks - 1) / chunks) * QUERY_TILE;
+  const int64_t used = (K + chunk - 1) / chunk;
+  POST_TRY(p->partial.reserve(sizeof(double) * Q * used));
+  const dim3 grid((unsigned)qtiles, (unsigned)used);
+  const size_t smem = query_smem((int32_t)A);
+  k_query_scan<false><<<grid, QUERY_THREADS, smem, st>>>(
+      (int32_t)Q, (int32_t)A, K, chunk, p->y.as<int32_t>(), p->voff.as<int32_t>(), p->norm.as<double>(),
+      p->x.as<int32_t>(), p->c0.as<double>(), p->c1.as<double>(), p->mask.as<unsigned long long>(),
+      p->hoff.as<long long>(), p->hcol.as<int32_t>(), p->hval.as<double>(), p->partial.as<double>(), nullptr, nullptr,
+      nullptr, 0);
+  k_query_logz<<<grid_for(Q), THREADS, 0, st>>>((int32_t)Q, (int32_t)used, p->partial.as<double>(),
+                                                (double)(p->M - K), logm_s, p->t, logz_s, p->thr.as<double>());
+  // the emitting scan; run again with a larger buffer when the first one overflowed it
+  unsigned long long n_emit = 0;
+  int flag = 0;
+  for (int pass = 0; pass < 2; ++pass) {
+    const unsigned long long room = p->emit.cap / sizeof(unsigned long long);
+    POST_TRY(cudaMemsetAsync(p->emit_n.p, 0, sizeof(unsigned long long), st));
+    k_query_scan<true><<<grid, QUERY_THREADS, smem, st>>>(
+        (int32_t)Q, (int32_t)A, K, chunk, p->y.as<int32_t>(), p->voff.as<int32_t>(), p->norm.as<double>(),
+        p->x.as<int32_t>(), p->c0.as<double>(), p->c1.as<double>(), p->mask.as<unsigned long long>(),
+        p->hoff.as<long long>(), p->hcol.as<int32_t>(), p->hval.as<double>(), nullptr, p->thr.as<double>(),
+        p->emit.as<unsigned long long>(), p->emit_n.as<unsigned long long>(), room);
+    POST_TRY(cudaGetLastError());
+    POST_TRY(cudaMemcpyAsync(&n_emit, p->emit_n.p, sizeof(n_emit), cudaMemcpyDeviceToHost, st));
+    POST_TRY(cudaMemcpyAsync(&flag, p->bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    POST_TRY(cudaStreamSynchronize(st));
+    if (flag || n_emit > (unsigned long long)p->emit_cap) return DBL_ERR_INVALID;
+    if (n_emit <= room) break;
+    POST_TRY(p->emit.reserve(sizeof(unsigned long long) * n_emit));
+  }
+  POST_TRY(p->len.reserve(sizeof(long long) * (n_emit + 1)));
+  POST_TRY(p->off.reserve(sizeof(long long) * (n_emit + 1)));
+
+  // the emitted clusters' records as keys q << 32 | r
+  const int64_t ne = (int64_t)n_emit;
+  size_t tb = 0;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, p->len.as<long long>(), p->off.as<long long>(), ne + 1, st));
+  POST_TRY(p->tmp.reserve(tb));
+  k_query_emit_sizes<<<grid_for(ne + 1), THREADS, 0, st>>>(ne, p->emit.as<unsigned long long>(),
+                                                           p->csize.as<int32_t>(), p->len.as<long long>());
+  tb = p->tmp.cap;
+  POST_TRY(cub::DeviceScan::ExclusiveSum(p->tmp.p, tb, p->len.as<long long>(), p->off.as<long long>(), ne + 1, st));
+  long long n = 0;
+  POST_TRY(cudaMemcpyAsync(&n, p->off.as<long long>() + ne, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  if (n > p->max_candidates) return DBL_ERR_INVALID;  // this sample alone does not fit
+  const size_t cap8 = sizeof(unsigned long long) * (size_t)p->max_candidates;
+  const size_t cap4 = sizeof(int32_t) * (size_t)(p->max_candidates + 1);
+  POST_TRY(p->key_in.reserve(sizeof(unsigned long long) * (size_t)n, cap8));
+  POST_TRY(p->key_s.reserve(sizeof(unsigned long long) * (size_t)n, cap8));
+  POST_TRY(p->is_new.reserve(sizeof(int32_t) * (size_t)(n + 1), cap4));
+  POST_TRY(p->rank.reserve(sizeof(int32_t) * (size_t)(n + 1), cap4));
+  if (n > 0) {
+    k_query_emit_keys<<<(int)std::min<int64_t>((ne + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, 8192), THREADS, 0, st>>>(
+        ne, p->emit.as<unsigned long long>(), p->cstart.as<int32_t>(), p->rec_s.as<int32_t>(), p->off.as<long long>(),
+        p->key_in.as<unsigned long long>());
+    size_t tbk = 0;
+    POST_TRY(cub::DeviceRadixSort::SortKeys(nullptr, tbk, (const unsigned long long *)nullptr,
+                                            (unsigned long long *)nullptr, (int64_t)n, 0, 32 + p->q_bits, st));
+    POST_TRY(p->tmp.reserve(tbk));
+    tbk = p->tmp.cap;
+    POST_TRY(cub::DeviceRadixSort::SortKeys(p->tmp.p, tbk, p->key_in.as<unsigned long long>(),
+                                            p->key_s.as<unsigned long long>(), (int64_t)n, 0, 32 + p->q_bits, st));
+  }
+
+  // merge into the spare set, then commit
+  const unsigned long long *keys = p->key_s.as<unsigned long long>();
+  const unsigned long long *held = p->tab_key[p->cur].as<unsigned long long>();
+  const int32_t *hcnt = p->tab_cnt[p->cur].as<int32_t>();
+  const int64_t H = p->H;
+  int64_t fresh = 0;
+  if (const int rc = probe_new_keys(n, keys, H, held, p->is_new, p->rank, p->tmp, st, &fresh); rc != DBL_OK) return rc;
+  const int64_t H2 = H + fresh;
+  if (H2 > p->max_candidates) return DBL_ERR_INVALID;  // the union does not fit: the held set stays as it is
+  const int nxt = p->cur ^ 1;
+  POST_TRY(p->tab_key[nxt].reserve(sizeof(unsigned long long) * (size_t)H2, cap8));
+  POST_TRY(p->tab_cnt[nxt].reserve(sizeof(int32_t) * (size_t)H2, sizeof(int32_t) * (size_t)p->max_candidates));
+  if (const int rc = merge_keys<int32_t>(H, held, hcnt, n, keys, nullptr, p->is_new, p->rank,
+                                         p->tab_key[nxt].as<unsigned long long>(), p->tab_cnt[nxt].as<int32_t>(), st);
+      rc != DBL_OK)
+    return rc;
+  const long long kc = K;
+  POST_TRY(cudaMemcpyAsync(p->kcount.as<long long>() + S, &kc, sizeof(long long), cudaMemcpyHostToDevice, st));
+  POST_TRY(cudaStreamSynchronize(st));
+  p->cur = nxt;
+  p->H = H2;
+  ++p->S;
+  return DBL_OK;
+}
+
+// Pass 2, one sample, in pass-1 order: the same checks and coefficients, then one thread per held candidate.  The
+// first call fixes L_q and zeroes the sums.  A refusal leaves the sums as they were.
+extern "C" int dbl_query_score_sample(dbl_query *p, const int32_t *labels, int32_t num_clusters, const int32_t *values,
+                                      const double *theta) {
+  if (!p || !labels || !values || !theta) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  if (p->S2 >= p->S) return DBL_ERR_INVALID;  // more pass-2 samples than pass-1 samples
+  DeviceScope ds(p->device);
+  const int64_t Q = p->Q, H = p->H, s = p->S2;
+  cudaStream_t st = p->stream;
+  long long kc = 0;
+  POST_TRY(cudaMemcpy(&kc, p->kcount.as<long long>() + s, sizeof(long long), cudaMemcpyDeviceToHost));
+  if (kc != num_clusters) return DBL_ERR_INVALID;  // not the pass-1 sample at this position
+  if (const int rc = query_take_sample(p, labels, num_clusters, values, theta, p->logm1.as<double>()); rc != DBL_OK)
+    return rc;
+  if (s == 0) {
+    POST_TRY(p->sums.reserve(sizeof(double) * (size_t)std::max<int64_t>(H, 1)));
+    POST_TRY(cudaMemsetAsync(p->sums.p, 0, sizeof(double) * (size_t)std::max<int64_t>(H, 1), st));
+    k_query_scale<<<grid_for(Q), THREADS, 0, st>>>((int32_t)Q, p->S, p->logz.as<double>(), p->scale.as<double>());
+  }
+  if (H > 0)
+    k_query_score<<<grid_for(H), THREADS, 0, st>>>(
+        H, p->A, p->tab_key[p->cur].as<unsigned long long>(), p->cluster.as<int32_t>(), p->y.as<int32_t>(),
+        p->voff.as<int32_t>(), p->norm.as<double>(), p->x.as<int32_t>(), p->c0.as<double>(), p->c1.as<double>(),
+        p->mask.as<unsigned long long>(), p->hoff.as<long long>(), p->hcol.as<int32_t>(), p->hval.as<double>(),
+        p->logm1.as<double>(), p->scale.as<double>(), p->sums.as<double>());
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  ++p->S2;
+  return DBL_OK;
+}
+
+extern "C" int dbl_query_num_candidates(const dbl_query *p, int64_t *n_out) {
+  if (!p || !n_out) return DBL_ERR_INVALID;
+  *n_out = p->H;
+  return DBL_OK;
+}
+
+// The held candidates in (query, record) order with their pass-2 sums, and per query L_q, sum Z~, sum Z~^2, the
+// new-entity sum and every pass-1 sample's log Z ([S][Q]).  Host or device outputs.
+extern "C" int dbl_query_read(dbl_query *p, int32_t *query, int32_t *record, double *sum, double *scale, double *zsum,
+                              double *zsq, double *fresh, double *logz) {
+  if (!p || (p->H > 0 && (!query || !record || !sum)) || !scale || !zsum || !zsq || !fresh || !logz)
+    return DBL_ERR_INVALID;
+  if (p->S == 0 || p->S2 != p->S) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  const int64_t Q = p->Q, H = p->H, S = p->S;
+  cudaStream_t st = p->stream;
+  Buf f, r, a, b, c;
+  POST_TRY(f.alloc(sizeof(int32_t) * std::max<int64_t>(H, 1)));
+  POST_TRY(r.alloc(sizeof(int32_t) * std::max<int64_t>(H, 1)));
+  POST_TRY(a.alloc(sizeof(double) * Q));
+  POST_TRY(b.alloc(sizeof(double) * Q));
+  POST_TRY(c.alloc(sizeof(double) * Q));
+  if (H > 0)
+    k_query_split<<<grid_for(H), THREADS, 0, st>>>(H, p->tab_key[p->cur].as<unsigned long long>(), f.as<int32_t>(),
+                                                   r.as<int32_t>());
+  k_query_totals<<<grid_for(Q), THREADS, 0, st>>>((int32_t)Q, (int32_t)S, p->logz.as<double>(), p->logm.as<double>(),
+                                                  p->kcount.as<long long>(), p->M, p->scale.as<double>(), a.as<double>(),
+                                                  b.as<double>(), c.as<double>());
+  POST_TRY(cudaGetLastError());
+  // host or device outputs: unified addressing picks the copy direction
+  if (H > 0) {
+    POST_TRY(cudaMemcpyAsync(query, f.p, sizeof(int32_t) * H, cudaMemcpyDefault, st));
+    POST_TRY(cudaMemcpyAsync(record, r.p, sizeof(int32_t) * H, cudaMemcpyDefault, st));
+    POST_TRY(cudaMemcpyAsync(sum, p->sums.p, sizeof(double) * H, cudaMemcpyDefault, st));
+  }
+  POST_TRY(cudaMemcpyAsync(scale, p->scale.p, sizeof(double) * Q, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(zsum, a.p, sizeof(double) * Q, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(zsq, b.p, sizeof(double) * Q, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(fresh, c.p, sizeof(double) * Q, cudaMemcpyDefault, st));
+  POST_TRY(cudaMemcpyAsync(logz, p->logz.p, sizeof(double) * Q * S, cudaMemcpyDefault, st));
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}

@@ -35,7 +35,7 @@ SUPPORTED_METRICS = (SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
                         "binder-search-clusters", "vi-clusters", "vi-search-clusters", "credible-ball",
-                        "entity-values", "pairwise-match-diagnostics", "clerical-review")
+                        "entity-values", "pairwise-match-diagnostics", "clerical-review", "distortion-probabilities")
 # the point estimates a credible ball may be centred on
 CREDIBLE_BALL_CENTERS = ("shared-most-probable-clusters", "binder-clusters", "binder-search-clusters", "vi-clusters",
                          "vi-search-clusters")
@@ -335,6 +335,22 @@ def _save_entity_values(prm):
     return {"save_entity_values": True} if save else {}
 
 
+def _save_distortion_probabilities(prm):
+    """{"save_distortion_probabilities": True} when the sample step records theta, else nothing."""
+    save = prm.get("saveDistortionProbabilities", False)
+    if not isinstance(save, bool):
+        raise ValueError("saveDistortionProbabilities must be a boolean.")
+    return {"save_distortion_probabilities": True} if save else {}
+
+
+def link_queries(tables, samples, num_records, population_size, min_link_probability):
+    """analysis_arrays.QueryResult of the query records against the samples: on the GPU when the platform has one
+    (analysis_gpu), else on the host (analysis_arrays).  Both give the same candidates and sums within rounding."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.link_queries(tables, samples, num_records, population_size, min_link_probability)
+    return analysis_arrays.link_queries(tables, samples, num_records, population_size, min_link_probability)
+
+
 def _searched_cost(false_link_cost):
     a, b = analysis_arrays.search_cost(false_link_cost)
     return a / b
@@ -445,7 +461,9 @@ class Project:
                          f"burninInterval={prm['burnin_interval']}, thinningInterval={prm['thinning_interval']} and "
                          f"sampler={prm['sampler']}"
                          + (", saving every sample's entity values (saveEntityValues=true)"
-                            if prm.get("save_entity_values") else ""))
+                            if prm.get("save_entity_values") else "")
+                         + (", saving every sample's distortion probabilities (saveDistortionProbabilities=true)"
+                            if prm.get("save_distortion_probabilities") else ""))
             elif name == "summarize":
                 L.append(f"  * SummarizeStep: Calculating summary quantities {braces(prm['quantities'])} along the "
                          f"chain for iterations >= {prm['lower_iteration_cutoff']}")
@@ -477,6 +495,9 @@ class Project:
                     L.append(f"  * SummarizeStep: entity-values is the most probable value of each attribute of the "
                              f"entity of each cluster of a point estimate, from the entity values saved with the "
                              f"samples, with {_center_settings(prm, 'entity_values_center', 'entityValuesCenter')}")
+                if "distortion-probabilities" in prm["quantities"]:
+                    L.append("  * SummarizeStep: distortion-probabilities summarises the distortion probabilities "
+                             "saved with the samples, per attribute and file")
                 if "clerical-review" in prm["quantities"]:
                     L.append(f"  * SummarizeStep: clerical-review ranks the clusters of a point estimate by their "
                              f"expected false and missed links, with {_clerical_review_settings(prm)}")
@@ -523,6 +544,11 @@ class Project:
                     L.append(f"  * EvaluateStep: Evaluating how soon the clerical review queue of a point estimate "
                              f"reaches its clusters that are not a true entity ({_clerical_review_settings(prm)}, "
                              f"iterations >= {prm['lower_iteration_cutoff']}) using {braces(review)} metrics")
+            elif name == "link-records":
+                L.append(f"  * LinkRecordsStep: Linking the records of '{prm['query_path']}' to the chain for "
+                         f"iterations >= {prm['lower_iteration_cutoff']}, reporting the records they share an entity "
+                         f"with at minLinkProbability={prm['min_link_probability']!r}; each query is scored against "
+                         f"the data alone: queries are not linked to each other and the chain is not updated")
             else:
                 L.append("  * CopyFilesStep: Copying {" + ", ".join(prm["file_names"]) + "} to destination "
                          + prm["destination_path"])
@@ -651,7 +677,7 @@ class Project:
                                            burnin_interval=int(prm.get("burninInterval", 0)),
                                            thinning_interval=int(prm.get("thinningInterval", 1)),
                                            resume=bool(prm.get("resume", True)), sampler=prm.get("sampler", "PCG-I"),
-                                           **_save_entity_values(prm))))
+                                           **_save_entity_values(prm), **_save_distortion_probabilities(prm))))
             elif name == "summarize":
                 q = list(prm["quantities"])
                 if not q or any(x not in SUPPORTED_QUANTITIES for x in q):
@@ -679,6 +705,13 @@ class Project:
                                              max_search_rounds=_max_search_rounds(prm),
                                              clerical_review_center=_clerical_review_center(prm),
                                              **_credible_ball_params(prm))))
+            elif name == "link-records":
+                if "queryPath" not in prm:
+                    raise ValueError("link-records needs queryPath.")
+                out.append(("link-records", dict(
+                    query_path=str(prm["queryPath"]), lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)),
+                    min_link_probability=analysis_arrays._check_min_link_probability(
+                        prm.get("minLinkProbability", 0.05)))))
             elif name == "copy-files":
                 out.append(("copy-files", dict(file_names=list(prm["fileNames"]),
                                                destination_path=prm["destinationPath"],
@@ -702,7 +735,9 @@ class Project:
                     f"thinningInterval={prm['thinning_interval']} sampler={prm['sampler']}")
                 chain.sample(eng, d["rec_ids"], [a.name for a in self.matching_attributes], prm["sample_size"],
                              self.output_path, prm["burnin_interval"], prm["thinning_interval"], sampler=prm["sampler"],
-                             entity_values=self.attribute_values() if prm.get("save_entity_values") else None)
+                             entity_values=self.attribute_values() if prm.get("save_entity_values") else None,
+                             distortion_columns=self.distortion_columns()
+                             if prm.get("save_distortion_probabilities") else None)
                 self.save_state(eng)  # Sampler.scala:120
             elif name == "summarize":
                 # array implementations (analysis_arrays): same quantities as analysis.py, no loop over clusters
@@ -770,6 +805,13 @@ class Project:
                                 f"credible-ball-{name}-{bound}.csv")
                     elif q == "entity-values":
                         self._summarize_entity_values(ch, prm)
+                    elif q == "distortion-probabilities":
+                        A, F = len(self.matching_attributes), len(self.load()["cache"].file_ids)
+                        theta = analysis_arrays.read_distortion_probabilities(self.chain_dirs(), ch, A, F)
+                        cols = [(a.name, f) for a in self.matching_attributes for f in self.load()["cache"].file_ids]
+                        writers.save_distortion_probabilities(
+                            [(a, f, vals[:5], vals[5]) for (a, f), vals in
+                             zip(cols, analysis_arrays.distortion_summary(theta))], self.output_path)
                     elif q == "clerical-review":
                         review = clerical_review_estimate(ch, prm["clerical_review_center"], prm["false_link_cost"],
                                                           prm["max_search_rounds"])
@@ -889,6 +931,8 @@ class Project:
                     text.append(analysis.format_clerical_review(res))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
+            elif name == "link-records":
+                self._link_records(prm)
             elif name == "copy-files":
                 os.makedirs(prm["destination_path"], exist_ok=True)
                 for fn in prm["file_names"]:
@@ -916,6 +960,91 @@ class Project:
 
         return [pa.array([ix.value_of(v) for v in range(ix.num_values)], pa.string())
                 for ix in self.load()["cache"].indexes]
+
+    def distortion_columns(self):
+        """The columns of distortion-probabilities-chain.csv: <attribute>[<file id>], attribute-major."""
+        return writers.distortion_columns([a.name for a in self.matching_attributes], self.load()["cache"].file_ids)
+
+    def read_queries(self, path):
+        """(query ids, x int32[Q][A] with -1 for missing and unseen values, file int32[Q], unseen attribute names per
+        query) of a query CSV with the data's record-id, matching-attribute and file-id columns."""
+        import csv
+        import gzip
+
+        d = self.load()
+        cache, names = d["cache"], [a.name for a in self.matching_attributes]
+        wanted = [self.rec_id_attribute] + names + ([self.file_id_attribute] if self.file_id_attribute else [])
+        with (gzip.open(path, "rt", newline="") if str(path).endswith(".gz") else open(path, newline="")) as fh:
+            header = next(csv.reader(fh), [])
+        missing = [c for c in wanted if c not in header]
+        if missing:
+            raise ValueError(f"the query file {path} lacks the column(s) {', '.join(missing)}")
+        ids, files, cols, _ = read_csv_columns(path, self.rec_id_attribute, names, self.file_id_attribute, None,
+                                               self.null_value)
+        ids = [str(i) for i in ids.to_pylist()]
+        if not ids:
+            raise ValueError(f"the query file {path} has no records")
+        if len(set(ids)) != len(ids):
+            raise ValueError(f"the query file {path} has duplicate record ids")
+        fpos = {f: i for i, f in enumerate(cache.file_ids)}
+        file = []
+        for f in files.to_pylist():
+            if str(f) not in fpos:
+                raise ValueError(f"the query file {path} has the file id {f!r}, which the data does not have")
+            file.append(fpos[str(f)])
+        Q = len(ids)
+        x = np.full((Q, len(names)), -1, np.int32)
+        unseen = [[] for _ in range(Q)]
+        for a, (ix, col) in enumerate(zip(cache.indexes, cols)):
+            for q, v in enumerate(col.to_pylist()):
+                if v is None:
+                    continue
+                i = ix.value_idx_of(v)
+                if i < 0:
+                    unseen[q].append(names[a])
+                else:
+                    x[q, a] = i
+        return ids, x, np.asarray(file, np.int32), unseen
+
+    def _link_records(self, prm):
+        """query-links.csv and query-summary.csv under outputPath: the query records of prm['query_path'] linked to
+        the samples at or after the cutoff (project.link_queries)."""
+        d = self.load()
+        cache = d["cache"]
+        ids, x, file, unseen = self.read_queries(prm["query_path"])
+        t = prm["min_link_probability"]
+        ch = self.read_chain(prm["lower_iteration_cutoff"])
+        if not ch.samples:
+            raise ValueError("link-records needs at least one sample at or after lowerIterationCutoff")
+        names, values = [a.name for a in self.matching_attributes], self.attribute_values()
+        A, F, R = len(names), len(cache.file_ids), ch.num_records
+        theta = analysis_arrays.read_distortion_probabilities(self.chain_dirs(), ch, A, F)
+        M = int(self.population_size or len(d["rec_ids"]))
+        tables = analysis_arrays.QueryTables(x, file, [ix.tables() for ix in cache.indexes],
+                                             [a.is_constant for a in self.matching_attributes], F)
+
+        def samples():
+            for s, v in enumerate(analysis_arrays.read_entity_values(self.chain_dirs(), ch, names, values)):
+                mem, off, _ = ch.samples[s]
+                yield analysis_arrays.query_sample_arrays(R, mem, off, v) + (theta[s],)
+
+        res = link_queries(tables, samples, R, M, t)
+        chain_ids = ch.record_ids.to_pylist()
+        data_pos = {r: i for i, r in enumerate(str(r) for r in d["rec_ids"])}
+        position = np.array([data_pos[r] for r in chain_ids], np.int64)
+        q, r, p = analysis_arrays.query_link_rows(res, t, position)
+        writers.save_query_links([(ids[a], chain_ids[b], c) for a, b, c in zip(q.tolist(), r.tolist(), p.tolist())],
+                                 self.output_path)
+        first = {}
+        for i, a in enumerate(q.tolist()):
+            first.setdefault(a, i)  # rows go by probability descending, then data order: the first is the best
+        rows = []
+        for a in range(len(ids)):
+            best = first.get(a)
+            rows.append((ids[a], repr(float(res.new_entity_probability[a])),
+                         "" if best is None else chain_ids[r[best]], "" if best is None else repr(float(p[best])),
+                         repr(float(res.effective_samples[a])), ";".join(unseen[a])))
+        writers.save_query_summary(rows, self.output_path)
 
     def _summarize_entity_values(self, ch, prm):
         """entity-values-clusters.csv (the center, line k = cluster k) and entity-values.csv (every cluster's most

@@ -2,14 +2,15 @@
 import os
 import shutil
 
-from .writers import (DiagnosticsWriter, EntityValuesChainWriter, LinkageChainWriter, cluster_layout,
-                      entity_values_arrow, linkage_structure_arrow)
+from .writers import (DISTORTION_CHAIN, DiagnosticsWriter, DistortionChainWriter, EntityValuesChainWriter,
+                      LinkageChainWriter, cluster_layout, entity_values_arrow, linkage_structure_arrow)
 
 SUPPORTED_SAMPLERS = ("PCG-I", "PCG-II", "Gibbs", "Gibbs-Sequential")  # ProjectStep.scala:35
 
 
 def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin_interval=0, thinning_interval=1,
-           write_buffer_size=10, sampler="PCG-I", population_size=None, on_sample=None, entity_values=None):
+           write_buffer_size=10, sampler="PCG-I", population_size=None, on_sample=None, entity_values=None,
+           distortion_columns=None):
     """Generates `sample_size` posterior samples by successively applying the transition operator; writes
     linkage-chain.parquet and diagnostics.csv under output_path.  Returns the number of sweeps performed.
     on_sample(summary, parts) sees every recorded sample; parts = {partition id: pyarrow ListArray of clusters}
@@ -24,7 +25,12 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
     every recorded sample; y comes from download_state (one chain), download_chains (K > 1) or, on a sharded engine,
     its download_state of y, block and link (a collective; rank 0 writes).  Not given, a new (not continued) chain
     removes the entity-values-chain.parquet an earlier chain left in its directory: the linkage chain it described
-    is replaced."""
+    is replaced.
+
+    distortion_columns: None, or the column names of theta[A][F] attribute-major (writers.distortion_columns).  Given,
+    each chain directory also gets distortion-probabilities-chain.csv (writers.DistortionChainWriter), theta of every
+    recorded sample from the summary the step reads anyway; not given, a new chain removes such a file left by an
+    earlier chain, as for entity values."""
     if sample_size <= 0:
         raise ValueError("`sampleSize` must be positive.")            # Sampler.scala:61
     if burnin_interval < 0:
@@ -43,9 +49,9 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
     pop = population_size if population_size is not None else engine.num_entities
     K = getattr(engine, "num_chains", 1)
     dirs = [output_path] if K == 1 else [os.path.join(output_path, f"chain-{k}") for k in range(K)]
-    lw = dw = ew = ids = None
+    lw = dw = ew = tw = ids = None
     if writer:
-        lw, dw, ew = [], [], []
+        lw, dw, ew, tw = [], [], [], []
         for d in dirs:
             os.makedirs(d, exist_ok=True)
             lw.append(LinkageChainWriter(os.path.join(d, "linkage-chain.parquet"), write_buffer_size, continue_chain))
@@ -58,6 +64,11 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
                 # a new chain without entity values: the values of an earlier chain in this directory would describe
                 # other linkage rows under the same iterations and file names, so they go with that chain
                 shutil.rmtree(ev_path)
+            th_path = os.path.join(d, DISTORTION_CHAIN)
+            if distortion_columns is not None:
+                tw.append(DistortionChainWriter(th_path, distortion_columns, continue_chain))
+            elif not continue_chain and os.path.exists(th_path):
+                os.remove(th_path)  # the distortion probabilities of the replaced chain
 
         import pyarrow as pa
 
@@ -90,6 +101,8 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
             if entity_values is not None:
                 ew[k].append(s["iteration"], entity_values_arrow(link, blk, y[k], values, layout))
             dw[k].write_row(s, pop)
+            if distortion_columns is not None:
+                tw[k].write_row(s["iteration"], s["theta"])
             if on_sample:
                 on_sample(s, parts)
 
@@ -109,6 +122,6 @@ def sample(engine, record_ids, attribute_names, sample_size, output_path, burnin
         record()
         count += 1
     if writer:
-        for w in lw + ew + dw:
+        for w in lw + ew + dw + tw:
             w.close()
     return done

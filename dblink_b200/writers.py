@@ -12,6 +12,8 @@
   save_binder_search   binder-search.csv: every round of the Binder search from each start
   save_vi_loss   vi-loss.csv: every sample's number of clusters and posterior expected variation of information
   save_entity_values   entity-values.csv: every cluster's most probable value of each attribute and its probability
+  DistortionChainWriter   distortion-probabilities-chain.csv: every recorded sample's distortion probabilities
+  save_query_links / save_query_summary   query-links.csv / query-summary.csv: new records linked to the chain
 """
 import os
 import time
@@ -196,6 +198,58 @@ class EntityValuesChainWriter:
         self.buf = []
 
     close = flush
+
+
+DISTORTION_CHAIN = "distortion-probabilities-chain.csv"
+
+
+def distortion_columns(attribute_names, file_ids):
+    """The theta columns of distortion-probabilities-chain.csv, attribute-major: <attribute>[<file id>]."""
+    return [f"{a}[{f}]" for a in attribute_names for f in file_ids]
+
+
+class DistortionChainWriter:
+    """distortion-probabilities-chain.csv: header iteration,<attribute>[<file id>],... (distortion_columns), then one
+    row per recorded sample, theta[A][F] attribute-major and written with repr, CSV-quoted where a name needs it.  A
+    continued chain appends to the file (writing the header only when there is none)."""
+
+    def __init__(self, path, columns, append=False):
+        import csv
+
+        new = not (append and os.path.exists(path))
+        self.fh = open(path, "a" if not new else "w", newline="")
+        self.out = csv.writer(self.fh, lineterminator="\n")
+        if new:
+            self.out.writerow(["iteration"] + list(columns))
+
+    def write_row(self, iteration, theta):
+        self.out.writerow([str(int(iteration))] + [repr(float(v)) for v in np.asarray(theta, np.float64).ravel()])
+
+    def close(self):
+        self.fh.close()
+
+
+def save_distortion_probabilities(rows, path):
+    """distortion-probabilities.csv under `path`: per attribute and file the pooled samples' mean, sd, 2.5 %, 50 % and
+    97.5 % quantiles and their number S (analysis_arrays.distortion_summary), floats written with repr."""
+    _save_csv(path, "distortion-probabilities.csv",
+              ("attribute", "file", "mean", "sd", "q2.5", "q50", "q97.5", "samples"),
+              [[a, f] + [repr(float(v)) for v in vals] + [s] for a, f, vals, s in rows])
+
+
+QUERY_LINKS_HEADER = ("queryId", "recordId", "probability")
+QUERY_SUMMARY_HEADER = ("queryId", "newEntityProbability", "bestRecordId", "bestProbability", "effectiveSamples",
+                        "unseenAttributes")
+
+
+def save_query_links(rows, path):
+    """query-links.csv under `path`: (query id, record id, probability) rows as project.py orders them."""
+    _save_csv(path, "query-links.csv", QUERY_LINKS_HEADER, [(q, r, repr(float(p))) for q, r, p in rows])
+
+
+def save_query_summary(rows, path):
+    """query-summary.csv under `path`: one row per query in query-file order."""
+    _save_csv(path, "query-summary.csv", QUERY_SUMMARY_HEADER, rows)
 
 
 def read_linkage_chain(path, lower_iteration_cutoff=0):

@@ -594,6 +594,50 @@ double dbl_link_kernel_ms(dbl_ctx *, int64_t *launches);
 int64_t dbl_phase_ms(dbl_ctx *, double *out4);
 const char *dbl_version(void);
 
+/* ---------------------------------------------------------------------------------------------------
+ * New records linked to a finished chain (the posterior predictive of a query record's entity), on the device that
+ * is current when dbl_query_create() is called.  Q query records, A attributes, F files; per (query, attribute) the
+ * value id x (-1 = missing), psi(x), sigma(x) = sum_y psi(y) norm(y) expsim(x, y), and the hit row of x: the value ids
+ * y with expsim(x, y) != 1, ascending, with their expsim (hit_offsets: Q A + 1 int64 offsets); norm = every
+ * attribute's 1/n(y) table, attribute after attribute (num_values[a] entries each; ones for a constant attribute).
+ * All host arrays, copied at create.  With c0 = (1 - theta) / h, c1 = theta psi(x) / h, h = psi(x) ((1 - theta) + theta
+ * sigma(x)), theta = theta[a][file of the query], a sample's weight of query q against cluster k is
+ * w = m(q) rho(q, k), m(q) = prod over observed a of h, rho = prod over observed a of (c0 [x = y_ka] + c1 norm(y_ka)
+ * expsim(x, y_ka)), and Z(q) = m(q) (sum_k rho(q, k) + M - K).  Samples: labels[R] in [0, K) (host or device, every
+ * cluster holding a record), values[K][A] entity value ids (host or device) and theta[A][F] in [0, 1] (host).
+ *   dbl_query_add_sample    pass 1: appends log Z(q) and merges the keys (q, r) of every record r of every cluster k
+ *                           with w(q, k) >= t Z(q) into the held candidate set.  DBL_ERR_INVALID, changing nothing: a
+ *                           NULL pointer, K outside [1, min(R, M)], a label or value out of range, an empty cluster,
+ *                           theta outside [0, 1], or a set that would exceed max_candidates.  DBL_ERR_STATE once pass
+ *                           2 has begun.
+ *   dbl_query_score_sample  pass 2, the same samples in the same order: per held candidate adds
+ *                           exp(log w(q, c(r)) - L_q), L_q = the largest log Z(q) of pass 1.  DBL_ERR_INVALID: as
+ *                           above, more samples than pass 1, or K differing from pass 1's sample at this position.
+ *                           DBL_ERR_STATE before pass 1.
+ *   dbl_query_read          (host or device) the H candidates in (query, record) order, their sums; per query L_q,
+ *                           sum_s Z~, sum_s Z~^2 and sum_s (M - K_s) m_s(q) / exp(L_q), Z~ = Z / exp(L_q); log Z as
+ *                           [S][Q].  DBL_ERR_STATE unless pass 2 has scored every pass-1 sample.
+ * DBL_ERR_INVALID at create: num_records outside [1, 2^31 - 1], M < 1, Q < 1, A outside [1, 32], F < 1, a NULL
+ * pointer, a file or value id out of range, an unsorted hit row, t outside (0, 1], max_candidates outside
+ * [1, 2^31 - 1].  DBL_ERR_CUDA: no device, or an allocation that fails.
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct dbl_query dbl_query;
+int dbl_query_create(dbl_query **out, int64_t num_records, int64_t population_size, int32_t num_queries,
+                     int32_t num_attrs, int32_t num_files, const int32_t *num_values /* A */,
+                     const double *norm /* sum V_a */, const int32_t *file /* Q */, const int32_t *x /* Q A */,
+                     const double *psi /* Q A */, const double *sigma /* Q A */,
+                     const int64_t *hit_offsets /* Q A + 1 */, const int32_t *hit_values, const double *hit_expsim,
+                     double min_link_probability, int64_t max_candidates);
+void dbl_query_free(dbl_query *);
+int32_t dbl_query_num_samples(const dbl_query *);
+int dbl_query_add_sample(dbl_query *, const int32_t *labels /* R */, int32_t num_clusters,
+                         const int32_t *values /* K A */, const double *theta /* A F, host */);
+int dbl_query_score_sample(dbl_query *, const int32_t *labels /* R */, int32_t num_clusters,
+                           const int32_t *values /* K A */, const double *theta /* A F, host */);
+int dbl_query_num_candidates(const dbl_query *, int64_t *n_out);
+int dbl_query_read(dbl_query *, int32_t *query, int32_t *record, double *sum /* H each */, double *scale,
+                   double *zsum, double *zsq, double *fresh /* Q each */, double *logz /* S Q */);
+
 #ifdef __cplusplus
 }
 #endif
