@@ -171,6 +171,11 @@ SIGNATURES = {
     "dbl_query_score_sample": (C.c_int, [vp, vp, C.c_int32, vp, f64p]),
     "dbl_query_num_candidates": (C.c_int, [vp, i64p]),
     "dbl_query_read": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "dbl_capture_create": (C.c_int, [C.POINTER(vp), C.c_int64, vp, C.c_int32, C.c_int32]),
+    "dbl_capture_free": (None, [vp]),
+    "dbl_capture_add_sample": (C.c_int, [vp, vp]),
+    "dbl_capture_num_samples": (C.c_int32, [vp]),
+    "dbl_capture_read": (C.c_int, [vp, vp, vp]),
     "dbl_version": (C.c_char_p, []),
 }
 

@@ -13,6 +13,8 @@
                                                              links against an estimate, for a review queue
   entity_value_counts / entity_value_modes                <- the posterior of the entity values of an estimate's
                                                              clusters
+  capture_histories                                       <- the sets of files each sample's clusters hold, and each
+                                                             record's links into every file
   cluster_size_distribution / partition_sizes             <- LinkageChain.scala:118-154
   pairwise_metrics                                        <- analysis/PairwiseMetrics.scala:44-63,
                                                              BinaryClassificationMetrics.scala:23-37
@@ -650,6 +652,44 @@ def entity_value_modes(counts, num_clusters, num_attributes):
             out[(k, a)] = (v, n)
     assert len(out) == num_clusters * num_attributes
     return out
+
+
+def capture_histories(chain, file, num_files):
+    """The capture histories restated with sets and Python integers: chain = [(iteration, {partition: [cluster of
+    ids]})], file = {record id: its file in [0, num_files)}.  Returns (H, L): H[s][h] = the clusters of sample s whose
+    set of files, as the bits of h, is exactly h (H[s][0] = 0), and L = {record id: [the samples in which its cluster
+    holds a record of file g other than itself, for g in files]}."""
+    H, L = [], {r: [0] * num_files for r in file}
+    for sample in chain:
+        row = [0] * (1 << num_files)
+        for c in clusters_of_sample(sample):
+            files = {file[r] for r in c}
+            row[sum(1 << f for f in files)] += 1
+            for r in c:
+                for g in {file[o] for o in c if o != r}:
+                    L[r][g] += 1
+        H.append(row)
+    return H, L
+
+
+def format_capture_histories(res, file_ids):
+    """The capture-histories section: res = analysis_arrays.capture_evaluation's summary."""
+    def interval(x):
+        mean, _, lo, _, hi, inf = x
+        return f"posterior mean {mean!r}, 95% interval [{lo!r}, {hi!r}]" + (f", infinite in {inf} samples" if inf
+                                                                              else "")
+
+    lines = (f" Samples:         {res['samples']}\n"
+             f" Histories:       {res['histories_inside']} of {res['histories']} with the truth inside the 95% "
+             f"interval\n"
+             f" Quantities:      {res['quantities_inside']} of {res['quantities']} with the truth inside the 95% "
+             f"interval\n"
+             f" Observed:        truth {res['observed'][0]}, {interval(res['observed'][1])}\n")
+    if "independence" in res:
+        lines += f" Independence:    truth {res['independence'][0]!r}, {interval(res['independence'][1])}\n"
+    lines += "".join(f" Brier [{f}]:{' ' * max(1, 8 - len(str(f)))}{b!r}\n" for f, b in zip(file_ids, res["brier"]))
+    return ("=====================================\n         Capture histories\n"
+            "-------------------------------------\n" + lines + "=====================================\n")
 
 
 def format_clerical_review(res):

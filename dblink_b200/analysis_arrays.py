@@ -1938,3 +1938,194 @@ def distortion_summary(theta):
     q = np.quantile(flat, [0.025, 0.5, 0.975], axis=0)
     return [(float(flat[:, j].mean()), float(flat[:, j].std()), float(q[0, j]), float(q[1, j]), float(q[2, j]), S)
             for j in range(flat.shape[1])]
+
+
+# ---- capture histories: how the files overlap ---------------------------------------------------------------------
+# Files are numbered f = 0 .. F-1 (RecordsCache.file_ids order).  Per sample s and cluster c the history is
+# h(c) = OR over records r of c of (1 << file[r]), a non-empty subset of the files:
+#   H[s][h]  the clusters of sample s whose history is h (H[s][0] = 0), and
+#   L[r][g]  the samples in which r's cluster holds a record of file g other than r itself,
+# so L / S is the probability that r has a counterpart in file g (a duplicate in its own file when g = file[r]).  Every
+# number written is computed from H and L by CaptureSummary, whichever path counted them.
+MAX_CAPTURE_FILES = 12  # 2^12 histories: the GPU's shared-memory histogram
+
+
+def check_capture_files(num_files):
+    """ValueError unless 1 <= F <= MAX_CAPTURE_FILES."""
+    if not 1 <= int(num_files) <= MAX_CAPTURE_FILES:
+        raise ValueError(f"capture-histories supports 1 to {MAX_CAPTURE_FILES} files (2^F histories); the data has "
+                         f"{int(num_files)}")
+
+
+class CaptureCounts:
+    """The numpy counter with analysis_gpu.Capture's interface: add_sample(cluster[R]) per sample, read() gives
+    (H int64[S, 2^F], L int64[R, F])."""
+
+    def __init__(self, file, num_files):
+        check_capture_files(num_files)
+        self.file = np.asarray(file, np.int64)
+        self.F = int(num_files)
+        if len(self.file) and (self.file.min() < 0 or self.file.max() >= self.F):
+            raise ValueError("a file number is outside [0, F)")
+        self.H = []
+        self.L = np.zeros((len(self.file), self.F), np.int64)
+
+    def add_sample(self, cluster):
+        R, F, file = len(self.file), self.F, self.file
+        lab = np.asarray(cluster, np.int64)
+        if lab.shape != (R,) or (R and (lab.min() < 0 or lab.max() >= R)):
+            raise ValueError("a sample needs one cluster label in [0, R) per record")
+        bit = np.left_shift(1, file)
+        hist = np.zeros(R, np.int64)
+        np.bitwise_or.at(hist, lab, bit)
+        twice = np.bincount(lab * F + file, minlength=R * F).reshape(R, F) >= 2
+        dup = (twice << np.arange(F)).sum(axis=1)
+        self.H.append(np.bincount(hist[hist > 0], minlength=1 << F))
+        links = (hist[lab] & ~bit) | (dup[lab] & bit)
+        self.L += (links[:, None] >> np.arange(F)) & 1
+
+    @property
+    def num_samples(self):
+        return len(self.H)
+
+    def read(self):
+        return np.asarray(self.H, np.int64).reshape(-1, 1 << self.F), self.L.copy()
+
+
+def capture_histories(chain, file, num_files, counter=CaptureCounts):
+    """(H int64[S, 2^F], L int64[R, F]) of a ChainArrays whose record i is in file[i]; counter = CaptureCounts or
+    analysis_gpu.Capture."""
+    R = chain.num_records
+    if not chain.samples:
+        raise ValueError("capture-histories needs at least one sample at or after lowerIterationCutoff")
+    cc = counter(file, num_files)
+    try:
+        for mem, off, _ in chain.samples:
+            lab = np.empty(R, np.int32)
+            lab[mem] = np.repeat(np.arange(len(off) - 1, dtype=np.int32), np.diff(off))
+            cc.add_sample(lab)
+        return cc.read()
+    finally:
+        if hasattr(cc, "close"):
+            cc.close()
+
+
+def independence_estimate(n, D):
+    """Darroch's (1958) Mt estimate of the population size per row: n int64[S, F] entities per file, D int64[S]
+    observed entities.  It maximises the conditional likelihood of the independence model with the capture
+    probabilities profiled out, l(N) = (1 - F) N log N - (N - D) log(N - D) + sum_f (N - n_f) log(N - n_f), whose
+    derivative is g(N) = sum_f log1p(-n_f / N) - log1p(-D / N): the root of g on N > D, found by bisection on x = D / N
+    in (0, 1) to the last bit.  +inf when sum_f n_f = D (no file overlaps another); D when a file holds every observed
+    entity (g < 0 on N > D, so l falls from N = D)."""
+    n = np.asarray(n, np.float64)
+    D = np.asarray(D, np.float64)
+    S = len(D)
+    out = np.full(S, np.inf)
+    total = n.sum(axis=1)
+    finite = total > D
+    whole = finite & (n.max(axis=1, initial=0.0) >= D)
+    out[whole] = D[whole]
+    todo = np.flatnonzero(finite & ~whole)
+    a = n[todo] / D[todo, None]
+    lo, hi = np.zeros(len(todo)), np.ones(len(todo))
+    for _ in range(2000):
+        mid = 0.5 * (lo + hi)
+        live = (mid > lo) & (mid < hi)
+        if not live.any():
+            break
+        g = np.log1p(-mid[:, None] * a).sum(axis=1) - np.log1p(-mid)
+        up = live & (g > 0)
+        hi = np.where(up, mid, hi)
+        lo = np.where(live & ~up, mid, lo)
+    out[todo] = D[todo] / (0.5 * (lo + hi))
+    return out
+
+
+def _moments(v):
+    """(mean, sd with ddof 0, 2.5 %, 50 %, 97.5 % quantiles -- numpy's default method, as distortion_summary) over the
+    finite values of v, NaN when there is none, and the number of infinite ones."""
+    v = np.asarray(v, np.float64)
+    f = v[np.isfinite(v)]
+    if not len(f):
+        return (float("nan"),) * 5 + (len(v),)
+    q = np.quantile(f, [0.025, 0.5, 0.975])
+    return (float(f.mean()), float(f.std()), float(q[0]), float(q[1]), float(q[2]), int(len(v) - len(f)))
+
+
+class CaptureSummary:
+    """Every number the capture-histories files hold, from H[S, 2^F], L[R, F] and the records of each file:
+    per sample the quantities (quantity names and int64 or float64 columns, in population-size.csv's order) and their
+    summaries, the history summaries and the record link probabilities L / S."""
+
+    def __init__(self, H, L, records_per_file):
+        H = np.asarray(H, np.int64)
+        self.H, self.L = H, np.asarray(L, np.int64)
+        self.S, cells = H.shape
+        self.F = F = cells.bit_length() - 1
+        self.records_per_file = np.asarray(records_per_file, np.int64)
+        hs = np.arange(cells)
+        member = ((hs[:, None] >> np.arange(F)) & 1).astype(np.int64)  # [2^F, F]
+        self.histories = member[1:]
+        D = H.sum(axis=1)
+        n = H @ member
+        names, cols = ["observed-entities"], [D]
+        names += [f"entities[{f}]" for f in range(F)]
+        cols += [n[:, f] for f in range(F)]
+        names += [f"duplicates[{f}]" for f in range(F)]
+        cols += [self.records_per_file[f] - n[:, f] for f in range(F)]
+        pairs = [(f, g) for f in range(F) for g in range(f + 1, F)]
+        m = {(f, g): H @ (member[:, f] & member[:, g]) for f, g in pairs}
+        names += [f"overlap[{f},{g}]" for f, g in pairs]
+        cols += [m[p] for p in pairs]
+        names += [f"chapman[{f},{g}]" for f, g in pairs]
+        cols += [(n[:, f] + 1.0) * (n[:, g] + 1.0) / (m[(f, g)] + 1.0) - 1.0 for f, g in pairs]
+        if F >= 2:
+            names.append("independence")
+            cols.append(independence_estimate(n, D))
+        self.names, self.columns = names, cols
+
+    def quantity_names(self, file_ids):
+        """The quantity names with file numbers replaced by file ids."""
+        out = []
+        for name in self.names:
+            if "[" in name:
+                head, idx = name[:-1].split("[")
+                out.append(head + "[" + ",".join(str(file_ids[int(i)]) for i in idx.split(",")) + "]")
+            else:
+                out.append(name)
+        return out
+
+    def quantity_summary(self):
+        """Per quantity (mean, sd, q2.5, q50, q97.5, infinite)."""
+        return [_moments(c) for c in self.columns]
+
+    def history_summary(self):
+        """Per history h = 1 .. 2^F - 1 (mean, sd, q2.5, q50, q97.5) of its cluster count, zeros included."""
+        return [_moments(self.H[:, h])[:5] for h in range(1, self.H.shape[1])]
+
+    def link_probabilities(self):
+        """float64[R, F]: L / S."""
+        return self.L / self.S
+
+
+def capture_evaluation(post, truth):
+    """The posterior against the ground truth (both CaptureSummary; truth of one sample): (rows of
+    capture-histories-evaluation.csv -- per history, then per quantity: index, truth, posterior mean, 2.5 % and
+    97.5 % quantiles, truth inside the interval -- and a summary dict: histories and quantities with the truth inside,
+    the truth's observed entities and independence estimate with their posterior summaries, and the Brier score of
+    L / S against the truth's 0/1 links per file)."""
+    rows_h, rows_q = [], []
+    for h, (mean, _, lo, _, hi) in enumerate(post.history_summary(), start=1):
+        t = int(truth.H[0, h])
+        rows_h.append((h, t, mean, lo, hi, bool(lo <= t <= hi)))
+    for j, (col, (mean, _, lo, _, hi, _)) in enumerate(zip(truth.columns, post.quantity_summary())):
+        t = col[0].item()
+        rows_q.append((j, t, mean, lo, hi, bool(lo <= t <= hi)))
+    brier = ((post.link_probabilities() - truth.L) ** 2).mean(axis=0) if len(post.L) else np.full(post.F, np.nan)
+    summary = dict(samples=post.S, histories=len(rows_h), histories_inside=sum(r[5] for r in rows_h),
+                   quantities=len(rows_q), quantities_inside=sum(r[5] for r in rows_q),
+                   observed=(rows_q[0][1], post.quantity_summary()[0]), brier=[float(b) for b in brier])
+    if "independence" in post.names:
+        j = post.names.index("independence")
+        summary["independence"] = (float(truth.columns[j][0]), post.quantity_summary()[j])
+    return rows_h, rows_q, summary

@@ -21,7 +21,9 @@ counts per attribute and merges each sample's run-length-encoded keys into it; t
 The per-pair split-R̂ and ESS equal analysis_arrays.pairwise_match_diagnostics bit for bit: a bit trace per held pair,
 then integer lag statistics and the same rounded double operations per pair on the device.  The links of every record
 against a point estimate and the appearances of its clusters, for clerical review, equal analysis_arrays.record_links
-and cluster_appearances exactly: integer atomics over the held pair table, and the sMPC's signatures compared.
+and cluster_appearances exactly: integer atomics over the held pair table, and the sMPC's signatures compared.  The
+capture histories and record links equal analysis_arrays.capture_histories exactly: integer atomics on per-cluster
+file words, then a shared-memory histogram of the words.
 """
 import ctypes as C
 
@@ -537,3 +539,40 @@ class Query(_Handle):
 def link_queries(tables, samples, num_records, population_size, min_link_probability):
     """analysis_arrays.link_queries on the device."""
     return analysis_arrays.link_queries(tables, samples, num_records, population_size, min_link_probability, Query)
+
+
+class Capture(_Handle):
+    """Owner of a dbl_capture handle: the records' files go in once, samples one at a time, read() gives (H int64[S,
+    2^F], L int64[R, F]) as analysis_arrays.CaptureCounts.read.  file may be a numpy array or a device pointer (int)
+    with num_records given."""
+
+    _prefix = "dbl_capture"
+
+    def __init__(self, file, num_files, max_samples=1 << 16, num_records=None):
+        if isinstance(file, int):
+            ptr, R = file, int(num_records)
+        else:
+            file = np.ascontiguousarray(file, np.int32)
+            ptr, R = file.ctypes.data, len(file)
+        self.F = int(num_files)
+        super().__init__(R, ptr, self.F, int(max_samples))
+
+    def add_sample(self, cluster):
+        if isinstance(cluster, int):  # a device pointer
+            self._call("add_sample", self._h, cluster)
+        else:
+            super().add_sample(cluster)
+
+    def read(self, record_links=True):
+        H = np.empty((self.num_samples, 1 << self.F), np.int64)
+        L = np.empty((self.num_records, self.F), np.int32) if record_links else None
+        self._call("read", self._h, H.ctypes.data, None if L is None else L.ctypes.data)
+        return H, None if L is None else L.astype(np.int64)
+
+
+def capture_histories(chain, file, num_files):
+    """(H, L), identical to analysis_arrays.capture_histories(chain, file, num_files): every sample goes into one
+    handle."""
+    analysis_arrays.check_capture_files(num_files)
+    return analysis_arrays.capture_histories(
+        chain, file, num_files, lambda f, F: Capture(f, F, max(len(chain.samples), 1)))

@@ -44,6 +44,12 @@
 // count, by one pass over the held pair table (dbl_pairs_record_links); per record the samples holding its cluster of
 // the estimate, by comparing its row of the sMPC signature matrix with the estimate's own signatures
 // (dbl_posterior_cluster_counts).
+//
+// Capture histories (dbl_capture_*, same integers as analysis_arrays.capture_histories): per sample the number of
+// clusters holding records of exactly each set of files, and per record the samples in which its cluster holds another
+// record of each file.  Per sample, every record ORs its file bit into its cluster's history word (and, when the bit
+// was already set, into its duplicate word), then one pass over the labels histograms the history words -- see
+// dbl_capture_add_sample.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -3175,6 +3181,139 @@ extern "C" int dbl_query_read(dbl_query *p, int32_t *query, int32_t *record, dou
   POST_TRY(cudaMemcpyAsync(zsq, b.p, sizeof(double) * Q, cudaMemcpyDefault, st));
   POST_TRY(cudaMemcpyAsync(fresh, c.p, sizeof(double) * Q, cudaMemcpyDefault, st));
   POST_TRY(cudaMemcpyAsync(logz, p->logz.p, sizeof(double) * Q * S, cudaMemcpyDefault, st));
+  POST_TRY(cudaStreamSynchronize(st));
+  return DBL_OK;
+}
+
+// ---- capture histories: which files each cluster of each sample holds ----------------------------------------------
+namespace {
+constexpr int CAPTURE_MAX_FILES = 12;  // 2^12 int32 histogram cells: 16 KB of shared memory per block
+
+// One pass over the records: hist[c] |= the file bit of every record of cluster c, and dup[c] gets the bits of the
+// files with two or more records in c.  A record whose atomicOr finds its bit already set is not its file's first in c;
+// only the first record of a file in c sees the bit clear, so the words are exact in any order.  The lanes of a warp
+// sharing a label OR their bits together first (and mark the files two of them share), so one update per label and
+// warp reaches memory: a cluster of thousands of records does not serialise on one word.
+__global__ void k_capture_or(int64_t R, const int32_t *__restrict__ cluster, const int32_t *__restrict__ file,
+                             unsigned *__restrict__ hist, unsigned *__restrict__ dup) {
+  const int lane = threadIdx.x & 31;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31); base < R; base += stride) {
+    const int64_t r = base + lane;
+    const unsigned live = __ballot_sync(0xffffffffu, r < R);
+    if (r >= R) continue;
+    const int32_t c = cluster[r];
+    const unsigned bit = 1u << file[r];
+    const unsigned peers = __match_any_sync(live, (unsigned long long)(uint32_t)c);
+    const unsigned same_file = __match_any_sync(live, (unsigned long long)(uint32_t)c << 32 | bit);
+    const unsigned word = __reduce_or_sync(peers, bit);
+    const unsigned twice = __reduce_or_sync(peers, __popc(same_file) > 1 ? bit : 0u);
+    if (lane == __ffs(peers) - 1) {
+      const unsigned old = atomicOr(&hist[c], word);
+      const unsigned d = (old & word) | twice;
+      if (d) atomicOr(&dup[c], d);
+    }
+  }
+}
+
+// One pass over [0, R): label i's history word, when non-zero, counts into a shared-memory histogram of the 2^F words,
+// flushed into row Hrow with 64-bit atomics; record i adds its cluster's bits to its own row of L -- the other files'
+// bits of the history and its own file's bit of the duplicate word (a thread owns its record's row: no atomics).
+__global__ void k_capture_count(int64_t R, int32_t F, const int32_t *__restrict__ cluster,
+                                const int32_t *__restrict__ file, const unsigned *__restrict__ hist,
+                                const unsigned *__restrict__ dup, unsigned long long *__restrict__ Hrow,
+                                int32_t *__restrict__ L) {
+  extern __shared__ int32_t cells[];
+  const int ncell = 1 << F;
+  for (int j = threadIdx.x; j < ncell; j += blockDim.x) cells[j] = 0;
+  __syncthreads();
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned w = hist[i];
+    if (w) atomicAdd(&cells[w], 1);
+    const int32_t c = cluster[i];
+    const unsigned own = 1u << file[i];
+    unsigned bits = (hist[c] & ~own) | (dup[c] & own);
+    int32_t *row = L + i * F;
+    while (bits) {
+      const int g = __ffs(bits) - 1;
+      bits &= bits - 1;
+      row[g] += 1;
+    }
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < ncell; j += blockDim.x)
+    if (cells[j]) atomicAdd(&Hrow[j], (unsigned long long)cells[j]);
+}
+}  // namespace
+
+struct dbl_capture : Handle {
+  int32_t F = 1, max_samples = 0;
+  Buf file;       // R file numbers in [0, F)
+  Buf hist, dup;  // R history words and R duplicate words of the sample being added
+  Buf H;          // [max_samples][2^F] int64 cluster counts per history
+  Buf L;          // [R][F] int32 record links
+};
+
+extern "C" int dbl_capture_create(dbl_capture **out, int64_t num_records, const int32_t *file, int32_t num_files,
+                                  int32_t max_samples) {
+  if (!out) return DBL_ERR_INVALID;
+  *out = nullptr;
+  if (num_records <= 0 || num_records > INT32_MAX || !file || num_files < 1 || num_files > CAPTURE_MAX_FILES ||
+      max_samples < 1)
+    return DBL_ERR_INVALID;
+  return open_handle(out, num_records, [&](dbl_capture *p) {
+    const size_t R = (size_t)num_records, cells = (size_t)1 << num_files;
+    p->F = num_files;
+    p->max_samples = max_samples;
+    if (p->file.alloc(sizeof(int32_t) * R) != cudaSuccess || p->hist.alloc(sizeof(unsigned) * R) != cudaSuccess ||
+        p->dup.alloc(sizeof(unsigned) * R) != cudaSuccess ||
+        p->H.alloc(sizeof(unsigned long long) * cells * (size_t)max_samples) != cudaSuccess ||
+        p->L.alloc(sizeof(int32_t) * R * (size_t)num_files) != cudaSuccess)
+      return DBL_ERR_CUDA;
+    if (const int rc = p->take_labels(file, p->file, num_files); rc != DBL_OK) return rc;
+    POST_TRY(cudaMemsetAsync(p->H.p, 0, sizeof(unsigned long long) * cells * (size_t)max_samples, p->stream));
+    POST_TRY(cudaMemsetAsync(p->L.p, 0, sizeof(int32_t) * R * (size_t)num_files, p->stream));
+    POST_TRY(cudaStreamSynchronize(p->stream));
+    return DBL_OK;
+  });
+}
+
+extern "C" void dbl_capture_free(dbl_capture *p) { free_handle(p); }
+
+extern "C" int32_t dbl_capture_num_samples(const dbl_capture *p) { return p ? p->S : 0; }
+
+// One sample: check the labels; clear the words; OR every record's file bit into its cluster's words; count the
+// history words into row S of H and every record's links into L.  S, H and L move only when the labels pass.
+extern "C" int dbl_capture_add_sample(dbl_capture *p, const int32_t *cluster) {
+  if (!p || !cluster || p->S >= p->max_samples) return DBL_ERR_INVALID;
+  DeviceScope ds(p->device);
+  if (const int rc = p->take_labels(cluster, p->cluster); rc != DBL_OK) return rc;
+  const int64_t R = p->R;
+  cudaStream_t st = p->stream;
+  const int32_t *c = p->cluster.as<int32_t>(), *f = p->file.as<int32_t>();
+  POST_TRY(cudaMemsetAsync(p->hist.p, 0, sizeof(unsigned) * R, st));
+  POST_TRY(cudaMemsetAsync(p->dup.p, 0, sizeof(unsigned) * R, st));
+  k_capture_or<<<grid_for(R), THREADS, 0, st>>>(R, c, f, p->hist.as<unsigned>(), p->dup.as<unsigned>());
+  const size_t cells = (size_t)1 << p->F;
+  k_capture_count<<<grid_for(R), THREADS, sizeof(int32_t) * cells, st>>>(
+      R, p->F, c, f, p->hist.as<unsigned>(), p->dup.as<unsigned>(), p->H.as<unsigned long long>() + cells * p->S,
+      p->L.as<int32_t>());
+  POST_TRY(cudaGetLastError());
+  POST_TRY(cudaStreamSynchronize(st));
+  ++p->S;
+  return DBL_OK;
+}
+
+extern "C" int dbl_capture_read(dbl_capture *p, int64_t *histories, int32_t *record_links) {
+  if (!p || !histories) return DBL_ERR_INVALID;
+  if (p->S == 0) return DBL_ERR_STATE;
+  DeviceScope ds(p->device);
+  cudaStream_t st = p->stream;
+  POST_TRY(cudaMemcpyAsync(histories, p->H.p, sizeof(int64_t) * ((size_t)1 << p->F) * (size_t)p->S,
+                           cudaMemcpyDeviceToHost, st));
+  if (record_links)  // host or device: unified addressing picks the copy direction
+    POST_TRY(cudaMemcpyAsync(record_links, p->L.p, sizeof(int32_t) * (size_t)p->R * (size_t)p->F, cudaMemcpyDefault,
+                             st));
   POST_TRY(cudaStreamSynchronize(st));
   return DBL_OK;
 }

@@ -30,12 +30,15 @@ VI_SEARCH_METRICS = ("vi-search-pairwise", "vi-search-cluster")
 CREDIBLE_BALL_METRICS = ("credible-ball",)
 # how well the clerical review queue of a point estimate finds its clusters that are not exactly a true entity
 CLERICAL_REVIEW_METRICS = ("clerical-review",)
+# the posterior capture histories, population sizes and file links against those of the ground truth
+CAPTURE_HISTORY_METRICS = ("capture-histories",)
 SUPPORTED_METRICS = (SMPC_METRICS + POSTERIOR_METRICS + BINDER_METRICS + BINDER_SEARCH_METRICS + VI_METRICS
-                     + VI_SEARCH_METRICS + CREDIBLE_BALL_METRICS + CLERICAL_REVIEW_METRICS)
+                     + VI_SEARCH_METRICS + CREDIBLE_BALL_METRICS + CLERICAL_REVIEW_METRICS + CAPTURE_HISTORY_METRICS)
 SUPPORTED_QUANTITIES = ("cluster-size-distribution", "partition-sizes", "shared-most-probable-clusters",  # :37
                         "pairwise-match-probabilities", "convergence-diagnostics", "binder-clusters",
                         "binder-search-clusters", "vi-clusters", "vi-search-clusters", "credible-ball",
-                        "entity-values", "pairwise-match-diagnostics", "clerical-review", "distortion-probabilities")
+                        "entity-values", "pairwise-match-diagnostics", "clerical-review", "distortion-probabilities",
+                        "capture-histories")
 # the point estimates a credible ball may be centred on
 CREDIBLE_BALL_CENTERS = ("shared-most-probable-clusters", "binder-clusters", "binder-search-clusters", "vi-clusters",
                          "vi-search-clusters")
@@ -343,6 +346,15 @@ def _save_distortion_probabilities(prm):
     return {"save_distortion_probabilities": True} if save else {}
 
 
+def capture_histories(chain, file, num_files):
+    """(H, L) of a ChainArrays whose record i is in file[i], the clusters of each sample per set of files and each
+    record's links into every file: on the GPU when the platform has one (analysis_gpu), else on the host
+    (analysis_arrays).  Both give identical arrays."""
+    if _lib.load().dbl_device_count() > 0:
+        return analysis_gpu.capture_histories(chain, file, num_files)
+    return analysis_arrays.capture_histories(chain, file, num_files)
+
+
 def link_queries(tables, samples, num_records, population_size, min_link_probability):
     """analysis_arrays.QueryResult of the query records against the samples: on the GPU when the platform has one
     (analysis_gpu), else on the host (analysis_arrays).  Both give the same candidates and sums within rounding."""
@@ -501,6 +513,10 @@ class Project:
                 if "clerical-review" in prm["quantities"]:
                     L.append(f"  * SummarizeStep: clerical-review ranks the clusters of a point estimate by their "
                              f"expected false and missed links, with {_clerical_review_settings(prm)}")
+                if "capture-histories" in prm["quantities"]:
+                    L.append("  * SummarizeStep: capture-histories counts every sample's clusters by the set of files "
+                             "they hold, every record's links into each file, and population-size estimates from "
+                             "those counts; their spread reflects linkage uncertainty only")
             elif name == "evaluate":
                 smpc = [m for m in prm["metrics"] if m in SMPC_METRICS]
                 post = [m for m in prm["metrics"] if m in POSTERIOR_METRICS]
@@ -544,6 +560,11 @@ class Project:
                     L.append(f"  * EvaluateStep: Evaluating how soon the clerical review queue of a point estimate "
                              f"reaches its clusters that are not a true entity ({_clerical_review_settings(prm)}, "
                              f"iterations >= {prm['lower_iteration_cutoff']}) using {braces(review)} metrics")
+                capture = [m for m in prm["metrics"] if m in CAPTURE_HISTORY_METRICS]
+                if capture:
+                    L.append(f"  * EvaluateStep: Evaluating the capture histories, population sizes and file links of "
+                             f"every sample against those of the ground truth (iterations >= "
+                             f"{prm['lower_iteration_cutoff']}) using {braces(capture)} metrics")
             elif name == "link-records":
                 L.append(f"  * LinkRecordsStep: Linking the records of '{prm['query_path']}' to the chain for "
                          f"iterations >= {prm['lower_iteration_cutoff']}, reporting the records they share an entity "
@@ -682,6 +703,8 @@ class Project:
                 q = list(prm["quantities"])
                 if not q or any(x not in SUPPORTED_QUANTITIES for x in q):
                     raise ValueError(f"quantities must be one of {SUPPORTED_QUANTITIES}.")
+                if "capture-histories" in q:
+                    analysis_arrays.check_capture_files(len(self.load()["cache"].file_ids))
                 if "convergence-diagnostics" in q and self.num_chains < 2:
                     raise ValueError("convergence-diagnostics needs numChains >= 2.")
                 # minMatchProbability: pairwise-match-probabilities.csv keeps the pairs at least this probable
@@ -699,6 +722,8 @@ class Project:
                 m = list(prm["metrics"])
                 if not m or any(x not in SUPPORTED_METRICS for x in m):
                     raise ValueError(f"metrics must be one of {SUPPORTED_METRICS}.")
+                if any(x in CAPTURE_HISTORY_METRICS for x in m):
+                    analysis_arrays.check_capture_files(len(self.load()["cache"].file_ids))
                 out.append(("evaluate", dict(lower_iteration_cutoff=int(prm.get("lowerIterationCutoff", 0)), metrics=m,
                                              use_existing_smpc=bool(prm.get("useExistingSMPC", False)),
                                              false_link_cost=_false_link_cost(prm),
@@ -812,6 +837,8 @@ class Project:
                         writers.save_distortion_probabilities(
                             [(a, f, vals[:5], vals[5]) for (a, f), vals in
                              zip(cols, analysis_arrays.distortion_summary(theta))], self.output_path)
+                    elif q == "capture-histories":
+                        self._summarize_capture_histories(ch)
                     elif q == "clerical-review":
                         review = clerical_review_estimate(ch, prm["clerical_review_center"], prm["false_link_cost"],
                                                           prm["max_search_rounds"])
@@ -929,6 +956,10 @@ class Project:
                     res["center"] = center
                     results["clerical-review"] = res
                     text.append(analysis.format_clerical_review(res))
+                if any(m in CAPTURE_HISTORY_METRICS for m in prm["metrics"]):
+                    ch = ch if ch is not None else self.read_chain(cut)
+                    results["capture-histories"] = res = self._evaluate_capture_histories(ch, true_labels)
+                    text.append(analysis.format_capture_histories(res, self.load()["cache"].file_ids))
                 with open(os.path.join(self.output_path, "evaluation-results.txt"), "w") as fh:
                     fh.write("\n".join(text) + "\n")
             elif name == "link-records":
@@ -1030,8 +1061,7 @@ class Project:
 
         res = link_queries(tables, samples, R, M, t)
         chain_ids = ch.record_ids.to_pylist()
-        data_pos = {r: i for i, r in enumerate(str(r) for r in d["rec_ids"])}
-        position = np.array([data_pos[r] for r in chain_ids], np.int64)
+        position = self._data_positions(ch)
         q, r, p = analysis_arrays.query_link_rows(res, t, position)
         writers.save_query_links([(ids[a], chain_ids[b], c) for a, b, c in zip(q.tolist(), r.tolist(), p.tolist())],
                                  self.output_path)
@@ -1045,6 +1075,53 @@ class Project:
                          "" if best is None else chain_ids[r[best]], "" if best is None else repr(float(p[best])),
                          repr(float(res.effective_samples[a])), ";".join(unseen[a])))
         writers.save_query_summary(rows, self.output_path)
+
+    def _data_positions(self, ch):
+        """int64[R]: the data row of each record of the chain."""
+        data_pos = {r: i for i, r in enumerate(str(r) for r in self.load()["rec_ids"])}
+        return np.array([data_pos[r] for r in ch.record_ids.to_pylist()], np.int64)
+
+    def _capture_summary(self, ch, labels=None):
+        """(CaptureSummary, data rows of the chain's records, their files) of the samples of ch, or of the one
+        labelling labels[R] (chain record order) when given."""
+        if not ch.samples:
+            raise ValueError("capture-histories needs at least one sample at or after lowerIterationCutoff")
+        d = self.load()
+        F = len(d["cache"].file_ids)
+        position = self._data_positions(ch)
+        file = np.asarray(d["file"], np.int64)[position]
+        if labels is None:
+            H, L = capture_histories(ch, file, F)
+        else:
+            cc = analysis_arrays.CaptureCounts(file, F)
+            cc.add_sample(analysis_arrays.canonical_clusters(labels))
+            H, L = cc.read()
+        return analysis_arrays.CaptureSummary(H, L, np.bincount(file, minlength=F)), position, file
+
+    def _summarize_capture_histories(self, ch):
+        """capture-histories-samples.csv, capture-histories.csv, population-size.csv, population-size-samples.csv and
+        file-links.csv (records in data order) under outputPath."""
+        summary, position, file = self._capture_summary(ch)
+        file_ids = self.load()["cache"].file_ids
+        writers.save_capture_histories(summary, ch.chains, ch.iterations, file_ids, self.output_path)
+        order = np.argsort(position, kind="stable")
+        ids = ch.record_ids.to_pylist()
+        writers.save_file_links([ids[i] for i in order], [file_ids[f] for f in file[order]],
+                                summary.link_probabilities()[order], file_ids, self.output_path)
+
+    def _evaluate_capture_histories(self, ch, true_labels):
+        """capture-histories-evaluation.csv under outputPath and the summary of analysis_arrays.capture_evaluation:
+        the samples of ch against the ground truth, whose H and L are counted by the same code as one sample."""
+        post, _, _ = self._capture_summary(ch)
+        truth, _, _ = self._capture_summary(ch, true_labels(ch.record_ids))
+        file_ids = [str(f) for f in self.load()["cache"].file_ids]
+        rows_h, rows_q, res = analysis_arrays.capture_evaluation(post, truth)
+        names = post.quantity_names(file_ids)
+        rows = [("history[" + ",".join(f for f, b in zip(file_ids, post.histories[r[0] - 1]) if b) + "]", *r[1:])
+                for r in rows_h]
+        rows += [(names[r[0]], *r[1:]) for r in rows_q]
+        writers.save_capture_histories_evaluation(rows, self.output_path)
+        return res
 
     def _summarize_entity_values(self, ch, prm):
         """entity-values-clusters.csv (the center, line k = cluster k) and entity-values.csv (every cluster's most

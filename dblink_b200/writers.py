@@ -525,3 +525,49 @@ def save_clerical_review_evaluation(rows, path):
     """clerical-review-evaluation.csv under `path`: per position of the review queue its cluster, whether it is not
     exactly a true entity (1) and the erroneous clusters found up to it."""
     _save_csv(path, "clerical-review-evaluation.csv", CLERICAL_REVIEW_EVALUATION_HEADER, rows)
+
+
+def _number(x):
+    """An integer as itself, a float with repr."""
+    return repr(float(x)) if isinstance(x, (float, np.floating)) else str(int(x))
+
+
+def save_capture_histories(summary, chains, iterations, file_ids, path):
+    """The capture-histories files under `path`, every number from an analysis_arrays.CaptureSummary over the pooled
+    samples (chain-major), floats written with repr:
+      capture-histories-samples.csv  chain, iteration, one 0/1 column per file id, entities: one row per sample and per
+                                     history with a non-zero count, histories ascending
+      capture-histories.csv          per history 1 .. 2^F - 1: its 0/1 columns, mean, sd and 2.5/50/97.5 % quantiles
+                                     of its count
+      population-size.csv            per quantity: mean, sd, quantiles over the samples where it is finite, and the
+                                     number where it is infinite
+      population-size-samples.csv    chain, iteration, one column per quantity"""
+    fids = [str(f) for f in file_ids]
+    H, hist = summary.H, summary.histories
+    rows = []
+    for k, it, row in zip(chains, iterations, H):
+        for h in np.flatnonzero(row[1:]) + 1:
+            rows.append([int(k), int(it)] + hist[h - 1].tolist() + [int(row[h])])
+    _save_csv(path, "capture-histories-samples.csv", ["chain", "iteration"] + fids + ["entities"], rows)
+    _save_csv(path, "capture-histories.csv", fids + ["mean", "sd", "q2.5", "q50", "q97.5"],
+              [m.tolist() + [repr(v) for v in vals] for m, vals in zip(hist, summary.history_summary())])
+    names = summary.quantity_names(fids)
+    _save_csv(path, "population-size.csv", ("quantity", "mean", "sd", "q2.5", "q50", "q97.5", "infinite"),
+              [[q] + [repr(v) for v in vals[:5]] + [vals[5]] for q, vals in zip(names, summary.quantity_summary())])
+    _save_csv(path, "population-size-samples.csv", ["chain", "iteration"] + names,
+              [[int(k), int(it)] + [_number(c[s]) for c in summary.columns]
+               for s, (k, it) in enumerate(zip(chains, iterations))])
+
+
+def save_file_links(record_ids, record_files, probabilities, file_ids, path):
+    """file-links.csv under `path`: per record in data order its id, its file id and, per file id, the probability
+    (written with repr) that its cluster holds another record of that file."""
+    _save_csv(path, "file-links.csv", ["recordId", "fileId"] + [str(f) for f in file_ids],
+              [[r, f] + [repr(float(p)) for p in row] for r, f, row in zip(record_ids, record_files, probabilities)])
+
+
+def save_capture_histories_evaluation(rows, path):
+    """capture-histories-evaluation.csv under `path`: rows (quantity, truth, posterior mean, 2.5 % and 97.5 %
+    quantiles, 1 when the truth lies inside them), floats written with repr."""
+    _save_csv(path, "capture-histories-evaluation.csv", ("quantity", "truth", "mean", "q2.5", "q97.5", "inside"),
+              [[q, _number(t)] + [repr(float(v)) for v in vals] + [int(inside)] for q, t, *vals, inside in rows])

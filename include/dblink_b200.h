@@ -638,6 +638,34 @@ int dbl_query_num_candidates(const dbl_query *, int64_t *n_out);
 int dbl_query_read(dbl_query *, int32_t *query, int32_t *record, double *sum /* H each */, double *scale,
                    double *zsum, double *zsq, double *fresh /* Q each */, double *logz /* S Q */);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Capture histories of the files a chain links, on the device that is current when dbl_capture_create() is called.
+ * file (R int32 in [0, F), host or device, uploaded once) gives each record its file; samples are fed one at a time as
+ * cluster[R], as for dbl_posterior_*.  For a cluster c of a sample, its history is h(c) = OR over records r of c of
+ * (1 << file[r]).  With S samples added:
+ *   H[s][h]  the clusters of sample s whose history is h, h in [0, 2^F), int64; H[s][0] = 0
+ *   L[r][g]  the samples in which r's cluster holds a record of file g other than r itself, int32
+ *   dbl_capture_add_sample  cluster may be a host or a device pointer (ready when the call is made); a NULL pointer, a
+ *                      label outside [0, R) or a sample beyond max_samples gives DBL_ERR_INVALID and changes nothing.
+ *                      Every record ORs its file bit into its cluster's history word and, when the word already had
+ *                      it, into its duplicate word (integer atomics, aggregated per warp and label); then one pass over
+ *                      the labels histograms the history words in shared memory into row s of H, and adds to row r of
+ *                      L the other files' bits of r's history and its own file's bit of the duplicate word.
+ *   dbl_capture_read   H as S x 2^F int64 into a host array and, unless record_links is NULL, L as R x F int32 (row-
+ *                      major, host or device).  DBL_ERR_INVALID: histories NULL; DBL_ERR_STATE before the first sample.
+ * DBL_ERR_INVALID: a NULL pointer, num_records outside [1, 2^31 - 1], F outside [1, 12], max_samples < 1 or a file
+ * outside [0, F) (no object is created).  DBL_ERR_CUDA: no device, or an allocation that fails (16 + 4 F bytes per
+ * record -- labels, files, the two words and L -- and 8 2^F bytes per sample, up front).
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct dbl_capture dbl_capture;
+int dbl_capture_create(dbl_capture **out, int64_t num_records, const int32_t *file /* R, host or device */,
+                       int32_t num_files, int32_t max_samples);
+void dbl_capture_free(dbl_capture *);
+int dbl_capture_add_sample(dbl_capture *, const int32_t *cluster /* R, host or device */);
+int32_t dbl_capture_num_samples(const dbl_capture *);
+int dbl_capture_read(dbl_capture *, int64_t *histories /* S x 2^F, host */,
+                     int32_t *record_links /* R x F, host or device, may be NULL */);
+
 #ifdef __cplusplus
 }
 #endif
