@@ -1374,7 +1374,7 @@ struct dbl_ctx {
   int perm[DBL_MAX_ATTRS] = {0};
   int n_str = 0;       // non-constant attributes
   int hslots = 32, hshift = 27;  // common hash-table size of the non-constant attributes; hslots = 0: none
-  Pcg2Format pcg2_fmt{};         // tile format of k_link_pcg2 (pcg2_format)
+  Pcg2Format pcg2_fmt{};         // tile format of k_link_pcg2 (pcg2_format; quad: pcg2_quad in alloc_blocks)
   std::vector<AttrDev> h_attrs;
   DevBuf<int> tree_buf;
   TreeDev tree{};
@@ -1823,7 +1823,10 @@ static int alloc_blocks(dbl_ctx *ctx) {
   const size_t max_tiles = (size_t)(ctx->E / TE) + (size_t)P + 1;
   CUDA_TRY(ctx->tiles.alloc(max_tiles * TileLayout::of(ctx->A).words()));
   if (int rc = alloc_tile_invn(ctx)) return rc;
-  // work item and grid of the persistent PCG-II kernel for this model shape (see Pcg2Format::rpw)
+  // work item and grid of the persistent PCG-II kernel for this model shape and size (see Pcg2Format::rpw)
+  const Pcg2Format f = pcg2_quad(ctx->pcg2_fmt, ctx->n_str, ctx->R / ctx->world, ctx->sm_count);
+  if (f.quad != ctx->pcg2_fmt.quad) ctx->pcg2_smem_cfg = 0;  // another instantiation: opt in to its shared memory
+  ctx->pcg2_fmt = f;
   ctx->pcg2_recs = LINK_WARPS * ctx->pcg2_fmt.rpw(ctx->n_str);
   ctx->pcg2_grid = ctx->sm_count * ctx->pcg2_fmt.ctas_per_sm(ctx->n_str);
   const size_t need = (size_t)ctx->pcg2_grid * ctx->pcg2_recs * 1024;

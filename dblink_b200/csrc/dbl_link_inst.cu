@@ -1,4 +1,4 @@
-// One translation unit per attribute count: compiled with -DDBL_INST_A=<A>; instantiates k_link_pcg2<A, 0..A, HC, PK>.
+// One translation unit per attribute count: compiled with -DDBL_INST_A=<A>; instantiates k_link_pcg2<A, 0..A, ...>.
 #include "dbl_link_pcg2.cuh"
 
 #ifndef DBL_INST_A

@@ -1,10 +1,12 @@
-// k_link_pcg2<A, NS, HC, PK, ID16, SC>: the PCG-II link update (updateEntityIdCollapsed, GU:363-395) with everything
-// about the model shape known at compile time: A attributes in kernel order, the last NS of them non-constant; HC = 32
-// when the hash tables have 32 slots (else the size is a run-time parameter); PK = the constant attributes arrive
-// byte-packed; ID16 (PK only) = the non-constant values arrive as 16-bit halves, two per word (every non-constant
-// value, or SC code, is < 65536); SC (PK only) = those values are slot codes (AttrDev::pcode, dbl_index::
-// build_slot_codes) whose low five bits are the value's slot in every record's table.  HC, PK, ID16 and SC are one
-// Pcg2Format, which pcg2_format decides once per model; the tiles, the launch and dbl_link_kernel's report follow it.
+// k_link_pcg2<A, NS, HC, PK, ID16, SC, QUAD>: the PCG-II link update (updateEntityIdCollapsed, GU:363-395) with
+// everything about the model shape known at compile time: A attributes in kernel order, the last NS of them
+// non-constant; HC = 32 when the hash tables have 32 slots (else the size is a run-time parameter); PK = the
+// constant attributes arrive byte-packed; ID16 (PK only) = the non-constant values arrive as 16-bit halves, two per
+// word (every non-constant value, or SC code, is < 65536); SC (PK only) = those values are slot codes (AttrDev::pcode,
+// dbl_index::build_slot_codes) whose low five bits are the value's slot in every record's table; QUAD (ID16 and SC
+// only) = four records per warp.  HC, PK, ID16 and SC are one Pcg2Format, which pcg2_format decides once per model,
+// and QUAD its quad bit, which pcg2_quad adds from the state's size; the tiles, the launch and dbl_link_kernel's
+// report follow it.
 //
 //  * persistent CTAs: the grid is a few CTAs per SM; each takes the next group of LINK_WARPS records of some block
 //    from a device-side counter until none is left (no empty CTAs on a shard that owns 1/8 of the records, no tail);
@@ -15,8 +17,8 @@
 //    (ID16: 3 words of values + the packed word) and the LDS.64 of N = 6 wavefronts per warp-step, against two
 //    LDS.128 + N = 10 with 32-bit values; the unpacking costs one LOP3 or SHF per value (6 per candidate, shared by
 //    the warp's two records; one PRMT per value with paired tables);
-//  * each consumer warp owns one record (two in the 32-slot shapes); its constants (value ids, hash multipliers
-//    unless SC) are registers;
+//  * each consumer warp owns one record (two in the 32-slot shapes, four with QUAD); its constants (value ids, hash
+//    multipliers unless SC) are registers;
 //  * constant attributes: the product of the exact-match multipliers comes from a 16-entry per-record table indexed
 //    by the byte-wise match mask of the packed values (PK), else from per-attribute compares;
 //  * non-constant attributes: ONE probe per (candidate, attribute) of a 32-slot perfect-hash table in shared memory
@@ -44,6 +46,7 @@ struct Pcg2Format {
   int hc;              // 32: the model's hash tables have 32 slots, a compile-time size; 0: p.hslots
   __host__ __device__ static constexpr int hc_of(int hslots) { return hslots == 32 ? 32 : 0; }
   bool pk, id16, sc;   // byte-packed constants; 16-bit non-constant values; slot codes in place of value ids
+  bool quad = false;   // four records per consumer warp (pcg2_quad decides it; the tiles do not change with it)
   // Words of an entity in the tiles (TileLayout): pk: the NS non-constant values then the byte-packed constants;
   // else all A values in kernel order.  id16: the NS values are 16-bit, two per word (value 2i in the low half of
   // word i), so A = 10 with 6 non-constant attributes needs one group instead of two.  pcg2_store writes them,
@@ -57,18 +60,21 @@ struct Pcg2Format {
   // tile loads and half the tile traffic through shared memory per (record, candidate) pair, two independent
   // dependency chains per warp; the price is registers (96 instead of 72: 2 CTAs per SM instead of 3) and twice the
   // per-record tables in shared memory -- so it is used for the 32-slot instantiations with up to 8 non-constant
-  // attributes (faster at A = 10, NS = 6; three records per warp spill).  Every shape has LINK_WARPS consumer warps:
-  // ONE CTA of 16 consumer warps per SM was slower than two CTAs of 8 (one ring per SM: every warp waits for the
-  // slowest at each stage).
-  __host__ __device__ constexpr int rpw(int NS) const { return (hc == 32 && NS >= 1 && NS <= 8) ? 2 : 1; }
+  // attributes (faster at A = 10, NS = 6).  With 4 (quad, paired tables only), the load, the unpacking and the
+  // probe slot of a candidate serve four records.  Every shape has LINK_WARPS consumer warps: ONE CTA of 16 consumer
+  // warps per SM was slower than two CTAs of 8 (one ring per SM: every warp waits for the slowest at each stage).
+  __host__ __device__ constexpr int rpw(int NS) const {
+    return (hc == 32 && NS >= 1 && NS <= 8) ? (quad ? 4 : 2) : 1;
+  }
   // 3 CTAs per SM (72 registers) only where one record per warp fits them: few non-constant attributes
   __host__ __device__ constexpr int ctas_per_sm(int NS) const { return (rpw(NS) >= 2 || NS > 6) ? 2 : 3; }
-  // the two records of a warp share paired key tables (PAIR_KEYS) when every code fits 16 bits
-  __host__ __device__ constexpr bool paired(int NS) const { return id16 && sc && rpw(NS) == 2; }
-  // as dbl_link_kernel reports it: +4 pk, +8 hc = 32, +16 id16, +32 sc, +64 paired, +128 two records per warp
+  // the records of a warp share paired key tables (PAIR_KEYS) when every code fits 16 bits
+  __host__ __device__ constexpr bool paired(int NS) const { return id16 && sc && rpw(NS) >= 2; }
+  // as dbl_link_kernel reports it: +4 pk, +8 hc = 32, +16 id16, +32 sc, +64 paired, +128 two records per warp,
+  // +512 four records per warp
   constexpr int bits(int NS) const {
     return (pk ? 4 : 0) + (hc == 32 ? 8 : 0) + (id16 ? 16 : 0) + (sc ? 32 : 0) + (paired(NS) ? 64 : 0) +
-           (rpw(NS) == 2 ? 128 : 0);
+           (rpw(NS) == 2 ? 128 : 0) + (rpw(NS) == 4 ? 512 : 0);
   }
 };
 
@@ -98,16 +104,32 @@ inline Pcg2Format pcg2_format(const dbl_model_desc *d, int hslots) {
   return f;
 }
 
+// Four records per warp (Pcg2Format::quad) for a sweep over `records` records (a rank's share) on `sms` SMs: paired
+// tables with at most 6 non-constant attributes (with 7, two CTAs' tables and 1/n(y) columns exceed an SM's shared
+// memory), and enough work.  A work item then holds twice the records and takes about twice as long, so a sweep with
+// few work items per persistent CTA would finish on fewer, longer items; the quad shape waits for QUAD_ITEMS_PER_CTA
+// of them per CTA.  DBL_NO_QUAD (tests) withholds it.
+constexpr int QUAD_ITEMS_PER_CTA = 8;
+inline Pcg2Format pcg2_quad(Pcg2Format f, int NS, int64_t records, int sms) {
+  f.quad = false;
+  const bool fits = f.paired(NS) && NS <= 6;
+  const int64_t items = records / (4 * LINK_WARPS);
+  f.quad = fits && items >= (int64_t)QUAD_ITEMS_PER_CTA * sms * f.ctas_per_sm(NS) && !getenv("DBL_NO_QUAD");
+  return f;
+}
+
 // Per (record, non-constant attribute): H key words then H f64 values, H = p.hslots (a power of two >= 32, the same
 // for every attribute of the model; 32 = one key per bank = conflict-free probes).
 __device__ __host__ __forceinline__ int pcg2_tab_bytes(int H) { return H * 12; }
 
-// Paired tables (16-bit slot codes, two records per warp: Pcg2Format::paired): per (warp, non-constant attribute) 32
-// key words, word s = the key of record 0 at slot s in the low half and record 1's in the high half (one word per
-// bank: one conflict-free probe serves both records), then record 0's 32 f64 values, then record 1's, PAIR_VALS bytes
-// further: both value loads of a probe share one address.  An empty half at slot s holds s ^ 1, which no code with
-// code & 31 == s equals.
-constexpr int PAIR_KEYS = 32 * 4, PAIR_VALS = 32 * 8, PAIR_ATTR_BYTES = PAIR_KEYS + 2 * PAIR_VALS;
+// Paired tables (16-bit slot codes, 2 or 4 records per warp: Pcg2Format::paired): per (warp, non-constant
+// attribute) one array of 32 key words per pair of records, word s = the key of the pair's first record at slot s in
+// the low half and the second's in the high half (one word per bank: one conflict-free probe serves both records),
+// then each record's 32 f64 values, PAIR_VALS bytes apart: every key and value load of a probe shares one address.
+// An empty half at slot s holds s ^ 1, which no code with code & 31 == s equals.  Key entries stay 4 bytes: with 8,
+// slots s and s + 16 would share a bank and a probe would take two wavefronts.
+constexpr int PAIR_KEYS = 32 * 4, PAIR_VALS = 32 * 8;
+__host__ __device__ constexpr int pair_attr_bytes(int rpw) { return rpw / 2 * PAIR_KEYS + rpw * PAIR_VALS; }
 
 // w *= r when y == x (shapes without the packed-constant table; ptxas turns any predicated form into DMUL + 2 FSEL)
 __device__ __forceinline__ void mul_if_eq(double &w, int y, int x, double r) {
@@ -263,18 +285,21 @@ __device__ __forceinline__ bool pcg2_half_hit(unsigned k, unsigned c2) {
   return hit != 0;
 }
 
-// Paired tables (Pcg2Format::paired): the weights of one candidate for the warp's records whose bit is set in `recs`, in w[0]
-// and w[1]; each is the product pcg2_weight forms, factor for factor in the same order.  Per (candidate, attribute):
-// one PRMT spreads the 16-bit code over both halves of a word, c2 = {code, code}; ONE key load at slot code & 31
-// serves both records, whose hits are the halves of k ^ c2 that are zero (pcg2_half_hit); one value address serves
-// both predicated value loads (record 1's values are PAIR_VALS bytes past record 0's).  inv: as in pcg2_weight.
-template <int A, int NS, bool MISSING = true>
-__device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc)[2], unsigned recs,
+// Paired tables (Pcg2Format::paired): the weights of one candidate for the warp's RPW = 2 or 4 records whose bit is set
+// in `recs`, in w[]; each is the product pcg2_weight forms, factor for factor in the same order.  Per (candidate,
+// attribute): one PRMT spreads the 16-bit code over both halves of a word, c2 = {code, code}; ONE key load at slot
+// code & 31 serves a pair of records, whose hits are the halves of k ^ c2 that are zero (pcg2_half_hit); the key
+// loads of the RPW / 2 pairs and the RPW predicated value loads each sit at a fixed offset from one slot address.
+// inv: as in pcg2_weight.
+template <int A, int NS, int RPW, bool MISSING = true>
+__device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc)[RPW], unsigned recs,
                                                  const char *tab, const double *ctab, const Pcg2Cand<A, NS, true> &cd,
-                                                 double (&w)[2], const double *inv) {
+                                                 double (&w)[RPW], const double *inv) {
   static_assert(NS >= 1 && NS < A, "paired tables: packed constants and at least one non-constant attribute");
+  static_assert(RPW == 2 || RPW == 4, "paired tables: pairs of records");
+  constexpr int AB = pair_attr_bytes(RPW);
 #pragma unroll
-  for (int ri = 0; ri < 2; ++ri)  // protocol 4.1: w = N * (product of the constant attributes' multipliers)
+  for (int ri = 0; ri < RPW; ++ri)  // protocol 4.1: w = N * (product of the constant attributes' multipliers)
     w[ri] = cd.N * *reinterpret_cast<const double *>(reinterpret_cast<const char *>(ctab + ri * 16) +
                                                      pcg2_const_offset(cd.ypack, rc[ri].xpack));
 #pragma unroll
@@ -282,14 +307,19 @@ __device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc
     const unsigned c2 = __byte_perm(cd.y16[q >> 1], 0u, (q & 1) ? 0x3232 : 0x1010);
     unsigned slot;  // opaque AND, as in pcg2_weight
     asm("and.b32 %0, %1, 31;" : "=r"(slot) : "r"(c2));
-    const unsigned k = reinterpret_cast<const unsigned *>(tab + q * PAIR_ATTR_BYTES)[slot];
-    const double *v = reinterpret_cast<const double *>(tab + q * PAIR_ATTR_BYTES + PAIR_KEYS) + slot;
-    if ((recs & 1u) && pcg2_half_hit<0>(k, c2)) w[0] = w[0] * v[0];
-    if ((recs & 2u) && pcg2_half_hit<1>(k, c2)) w[1] = w[1] * v[PAIR_VALS / 8];
+    const unsigned *kp = reinterpret_cast<const unsigned *>(tab + q * AB) + slot;
+    const double *v = reinterpret_cast<const double *>(tab + q * AB + RPW / 2 * PAIR_KEYS) + slot;
+#pragma unroll
+    for (int pi = 0; pi < RPW / 2; ++pi) {
+      const unsigned k = kp[pi * (PAIR_KEYS / 4)];
+      if (((recs >> (2 * pi)) & 1u) && pcg2_half_hit<0>(k, c2)) w[2 * pi] = w[2 * pi] * v[2 * pi * (PAIR_VALS / 8)];
+      if (((recs >> (2 * pi + 1)) & 1u) && pcg2_half_hit<1>(k, c2))
+        w[2 * pi + 1] = w[2 * pi + 1] * v[(2 * pi + 1) * (PAIR_VALS / 8)];
+    }
   }
   if (MISSING) {
 #pragma unroll
-    for (int ri = 0; ri < 2; ++ri) {
+    for (int ri = 0; ri < RPW; ++ri) {
       if (!((recs >> ri) & 1u) || !rc[ri].mmask) continue;
 #pragma unroll
       for (int q = 0; q < NS; ++q)
@@ -300,16 +330,23 @@ __device__ __forceinline__ void pcg2_weight_pair(const Pcg2Rec<A, NS, true> (&rc
 
 // bytes of one consumer warp's hash tables (H = the table size of the model)
 __host__ __device__ inline int pcg2_warp_tab_bytes(Pcg2Format f, int NS, int H) {
-  return f.paired(NS) ? NS * PAIR_ATTR_BYTES : f.rpw(NS) * (NS > 0 ? NS : 1) * pcg2_tab_bytes(H);
+  return f.paired(NS) ? NS * pair_attr_bytes(f.rpw(NS)) : f.rpw(NS) * (NS > 0 ? NS : 1) * pcg2_tab_bytes(H);
 }
 
-template <int A, int NS, int HC, bool PK, bool ID16, bool SC>
-__global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16, SC}.ctas_per_sm(NS)) k_link_pcg2(LinkParams p) {
+// doubles of a CTA's pass-1 chunk totals (paired tables: 32 per record, so that the records' running totals and
+// check-points need no registers in the tile loop; other shapes keep them in registers)
+__host__ __device__ constexpr int pcg2_chunk_totals(Pcg2Format f, int NS) {
+  return f.paired(NS) ? LINK_WARPS * f.rpw(NS) * 32 : 0;
+}
+
+template <int A, int NS, int HC, bool PK, bool ID16, bool SC, bool QUAD>
+__global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16, SC, QUAD}.ctas_per_sm(NS))
+    k_link_pcg2(LinkParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ int s_cta;
   if (sweep_dead(p.ctl)) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr Pcg2Format FMT{HC, PK, ID16, SC};
+  constexpr Pcg2Format FMT{HC, PK, ID16, SC, QUAD};
   constexpr int TW = FMT.layout(A, NS).words();
   constexpr int NC = A - NS;
   constexpr int RPW = FMT.rpw(NS);
@@ -327,12 +364,14 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
   // a compile-time 1 moves ptxas's spills and cost 1.2 % at A = 11, NS = 5 (H100 SXM, 700 W)
   const int wtab = pcg2_warp_tab_bytes(HC ? FMT : Pcg2Format{Pcg2Format::hc_of(p.hslots)}, NS, HC ? HC : p.hslots);
   char *tab0 = reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 + (size_t)warp * wtab;
+  double *dbl0 = reinterpret_cast<double *>(reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 +
+                                           (size_t)WARPS * wtab);
   // PK: products of the matching constant attributes, by match mask, 16 entries per record
-  double *ctab0 = reinterpret_cast<double *>(reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 +
-                                            (size_t)WARPS * wtab) + warp * RPW * 16;
+  double *ctab0 = dbl0 + warp * RPW * 16;
+  // PAIR: each record's chunk totals of pass 1, [record][chunk] (see pcg2_chunk_totals)
+  double *tot0 = dbl0 + WARPS * RPW * 16 + warp * RPW * 32;
   // the 1/n(y) columns of the staged tiles (only when p.tile_invn: see pcg2_smem_bytes)
-  rg.cols = reinterpret_cast<double *>(reinterpret_cast<char *>(smem) + (size_t)LINK_STAGES * TW * 4 + 128 +
-                                       (size_t)WARPS * wtab) + WARPS * RPW * 16;
+  rg.cols = dbl0 + WARPS * RPW * 16 + pcg2_chunk_totals(FMT, NS);
   rg.ncols = NS;
   ring_init(rg, WARPS);
   const int total_ctas = p.cta_ptr[p.P];
@@ -368,21 +407,21 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
 
     // ---- per-record constants: lane k prepares kernel-order attribute k, then everything is broadcast
     Pcg2Rec<A, NS, SC> rc[RPW];
-    int rr[RPW];
-    bool act[RPW];
+    // (the record ids are read again in pass 2 rather than kept live through the tile loop)
+    const int nact = min(RPW, p.rec_ptr[b + 1] - (rec0 + warp * RPW));  // the warp's records, 0..RPW
 #pragma unroll
     for (int ri = 0; ri < RPW; ++ri) {
       const int ridx = rec0 + warp * RPW + ri;
-      act[ri] = ridx < p.rec_ptr[b + 1];
-      rr[ri] = act[ri] ? p.rec_sorted[ridx] : -1;
-      const int r = rr[ri];
+      const bool act = ri < nact;
+      const int r = act ? p.rec_sorted[ridx] : -1;
       char *tab = PAIR ? tab0 : tab0 + ri * tabrec;
+      constexpr int PAB = pair_attr_bytes(RPW);
       double *ctab = ctab0 + ri * 16;
       int xv = -1;
       double rmv = 1.0;
       unsigned hmv = 0;
       bool is_m = false;
-      if (act[ri] && lane < A) {
+      if (act && lane < A) {
         const int a = p.perm[lane];
         const AttrDev &at = p.attrs[a];
         xv = p.x[(int64_t)r * A + a];
@@ -418,9 +457,9 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
 #pragma unroll
       for (int q = 0; q < NS; ++q) {
         const AttrDev &at = p.attrs[p.perm[A - NS + q]];
-        char *tq = tab + q * (PAIR ? PAIR_ATTR_BYTES : pcg2_tab_bytes(H));
-        int *kd = reinterpret_cast<int *>(tq);
-        double *vd = reinterpret_cast<double *>(tq + (PAIR ? PAIR_KEYS + ri * PAIR_VALS : H * 4));
+        char *tq = tab + q * (PAIR ? PAB : pcg2_tab_bytes(H));
+        int *kd = reinterpret_cast<int *>(tq + (PAIR ? (ri >> 1) * PAIR_KEYS : 0));
+        double *vd = reinterpret_cast<double *>(tq + (PAIR ? RPW / 2 * PAIR_KEYS + ri * PAIR_VALS : H * 4));
         const int xq = rc[ri].x[A - NS + q];
         // SC: the code-keyed tables, each value at the slot its code names
         const int *hkeys = SC ? at.sckeys : at.hkeys;
@@ -430,8 +469,8 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
         else own = (xq >= 0) ? (((unsigned)xq * rc[ri].hm[q]) >> hshift) : 0xFFFFFFFFu;
         for (int i = lane; i < H; i += 32) {
           const int key = (xq >= 0) ? hkeys[(size_t)xq * H + i] : -1;
-          if constexpr (PAIR)  // the record's half of the paired key word; empty: i ^ 1
-            reinterpret_cast<unsigned short *>(kd)[2 * i + ri] = (unsigned short)(key >= 0 ? key : i ^ 1);
+          if constexpr (PAIR)  // the record's half of its pair's key word; empty: i ^ 1
+            reinterpret_cast<unsigned short *>(kd)[2 * i + (ri & 1)] = (unsigned short)(key >= 0 ? key : i ^ 1);
           else
             kd[i] = key;
           vd[i] = ((unsigned)i == own) ? rc[ri].rm[A - NS + q] : ((xq >= 0) ? hvals[(size_t)xq * H + i] : 1.0);
@@ -471,7 +510,7 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
         const int g = tbase + t;
         const int s = g % LINK_STAGES;
         mbar_wait(&rg.full[s], (g / LINK_STAGES) & 1);
-        if (act[0]) {  // (the second record of a warp is only there when the first is)
+        if (nact > 0) {
           const int *tile = rg.tiles + (size_t)s * TW;
           const double *cols = rg.cols + (size_t)s * NS * TE + lane;  // the staged 1/n(y) columns (MISSING)
 #pragma unroll
@@ -479,10 +518,10 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
             Pcg2Cand<A, NS, PK> cd;
             pcg2_load<A, NS, PK, ID16>(cd, tile, q * 32 + lane);
             if constexpr (PAIR) {
-              double w[2];
-              pcg2_weight_pair<A, NS, MISSING>(rc, 3u, tab0, ctab0, cd, w, cols + q * 32);
-              acc[0] = acc[0] + w[0];
-              acc[1] = acc[1] + w[1];
+              double w[RPW];
+              pcg2_weight_pair<A, NS, RPW, MISSING>(rc, (1u << RPW) - 1, tab0, ctab0, cd, w, cols + q * 32);
+#pragma unroll
+              for (int ri = 0; ri < RPW; ++ri) acc[ri] = acc[ri] + w[ri];
             } else {
 #pragma unroll
               for (int ri = 0; ri < RPW; ++ri)
@@ -494,7 +533,12 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
 #pragma unroll
             for (int ri = 0; ri < RPW; ++ri) {
               my_sums[ri * 1024 + chunk * 32 + lane] = acc[ri];  // pass 2 reads the chosen chunk's sums back
-              close_chunk(lane, chunk, acc[ri], run[ri], Q[ri]);
+              if constexpr (PAIR) {  // the chunk total, as close_chunk forms it; the check-points after the loop
+                const double tot = butterfly_sum(acc[ri]);
+                if (lane == 0) tot0[ri * 32 + chunk] = tot;
+              } else {
+                close_chunk(lane, chunk, acc[ri], run[ri], Q[ri]);
+              }
               acc[ri] = 0.0;
             }
             ++chunk;
@@ -507,12 +551,20 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
     };
     if (any_missing) pass1(std::true_type{}); else pass1(std::false_type{});
     tbase += ntiles;
+    if constexpr (PAIR) {  // close_chunk's running totals and check-points, in chunk order, from the stored totals
+#pragma unroll
+      for (int ri = 0; ri < RPW; ++ri)
+        for (int c = 0; c < chunk; ++c) {
+          run[ri] = run[ri] + tot0[ri * 32 + c];
+          if (lane == c) Q[ri] = run[ri];
+        }
+    }
 
     // ---- pass 2 from the L2-resident copy of the tiles, one record after the other
 #pragma unroll
     for (int ri = 0; ri < RPW; ++ri) {
-      if (!act[ri]) continue;
-      const int r = rr[ri];
+      if (ri >= nact) continue;
+      const int r = p.rec_sorted[rec0 + warp * RPW + ri];
       if (!check_mass(p, lane, r, run[ri])) continue;
       auto wf = [&](int j) -> double {
         if (j >= n) return 0.0;
@@ -520,10 +572,10 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
         pcg2_load<A, NS, PK, ID16>(cd, gtiles + (size_t)(j / TE) * TW, j % TE);
         // the candidate's 1/n(y) in global memory (read only when the record misses a value: then gcols is set)
         const double *inv = gcols + (size_t)(j / TE) * NS * TE + j % TE;
-        if constexpr (PAIR) {  // record ri's half of the paired tables
-          double w[2];
-          pcg2_weight_pair<A, NS>(rc, 1u << ri, tab0, ctab0, cd, w, inv);
-          return ri ? w[1] : w[0];
+        if constexpr (PAIR) {  // record ri's half of its pair's tables
+          double w[RPW];
+          pcg2_weight_pair<A, NS, RPW>(rc, 1u << ri, tab0, ctab0, cd, w, inv);
+          return w[ri];
         } else {
           return pcg2_weight<A, NS, HC, PK, SC>(rc[ri], p, tab0 + ri * tabrec, ctab0 + ri * 16, cd, inv);
         }
@@ -539,7 +591,8 @@ __global__ void __launch_bounds__((LINK_WARPS + 1) * 32, Pcg2Format{HC, PK, ID16
 // stage (LinkParams::tile_invn set: some record misses a non-constant value)
 inline size_t pcg2_smem_bytes(Pcg2Format f, int A, int NS, int H, bool invn) {
   return (size_t)LINK_STAGES * f.layout(A, NS).words() * 4 + 128 + (size_t)LINK_WARPS * pcg2_warp_tab_bytes(f, NS, H) +
-         (size_t)LINK_WARPS * f.rpw(NS) * 16 * sizeof(double) + (invn ? (size_t)LINK_STAGES * NS * TE * sizeof(double) : 0);
+         (size_t)(LINK_WARPS * f.rpw(NS) * 16 + pcg2_chunk_totals(f, NS)) * sizeof(double) +
+         (invn ? (size_t)LINK_STAGES * NS * TE * sizeof(double) : 0);
 }
 
 // k_link_pcg2<A, NS, ...> of format f for a runtime NS in [0, A] (nullptr: none); the `if constexpr` guards only keep
@@ -552,12 +605,19 @@ Pcg2Kernel pcg2_kernel(int ns, Pcg2Format f) {
     return nullptr;
   }
   if constexpr (A - NS >= 1 && A - NS <= 4) {
-    if constexpr (NS >= 1) {
-      if (f.sc) return f.id16 ? k_link_pcg2<A, NS, 32, true, true, true> : k_link_pcg2<A, NS, 32, true, false, true>;
+    if constexpr (NS >= 1 && NS <= 6) {
+      if (f.sc && f.id16 && f.quad) return k_link_pcg2<A, NS, 32, true, true, true, true>;
     }
-    if (f.pk) return f.id16 ? k_link_pcg2<A, NS, 32, true, true, false> : k_link_pcg2<A, NS, 32, true, false, false>;
+    if constexpr (NS >= 1) {
+      if (f.sc)
+        return f.id16 ? k_link_pcg2<A, NS, 32, true, true, true, false>
+                      : k_link_pcg2<A, NS, 32, true, false, true, false>;
+    }
+    if (f.pk)
+      return f.id16 ? k_link_pcg2<A, NS, 32, true, true, false, false>
+                    : k_link_pcg2<A, NS, 32, true, false, false, false>;
   }
-  return f.hc ? k_link_pcg2<A, NS, 32, false, false, false> : k_link_pcg2<A, NS, 0, false, false, false>;
+  return f.hc ? k_link_pcg2<A, NS, 32, false, false, false, false> : k_link_pcg2<A, NS, 0, false, false, false, false>;
 }
 
 // launch kernel k on `grid` CTAs with `smem` bytes of dynamic shared memory; lp == nullptr: load the kernel without

@@ -551,14 +551,15 @@ class GibbsEngine:
 
     def link_tile_format(self, sampler="PCG-II"):
         """Tile format of the k_link_pcg2 instantiation a sweep with this sampler launches: {"id16": 16-bit
-        non-constant values, "slot_codes": slot codes instead of value ids, "paired": the warp's two records share
-        their key tables, "records_per_warp": 1 or 2}; None when the sampler gets another link kernel."""
+        non-constant values, "slot_codes": slot codes instead of value ids, "paired": the warp's records share their
+        key tables in pairs, "records_per_warp": 1, 2 or 4}; None when the sampler gets another link kernel.  Four
+        records per warp need a state with enough records (pcg2_quad), so the report can change with the state."""
         s = SAMPLERS[sampler] if isinstance(sampler, str) else int(sampler)
         k = _lib.load().dbl_link_kernel(self._h, s)
         if (k & 3) != 3:
             return None
         return {"id16": bool(k & 16), "slot_codes": bool(k & 32), "paired": bool(k & 64),
-                "records_per_warp": 2 if k & 128 else 1}
+                "records_per_warp": 4 if k & 512 else 2 if k & 128 else 1}
 
     def set_link_mass_capture(self, on=True):
         """Checking aid: make every link kernel store the total mass of each record's categorical (off by default)."""

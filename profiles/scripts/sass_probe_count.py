@@ -6,14 +6,14 @@ A pass-1 tile loop is a loop of the kernel (a backward branch and its target) th
 (`SYNCS.PHASECHK`, the ring's full barrier) and the `DMUL`s of the scoring: the TE / 32 = 4 unrolled warp-steps of a
 tile, the ring wait, the chunk close and the arrive on the empty barrier.  The wait's retry path lies outside the loop
 and is not counted.  The branch-free loop (records without a missing non-constant value) has no global load; the
-missing-value loop gathers 1/n(y) with `LDG`.  Default kernel: k_link_pcg2<10, 6, 32, PK, ID16, SC>, the benchmark's.
+missing-value loop gathers 1/n(y) with `LDG`.  Default kernel: k_link_pcg2<10, 6, 32, PK, ID16, SC, QUAD>, the benchmark's.
 """
 import argparse
 import collections
 import re
 import subprocess
 
-KERNEL = "_Z11k_link_pcg2ILi10ELi6ELi32ELb1ELb1ELb1EEv10LinkParams"
+KERNEL = "_Z11k_link_pcg2ILi10ELi6ELi32ELb1ELb1ELb1ELb1EEv10LinkParams"
 INSN = re.compile(r"/\*([0-9a-f]{4,})\*/\s+(@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)([^;]*);")
 
 
